@@ -2,20 +2,21 @@
 //
 // Mapping (H100 / sm_90a):
 //   * persistent CTAs of 128 threads; one CTA processes tiles of 128 consecutive filters;
-//   * per tile, ONE elected thread issues 7 TMA tensor copies (cp.async.bulk.tensor) that pull the
-//     tile's x, P, F, Q, H, R, z blocks — contiguous byte ranges of the dense AoS arrays the API is
-//     handed — into a shared-memory stage and complete on an mbarrier; a 2-stage ring keeps the
+//   * per tile, ONE elected thread issues 7 1-D bulk copies (cp.async.bulk, SASS UBLKCP) that pull
+//     the tile's x, P, F, Q, H, R, z blocks — contiguous byte ranges of the dense AoS arrays the API
+//     is handed — into a shared-memory stage and complete on an mbarrier; a 2-stage ring keeps the
 //     next tiles' 33 KB in flight while the current tile computes (HBM latency is hidden by the
-//     ring, not by occupancy);
-//   * the 64-byte P/F/Q rows and 32-byte H rows land through the TMA 64B/32B swizzle, so that
-//     thread t reading ITS filter's row with LDS.128 (16-byte chunk c at position c ^ f(t)) is
-//     bank-conflict-free although the rows are 64 B apart;
-//   * each thread then owns one filter: the whole predict+update runs in registers
-//     (kf_regtile.cuh), results are written with 16-byte stores.
+//     ring, not by occupancy); the ragged last tile copies only its own bytes;
+//   * each thread then owns one filter: it reads its rows of the linear stage with LDS.128 in a
+//     rotated, bank-conflict-free chunk order (lds_row), the
+//     whole predict+update runs in registers (kf_regtile.cuh), results are written with 16-byte
+//     stores;
+//   * consecutive launches overlap at their edges (programmatic dependent launch): a CTA's
+//     prologue runs before griddepcontrol.wait, every global access after it, and a CTA releases
+//     the next launch once it has issued the loads of its last tile.
 // Shared models (stride 0) are read once per thread through the read-only path instead of TMA.
 //
 // Reference arithmetic: filterpy/kalman/kalman_filter.py:471-478, 533-556 (see kf_regtile.cuh).
-#include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
 #include "bke_internal.cuh"
@@ -49,28 +50,25 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
         "DONE:\n"
         "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar)
+// 1-D bulk copy of `bytes` (a multiple of 16, both addresses 16-byte aligned) into shared memory
+__device__ __forceinline__ void bulk_load(void *dst, const void *src, uint32_t bytes, uint64_t *bar)
 {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-// variants with an L2 eviction-priority hint (createpolicy): the state x, P is re-read by the NEXT
+// variant with an L2 eviction-priority hint (createpolicy): the state x, P is re-read by the NEXT
 // step and, for banks whose state is at most 38 MB (about 498 k filters; a bound scaled from an earlier target, not
 // measured on the H100), fits the 50 MB L2 -> evict_last; the models and measurements
 // stream through once per step -> evict_first, so that they do not push the state out.
-__device__ __forceinline__ void tma_load_2d_hint(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar, uint64_t pol)
+__device__ __forceinline__ void bulk_load_hint(void *dst, const void *src, uint32_t bytes, uint64_t *bar, uint64_t pol)
 {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(pol) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
 }
-__device__ __forceinline__ void tma_load_1d_hint(void *dst, const CUtensorMap *map, int c0, uint64_t *bar, uint64_t pol)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.1d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3}], [%2], %4;"
-        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "l"(pol) : "memory");
-}
+// programmatic dependent launch: wait until the previous kernel on the stream has completed and its
+// writes are visible / allow the next one (launched with programmatic stream serialization) to start
+__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ uint64_t policy_evict_first()
 {
     uint64_t p;
@@ -89,13 +87,6 @@ __device__ __forceinline__ void st_hint(float *addr, float4 v, uint64_t pol)
                  ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
 }
 
-__device__ __forceinline__ void tma_load_1d(void *dst, const CUtensorMap *map, int c0, uint64_t *bar)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.1d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0) : "memory");
-}
-
 // ---------------------------------------------------------------------------- tile geometry
 constexpr int TILE = 128;       // filters per tile == threads per CTA
 
@@ -107,8 +98,8 @@ struct Stage {
     static constexpr int HB = TILE * M * N * sizeof(T);
     static constexpr int RB = TILE * M * M * sizeof(T);
     static constexpr int ZB = TILE * M * sizeof(T);
-    // offsets (all 1024-byte aligned: swizzled TMA destinations need it)
-    static constexpr int align_up(int v) { return (v + 1023) & ~1023; }
+    // offsets (bulk-copy destinations must be 16-byte aligned; 128 keeps every block on its own lines)
+    static constexpr int align_up(int v) { return (v + 127) & ~127; }
     // (a bank that shares its models stages only P, x, z: a third of the bytes, so more stages and CTAs fit)
     static constexpr int OP = 0;
     static constexpr int OF = OP + align_up(PB);
@@ -120,20 +111,42 @@ struct Stage {
     static constexpr int BYTES = OZ + align_up(ZB);
 };
 
-// read the 16-byte chunk c of row `row` (ROWB bytes per row) from a TMA-swizzled tile
+// read the 16-byte chunk c of row `row` (ROWB bytes per row) from a linear tile
 template <int ROWB>
 __device__ __forceinline__ float4 lds_chunk(const unsigned char *base, int row, int c)
 {
-    uint32_t off = (uint32_t)row * ROWB + (uint32_t)c * 16;
-    if constexpr (ROWB == 128) off ^= ((off >> 7) & 7u) << 4;
-    else if constexpr (ROWB == 64) off ^= ((off >> 7) & 3u) << 4;
-    else if constexpr (ROWB == 32) off ^= ((off >> 7) & 1u) << 4;
-    return *reinterpret_cast<const float4 *>(base + off);
+    return *reinterpret_cast<const float4 *>(base + row * ROWB + c * 16);
 }
 
-struct Maps {
-    CUtensorMap x, P, F, Q, H, R, z;
-};
+// Read the whole row `row` of a linear tile with rows of ROWS 16-byte chunks (4: P, F, Q; 2: H) into
+// m[ROWS][4].  Read in order, the 8 threads served by one LDS.128 wavefront would land on 2 (4) of
+// the 8 16-byte bank groups: a 4-way (2-way) conflict.  Thread t starts instead at chunk
+// r = (t / (8 / ROWS)) mod ROWS, which spreads the 8 threads over all 8 groups, and rotates the
+// chunks back into place with selects (two rotation steps for 4 chunks, one for 2).
+template <int ROWS>
+__device__ __forceinline__ void lds_row(const unsigned char *base, int row, float (&m)[ROWS][4])
+{
+    const int r = (row / (8 / ROWS)) & (ROWS - 1);
+    float4 v[ROWS];
+#pragma unroll
+    for (int c = 0; c < ROWS; c++)
+        v[c] = *reinterpret_cast<const float4 *>(base + row * ROWS * 16 + ((c + r) & (ROWS - 1)) * 16);
+    // v[c] holds chunk (c + r) mod ROWS; chunk i is v[(i - r) mod ROWS]
+#pragma unroll
+    for (int step = 1; step < ROWS; step <<= 1) {
+        const bool rot = r & step;
+        float4 w[ROWS];
+#pragma unroll
+        for (int i = 0; i < ROWS; i++) {
+            const float4 a = v[i], b = v[(i - step) & (ROWS - 1)];
+            w[i] = make_float4(rot ? b.x : a.x, rot ? b.y : a.y, rot ? b.z : a.z, rot ? b.w : a.w);
+        }
+#pragma unroll
+        for (int i = 0; i < ROWS; i++) v[i] = w[i];
+    }
+#pragma unroll
+    for (int i = 0; i < ROWS; i++) { m[i][0] = v[i].x; m[i][1] = v[i].y; m[i][2] = v[i].z; m[i][3] = v[i].w; }
+}
 
 template <int N, int M>
 struct FastP {
@@ -141,7 +154,8 @@ struct FastP {
     int num_tiles;
     int l2_hints;                   // 1: keep x, P in L2 between steps (evict_last), stream the rest (evict_first)
     float alpha_sq;
-    const float *F, *Q, *H, *R;     // used when SHARED == 1
+    const float *x, *P, *z;         // the prior state and the measurements (dense AoS)
+    const float *F, *Q, *H, *R;     // per-filter models (SHARED == 0) or the bank's one model (SHARED == 1)
     float Fh[N * N], Qh[N * N], Hh[M * N], Rh[M * M];   // used when SHARED == 2: the shared models ride in the launch
                                                         // parameters, so every product with them reads the constant bank
     float *x_out, *P_out;
@@ -152,69 +166,57 @@ struct FastP {
 };
 
 // MODE: 3 = predict+update, 1 = predict only, 2 = update only
-// SHARED: 0 = per-filter models (staged by TMA), 1 = one model for the bank read from device memory,
-// 2 = one model for the bank carried in the kernel parameters
+// SHARED: 0 = per-filter models (staged by bulk copies), 1 = one model for the bank read from device
+// memory, 2 = one model for the bank carried in the kernel parameters
 template <int MODE, int SHARED, bool EXTRAS, int STAGES>
 __global__ void __launch_bounds__(TILE, SHARED == 2 ? 5 : (SHARED ? 4 : 3))
-kf42_f32_kernel(const __grid_constant__ Maps maps, const FastP<4, 2> p)
+kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 {
     constexpr int N = 4, M = 2;
     using St = Stage<float, N, M, SHARED != 0>;
     constexpr bool DO_P = MODE & 1, DO_U = MODE & 2;
-    extern __shared__ __align__(1024) unsigned char smem[];
+    extern __shared__ __align__(128) unsigned char smem[];
     __shared__ __align__(8) uint64_t full[STAGES];
 
     const int tid = threadIdx.x;
-    uint32_t tx_bytes = St::XB + St::PB;
-    if (!SHARED && DO_P) tx_bytes += 2 * St::PB;
-    if (!SHARED && DO_U) tx_bytes += St::HB + St::RB;
-    if (DO_U) tx_bytes += St::ZB;
 
     const uint64_t pol_first = policy_evict_first(), pol_last = policy_evict_last();
+    // the tile's blocks are contiguous byte ranges; a ragged last tile copies only its own filters
+    // (z: 8 B per filter, rounded down to the 16-byte granule; an odd last filter reads its own z)
     auto issue = [&](int tile, int stage) {
         unsigned char *sb = smem + stage * St::BYTES;
         uint64_t *bar = &full[stage];
-        const int row0 = tile * TILE;
-        mbar_expect_tx(bar, tx_bytes);
-        if (p.l2_hints) {
-            tma_load_2d_hint(sb + St::OP, &maps.P, 0, row0, bar, pol_last);
-            tma_load_2d_hint(sb + St::OX, &maps.x, 0, row0, bar, pol_last);
-            if (!SHARED && DO_P) {
-                tma_load_2d_hint(sb + St::OF, &maps.F, 0, row0, bar, pol_first);
-                tma_load_2d_hint(sb + St::OQ, &maps.Q, 0, row0, bar, pol_first);
-            }
-            if (!SHARED && DO_U) {
-                tma_load_2d_hint(sb + St::OH, &maps.H, 0, row0, bar, pol_first);
-                tma_load_2d_hint(sb + St::OR_, &maps.R, 0, row0, bar, pol_first);
-            }
-            if (DO_U) tma_load_1d_hint(sb + St::OZ, &maps.z, row0 * M, bar, pol_first);
-            return;
-        }
-        tma_load_2d(sb + St::OP, &maps.P, 0, row0, bar);
-        tma_load_2d(sb + St::OX, &maps.x, 0, row0, bar);
+        const int64_t f0 = (int64_t)tile * TILE;
+        const int64_t left = p.N_filters - f0;
+        const uint32_t nf = left < TILE ? (uint32_t)left : (uint32_t)TILE;
+        const uint32_t zb = (nf * M * 4) & ~15u;
+        uint32_t tx = nf * (N + N * N) * 4;
+        if (!SHARED && DO_P) tx += nf * 2 * N * N * 4;
+        if (!SHARED && DO_U) tx += nf * (M * N + M * M) * 4;
+        if (DO_U) tx += zb;
+        mbar_expect_tx(bar, tx);
+        auto load = [&](int off, const float *src, int per_filter, uint32_t bytes, uint64_t pol) {
+            if (p.l2_hints) bulk_load_hint(sb + off, src + f0 * per_filter, bytes, bar, pol);
+            else bulk_load(sb + off, src + f0 * per_filter, bytes, bar);
+        };
+        load(St::OP, p.P, N * N, nf * N * N * 4, pol_last);
+        load(St::OX, p.x, N, nf * N * 4, pol_last);
         if (!SHARED && DO_P) {
-            tma_load_2d(sb + St::OF, &maps.F, 0, row0, bar);
-            tma_load_2d(sb + St::OQ, &maps.Q, 0, row0, bar);
+            load(St::OF, p.F, N * N, nf * N * N * 4, pol_first);
+            load(St::OQ, p.Q, N * N, nf * N * N * 4, pol_first);
         }
         if (!SHARED && DO_U) {
-            tma_load_2d(sb + St::OH, &maps.H, 0, row0, bar);
-            tma_load_2d(sb + St::OR_, &maps.R, 0, row0, bar);
+            load(St::OH, p.H, M * N, nf * M * N * 4, pol_first);
+            load(St::OR_, p.R, M * M, nf * M * M * 4, pol_first);
         }
-        if (DO_U) tma_load_1d(sb + St::OZ, &maps.z, row0 * M, bar);
+        if (DO_U && zb) load(St::OZ, p.z, M, zb, pol_first);
     };
 
+    // prologue: nothing here touches global memory, so it may overlap the previous launch
     if (tid == 0) {
         for (int s = 0; s < STAGES; s++) mbar_init(&full[s], 1);
         fence_mbar_init();
     }
-    __syncthreads();
-    if (tid == 0) {
-        for (int s = 0; s < STAGES; s++) {
-            int tile = blockIdx.x + s * gridDim.x;
-            if (tile < p.num_tiles) issue(tile, s);
-        }
-    }
-
     float F[N][N], Q[N][N], H[M][N], R[M][M];
     if (SHARED == 2) {
 #pragma unroll
@@ -227,6 +229,17 @@ kf42_f32_kernel(const __grid_constant__ Maps maps, const FastP<4, 2> p)
             for (int j = 0; j < N; j++) H[a][j] = p.Hh[a * N + j];
 #pragma unroll
             for (int b = 0; b < M; b++) R[a][b] = p.Rh[a * M + b];
+        }
+    }
+    // Every read and write of global memory comes after this point: the previous kernel on the
+    // stream (the previous step, or whatever produced z) may have written any of it, and only
+    // griddepcontrol.wait makes those writes visible.
+    griddep_wait();
+    __syncthreads();
+    if (tid == 0) {
+        for (int s = 0; s < STAGES; s++) {
+            int tile = blockIdx.x + s * gridDim.x;
+            if (tile < p.num_tiles) issue(tile, s);
         }
     }
     if (SHARED == 1) {
@@ -259,31 +272,23 @@ kf42_f32_kernel(const __grid_constant__ Maps maps, const FastP<4, 2> p)
             float4 v = lds_chunk<16>(sb + St::OX, tid, 0);
             x[0] = v.x; x[1] = v.y; x[2] = v.z; x[3] = v.w;
         }
-#pragma unroll
-        for (int i = 0; i < N; i++) {
-            float4 v = lds_chunk<64>(sb + St::OP, tid, i);
-            P[i][0] = v.x; P[i][1] = v.y; P[i][2] = v.z; P[i][3] = v.w;
-        }
+        lds_row<N>(sb + St::OP, tid, P);
         if (!SHARED && DO_P) {
-#pragma unroll
-            for (int i = 0; i < N; i++) {
-                float4 v = lds_chunk<64>(sb + St::OF, tid, i);
-                F[i][0] = v.x; F[i][1] = v.y; F[i][2] = v.z; F[i][3] = v.w;
-                float4 q = lds_chunk<64>(sb + St::OQ, tid, i);
-                Q[i][0] = q.x; Q[i][1] = q.y; Q[i][2] = q.z; Q[i][3] = q.w;
-            }
+            lds_row<N>(sb + St::OF, tid, F);
+            lds_row<N>(sb + St::OQ, tid, Q);
         }
         if (!SHARED && DO_U) {
-#pragma unroll
-            for (int a = 0; a < M; a++) {
-                float4 v = lds_chunk<32>(sb + St::OH, tid, a);
-                H[a][0] = v.x; H[a][1] = v.y; H[a][2] = v.z; H[a][3] = v.w;
-            }
+            lds_row<M>(sb + St::OH, tid, H);
             float4 r = lds_chunk<16>(sb + St::OR_, tid, 0);
             R[0][0] = r.x; R[0][1] = r.y; R[1][0] = r.z; R[1][1] = r.w;
         }
+        const int64_t f = (int64_t)tile * TILE + tid;
+        const bool live = f < p.N_filters;
         if (DO_U) {
-            float2 v = *reinterpret_cast<const float2 *>(sb + St::OZ + tid * 8);
+            // the stage holds z up to the last whole 16 bytes: only an odd last filter misses its own
+            const bool own = live && (p.N_filters & 1) && f == p.N_filters - 1;
+            float2 v = own ? *reinterpret_cast<const float2 *>(p.z + f * M)
+                           : *reinterpret_cast<const float2 *>(sb + St::OZ + tid * 8);
             z[0] = v.x; z[1] = v.y;
         }
         // The stage is about to be handed back to the TMA engine (async proxy).  A plain barrier
@@ -319,13 +324,15 @@ kf42_f32_kernel(const __grid_constant__ Maps maps, const FastP<4, 2> p)
         if (DO_U) acc ^= __float_as_uint(z[0]) ^ __float_as_uint(z[1]);
         const int never = __syncthreads_and(acc == 0x7fc0beefu);     // every thread has drained the stage
         if (never && p.num_tiles < 0) p.x_out[0] = 0.f;              // keeps `acc` alive; cannot happen
-        if (tid == 0) {
-            int nt = tile + STAGES * gridDim.x;
-            if (nt < p.num_tiles) issue(nt, stage);
+        const int nt = tile + STAGES * gridDim.x;
+        if (nt < p.num_tiles) {
+            if (tid == 0) issue(nt, stage);
+        } else {
+            // this CTA has issued the loads of its last tile: the next launch on the stream may
+            // take the SM slots this grid frees and run its prologue (it waits before touching memory)
+            griddep_launch_dependents();
         }
 
-        const int64_t f = (int64_t)tile * TILE + tid;
-        const bool live = f < p.N_filters;
         int st = BKE_STATUS_OK;
         if (DO_P) {
             reg_predict<float, N>(x, P, F, Q, p.alpha_sq);
@@ -399,62 +406,8 @@ int env_int(const char *name, int dflt)
     return v ? atoi(v) : dflt;
 }
 
-typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                             const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                             CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeFn get_encode()
-{
-    static EncodeFn fn = nullptr;
-    static bool tried = false;
-    if (!tried) {
-        tried = true;
-        void *p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (EncodeFn)p;
-    }
-    return fn;
-}
-
-// rows of `row_elems` floats, `rows` of them; box = TILE rows
-bool make_map_2d(CUtensorMap *m, const void *base, int64_t rows, int row_elems)
-{
-    EncodeFn enc = get_encode();
-    if (!enc) return false;
-    cuuint64_t gdim[2] = {(cuuint64_t)row_elems, (cuuint64_t)rows};
-    cuuint64_t gstride[1] = {(cuuint64_t)row_elems * sizeof(float)};
-    cuuint32_t box[2] = {(cuuint32_t)row_elems, (cuuint32_t)TILE};
-    cuuint32_t estr[2] = {1, 1};
-    int rowb = row_elems * (int)sizeof(float);
-    CUtensorMapSwizzle sw = rowb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                          : rowb == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                          : rowb == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
-                                       : CU_TENSOR_MAP_SWIZZLE_NONE;
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(base), gdim, gstride, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
-}
-
-bool make_map_1d(CUtensorMap *m, const void *base, int64_t elems, int box_elems)
-{
-    EncodeFn enc = get_encode();
-    if (!enc) return false;
-    cuuint64_t gdim[1] = {(cuuint64_t)elems};
-    cuuint64_t gstride[1] = {0};
-    cuuint32_t box[1] = {(cuuint32_t)box_elems};
-    cuuint32_t estr[1] = {1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 1, const_cast<void *>(base), gdim, gstride, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
-}
-
-
 template <int MODE, int SHARED, bool EXTRAS, int STAGES>
-int launch_variant_s(const Maps &maps, const FastP<4, 2> &p, cudaStream_t s, int ctas_per_sm)
+int launch_variant_s(const FastP<4, 2> &p, cudaStream_t s, int ctas_per_sm)
 {
     using St = Stage<float, 4, 2, SHARED != 0>;
     auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, STAGES>;
@@ -468,24 +421,36 @@ int launch_variant_s(const Maps &maps, const FastP<4, 2> &p, cudaStream_t s, int
     }
     int grid = sm_count() * ctas_per_sm;
     if (grid > p.num_tiles) grid = p.num_tiles;
-    kern<<<grid, TILE, smem, s>>>(maps, p);
-    return check_cuda(cudaGetLastError(), "kf42_f32_kernel launch");
+    // programmatic stream serialization: this launch may start while the previous kernel on the
+    // stream drains (the kernel waits with griddepcontrol.wait before it touches memory); under
+    // stream capture it becomes a programmatic edge of the graph
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(TILE);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = s;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return check_cuda(cudaLaunchKernelEx(&cfg, kern, p), "kf42_f32_kernel launch");
 }
 
 template <int MODE, int SHARED, bool EXTRAS>
-int launch_variant(const Maps &maps, const FastP<4, 2> &p, cudaStream_t s)
+int launch_variant(const FastP<4, 2> &p, cudaStream_t s)
 {
     static const int stages_env = env_int("BKE_KF_STAGES", 0);
     static const int ctas_env = env_int("BKE_KF_CTAS", 0);
     if (SHARED) {      // 11 KB per stage
         constexpr int MAXC = SHARED == 2 ? 7 : 4, DEFC = SHARED == 2 ? 5 : 4;
         const int ctas = ctas_env > 0 ? (ctas_env > MAXC ? MAXC : ctas_env) : DEFC;
-        if (stages_env == 3) return launch_variant_s<MODE, SHARED, EXTRAS, 3>(maps, p, s, ctas);
-        return launch_variant_s<MODE, SHARED, EXTRAS, 2>(maps, p, s, ctas);
+        if (stages_env == 3) return launch_variant_s<MODE, SHARED, EXTRAS, 3>(p, s, ctas);
+        return launch_variant_s<MODE, SHARED, EXTRAS, 2>(p, s, ctas);
     }
     const int ctas = ctas_env > 0 ? ctas_env : 3;
-    if (stages_env == 3) return launch_variant_s<MODE, SHARED, EXTRAS, 3>(maps, p, s, ctas > 2 ? 2 : ctas);
-    return launch_variant_s<MODE, SHARED, EXTRAS, 2>(maps, p, s, ctas > 3 ? 3 : ctas);
+    if (stages_env == 3) return launch_variant_s<MODE, SHARED, EXTRAS, 3>(p, s, ctas > 2 ? 2 : ctas);
+    return launch_variant_s<MODE, SHARED, EXTRAS, 2>(p, s, ctas > 3 ? 3 : ctas);
 }
 
 }  // namespace
@@ -502,35 +467,13 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s)
     if (du) { all_shared &= (a.H_stride == 0 && a.R_stride == 0); all_dense &= (a.H_stride != 0 && a.R_stride != 0); }
     if (!all_shared && !all_dense) return BKE_ERR_UNSUPPORTED;
     if (a.n_filters >= (int64_t)1 << 30) return BKE_ERR_UNSUPPORTED;
-    // TMA needs 16-byte aligned global bases
+    // bulk copies and the 16-byte stores need 16-byte aligned global bases
     auto mis = [](const void *p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15u) != 0; };
     if (mis(a.x) || mis(a.P) || mis(a.F) || mis(a.Q) || mis(a.H) || mis(a.R) || mis(a.z) || mis(a.x_out) || mis(a.P_out) ||
         mis(a.x_prior) || mis(a.P_prior) || mis(a.K) || mis(a.S) || mis(a.SI) || (a.y && (reinterpret_cast<uintptr_t>(a.y) & 7u)))
         return BKE_ERR_UNSUPPORTED;
-    if (!get_encode()) return BKE_ERR_UNSUPPORTED;
 
     const int64_t N = a.n_filters;
-    // Tensor maps are pure functions of (base pointer, rows): a per-thread cache re-encodes only
-    // the ones whose array changed since the last call (in a filter loop: just z).
-    static thread_local Maps maps;
-    static thread_local const void *key_ptr[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    static thread_local int64_t key_n[7] = {-1, -1, -1, -1, -1, -1, -1};
-    bool ok = true;
-    auto cached2d = [&](int slot, CUtensorMap *m, const void *ptr, int row_elems) {
-        if (key_ptr[slot] == ptr && key_n[slot] == N) return;
-        ok = ok && make_map_2d(m, ptr, N, row_elems);
-        key_ptr[slot] = ptr; key_n[slot] = ok ? N : -1;
-    };
-    cached2d(0, &maps.x, a.x, 4);
-    cached2d(1, &maps.P, a.P, 16);
-    if (all_dense && dp) { cached2d(2, &maps.F, a.F, 16); cached2d(3, &maps.Q, a.Q, 16); }
-    if (all_dense && du) { cached2d(4, &maps.H, a.H, 8); cached2d(5, &maps.R, a.R, 4); }
-    if (du && !(key_ptr[6] == a.z && key_n[6] == N)) {
-        ok = ok && make_map_1d(&maps.z, a.z, N * 2, TILE * 2);
-        key_ptr[6] = a.z; key_n[6] = ok ? N : -1;
-    }
-    if (!ok) { set_error("cuTensorMapEncodeTiled failed"); return BKE_ERR_CUDA; }
-
     FastP<4, 2> p;
     p.N_filters = N;
     p.num_tiles = (int)((N + TILE - 1) / TILE);
@@ -540,6 +483,7 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s)
         static const int l2_env = env_int("BKE_KF_L2", 1);
         p.l2_hints = l2_env && (N * 80 <= (int64_t)38 << 20) && a.x_out == a.x && a.P_out == a.P;
     }
+    p.x = (const float *)a.x; p.P = (const float *)a.P; p.z = (const float *)a.z;
     p.F = (const float *)a.F; p.Q = (const float *)a.Q; p.H = (const float *)a.H; p.R = (const float *)a.R;
     p.x_out = (float *)a.x_out; p.P_out = (float *)a.P_out;
     p.valid = a.z_valid;
@@ -557,12 +501,12 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s)
 
 #define BKE_DISPATCH(MODE)                                                                   \
     do {                                                                                     \
-        if (host_models) return extras ? launch_variant<MODE, 2, true>(maps, p, s)           \
-                                       : launch_variant<MODE, 2, false>(maps, p, s);         \
-        if (all_shared) return extras ? launch_variant<MODE, 1, true>(maps, p, s)            \
-                                      : launch_variant<MODE, 1, false>(maps, p, s);          \
-        return extras ? launch_variant<MODE, 0, true>(maps, p, s)                            \
-                      : launch_variant<MODE, 0, false>(maps, p, s);                          \
+        if (host_models) return extras ? launch_variant<MODE, 2, true>(p, s)           \
+                                       : launch_variant<MODE, 2, false>(p, s);         \
+        if (all_shared) return extras ? launch_variant<MODE, 1, true>(p, s)            \
+                                      : launch_variant<MODE, 1, false>(p, s);          \
+        return extras ? launch_variant<MODE, 0, true>(p, s)                            \
+                      : launch_variant<MODE, 0, false>(p, s);                          \
     } while (0)
     if (dp && du) BKE_DISPATCH(3);
     if (dp) BKE_DISPATCH(1);

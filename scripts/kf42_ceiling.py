@@ -1,0 +1,173 @@
+"""Where the time of the 4/2 fp32 bank step goes: the card's ceiling for its traffic, and the step's
+fixed cost and streaming rate.
+
+    python scripts/kf42_ceiling.py [--out DIR] [--rounds R]
+
+Prints JSON lines (and writes them to DIR/kf42_ceiling.jsonl with --out):
+
+  card       name, power limit and maximum SM clock (nvidia-smi query)
+  ceiling    scripts/kf42_ceiling.cu: a memory-only kernel that moves exactly the step's 344 B per
+             filter (264 B read, 80 B written in place) with flat coalesced 16-byte accesses, 2^20
+             filters; GB/s and its share of the data sheet's 3.35 TB/s
+  step       the shipped step (KalmanFilter.predict + update, per-filter F/H/Q/R) replayed as CUDA
+             graphs of 4 steps like bench.py, at N = 2^19 .. 2^22 (all above the bound under which
+             the L2 hints are used); per-step time and GB/s for every N
+  fit        t(N) = a + b N over those sizes: a is the fixed cost of a step, 344 B / b its
+             streaming rate
+  shared     the same graph of 4 steps for a 2^20-filter bank whose F/H/Q/R are shared (one model
+             for the bank, carried in the launch parameters)
+
+The ceiling kernel is compiled with nvcc into scripts/kf42_ceiling.so (git-ignored) when that file
+is missing or older than its source.  BKE_LIB_PATH selects the engine library as everywhere else.
+"""
+import argparse
+import ctypes
+import json
+import os
+import shutil
+import subprocess
+import sys
+
+import numpy as np
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(HERE)
+sys.path.insert(0, ROOT)
+
+SRC = os.path.join(HERE, "kf42_ceiling.cu")
+LIB = os.path.join(HERE, "kf42_ceiling.so")
+BYTES = 344                 # per filter-step: x, P, F, Q, H, R, z read (264 B), x, P written (80 B)
+PEAK_GBS = 3350.0           # H100 SXM data sheet, HBM3
+RING = 4                    # steps per graph replay, as in bench.py
+
+
+def build_lib():
+    if os.path.exists(LIB) and os.path.getmtime(LIB) >= os.path.getmtime(SRC):
+        return LIB
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-shared", "-Xcompiler", "-fPIC",
+                    SRC, "-o", LIB + ".tmp"], check=True)
+    os.replace(LIB + ".tmp", LIB)
+    return LIB
+
+
+def card():
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=60)
+        name, power, sm = [s.strip() for s in r.stdout.strip().splitlines()[0].split(",")]
+        return {"name": name, "power_limit": power, "sm_max_clock": sm}
+    except Exception as e:
+        return {"error": "%s: %s" % (type(e).__name__, e)}
+
+
+def time_ms(fn, reps, torch):
+    """Device time of `reps` calls of fn (CUDA events), in ms per call."""
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+def reps_for(n_filters, seconds=0.3):
+    return max(8, int(seconds / (n_filters * BYTES / 2.5e12)))
+
+
+def ceiling(torch, rounds):
+    lib = ctypes.CDLL(build_lib())
+    lib.kf42_traffic.restype = ctypes.c_int
+    lib.kf42_traffic.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_int64, ctypes.c_int, ctypes.c_void_p]
+    N = 1 << 20
+    dev = torch.device("cuda")
+    g = torch.Generator(device=dev).manual_seed(5)
+    arr = {k: torch.randn(N * e, device=dev, generator=g) for k, e in
+           (("x", 4), ("P", 16), ("F", 16), ("Q", 16), ("H", 8), ("R", 4), ("z", 2))}
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    stream = torch.cuda.current_stream().cuda_stream
+    out = {}
+    for per_sm in (4, 8):
+        grid = sms * per_sm
+
+        def run():
+            rc = lib.kf42_traffic(*[arr[k].data_ptr() for k in "xPFQHRz"], N, grid, stream)
+            assert rc == 0, rc
+        for _ in range(5):
+            run()
+        torch.cuda.synchronize()
+        ms = float(np.median([time_ms(run, reps_for(N), torch) for _ in range(rounds)]))
+        gbs = BYTES * N / (ms * 1e-3) / 1e9
+        out["ctas_per_sm_%d" % per_sm] = {"ms": ms, "GBps": gbs, "frac_of_3350": gbs / PEAK_GBS}
+    best = max(out.values(), key=lambda v: v["GBps"])
+    return {"what": "ceiling", "n_filters": N, "bytes_per_filter": BYTES, "ms": best["ms"], "GBps": best["GBps"],
+            "frac_of_3350": best["frac_of_3350"], "by_grid": out}
+
+
+def bank(torch, N, shared=False):
+    from filterpy_b200.kalman import KalmanFilter
+    from filterpy_b200.common import workloads as wl
+    base = 1 << 19
+    w = wl.kf_bank_cv2d(base, seed=1234, steps=RING, dtype=np.float32)
+    r = N // base
+    kf = KalmanFilter(4, 2, n_filters=N, dtype=np.float32, device="cuda", diagnostics=False)
+    kf.x = np.tile(w["x"], (r, 1))
+    kf.P = np.tile(w["P"], (r, 1, 1))
+    for k in "FHQR":
+        setattr(kf, k, w[k][0] if shared else np.tile(w[k], (r, 1, 1)))
+    zs = [torch.from_numpy(np.tile(w["zs"][i], (r, 1))).cuda() for i in range(RING)]
+
+    def ring():
+        for i in range(RING):
+            kf.predict()
+            kf.update(zs[i])
+    return kf, kf.capture(ring)
+
+
+def step_ms(torch, graph, N, rounds):
+    for _ in range(3):
+        graph.replay()
+    torch.cuda.synchronize()
+    reps = max(4, reps_for(N) // RING)
+    return [time_ms(graph.replay, reps, torch) / RING for _ in range(rounds)]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default=None, help="also write the JSON lines to OUT/kf42_ceiling.jsonl")
+    ap.add_argument("--rounds", type=int, default=5, help="timed rounds per measurement (the median is reported)")
+    args = ap.parse_args()
+    import torch
+    assert torch.cuda.is_available(), "kf42_ceiling.py measures on a GPU"
+    lines = [dict(what="card", **card()), dict(what="library", path=os.environ.get("BKE_LIB_PATH") or "in-tree")]
+    lines.append(ceiling(torch, args.rounds))
+    sizes, times = [], []
+    for lg in (19, 20, 21, 22):
+        N = 1 << lg
+        kf, graph = bank(torch, N)
+        t = step_ms(torch, graph, N, args.rounds)
+        ms = float(np.median(t))
+        sizes.append(N); times.append(ms)
+        lines.append({"what": "step", "n_filters": N, "ms": ms, "ms_rounds": t, "GBps": BYTES * N / (ms * 1e-3) / 1e9})
+        del kf, graph
+        torch.cuda.empty_cache()
+    b, a = np.polyfit(np.array(sizes, dtype=np.float64), np.array(times, dtype=np.float64), 1)
+    resid = np.array(times) - (a + b * np.array(sizes))
+    lines.append({"what": "fit", "fixed_us": a * 1e3, "stream_GBps": BYTES / (b * 1e-3) / 1e9,
+                  "stream_frac_of_3350": BYTES / (b * 1e-3) / 1e9 / PEAK_GBS,
+                  "max_abs_residual_us": float(np.abs(resid).max() * 1e3)})
+    N = 1 << 20
+    kf, graph = bank(torch, N, shared=True)
+    t = step_ms(torch, graph, N, args.rounds)
+    lines.append({"what": "shared", "n_filters": N, "ms": float(np.median(t)), "ms_rounds": t})
+    text = "\n".join(json.dumps(l) for l in lines)
+    print(text, flush=True)
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        with open(os.path.join(args.out, "kf42_ceiling.jsonl"), "a") as f:
+            f.write(text + "\n")
+
+
+if __name__ == "__main__":
+    main()
