@@ -56,7 +56,10 @@ class StepGraph(object):
     ring of measurement buffers).  Replaying it re-runs exactly those kernels on the same device
     buffers with one launch: the inner loop of a tracker that refills ``z_buf`` every epoch pays no
     per-kernel launch latency.  Capture needs calls that neither allocate nor synchronise, i.e. banks
-    built with ``diagnostics=False`` and device-resident inputs."""
+    built with ``diagnostics=False`` and device-resident inputs.  One exception to "the same device
+    buffers": a 4/2 float32 bank with symmetric per-filter Q and R is captured reading a packed copy
+    of them, so its Q and R are frozen at capture (``KalmanFilter.capture``); re-capture after
+    changing them."""
 
     def __init__(self, fn, device, warmup=2):
         side = torch.cuda.Stream(device)

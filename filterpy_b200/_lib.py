@@ -22,6 +22,7 @@ BKE_FX_USER = BKE_HX_USER = 100
 EXPORTED_SYMBOLS = [
     "bke_abi_version", "bke_last_error", "bke_device_count",
     "bke_kf_step", "bke_kf_batch_filter", "bke_ukf_step",
+    "bke_kf_sym_models_bytes", "bke_kf_pack_sym_models", "bke_kf_step_sym",
     "bke_resample_workspace_bytes", "bke_systematic_resample", "bke_stratified_resample",
     "bke_weights_sum", "bke_weights_scale", "bke_resample_shard", "bke_resample_normalized",
     "bke_resample_composite_bytes", "bke_resample_shard_compose", "bke_resample_compose_carry", "bke_resample_shard_stage",
@@ -210,6 +211,13 @@ def load():
     lib.bke_device_count.restype = ctypes.c_int
     lib.bke_kf_step.argtypes = [ctypes.POINTER(KfArgs), c_void_p]
     lib.bke_kf_step.restype = ctypes.c_int
+    lib.bke_kf_sym_models_bytes.argtypes = [c_int64]
+    lib.bke_kf_sym_models_bytes.restype = c_size_t
+    lib.bke_kf_pack_sym_models.argtypes = [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p]
+    lib.bke_kf_pack_sym_models.restype = ctypes.c_int
+    lib.bke_kf_step_sym.argtypes = [ctypes.POINTER(KfArgs), c_void_p, c_void_p]
+    lib.bke_kf_step_sym.restype = ctypes.c_int
     lib.bke_kf_batch_filter.argtypes = [ctypes.POINTER(KfBatchArgs), c_void_p]
     lib.bke_kf_batch_filter.restype = ctypes.c_int
     lib.bke_ukf_step.argtypes = [ctypes.POINTER(UkfArgs), c_void_p]

@@ -115,6 +115,38 @@ int bke_kf_step(const bke_kf_args *args, void *stream)
     return launch_kf_any(*args, s);
 }
 
+size_t bke_kf_sym_models_bytes(int64_t n_filters) { return kf_sym_models_bytes(n_filters); }
+
+int bke_kf_pack_sym_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *Q,
+                           const void *R, void *record, int32_t *asymmetric, void *stream)
+{
+    if (n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    if (n_filters > 0 && (!Q || !R || !record)) { set_error("Q, R and record must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if (!asymmetric) { set_error("asymmetric must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if (!(dim_x == 4 && dim_z == 2 && dtype == BKE_F32)) {
+        set_error("packed symmetric models exist for dim_x = 4, dim_z = 2, BKE_F32 only");
+        return BKE_ERR_UNSUPPORTED;
+    }
+    int rc = require_device();
+    if (rc) return rc;
+    return launch_kf_pack_sym(n_filters, Q, R, record, asymmetric, (cudaStream_t)stream);
+}
+
+int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream)
+{
+    int rc = validate_kf(args, true);
+    if (rc) return rc;
+    if (!record) { set_error("record is NULL"); return BKE_ERR_BAD_ARG; }
+    if ((rc = require_device())) return rc;
+    if (args->n_filters == 0) return BKE_OK;
+    g_err[0] = '\0';
+    rc = launch_kf_fast(*args, (cudaStream_t)stream, record);
+    if (rc == BKE_ERR_UNSUPPORTED && g_err[0] == '\0')      // (launch_kf_fast names some causes itself)
+        set_error("the packed symmetric models cover per-filter models of dim_x = 4, dim_z = 2, BKE_F32 banks "
+                  "without control input, on 16-byte aligned arrays");
+    return rc;
+}
+
 int bke_kf_batch_filter(const bke_kf_batch_args *args, void *stream)
 {
     if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }

@@ -15,6 +15,9 @@
 //     prologue runs before griddepcontrol.wait, every global access after it, and a CTA releases
 //     the next launch once it has issued the loads of its last tile.
 // Shared models (stride 0) are read once per thread through the read-only path instead of TMA.
+// A bank whose per-filter Q and R are exactly symmetric may instead hand over a packed copy of their
+// upper triangles (bke_kf_pack_sym_models, SYM = true): one bulk copy per tile replaces the two of
+// Q and R, 52 instead of 80 B per filter, and the lower triangles are rebuilt in registers.
 //
 // Reference arithmetic: filterpy/kalman/kalman_filter.py:471-478, 533-556 (see kf_regtile.cuh).
 #include <stdlib.h>
@@ -90,7 +93,13 @@ __device__ __forceinline__ void st_hint(float *addr, float4 v, uint64_t pol)
 // ---------------------------------------------------------------------------- tile geometry
 constexpr int TILE = 128;       // filters per tile == threads per CTA
 
-template <typename T, int N, int M, bool SHARED = false>
+// The packed symmetric models of a 4/2 bank: one record per tile of TILE filters, structure of arrays,
+// plane k holding word k of every filter: Q00 Q01 Q02 Q03 Q11 Q12 Q13 Q22 Q23 Q33 | R00 R01 R11.
+// Thread t reads word t of each plane (no bank conflicts); a tile's record is SYM_PLANES * TILE * 4 =
+// 6656 B, and the record of the whole bank is padded to whole tiles, so every copy has the same size.
+constexpr int SYM_Q_PLANES = 10, SYM_PLANES = 13;
+
+template <typename T, int N, int M, bool SHARED = false, bool SYM = false>
 struct Stage {
     // byte sizes of one tile of each array
     static constexpr int XB = TILE * N * sizeof(T);
@@ -98,16 +107,17 @@ struct Stage {
     static constexpr int HB = TILE * M * N * sizeof(T);
     static constexpr int RB = TILE * M * M * sizeof(T);
     static constexpr int ZB = TILE * M * sizeof(T);
+    static constexpr int QB = SYM ? TILE * SYM_PLANES * sizeof(T) : PB;    // SYM: the packed record (Q and R)
     // offsets (bulk-copy destinations must be 16-byte aligned; 128 keeps every block on its own lines)
     static constexpr int align_up(int v) { return (v + 127) & ~127; }
     // (a bank that shares its models stages only P, x, z: a third of the bytes, so more stages and CTAs fit)
     static constexpr int OP = 0;
     static constexpr int OF = OP + align_up(PB);
     static constexpr int OQ = OF + (SHARED ? 0 : align_up(PB));
-    static constexpr int OH = OQ + (SHARED ? 0 : align_up(PB));
+    static constexpr int OH = OQ + (SHARED ? 0 : align_up(QB));
     static constexpr int OX = OH + (SHARED ? 0 : align_up(HB));
     static constexpr int OR_ = OX + align_up(XB);
-    static constexpr int OZ = OR_ + (SHARED ? 0 : align_up(RB));
+    static constexpr int OZ = OR_ + (SHARED || SYM ? 0 : align_up(RB));
     static constexpr int BYTES = OZ + align_up(ZB);
 };
 
@@ -156,6 +166,7 @@ struct FastP {
     float alpha_sq;
     const float *x, *P, *z;         // the prior state and the measurements (dense AoS)
     const float *F, *Q, *H, *R;     // per-filter models (SHARED == 0) or the bank's one model (SHARED == 1)
+    const float *sym;               // SYM: the packed record of Q and R (replaces Q, R)
     float Fh[N * N], Qh[N * N], Hh[M * N], Rh[M * M];   // used when SHARED == 2: the shared models ride in the launch
                                                         // parameters, so every product with them reads the constant bank
     float *x_out, *P_out;
@@ -168,12 +179,18 @@ struct FastP {
 // MODE: 3 = predict+update, 1 = predict only, 2 = update only
 // SHARED: 0 = per-filter models (staged by bulk copies), 1 = one model for the bank read from device
 // memory, 2 = one model for the bank carried in the kernel parameters
-template <int MODE, int SHARED, bool EXTRAS, int STAGES>
+// SYM (SHARED == 0 only): Q and R come from the packed record p.sym instead of p.Q, p.R
+template <int MODE, int SHARED, bool EXTRAS, int STAGES, bool SYM = false>
 __global__ void __launch_bounds__(TILE, SHARED == 2 ? 5 : (SHARED ? 4 : 3))
 kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 {
     constexpr int N = 4, M = 2;
-    using St = Stage<float, N, M, SHARED != 0>;
+    static_assert(!(SYM && SHARED), "the packed record holds per-filter models");
+    using St = Stage<float, N, M, SHARED != 0, SYM>;
+    // SYM: the part of a tile's record this MODE reads (the Q planes, the R planes or both)
+    constexpr int SYM_FIRST = (MODE & 1) ? 0 : SYM_Q_PLANES;
+    constexpr int SYM_LAST = (MODE & 2) ? SYM_PLANES : SYM_Q_PLANES;
+    constexpr uint32_t SYM_BYTES = (SYM_LAST - SYM_FIRST) * TILE * 4;
     constexpr bool DO_P = MODE & 1, DO_U = MODE & 2;
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ __align__(8) uint64_t full[STAGES];
@@ -191,8 +208,9 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
         const uint32_t nf = left < TILE ? (uint32_t)left : (uint32_t)TILE;
         const uint32_t zb = (nf * M * 4) & ~15u;
         uint32_t tx = nf * (N + N * N) * 4;
-        if (!SHARED && DO_P) tx += nf * 2 * N * N * 4;
-        if (!SHARED && DO_U) tx += nf * (M * N + M * M) * 4;
+        if (!SHARED && DO_P) tx += nf * (SYM ? 1 : 2) * N * N * 4;
+        if (!SHARED && DO_U) tx += nf * (M * N + (SYM ? 0 : M * M)) * 4;
+        if (SYM) tx += SYM_BYTES;           // the record is padded to whole tiles: always the full planes
         if (DO_U) tx += zb;
         mbar_expect_tx(bar, tx);
         auto load = [&](int off, const float *src, int per_filter, uint32_t bytes, uint64_t pol) {
@@ -203,12 +221,13 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
         load(St::OX, p.x, N, nf * N * 4, pol_last);
         if (!SHARED && DO_P) {
             load(St::OF, p.F, N * N, nf * N * N * 4, pol_first);
-            load(St::OQ, p.Q, N * N, nf * N * N * 4, pol_first);
+            if (!SYM) load(St::OQ, p.Q, N * N, nf * N * N * 4, pol_first);
         }
         if (!SHARED && DO_U) {
             load(St::OH, p.H, M * N, nf * M * N * 4, pol_first);
-            load(St::OR_, p.R, M * M, nf * M * M * 4, pol_first);
+            if (!SYM) load(St::OR_, p.R, M * M, nf * M * M * 4, pol_first);
         }
+        if (SYM) load(St::OQ + SYM_FIRST * TILE * 4, p.sym + SYM_FIRST * TILE, SYM_PLANES, SYM_BYTES, pol_first);
         if (DO_U && zb) load(St::OZ, p.z, M, zb, pol_first);
     };
 
@@ -273,14 +292,30 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
             x[0] = v.x; x[1] = v.y; x[2] = v.z; x[3] = v.w;
         }
         lds_row<N>(sb + St::OP, tid, P);
+        // SYM: word `tid` of plane k of the record; the lower triangles are the same registers
+        const float *rec = reinterpret_cast<const float *>(sb + St::OQ) + tid;
         if (!SHARED && DO_P) {
             lds_row<N>(sb + St::OF, tid, F);
-            lds_row<N>(sb + St::OQ, tid, Q);
+            if (SYM) {
+                int k = 0;
+#pragma unroll
+                for (int i = 0; i < N; i++)
+#pragma unroll
+                    for (int j = i; j < N; j++, k++) Q[i][j] = Q[j][i] = rec[k * TILE];
+            } else {
+                lds_row<N>(sb + St::OQ, tid, Q);
+            }
         }
         if (!SHARED && DO_U) {
             lds_row<M>(sb + St::OH, tid, H);
-            float4 r = lds_chunk<16>(sb + St::OR_, tid, 0);
-            R[0][0] = r.x; R[0][1] = r.y; R[1][0] = r.z; R[1][1] = r.w;
+            if (SYM) {
+                R[0][0] = rec[SYM_Q_PLANES * TILE];
+                R[0][1] = R[1][0] = rec[(SYM_Q_PLANES + 1) * TILE];
+                R[1][1] = rec[(SYM_Q_PLANES + 2) * TILE];
+            } else {
+                float4 r = lds_chunk<16>(sb + St::OR_, tid, 0);
+                R[0][0] = r.x; R[0][1] = r.y; R[1][0] = r.z; R[1][1] = r.w;
+            }
         }
         const int64_t f = (int64_t)tile * TILE + tid;
         const bool live = f < p.N_filters;
@@ -306,11 +341,15 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 #pragma unroll
             for (int j = 0; j < N; j++) acc ^= __float_as_uint(P[i][j]);
         }
+        // (SYM: each loaded word once; folding a mirrored pair would cancel it out of the predicate)
         if (!SHARED && DO_P) {
 #pragma unroll
             for (int i = 0; i < N; i++)
 #pragma unroll
-                for (int j = 0; j < N; j++) acc ^= __float_as_uint(F[i][j]) ^ __float_as_uint(Q[i][j]);
+                for (int j = 0; j < N; j++) {
+                    acc ^= __float_as_uint(F[i][j]);
+                    if (!SYM || j >= i) acc ^= __float_as_uint(Q[i][j]);
+                }
         }
         if (!SHARED && DO_U) {
 #pragma unroll
@@ -318,7 +357,8 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 #pragma unroll
                 for (int j = 0; j < N; j++) acc ^= __float_as_uint(H[a][j]);
 #pragma unroll
-                for (int b = 0; b < M; b++) acc ^= __float_as_uint(R[a][b]);
+                for (int b = 0; b < M; b++)
+                    if (!SYM || b >= a) acc ^= __float_as_uint(R[a][b]);
             }
         }
         if (DO_U) acc ^= __float_as_uint(z[0]) ^ __float_as_uint(z[1]);
@@ -406,11 +446,11 @@ int env_int(const char *name, int dflt)
     return v ? atoi(v) : dflt;
 }
 
-template <int MODE, int SHARED, bool EXTRAS, int STAGES>
+template <int MODE, int SHARED, bool EXTRAS, int STAGES, bool SYM>
 int launch_variant_s(const FastP<4, 2> &p, cudaStream_t s, int ctas_per_sm)
 {
-    using St = Stage<float, 4, 2, SHARED != 0>;
-    auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, STAGES>;
+    using St = Stage<float, 4, 2, SHARED != 0, SYM>;
+    auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, STAGES, SYM>;
     const int smem = STAGES * St::BYTES;
     static bool configured[64] = {false};
     int dev = 0;
@@ -437,7 +477,7 @@ int launch_variant_s(const FastP<4, 2> &p, cudaStream_t s, int ctas_per_sm)
     return check_cuda(cudaLaunchKernelEx(&cfg, kern, p), "kf42_f32_kernel launch");
 }
 
-template <int MODE, int SHARED, bool EXTRAS>
+template <int MODE, int SHARED, bool EXTRAS, bool SYM = false>
 int launch_variant(const FastP<4, 2> &p, cudaStream_t s)
 {
     static const int stages_env = env_int("BKE_KF_STAGES", 0);
@@ -445,18 +485,91 @@ int launch_variant(const FastP<4, 2> &p, cudaStream_t s)
     if (SHARED) {      // 11 KB per stage
         constexpr int MAXC = SHARED == 2 ? 7 : 4, DEFC = SHARED == 2 ? 5 : 4;
         const int ctas = ctas_env > 0 ? (ctas_env > MAXC ? MAXC : ctas_env) : DEFC;
-        if (stages_env == 3) return launch_variant_s<MODE, SHARED, EXTRAS, 3>(p, s, ctas);
-        return launch_variant_s<MODE, SHARED, EXTRAS, 2>(p, s, ctas);
+        if (stages_env == 3) return launch_variant_s<MODE, SHARED, EXTRAS, 3, false>(p, s, ctas);
+        return launch_variant_s<MODE, SHARED, EXTRAS, 2, false>(p, s, ctas);
     }
+    // per-filter models: 33 KB per stage (29.5 KB with the packed record), so 2 stages x 3 CTAs or
+    // 3 x 2 fit the 227 KB of shared memory of an SM either way
     const int ctas = ctas_env > 0 ? ctas_env : 3;
-    if (stages_env == 3) return launch_variant_s<MODE, SHARED, EXTRAS, 3>(p, s, ctas > 2 ? 2 : ctas);
-    return launch_variant_s<MODE, SHARED, EXTRAS, 2>(p, s, ctas > 3 ? 3 : ctas);
+    if (stages_env == 3) return launch_variant_s<MODE, SHARED, EXTRAS, 3, SYM>(p, s, ctas > 2 ? 2 : ctas);
+    return launch_variant_s<MODE, SHARED, EXTRAS, 2, SYM>(p, s, ctas > 3 ? 3 : ctas);
 }
+
+// Pack the per-filter Q [N,4,4] and R [N,2,2] of a bank into the record described at SYM_PLANES, one
+// thread per filter slot (the padding of the last tile is written with zeros), and set *asym when a
+// filter's Q or R differs from its transpose in any bit.
+__global__ void __launch_bounds__(256)
+kf42_pack_sym_kernel(int64_t n_filters, int64_t slots, const float4 *__restrict__ Q, const float4 *__restrict__ R,
+                     float *__restrict__ rec, int32_t *asym)
+{
+    for (int64_t f = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; f < slots; f += (int64_t)gridDim.x * blockDim.x) {
+        float v[SYM_PLANES] = {};
+        bool bad = false;
+        if (f < n_filters) {
+            float q[4][4];
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const float4 r = Q[f * 4 + i];
+                q[i][0] = r.x; q[i][1] = r.y; q[i][2] = r.z; q[i][3] = r.w;
+            }
+            const float4 r = R[f];
+            int k = 0;
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = i; j < 4; j++, k++) {
+                    v[k] = q[i][j];
+                    bad |= __float_as_uint(q[i][j]) != __float_as_uint(q[j][i]);
+                }
+            v[SYM_Q_PLANES] = r.x; v[SYM_Q_PLANES + 1] = r.y; v[SYM_Q_PLANES + 2] = r.w;
+            bad |= __float_as_uint(r.y) != __float_as_uint(r.z);
+        }
+        float *out = rec + (f / TILE) * (SYM_PLANES * TILE) + (f % TILE);
+#pragma unroll
+        for (int k = 0; k < SYM_PLANES; k++) out[k * TILE] = v[k];
+        if (bad) *asym = 1;
+    }
+}
+
+// BKE_KF_SYM = 0 turns the packed record off (both entry points report BKE_ERR_UNSUPPORTED)
+bool sym_enabled()
+{
+    static const int env = env_int("BKE_KF_SYM", 1);
+    return env != 0;
+}
+
+bool misaligned16(const void *p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15u) != 0; }
 
 }  // namespace
 
-int launch_kf_fast(const bke_kf_args &a, cudaStream_t s)
+size_t kf_sym_models_bytes(int64_t n_filters)
 {
+    if (n_filters <= 0) return 0;
+    return (size_t)((n_filters + TILE - 1) / TILE) * SYM_PLANES * TILE * sizeof(float);
+}
+
+int launch_kf_pack_sym(int64_t n_filters, const void *Q, const void *R, void *record, int32_t *asym, cudaStream_t s)
+{
+    if (!sym_enabled()) { set_error("the packed symmetric models are disabled (BKE_KF_SYM=0)"); return BKE_ERR_UNSUPPORTED; }
+    if (n_filters >= (int64_t)1 << 30) { set_error("the packed symmetric models take at most 2^30 filters"); return BKE_ERR_UNSUPPORTED; }
+    if (misaligned16(Q) || misaligned16(R) || misaligned16(record)) {
+        set_error("Q, R and record must be 16-byte aligned");
+        return BKE_ERR_UNSUPPORTED;
+    }
+    if (check_cuda(cudaMemsetAsync(asym, 0, sizeof(int32_t), s), "cudaMemsetAsync")) return BKE_ERR_CUDA;
+    const int64_t slots = (n_filters + TILE - 1) / TILE * TILE;
+    if (slots == 0) return BKE_OK;
+    int64_t grid = (slots + 255) / 256;
+    if (grid > (int64_t)sm_count() * 16) grid = (int64_t)sm_count() * 16;
+    kf42_pack_sym_kernel<<<(int)grid, 256, 0, s>>>(n_filters, slots, (const float4 *)Q, (const float4 *)R,
+                                                   (float *)record, asym);
+    return check_cuda(cudaGetLastError(), "kf42_pack_sym_kernel launch");
+}
+
+int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *sym)
+{
+    if (sym && !sym_enabled()) { set_error("the packed symmetric models are disabled (BKE_KF_SYM=0)"); return BKE_ERR_UNSUPPORTED; }
+    if (sym && misaligned16(sym)) { set_error("record must be 16-byte aligned"); return BKE_ERR_UNSUPPORTED; }
     if (!(a.dtype == BKE_F32 && a.dim_x == 4 && a.dim_z == 2)) return BKE_ERR_UNSUPPORTED;
     if (a.B != nullptr && a.u != nullptr) return BKE_ERR_UNSUPPORTED;
     if (a.flags & BKE_UPDATE_FIRST) return BKE_ERR_UNSUPPORTED;
@@ -466,9 +579,10 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s)
     if (dp) { all_shared &= (a.F_stride == 0 && a.Q_stride == 0); all_dense &= (a.F_stride != 0 && a.Q_stride != 0); }
     if (du) { all_shared &= (a.H_stride == 0 && a.R_stride == 0); all_dense &= (a.H_stride != 0 && a.R_stride != 0); }
     if (!all_shared && !all_dense) return BKE_ERR_UNSUPPORTED;
+    if (sym && !all_dense) return BKE_ERR_UNSUPPORTED;
     if (a.n_filters >= (int64_t)1 << 30) return BKE_ERR_UNSUPPORTED;
     // bulk copies and the 16-byte stores need 16-byte aligned global bases
-    auto mis = [](const void *p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15u) != 0; };
+    const auto mis = misaligned16;
     if (mis(a.x) || mis(a.P) || mis(a.F) || mis(a.Q) || mis(a.H) || mis(a.R) || mis(a.z) || mis(a.x_out) || mis(a.P_out) ||
         mis(a.x_prior) || mis(a.P_prior) || mis(a.K) || mis(a.S) || mis(a.SI) || (a.y && (reinterpret_cast<uintptr_t>(a.y) & 7u)))
         return BKE_ERR_UNSUPPORTED;
@@ -485,6 +599,7 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s)
     }
     p.x = (const float *)a.x; p.P = (const float *)a.P; p.z = (const float *)a.z;
     p.F = (const float *)a.F; p.Q = (const float *)a.Q; p.H = (const float *)a.H; p.R = (const float *)a.R;
+    p.sym = (const float *)sym;
     p.x_out = (float *)a.x_out; p.P_out = (float *)a.P_out;
     p.valid = a.z_valid;
     p.x_prior = (float *)a.x_prior; p.P_prior = (float *)a.P_prior; p.K = (float *)a.K; p.y = (float *)a.y;
@@ -505,6 +620,8 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s)
                                        : launch_variant<MODE, 2, false>(p, s);         \
         if (all_shared) return extras ? launch_variant<MODE, 1, true>(p, s)            \
                                       : launch_variant<MODE, 1, false>(p, s);          \
+        if (sym) return extras ? launch_variant<MODE, 0, true, true>(p, s)             \
+                               : launch_variant<MODE, 0, false, true>(p, s);           \
         return extras ? launch_variant<MODE, 0, true>(p, s)                            \
                       : launch_variant<MODE, 0, false>(p, s);                          \
     } while (0)

@@ -112,6 +112,17 @@ class KalmanFilter(object):
         self._post_alias = False      # True: x_post / P_post are the live x / P (nothing has moved them since the update)
         self._version = 0            # bumped whenever a tensor the kernels read is re-bound
         self._args_cache = {}
+        # Packed copy of per-filter Q and R (bke_kf_pack_sym_models): derived data, valid for one state
+        # of Q and R.  _qr_version counts re-bindings of Q / R and hand-outs of the live tensors;
+        # together with the tensors' own version counters it names that state (_qr_token).
+        self._sym_ok = not self._single and N > 0 and (n, m) == (4, 2) and self._dtype == torch.float32
+        self._sym_buf = None          # the current record, re-packed in place until a captured graph reads it
+        self._sym_pinned = False      # True: a captured graph reads _sym_buf, so it is never written again
+        self._sym_held = []           # earlier records captured graphs read (kept for the bank's lifetime)
+        self._sym_flag = None         # int32 on the device: 1 = the last pack found an asymmetric filter
+        self._sym_state = None        # (token, usable) of _sym_buf's pack
+        self._qr_version = 0
+        self._qr_last = None          # the token of the previous launch
 
     # ------------------------------------------------------------------ helpers
     def _model(self, a, rows, cols, name):
@@ -222,16 +233,20 @@ class KalmanFilter(object):
                 return _Linked(t.cpu().numpy(), self, name)
             # the caller may edit the live tensor in place: a deferred predict must run with the
             # model it was issued with (the reference's predict has already happened), and the
-            # host copy can no longer be trusted
+            # host copy can no longer be trusted, nor can the packed copy of Q and R
             self._flush()
             if self._host.pop(name, None) is not None:
                 self._version += 1
+            if name in "QR":
+                self._qr_version += 1
             return t
 
         def set_(self, v):
             self._flush()                                   # predict(); kf.F = F2; update(): the predict used the OLD F
             self._version += 1
             self._host.pop(name, None)
+            if name in "QR":
+                self._qr_version += 1
             if v is None:
                 setattr(self, priv, None)
                 return
@@ -392,18 +407,95 @@ class KalmanFilter(object):
         self._launch(flags, pend, zt, vt, R, H)
         self._z = zt
 
-    def _call(self, a):
+    def _call(self, a, rec=None):
         if torch.cuda.current_device() == self._device.index:
-            _lib.check(self._lib.bke_kf_step(a, stream_ptr(self._device)))
+            self._step(a, rec)
         else:
             with torch.cuda.device(self._device):
-                _lib.check(self._lib.bke_kf_step(a, stream_ptr(self._device)))
+                self._step(a, rec)
+
+    def _step(self, a, rec):
+        s = stream_ptr(self._device)
+        if rec is not None:
+            rc = self._lib.bke_kf_step_sym(a, ptr(rec), s)
+            if rc != _lib.BKE_ERR_UNSUPPORTED:
+                _lib.check(rc)
+                return
+            # BKE_KF_SYM=0, or arrays the packed kernel does not take (not 16-byte aligned): the dense
+            # models from now on
+            self._sym_ok = False
+            self._sym_drop()
+        _lib.check(self._lib.bke_kf_step(a, s))
+
+    def _capturing(self):
+        if torch.cuda.current_device() == self._device.index:
+            return torch.cuda.is_current_stream_capturing()
+        with torch.cuda.device(self._device):
+            return torch.cuda.is_current_stream_capturing()
+
+    def _sym_drop(self):
+        """Stop using the current record.  One that a captured graph reads is kept, unchanged, for the
+        bank's lifetime (_sym_held); any other is freed once no cached argument struct holds it."""
+        if self._sym_buf is not None and self._sym_pinned:
+            self._sym_held.append(self._sym_buf)
+        self._sym_buf = self._sym_state = None
+        self._sym_pinned = False
+
+    def _sym_record(self):
+        """The packed copy of the per-filter Q and R for a launch with the bank's own models, or None
+        (the kernels then read the dense Q and R).
+
+        The copy is derived data and must never go stale: it is used only while Q and R are in the
+        state it was packed from, i.e. neither re-assigned, nor handed out by their getters, nor edited
+        in place through torch (the tensors' version counters).  It is (re)packed only outside stream
+        capture, and only when Q and R are the same as at the previous launch, so a loop that assigns
+        Q or R every step never pays for a pack (about 132 B per filter, once); a bank with an
+        asymmetric filter is packed once per state of Q and R and then runs on the dense models.
+        A record that a CUDA graph was captured with is never written again: the graph keeps reading
+        the Q and R of its capture (see ``capture``), and a later pack goes to a new record."""
+        if not self._sym_ok:
+            return None
+        F, Q, H, R = self._F, self._Q, self._H, self._R
+        # the packed kernel takes per-filter models only, not a mixture with shared ones
+        if any(t is None or t.dim() != 3 for t in (F, Q, H, R)):
+            self._sym_drop()
+            return None
+        token = (self._qr_version, Q._version, R._version)
+        last, self._qr_last = self._qr_last, token
+        if self._sym_state is not None and self._sym_state[0] == token:
+            if not self._sym_state[1]:
+                return None
+            if not self._sym_pinned and self._capturing():
+                self._sym_pinned = True
+            return self._sym_buf
+        if token != last or self._capturing():
+            return None
+        if self._sym_pinned:
+            self._sym_drop()
+        with torch.cuda.device(self._device):
+            if self._sym_buf is None:
+                nb = self._lib.bke_kf_sym_models_bytes(self.n_filters)
+                self._sym_buf = torch.empty(nb // 4, dtype=torch.float32, device=self._device)
+                self._version += 1                          # the cached argument structs must keep the record alive
+            if self._sym_flag is None:
+                self._sym_flag = torch.empty(1, dtype=torch.int32, device=self._device)
+            rc = self._lib.bke_kf_pack_sym_models(self.n_filters, 4, 2, _lib.BKE_F32, ptr(Q), ptr(R), ptr(self._sym_buf),
+                                                  ptr(self._sym_flag), stream_ptr(self._device))
+            if rc == _lib.BKE_ERR_UNSUPPORTED:
+                self._sym_ok = False
+                self._sym_drop()
+                return None
+            _lib.check(rc)
+            usable = int(self._sym_flag.item()) == 0
+        self._sym_state = (token, usable)
+        return self._sym_buf if usable else None
 
     def _launch(self, flags, pend, zt, vt, R, H):
         # steady state of a filter loop: nothing but z changed since the last identical call ->
         # reuse the argument struct (the Python side of a launch drops to a few microseconds)
         plain = R is None and H is None and (pend is None or (pend.get("u") is None and pend.get("B") is None
                                                                and pend.get("F") is None and pend.get("Q") is None))
+        rec = self._sym_record() if plain else None
         if plain:
             hit = self._args_cache.get(flags)
             if hit is not None and hit[0] == self._version:
@@ -411,7 +503,7 @@ class KalmanFilter(object):
                 a.z = ptr(zt); a.z_valid = ptr(vt)
                 if not (flags & _lib.BKE_DO_UPDATE):
                     self._snapshot_post()                   # a predict on its own is about to move x, P
-                self._call(a)
+                self._call(a, rec)
                 if self.diagnostics and (flags & _lib.BKE_DO_UPDATE):
                     self._post_alias = True
                     if self._single:
@@ -457,6 +549,8 @@ class KalmanFilter(object):
             hm = [self._host[k] for k in "FQHR"]
             a.F_host, a.Q_host, a.H_host, a.R_host = (h.ctypes.data for h in hm)
             keep += hm
+        if self._sym_buf is not None:
+            keep.append(self._sym_buf)
         if self.diagnostics:
             if flags & _lib.BKE_DO_PREDICT:
                 a.x_prior, a.P_prior = ptr(self._x_prior), ptr(self._P_prior)
@@ -466,7 +560,7 @@ class KalmanFilter(object):
                 a.status = ptr(self._status)
         if not (flags & _lib.BKE_DO_UPDATE):
             self._snapshot_post()                           # a predict on its own is about to move x, P
-        self._call(a)
+        self._call(a, rec)
         if plain:
             self._args_cache[flags] = (self._version, a, keep)      # keep: the tensors `a` points into
         if self.diagnostics and (flags & _lib.BKE_DO_UPDATE):
@@ -477,7 +571,13 @@ class KalmanFilter(object):
     def capture(self, fn, warmup=2):
         """Capture ``fn`` — a fixed sequence of ``predict()/update(z_buffer)`` calls on this bank —
         into a CUDA graph; ``.replay()`` re-runs it with a single launch (see ``StepGraph``).  The
-        state is NOT rolled back after the warm-up / capture runs: set ``x`` / ``P`` afterwards."""
+        state is NOT rolled back after the warm-up / capture runs: set ``x`` / ``P`` afterwards.
+
+        A 4/2 float32 bank whose models are all per filter and whose Q and R are exactly symmetric
+        steps from a packed copy of Q and R (DESIGN.md §2): the graph reads the copy taken before
+        the capture, so Q and R are frozen into it.  Re-capture after changing Q or R, whether by
+        assignment or in place; refilling z, x or P (or F, H) in place between replays works as for
+        any graph."""
         self._flush()
         return StepGraph(fn, self._device, warmup)
 

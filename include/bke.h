@@ -115,6 +115,28 @@ typedef struct bke_kf_args {
 
 int bke_kf_step(const bke_kf_args *args, void *stream);
 
+/* Packed symmetric models of a dim_x = 4, dim_z = 2, BKE_F32 bank (per-filter Q and R).
+ * Q and R are covariances: when every filter's Q and R equal their transposes bit for bit, a step
+ * only needs their upper triangles, 52 instead of 80 B per filter.  The record holds them tile-major,
+ * one tile of 128 filters after the other, each tile 13 planes of 128 floats (Q00 Q01 Q02 Q03 Q11
+ * Q12 Q13 Q22 Q23 Q33 R00 R01 R11, plane k holding word k of each filter of the tile), padded to a
+ * whole last tile.
+ *   bke_kf_sym_models_bytes  the size of the record of n_filters filters (the caller allocates it,
+ *                            16-byte aligned);
+ *   bke_kf_pack_sym_models   fills `record` from the dense Q[N,4,4] and R[N,2,2] and sets the device
+ *                            int32 *asymmetric to 0 when every filter is exactly symmetric, 1 when
+ *                            one is not (compared as bits: -0.0 against +0.0 or two NaN payloads
+ *                            count as asymmetric); only in the first case may the record be used;
+ *   bke_kf_step_sym          bke_kf_step with the record standing in for args->Q and args->R (which
+ *                            must still be the per-filter arrays it was packed from, unchanged since);
+ *                            the results are bit-identical to bke_kf_step's.
+ * Both calls return BKE_ERR_UNSUPPORTED for other shapes, dtypes, shared models or misaligned pointers,
+ * and when the environment sets BKE_KF_SYM=0; bke_kf_step is then the call to make. */
+size_t bke_kf_sym_models_bytes(int64_t n_filters);
+int bke_kf_pack_sym_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *Q,
+                           const void *R, void *record, int32_t *asymmetric, void *stream);
+int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream);
+
 /* KalmanFilter.batch_filter over T epochs for a bank (kalman_filter.py:826-993; procedural
  * twin :1664-1788): the time loop runs inside one kernel with the models resident on chip.
  *   zs[T,N,m], zs_valid[T,N] (or NULL)

@@ -6,13 +6,16 @@ fixed cost and streaming rate.
 Prints JSON lines (and writes them to DIR/kf42_ceiling.jsonl with --out):
 
   card       name, power limit and maximum SM clock (nvidia-smi query)
-  ceiling    scripts/kf42_ceiling.cu: a memory-only kernel that moves exactly the step's 344 B per
-             filter (264 B read, 80 B written in place) with flat coalesced 16-byte accesses, 2^20
+  ceiling    scripts/kf42_ceiling.cu: a memory-only kernel that moves exactly the dense step's 344 B
+             per filter (264 B read, 80 B written in place) with flat coalesced 16-byte accesses, 2^20
              filters; GB/s and its share of the data sheet's 3.35 TB/s
+  ceiling_sym  the same twin with Q and R replaced by the packed 52 B-per-filter stream a symmetric
+             bank's step reads instead (bke_kf_pack_sym_models): 316 B per filter
   step       the shipped step (KalmanFilter.predict + update, per-filter F/H/Q/R) replayed as CUDA
              graphs of 4 steps like bench.py, at N = 2^19 .. 2^22 (all above the bound under which
-             the L2 hints are used); per-step time and GB/s for every N
-  fit        t(N) = a + b N over those sizes: a is the fixed cost of a step, 344 B / b its
+             the L2 hints are used); per-step time and GB/s for every N, counted with the bytes the
+             step moves (316 when it reads the packed Q / R, 344 with BKE_KF_SYM=0)
+  fit        t(N) = a + b N over those sizes: a is the fixed cost of a step, bytes / b its
              streaming rate
   shared     the same graph of 4 steps for a 2^20-filter bank whose F/H/Q/R are shared (one model
              for the bank, carried in the launch parameters)
@@ -37,6 +40,7 @@ sys.path.insert(0, ROOT)
 SRC = os.path.join(HERE, "kf42_ceiling.cu")
 LIB = os.path.join(HERE, "kf42_ceiling.so")
 BYTES = 344                 # per filter-step: x, P, F, Q, H, R, z read (264 B), x, P written (80 B)
+BYTES_SYM = 316             # the same with Q and R read as their packed upper triangles (52 B instead of 80)
 PEAK_GBS = 3350.0           # H100 SXM data sheet, HBM3
 RING = 4                    # steps per graph replay, as in bench.py
 
@@ -76,15 +80,16 @@ def reps_for(n_filters, seconds=0.3):
     return max(8, int(seconds / (n_filters * BYTES / 2.5e12)))
 
 
-def ceiling(torch, rounds):
+def ceiling(torch, rounds, sym=False):
     lib = ctypes.CDLL(build_lib())
     lib.kf42_traffic.restype = ctypes.c_int
-    lib.kf42_traffic.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_int64, ctypes.c_int, ctypes.c_void_p]
+    lib.kf42_traffic.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     N = 1 << 20
     dev = torch.device("cuda")
     g = torch.Generator(device=dev).manual_seed(5)
     arr = {k: torch.randn(N * e, device=dev, generator=g) for k, e in
            (("x", 4), ("P", 16), ("F", 16), ("Q", 16), ("H", 8), ("R", 4), ("z", 2))}
+    nbytes = BYTES_SYM if sym else BYTES
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
     stream = torch.cuda.current_stream().cuda_stream
     out = {}
@@ -92,16 +97,17 @@ def ceiling(torch, rounds):
         grid = sms * per_sm
 
         def run():
-            rc = lib.kf42_traffic(*[arr[k].data_ptr() for k in "xPFQHRz"], N, grid, stream)
+            rc = lib.kf42_traffic(*[arr[k].data_ptr() for k in "xPFQHRz"], N, grid, int(sym), stream)
             assert rc == 0, rc
         for _ in range(5):
             run()
         torch.cuda.synchronize()
         ms = float(np.median([time_ms(run, reps_for(N), torch) for _ in range(rounds)]))
-        gbs = BYTES * N / (ms * 1e-3) / 1e9
+        gbs = nbytes * N / (ms * 1e-3) / 1e9
         out["ctas_per_sm_%d" % per_sm] = {"ms": ms, "GBps": gbs, "frac_of_3350": gbs / PEAK_GBS}
     best = max(out.values(), key=lambda v: v["GBps"])
-    return {"what": "ceiling", "n_filters": N, "bytes_per_filter": BYTES, "ms": best["ms"], "GBps": best["GBps"],
+    return {"what": "ceiling_sym" if sym else "ceiling", "n_filters": N, "bytes_per_filter": nbytes, "ms": best["ms"],
+            "GBps": best["GBps"],
             "frac_of_3350": best["frac_of_3350"], "by_grid": out}
 
 
@@ -142,20 +148,25 @@ def main():
     assert torch.cuda.is_available(), "kf42_ceiling.py measures on a GPU"
     lines = [dict(what="card", **card()), dict(what="library", path=os.environ.get("BKE_LIB_PATH") or "in-tree")]
     lines.append(ceiling(torch, args.rounds))
+    lines.append(ceiling(torch, args.rounds, sym=True))
     sizes, times = [], []
+    moved = BYTES
     for lg in (19, 20, 21, 22):
         N = 1 << lg
         kf, graph = bank(torch, N)
         t = step_ms(torch, graph, N, args.rounds)
         ms = float(np.median(t))
         sizes.append(N); times.append(ms)
-        lines.append({"what": "step", "n_filters": N, "ms": ms, "ms_rounds": t, "GBps": BYTES * N / (ms * 1e-3) / 1e9})
+        packed = kf._sym_state is not None and kf._sym_state[1]
+        moved = BYTES_SYM if packed else BYTES
+        lines.append({"what": "step", "n_filters": N, "packed_QR": packed, "bytes_per_filter": moved, "ms": ms,
+                      "ms_rounds": t, "GBps": moved * N / (ms * 1e-3) / 1e9})
         del kf, graph
         torch.cuda.empty_cache()
     b, a = np.polyfit(np.array(sizes, dtype=np.float64), np.array(times, dtype=np.float64), 1)
     resid = np.array(times) - (a + b * np.array(sizes))
-    lines.append({"what": "fit", "fixed_us": a * 1e3, "stream_GBps": BYTES / (b * 1e-3) / 1e9,
-                  "stream_frac_of_3350": BYTES / (b * 1e-3) / 1e9 / PEAK_GBS,
+    lines.append({"what": "fit", "fixed_us": a * 1e3, "stream_GBps": moved / (b * 1e-3) / 1e9,
+                  "stream_frac_of_3350": moved / (b * 1e-3) / 1e9 / PEAK_GBS,
                   "max_abs_residual_us": float(np.abs(resid).max() * 1e3)})
     N = 1 << 20
     kf, graph = bank(torch, N, shared=True)
