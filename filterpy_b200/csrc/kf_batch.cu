@@ -174,9 +174,8 @@ int launch_reg(const bke_kf_batch_args &a, cudaStream_t s)
     p.status = k.status;
     int64_t grid = (p.N + 127) / 128;
     // an epoch's slice of every output array must start on a 16-byte boundary for the bulk copies (the arrays
-    // themselves are checked by the caller); BKE_BATCH_DIRECT=1 keeps the per-thread stores (A/B measurements)
-    static const bool direct = [] { const char *e = getenv("BKE_BATCH_DIRECT"); return e && e[0] == '1'; }();
-    const bool staged = !direct && ((size_t)p.N * N * sizeof(T)) % 16 == 0 && p.N >= 32;
+    // themselves are checked by the caller); otherwise every thread stores its own outputs
+    const bool staged = ((size_t)p.N * N * sizeof(T)) % 16 == 0 && p.N >= 32;
     if (staged) {
         constexpr int smem = 4 * 2 * BatchStage<T, N>::BYTES;
         auto kern = kf_batch_kernel<T, N, M, true>;

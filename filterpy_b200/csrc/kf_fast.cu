@@ -180,8 +180,14 @@ struct FastP {
 // SHARED: 0 = per-filter models (staged by bulk copies), 1 = one model for the bank read from device
 // memory, 2 = one model for the bank carried in the kernel parameters
 // SYM (SHARED == 0 only): Q and R come from the packed record p.sym instead of p.Q, p.R
-template <int MODE, int SHARED, bool EXTRAS, int STAGES, bool SYM = false>
-__global__ void __launch_bounds__(TILE, SHARED == 2 ? 5 : (SHARED ? 4 : 3))
+// Each CTA keeps STAGES tiles in flight.  Resident CTAs per SM: 3 with per-filter models (33 KB per
+// stage, 29.5 KB with the packed record), 4 with one shared model (11 KB per stage), 5 when that model
+// rides in the launch parameters.
+constexpr int STAGES = 2;
+constexpr int kf42_ctas_per_sm(int shared) { return shared == 2 ? 5 : (shared ? 4 : 3); }
+
+template <int MODE, int SHARED, bool EXTRAS, bool SYM = false>
+__global__ void __launch_bounds__(TILE, kf42_ctas_per_sm(SHARED))
 kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 {
     constexpr int N = 4, M = 2;
@@ -438,19 +444,19 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 }
 
 // ---------------------------------------------------------------------------- host side
-// tuning knobs (environment, read once): BKE_KF_STAGES in {2,3}, BKE_KF_CTAS = resident CTAs per SM,
-// BKE_KF_L2 = 0 disables the L2 eviction-priority hints
+// switches (environment, read once): BKE_KF_L2 = 0 disables the L2 eviction-priority hints,
+// BKE_KF_SYM = 0 the packed record, BKE_KF_HOST_MODELS = 0 the shared models in the launch parameters
 int env_int(const char *name, int dflt)
 {
     const char *v = getenv(name);
     return v ? atoi(v) : dflt;
 }
 
-template <int MODE, int SHARED, bool EXTRAS, int STAGES, bool SYM>
-int launch_variant_s(const FastP<4, 2> &p, cudaStream_t s, int ctas_per_sm)
+template <int MODE, int SHARED, bool EXTRAS, bool SYM = false>
+int launch_variant(const FastP<4, 2> &p, cudaStream_t s)
 {
     using St = Stage<float, 4, 2, SHARED != 0, SYM>;
-    auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, STAGES, SYM>;
+    auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, SYM>;
     const int smem = STAGES * St::BYTES;
     static bool configured[64] = {false};
     int dev = 0;
@@ -459,7 +465,7 @@ int launch_variant_s(const FastP<4, 2> &p, cudaStream_t s, int ctas_per_sm)
         if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
         if (dev >= 0 && dev < 64) configured[dev] = true;
     }
-    int grid = sm_count() * ctas_per_sm;
+    int grid = sm_count() * kf42_ctas_per_sm(SHARED);
     if (grid > p.num_tiles) grid = p.num_tiles;
     // programmatic stream serialization: this launch may start while the previous kernel on the
     // stream drains (the kernel waits with griddepcontrol.wait before it touches memory); under
@@ -475,24 +481,6 @@ int launch_variant_s(const FastP<4, 2> &p, cudaStream_t s, int ctas_per_sm)
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     return check_cuda(cudaLaunchKernelEx(&cfg, kern, p), "kf42_f32_kernel launch");
-}
-
-template <int MODE, int SHARED, bool EXTRAS, bool SYM = false>
-int launch_variant(const FastP<4, 2> &p, cudaStream_t s)
-{
-    static const int stages_env = env_int("BKE_KF_STAGES", 0);
-    static const int ctas_env = env_int("BKE_KF_CTAS", 0);
-    if (SHARED) {      // 11 KB per stage
-        constexpr int MAXC = SHARED == 2 ? 7 : 4, DEFC = SHARED == 2 ? 5 : 4;
-        const int ctas = ctas_env > 0 ? (ctas_env > MAXC ? MAXC : ctas_env) : DEFC;
-        if (stages_env == 3) return launch_variant_s<MODE, SHARED, EXTRAS, 3, false>(p, s, ctas);
-        return launch_variant_s<MODE, SHARED, EXTRAS, 2, false>(p, s, ctas);
-    }
-    // per-filter models: 33 KB per stage (29.5 KB with the packed record), so 2 stages x 3 CTAs or
-    // 3 x 2 fit the 227 KB of shared memory of an SM either way
-    const int ctas = ctas_env > 0 ? ctas_env : 3;
-    if (stages_env == 3) return launch_variant_s<MODE, SHARED, EXTRAS, 3, SYM>(p, s, ctas > 2 ? 2 : ctas);
-    return launch_variant_s<MODE, SHARED, EXTRAS, 2, SYM>(p, s, ctas > 3 ? 3 : ctas);
 }
 
 // Pack the per-filter Q [N,4,4] and R [N,2,2] of a bank into the record described at SYM_PLANES, one

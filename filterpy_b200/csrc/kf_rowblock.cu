@@ -7,16 +7,15 @@
 //     a filter (broadcast), 8-byte words of different filters fall into different banks;
 //   * per warp, FPW = 32/G filters form a tile; ONE lane pulls the tile's x, P, F, Q, H, R, z blocks
 //     (contiguous byte ranges of the dense AoS arrays) with 1-D bulk TMA copies
-//     (cp.async.bulk.shared::cluster.global, SASS UBLKCP) into a 2-stage ring with an mbarrier per
-//     stage; every warp runs its own ring (no block barriers anywhere);
+//     (cp.async.bulk.shared::cluster.global, SASS UBLKCP) into its own stage with an mbarrier; every
+//     warp runs on its own (no block barriers anywhere);
 //   * intermediates reuse the stage: P' overwrites P, (I-KH) overwrites F, K / PH' overwrite Q;
-//   * the posterior rows go to a small staging buffer and leave with bulk TMA stores
+//   * the posterior rows overwrite the stage's x / P slots and leave with bulk TMA stores
 //     (cp.async.bulk.global.shared::cta); the cross-proxy fence that publishes them also orders
 //     every earlier shared-memory read before the stage is handed back to the TMA engine.
 //
 // Arithmetic per filter: filterpy/kalman/kalman_filter.py:471-478 (predict) and :533-556 (update,
 // Joseph form), reference @ 3b51149.  Algorithmic bytes per filter-step (9/3 fp64): 3048.
-#include <stdlib.h>
 #include <type_traits>
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
@@ -86,7 +85,12 @@ constexpr int pick_fpw(int g)
     return 0;
 }
 
-template <typename T, int N, int M, int RPL, int RB_STAGES>
+// One stage per warp and 8 warps per CTA, one CTA per SM: on 9/3 fp64 two warps per scheduler (the FP64
+// pipe of one warp's dependent DFMA chains is covered by the other) beat a 2-stage ring with 4 warps.
+// (9 warps fit the shared memory but cap the kernel at 168 registers.)
+constexpr int RB_STAGES = 1, RB_WARPS = 8;
+
+template <typename T, int N, int M, int RPL>
 struct RbGeom {
     static constexpr int G = N / RPL;                 // lanes per filter
     static constexpr int FPW = pick_fpw<T, N, M>(G);  // filters per warp tile
@@ -104,10 +108,8 @@ struct RbGeom {
     static constexpr int OR_ = OH + a16(HB);
     static constexpr int OZ = OR_ + a16(RBY);
     static constexpr int STAGE = a16(OZ + a16(ZB));
-    // posterior staging (x then P): a separate buffer with a 2-stage ring; with ONE stage per warp
-    // the posterior is staged in the stage's own x / P slots (more warps fit an SM instead)
-    static constexpr int OUT = RB_STAGES > 1 ? a16(XB) + a16(PB) : 0;
-    static constexpr int WARP_BYTES = RB_STAGES * STAGE + OUT;
+    // the posterior is staged in the stage's own x / P slots
+    static constexpr int WARP_BYTES = RB_STAGES * STAGE;
     // one copy of F, Q, H, R per warp for banks that share their models (kept for the whole launch)
     static constexpr int SH_ELEMS = 2 * N * N + M * N + M * M;
     static constexpr int SH_BYTES = a16(SH_ELEMS * (int)sizeof(T));
@@ -133,20 +135,19 @@ struct RbGeom {
 // loaded nor computed)
 // SHARED: F, H, Q, R are one matrix each for the whole bank (stride 0): every warp keeps a copy in
 // shared memory for the launch and the tiles carry only x, P, z
-template <typename T, int N, int M, int RPL, int RB_STAGES, int RB_WARPS, bool EXTRAS, int MODE, bool SHARED>
+template <typename T, int N, int M, int RPL, bool EXTRAS, int MODE, bool SHARED>
 __global__ void __launch_bounds__(RB_WARPS * 32, 1) kf_rowblock_kernel(RbP<T> p)
 {
-    using Gm = RbGeom<T, N, M, RPL, RB_STAGES>;
+    using Gm = RbGeom<T, N, M, RPL>;
     constexpr int G = Gm::G, FPW = Gm::FPW;
     extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ __align__(8) uint64_t bars[RB_WARPS][RB_STAGES];
+    __shared__ __align__(8) uint64_t bars[RB_WARPS];
 
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     constexpr int WB = Gm::WARP_BYTES + (EXTRAS ? Gm::EX_BYTES : 0);
     unsigned char *wbase = smem + (size_t)wib * WB;
-    unsigned char *outb = wbase + RB_STAGES * Gm::STAGE;
     unsigned char *exb = wbase + Gm::WARP_BYTES;             // EXTRAS: staging of K, y, S, SI, log-likelihood
-    uint64_t *bar = bars[wib];
+    uint64_t *bar = &bars[wib];
     const bool active = lane < FPW * G;
     const int fl = active ? lane / G : FPW - 1;            // filter within the tile (idle lanes mirror the last one)
     const int rb = active ? lane % G : 0;
@@ -216,8 +217,8 @@ __global__ void __launch_bounds__(RB_WARPS * 32, 1) kf_rowblock_kernel(RbP<T> p)
         const T *rF = SHARED ? shF : sF;            // the MODELS F, Q (sF / sQ are also scratch for I - K H, K, P H')
         const T *rQ = SHARED ? shQ : sQ;
         const T *sz = reinterpret_cast<const T *>(sb + Gm::OZ) + fl * M;
-        unsigned char *out_x = RB_STAGES > 1 ? outb : sb + Gm::OX;
-        unsigned char *out_P = RB_STAGES > 1 ? outb + Gm::a16(Gm::XB) : sb + Gm::OP;
+        unsigned char *out_x = sb + Gm::OX;
+        unsigned char *out_P = sb + Gm::OP;
         T *ox = reinterpret_cast<T *>(out_x) + fl * N;
         T *oP = reinterpret_cast<T *>(out_P) + fl * N * N;
         const int64_t f = tile * FPW + fl;
@@ -286,7 +287,7 @@ __global__ void __launch_bounds__(RB_WARPS * 32, 1) kf_rowblock_kernel(RbP<T> p)
         if (EXTRAS && (p.x_prior || p.P_prior)) {
             // optional outputs: the prior sits in the stage exactly as x_prior / P_prior want it (FPW filters,
             // dense) — two bulk stores; they have the whole update to read the stage before the posterior
-            // (1 stage) or the next tile's loads (ring) overwrite it
+            // overwrites it
             fence_proxy_async();
             __syncwarp();
             if (lane == 0) {
@@ -502,9 +503,8 @@ __global__ void __launch_bounds__(RB_WARPS * 32, 1) kf_rowblock_kernel(RbP<T> p)
             }
         }
         // ---------------- posterior rows -> staging -> bulk TMA store ---------------------------
-        // the previous tile's stores have read the staging buffer (ring) / the prior's stores have read the
-        // stage slots the posterior is about to overwrite (one stage, optional outputs)
-        if (lane == 0 && ((RB_STAGES > 1 && it > 0) || (EXTRAS && RB_STAGES == 1))) bulk_wait_read();
+        // the prior's stores (optional outputs) have read the stage slots the posterior is about to overwrite
+        if (lane == 0 && EXTRAS) bulk_wait_read();
         __syncwarp();                                       // every lane is done with P', (I-KH), K in the stage
         if (active) {
 #pragma unroll
@@ -529,9 +529,8 @@ __global__ void __launch_bounds__(RB_WARPS * 32, 1) kf_rowblock_kernel(RbP<T> p)
                 if (Gm::LL_BULK && p.ll) bulk_store(p.ll + f0, exb + Gm::ELL, Gm::LLB);
             }
             bulk_commit();
-            // the stores have read the stage (one stage) / the stage's prior and the staging area (optional
-            // outputs): it may be refilled
-            if (RB_STAGES == 1 || EXTRAS) bulk_wait_read();
+            // the stores have read the stage (and the staging area of the optional outputs): it may be refilled
+            bulk_wait_read();
             const int64_t nt = tile + RB_STAGES * wstride;
             if (nt < tiles) issue(nt, stage);
         }
@@ -540,11 +539,11 @@ __global__ void __launch_bounds__(RB_WARPS * 32, 1) kf_rowblock_kernel(RbP<T> p)
     if (lane == 0) bulk_wait_all();
 }
 
-template <typename T, int N, int M, int RPL, int RB_STAGES, int RB_WARPS>
+template <typename T, int N, int M, int RPL>
 int launch_rb(const bke_kf_args &a, cudaStream_t s)
 {
     const int mode = (int)(a.flags & (BKE_DO_PREDICT | BKE_DO_UPDATE));
-    using Gm = RbGeom<T, N, M, RPL, RB_STAGES>;
+    using Gm = RbGeom<T, N, M, RPL>;
     const int64_t Nmain = (a.n_filters / Gm::FPW) * Gm::FPW;
     const int64_t rem = a.n_filters - Nmain;
     if (Nmain > 0) {
@@ -559,14 +558,14 @@ int launch_rb(const bke_kf_args &a, cudaStream_t s)
         // every model the call reads is shared by the bank (stride 0)?  (a mix goes to the catch-all kernel)
         const bool dp = a.flags & BKE_DO_PREDICT, du = a.flags & BKE_DO_UPDATE;
         const bool shared = (!dp || (a.F_stride == 0 && a.Q_stride == 0)) && (!du || (a.H_stride == 0 && a.R_stride == 0));
-        auto kern = extras ? kf_rowblock_kernel<T, N, M, RPL, RB_STAGES, RB_WARPS, true, 3, false>
-                           : kf_rowblock_kernel<T, N, M, RPL, RB_STAGES, RB_WARPS, false, 3, false>;
-        if (mode == 1) kern = kf_rowblock_kernel<T, N, M, RPL, RB_STAGES, RB_WARPS, true, 1, false>;     // the single-mode and the
-        if (mode == 2) kern = kf_rowblock_kernel<T, N, M, RPL, RB_STAGES, RB_WARPS, true, 2, false>;     // shared-model kernels always
+        auto kern = extras ? kf_rowblock_kernel<T, N, M, RPL, true, 3, false>
+                           : kf_rowblock_kernel<T, N, M, RPL, false, 3, false>;
+        if (mode == 1) kern = kf_rowblock_kernel<T, N, M, RPL, true, 1, false>;     // the single-mode and the
+        if (mode == 2) kern = kf_rowblock_kernel<T, N, M, RPL, true, 2, false>;     // shared-model kernels always
         if (shared) {                                                                                     // carry the optional outputs
-            kern = kf_rowblock_kernel<T, N, M, RPL, RB_STAGES, RB_WARPS, true, 3, true>;
-            if (mode == 1) kern = kf_rowblock_kernel<T, N, M, RPL, RB_STAGES, RB_WARPS, true, 1, true>;
-            if (mode == 2) kern = kf_rowblock_kernel<T, N, M, RPL, RB_STAGES, RB_WARPS, true, 2, true>;
+            kern = kf_rowblock_kernel<T, N, M, RPL, true, 3, true>;
+            if (mode == 1) kern = kf_rowblock_kernel<T, N, M, RPL, true, 1, true>;
+            if (mode == 2) kern = kf_rowblock_kernel<T, N, M, RPL, true, 2, true>;
         }
         const bool kern_extras = extras || mode != 3 || shared;      // the instance selected above carries them
         const int smem = RB_WARPS * (Gm::WARP_BYTES + (kern_extras ? Gm::EX_BYTES : 0) + (shared ? Gm::SH_BYTES : 0));
@@ -626,25 +625,20 @@ int launch_kf_rowblock(const bke_kf_args &a, cudaStream_t s)
     // the optional outputs leave with bulk stores too
     if (!(al16(a.x_prior) && al16(a.P_prior) && al16(a.K) && al16(a.y) && al16(a.S) && al16(a.SI) && al16(a.log_likelihood))) return BKE_ERR_UNSUPPORTED;
     const int n = a.dim_x, m = a.dim_z;
-    // 9/3 fp64: one stage per warp and 8 warps per SM (two per scheduler: the FP64 pipe of one warp's
-    // dependent DFMA chains is covered by the other) beat a 2-stage ring with 4 warps; BKE_RB_RING=1
-    // selects the ring for comparison.
-    static const bool ring = getenv("BKE_RB_RING") && atoi(getenv("BKE_RB_RING")) != 0;
     if (a.dtype == BKE_F64) {
-        // (9 warps fit the shared memory but cap the kernel at 168 registers)
-        if (n == 9 && m == 3) return ring ? launch_rb<double, 9, 3, 3, 2, 4>(a, s) : launch_rb<double, 9, 3, 3, 1, 8>(a, s);
-        if (n == 4 && m == 2) return ring ? launch_rb<double, 4, 2, 2, 2, 4>(a, s) : launch_rb<double, 4, 2, 2, 1, 8>(a, s);
-        if (n == 6 && m == 3) return ring ? launch_rb<double, 6, 3, 3, 2, 4>(a, s) : launch_rb<double, 6, 3, 3, 1, 8>(a, s);
+        if (n == 9 && m == 3) return launch_rb<double, 9, 3, 3>(a, s);
+        if (n == 4 && m == 2) return launch_rb<double, 4, 2, 2>(a, s);
+        if (n == 6 && m == 3) return launch_rb<double, 6, 3, 3>(a, s);
         // dim_x = 16: one row per lane, 16 lanes per filter, 2 filters per warp tile
-        if (n == 16 && m == 4) return launch_rb<double, 16, 4, 1, 1, 8>(a, s);
-        if (n == 16 && m == 2) return launch_rb<double, 16, 2, 1, 1, 8>(a, s);
+        if (n == 16 && m == 4) return launch_rb<double, 16, 4, 1>(a, s);
+        if (n == 16 && m == 2) return launch_rb<double, 16, 2, 1>(a, s);
     } else {
-        if (n == 16 && m == 4) return launch_rb<float, 16, 4, 2, 1, 8>(a, s);   // two rows per lane, 4 filters per warp tile
-        if (n == 16 && m == 2) return launch_rb<float, 16, 2, 2, 1, 8>(a, s);
+        if (n == 16 && m == 4) return launch_rb<float, 16, 4, 2>(a, s);   // two rows per lane, 4 filters per warp tile
+        if (n == 16 && m == 2) return launch_rb<float, 16, 2, 2>(a, s);
         // dim_x = 32: one row per lane, the whole warp on one filter (the update half of the tensor-core predict, kf_tc.cu)
-        if (n == 32 && m == 4) return launch_rb<float, 32, 4, 1, 1, 8>(a, s);
-        if (n == 6 && m == 3) return ring ? launch_rb<float, 6, 3, 3, 2, 4>(a, s) : launch_rb<float, 6, 3, 3, 1, 8>(a, s);
-        if (n == 9 && m == 3) return launch_rb<float, 9, 3, 3, 1, 8>(a, s);        // 8 filters per warp tile (see pick_fpw)
+        if (n == 32 && m == 4) return launch_rb<float, 32, 4, 1>(a, s);
+        if (n == 6 && m == 3) return launch_rb<float, 6, 3, 3>(a, s);
+        if (n == 9 && m == 3) return launch_rb<float, 9, 3, 3>(a, s);        // 8 filters per warp tile (see pick_fpw)
     }
     return BKE_ERR_UNSUPPORTED;
 }

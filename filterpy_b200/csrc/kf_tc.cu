@@ -438,12 +438,9 @@ int launch_t(const TcP &p, cudaStream_t s)
         if (dev >= 0 && dev < 64) configured[dev] = true;
     }
     const int64_t tiles = (p.N * NX + 127) / 128;
-    // CTAs per SM: registers (launch bounds) and shared memory (+1 KB the runtime reserves per CTA);
-    // BKE_KF_TC_CTAS overrides (tuning)
-    static const int env_ctas = [] { const char *e = getenv("BKE_KF_TC_CTAS"); return e ? atoi(e) : 0; }();
+    // CTAs per SM: registers (launch bounds) and shared memory (+1 KB the runtime reserves per CTA)
     int occ = tc_ctas(NX, M);
     if (occ > (227 * 1024) / (G::SMEM + 1024)) occ = (227 * 1024) / (G::SMEM + 1024);
-    if (env_ctas > 0 && env_ctas < occ) occ = env_ctas;
     const int64_t cap = (int64_t)sm_count() * occ;
     kf_cov_tc_kernel<NX, M><<<(unsigned)(tiles < cap ? tiles : cap), 128, G::SMEM, s>>>(p);
     return check_cuda(cudaGetLastError(), "kf_cov_tc_kernel launch");

@@ -361,53 +361,8 @@ struct MapsShared {
 
 // Fast kernel: every tile whose adds are all clean and tie-free in ONE binade (decided from the two
 // approximate tile prefixes and the elements themselves) gets its map as a plain int64 sum, straight
-// from the striped registers.  Everything else is queued for the general kernel.
-__global__ void __launch_bounds__(BLOCK, 3) k_tile_maps_fast(Params p)
-{
-    __shared__ i64 shi[BLOCK / 32 + 1];
-    if (p.ws.hdr->fallback) return;
-    const int T = p.ws.T;
-    double2 g[IPT / 2], gn[IPT / 2];
-    if ((int)blockIdx.x < T) fetch_tile(p, blockIdx.x, gn);
-    for (int t = blockIdx.x; t < T; t += gridDim.x) {
-#pragma unroll
-        for (int i = 0; i < IPT / 2; i++) g[i] = gn[i];
-        if (t + (int)gridDim.x < T) fetch_tile(p, t + gridDim.x, gn);     // next tile's loads fly during this tile
-        const double tp = p.ws.tile_prefix[t], tp_next = p.ws.tile_prefix[t + 1];
-        int e0;
-        const bool tile_clean = clean_add(tp, tp_next, p.eb, &e0);     // the whole tile stays deep inside binade e0
-        const i64 base = (i64)e0 << 52;
-        const double B0 = __longlong_as_double(base), B1 = __longlong_as_double(base + 1);
-        i64 acc = 0;
-        bool ok = tile_clean, nz = false;
-#pragma unroll
-        for (int i = 0; i < IPT / 2; i++) {
-            const double w2[2] = {g[i].x, g[i].y};
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const i64 d0 = __double_as_longlong(__dadd_rn(B0, w2[h])) - base;
-                const i64 d1 = __double_as_longlong(__dadd_rn(B1, w2[h])) - (base + 1);
-                ok = ok && (d0 == d1);
-                nz = nz || (w2[h] != 0.0);
-                acc += d0;
-            }
-        }
-        if (__syncthreads_and(ok)) {
-            i64 total;
-            block_excl_scan_i64(acc, &total, shi);
-            const int any_nz = __syncthreads_or(nz);
-            if (threadIdx.x == 0) {
-                p.ws.tile_k[t] = any_nz ? e0 : K_ID; p.ws.tile_d[t] = total; p.ws.tile_t[t] = 0;
-                p.ws.tile_slot[t] = SLOT_FAST;
-            }
-        } else if (threadIdx.x == 0) {
-            p.ws.slow_list[atomicAdd(&p.ws.hdr->n_slow, 1)] = t;
-        }
-    }
-}
-
-// The same, one tile per CTA and no register double-buffer (the default): fewer registers, more resident CTAs —
-// the way pass A reaches the HBM roofline.
+// from the striped registers.  Everything else is queued for the general kernel.  One tile per CTA and no
+// register double-buffer: few registers, many resident CTAs — the way pass A reaches the HBM roofline.
 __global__ void __launch_bounds__(BLOCK, 5) k_tile_maps_fast1(Params p)
 {
     __shared__ i64 shi[BLOCK / 32 + 1];
@@ -452,7 +407,7 @@ __global__ void __launch_bounds__(BLOCK, 5) k_tile_maps_fast1(Params p)
 // word (value with the two low mantissa bits replaced by a flag: 1 = aggregate, 2 = inclusive prefix;
 // the perturbation is far inside the classification margin eb), warp 0 looks back over the earlier
 // tiles' words for the approximate exclusive prefix (decoupled look-back, one warp-wide window of 32
-// tiles per poll), and the fast-path map of k_tile_maps_fast is then computed from the registers the
+// tiles per poll), and the fast-path map of k_tile_maps_fast1 is then computed from the registers the
 // loads landed in.  The approximate prefixes only have to be within eb of the exact running sum, which
 // holds for any summation order of non-negative terms.
 constexpr u64 ST_AGG = 1, ST_INCL = 2;
@@ -1224,8 +1179,8 @@ __global__ void __launch_bounds__(BLOCK, 2) k_emit_fast(Params p)
 // conflict-free LDS.128) while the consumers work on the current one.  Expansion: every particle with
 // >= 1 copies stores (local index + 1) at its first output slot of a zeroed window, a max-scan over the
 // slots fills the runs (no divergent copy loop) and every thread leaves with 16-byte stores of 20
-// consecutive indexes.  (The same consumer code is the emit phase of the experimental single-pass
-// kernel, csrc/resample_fused.cu.)
+// consecutive indexes.  (The same consumer code is the emit phase of the single-pass kernel behind
+// bke_resample_normalized, csrc/resample_fused.cu.)
 constexpr int E2_NW = 8, E2_NT = E2_NW * 32, E2_SPT = 20, E2_WIN = E2_NT * E2_SPT;
 static_assert(E2_NT * IPT == TILE, "the second-generation emit uses the tile size of passes A-D");
 
@@ -1241,7 +1196,8 @@ struct Emit2Shared {
 
 // <E2_STAGES, E2_CTAS>: <2, 2> two 32 KB stages, 96 registers; <1, 3> one stage (the next tile's TMA is
 // issued as soon as the warps hold the current one in registers and lands long before it is needed),
-// 72 registers, three CTAs per SM
+// 72 registers, three CTAs per SM.  <2, 2> is the default; BKE_RS_E2=1 selects <1, 3>, which on the H100
+// is slower for systematic but about 17 % faster for stratified resampling (DESIGN.md §3.6)
 template <bool STRAT, int E2_STAGES, int E2_CTAS>
 __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_constant__ CUtensorMap wmap, Params p)
 {
@@ -1712,26 +1668,8 @@ struct RunArgs {
     int phase;           // bit 0: passes A-C (need carry_approx), bit 1: pass D chain (needs carry_exact), bit 2: passes E-G
 };
 
-// BKE_RS_IMPL=fused (or "new") selects the experimental single-pass kernel of resample_fused.cu for
-// whole-array calls: 12 B/particle of HBM traffic instead of 28, bit-exact on every test, but its
-// two-stage look-back chain does not yet keep up with the emit (DESIGN.md §3.6): the default
-// is the multi-pass pipeline below with the second-generation emit kernel.
-static bool use_fused()
-{
-    const char *e = getenv("BKE_RS_IMPL");
-    return e && (e[0] == 'f' || e[0] == 'n');
-}
-
 int run(const RunArgs &a, cudaStream_t s)
 {
-    if ((a.phase & 7) == 7 && use_fused()) {
-        FRunArgs f;
-        f.n = a.n; f.ng = a.ng; f.j0 = a.j0; f.cap = a.cap; f.w = a.w; f.U = a.U; f.u = a.u; f.idx = a.idx;
-        f.workspace = a.workspace; f.ws_bytes = a.ws_bytes; f.info = a.info; f.cumsum_last = a.cumsum_last;
-        f.carry_approx = a.carry_approx; f.carry_exact = a.carry_exact; f.out_range = a.out_range; f.is_last = a.is_last;
-        f.cumsum_out = a.cumsum_out; f.last_one = a.last_one; f.div = nullptr; f.wnorm_out = nullptr;
-        return f_run(f, s);
-    }
     const i64 n = a.n;
     if (n < 0 || a.ng < n || a.j0 < 0) { set_error("bad particle counts"); return BKE_ERR_BAD_ARG; }
     if (n == 0) return BKE_OK;
@@ -1771,8 +1709,8 @@ int run(const RunArgs &a, cudaStream_t s)
     if (a.phase & 1) {
         // BKE_RS_FRONT=1: tile sums, their scan (decoupled look-back) and the fast maps in ONE pass over the
         // weights.  Slower than the three launches it replaces on an earlier target (with hundreds of tiles in
-        // flight the nearest inclusive prefix is far back and the polling competes with the streaming loads),
-        // so it is an experiment, not the default.
+        // flight the nearest inclusive prefix is far back and the polling competes with the streaming loads);
+        // about 6 % faster on the H100 (DESIGN.md §3.6), not yet the default.
         static const bool fused_front = [] { const char *e = getenv("BKE_RS_FRONT"); return e && e[0] == '1'; }();
         if (!(a.phase & 8) && fused_front) {
             const size_t clr = (size_t)((unsigned char *)(p.ws.st1 + T) - (unsigned char *)p.ws.hdr);
@@ -1784,18 +1722,13 @@ int run(const RunArgs &a, cudaStream_t s)
                 k_tile_sums<<<T, BLOCK, 0, s>>>(p);
             }
             k_scan_tiles<<<1, CHAIN_THREADS, 0, s>>>(p);
-            // one tile per CTA (5 CTAs/SM) by default; the persistent kernel with a register double-buffer
-            // (3 CTAs/SM) was slower on an earlier target and stays for comparison (BKE_RS_MAPS=0)
-            static const bool maps_persistent = [] { const char *e = getenv("BKE_RS_MAPS"); return e && e[0] == '0'; }();
-            if (maps_persistent) k_tile_maps_fast<<<T < sms * 3 ? T : sms * 3, BLOCK, 0, s>>>(p);
-            else k_tile_maps_fast1<<<T, BLOCK, 0, s>>>(p);
+            k_tile_maps_fast1<<<T, BLOCK, 0, s>>>(p);
         }
         k_tile_maps<<<slow_grid, BLOCK, 0, s>>>(p);
     }
     if (a.phase & 2) {
-        // a cluster of CHAIN_CTAS CTAs once there are enough tiles to share out (BKE_RS_CHAIN=1: always one CTA)
-        static const bool one_cta = [] { const char *e = getenv("BKE_RS_CHAIN"); return e && e[0] == '1'; }();
-        if (T >= 2048 && !one_cta) {
+        // a cluster of CHAIN_CTAS CTAs once there are enough tiles to share out
+        if (T >= 2048) {
             if (a.U) k_chain_cluster<true><<<CHAIN_CTAS, CHAIN_THREADS, 0, s>>>(p);
             else k_chain_cluster<false><<<CHAIN_CTAS, CHAIN_THREADS, 0, s>>>(p);
         } else if (a.U) k_chain<true><<<1, CHAIN_THREADS, 0, s>>>(p);
@@ -1804,10 +1737,9 @@ int run(const RunArgs &a, cudaStream_t s)
     if (a.phase & 4) {
         const int fast_grid = T < sms * 2 ? T : sms * 2;
         // second-generation emit (TMA-staged, marker / max-scan expansion) whenever the weights qualify for
-        // TMA and indexes are produced; BKE_RS_EMIT=1 keeps the first-generation kernel
+        // TMA and indexes are produced; otherwise the first-generation kernel
         CUtensorMap wmap;
-        const char *emit_env = getenv("BKE_RS_EMIT");
-        const bool emit2 = !(emit_env && emit_env[0] == '1') && !a.cumsum_out && (n % 16) == 0 && f_weights_map(a.w, n, E2_NT, &wmap);
+        const bool emit2 = !a.cumsum_out && (n % 16) == 0 && f_weights_map(a.w, n, E2_NT, &wmap);
         if (emit2) {
             static const int e2_variant = [] { const char *e = getenv("BKE_RS_E2"); return e ? atoi(e) : 0; }();
             auto launch2 = [&](auto kern, int smem2, int ctas) -> int {
@@ -1885,10 +1817,9 @@ int bke_resample_normalized(int64_t n, const double *weights, double u, const do
     int rc = bke_weights_sum(n, weights, sum_out, workspace, workspace_bytes, stream);
     if (rc != BKE_OK) return rc;
     rs::FRunArgs f;
-    f.n = n; f.ng = n; f.j0 = 0; f.cap = n; f.w = weights; f.U = uniforms; f.u = u; f.idx = indexes;
+    f.n = n; f.w = weights; f.U = uniforms; f.u = u; f.idx = indexes;
     f.workspace = workspace; f.ws_bytes = workspace_bytes; f.info = info; f.cumsum_last = cumsum_last;
-    f.carry_approx = nullptr; f.carry_exact = nullptr; f.out_range = nullptr; f.is_last = 1;
-    f.cumsum_out = nullptr; f.last_one = 0; f.div = sum_out; f.wnorm_out = weights_out;
+    f.div = sum_out; f.wnorm_out = weights_out;
     return rs::f_run(f, (cudaStream_t)stream);
 }
 
@@ -1970,10 +1901,6 @@ int bke_resample_compose_carry(int32_t n_shards_before, const void *composites, 
     rs::k_compose_carry<<<1, 32, 0, (cudaStream_t)stream>>>(n_shards_before, (const rs::Composite *)composites, carry_exact, status);
     return check_cuda(cudaGetLastError(), "compose carry launch");
 }
-
-/* debugging aid (not part of the documented ABI): device buffer of uint64[T][10] that receives the
- * global-timer stamps of every tile's pipeline events in the single-pass kernel; NULL switches it off */
-void bke_debug_resample_trace(void *device_buffer) { rs::f_set_trace(device_buffer); }
 
 int bke_resample_shard(const bke_resample_shard_args *args, void *stream)
 {

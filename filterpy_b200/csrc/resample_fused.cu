@@ -1,5 +1,6 @@
-// resample_fused.cu — systematic / stratified resampling and the exact cumulative sum as ONE
-// single-pass kernel: every weight is read from HBM once (8 B in, 4 B out per particle).
+// resample_fused.cu — systematic / stratified resampling of a whole array of weights, normalised on
+// the fly, as ONE single-pass kernel: every weight is read from HBM once (8 B in, 4 B out per
+// particle).  It is the engine of bke_resample_normalized.
 //
 //   indexes[i] = #{ j : c_j <= pos_i },  c_j = fl(c_{j-1} + w_j)   (filterpy/monte_carlo/resampling.py:141-149)
 //   pos_i = fl(fl(u + i) / N) (:139)  or  fl(fl(U_i + i) / N) (:103)
@@ -30,26 +31,14 @@
 // Everything is verified with the exact values (tile start / end inside the assumed binade); a
 // failed check or a negative / non-finite weight switches to the literal sequential kernel.
 #include <cuda.h>
-#include <stdlib.h>
 #include "resample_common.cuh"
 #include "resample_fused.cuh"
 
 namespace bke {
 namespace rs {
 
-// ------------------------------------------------------------------ event trace (debugging aid)
-// bke_debug_resample_trace(buf): every tile writes the global-timer time of 10 pipeline events
-__device__ __forceinline__ void f_trace(const FParams &p, int t, int ev)
-{
-    if (p.trace) {
-        unsigned long long now;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-        p.trace[(size_t)t * 10 + ev] = now;
-    }
-}
-
 // ------------------------------------------------------------------ status words
-// st1[i], st2[i] describe tile i-1; entry 0 is the carry into the call (always INCLUSIVE).
+// st1[i], st2[i] describe tile i-1; entry 0 is the empty sum before the first tile (INCLUSIVE).
 //   st1: bits of an fp64 sum with the two lowest mantissa bits replaced by the flag
 //        (1 = this tile's sum, 2 = sum of everything up to and including this tile)
 //   st2: bit 63 = INCLUSIVE: bits 0..62 = exact running sum after the tile (a non-negative double)
@@ -60,18 +49,17 @@ constexpr int SPIN_LIMIT = 1 << 22;
 
 __device__ __forceinline__ u64 st2_pack_agg(i64 d, int t) { return ST2_AGG | ((u64)(t + 1) << 60) | ((u64)d & ((1ull << 60) - 1)); }
 
-// Look-back windows: every round a warp fetches up to 32 * LBK_MAX status words at once (ONE L2 round
-// trip), walks them in groups of 32 from the nearest predecessor outwards and stops at the nearest
+// Look-back windows: every round a warp fetches 32 * LBK status words at once (ONE L2 round trip),
+// walks them in groups of 32 from the nearest predecessor outwards and stops at the nearest
 // INCLUSIVE word.  All tiles of a persistent grid start together, so a tile is typically a few
 // hundred tiles ahead of the inclusive frontier: the width of the window, not the number of
 // resident CTAs, sets how many round trips a look-back costs.
-constexpr int LBK_MAX = 8;
+constexpr int LBK = 4;
 
-// a blocked round (an unpublished word in front of the nearest inclusive one): back off, and give up
+// a blocked round (an unpublished word in front of the nearest inclusive one): poll again, and give up
 // after SPIN_LIMIT rounds or once any look-back has given up (the result then comes from the fallback)
-__device__ __forceinline__ bool f_blocked(FHeader *hdr, int &spins, int sleep_ns)
+__device__ __forceinline__ bool f_blocked(FHeader *hdr, int &spins)
 {
-    if (sleep_ns > 0) __nanosleep(sleep_ns);
     spins++;
     if ((spins & 1023) == 0 && *reinterpret_cast<volatile int *>(&hdr->timeout)) return true;
     if (spins >= SPIN_LIMIT) { hdr->timeout = 1; hdr->fallback = 1; return true; }
@@ -86,17 +74,17 @@ __device__ __forceinline__ double f_lookback_sum(const FParams &p, int t, int la
     int spins = 0;
     bool done = false;
     while (!done) {
-        u64 v[LBK_MAX];
+        u64 v[LBK];
 #pragma unroll
-        for (int j = 0; j < LBK_MAX; j++) {
+        for (int j = 0; j < LBK; j++) {
             const int i = idx - 32 * j;
-            v[j] = ST1_INCL;                               // beyond the carry: 0.0, inclusive
-            if (j < p.lbk && i >= 0) v[j] = f_ld(p.st1 + i);
+            v[j] = ST1_INCL;                               // before entry 0: 0.0, inclusive
+            if (i >= 0) v[j] = f_ld(p.st1 + i);
         }
         bool blocked = false;
 #pragma unroll
-        for (int j = 0; j < LBK_MAX; j++) {
-            if (j < p.lbk && !done && !blocked) {
+        for (int j = 0; j < LBK; j++) {
+            if (!done && !blocked) {
                 const unsigned incl = __ballot_sync(FULL, (v[j] & 3) == ST1_INCL);
                 const unsigned empty = __ballot_sync(FULL, (v[j] & 3) == 0);
                 const int first = incl ? __ffs(incl) - 1 : 32;
@@ -108,7 +96,7 @@ __device__ __forceinline__ double f_lookback_sum(const FParams &p, int t, int la
                 }
             }
         }
-        if (blocked && f_blocked(p.hdr, spins, p.sleep_ns)) break;
+        if (blocked && f_blocked(p.hdr, spins)) break;
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(FULL, part, o);
@@ -128,17 +116,17 @@ __device__ __forceinline__ i64 f_lookback_state(const FParams &p, int t, int lan
     int spins = 0;
     bool done = false;
     while (!done) {
-        u64 v[LBK_MAX];
+        u64 v[LBK];
 #pragma unroll
-        for (int j = 0; j < LBK_MAX; j++) {
+        for (int j = 0; j < LBK; j++) {
             const int i = idx - 32 * j;
             v[j] = ST2_INCL;
-            if (j < p.lbk && i >= 0) v[j] = f_ld(p.st2 + i);
+            if (i >= 0) v[j] = f_ld(p.st2 + i);
         }
         bool blocked = false;
 #pragma unroll
-        for (int j = 0; j < LBK_MAX; j++) {
-            if (j < p.lbk && !done && !blocked) {
+        for (int j = 0; j < LBK; j++) {
+            if (!done && !blocked) {
                 const unsigned incl = __ballot_sync(FULL, (v[j] & ST2_INCL) != 0);
                 const unsigned empty = __ballot_sync(FULL, (v[j] & (ST2_INCL | ST2_AGG)) == 0);
                 const int first = incl ? __ffs(incl) - 1 : 32;
@@ -173,7 +161,7 @@ __device__ __forceinline__ i64 f_lookback_state(const FParams &p, int t, int lan
                 else idx -= 32;
             }
         }
-        if (blocked && f_blocked(p.hdr, spins, p.sleep_ns)) break;
+        if (blocked && f_blocked(p.hdr, spins)) break;
     }
     if (!general) {
 #pragma unroll
@@ -188,6 +176,11 @@ enum { TM_FAST = 0, TM_SLOW = 1, TM_BAD = 2 };                       // what the
 enum { TK_CLEAN = 0, TK_CROSS = 1, TK_TIES = 2, TK_BAD = 3 };        // what stage 1 found out about it
 constexpr int MAX_CROSS = 24;                                        // crossing rows resolved by the chain warp
 constexpr int RING = 8;                                              // tiles a CTA has between "fronted" and "emitted"
+// NW consumer warps per CTA (+ 4 helper warps), F_CTAS CTAs per SM (what the shared memory allows),
+// and the emit runs DELTA tiles of the CTA behind the front
+constexpr int NW = 8, NT = NW * 32, F_TILE = NT * F_IPT, WIN = NT * F_SPT;
+constexpr int F_CTAS = 2, DELTA = 3;
+static_assert(DELTA + 2 <= RING, "ring too small");
 
 // one tile of this CTA on its way from front (sum + map) to emit
 struct FSlot {
@@ -203,11 +196,9 @@ struct FSlot {
     i64 S_in, lo, cnt;      // C2: exact state before the tile, its output range
 };
 
-template <int NW>
 struct FSmem {
-    static constexpr int NT = NW * 32, TILE = NT * F_IPT, WIN = NT * F_SPT;
-    double wf[TILE];                   // front buffer  \\ TMA destinations (128-byte swizzle): must stay first,
-    double we[TILE];                   // emit buffer   /  1024-aligned
+    double wf[F_TILE];                 // front buffer  \\ TMA destinations (128-byte swizzle): must stay first,
+    double we[F_TILE];                 // emit buffer   /  1024-aligned
     int win[WIN];                      // output window (all zero between tiles)
     i64 xrow[NT];                      // crossing pool: exact state before every row of ONE tile that leaves its binade
     unsigned xmask[NT / 32];           // ... and the rows (consumer threads) that are walked with true adds
@@ -220,7 +211,6 @@ struct FSmem {
     uint64_t claimed[RING], fronted[RING], mapped[RING], resolved[RING], freed[RING];
     FSlot ring[RING];
     int e_last;                        // binade of the last tile the chain resolved (the front's guess)
-    int last_t;                        // trace: the tile the consumers emitted last
     i64 bc_S_in, bc_lo, bc_cnt;
     int bc_ok, bc_skip;
     // slow path (tiles with ties)
@@ -234,27 +224,27 @@ struct FSmem {
 };
 
 
-template <int NW> __device__ __forceinline__ double f_scan_d(double v, double *total, double *sh, int lane, int wid)
+__device__ __forceinline__ double f_scan_d(double v, double *total, double *sh, int lane, int wid)
 {
     const double inc = warp_incl_scan_d(v, lane);
     if (lane == 31) sh[wid] = inc;
-    f_bar<NW * 32>();
+    f_bar<NT>();
     double base = 0.0, tot = 0.0;
 #pragma unroll
     for (int i = 0; i < NW; i++) { const double x = sh[i]; if (i < wid) base += x; tot += x; }
-    f_bar<NW * 32>();
+    f_bar<NT>();
     *total = tot;
     return base + (inc - v);
 }
 
-template <int NW> __device__ __forceinline__ SM f_scan_sm(SM v, SM *total, SM *sh, int lane, int wid)
+__device__ __forceinline__ SM f_scan_sm(SM v, SM *total, SM *sh, int lane, int wid)
 {
     const SM inc = warp_incl_scan_sm(v, lane);
     if (lane == 31) sh[wid] = inc;
-    f_bar<NW * 32>();
+    f_bar<NT>();
     SM base = sm_identity(), tot = sm_identity();
     for (int i = 0; i < NW; i++) { const SM x = sh[i]; if (i < wid) base = combine(base, x); tot = combine(tot, x); }
-    f_bar<NW * 32>();
+    f_bar<NT>();
     *total = tot;
     SM prev = shfl_up_sm(inc, 1);
     if (lane == 0) prev = sm_identity();
@@ -264,14 +254,14 @@ template <int NW> __device__ __forceinline__ SM f_scan_sm(SM v, SM *total, SM *s
 template <int MODE>
 __device__ __forceinline__ i64 f_count_below(const FParams &p, double c)
 {
-    const double Ngd = (double)p.ng;
-    return (MODE == F_STRAT) ? count_below_str(c, p.U, p.ng, Ngd) : count_below_sys(c, p.u, p.ng, Ngd, p.tau);
+    const double Ngd = (double)p.n;
+    return (MODE == F_STRAT) ? count_below_str(c, p.U, p.n, Ngd) : count_below_sys(c, p.u, p.n, Ngd, p.tau);
 }
 
 __device__ __forceinline__ void f_put_index(const FParams &p, i64 out_begin, i64 o, int value)
 {
     const i64 rel = o - out_begin;
-    if (rel >= 0 && rel < p.cap) p.idx[rel] = value;
+    if (rel >= 0 && rel < p.n) p.idx[rel] = value;
     else p.hdr->cap_overflow = 1;
 }
 
@@ -281,7 +271,7 @@ template <int MODE>
 __device__ __forceinline__ void f_finish_tile(const FParams &p, int t, i64 S_in, i64 S_out, int &good, i64 &lo, i64 &cnt)
 {
     lo = 0; cnt = 0;
-    if (MODE != F_CUMSUM && good) {
+    if (good) {
         lo = f_count_below<MODE>(p, __longlong_as_double(S_in));
         cnt = f_count_below<MODE>(p, __longlong_as_double(S_out)) - lo;
         if (cnt < 0) { cnt = 0; good = 0; }
@@ -289,17 +279,14 @@ __device__ __forceinline__ void f_finish_tile(const FParams &p, int t, i64 S_in,
     if (!good) { p.hdr->fallback = 1; p.hdr->chain_bad = 1; }
     if (t == p.T - 1) {
         if (p.cumsum_last) *p.cumsum_last = __longlong_as_double(S_out);
-        if (MODE != F_CUMSUM) {
-            i64 O1 = lo + cnt;
-            if (p.is_last && O1 < p.ng) {                  // resampling.py:145 would raise IndexError
-                p.hdr->overflow = (int)(p.ng - O1 > 0x7fffffff ? 0x7fffffff : p.ng - O1);
-                const int r = atomicAdd(&p.hdr->n_runs, 1);
-                if (r < p.max_runs) p.runs[r] = Run{O1, p.ng, (int)(p.ng - 1), 0};
-                O1 = p.ng;
-            }
-            p.hdr->out_end = O1;
-            if (p.out_range) { p.out_range[0] = p.hdr->out_begin; p.out_range[1] = O1; }
+        i64 O1 = lo + cnt;
+        if (O1 < p.n) {                                    // resampling.py:145 would raise IndexError
+            p.hdr->overflow = (int)(p.n - O1 > 0x7fffffff ? 0x7fffffff : p.n - O1);
+            const int r = atomicAdd(&p.hdr->n_runs, 1);
+            if (r < p.max_runs) p.runs[r] = Run{O1, p.n, (int)(p.n - 1), 0};
+            O1 = p.n;
         }
+        p.hdr->out_end = O1;
     }
 }
 
@@ -307,10 +294,9 @@ __device__ __forceinline__ void f_finish_tile(const FParams &p, int t, i64 S_in,
 // Leaves the exact c_j (bit patterns) of the tile in the stage buffer, at the positions of the
 // weights they belong to; returns 1 if the tile verified.  Everything up to the segment export
 // runs BEFORE the exact start state is known; only the walk over <= RMAX segments is serial.
-template <int NW, int MODE>
-__device__ __noinline__ int f_slow_tile(const FParams &p, FSmem<NW> &sm, int t, i64 S_in_known)
+template <int MODE>
+__device__ __noinline__ int f_slow_tile(const FParams &p, FSmem &sm, int t, i64 S_in_known)
 {
-    constexpr int NT = NW * 32;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     unsigned char *sb = reinterpret_cast<unsigned char *>(sm.we);
     double w[F_IPT];
@@ -324,7 +310,7 @@ __device__ __noinline__ int f_slow_tile(const FParams &p, FSmem<NW> &sm, int t, 
     for (int k = 0; k < F_IPT; k++) ssum += w[k];
     double tot;
     // the exact state before the tile is known (chain warp C2): it is the "approximate" prefix of the classification
-    double before = __longlong_as_double(S_in_known) + f_scan_d<NW>(ssum, &tot, sm.warp_d, lane, wid);
+    double before = __longlong_as_double(S_in_known) + f_scan_d(ssum, &tot, sm.warp_d, lane, wid);
     SM inc[F_IPT];
     int ek[F_IPT];
     SM run = sm_identity();
@@ -343,7 +329,7 @@ __device__ __noinline__ int f_slow_tile(const FParams &p, FSmem<NW> &sm, int t, 
         before = after;
     }
     SM total;
-    const SM excl = f_scan_sm<NW>(run, &total, sm.warp_sm, lane, wid);
+    const SM excl = f_scan_sm(run, &total, sm.warp_sm, lane, wid);
 #pragma unroll
     for (int k = 0; k < F_IPT; k++) inc[k] = combine(excl, inc[k]);
     const int nraw = total.cnt;
@@ -434,27 +420,10 @@ __device__ __noinline__ int f_slow_tile(const FParams &p, FSmem<NW> &sm, int t, 
     return f_bar_and<NT>(!bad && sm.bc_ok);
 }
 
-// cumsum mode: the exact running sums leave as they are (each thread owns 16 consecutive elements = one 128-byte line)
-__device__ __forceinline__ void f_store_cumsum(const FParams &p, i64 j, const i64 (&cb)[F_IPT])
-{
-    double *o = p.cumsum_out + j;
-    if (j + F_IPT <= p.n && (reinterpret_cast<uintptr_t>(o) & 15) == 0 && !(p.last_one && j + F_IPT == p.n)) {
-#pragma unroll
-        for (int k = 0; k < F_IPT; k += 2)
-            *reinterpret_cast<double2 *>(o + k) = make_double2(__longlong_as_double(cb[k]), __longlong_as_double(cb[k + 1]));
-    } else {
-#pragma unroll
-        for (int k = 0; k < F_IPT; k++)
-            if (j + k < p.n) o[k] = (p.last_one && j + k == p.n - 1) ? 1.0 : __longlong_as_double(cb[k]);
-    }
-}
-
 // read this thread's F_SPT window slots (and clear them), running maximum, block max-scan:
 // m[i] = marker (local particle index + 1) of the particle that owns slot tid*F_SPT + i
-template <int NW>
-__device__ __forceinline__ void f_window_scan(FSmem<NW> &sm, int tid, int lane, int wid, int (&m)[F_SPT])
+__device__ __forceinline__ void f_window_scan(FSmem &sm, int tid, int lane, int wid, int (&m)[F_SPT])
 {
-    constexpr int NT = NW * 32;
     int4 *wv = reinterpret_cast<int4 *>(sm.win) + tid * (F_SPT / 4);
 #pragma unroll
     for (int i = 0; i < F_SPT / 4; i++) {
@@ -482,7 +451,6 @@ __device__ __forceinline__ void f_window_scan(FSmem<NW> &sm, int tid, int lane, 
 // of the chain warps: a wrong binade guess, a tile that leaves its binade).  Lane L owns rows
 // L, L + 32, ...: rs[i] belongs to row 32 i + L (0 for rows < r0); bit i of the result is set when
 // that row holds an exact tie.
-template <int NW>
 __device__ __noinline__ unsigned f_row_sums_g(const FParams &p, int t, int e, int r0, int lane, double divisor, i64 (&rs)[NW])
 {
     const i64 base = (i64)e << 52;
@@ -518,10 +486,8 @@ __device__ __noinline__ unsigned f_row_sums_g(const FParams &p, int t, int e, in
 // maps; the row that leaves it is walked with true adds; the rows after it are maps of the next
 // binade, and so on.  On success sm.xrow[r] = exact state before row r, sm.xmask marks the walked
 // rows, *S_out = state after the tile.  false: a tie in a mapped row, or more than MAX_CROSS crossings.
-template <int NW>
-__device__ __noinline__ bool f_resolve_exact(const FParams &p, FSmem<NW> &sm, int t, i64 S_in, i64 *S_out, int lane, double divisor)
+__device__ __noinline__ bool f_resolve_exact(const FParams &p, FSmem &sm, int t, i64 S_in, i64 *S_out, int lane, double divisor)
 {
-    constexpr int NT = NW * 32;
     if (lane < NT / 32) sm.xmask[lane] = 0;
     __syncwarp();
     int r0 = 0;
@@ -530,7 +496,7 @@ __device__ __noinline__ bool f_resolve_exact(const FParams &p, FSmem<NW> &sm, in
         if (round > MAX_CROSS) return false;
         const int e = (int)(S >> 52);
         i64 rsum[NW];
-        const unsigned ties = f_row_sums_g<NW>(p, t, e, r0, lane, divisor, rsum);
+        const unsigned ties = f_row_sums_g(p, t, e, r0, lane, divisor, rsum);
         i64 carry = S;                                     // state before row 32 i (rows < r0 contribute 0)
         int found = -1;
         i64 S_row = 0;
@@ -573,9 +539,6 @@ __device__ __noinline__ bool f_resolve_exact(const FParams &p, FSmem<NW> &sm, in
 }
 
 // ------------------------------------------------------------------ the kernel
-// resident CTAs per SM that the shared-memory footprint of a variant allows (227 KB per SM)
-constexpr int f_ctas(int nw) { return nw == 8 ? 2 : 4; }
-
 // Roles inside a CTA (NW consumer warps + 3 helper warps):
 //   consumers  iteration k: FRONT tile k of this CTA (sum, validation, parity map in the guessed
 //              binade -> stage-1 AGGREGATE published at once), then EMIT tile k - DELTA (by then the
@@ -585,14 +548,12 @@ constexpr int f_ctas(int nw) { return nw == 8 ? 2 : 4; }
 //   C2         stage-2 look-back: exact state before the tile -> INCLUSIVE; tiles that leave their binade
 // The chain (C1, C2) runs DELTA tiles per CTA — several hundred tiles of the grid — ahead of the
 // emit front, so a look-back never stalls the warps that do the work.
-template <int NW, int DELTA, int MODE>
-__global__ void __launch_bounds__(NW * 32 + 128, f_ctas(NW))
+template <int MODE>
+__global__ void __launch_bounds__(NT + 128, F_CTAS)
 k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
 {
-    constexpr int NT = NW * 32, TILE = NT * F_IPT, WIN = NT * F_SPT;
-    static_assert(DELTA + 2 <= RING, "ring too small");
     extern __shared__ __align__(1024) unsigned char f_smem_raw[];
-    FSmem<NW> &sm = *reinterpret_cast<FSmem<NW> *>(f_smem_raw);
+    FSmem &sm = *reinterpret_cast<FSmem *>(f_smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
 
     if (tid == 0) {
@@ -602,7 +563,6 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
             f_mbar_init(&sm.claimed[i], 1); f_mbar_init(&sm.fronted[i], 1); f_mbar_init(&sm.mapped[i], 1); f_mbar_init(&sm.resolved[i], 1); f_mbar_init(&sm.freed[i], NW);
         }
         sm.e_last = 1022;              // binade [0.5, 1): where a normalised running sum spends most of its life
-        sm.last_t = -1;
         f_fence_mbar_init();
     }
     for (int q = tid; q < WIN; q += NT + 128) sm.win[q] = 0;
@@ -616,11 +576,11 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
         // and LE (emit buffer: the same tiles again DELTA iterations later, from L2).  Both block on mbarriers only.
         auto load_tile = [&](int t, double *dst, uint64_t *full) {
             if (p.use_tma && !(tail_generic && t == p.T - 1)) {
-                if (lane == 0) { f_mbar_expect_tx(full, TILE * 8); f_tma_load_2d(dst, &wmap, 0, t * NT, full); }
+                if (lane == 0) { f_mbar_expect_tx(full, F_TILE * 8); f_tma_load_2d(dst, &wmap, 0, t * NT, full); }
             } else {
                 unsigned char *sb = reinterpret_cast<unsigned char *>(dst);
-                const i64 j0 = (i64)t * TILE;
-                for (int i = lane; i < TILE; i += 32) {
+                const i64 j0 = (i64)t * F_TILE;
+                for (int i = lane; i < F_TILE; i += 32) {
                     const i64 j = j0 + i;
                     const double v = (j < p.n) ? p.w[j] : 0.0;
                     *reinterpret_cast<double *>(sb + f_swz(i >> 4, (i >> 1) & 7) + (i & 1) * 8) = v;
@@ -643,7 +603,6 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
                 if (lane == 0) {
                     sm.ring[slot].eg = *reinterpret_cast<volatile int *>(&sm.e_last);
                     sm.ring[slot].t = t;
-                    if (t >= 0) f_trace(p, t, 0);
                 }
                 __syncwarp();
                 if (lane == 0) f_mbar_arrive(&sm.claimed[slot]);       // LE may read the slot's tile
@@ -666,26 +625,21 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
         // ============================================================ chain warp C1 (stage 1)
         // approximate prefix -> which binade the tile lives in -> for a tile deep inside one binade the
         // stage-2 AGGREGATE (its parity map D), published right away (C1 never waits for stage 2)
-        long long pf[3] = {0, 0, 0}, tk = clock64();
-        auto lap = [&](int i) { const long long now = clock64(); pf[i] += now - tk; tk = now; };
         for (int k = 0;; k++) {
             const int si = k % RING, use = k / RING;
             FSlot &sl = sm.ring[si];
             f_mbar_wait(&sm.fronted[si], use & 1);
-            lap(0);
             const int t = sl.t;
             if (t < 0) {
                 if (lane == 0) f_mbar_arrive(&sm.mapped[si]);
                 break;
             }
-            if (lane == 0) f_trace(p, t, 3);
             const double tot = sl.tot;
             const int bad = sl.bad, eg = sl.eg;
             int any_tie = sl.tie;
             i64 D = sl.D;
             const double tp = f_lookback_sum(p, t, lane);
-            if (lane == 0) { f_st(p.st1 + t + 1, ((u64)__double_as_longlong(tp + tot) & ~3ull) | ST1_INCL); f_trace(p, t, 4); }
-            lap(1);
+            if (lane == 0) f_st(p.st1 + t + 1, ((u64)__double_as_longlong(tp + tot) & ~3ull) | ST1_INCL);
             int e0;
             const bool ca = clean_add(tp, tp + tot, p.eb, &e0);
             int kind = bad ? TK_BAD : ((ca || tot == 0.0) ? TK_CLEAN : TK_CROSS);
@@ -695,7 +649,7 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
                 else if (e0 != eg) {
                     // the front's guess was wrong (first tiles, a new binade): the map again, in binade e0
                     i64 rsum[NW];
-                    any_tie = f_row_sums_g<NW>(p, t, e0, 0, lane, divisor, rsum) != 0;
+                    any_tie = f_row_sums_g(p, t, e0, 0, lane, divisor, rsum) != 0;
                     any_tie = __any_sync(FULL, any_tie);
                     D = 0;
 #pragma unroll
@@ -706,28 +660,22 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
                 if (tot != 0.0 && lane == 0) sm.e_last = e0;
                 if (any_tie) kind = TK_TIES;               // ties: the general parity maps of the slow path
             }
-            if (kind == TK_CLEAN && lane == 0) { f_st(p.st2 + t + 1, st2_pack_agg(D, 0)); f_trace(p, t, 5); }
+            if (kind == TK_CLEAN && lane == 0) f_st(p.st2 + t + 1, st2_pack_agg(D, 0));
             if (lane == 0) { sl.kind = kind; sl.e0 = e0; sl.D = D; }
             __syncwarp();
             if (lane == 0) f_mbar_arrive(&sm.mapped[si]);
-            lap(2);
         }
-        if (p.prof && lane == 0)
-            for (int i = 0; i < 3; i++) atomicAdd(reinterpret_cast<unsigned long long *>(&p.hdr->prof[3 + i]), (unsigned long long)pf[i]);
         return;
     }
     if (wid == NW + 2) {
         // ============================================================ chain warp C2 (stage 2)
         // exact state before the tile; tiles that may leave their binade are resolved here, exactly,
         // from that state (no margins)
-        long long pf[3] = {0, 0, 0}, tk = clock64();
-        auto lap = [&](int i) { const long long now = clock64(); pf[i] += now - tk; tk = now; };
         int xuse = 0;
         for (int k = 0;; k++) {
             const int si = k % RING, use = k / RING;
             FSlot &sl = sm.ring[si];
             f_mbar_wait(&sm.mapped[si], use & 1);
-            lap(0);
             const int t = sl.t;
             if (t < 0) {
                 if (lane == 0) f_mbar_arrive(&sm.resolved[si]);
@@ -737,7 +685,6 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
             const double tot = sl.tot;
             const i64 D = sl.D;
             const i64 S_in = f_lookback_state(p, t, lane);
-            lap(1);
             int mode, good = 1, cross = 0;
             i64 S_out = S_in, lo = 0, cnt = 0;
             if (kind == TK_CLEAN) {
@@ -750,7 +697,7 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
                 mode = TM_SLOW;                            // ties / too many crossings: the consumers' general path publishes
                 if (kind == TK_CROSS) {
                     if (xuse > 0) f_mbar_wait(&sm.xfree, (xuse - 1) & 1);       // the pool's previous tile has been emitted
-                    if (f_resolve_exact<NW>(p, sm, t, S_in, &S_out, lane, divisor)) {
+                    if (f_resolve_exact(p, sm, t, S_in, &S_out, lane, divisor)) {
                         mode = TM_FAST; cross = 1; xuse++;
                         if (lane == 0) { atomicAdd(&p.hdr->n_unclean, 1); sm.e_last = (int)(S_out >> 52); }
                     }
@@ -758,31 +705,24 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
             }
             // a failed resolve leaves the pool unused: keep xfree's phase in step by not counting the use
             if (lane == 0) {
-                if (mode != TM_SLOW) { f_st(p.st2 + t + 1, ST2_INCL | (u64)S_out); f_trace(p, t, 6); }
+                if (mode != TM_SLOW) f_st(p.st2 + t + 1, ST2_INCL | (u64)S_out);
                 if (mode == TM_FAST) f_finish_tile<MODE>(p, t, S_in, S_out, good, lo, cnt);
                 sl.mode = mode; sl.good = good; sl.cross = cross; sl.S_in = S_in; sl.lo = lo; sl.cnt = cnt;
-                f_trace(p, t, 7);
             }
             __syncwarp();
             if (lane == 0) f_mbar_arrive(&sm.resolved[si]);
-            lap(2);
         }
-        if (p.prof && lane == 0)
-            for (int i = 0; i < 3; i++) atomicAdd(reinterpret_cast<unsigned long long *>(&p.hdr->prof[6 + i]), (unsigned long long)pf[i]);
         return;
     }
 
     // ================================================================ consumer warps
     const i64 out_begin = p.hdr->out_begin;
-    const double Nd = (double)p.ng;
-    long long cwait = 0, cfront = 0, cemit = 0, ctk = clock64();
-    auto clap = [&](long long &acc) { const long long now = clock64(); acc += now - ctk; ctk = now; };
+    const double Nd = (double)p.n;
     bool front_done = false;
     for (int k = 0;; k++) {
         // ------------------------------------------------------------ FRONT tile k of this CTA
         if (!front_done) {
             f_mbar_wait(&sm.full_f, k & 1);
-            clap(cwait);
             FSlot &sl = sm.ring[k % RING];
             const int t = sl.t;
             if (t < 0) {
@@ -846,11 +786,9 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
                     if (tbad) { tt = 0.0; p.hdr->fallback = 1; }
                     f_st(p.st1 + t + 1, ((u64)__double_as_longlong(tt) & ~3ull) | ST1_AGG);
                     sl.tot = tt; sl.D = D; sl.tie = ttie; sl.D1 = Dh; sl.tie1 = ttieh; sl.bad = tbad;
-                    f_trace(p, t, 2);
                     f_mbar_arrive(&sm.fronted[k % RING]);
                 }
             }
-            clap(cfront);
         }
         if (k < DELTA) continue;
         // ------------------------------------------------------------ EMIT tile k - DELTA of this CTA
@@ -860,20 +798,17 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
         const int t = sl.t;
         if (t < 0) break;
         f_mbar_wait(&sm.full_e, m_idx & 1);
-        clap(cwait);
         const int mode = sl.mode, cross = sl.cross;
         int good = sl.good;
         const i64 S_in = sl.S_in;
         i64 tile_lo = sl.lo, tile_cnt = sl.cnt;
-        if (tid == 0) { f_trace(p, t, 8); if (sm.last_t >= 0) f_trace(p, sm.last_t, 9); sm.last_t = t; }
         unsigned char *sb = reinterpret_cast<unsigned char *>(sm.we);
-        const i64 jthread = (i64)t * TILE + (i64)tid * F_IPT;       // first particle of this thread (local numbering)
+        const i64 jthread = (i64)t * F_TILE + (i64)tid * F_IPT;       // first particle of this thread (local numbering)
         i64 cb[F_IPT];
         i64 thread_start = 0;                               // exact state before this thread's first particle
         if (mode == TM_BAD) {
             __syncwarp();
             if (lane == 0) { f_mbar_arrive(&sm.empty_e); f_mbar_arrive(&sm.freed[si]); }
-            clap(cemit);
             continue;
         }
         if (mode == TM_FAST) {
@@ -951,7 +886,7 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
                 }
                 f_bar<NT>();
             }
-            good = f_slow_tile<NW, MODE>(p, sm, t, S_in);
+            good = f_slow_tile<MODE>(p, sm, t, S_in);
 #pragma unroll
             for (int c = 0; c < F_IPT / 2; c++) {
                 const longlong2 v = *reinterpret_cast<const longlong2 *>(sb + f_swz(tid, c));
@@ -966,15 +901,14 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
             __syncwarp();
             if (lane == 0) { f_fence_proxy_async(); f_mbar_arrive(&sm.empty_e); f_mbar_arrive(&sm.freed[si]); }
         }
-        if (!good) { f_bar<NT>(); clap(cemit); continue; }
-        if (MODE == F_CUMSUM) { f_store_cumsum(p, jthread, cb); f_bar<NT>(); clap(cemit); continue; }
+        if (!good) { f_bar<NT>(); continue; }
 
         // ---- output range end of every particle, relative to tile_lo: hv[k] = #{positions < c_k} - tile_lo
         int hv[F_IPT], hv_prev;
         if (MODE == F_SYS) {
             // branch-free: floor(c N - u) + 1 away from integers; the rare near-integer cases are redone exactly
             const double u = p.u, half_m = 0.5 - p.tau;
-            const int n_m1 = (int)p.ng - 1, lo_m1 = (int)tile_lo - 1;
+            const int n_m1 = (int)p.n - 1, lo_m1 = (int)tile_lo - 1;
             unsigned slow = 0;
             auto count1 = [&](i64 cbits, unsigned bit) -> int {
                 const double v = fma(__longlong_as_double(cbits), Nd, -u);    // >= -u > -1
@@ -999,10 +933,10 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
         }
 
         // ---- expansion
-        const int base_j = (int)(p.j0 + (i64)t * TILE) - 1;                   // markers are local index + 1
+        const int base_j = (int)((i64)t * F_TILE) - 1;                        // markers are local index + 1
         const i64 rel_lo = tile_lo - out_begin;
         const int mis = (int)(((reinterpret_cast<uintptr_t>(p.idx) >> 2) + (uintptr_t)rel_lo) & 3);
-        if (tile_cnt + 3 <= WIN && rel_lo >= 0 && rel_lo + tile_cnt <= p.cap) {
+        if (tile_cnt + 3 <= WIN && rel_lo >= 0 && rel_lo + tile_cnt <= p.n) {
             // one window; slot 0 is 16-byte aligned in the index array, the tile's first output is slot `mis`
             const int total = (int)tile_cnt + mis;
             int l = hv_prev + mis;
@@ -1014,7 +948,7 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
             }
             f_bar<NT>();
             int m[F_SPT];
-            f_window_scan<NW>(sm, tid, lane, wid, m);
+            f_window_scan(sm, tid, lane, wid, m);
             const int s0 = tid * F_SPT;
             int *dst = p.idx + (rel_lo - mis) + s0;
             if (s0 >= mis && s0 + F_SPT <= total) {
@@ -1026,7 +960,6 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
                 for (int i = 0; i < F_SPT; i++)
                     if (s0 + i >= mis && s0 + i < total) dst[i] = base_j + m[i];
             }
-            clap(cemit);
             continue;      // the next barrier separates these window reads from the next tile's marker writes
         }
         // general expansion: several windows, runs of BIGRUN or more copies go to the fill kernel
@@ -1066,7 +999,7 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
             }
             f_bar<NT>();
             int m[F_SPT];
-            f_window_scan<NW>(sm, tid, lane, wid, m);
+            f_window_scan(sm, tid, lane, wid, m);
 #pragma unroll
             for (int i = 0; i < F_SPT; i++) {
                 const int sl2 = tid * F_SPT + i;
@@ -1076,12 +1009,6 @@ k_fused(const __grid_constant__ CUtensorMap wmap, const FParams p)
             cs = ce;
         }
         f_bar<NT>();
-        clap(cemit);
-    }
-    if (p.prof && tid == 0) {
-        atomicAdd(reinterpret_cast<unsigned long long *>(&p.hdr->prof[9]), (unsigned long long)cwait);
-        atomicAdd(reinterpret_cast<unsigned long long *>(&p.hdr->prof[10]), (unsigned long long)cfront);
-        atomicAdd(reinterpret_cast<unsigned long long *>(&p.hdr->prof[11]), (unsigned long long)cemit);
     }
 }
 
@@ -1093,13 +1020,11 @@ __global__ void __launch_bounds__(256) k_finit(FParams p)
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         FHeader h;
         memset(&h, 0, sizeof(h));
-        const double ca = p.carry_approx ? *p.carry_approx : 0.0;
-        const double ce = p.carry_exact ? *p.carry_exact : 0.0;
-        const double Ngd = (double)p.ng;
-        h.out_begin = p.cumsum_out ? 0 : (p.U ? count_below_str(ce, p.U, p.ng, Ngd) : count_below_sys(ce, p.u, p.ng, Ngd, p.tau));
+        const double Ngd = (double)p.n;
+        h.out_begin = p.U ? count_below_str(0.0, p.U, p.n, Ngd) : count_below_sys(0.0, p.u, p.n, Ngd, p.tau);
         *p.hdr = h;
-        p.st1[0] = ((u64)__double_as_longlong(ca) & ~3ull) | ST1_INCL;
-        p.st2[0] = ST2_INCL | (u64)__double_as_longlong(ce);
+        p.st1[0] = ST1_INCL;                       // the sums before the first tile: 0.0
+        p.st2[0] = ST2_INCL;
     }
 }
 
@@ -1108,7 +1033,7 @@ __global__ void __launch_bounds__(256) k_finit(FParams p)
 __global__ void __launch_bounds__(256) k_fepilogue(FParams p)
 {
     FHeader *hdr = p.hdr;
-    if (!hdr->fallback && p.idx) {
+    if (!hdr->fallback) {
         int nr = hdr->n_runs;
         if (nr > p.max_runs) nr = p.max_runs;
         const i64 ob = hdr->out_begin;
@@ -1116,18 +1041,12 @@ __global__ void __launch_bounds__(256) k_fepilogue(FParams p)
             const Run run = p.runs[r];
             for (i64 i = run.lo + (i64)blockIdx.x * blockDim.x + threadIdx.x; i < run.hi; i += (i64)gridDim.x * blockDim.x) {
                 const i64 rel = i - ob;
-                if (rel >= 0 && rel < p.cap) p.idx[rel] = run.j;
+                if (rel >= 0 && rel < p.n) p.idx[rel] = run.j;
                 else hdr->cap_overflow = 1;
             }
         }
     }
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
-    if (p.prof) {
-        const double T = (double)p.T;
-printf("RSPROF tiles=%d cycles/tile: C1[wait-fronted %.0f | lookback1 %.0f | map %.0f]  C2[wait-mapped %.0f | lookback2 %.0f | finish %.0f]  cons[wait %.0f | front %.0f | emit %.0f]  crossing=%d slow=%d general=%d\n",
-               p.T, hdr->prof[3] / T, hdr->prof[4] / T, hdr->prof[5] / T, hdr->prof[6] / T, hdr->prof[7] / T, hdr->prof[8] / T,
-               hdr->prof[9] / T, hdr->prof[10] / T, hdr->prof[11] / T, hdr->n_unclean, hdr->n_slow, hdr->n_general);
-    }
     auto write_info = [&](int overflow, int fb) {
         if (p.info) {
             p.info[0] = overflow; p.info[1] = fb; p.info[2] = hdr->n_unclean; p.info[3] = hdr->n_runs;
@@ -1138,21 +1057,12 @@ printf("RSPROF tiles=%d cycles/tile: C1[wait-fronted %.0f | lookback1 %.0f | map
     const double S = p.div ? *p.div : 1.0;
     auto W = [&](i64 q) { return p.div ? __ddiv_rn(p.w[q], S) : p.w[q]; };
     if (p.div && p.wnorm_out) for (i64 q = 0; q < p.n; q++) p.wnorm_out[q] = W(q);
-    if (p.cumsum_out) {                          // cumsum mode: np.cumsum, one add at a time
-        double c = 0.0;
-        for (i64 q = 0; q < p.n; q++) { c = (q == 0) ? W(0) : __dadd_rn(c, W(q)); p.cumsum_out[q] = c; }
-        if (p.cumsum_last) *p.cumsum_last = c;
-        if (p.last_one) p.cumsum_out[p.n - 1] = 1.0;
-        write_info(0, 1);
-        return;
-    }
-    // resampling.py:141-149 — cumulative sum and two-pointer merge, one element at a time.  A shard
-    // starts from the exact running sum of the earlier shards and owns the positions from
-    // count_below(carry) up to count_below(its last cumulative sum).
-    const double Ngd = (double)p.ng;
-    const double carry = p.carry_exact ? *p.carry_exact : 0.0;
+    // resampling.py:141-149 — cumulative sum and two-pointer merge, one element at a time, over the
+    // positions from count_below(0.0)
+    const double Ngd = (double)p.n;
+    const double carry = 0.0;
     auto pos = [&](i64 i) { return p.U ? pos_str(i, p.U, Ngd) : pos_sys(i, p.u, Ngd); };
-    i64 lo = 0, hi = p.ng;                       // first i with pos_i >= carry (positions are non-decreasing)
+    i64 lo = 0, hi = p.n;                        // first i with pos_i >= carry (positions are non-decreasing)
     while (lo < hi) {
         const i64 mid = (lo + hi) >> 1;
         if (pos(mid) < carry) lo = mid + 1; else hi = mid;
@@ -1161,19 +1071,17 @@ printf("RSPROF tiles=%d cycles/tile: C1[wait-fronted %.0f | lookback1 %.0f | map
     hdr->out_begin = ob;
     hdr->cap_overflow = 0;
     i64 i = ob, j = 0;
-    double c = (carry == 0.0) ? W(0) : __dadd_rn(carry, W(0));
+    double c = W(0);
     int overflow = 0;
-    while (i < p.ng) {
+    while (i < p.n) {
         if (pos(i) < c) {
-            if (i - ob < p.cap) p.idx[i - ob] = (int)(p.j0 + j); else hdr->cap_overflow = 1;
+            if (i - ob < p.n) p.idx[i - ob] = (int)j; else hdr->cap_overflow = 1;
             i++;
         } else {
             j++;
             if (j >= p.n) {
-                if (p.is_last) {
-                    overflow = (int)(p.ng - i);
-                    for (; i < p.ng; i++) { if (i - ob < p.cap) p.idx[i - ob] = (int)(p.ng - 1); else hdr->cap_overflow = 1; }
-                }
+                overflow = (int)(p.n - i);
+                for (; i < p.n; i++) { if (i - ob < p.n) p.idx[i - ob] = (int)(p.n - 1); else hdr->cap_overflow = 1; }
                 break;
             }
             c = __dadd_rn(c, W(j));
@@ -1182,7 +1090,6 @@ printf("RSPROF tiles=%d cycles/tile: C1[wait-fronted %.0f | lookback1 %.0f | map
     for (i64 q = j + 1; q < p.n; q++) c = __dadd_rn(c, W(q));
     if (p.cumsum_last) *p.cumsum_last = c;
     hdr->out_end = i;
-    if (p.out_range) { p.out_range[0] = ob; p.out_range[1] = i; }
     write_info(overflow, 1);
 }
 
@@ -1241,17 +1148,11 @@ bool f_weights_map(const double *w, int64_t n, int box_rows, CUtensorMap *out)
 
 namespace {
 
-int f_env_int(const char *name, int dflt)
-{
-    const char *v = getenv(name);
-    return v ? atoi(v) : dflt;
-}
-
-template <int NW, int DELTA, int MODE>
+template <int MODE>
 int f_launch(const CUtensorMap &map, const FParams &p, cudaStream_t s)
 {
-    auto kern = k_fused<NW, DELTA, MODE>;
-    const int smem = (int)sizeof(FSmem<NW>);
+    auto kern = k_fused<MODE>;
+    const int smem = (int)sizeof(FSmem);
     static bool configured[64] = {false};
     int dev = 0;
     cudaGetDevice(&dev);
@@ -1259,31 +1160,17 @@ int f_launch(const CUtensorMap &map, const FParams &p, cudaStream_t s)
         if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
         if (dev >= 0 && dev < 64) configured[dev] = true;
     }
-    const int ctas_env = f_env_int("BKE_RS_CTAS", 0);
-    const int per_sm = ctas_env > 0 ? ctas_env : f_ctas(NW);
-    int grid = sm_count() * per_sm;
+    int grid = sm_count() * F_CTAS;
     if (grid > p.T) grid = p.T;
-    kern<<<grid, NW * 32 + 128, smem, s>>>(map, p);
+    kern<<<grid, NT + 128, smem, s>>>(map, p);
     return check_cuda(cudaGetLastError(), "k_fused launch");
-}
-
-template <int NW, int DELTA>
-int f_launch_mode(int mode, const CUtensorMap &map, const FParams &p, cudaStream_t s)
-{
-    if (mode == F_CUMSUM) return f_launch<NW, DELTA, F_CUMSUM>(map, p, s);
-    if (mode == F_STRAT) return f_launch<NW, DELTA, F_STRAT>(map, p, s);
-    return f_launch<NW, DELTA, F_SYS>(map, p, s);
 }
 
 }  // namespace
 
-static unsigned long long *g_trace = nullptr;
-void f_set_trace(void *buf) { g_trace = (unsigned long long *)buf; }
-
 size_t f_carve(int64_t n, unsigned char *base, FParams *p)
 {
-    // the smallest tile any variant uses decides the number of status words
-    const int64_t Tmax = (n + 4 * 32 * F_IPT - 1) / (4 * 32 * F_IPT);
+    const int64_t Tmax = (n + F_TILE - 1) / F_TILE;
     size_t off = 0;
     auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
     auto take = [&](size_t bytes) { size_t o = off; off += al(bytes); return base ? base + o : nullptr; };
@@ -1299,50 +1186,35 @@ size_t f_carve(int64_t n, unsigned char *base, FParams *p)
 int f_run(const FRunArgs &a, cudaStream_t s)
 {
     const i64 n = a.n;
-    if (n < 0 || a.ng < n || a.j0 < 0) { set_error("bad particle counts"); return BKE_ERR_BAD_ARG; }
+    if (n < 0) { set_error("bad particle counts"); return BKE_ERR_BAD_ARG; }
     if (n == 0) return BKE_OK;
-    if (a.ng >= ((i64)1 << 31)) { set_error("n must be < 2^31 (indexes are int32, resampling.py:141)"); return BKE_ERR_BAD_ARG; }
-    if (!a.w || !(a.idx || a.cumsum_out) || !a.workspace) { set_error("weights, indexes and workspace must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    if (!a.U && !a.cumsum_out && !(a.u >= 0.0 && a.u < 1.0)) { set_error("u must be in [0, 1)"); return BKE_ERR_BAD_ARG; }
+    if (n >= ((i64)1 << 31)) { set_error("n must be < 2^31 (indexes are int32, resampling.py:141)"); return BKE_ERR_BAD_ARG; }
+    if (!a.w || !a.idx || !a.workspace) { set_error("weights, indexes and workspace must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if (!a.U && !(a.u >= 0.0 && a.u < 1.0)) { set_error("u must be in [0, 1)"); return BKE_ERR_BAD_ARG; }
     const size_t need = f_carve(n, nullptr, nullptr);
     if (a.ws_bytes < need) { set_error("workspace too small: %zu < %zu", a.ws_bytes, need); return BKE_ERR_BAD_ARG; }
     if (reinterpret_cast<uintptr_t>(a.workspace) & 255) { set_error("workspace must be 256-byte aligned"); return BKE_ERR_BAD_ARG; }
     FParams p;
     memset(&p, 0, sizeof(p));
     f_carve(n, (unsigned char *)a.workspace, &p);
-    const int nw_env = f_env_int("BKE_RS_WARPS", 8);
-    const int NW = (nw_env == 4) ? 4 : 8;
-    p.sleep_ns = f_env_int("BKE_RS_SLEEP", 0);
-    p.prof = f_env_int("BKE_RS_PROF", 0);
-    p.trace = g_trace;
-    p.lbk = f_env_int("BKE_RS_LBK", 4);
-    if (p.lbk < 1) p.lbk = 1;
-    if (p.lbk > LBK_MAX) p.lbk = LBK_MAX;
-    const int tile = NW * 32 * F_IPT;
-    p.w = a.w; p.n = n; p.ng = a.ng; p.j0 = a.j0; p.cap = a.cap; p.is_last = a.is_last;
-    p.carry_approx = a.carry_approx; p.carry_exact = a.carry_exact; p.out_range = a.out_range;
+    p.w = a.w; p.n = n;
     p.u = a.u; p.U = a.U; p.idx = a.idx; p.info = a.info; p.cumsum_last = a.cumsum_last;
-    p.cumsum_out = a.cumsum_out; p.last_one = a.last_one; p.div = a.div; p.wnorm_out = a.wnorm_out;
-    p.T = (int)((n + tile - 1) / tile);
+    p.div = a.div; p.wnorm_out = a.wnorm_out;
+    p.T = (int)((n + F_TILE - 1) / F_TILE);
     // |exact sequential sum - approximate sum| in ulps of the running sum: N adds of the reference,
     // the tree sums inside a tile, the T sequential adds and the 2 flag bits per published word of
     // the look-back (and the division of a normalised call); doubled, plus slack.
-    const i64 Tg = a.ng / tile + 2;
-    p.eb = 2 * (a.ng + 16 * Tg + 2 * tile) + (a.ng >> 4);
-    const double tau = ldexp((double)a.ng, -46);
+    const i64 Tg = n / F_TILE + 2;
+    p.eb = 2 * (n + 16 * Tg + 2 * F_TILE) + (n >> 4);
+    const double tau = ldexp((double)n, -46);
     p.tau = tau > 1e-6 ? tau : 1e-6;
     // TMA path: 16-byte aligned base and at least one full row of 16 weights
     CUtensorMap map;
     memset(&map, 0, sizeof(map));
-    p.use_tma = f_env_int("BKE_RS_TMA", 1) && f_weights_map(a.w, n, NW * 32, &map);
+    p.use_tma = f_weights_map(a.w, n, NT, &map);
     const int init_blocks = (int)((p.T + 1 + 255) / 256) < 64 ? (int)((p.T + 1 + 255) / 256) : 64;
     k_finit<<<init_blocks, 256, 0, s>>>(p);
-    int rc;
-    const int mode = a.cumsum_out ? F_CUMSUM : (a.U ? F_STRAT : F_SYS);
-    // BKE_RS_STAGES = DELTA: how many tiles per CTA the front (sum, map, chain) runs ahead of the emit
-    const int st = f_env_int("BKE_RS_STAGES", 3);
-    if (NW == 4) rc = st <= 2 ? f_launch_mode<4, 2>(mode, map, p, s) : (st == 3 ? f_launch_mode<4, 3>(mode, map, p, s) : f_launch_mode<4, 5>(mode, map, p, s));
-    else rc = st <= 2 ? f_launch_mode<8, 2>(mode, map, p, s) : (st == 3 ? f_launch_mode<8, 3>(mode, map, p, s) : f_launch_mode<8, 5>(mode, map, p, s));
+    const int rc = a.U ? f_launch<F_STRAT>(map, p, s) : f_launch<F_SYS>(map, p, s);
     if (rc != BKE_OK) return rc;
     k_fepilogue<<<sm_count() * 4, 256, 0, s>>>(p);
     return check_cuda(cudaGetLastError(), "resample launch");

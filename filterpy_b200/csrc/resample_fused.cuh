@@ -1,4 +1,5 @@
-// resample_fused.cuh — interface of the single-pass resampling kernel (csrc/resample_fused.cu).
+// resample_fused.cuh — interface of the single-pass resampling kernel behind bke_resample_normalized
+// (csrc/resample_fused.cu), and the PTX wrappers the multi-pass emit kernel shares with it.
 #pragma once
 #include <cuda.h>
 #include "resample_common.cuh"
@@ -9,7 +10,7 @@ namespace rs {
 constexpr int F_IPT = 16;        // particles per consumer thread and tile
 constexpr int F_SPT = 20;        // output-window slots per consumer thread (5 x 16 bytes)
 constexpr int F_STAGES = 2;      // shared-memory tiles per CTA (one in flight while one is processed)
-enum { F_SYS = 0, F_STRAT = 1, F_CUMSUM = 2 };
+enum { F_SYS = 0, F_STRAT = 1 };
 
 struct FHeader {
     int fallback;       // 1 -> the sequential kernel must produce the result
@@ -18,28 +19,20 @@ struct FHeader {
     int overflow;       // positions >= cumsum[-1]
     int chain_bad;      // a verified assumption failed
     int n_seq;          // tiles walked element by element
-    int cap_overflow;   // outputs that did not fit the caller's index buffer (sharded calls)
+    int cap_overflow;   // outputs that did not fit the index buffer (never expected)
     int n_slow;         // tiles that took the slow path (ties / raw elements)
     int tile_counter;   // next tile to hand out
     int timeout;        // a look-back gave up waiting (never expected)
     int n_general;      // tiles expanded through more than one window
     int pad;
-    i64 out_begin;      // first global output position owned by this call
+    i64 out_begin;      // first output position owned by this call (0)
     i64 out_end;        // one past the last
-    i64 prof[12];       // BKE_RS_PROF: cycles summed over CTAs (producer phases 0-5, consumer wait / work)
 };
 
 struct FParams {
     const double *w;
-    i64 n;                 // particles in this call (this shard)
-    i64 ng;                // particles of the whole set: positions are (u + i) / ng
-    i64 j0;                // global index of this call's first particle
-    i64 cap;               // capacity of idx
-    int is_last;           // this call holds the end of the particle set
+    i64 n;                 // particles: positions are (u + i) / n, idx holds n indexes
     int use_tma;           // weights are 16-byte aligned: tiles arrive by TMA
-    const double *carry_approx;   // device: approximate sum of the earlier shards (NULL = 0)
-    const double *carry_exact;    // device: exact running sum before this shard (NULL = 0)
-    i64 *out_range;        // device int64[2] (NULL ok)
     double u;              // systematic offset
     const double *U;       // stratified uniforms (NULL = systematic)
     int *idx;
@@ -47,8 +40,6 @@ struct FParams {
     double tau;            // fast-path margin of the position search
     int *info;             // user info[8] or NULL
     double *cumsum_last;   // or NULL
-    double *cumsum_out;    // non-NULL: write the exact np.cumsum(w) here instead of emitting indexes
-    int last_one;          // cumsum mode: store 1.0 as the last element (resampling.py:174)
     const double *div;     // non-NULL: every weight is divided by *div first (fused normalisation)
     double *wnorm_out;     // optional: the normalised weights
     FHeader *hdr;
@@ -56,23 +47,15 @@ struct FParams {
     Run *runs;
     int max_runs;
     int T;
-    int sleep_ns;          // back-off between two polls of a status word (0 = spin)
-    unsigned long long *trace;   // debugging: [T][10] global-timer stamps of pipeline events, or NULL
-    int prof;              // BKE_RS_PROF=1: per-phase cycle counters, printed by the epilogue kernel
-    int lbk;               // status words per lane and look-back round (window = 32 * lbk tiles)
 };
 
 struct FRunArgs {
-    i64 n, ng, j0, cap;
+    i64 n;
     const double *w, *U;
     double u;
     int *idx;
     void *workspace; size_t ws_bytes;
     int *info; double *cumsum_last;
-    const double *carry_approx, *carry_exact;
-    i64 *out_range;
-    int is_last;
-    double *cumsum_out; int last_one;
     const double *div; double *wnorm_out;
 };
 
@@ -141,7 +124,6 @@ bool f_weights_map(const double *w, int64_t n, int box_rows, CUtensorMap *out);
 
 size_t f_carve(int64_t n, unsigned char *base, FParams *p);
 int f_run(const FRunArgs &a, cudaStream_t s);
-void f_set_trace(void *buf);
 
 }  // namespace rs
 }  // namespace bke

@@ -1,7 +1,6 @@
 // ukf.cu — host side of the unscented Kalman filter bank: the closed set of pre-built (dim_x, dim_z,
 // fx, hx) instances of the kernel in ukf_kernel.cuh and their launch.  (Instances around user-supplied
 // fx / hx are compiled at run time: ukf_rtc.cu.)
-#include <stdlib.h>
 #include "ukf_kernel.cuh"
 #include "ukf_launch.cuh"
 
@@ -15,17 +14,9 @@ int launch_inst(const bke_ukf_args &a, cudaStream_t s)
     UkfP<T> p;
     ukf_fill_params<T>(a, N, p);
     const size_t smem = ukf_smem_bytes<T>(N, M, FX == BKE_FX_LINEAR, a.F_stride == 0, HX == BKE_HX_LINEAR, a.H_stride == 0);
-    // resident CTAs per SM the kernel is compiled for (registers are capped accordingly): for n = 6, 3 in fp64
-    // and 5 in fp32 (BKE_UKF_OCC overrides)
-    static const int occ_env = [] { const char *e = getenv("BKE_UKF_OCC"); return e ? atoi(e) : 0; }();
-    constexpr int OCC_DEFAULT = N >= 6 ? (sizeof(T) == 8 ? 3 : 5) : 1;
-    const int occ = (occ_env >= 1 && occ_env <= 5 && N >= 6) ? occ_env : OCC_DEFAULT;
+    constexpr int OCC = ukf_occupancy(N, sizeof(T) == 8);
     const bool ex = a.x_prior || a.P_prior || a.K || a.y || a.S || a.SI || a.log_likelihood;
-    constexpr int O3 = N >= 6 ? 3 : 1, O4 = N >= 6 ? 4 : 1, O5 = N >= 6 ? 5 : 1;
-    auto kern = ex ? ukf_kernel<T, N, M, FX, HX, 1, true> : ukf_kernel<T, N, M, FX, HX, 1, false>;
-    if (occ == 3) kern = ex ? ukf_kernel<T, N, M, FX, HX, O3, true> : ukf_kernel<T, N, M, FX, HX, O3, false>;
-    if (occ == 4) kern = ex ? ukf_kernel<T, N, M, FX, HX, O4, true> : ukf_kernel<T, N, M, FX, HX, O4, false>;
-    if (occ == 5) kern = ex ? ukf_kernel<T, N, M, FX, HX, O5, true> : ukf_kernel<T, N, M, FX, HX, O5, false>;
+    auto kern = ex ? ukf_kernel<T, N, M, FX, HX, OCC, true> : ukf_kernel<T, N, M, FX, HX, OCC, false>;
     if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
     int64_t grid = (p.N + UB - 1) / UB;
     kern<<<(unsigned)grid, UB, smem, s>>>(p);

@@ -5,6 +5,13 @@
 
 namespace bke {
 
+// resident CTAs per SM an instance is compiled for (its registers are capped accordingly): for n >= 6,
+// 3 in fp64 and 5 in fp32; smaller states need no cap
+constexpr int ukf_occupancy(int n, bool f64)
+{
+    return n >= 6 ? (f64 ? 3 : 5) : 1;
+}
+
 template <typename T>
 inline void ukf_fill_params(const bke_ukf_args &a, int N, ukfk::UkfP<T> &p)
 {

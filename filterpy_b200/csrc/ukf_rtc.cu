@@ -138,8 +138,7 @@ static int compile_cubin(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx
     if (uhx) text += "template <> __device__ __forceinline__ void bke_user_hx<real>(const real *x, real *z, const real *args) { ::hx(x, z, args); }\n";
     text += "} }\n";
 
-    // resident CTAs the instance is compiled for: the pre-built kernels' choice (ukf.cu)
-    const int occ = dim_x >= 6 ? (dtype == BKE_F64 ? 3 : 5) : 1;
+    const int occ = ukf_occupancy(dim_x, dtype == BKE_F64);
     bke_ukf_model tmp;
     tmp.n = dim_x; tmp.m = dim_z; tmp.fx_model = fx_model; tmp.hx_model = hx_model;
     nvrtcProgram prog;
