@@ -16,6 +16,7 @@
 #include <type_traits>
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
+#include "ptx.cuh"
 
 namespace bke {
 namespace {
@@ -31,16 +32,6 @@ struct BatchP {
     T *x_out, *P_out, *means, *covs, *means_p, *covs_p;
     int32_t *status;
 };
-
-__device__ __forceinline__ uint32_t bsmem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void b_fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void b_bulk_store(void *dst, const void *src, uint32_t bytes)
-{
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(bsmem_u32(src)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void b_bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void b_bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-__device__ __forceinline__ void b_bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 template <typename T, int CNT>
 __device__ __forceinline__ void load_vec(T *dst, const T *src)
@@ -103,7 +94,7 @@ __global__ void __launch_bounds__(128) kf_batch_kernel(BatchP<T> p)
         const int64_t tf = t * p.N + f;
         unsigned char *buf = wst + (t & 1) * St::BYTES;
         if (staged) {
-            if (lane == 0) b_bulk_wait_read1();               // the copies of epoch t-2 have read this buffer
+            if (lane == 0) bulk_wait_read<1>();               // the copies of epoch t-2 have read this buffer
             __syncwarp();
         }
         T z[M];
@@ -140,19 +131,19 @@ __global__ void __launch_bounds__(128) kf_batch_kernel(BatchP<T> p)
         };
         if (p.update_first) { upd(); pred(); } else { pred(); upd(); }
         if (staged) {
-            b_fence_proxy_async();                            // the staged rows become visible to the copy engine
+            fence_proxy_async();                              // the staged rows become visible to the copy engine
             __syncwarp();
             if (lane == 0) {
                 const int64_t e0 = t * p.N + f0;
-                if (p.means_p) b_bulk_store(p.means_p + e0 * N, buf + St::O_XP, St::XB);
-                if (p.covs_p) b_bulk_store(p.covs_p + e0 * N * N, buf + St::O_PP, St::PB);
-                if (p.means) b_bulk_store(p.means + e0 * N, buf + St::O_X, St::XB);
-                if (p.covs) b_bulk_store(p.covs + e0 * N * N, buf + St::O_P, St::PB);
-                b_bulk_commit();
+                if (p.means_p) bulk_store(p.means_p + e0 * N, buf + St::O_XP, St::XB);
+                if (p.covs_p) bulk_store(p.covs_p + e0 * N * N, buf + St::O_PP, St::PB);
+                if (p.means) bulk_store(p.means + e0 * N, buf + St::O_X, St::XB);
+                if (p.covs) bulk_store(p.covs + e0 * N * N, buf + St::O_P, St::PB);
+                bulk_commit();
             }
         }
     }
-    if (staged && lane == 0) b_bulk_wait_all();
+    if (staged && lane == 0) bulk_wait_all();
     store_vec<T, N>(p.x_out + f * N, x);
     store_vec<T, N * N>(p.P_out + f * N * N, &P[0][0]);
     if (p.status) p.status[f] = st;

@@ -24,66 +24,15 @@
 #include <string.h>
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
+#include "ptx.cuh"
 
 namespace bke {
 namespace {
 
-// ---------------------------------------------------------------------------- PTX wrappers
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// 1-D bulk copy of `bytes` (a multiple of 16, both addresses 16-byte aligned) into shared memory
-__device__ __forceinline__ void bulk_load(void *dst, const void *src, uint32_t bytes, uint64_t *bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-// variant with an L2 eviction-priority hint (createpolicy): the state x, P is re-read by the NEXT
-// step and, for banks whose state is at most 38 MB (about 498 k filters; a bound scaled from an earlier target, not
+// L2 eviction priorities (bulk_load_hint, st_hint): the state x, P is re-read by the NEXT step and, for
+// banks whose state is at most 38 MB (about 498 k filters; a bound scaled from an earlier target, not
 // measured on the H100), fits the 50 MB L2 -> evict_last; the models and measurements
 // stream through once per step -> evict_first, so that they do not push the state out.
-__device__ __forceinline__ void bulk_load_hint(void *dst, const void *src, uint32_t bytes, uint64_t *bar, uint64_t pol)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
-                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
-}
-// programmatic dependent launch: wait until the previous kernel on the stream has completed and its
-// writes are visible / allow the next one (launched with programmatic stream serialization) to start
-__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ uint64_t policy_evict_first()
-{
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-__device__ __forceinline__ uint64_t policy_evict_last()
-{
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
 __device__ __forceinline__ void st_hint(float *addr, float4 v, uint64_t pol)
 {
     asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;"

@@ -19,45 +19,10 @@
 #include <type_traits>
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
+#include "ptx.cuh"
 
 namespace bke {
 namespace {
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "RB_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra RB_DONE;\n"
-        "bra RB_WAIT;\n"
-        "RB_DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_load(void *dst, const void *src, uint32_t bytes, uint64_t *bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void bulk_store(void *dst, const void *src, uint32_t bytes)
-{
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(smem_u32(src)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 template <typename T>
 struct RbP {
@@ -504,7 +469,7 @@ __global__ void __launch_bounds__(RB_WARPS * 32, 1) kf_rowblock_kernel(RbP<T> p)
         }
         // ---------------- posterior rows -> staging -> bulk TMA store ---------------------------
         // the prior's stores (optional outputs) have read the stage slots the posterior is about to overwrite
-        if (lane == 0 && EXTRAS) bulk_wait_read();
+        if (lane == 0 && EXTRAS) bulk_wait_read<0>();
         __syncwarp();                                       // every lane is done with P', (I-KH), K in the stage
         if (active) {
 #pragma unroll
@@ -530,7 +495,7 @@ __global__ void __launch_bounds__(RB_WARPS * 32, 1) kf_rowblock_kernel(RbP<T> p)
             }
             bulk_commit();
             // the stores have read the stage (and the staging area of the optional outputs): it may be refilled
-            bulk_wait_read();
+            bulk_wait_read<0>();
             const int64_t nt = tile + RB_STAGES * wstride;
             if (nt < tiles) issue(nt, stage);
         }

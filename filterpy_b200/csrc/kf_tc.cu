@@ -31,11 +31,10 @@
 #include <stdlib.h>
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
+#include "ptx.cuh"
 
 namespace bke {
 namespace tc {
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 template <int NX>
 struct Geom {
@@ -98,7 +97,6 @@ template <> __device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint6
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // accumulator fragment of m64nNk8 (fp32): register 4 q + 2 h + e of thread (warp w, lane l) holds
 // row 16 w + l / 4 + 8 h, column 8 q + 2 (l % 4) + e of the 64-row half

@@ -1,0 +1,114 @@
+// ptx.cuh — Hopper (sm_90a) PTX wrappers shared by the kernels: mbarriers, bulk and tensor copies
+// (cp.async.bulk), programmatic dependent launch, L2 cache policies and relaxed global loads / stores.
+#pragma once
+#include <cuda.h>
+#include <stdint.h>
+
+namespace bke {
+
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// ---------------------------------------------------------------------------- mbarriers
+__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count)
+{
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+}
+__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes)
+{
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar)
+{
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// one test of the phase with the given parity (true: it has completed)
+__device__ __forceinline__ bool mbar_try(uint64_t *bar, uint32_t parity)
+{
+    uint32_t ok;
+    asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
+                 : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+    return ok != 0;
+}
+// wait for the phase with the given parity (the try-wait loop in PTX)
+__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
+{
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "WAIT_LOOP:\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+        "@p bra DONE;\n"
+        "bra WAIT_LOOP;\n"
+        "DONE:\n"
+        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
+}
+
+// orders this thread's generic-proxy shared-memory accesses before later async-proxy (bulk copy) ones
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ---------------------------------------------------------------------------- bulk copies
+// 1-D bulk copy of `bytes` (a multiple of 16, both addresses 16-byte aligned) into shared memory
+__device__ __forceinline__ void bulk_load(void *dst, const void *src, uint32_t bytes, uint64_t *bar)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+// the same with an L2 cache policy (policy_evict_first / policy_evict_last)
+__device__ __forceinline__ void bulk_load_hint(void *dst, const void *src, uint32_t bytes, uint64_t *bar, uint64_t pol)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
+}
+// 1-D bulk copy from shared to global memory, tracked by bulk groups (bulk_commit / bulk_wait_*)
+__device__ __forceinline__ void bulk_store(void *dst, const void *src, uint32_t bytes)
+{
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(smem_u32(src)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N committed groups still read their shared-memory source
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// 2-D tensor copy of the box at (c0, c1) of `map` into shared memory
+__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar)
+{
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
+}
+
+// ---------------------------------------------------------------------------- grid dependency control
+// programmatic dependent launch: wait until the previous kernel on the stream has completed and its
+// writes are visible / allow the next one (launched with programmatic stream serialization) to start
+__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+// ---------------------------------------------------------------------------- L2 cache policies
+__device__ __forceinline__ uint64_t policy_evict_first()
+{
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t policy_evict_last()
+{
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+
+// ---------------------------------------------------------------------------- relaxed global accesses
+// (status words that other CTAs poll: never served from a stale L1 line)
+__device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long long *p)
+{
+    unsigned long long v;
+    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_relaxed_u64(unsigned long long *p, unsigned long long v)
+{
+    asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+
+}  // namespace bke

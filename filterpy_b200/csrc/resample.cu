@@ -30,7 +30,7 @@
 //   F  long runs (one particle copied >= 8192 times)             writes indexes
 //   G  sequential fallback (normally exits at once), info
 #include "resample_common.cuh"
-#include "resample_fused.cuh"
+#include "ptx.cuh"
 #include <stdlib.h>
 
 namespace bke {
@@ -139,21 +139,45 @@ struct Params {
     int last_one;          // cumsum mode: store 1.0 as the last element (resampling.py:174)
     int scan_done;         // the segmented scan of the tile maps (chain_scan) has been run by k_compose
     Ws ws;
+    const double *div;     // NORM instances: every weight is divided by *div where it is read
+    double *wnorm_out;     // NORM instances, optional: pass A writes the divided weights here
 };
 
+// A normalised call (bke_resample_normalized) resamples w / S: its kernels are the NORM = true instances,
+// which read d = *p.div once and divide every weight they load, __ddiv_rn(w, d) as NumPy's w / w.sum().
+// Everything downstream, validation included, sees the divided values.  NORM = false reads w as it is.
+template <bool NORM> __device__ __forceinline__ double divisor(const Params &p) { return NORM ? *p.div : 1.0; }
+template <bool NORM> __device__ __forceinline__ double wdiv(double w, double d) { return NORM ? __ddiv_rn(w, d) : w; }
+template <bool NORM> __device__ __forceinline__ void normalise(double2 (&g)[IPT / 2], double d)
+{
+#pragma unroll
+    for (int i = 0; i < IPT / 2; i++) { g[i].x = wdiv<NORM>(g[i].x, d); g[i].y = wdiv<NORM>(g[i].y, d); }
+}
+
 // ------------------------------------------------------------------ pass A: tile sums
+// (NORM: also writes the divided weights to p.wnorm_out when it is non-NULL)
+template <bool NORM>
 __global__ void __launch_bounds__(BLOCK) k_tile_sums(Params p)
 {
     __shared__ double sh[BLOCK / 32 + 1];
     const int t = blockIdx.x;
     const i64 base = (i64)t * TILE;
+    const double d = divisor<NORM>(p);
     double s = 0.0;
     bool bad = false;
     if (p.aligned16 && base + TILE <= p.n) {
         const double2 *src = reinterpret_cast<const double2 *>(p.w + base);
 #pragma unroll
         for (int i = 0; i < IPT / 2; i++) {
-            const double2 v = src[i * BLOCK + threadIdx.x];
+            double2 v = src[i * BLOCK + threadIdx.x];
+            if (NORM) {
+                v.x = wdiv<NORM>(v.x, d); v.y = wdiv<NORM>(v.y, d);
+                if (p.wnorm_out) {
+                    double *o = p.wnorm_out + base + 2 * (i * BLOCK + threadIdx.x);
+                    if ((reinterpret_cast<uintptr_t>(o) & 15) == 0) *reinterpret_cast<double2 *>(o) = v;
+                    else { o[0] = v.x; o[1] = v.y; }
+                }
+            }
             if (!(v.x >= 0.0) || !(v.y >= 0.0) || isinf(v.x) || isinf(v.y)) bad = true;
             s += v.x + v.y;
         }
@@ -161,7 +185,8 @@ __global__ void __launch_bounds__(BLOCK) k_tile_sums(Params p)
 #pragma unroll
         for (int i = 0; i < IPT; i++) {
             const i64 j = base + i * BLOCK + threadIdx.x;
-            const double w = (j < p.n) ? p.w[j] : 0.0;
+            const double w = (j < p.n) ? wdiv<NORM>(p.w[j], d) : 0.0;
+            if (NORM && p.wnorm_out && j < p.n) p.wnorm_out[j] = w;
             if (!(w >= 0.0) || isinf(w)) bad = true;
             s += w;
         }
@@ -363,14 +388,17 @@ struct MapsShared {
 // approximate tile prefixes and the elements themselves) gets its map as a plain int64 sum, straight
 // from the striped registers.  Everything else is queued for the general kernel.  One tile per CTA and no
 // register double-buffer: few registers, many resident CTAs — the way pass A reaches the HBM roofline.
+template <bool NORM>
 __global__ void __launch_bounds__(BLOCK, 5) k_tile_maps_fast1(Params p)
 {
     __shared__ i64 shi[BLOCK / 32 + 1];
     const int t = blockIdx.x;
+    const double d = divisor<NORM>(p);
     const double tp = p.ws.tile_prefix[t], tp_next = p.ws.tile_prefix[t + 1];
     double2 g[IPT / 2];
     fetch_tile(p, t, g);
     if (p.ws.hdr->fallback) return;
+    normalise<NORM>(g, d);
     int e0;
     const bool tile_clean = clean_add(tp, tp_next, p.eb, &e0);
     const i64 base = (i64)e0 << 52;
@@ -414,6 +442,20 @@ constexpr u64 ST_AGG = 1, ST_INCL = 2;
 constexpr int FRONT_SPINS = 1 << 20;      // polls of a blocked window before giving up (-> sequential fallback)
 constexpr int FRONT_LBK = 8;              // status words per lane and poll: a window of 256 tiles
 
+// named barrier 1 of the first NT threads (k_front: the data warps, k_emit2: the consumer warps; the
+// remaining warp never joins it)
+template <int NT> __device__ __forceinline__ void bar_sync()
+{
+    asm volatile("barrier.cta.sync 1, %0;" ::"n"(NT) : "memory");
+}
+template <int NT> __device__ __forceinline__ int bar_and(int pred)
+{
+    int out;
+    asm volatile("{\n.reg .pred p, q;\nsetp.ne.b32 p, %1, 0;\nbarrier.cta.red.and.pred q, 1, %2, p;\nselp.b32 %0, 1, 0, q;\n}\n"
+                 : "=r"(out) : "r"(pred), "n"(NT) : "memory");
+    return out;
+}
+
 // With ~600 tiles in flight and one tile retiring every ~6 ns the nearest tile that already owns an
 // inclusive prefix is ~200 tiles back (poll latency / tile period), so a 32-tile window would need
 // 6-7 dependent polls; eight independent loads per lane cover that distance in one round trip.
@@ -428,7 +470,7 @@ __device__ __forceinline__ double front_lookback(const Params &p, int t, int lan
 #pragma unroll
         for (int j = 0; j < FRONT_LBK; j++) {
             const int i = idx - 32 * j;
-            v[j] = (i >= 0) ? f_ld(p.ws.st1 + i) : ST_INCL;           // before the first tile: 0.0, inclusive
+            v[j] = (i >= 0) ? ld_relaxed_u64(p.ws.st1 + i) : ST_INCL;           // before the first tile: 0.0, inclusive
         }
         bool blocked = false;
 #pragma unroll
@@ -470,7 +512,7 @@ __global__ void __launch_bounds__(BLOCK + 32, 4) k_front(Params p)
         __syncthreads();
         if (lane == 0) {
             const double tot = s_tot;
-            f_st(p.ws.st1 + t, ((u64)__double_as_longlong(ex + tot) & ~3ull) | ST_INCL);
+            st_relaxed_u64(p.ws.st1 + t, ((u64)__double_as_longlong(ex + tot) & ~3ull) | ST_INCL);
             const double tp = (p.carry_approx ? *p.carry_approx : 0.0) + ex;
             p.ws.tile_prefix[t] = tp;
             if (t == T - 1) p.ws.tile_prefix[T] = tp + tot;
@@ -491,12 +533,12 @@ __global__ void __launch_bounds__(BLOCK + 32, 4) k_front(Params p)
     if (lane == 0) shd[wid] = s;
     if (threadIdx.x == 0) shi[BLOCK / 32] = 0;             // "some weight of the tile is non-zero"
     if (bad) p.ws.hdr->fallback = 1;
-    f_bar<BLOCK>();
+    bar_sync<BLOCK>();
     if (wid == 0) {
         double tot = 0.0;
 #pragma unroll
         for (int i = 0; i < BLOCK / 32; i++) tot += shd[i];
-        if (lane == 0) { f_st(p.ws.st1 + t, ((u64)__double_as_longlong(tot) & ~3ull) | ST_AGG); p.ws.tile_sum[t] = tot; s_tot = tot; }
+        if (lane == 0) { st_relaxed_u64(p.ws.st1 + t, ((u64)__double_as_longlong(tot) & ~3ull) | ST_AGG); p.ws.tile_sum[t] = tot; s_tot = tot; }
     }
     __syncthreads();
     const double tp = (p.carry_approx ? *p.carry_approx : 0.0) + s_ex;
@@ -522,7 +564,7 @@ __global__ void __launch_bounds__(BLOCK + 32, 4) k_front(Params p)
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(FULL, acc, o);
     nz = __any_sync(FULL, nz);
     if (lane == 0) { shi[wid] = acc; if (nz) shi[BLOCK / 32] = 1; }
-    if (f_bar_and<BLOCK>(ok)) {
+    if (bar_and<BLOCK>(ok)) {
         if (threadIdx.x == 0) {
             i64 total = 0;
 #pragma unroll
@@ -536,16 +578,19 @@ __global__ void __launch_bounds__(BLOCK + 32, 4) k_front(Params p)
 }
 
 // General kernel over the slow list: ties, raw elements, sequential tiles.
+template <bool NORM>
 __global__ void __launch_bounds__(BLOCK, 2) k_tile_maps(Params p)
 {
     __shared__ MapsShared sm;
     if (p.ws.hdr->fallback) return;
+    const double d = divisor<NORM>(p);
     const int n_slow = p.ws.hdr->n_slow;
     for (int li = blockIdx.x; li < n_slow; li += gridDim.x) {
         const int t = p.ws.slow_list[li];
         const double tp = p.ws.tile_prefix[t];
         double2 g[IPT / 2];
         fetch_tile(p, t, g);
+        normalise<NORM>(g, d);
         TileAn an;
         to_blocked(g, an.w, sm.buf);
         double s = 0.0;
@@ -700,7 +745,7 @@ __device__ __forceinline__ void chain_scan(const Ws &ws, SM *wtot, int &bad, int
 // NC = 1: one CTA; NC = CHAIN_CTAS: one thread-block cluster, every CTA scans / finishes its own range of
 // tiles (the single CTA was bound by what one SM can move: ~4.6 MB of tile records at 2^26), CTA 0 walks
 // the tiles with raw elements while the others wait at the cluster barrier.
-template <bool STRAT, int NC>
+template <bool STRAT, int NC, bool NORM>
 __device__ __forceinline__ void chain_body(const Params &p, int rank)
 {
     auto csync = [] {
@@ -717,6 +762,7 @@ __device__ __forceinline__ void chain_body(const Params &p, int rank)
     __shared__ int s_bad;
     const Ws &ws = p.ws;
     if (ws.hdr->fallback) return;
+    const double d = divisor<NORM>(p);
     const int T = ws.T;
     const int lane = threadIdx.x & 31;
     if (threadIdx.x == 0) s_bad = 0;
@@ -744,7 +790,7 @@ __device__ __forceinline__ void chain_body(const Params &p, int rank)
             if (ws.tile_slot[t_first] == SLOT_SEQ) {
                 // sequential tile: stage its weights, one thread adds them one by one
                 const i64 base = (i64)t_first * TILE;
-                for (int q = threadIdx.x; q < TILE; q += CHAIN_THREADS) s_w[q] = (base + q < p.n) ? p.w[base + q] : 0.0;
+                for (int q = threadIdx.x; q < TILE; q += CHAIN_THREADS) s_w[q] = (base + q < p.n) ? wdiv<NORM>(p.w[base + q], d) : 0.0;
                 if (threadIdx.x == 0) s_rm[0] = SM{ws.run_d[t_first], ws.run_t[t_first], 0, ws.run_k[t_first]};
                 __syncthreads();
                 if (threadIdx.x == 0) {
@@ -832,13 +878,13 @@ __device__ __forceinline__ void chain_body(const Params &p, int rank)
     }
 }
 
-template <bool STRAT>
-__global__ void __launch_bounds__(CHAIN_THREADS) k_chain(Params p) { chain_body<STRAT, 1>(p, 0); }
+template <bool STRAT, bool NORM>
+__global__ void __launch_bounds__(CHAIN_THREADS) k_chain(Params p) { chain_body<STRAT, 1, NORM>(p, 0); }
 
-template <bool STRAT>
+template <bool STRAT, bool NORM>
 __global__ void __cluster_dims__(CHAIN_CTAS, 1, 1) __launch_bounds__(CHAIN_THREADS) k_chain_cluster(Params p)
 {
-    chain_body<STRAT, CHAIN_CTAS>(p, (int)blockIdx.x);
+    chain_body<STRAT, CHAIN_CTAS, NORM>(p, (int)blockIdx.x);
 }
 
 // ------------------------------------------------------------------ multi-GPU: the shard's composite
@@ -1137,17 +1183,19 @@ __device__ __forceinline__ void emit_tile(const Params &p, EmitShared &sm, int t
 
 // Fast emit: the tiles pass C marked SLOT_FAST (clean, tie-free, one binade):
 // c_j = S_in + prefix sum of rne(w_j / ulp), one IEEE add per element.
-template <bool STRAT>
+template <bool STRAT, bool NORM>
 __global__ void __launch_bounds__(BLOCK, 2) k_emit_fast(Params p)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     EmitShared &sm = *reinterpret_cast<EmitShared *>(smem_raw);
     const Ws &ws = p.ws;
     if (ws.hdr->fallback) return;
+    const double d = divisor<NORM>(p);
     double2 g[IPT / 2];
     if ((int)blockIdx.x < ws.T) fetch_tile(p, blockIdx.x, g);
     for (int t = blockIdx.x; t < ws.T; t += gridDim.x) {
         double w[IPT];
+        normalise<NORM>(g, d);
         to_blocked(g, w, sm.buf);
         if (t + (int)gridDim.x < ws.T) fetch_tile(p, t + gridDim.x, g);      // next tile's loads fly during this tile
         if (ws.tile_slot[t] != SLOT_FAST) continue;                           // the general kernel owns this tile
@@ -1179,10 +1227,66 @@ __global__ void __launch_bounds__(BLOCK, 2) k_emit_fast(Params p)
 // conflict-free LDS.128) while the consumers work on the current one.  Expansion: every particle with
 // >= 1 copies stores (local index + 1) at its first output slot of a zeroed window, a max-scan over the
 // slots fills the runs (no divergent copy loop) and every thread leaves with 16-byte stores of 20
-// consecutive indexes.  (The same consumer code is the emit phase of the single-pass kernel behind
-// bke_resample_normalized, csrc/resample_fused.cu.)
+// consecutive indexes.
 constexpr int E2_NW = 8, E2_NT = E2_NW * 32, E2_SPT = 20, E2_WIN = E2_NT * E2_SPT;
 static_assert(E2_NT * IPT == TILE, "the second-generation emit uses the tile size of passes A-D");
+
+// byte offset of weight (row r = owning thread, 16-byte chunk c) inside a swizzled stage
+__device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)r * 128u + (uint32_t)((c ^ (r & 7)) << 4); }
+
+namespace {
+
+typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
+                             const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
+                             CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+EncodeFn get_encode()
+{
+    static EncodeFn fn = nullptr;
+    static bool tried = false;
+    if (!tried) {
+        tried = true;
+        void *ptr = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
+            qres == cudaDriverEntryPointSuccess)
+            fn = (EncodeFn)ptr;
+    }
+    return fn;
+}
+
+// the weights as rows of 16 doubles (128 bytes); a tile is a box of `box_rows` rows
+bool make_weights_map(CUtensorMap *m, const double *base, int64_t rows, int box_rows)
+{
+    EncodeFn enc = get_encode();
+    if (!enc || rows < 1) return false;
+    cuuint64_t gdim[2] = {16, (cuuint64_t)rows};
+    cuuint64_t gstride[1] = {128};
+    cuuint32_t box[2] = {16, (cuuint32_t)box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, const_cast<double *>(base), gdim, gstride, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// tensor map of the weights as rows of 16 doubles with a box of `box_rows` rows (cached per thread);
+// false when the driver entry point is missing or the pointer / size does not qualify for TMA
+bool weights_map(const double *w, int64_t n, int box_rows, CUtensorMap *out)
+{
+    static thread_local CUtensorMap map;
+    static thread_local const void *map_ptr = nullptr;
+    static thread_local int64_t map_n = -1;
+    static thread_local int map_rows = 0;
+    if ((reinterpret_cast<uintptr_t>(w) & 15) != 0 || (n >> 4) < 1 || get_encode() == nullptr) return false;
+    if (!(map_ptr == w && map_n == n && map_rows == box_rows)) {
+        if (!make_weights_map(&map, w, n >> 4, box_rows)) { map_ptr = nullptr; return false; }
+        map_ptr = w; map_n = n; map_rows = box_rows;
+    }
+    *out = map;
+    return true;
+}
+
+}  // namespace
 
 template <int E2_STAGES>
 struct Emit2Shared {
@@ -1198,7 +1302,7 @@ struct Emit2Shared {
 // issued as soon as the warps hold the current one in registers and lands long before it is needed),
 // 72 registers, three CTAs per SM.  <2, 2> is the default; BKE_RS_E2=1 selects <1, 3>, which on the H100
 // is slower for systematic but about 17 % faster for stratified resampling (DESIGN.md §3.6)
-template <bool STRAT, int E2_STAGES, int E2_CTAS>
+template <bool STRAT, int E2_STAGES, int E2_CTAS, bool NORM>
 __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_constant__ CUtensorMap wmap, Params p)
 {
     constexpr int NT = E2_NT, NW = E2_NW, WIN = E2_WIN, SPT = E2_SPT;
@@ -1207,8 +1311,8 @@ __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_cons
     const Ws &ws = p.ws;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     if (tid == 0) {
-        for (int s = 0; s < E2_STAGES; s++) { f_mbar_init(&sm.full[s], 1); f_mbar_init(&sm.empty[s], NW); }
-        f_fence_mbar_init();
+        for (int s = 0; s < E2_STAGES; s++) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], NW); }
+        fence_mbar_init();
     }
     for (int q = tid; q < WIN; q += NT + 32) sm.win[q] = 0;
     __syncthreads();
@@ -1220,14 +1324,15 @@ __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_cons
         for (int t = blockIdx.x; t < T; t += gridDim.x) {
             if (ws.tile_slot[t] != SLOT_FAST) continue;
             const int s = q % E2_STAGES, use = q / E2_STAGES;
-            if (use > 0) f_mbar_wait(&sm.empty[s], (use - 1) & 1);
-            if (lane == 0) { f_mbar_expect_tx(&sm.full[s], TILE * 8); f_tma_load_2d(sm.w[s], &wmap, 0, t * NT, &sm.full[s]); }
+            if (use > 0) while (!mbar_try(&sm.empty[s], (use - 1) & 1)) {}
+            if (lane == 0) { mbar_expect_tx(&sm.full[s], TILE * 8); tma_load_2d(sm.w[s], &wmap, 0, t * NT, &sm.full[s]); }
             q++;
         }
         return;
     }
     const i64 out_begin = ws.hdr->out_begin;
     const double Nd = (double)p.ng;
+    const double d = divisor<NORM>(p);
     int q = 0;
     for (int t = blockIdx.x; t < T; t += gridDim.x) {
         if (ws.tile_slot[t] != SLOT_FAST) continue;                           // the general kernel owns this tile
@@ -1235,7 +1340,7 @@ __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_cons
         q++;
         const i64 S_in = ws.S_in[t];
         const int tk = ws.tile_k[t];
-        f_mbar_wait(&sm.full[s], use & 1);
+        while (!mbar_try(&sm.full[s], use & 1)) {}
         const unsigned char *sb = reinterpret_cast<const unsigned char *>(sm.w[s]);
         const i64 base = (i64)(tk >= 0 ? tk : 0) << 52;
         const double B0 = __longlong_as_double(base);
@@ -1243,15 +1348,15 @@ __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_cons
         i64 acc = 0;
 #pragma unroll
         for (int c = 0; c < IPT / 2; c++) {
-            const double2 v = *reinterpret_cast<const double2 *>(sb + f_swz(tid, c));
-            acc += __double_as_longlong(__dadd_rn(B0, v.x)) - base; cb[2 * c] = acc;
-            acc += __double_as_longlong(__dadd_rn(B0, v.y)) - base; cb[2 * c + 1] = acc;
+            const double2 v = *reinterpret_cast<const double2 *>(sb + swz(tid, c));
+            acc += __double_as_longlong(__dadd_rn(B0, wdiv<NORM>(v.x, d))) - base; cb[2 * c] = acc;
+            acc += __double_as_longlong(__dadd_rn(B0, wdiv<NORM>(v.y, d))) - base; cb[2 * c + 1] = acc;
         }
         const i64 inc = warp_incl_scan_i64(acc, lane);
         if (lane == 31) sm.warp_tot[wid] = inc;
         __syncwarp();
-        if (lane == 0) f_mbar_arrive(&sm.empty[s]);                           // this warp holds its weights in registers
-        f_bar<NT>();
+        if (lane == 0) mbar_arrive(&sm.empty[s]);                           // this warp holds its weights in registers
+        bar_sync<NT>();
         i64 ex = inc - acc, D = 0;
 #pragma unroll
         for (int i = 0; i < NW; i++) { const i64 v = sm.warp_tot[i]; if (i < wid) ex += v; D += v; }
@@ -1316,7 +1421,7 @@ __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_cons
             int basem = __shfl_up_sync(FULL, incm, 1);
             if (lane == 0) basem = 0;
             if (lane == 31) sm.warp_max[wid] = incm;
-            f_bar<NT>();
+            bar_sync<NT>();
 #pragma unroll
             for (int i = 0; i < NW; i++) { const int x = sm.warp_max[i]; if (i < wid) basem = max(basem, x); }
 #pragma unroll
@@ -1335,7 +1440,7 @@ __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_cons
                 if (h > l) sm.win[l] = tid * IPT + i + 1;
                 l = h;
             }
-            f_bar<NT>();
+            bar_sync<NT>();
             int m[SPT];
             window_scan(m);
             const int s0 = tid * SPT;
@@ -1356,7 +1461,7 @@ __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_cons
         int cs = 0;
         while (cs < cnt) {
             if (tid == 0) sm.skip = -1;
-            f_bar<NT>();
+            bar_sync<NT>();
             {
                 int l = hv_prev;
 #pragma unroll
@@ -1371,9 +1476,9 @@ __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_cons
                     l = h;
                 }
             }
-            f_bar<NT>();
+            bar_sync<NT>();
             const int skip = sm.skip;
-            if (skip >= 0) { cs = skip; f_bar<NT>(); continue; }
+            if (skip >= 0) { cs = skip; bar_sync<NT>(); continue; }
             const int ce = (cnt - cs > WIN) ? cs + WIN : cnt;
             {
                 int l = hv_prev;
@@ -1385,7 +1490,7 @@ __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_cons
                     l = h;
                 }
             }
-            f_bar<NT>();
+            bar_sync<NT>();
             int m[SPT];
             window_scan(m);
 #pragma unroll
@@ -1393,27 +1498,29 @@ __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_cons
                 const int sl = tid * SPT + i;
                 if (sl < ce - cs) put_index(p, tile_lo + cs + sl, base_j + m[i]);
             }
-            f_bar<NT>();
+            bar_sync<NT>();
             cs = ce;
         }
-        f_bar<NT>();
+        bar_sync<NT>();
     }
 }
 
 // General emit over the slow list: ties, raw elements, sequential tiles.
-template <bool STRAT>
+template <bool STRAT, bool NORM>
 __global__ void __launch_bounds__(BLOCK, 2) k_emit_slow(Params p)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     EmitShared &sm = *reinterpret_cast<EmitShared *>(smem_raw);
     const Ws &ws = p.ws;
     if (ws.hdr->fallback) return;
+    const double d = divisor<NORM>(p);
     const int tid = threadIdx.x;
     const int n_slow = ws.hdr->n_slow;
     for (int li = blockIdx.x; li < n_slow; li += gridDim.x) {
         const int t = ws.slow_list[li];
         double2 g[IPT / 2];
         fetch_tile(p, t, g);
+        normalise<NORM>(g, d);
         TileAn an;
         to_blocked(g, an.w, sm.buf);
         const i64 S_in = ws.S_in[t];
@@ -1494,11 +1601,13 @@ __global__ void __launch_bounds__(256) k_fill_runs(Params p)
 }
 
 // ------------------------------------------------------------------ pass G: literal sequential fallback
-template <bool STRAT>
+template <bool STRAT, bool NORM>
 __global__ void k_sequential(Params p)
 {
     const Ws &ws = p.ws;
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    const double d = divisor<NORM>(p);
+    auto W = [&](i64 q) { return wdiv<NORM>(p.w[q], d); };
     auto write_info = [&](int overflow, int fb) {
         if (p.info) {
             p.info[0] = overflow; p.info[1] = fb; p.info[2] = ws.hdr->n_unclean; p.info[3] = ws.hdr->n_runs;
@@ -1508,7 +1617,7 @@ __global__ void k_sequential(Params p)
     if (!ws.hdr->fallback) { write_info(ws.hdr->overflow, 0); return; }
     if (p.cumsum_out) {                          // cumsum mode: np.cumsum, one add at a time
         double c = 0.0;
-        for (i64 q = 0; q < p.n; q++) { c = (q == 0) ? p.w[0] : __dadd_rn(c, p.w[q]); p.cumsum_out[q] = c; }
+        for (i64 q = 0; q < p.n; q++) { c = (q == 0) ? W(0) : __dadd_rn(c, W(q)); p.cumsum_out[q] = c; }
         if (p.cumsum_last) *p.cumsum_last = c;
         if (p.last_one) p.cumsum_out[p.n - 1] = 1.0;
         write_info(0, 1);
@@ -1529,7 +1638,7 @@ __global__ void k_sequential(Params p)
     ws.hdr->out_begin = ob;
     ws.hdr->cap_overflow = 0;
     i64 i = ob, j = 0;
-    double c = (carry == 0.0) ? p.w[0] : __dadd_rn(carry, p.w[0]);
+    double c = (carry == 0.0) ? W(0) : __dadd_rn(carry, W(0));
     int overflow = 0;
     while (i < p.ng) {
         const double pos = STRAT ? pos_str(i, p.U, Ngd) : pos_sys(i, p.u, Ngd);
@@ -1545,10 +1654,10 @@ __global__ void k_sequential(Params p)
                 }
                 break;
             }
-            c = __dadd_rn(c, p.w[j]);
+            c = __dadd_rn(c, W(j));
         }
     }
-    for (i64 q = j + 1; q < p.n; q++) c = __dadd_rn(c, p.w[q]);
+    for (i64 q = j + 1; q < p.n; q++) c = __dadd_rn(c, W(q));
     if (p.cumsum_last) *p.cumsum_last = c;
     ws.hdr->out_end = i;
     if (p.out_range) { p.out_range[0] = ob; p.out_range[1] = i; }
@@ -1666,7 +1775,81 @@ struct RunArgs {
     int is_last;
     double *cumsum_out; int last_one;
     int phase;           // bit 0: passes A-C (need carry_approx), bit 1: pass D chain (needs carry_exact), bit 2: passes E-G
+    const double *div;   // non-NULL: resample w / *div (the NORM instances)
+    double *wnorm_out;   // with div, optional: receives w / *div
 };
+
+// The passes a.phase selects.  NORM (a normalised call) always runs passes A, B and C as separate launches
+// and the default second-generation emit: BKE_RS_FRONT and BKE_RS_E2 have no NORM instances.
+template <bool NORM>
+int launch(const RunArgs &a, const Params &p, cudaStream_t s)
+{
+    const i64 n = a.n;
+    const int T = p.ws.T;
+    const int emit_smem = (int)sizeof(EmitShared);
+    const int sms = sm_count();
+    const int slow_grid = T < sms * 2 ? T : sms * 2;
+    if (a.phase & 1) {
+        // BKE_RS_FRONT=1: tile sums, their scan (decoupled look-back) and the fast maps in ONE pass over the
+        // weights.  Slower than the three launches it replaces on an earlier target (with hundreds of tiles in
+        // flight the nearest inclusive prefix is far back and the polling competes with the streaming loads);
+        // about 6 % faster on the H100 (DESIGN.md §3.6), not yet the default.
+        static const bool fused_front = [] { const char *e = getenv("BKE_RS_FRONT"); return e && e[0] == '1'; }();
+        if (!NORM && !(a.phase & 8) && fused_front) {
+            const size_t clr = (size_t)((unsigned char *)(p.ws.st1 + T) - (unsigned char *)p.ws.hdr);
+            if (check_cuda(cudaMemsetAsync(p.ws.hdr, 0, clr, s), "memset header + status words")) return BKE_ERR_CUDA;
+            k_front<<<T, BLOCK + 32, 0, s>>>(p);
+        } else {
+            if (!(a.phase & 8)) {                   // bit 8: the header reset and pass A have run already (bke_resample_shard_stage)
+                if (check_cuda(cudaMemsetAsync(p.ws.hdr, 0, sizeof(Header), s), "memset header")) return BKE_ERR_CUDA;
+                k_tile_sums<NORM><<<T, BLOCK, 0, s>>>(p);
+            }
+            k_scan_tiles<<<1, CHAIN_THREADS, 0, s>>>(p);
+            k_tile_maps_fast1<NORM><<<T, BLOCK, 0, s>>>(p);
+        }
+        k_tile_maps<NORM><<<slow_grid, BLOCK, 0, s>>>(p);
+    }
+    if (a.phase & 2) {
+        // a cluster of CHAIN_CTAS CTAs once there are enough tiles to share out
+        if (T >= 2048) {
+            if (a.U) k_chain_cluster<true, NORM><<<CHAIN_CTAS, CHAIN_THREADS, 0, s>>>(p);
+            else k_chain_cluster<false, NORM><<<CHAIN_CTAS, CHAIN_THREADS, 0, s>>>(p);
+        } else if (a.U) k_chain<true, NORM><<<1, CHAIN_THREADS, 0, s>>>(p);
+        else k_chain<false, NORM><<<1, CHAIN_THREADS, 0, s>>>(p);
+    }
+    if (a.phase & 4) {
+        const int fast_grid = T < sms * 2 ? T : sms * 2;
+        // second-generation emit (TMA-staged, marker / max-scan expansion) whenever the weights qualify for
+        // TMA and indexes are produced; otherwise the first-generation kernel
+        CUtensorMap wmap;
+        const bool emit2 = !a.cumsum_out && (n % 16) == 0 && weights_map(a.w, n, E2_NT, &wmap);
+        if (emit2) {
+            static const int e2_variant = [] { const char *e = getenv("BKE_RS_E2"); return e ? atoi(e) : 0; }();
+            auto launch2 = [&](auto kern, int smem2, int ctas) -> int {
+                if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
+                const int g = T < sms * ctas ? T : sms * ctas;
+                kern<<<g, E2_NT + 32, smem2, s>>>(wmap, p);
+                return BKE_OK;
+            };
+            int rc2;
+            if (!NORM && e2_variant == 1) rc2 = a.U ? launch2(k_emit2<true, 1, 3, false>, (int)sizeof(Emit2Shared<1>), 3) : launch2(k_emit2<false, 1, 3, false>, (int)sizeof(Emit2Shared<1>), 3);
+            else rc2 = a.U ? launch2(k_emit2<true, 2, 2, NORM>, (int)sizeof(Emit2Shared<2>), 2) : launch2(k_emit2<false, 2, 2, NORM>, (int)sizeof(Emit2Shared<2>), 2);
+            if (rc2 != BKE_OK) return rc2;
+            if (a.U) k_emit_slow<true, NORM><<<slow_grid, BLOCK, emit_smem, s>>>(p);
+            else k_emit_slow<false, NORM><<<slow_grid, BLOCK, emit_smem, s>>>(p);
+        } else if (a.U) {
+            k_emit_fast<true, NORM><<<fast_grid, BLOCK, emit_smem, s>>>(p);
+            k_emit_slow<true, NORM><<<slow_grid, BLOCK, emit_smem, s>>>(p);
+        } else {
+            k_emit_fast<false, NORM><<<fast_grid, BLOCK, emit_smem, s>>>(p);
+            k_emit_slow<false, NORM><<<slow_grid, BLOCK, emit_smem, s>>>(p);
+        }
+        k_fill_runs<<<sms * 4, 256, 0, s>>>(p);
+        if (a.U) k_sequential<true, NORM><<<1, 32, 0, s>>>(p);
+        else k_sequential<false, NORM><<<1, 32, 0, s>>>(p);
+    }
+    return check_cuda(cudaGetLastError(), "resample launch");
+}
 
 int run(const RunArgs &a, cudaStream_t s)
 {
@@ -1686,86 +1869,25 @@ int run(const RunArgs &a, cudaStream_t s)
     p.u = a.u; p.U = a.U; p.idx = a.idx; p.info = a.info; p.cumsum_last = a.cumsum_last;
     p.cumsum_out = a.cumsum_out; p.last_one = a.last_one;
     p.scan_done = (a.phase & 16) ? 1 : 0;
+    p.div = a.div; p.wnorm_out = a.wnorm_out;
     // |exact sequential sum - approximate tree sum| <= (N + 4096) * 2^-53 relative (non-negative
     // terms), i.e. less than (N + 4096) ulps of the running sum; doubled, plus slack.
     p.eb = 2 * (a.ng + 4096) + (a.ng >> 4);
     const double tau = ldexp((double)a.ng, -46);
     p.tau = tau > 1e-6 ? tau : 1e-6;
     p.aligned16 = (reinterpret_cast<uintptr_t>(a.w) & 15) == 0;
-    const int T = p.ws.T;
-    const int emit_smem = (int)sizeof(EmitShared);
     static bool configured[64] = {false};
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64 || !configured[dev]) {
-        if (check_cuda(cudaFuncSetAttribute(k_emit_fast<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, emit_smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
-        if (check_cuda(cudaFuncSetAttribute(k_emit_fast<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, emit_smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
-        if (check_cuda(cudaFuncSetAttribute(k_emit_slow<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, emit_smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
-        if (check_cuda(cudaFuncSetAttribute(k_emit_slow<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, emit_smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
+        for (const void *k : {(const void *)k_emit_fast<false, false>, (const void *)k_emit_fast<true, false>,
+                              (const void *)k_emit_slow<false, false>, (const void *)k_emit_slow<true, false>,
+                              (const void *)k_emit_fast<false, true>, (const void *)k_emit_fast<true, true>,
+                              (const void *)k_emit_slow<false, true>, (const void *)k_emit_slow<true, true>})
+            if (check_cuda(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EmitShared)), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
         if (dev >= 0 && dev < 64) configured[dev] = true;
     }
-    const int sms = sm_count();
-    const int slow_grid = T < sms * 2 ? T : sms * 2;
-    if (a.phase & 1) {
-        // BKE_RS_FRONT=1: tile sums, their scan (decoupled look-back) and the fast maps in ONE pass over the
-        // weights.  Slower than the three launches it replaces on an earlier target (with hundreds of tiles in
-        // flight the nearest inclusive prefix is far back and the polling competes with the streaming loads);
-        // about 6 % faster on the H100 (DESIGN.md §3.6), not yet the default.
-        static const bool fused_front = [] { const char *e = getenv("BKE_RS_FRONT"); return e && e[0] == '1'; }();
-        if (!(a.phase & 8) && fused_front) {
-            const size_t clr = (size_t)((unsigned char *)(p.ws.st1 + T) - (unsigned char *)p.ws.hdr);
-            if (check_cuda(cudaMemsetAsync(p.ws.hdr, 0, clr, s), "memset header + status words")) return BKE_ERR_CUDA;
-            k_front<<<T, BLOCK + 32, 0, s>>>(p);
-        } else {
-            if (!(a.phase & 8)) {                   // bit 8: the header reset and pass A have run already (bke_resample_shard_stage)
-                if (check_cuda(cudaMemsetAsync(p.ws.hdr, 0, sizeof(Header), s), "memset header")) return BKE_ERR_CUDA;
-                k_tile_sums<<<T, BLOCK, 0, s>>>(p);
-            }
-            k_scan_tiles<<<1, CHAIN_THREADS, 0, s>>>(p);
-            k_tile_maps_fast1<<<T, BLOCK, 0, s>>>(p);
-        }
-        k_tile_maps<<<slow_grid, BLOCK, 0, s>>>(p);
-    }
-    if (a.phase & 2) {
-        // a cluster of CHAIN_CTAS CTAs once there are enough tiles to share out
-        if (T >= 2048) {
-            if (a.U) k_chain_cluster<true><<<CHAIN_CTAS, CHAIN_THREADS, 0, s>>>(p);
-            else k_chain_cluster<false><<<CHAIN_CTAS, CHAIN_THREADS, 0, s>>>(p);
-        } else if (a.U) k_chain<true><<<1, CHAIN_THREADS, 0, s>>>(p);
-        else k_chain<false><<<1, CHAIN_THREADS, 0, s>>>(p);
-    }
-    if (a.phase & 4) {
-        const int fast_grid = T < sms * 2 ? T : sms * 2;
-        // second-generation emit (TMA-staged, marker / max-scan expansion) whenever the weights qualify for
-        // TMA and indexes are produced; otherwise the first-generation kernel
-        CUtensorMap wmap;
-        const bool emit2 = !a.cumsum_out && (n % 16) == 0 && f_weights_map(a.w, n, E2_NT, &wmap);
-        if (emit2) {
-            static const int e2_variant = [] { const char *e = getenv("BKE_RS_E2"); return e ? atoi(e) : 0; }();
-            auto launch2 = [&](auto kern, int smem2, int ctas) -> int {
-                if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
-                const int g = T < sms * ctas ? T : sms * ctas;
-                kern<<<g, E2_NT + 32, smem2, s>>>(wmap, p);
-                return BKE_OK;
-            };
-            int rc2;
-            if (e2_variant == 1) rc2 = a.U ? launch2(k_emit2<true, 1, 3>, (int)sizeof(Emit2Shared<1>), 3) : launch2(k_emit2<false, 1, 3>, (int)sizeof(Emit2Shared<1>), 3);
-            else rc2 = a.U ? launch2(k_emit2<true, 2, 2>, (int)sizeof(Emit2Shared<2>), 2) : launch2(k_emit2<false, 2, 2>, (int)sizeof(Emit2Shared<2>), 2);
-            if (rc2 != BKE_OK) return rc2;
-            if (a.U) k_emit_slow<true><<<slow_grid, BLOCK, emit_smem, s>>>(p);
-            else k_emit_slow<false><<<slow_grid, BLOCK, emit_smem, s>>>(p);
-        } else if (a.U) {
-            k_emit_fast<true><<<fast_grid, BLOCK, emit_smem, s>>>(p);
-            k_emit_slow<true><<<slow_grid, BLOCK, emit_smem, s>>>(p);
-        } else {
-            k_emit_fast<false><<<fast_grid, BLOCK, emit_smem, s>>>(p);
-            k_emit_slow<false><<<slow_grid, BLOCK, emit_smem, s>>>(p);
-        }
-        k_fill_runs<<<sms * 4, 256, 0, s>>>(p);
-        if (a.U) k_sequential<true><<<1, 32, 0, s>>>(p);
-        else k_sequential<false><<<1, 32, 0, s>>>(p);
-    }
-    return check_cuda(cudaGetLastError(), "resample launch");
+    return a.div ? launch<true>(a, p, s) : launch<false>(a, p, s);
 }
 
 }  // namespace rs
@@ -1778,8 +1900,7 @@ extern "C" {
 size_t bke_resample_workspace_bytes(int64_t n)
 {
     if (n <= 0) return 256;
-    const size_t a = rs::carve(n, nullptr, nullptr), b = rs::f_carve(n, nullptr, nullptr);
-    return a > b ? a : b;
+    return rs::carve(n, nullptr, nullptr);
 }
 
 static rs::RunArgs whole_array(int64_t n, const double *weights, double u, const double *U, int32_t *indexes,
@@ -1789,7 +1910,7 @@ static rs::RunArgs whole_array(int64_t n, const double *weights, double u, const
     a.n = n; a.ng = n; a.j0 = 0; a.cap = n; a.w = weights; a.U = U; a.u = u; a.idx = indexes;
     a.workspace = workspace; a.ws_bytes = workspace_bytes; a.info = info; a.cumsum_last = cumsum_last;
     a.carry_approx = nullptr; a.carry_exact = nullptr; a.out_range = nullptr; a.is_last = 1; a.phase = 7;
-    a.cumsum_out = nullptr; a.last_one = 0;
+    a.cumsum_out = nullptr; a.last_one = 0; a.div = nullptr; a.wnorm_out = nullptr;
     return a;
 }
 
@@ -1812,15 +1933,13 @@ int bke_resample_normalized(int64_t n, const double *weights, double u, const do
 {
     if (n < 0 || !sum_out) { set_error("bad arguments"); return BKE_ERR_BAD_ARG; }
     if (n == 0) return BKE_OK;
-    // the sum S first (the only quantity a multi-GPU caller all-reduces), then ONE pass that divides,
-    // scans and emits: the oracle is systematic_resample(w / S) with this S
+    // the sum S first (the only quantity a multi-GPU caller all-reduces), then the passes on w / S, each
+    // dividing the weights it reads: the oracle is systematic_resample(w / S) with this S
     int rc = bke_weights_sum(n, weights, sum_out, workspace, workspace_bytes, stream);
     if (rc != BKE_OK) return rc;
-    rs::FRunArgs f;
-    f.n = n; f.w = weights; f.U = uniforms; f.u = u; f.idx = indexes;
-    f.workspace = workspace; f.ws_bytes = workspace_bytes; f.info = info; f.cumsum_last = cumsum_last;
-    f.div = sum_out; f.wnorm_out = weights_out;
-    return rs::f_run(f, (cudaStream_t)stream);
+    rs::RunArgs a = whole_array(n, weights, u, uniforms, indexes, workspace, workspace_bytes, info, cumsum_last);
+    a.div = sum_out; a.wnorm_out = weights_out;
+    return rs::run(a, (cudaStream_t)stream);
 }
 
 namespace bke { namespace rs {
@@ -1851,7 +1970,7 @@ int bke_resample_shard_stage(const bke_resample_shard_args *args, const bke_resa
         p.w = a.weights; p.n = a.n_local;
         p.aligned16 = (reinterpret_cast<uintptr_t>(a.weights) & 15) == 0;
         if (check_cuda(cudaMemsetAsync(p.ws.hdr, 0, sizeof(rs::Header), s), "memset header")) return BKE_ERR_CUDA;
-        rs::k_tile_sums<<<p.ws.T, rs::BLOCK, 0, s>>>(p);
+        rs::k_tile_sums<false><<<p.ws.T, rs::BLOCK, 0, s>>>(p);
         rs::k_sum_tiles<<<1, rs::CHAIN_THREADS, 0, s>>>(p.ws.tile_sum, p.ws.T, ext->shard_sum_out);
         return check_cuda(cudaGetLastError(), "shard stage 1 launch");
     }
@@ -1913,6 +2032,7 @@ int bke_resample_shard(const bke_resample_shard_args *args, void *stream)
     a.workspace = args->workspace; a.ws_bytes = args->workspace_bytes; a.info = args->info; a.cumsum_last = args->carry_out;
     a.carry_approx = args->carry_approx; a.carry_exact = args->carry_exact; a.out_range = reinterpret_cast<rs::i64 *>(args->out_range);
     a.is_last = args->is_last; a.phase = args->phase; a.cumsum_out = nullptr; a.last_one = 0;
+    a.div = nullptr; a.wnorm_out = nullptr;
     if (a.j0 + a.n > a.ng) { set_error("shard exceeds the global particle count"); return BKE_ERR_BAD_ARG; }
     return rs::run(a, (cudaStream_t)stream);
 }
@@ -1931,7 +2051,7 @@ int bke_weights_sum(int64_t n, const double *weights, double *sum_out, void *wor
     p.w = weights; p.n = n;
     p.aligned16 = (reinterpret_cast<uintptr_t>(weights) & 15) == 0;
     if (check_cuda(cudaMemsetAsync(p.ws.hdr, 0, sizeof(rs::Header), s), "memset header")) return BKE_ERR_CUDA;
-    rs::k_tile_sums<<<p.ws.T, rs::BLOCK, 0, s>>>(p);
+    rs::k_tile_sums<false><<<p.ws.T, rs::BLOCK, 0, s>>>(p);
     rs::k_sum_tiles<<<1, rs::CHAIN_THREADS, 0, s>>>(p.ws.tile_sum, p.ws.T, sum_out);
     return check_cuda(cudaGetLastError(), "weights_sum launch");
 }

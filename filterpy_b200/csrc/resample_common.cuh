@@ -1,5 +1,5 @@
-// resample_common.cuh — device primitives shared by the resampling kernels (csrc/resample.cu,
-// csrc/resample_fused.cu): parity maps of the exact sequential fp64 cumulative sum
+// resample_common.cuh — device primitives of the resampling kernels (csrc/resample.cu): parity maps
+// of the exact sequential fp64 cumulative sum
 // (filterpy/monte_carlo/resampling.py:142), warp scans, the position count of :139 / :103.
 #pragma once
 #include "bke_internal.cuh"

@@ -261,13 +261,12 @@ int bke_stratified_resample(int64_t n, const double *weights, const double *unif
                             int32_t *indexes, void *workspace, size_t workspace_bytes,
                             int32_t *info, double *cumsum_last, void *stream);
 
-/* Fused normalise + resample (north_star: "single fused weight-normalise + inclusive-scan +
- * inverse-CDF kernel"): S = sum(weights) (tree order, written to sum_out), then ONE pass over the
- * weights that forms w / S (IEEE division, what NumPy's `w / w.sum()` computes given S), its exact
- * sequential cumulative sum and the indexes — i.e. systematic_resample(weights / S)
- * (resampling.py:117-150; stratified when `uniforms` != NULL, :80-114).  weights_out (optional)
- * receives the normalised weights.  The un-normalised weights are read twice (sum, resample);
- * nothing else is written. */
+/* Fused normalise + resample: S = sum(weights) (tree order, written to sum_out), then the resampling
+ * passes on w / S — systematic_resample(weights / S) (resampling.py:117-150; stratified when
+ * `uniforms` != NULL, :80-114).  Every pass that reads the weights divides them by S as it reads them
+ * (IEEE division, what NumPy's `w / w.sum()` computes given S): the sum and passes A, C and E read the
+ * un-normalised weights.  No normalised array is written unless weights_out (optional) is given; it
+ * then receives w / S.  info and cumsum_last as for bke_systematic_resample, on w / S. */
 int bke_resample_normalized(int64_t n, const double *weights, double u, const double *uniforms,
                             int32_t *indexes, double *weights_out, double *sum_out,
                             void *workspace, size_t workspace_bytes,

@@ -1,6 +1,6 @@
-"""ResamplePlan.normalized (bke_resample_normalized, the single-pass kernel of csrc/resample_fused.cu):
-the indexes of systematic_resample(w / S) (stratified_resample with uniforms), S the engine's sum of
-the weights, bit for bit; and weights_out == w / S."""
+"""ResamplePlan.normalized (bke_resample_normalized: the multi-pass pipeline of csrc/resample.cu with every
+weight divided by S where it is read): the indexes of systematic_resample(w / S) (stratified_resample with
+uniforms), S the engine's sum of the weights, bit for bit; and weights_out == w / S."""
 import numpy as np
 import pytest
 
@@ -24,7 +24,7 @@ def _expected(wn, positions):
         return np.minimum(idx, len(wn) - 1).astype("i"), over
 
 
-def _run(w, u=None, U=None, offset=0):
+def _run(w, u=None, U=None, offset=0, with_wout=True):
     """One normalized call on a copy of w that starts `offset` doubles into its device buffer."""
     import torch
     from filterpy_b200.monte_carlo import ResamplePlan
@@ -36,22 +36,27 @@ def _run(w, u=None, U=None, offset=0):
     plan.indexes.fill_(-7)
     wout = torch.full((n,), -1.0, dtype=torch.float64, device="cuda")
     Ud = torch.from_numpy(U).cuda() if U is not None else None
-    idx, S = plan.normalized(wd, u=u, uniforms=Ud, weights_out=wout)
+    idx, S = plan.normalized(wd, u=u, uniforms=Ud, weights_out=wout if with_wout else None)
     return idx.cpu().numpy(), float(S.item()), wout.cpu().numpy(), plan.info(), float(plan.cumsum_last.item())
 
 
-def _check(w, u=None, U=None, offset=0):
+def _check(w, u=None, U=None, offset=0, with_wout=True):
+    """Checks one call and returns its info."""
     from oracle import resample as ors
     n = len(w)
-    idx, S, wout, info, clast = _run(w, u=u, U=U, offset=offset)
+    idx, S, wout, info, clast = _run(w, u=u, U=U, offset=offset, with_wout=with_wout)
     wn = w / S
-    assert np.array_equal(wout, wn), "weights_out != w / S"
+    if with_wout:
+        assert np.array_equal(wout, wn), "weights_out != w / S"
+    else:
+        assert (wout == -1.0).all(), "a buffer that was not passed was written"
     pos = ors.positions_stratified(n, U) if U is not None else ors.positions_systematic(n, u)
     want, over = _expected(wn, pos)
     bad = np.flatnonzero(idx != want)[:4]
     assert len(bad) == 0, ("indexes differ at", bad.tolist(), info.tolist())
     assert info[0] == over and info[1] == 0, info.tolist()
     assert clast == np.cumsum(wn)[-1]
+    return info
 
 
 @pytest.mark.parametrize("kind", KINDS)
@@ -105,3 +110,29 @@ def test_negative_weight_takes_the_literal_fallback():
     assert info[1] == 1, info.tolist()
     assert np.array_equal(wout, wn)
     assert np.array_equal(idx, ors.resample_loop(wn, ors.positions_systematic(3000, 0.4)))
+
+
+TILE = 4096      # particles per tile of the pipeline (resample_common.cuh)
+
+
+@pytest.mark.parametrize("stratified", [False, True])
+def test_cluster_chain(stratified):
+    """at least 2048 tiles: the exact chain over the tiles runs as a thread-block cluster"""
+    from filterpy_b200.common import workloads as wl
+    n = (1 << 23) + 1
+    assert -(-n // TILE) >= 2048
+    U = np.random.default_rng(5).random(n) if stratified else None
+    _check(wl.resample_weights(n, "heavy", seed=11), u=None if stratified else U_SYS, U=U)
+
+
+def test_sequential_tile():
+    """A tile in which every add starts exactly on a binade boundary (w / S = 0.5 before it, each of its
+    weights far below half an ulp there) is walked element by element (info[5] counts such tiles)."""
+    w = np.concatenate([np.full(TILE, 2.0 ** -12), np.full(TILE, 2.0 ** -80), np.full(TILE, 2.0 ** -12)])
+    info = _check(w, u=0.3)
+    assert info[5] > 0, info.tolist()
+
+
+def test_without_weights_out():
+    from filterpy_b200.common import workloads as wl
+    _check(wl.resample_weights(300007, "heavy", seed=5), u=U_SYS, with_wout=False)
