@@ -6,7 +6,7 @@ point reports no CUDA device, an exception is raised.
 """
 import ctypes
 import os
-from ctypes import c_double, c_int32, c_int64, c_size_t, c_uint32, c_void_p
+from ctypes import c_double, c_int32, c_int64, c_size_t, c_uint32, c_uint64, c_void_p
 
 from . import _build
 
@@ -23,6 +23,7 @@ EXPORTED_SYMBOLS = [
     "bke_abi_version", "bke_last_error", "bke_device_count",
     "bke_kf_step", "bke_kf_batch_filter", "bke_ukf_step",
     "bke_kf_sym_models_bytes", "bke_kf_pack_sym_models", "bke_kf_step_sym",
+    "bke_kf_scan_models", "bke_kf_packed_models_bytes", "bke_kf_pack_models", "bke_kf_step_packed",
     "bke_resample_workspace_bytes", "bke_systematic_resample", "bke_stratified_resample",
     "bke_weights_sum", "bke_weights_scale", "bke_resample_shard", "bke_resample_normalized",
     "bke_resample_composite_bytes", "bke_resample_shard_compose", "bke_resample_compose_carry", "bke_resample_shard_stage",
@@ -55,6 +56,17 @@ class KfArgs(ctypes.Structure):
         ("log_likelihood", c_void_p),
         ("status", c_void_p),
         ("F_host", c_void_p), ("Q_host", c_void_p), ("H_host", c_void_p), ("R_host", c_void_p),
+    ]
+
+
+BKE_KF42_MODEL_WORDS = 37
+
+
+class KfModelMap(ctypes.Structure):
+    _fields_ = [
+        ("varying", c_uint64),
+        ("asymmetric", c_int32), ("reserved", c_int32),
+        ("words", ctypes.c_float * BKE_KF42_MODEL_WORDS),
     ]
 
 
@@ -218,6 +230,16 @@ def load():
     lib.bke_kf_pack_sym_models.restype = ctypes.c_int
     lib.bke_kf_step_sym.argtypes = [ctypes.POINTER(KfArgs), c_void_p, c_void_p]
     lib.bke_kf_step_sym.restype = ctypes.c_int
+    lib.bke_kf_scan_models.argtypes = [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_void_p]
+    lib.bke_kf_scan_models.restype = ctypes.c_int
+    lib.bke_kf_packed_models_bytes.argtypes = [c_int64, c_uint64]
+    lib.bke_kf_packed_models_bytes.restype = c_size_t
+    lib.bke_kf_pack_models.argtypes = [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_uint64, c_void_p, c_void_p]
+    lib.bke_kf_pack_models.restype = ctypes.c_int
+    lib.bke_kf_step_packed.argtypes = [ctypes.POINTER(KfArgs), c_void_p, ctypes.POINTER(KfModelMap), c_void_p]
+    lib.bke_kf_step_packed.restype = ctypes.c_int
     lib.bke_kf_batch_filter.argtypes = [ctypes.POINTER(KfBatchArgs), c_void_p]
     lib.bke_kf_batch_filter.restype = ctypes.c_int
     lib.bke_ukf_step.argtypes = [ctypes.POINTER(UkfArgs), c_void_p]

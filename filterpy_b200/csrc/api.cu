@@ -147,6 +147,60 @@ int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream)
     return rc;
 }
 
+static int validate_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *F, const void *Q,
+                           const void *H, const void *R)
+{
+    if (n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    if (n_filters > 0 && (!F || !Q || !H || !R)) { set_error("F, Q, H and R must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if (!(dim_x == 4 && dim_z == 2 && dtype == BKE_F32)) {
+        set_error("packed models exist for dim_x = 4, dim_z = 2, BKE_F32 only");
+        return BKE_ERR_UNSUPPORTED;
+    }
+    return BKE_OK;
+}
+
+static bool bad_mask(uint64_t varying) { return (varying >> BKE_KF42_MODEL_WORDS) != 0; }
+
+int bke_kf_scan_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *F, const void *Q,
+                       const void *H, const void *R, bke_kf_model_map *map, void *stream)
+{
+    int rc = validate_models(n_filters, dim_x, dim_z, dtype, F, Q, H, R);
+    if (rc) return rc;
+    if (!map) { set_error("map must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if ((rc = require_device())) return rc;
+    return launch_kf_scan_models(n_filters, F, Q, H, R, map, (cudaStream_t)stream);
+}
+
+size_t bke_kf_packed_models_bytes(int64_t n_filters, uint64_t varying) { return kf_packed_models_bytes(n_filters, varying); }
+
+int bke_kf_pack_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *F, const void *Q,
+                       const void *H, const void *R, uint64_t varying, void *record, void *stream)
+{
+    int rc = validate_models(n_filters, dim_x, dim_z, dtype, F, Q, H, R);
+    if (rc) return rc;
+    if (bad_mask(varying)) { set_error("varying has bits above word %d", BKE_KF42_MODEL_WORDS - 1); return BKE_ERR_BAD_ARG; }
+    if (n_filters > 0 && varying && !record) { set_error("record must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if ((rc = require_device())) return rc;
+    return launch_kf_pack_models(n_filters, F, Q, H, R, varying, record, (cudaStream_t)stream);
+}
+
+int bke_kf_step_packed(const bke_kf_args *args, const void *record, const bke_kf_model_map *host_map, void *stream)
+{
+    int rc = validate_kf(args, true);
+    if (rc) return rc;
+    if (!host_map) { set_error("host_map is NULL"); return BKE_ERR_BAD_ARG; }
+    if (bad_mask(host_map->varying)) { set_error("varying has bits above word %d", BKE_KF42_MODEL_WORDS - 1); return BKE_ERR_BAD_ARG; }
+    if (host_map->varying && !record) { set_error("record is NULL"); return BKE_ERR_BAD_ARG; }
+    if ((rc = require_device())) return rc;
+    if (args->n_filters == 0) return BKE_OK;
+    g_err[0] = '\0';
+    rc = launch_kf_fast(*args, (cudaStream_t)stream, record, host_map);
+    if (rc == BKE_ERR_UNSUPPORTED && g_err[0] == '\0')      // (launch_kf_fast names some causes itself)
+        set_error("the packed models cover per-filter models of dim_x = 4, dim_z = 2, BKE_F32 banks without "
+                  "control input, on 16-byte aligned arrays");
+    return rc;
+}
+
 int bke_kf_batch_filter(const bke_kf_batch_args *args, void *stream)
 {
     if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }

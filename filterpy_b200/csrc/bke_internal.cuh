@@ -29,11 +29,17 @@ constexpr double LOG_2PI = 1.8378770664093454835606594728112;
 #ifndef __CUDACC_RTC__
 // ---- launchers implemented in the .cu files ---------------------------------------------
 int launch_kf_generic(const bke_kf_args &a, cudaStream_t s);
-// returns BKE_ERR_UNSUPPORTED when the specialised kernel does not cover the call; `sym` (optional) is a
-// record filled by launch_kf_pack_sym that replaces the per-filter Q and R
-int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *sym = nullptr);
+// returns BKE_ERR_UNSUPPORTED when the specialised kernel does not cover the call.  Optional: `rec` alone is a
+// record filled by launch_kf_pack_sym that replaces the per-filter Q and R; `rec` with the HOST copy of a map
+// filled by launch_kf_scan_models is a record filled by launch_kf_pack_models that replaces F, Q, H and R
+int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec = nullptr, const bke_kf_model_map *map = nullptr);
 size_t kf_sym_models_bytes(int64_t n_filters);
 int launch_kf_pack_sym(int64_t n_filters, const void *Q, const void *R, void *record, int32_t *asym, cudaStream_t s);
+size_t kf_packed_models_bytes(int64_t n_filters, uint64_t varying);
+int launch_kf_scan_models(int64_t n_filters, const void *F, const void *Q, const void *H, const void *R,
+                          bke_kf_model_map *map, cudaStream_t s);
+int launch_kf_pack_models(int64_t n_filters, const void *F, const void *Q, const void *H, const void *R, uint64_t varying,
+                          void *record, cudaStream_t s);
 int launch_kf_rowblock(const bke_kf_args &a, cudaStream_t s);
 int launch_kf_direct(const bke_kf_args &a, cudaStream_t s);
 // wgmma covariance propagation for shared-model fp32 banks with dim_x = 16 / 32 (kf_tc.cu); a fused step runs

@@ -16,8 +16,12 @@
 //     the next launch once it has issued the loads of its last tile.
 // Shared models (stride 0) are read once per thread through the read-only path instead of TMA.
 // A bank whose per-filter Q and R are exactly symmetric may instead hand over a packed copy of their
-// upper triangles (bke_kf_pack_sym_models, SYM = true): one bulk copy per tile replaces the two of
+// upper triangles (bke_kf_pack_sym_models, REC == 1): one bulk copy per tile replaces the two of
 // Q and R, 52 instead of 80 B per filter, and the lower triangles are rebuilt in registers.
+// Such a bank may go further and hand over only the model words that differ between its filters
+// (bke_kf_scan_models + bke_kf_pack_models, REC == 2): one bulk copy per tile brings those planes,
+// and every word the whole bank shares rides in the launch parameters (40 instead of 148 B of
+// models per filter for the kf_bank_cv2d template).
 //
 // Reference arithmetic: filterpy/kalman/kalman_filter.py:471-478, 533-556 (see kf_regtile.cuh).
 #include <stdlib.h>
@@ -48,7 +52,16 @@ constexpr int TILE = 128;       // filters per tile == threads per CTA
 // 6656 B, and the record of the whole bank is padded to whole tiles, so every copy has the same size.
 constexpr int SYM_Q_PLANES = 10, SYM_PLANES = 13;
 
-template <typename T, int N, int M, bool SHARED = false, bool SYM = false>
+// The packed model words of a 4/2 bank (REC == 2): the 37 words of a filter's models, in this order
+// (bit e of a map's `varying` stands for word e):
+//   F 0..15 (row-major) | Q 16..25 (upper triangle, as above) | H 26..33 (row-major) | R 34..36 (R00 R01 R11).
+// The record holds only the words that differ between filters, tile-major like the one above with
+// k = popcount(varying) planes per tile, so predict reads a prefix of a tile (F, Q) and update a suffix (H, R).
+constexpr int WORDS = BKE_KF42_MODEL_WORDS, W_F = 0, W_Q = 16, W_H = 26, W_R = 34;
+constexpr uint64_t PREDICT_WORDS = (1ull << W_H) - 1;      // F and Q
+
+// REC: 0 = dense models, 1 = the packed Q / R record, 2 = the packed model words (stage sized for all 37)
+template <typename T, int N, int M, bool SHARED = false, int REC = 0>
 struct Stage {
     // byte sizes of one tile of each array
     static constexpr int XB = TILE * N * sizeof(T);
@@ -56,17 +69,17 @@ struct Stage {
     static constexpr int HB = TILE * M * N * sizeof(T);
     static constexpr int RB = TILE * M * M * sizeof(T);
     static constexpr int ZB = TILE * M * sizeof(T);
-    static constexpr int QB = SYM ? TILE * SYM_PLANES * sizeof(T) : PB;    // SYM: the packed record (Q and R)
+    static constexpr int QB = REC == 1 ? TILE * SYM_PLANES * sizeof(T) : REC == 2 ? TILE * WORDS * sizeof(T) : PB;
     // offsets (bulk-copy destinations must be 16-byte aligned; 128 keeps every block on its own lines)
     static constexpr int align_up(int v) { return (v + 127) & ~127; }
     // (a bank that shares its models stages only P, x, z: a third of the bytes, so more stages and CTAs fit)
     static constexpr int OP = 0;
     static constexpr int OF = OP + align_up(PB);
-    static constexpr int OQ = OF + (SHARED ? 0 : align_up(PB));
+    static constexpr int OQ = OF + (SHARED || REC == 2 ? 0 : align_up(PB));     // Q, or the record
     static constexpr int OH = OQ + (SHARED ? 0 : align_up(QB));
-    static constexpr int OX = OH + (SHARED ? 0 : align_up(HB));
+    static constexpr int OX = OH + (SHARED || REC == 2 ? 0 : align_up(HB));
     static constexpr int OR_ = OX + align_up(XB);
-    static constexpr int OZ = OR_ + (SHARED || SYM ? 0 : align_up(RB));
+    static constexpr int OZ = OR_ + (SHARED || REC ? 0 : align_up(RB));
     static constexpr int BYTES = OZ + align_up(ZB);
 };
 
@@ -115,34 +128,40 @@ struct FastP {
     float alpha_sq;
     const float *x, *P, *z;         // the prior state and the measurements (dense AoS)
     const float *F, *Q, *H, *R;     // per-filter models (SHARED == 0) or the bank's one model (SHARED == 1)
-    const float *sym;               // SYM: the packed record of Q and R (replaces Q, R)
+    const float *rec;               // REC: the packed record (replaces Q, R; with REC == 2 F and H as well)
     float Fh[N * N], Qh[N * N], Hh[M * N], Rh[M * M];   // used when SHARED == 2: the shared models ride in the launch
-                                                        // parameters, so every product with them reads the constant bank
+                                                        // parameters, so every product with them reads the constant bank;
+                                                        // REC == 2: the words the whole bank shares
     float *x_out, *P_out;
     const uint8_t *valid;
     float *x_prior, *P_prior, *K, *y, *S, *SI, *ll;
     int32_t *status;
     int sticky;                       // BKE_STATUS_STICKY: write status only on failure
+    uint64_t varying;               // REC == 2: bit e set = word e is read from the record...
+    int slot_off[WORDS];            // ...at this byte offset into a tile's record (its plane * TILE * 4)
+    int rec_planes;                 // REC == 2: planes per tile of the record,
+    int rec_first, rec_copy;        // the first plane this MODE reads and how many it reads
 };
 
 // MODE: 3 = predict+update, 1 = predict only, 2 = update only
 // SHARED: 0 = per-filter models (staged by bulk copies), 1 = one model for the bank read from device
 // memory, 2 = one model for the bank carried in the kernel parameters
-// SYM (SHARED == 0 only): Q and R come from the packed record p.sym instead of p.Q, p.R
+// REC (SHARED == 0 only): 1 = Q and R come from the packed record p.rec instead of p.Q, p.R;
+// 2 = every model word the bank's filters differ in comes from p.rec, the others from p.Fh .. p.Rh
 // Each CTA keeps STAGES tiles in flight.  Resident CTAs per SM: 3 with per-filter models (33 KB per
-// stage, 29.5 KB with the packed record), 4 with one shared model (11 KB per stage), 5 when that model
+// stage, 29.5 KB with either record), 4 with one shared model (11 KB per stage), 5 when that model
 // rides in the launch parameters.
 constexpr int STAGES = 2;
 constexpr int kf42_ctas_per_sm(int shared) { return shared == 2 ? 5 : (shared ? 4 : 3); }
 
-template <int MODE, int SHARED, bool EXTRAS, bool SYM = false>
+template <int MODE, int SHARED, bool EXTRAS, int REC = 0>
 __global__ void __launch_bounds__(TILE, kf42_ctas_per_sm(SHARED))
 kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 {
     constexpr int N = 4, M = 2;
-    static_assert(!(SYM && SHARED), "the packed record holds per-filter models");
-    using St = Stage<float, N, M, SHARED != 0, SYM>;
-    // SYM: the part of a tile's record this MODE reads (the Q planes, the R planes or both)
+    static_assert(!(REC && SHARED), "the packed records hold per-filter models");
+    using St = Stage<float, N, M, SHARED != 0, REC>;
+    // REC == 1: the part of a tile's record this MODE reads (the Q planes, the R planes or both)
     constexpr int SYM_FIRST = (MODE & 1) ? 0 : SYM_Q_PLANES;
     constexpr int SYM_LAST = (MODE & 2) ? SYM_PLANES : SYM_Q_PLANES;
     constexpr uint32_t SYM_BYTES = (SYM_LAST - SYM_FIRST) * TILE * 4;
@@ -163,9 +182,11 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
         const uint32_t nf = left < TILE ? (uint32_t)left : (uint32_t)TILE;
         const uint32_t zb = (nf * M * 4) & ~15u;
         uint32_t tx = nf * (N + N * N) * 4;
-        if (!SHARED && DO_P) tx += nf * (SYM ? 1 : 2) * N * N * 4;
-        if (!SHARED && DO_U) tx += nf * (M * N + (SYM ? 0 : M * M)) * 4;
-        if (SYM) tx += SYM_BYTES;           // the record is padded to whole tiles: always the full planes
+        if (!SHARED && REC != 2 && DO_P) tx += nf * (REC ? 1 : 2) * N * N * 4;
+        if (!SHARED && REC != 2 && DO_U) tx += nf * (M * N + (REC ? 0 : M * M)) * 4;
+        // the records are padded to whole tiles: always the full planes
+        if (REC == 1) tx += SYM_BYTES;
+        if (REC == 2) tx += (uint32_t)p.rec_copy * TILE * 4;
         if (DO_U) tx += zb;
         mbar_expect_tx(bar, tx);
         auto load = [&](int off, const float *src, int per_filter, uint32_t bytes, uint64_t pol) {
@@ -174,15 +195,17 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
         };
         load(St::OP, p.P, N * N, nf * N * N * 4, pol_last);
         load(St::OX, p.x, N, nf * N * 4, pol_last);
-        if (!SHARED && DO_P) {
+        if (!SHARED && REC != 2 && DO_P) {
             load(St::OF, p.F, N * N, nf * N * N * 4, pol_first);
-            if (!SYM) load(St::OQ, p.Q, N * N, nf * N * N * 4, pol_first);
+            if (!REC) load(St::OQ, p.Q, N * N, nf * N * N * 4, pol_first);
         }
-        if (!SHARED && DO_U) {
+        if (!SHARED && REC != 2 && DO_U) {
             load(St::OH, p.H, M * N, nf * M * N * 4, pol_first);
-            if (!SYM) load(St::OR_, p.R, M * M, nf * M * M * 4, pol_first);
+            if (!REC) load(St::OR_, p.R, M * M, nf * M * M * 4, pol_first);
         }
-        if (SYM) load(St::OQ + SYM_FIRST * TILE * 4, p.sym + SYM_FIRST * TILE, SYM_PLANES, SYM_BYTES, pol_first);
+        if (REC == 1) load(St::OQ + SYM_FIRST * TILE * 4, p.rec + SYM_FIRST * TILE, SYM_PLANES, SYM_BYTES, pol_first);
+        if (REC == 2 && p.rec_copy)
+            load(St::OQ + p.rec_first * TILE * 4, p.rec + p.rec_first * TILE, p.rec_planes, p.rec_copy * TILE * 4, pol_first);
         if (DO_U && zb) load(St::OZ, p.z, M, zb, pol_first);
     };
 
@@ -247,26 +270,47 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
             x[0] = v.x; x[1] = v.y; x[2] = v.z; x[3] = v.w;
         }
         lds_row<N>(sb + St::OP, tid, P);
-        // SYM: word `tid` of plane k of the record; the lower triangles are the same registers
-        const float *rec = reinterpret_cast<const float *>(sb + St::OQ) + tid;
+        // REC: word `tid` of a plane of the record (no bank conflicts); the lower triangles are the same
+        // registers.  REC == 1 holds all 13 Q / R words, in order; REC == 2 the words in p.varying, and
+        // the others are the bank's shared values.  (The shared values are run-time parameters, so the
+        // arithmetic is the same instructions as with a dense model: nothing is folded away.)
+        const unsigned char *rec = sb + St::OQ + tid * 4;
+        auto word = [&](int e, float shared) -> float {
+            if (REC == 1) return *reinterpret_cast<const float *>(rec + (e < W_H ? e - W_Q : e - W_R + SYM_Q_PLANES) * TILE * 4);
+            return (p.varying >> e) & 1 ? *reinterpret_cast<const float *>(rec + p.slot_off[e]) : shared;
+        };
         if (!SHARED && DO_P) {
-            lds_row<N>(sb + St::OF, tid, F);
-            if (SYM) {
-                int k = 0;
+            if (REC == 2) {
 #pragma unroll
                 for (int i = 0; i < N; i++)
 #pragma unroll
-                    for (int j = i; j < N; j++, k++) Q[i][j] = Q[j][i] = rec[k * TILE];
+                    for (int j = 0; j < N; j++) F[i][j] = word(W_F + i * N + j, p.Fh[i * N + j]);
+            } else {
+                lds_row<N>(sb + St::OF, tid, F);
+            }
+            if (REC) {
+                int k = W_Q;
+#pragma unroll
+                for (int i = 0; i < N; i++)
+#pragma unroll
+                    for (int j = i; j < N; j++, k++) Q[i][j] = Q[j][i] = word(k, p.Qh[i * N + j]);
             } else {
                 lds_row<N>(sb + St::OQ, tid, Q);
             }
         }
         if (!SHARED && DO_U) {
-            lds_row<M>(sb + St::OH, tid, H);
-            if (SYM) {
-                R[0][0] = rec[SYM_Q_PLANES * TILE];
-                R[0][1] = R[1][0] = rec[(SYM_Q_PLANES + 1) * TILE];
-                R[1][1] = rec[(SYM_Q_PLANES + 2) * TILE];
+            if (REC == 2) {
+#pragma unroll
+                for (int a = 0; a < M; a++)
+#pragma unroll
+                    for (int j = 0; j < N; j++) H[a][j] = word(W_H + a * N + j, p.Hh[a * N + j]);
+            } else {
+                lds_row<M>(sb + St::OH, tid, H);
+            }
+            if (REC) {
+                R[0][0] = word(W_R, p.Rh[0]);
+                R[0][1] = R[1][0] = word(W_R + 1, p.Rh[1]);
+                R[1][1] = word(W_R + 2, p.Rh[3]);
             } else {
                 float4 r = lds_chunk<16>(sb + St::OR_, tid, 0);
                 R[0][0] = r.x; R[0][1] = r.y; R[1][0] = r.z; R[1][1] = r.w;
@@ -296,14 +340,15 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 #pragma unroll
             for (int j = 0; j < N; j++) acc ^= __float_as_uint(P[i][j]);
         }
-        // (SYM: each loaded word once; folding a mirrored pair would cancel it out of the predicate)
+        // (REC: each loaded word once; folding a mirrored pair would cancel it out of the predicate.
+        // REC == 2 folds every model word: a shared one is a launch parameter and harmless in it)
         if (!SHARED && DO_P) {
 #pragma unroll
             for (int i = 0; i < N; i++)
 #pragma unroll
                 for (int j = 0; j < N; j++) {
                     acc ^= __float_as_uint(F[i][j]);
-                    if (!SYM || j >= i) acc ^= __float_as_uint(Q[i][j]);
+                    if (!REC || j >= i) acc ^= __float_as_uint(Q[i][j]);
                 }
         }
         if (!SHARED && DO_U) {
@@ -313,7 +358,7 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
                 for (int j = 0; j < N; j++) acc ^= __float_as_uint(H[a][j]);
 #pragma unroll
                 for (int b = 0; b < M; b++)
-                    if (!SYM || b >= a) acc ^= __float_as_uint(R[a][b]);
+                    if (!REC || b >= a) acc ^= __float_as_uint(R[a][b]);
             }
         }
         if (DO_U) acc ^= __float_as_uint(z[0]) ^ __float_as_uint(z[1]);
@@ -394,18 +439,18 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 
 // ---------------------------------------------------------------------------- host side
 // switches (environment, read once): BKE_KF_L2 = 0 disables the L2 eviction-priority hints,
-// BKE_KF_SYM = 0 the packed record, BKE_KF_HOST_MODELS = 0 the shared models in the launch parameters
+// BKE_KF_SYM = 0 both packed records, BKE_KF_HOST_MODELS = 0 the shared models in the launch parameters
 int env_int(const char *name, int dflt)
 {
     const char *v = getenv(name);
     return v ? atoi(v) : dflt;
 }
 
-template <int MODE, int SHARED, bool EXTRAS, bool SYM = false>
+template <int MODE, int SHARED, bool EXTRAS, int REC = 0>
 int launch_variant(const FastP<4, 2> &p, cudaStream_t s)
 {
-    using St = Stage<float, 4, 2, SHARED != 0, SYM>;
-    auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, SYM>;
+    using St = Stage<float, 4, 2, SHARED != 0, REC>;
+    auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, REC>;
     const int smem = STAGES * St::BYTES;
     static bool configured[64] = {false};
     int dev = 0;
@@ -468,7 +513,99 @@ kf42_pack_sym_kernel(int64_t n_filters, int64_t slots, const float4 *__restrict_
     }
 }
 
-// BKE_KF_SYM = 0 turns the packed record off (both entry points report BKE_ERR_UNSUPPORTED)
+// The 37 model words of filter f (order at WORDS) from the dense F [N,4,4], Q [N,4,4], H [N,2,4], R [N,2,2];
+// *asym is set when Q or R differs from its transpose in any bit.
+__device__ __forceinline__ void kf42_model_words(const float4 *__restrict__ F, const float4 *__restrict__ Q,
+                                                 const float4 *__restrict__ H, const float4 *__restrict__ R,
+                                                 int64_t f, float (&w)[WORDS], bool &asym)
+{
+    float q[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const float4 a = F[f * 4 + i], b = Q[f * 4 + i];
+        w[W_F + 4 * i] = a.x; w[W_F + 4 * i + 1] = a.y; w[W_F + 4 * i + 2] = a.z; w[W_F + 4 * i + 3] = a.w;
+        q[i][0] = b.x; q[i][1] = b.y; q[i][2] = b.z; q[i][3] = b.w;
+    }
+    asym = false;
+    int k = W_Q;
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int j = i; j < 4; j++, k++) {
+            w[k] = q[i][j];
+            asym |= __float_as_uint(q[i][j]) != __float_as_uint(q[j][i]);
+        }
+#pragma unroll
+    for (int a = 0; a < 2; a++) {
+        const float4 h = H[f * 2 + a];
+        w[W_H + 4 * a] = h.x; w[W_H + 4 * a + 1] = h.y; w[W_H + 4 * a + 2] = h.z; w[W_H + 4 * a + 3] = h.w;
+    }
+    const float4 r = R[f];
+    w[W_R] = r.x; w[W_R + 1] = r.y; w[W_R + 2] = r.w;
+    asym |= __float_as_uint(r.y) != __float_as_uint(r.z);
+}
+
+// Scan pass: OR into map->varying the words in which a filter differs from filter 0 (as bits), and set
+// map->asymmetric when one is asymmetric; block 0 also writes filter 0's words.  The caller zeroed both.
+__global__ void __launch_bounds__(256)
+kf42_scan_models_kernel(int64_t n_filters, const float4 *__restrict__ F, const float4 *__restrict__ Q,
+                        const float4 *__restrict__ H, const float4 *__restrict__ R, bke_kf_model_map *map)
+{
+    float w0[WORDS], w[WORDS];
+    bool asym = false, a;
+    kf42_model_words(F, Q, H, R, 0, w0, a);
+    uint32_t lo = 0, hi = 0;
+    for (int64_t f = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; f < n_filters; f += (int64_t)gridDim.x * blockDim.x) {
+        kf42_model_words(F, Q, H, R, f, w, a);
+        asym |= a;
+#pragma unroll
+        for (int e = 0; e < WORDS; e++) {
+            const uint32_t d = __float_as_uint(w[e]) != __float_as_uint(w0[e]);
+            if (e < 32) lo |= d << e;
+            else hi |= d << (e - 32);
+        }
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+#pragma unroll
+        for (int e = 0; e < WORDS; e++) map->words[e] = w0[e];
+    }
+    __shared__ uint32_t red[3][8];
+    lo = __reduce_or_sync(FULL, lo);
+    hi = __reduce_or_sync(FULL, hi);
+    const uint32_t as = __reduce_or_sync(FULL, asym ? 1u : 0u);
+    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+    if (lane == 0) { red[0][warp] = lo; red[1][warp] = hi; red[2][warp] = as; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int i = 1; i < (int)blockDim.x / 32; i++) { lo |= red[0][i]; hi |= red[1][i]; }
+        uint32_t as_all = 0;
+        for (int i = 0; i < (int)blockDim.x / 32; i++) as_all |= red[2][i];
+        const unsigned long long v = (unsigned long long)hi << 32 | lo;
+        if (v) atomicOr(reinterpret_cast<unsigned long long *>(&map->varying), v);
+        if (as_all) atomicOr(&map->asymmetric, 1);
+    }
+}
+
+// Pack pass: the words in `varying` of every filter slot into the record described at WORDS (the
+// padding of the last tile is written with zeros), one thread per slot.
+__global__ void __launch_bounds__(256)
+kf42_pack_models_kernel(int64_t n_filters, int64_t slots, const float4 *__restrict__ F, const float4 *__restrict__ Q,
+                        const float4 *__restrict__ H, const float4 *__restrict__ R, uint64_t varying, int planes,
+                        float *__restrict__ rec)
+{
+    for (int64_t f = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; f < slots; f += (int64_t)gridDim.x * blockDim.x) {
+        float w[WORDS] = {};
+        bool a;
+        if (f < n_filters) kf42_model_words(F, Q, H, R, f, w, a);
+        float *out = rec + (f / TILE) * ((int64_t)planes * TILE) + (f % TILE);
+        int s = 0;
+#pragma unroll
+        for (int e = 0; e < WORDS; e++)
+            if ((varying >> e) & 1) out[(s++) * TILE] = w[e];
+    }
+}
+
+// BKE_KF_SYM = 0 turns the packed records off (their entry points report BKE_ERR_UNSUPPORTED)
 bool sym_enabled()
 {
     static const int env = env_int("BKE_KF_SYM", 1);
@@ -503,10 +640,64 @@ int launch_kf_pack_sym(int64_t n_filters, const void *Q, const void *R, void *re
     return check_cuda(cudaGetLastError(), "kf42_pack_sym_kernel launch");
 }
 
-int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *sym)
+size_t kf_packed_models_bytes(int64_t n_filters, uint64_t varying)
 {
-    if (sym && !sym_enabled()) { set_error("the packed symmetric models are disabled (BKE_KF_SYM=0)"); return BKE_ERR_UNSUPPORTED; }
-    if (sym && misaligned16(sym)) { set_error("record must be 16-byte aligned"); return BKE_ERR_UNSUPPORTED; }
+    if (n_filters <= 0 || (varying >> WORDS) != 0) return 0;
+    return (size_t)((n_filters + TILE - 1) / TILE) * __builtin_popcountll(varying) * TILE * sizeof(float);
+}
+
+static int check_models(int64_t n_filters, const void *F, const void *Q, const void *H, const void *R, const void *out)
+{
+    if (!sym_enabled()) { set_error("the packed models are disabled (BKE_KF_SYM=0)"); return BKE_ERR_UNSUPPORTED; }
+    if (n_filters >= (int64_t)1 << 30) { set_error("the packed models take at most 2^30 filters"); return BKE_ERR_UNSUPPORTED; }
+    if (misaligned16(F) || misaligned16(Q) || misaligned16(H) || misaligned16(R) || misaligned16(out)) {
+        set_error("F, Q, H, R and the map or record must be 16-byte aligned");
+        return BKE_ERR_UNSUPPORTED;
+    }
+    return BKE_OK;
+}
+
+static int64_t pass_grid(int64_t threads)
+{
+    const int64_t grid = (threads + 255) / 256;
+    return grid < (int64_t)sm_count() * 16 ? grid : (int64_t)sm_count() * 16;
+}
+
+int launch_kf_scan_models(int64_t n_filters, const void *F, const void *Q, const void *H, const void *R,
+                          bke_kf_model_map *map, cudaStream_t s)
+{
+    int rc = check_models(n_filters, F, Q, H, R, map);
+    if (rc) return rc;
+    // varying and asymmetric start at zero; filter 0's words are written by the kernel
+    if (check_cuda(cudaMemsetAsync(map, 0, sizeof(bke_kf_model_map), s), "cudaMemsetAsync")) return BKE_ERR_CUDA;
+    if (n_filters == 0) return BKE_OK;
+    kf42_scan_models_kernel<<<(int)pass_grid(n_filters), 256, 0, s>>>(n_filters, (const float4 *)F, (const float4 *)Q,
+                                                                      (const float4 *)H, (const float4 *)R, map);
+    return check_cuda(cudaGetLastError(), "kf42_scan_models_kernel launch");
+}
+
+int launch_kf_pack_models(int64_t n_filters, const void *F, const void *Q, const void *H, const void *R, uint64_t varying,
+                          void *record, cudaStream_t s)
+{
+    int rc = check_models(n_filters, F, Q, H, R, record);
+    if (rc) return rc;
+    const int64_t slots = (n_filters + TILE - 1) / TILE * TILE;
+    if (slots == 0 || varying == 0) return BKE_OK;
+    kf42_pack_models_kernel<<<(int)pass_grid(slots), 256, 0, s>>>(n_filters, slots, (const float4 *)F, (const float4 *)Q,
+                                                                  (const float4 *)H, (const float4 *)R, varying,
+                                                                  __builtin_popcountll(varying), (float *)record);
+    return check_cuda(cudaGetLastError(), "kf42_pack_models_kernel launch");
+}
+
+int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const bke_kf_model_map *map)
+{
+    const bool packed = map != nullptr, sym = rec != nullptr && !packed;
+    if ((sym || packed) && !sym_enabled()) {
+        set_error(sym ? "the packed symmetric models are disabled (BKE_KF_SYM=0)" : "the packed models are disabled (BKE_KF_SYM=0)");
+        return BKE_ERR_UNSUPPORTED;
+    }
+    if (misaligned16(rec)) { set_error("record must be 16-byte aligned"); return BKE_ERR_UNSUPPORTED; }
+    if (packed && map->asymmetric) { set_error("the map reports an asymmetric Q or R: the bank runs on bke_kf_step"); return BKE_ERR_UNSUPPORTED; }
     if (!(a.dtype == BKE_F32 && a.dim_x == 4 && a.dim_z == 2)) return BKE_ERR_UNSUPPORTED;
     if (a.B != nullptr && a.u != nullptr) return BKE_ERR_UNSUPPORTED;
     if (a.flags & BKE_UPDATE_FIRST) return BKE_ERR_UNSUPPORTED;
@@ -516,7 +707,7 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *sym)
     if (dp) { all_shared &= (a.F_stride == 0 && a.Q_stride == 0); all_dense &= (a.F_stride != 0 && a.Q_stride != 0); }
     if (du) { all_shared &= (a.H_stride == 0 && a.R_stride == 0); all_dense &= (a.H_stride != 0 && a.R_stride != 0); }
     if (!all_shared && !all_dense) return BKE_ERR_UNSUPPORTED;
-    if (sym && !all_dense) return BKE_ERR_UNSUPPORTED;
+    if ((sym || packed) && !all_dense) return BKE_ERR_UNSUPPORTED;
     if (a.n_filters >= (int64_t)1 << 30) return BKE_ERR_UNSUPPORTED;
     // bulk copies and the 16-byte stores need 16-byte aligned global bases
     const auto mis = misaligned16;
@@ -536,7 +727,7 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *sym)
     }
     p.x = (const float *)a.x; p.P = (const float *)a.P; p.z = (const float *)a.z;
     p.F = (const float *)a.F; p.Q = (const float *)a.Q; p.H = (const float *)a.H; p.R = (const float *)a.R;
-    p.sym = (const float *)sym;
+    p.rec = (const float *)rec;
     p.x_out = (float *)a.x_out; p.P_out = (float *)a.P_out;
     p.valid = a.z_valid;
     p.x_prior = (float *)a.x_prior; p.P_prior = (float *)a.P_prior; p.K = (float *)a.K; p.y = (float *)a.y;
@@ -549,6 +740,25 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *sym)
         memcpy(p.Fh, a.F_host, sizeof(p.Fh)); memcpy(p.Qh, a.Q_host, sizeof(p.Qh));
         memcpy(p.Hh, a.H_host, sizeof(p.Hh)); memcpy(p.Rh, a.R_host, sizeof(p.Rh));
     }
+    if (packed) {
+        // the shared words ride in the launch parameters (lower triangles mirrored), the others are
+        // read from the record at their plane
+        const float *w = map->words;
+        memcpy(p.Fh, w + W_F, sizeof(p.Fh));
+        memcpy(p.Hh, w + W_H, sizeof(p.Hh));
+        for (int i = 0, k = W_Q; i < 4; i++)
+            for (int j = i; j < 4; j++, k++) p.Qh[i * 4 + j] = p.Qh[j * 4 + i] = w[k];
+        p.Rh[0] = w[W_R]; p.Rh[1] = p.Rh[2] = w[W_R + 1]; p.Rh[3] = w[W_R + 2];
+        p.varying = map->varying;
+        for (int e = 0, k = 0; e < WORDS; e++) {
+            p.slot_off[e] = k * TILE * 4;
+            k += (map->varying >> e) & 1;
+        }
+        const int k_all = __builtin_popcountll(map->varying), k_p = __builtin_popcountll(map->varying & PREDICT_WORDS);
+        p.rec_planes = k_all;
+        p.rec_first = dp ? 0 : k_p;
+        p.rec_copy = (du ? k_all : k_p) - p.rec_first;
+    }
     const bool extras = a.x_prior || a.P_prior || a.K || a.y || a.S || a.SI || a.log_likelihood || a.status;
 
 #define BKE_DISPATCH(MODE)                                                                   \
@@ -557,8 +767,10 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *sym)
                                        : launch_variant<MODE, 2, false>(p, s);         \
         if (all_shared) return extras ? launch_variant<MODE, 1, true>(p, s)            \
                                       : launch_variant<MODE, 1, false>(p, s);          \
-        if (sym) return extras ? launch_variant<MODE, 0, true, true>(p, s)             \
-                               : launch_variant<MODE, 0, false, true>(p, s);           \
+        if (packed) return extras ? launch_variant<MODE, 0, true, 2>(p, s)             \
+                                  : launch_variant<MODE, 0, false, 2>(p, s);           \
+        if (sym) return extras ? launch_variant<MODE, 0, true, 1>(p, s)                \
+                               : launch_variant<MODE, 0, false, 1>(p, s);              \
         return extras ? launch_variant<MODE, 0, true>(p, s)                            \
                       : launch_variant<MODE, 0, false>(p, s);                          \
     } while (0)

@@ -19,6 +19,7 @@ Two modes:
 ``predict()`` followed by ``update(z)`` is fused into ONE kernel launch (the predict is deferred
 until the next ``update`` or until somebody looks at the state).
 """
+import ctypes
 import math
 import sys
 
@@ -112,17 +113,19 @@ class KalmanFilter(object):
         self._post_alias = False      # True: x_post / P_post are the live x / P (nothing has moved them since the update)
         self._version = 0            # bumped whenever a tensor the kernels read is re-bound
         self._args_cache = {}
-        # Packed copy of per-filter Q and R (bke_kf_pack_sym_models): derived data, valid for one state
-        # of Q and R.  _qr_version counts re-bindings of Q / R and hand-outs of the live tensors;
-        # together with the tensors' own version counters it names that state (_qr_token).
+        # Packed copy of the per-filter model words that differ between filters (bke_kf_scan_models,
+        # bke_kf_pack_models): derived data, valid for one state of F, Q, H and R.  _model_version counts
+        # re-bindings of F / Q / H / R and hand-outs of the live tensors; together with the tensors' own
+        # version counters it names that state (the token of _sym_record).
         self._sym_ok = not self._single and N > 0 and (n, m) == (4, 2) and self._dtype == torch.float32
         self._sym_buf = None          # the current record, re-packed in place until a captured graph reads it
         self._sym_pinned = False      # True: a captured graph reads _sym_buf, so it is never written again
         self._sym_held = []           # earlier records captured graphs read (kept for the bank's lifetime)
-        self._sym_flag = None         # int32 on the device: 1 = the last pack found an asymmetric filter
+        self._sym_map = None          # bke_kf_model_map on the device, filled by the scan
+        self._sym_host_map = None     # the host copy of the map _sym_buf was packed with (launch parameters)
         self._sym_state = None        # (token, usable) of _sym_buf's pack
-        self._qr_version = 0
-        self._qr_last = None          # the token of the previous launch
+        self._model_version = 0
+        self._model_last = None       # the token of the previous launch
 
     # ------------------------------------------------------------------ helpers
     def _model(self, a, rows, cols, name):
@@ -233,20 +236,20 @@ class KalmanFilter(object):
                 return _Linked(t.cpu().numpy(), self, name)
             # the caller may edit the live tensor in place: a deferred predict must run with the
             # model it was issued with (the reference's predict has already happened), and the
-            # host copy can no longer be trusted, nor can the packed copy of Q and R
+            # host copy can no longer be trusted, nor can the packed model words
             self._flush()
             if self._host.pop(name, None) is not None:
                 self._version += 1
-            if name in "QR":
-                self._qr_version += 1
+            if name in "FQHR":
+                self._model_version += 1
             return t
 
         def set_(self, v):
             self._flush()                                   # predict(); kf.F = F2; update(): the predict used the OLD F
             self._version += 1
             self._host.pop(name, None)
-            if name in "QR":
-                self._qr_version += 1
+            if name in "FQHR":
+                self._model_version += 1
             if v is None:
                 setattr(self, priv, None)
                 return
@@ -417,7 +420,7 @@ class KalmanFilter(object):
     def _step(self, a, rec):
         s = stream_ptr(self._device)
         if rec is not None:
-            rc = self._lib.bke_kf_step_sym(a, ptr(rec), s)
+            rc = self._lib.bke_kf_step_packed(a, ptr(rec) if rec.numel() else None, self._sym_host_map, s)
             if rc != _lib.BKE_ERR_UNSUPPORTED:
                 _lib.check(rc)
                 return
@@ -438,21 +441,24 @@ class KalmanFilter(object):
         bank's lifetime (_sym_held); any other is freed once no cached argument struct holds it."""
         if self._sym_buf is not None and self._sym_pinned:
             self._sym_held.append(self._sym_buf)
-        self._sym_buf = self._sym_state = None
+        self._sym_buf = self._sym_state = self._sym_host_map = None
         self._sym_pinned = False
 
     def _sym_record(self):
-        """The packed copy of the per-filter Q and R for a launch with the bank's own models, or None
-        (the kernels then read the dense Q and R).
+        """The packed copy of the per-filter model words for a launch with the bank's own models, or
+        None (the kernels then read the dense F, Q, H and R).
 
-        The copy is derived data and must never go stale: it is used only while Q and R are in the
+        Most per-filter banks are a template plus a few per-filter parameters: the scan finds the words
+        of F, the upper triangle of Q, H and the upper triangle of R that differ between filters, the
+        record holds only those, and the words the whole bank shares ride in the launch parameters.
+        The copy is derived data and must never go stale: it is used only while F, Q, H and R are in the
         state it was packed from, i.e. neither re-assigned, nor handed out by their getters, nor edited
         in place through torch (the tensors' version counters).  It is (re)packed only outside stream
-        capture, and only when Q and R are the same as at the previous launch, so a loop that assigns
-        Q or R every step never pays for a pack (about 132 B per filter, once); a bank with an
-        asymmetric filter is packed once per state of Q and R and then runs on the dense models.
-        A record that a CUDA graph was captured with is never written again: the graph keeps reading
-        the Q and R of its capture (see ``capture``), and a later pack goes to a new record."""
+        capture, and only when the models are the same as at the previous launch, so a loop that assigns
+        a model every step never pays for a pack (two passes over the 176 B of models per filter, once);
+        a bank with an asymmetric Q or R is scanned once per state of the models and then runs on the
+        dense models.  A record that a CUDA graph was captured with is never written again: the graph
+        keeps reading the models of its capture (see ``capture``), and a later pack goes to a new record."""
         if not self._sym_ok:
             return None
         F, Q, H, R = self._F, self._Q, self._H, self._R
@@ -460,8 +466,8 @@ class KalmanFilter(object):
         if any(t is None or t.dim() != 3 for t in (F, Q, H, R)):
             self._sym_drop()
             return None
-        token = (self._qr_version, Q._version, R._version)
-        last, self._qr_last = self._qr_last, token
+        token = (self._model_version, F._version, Q._version, H._version, R._version)
+        last, self._model_last = self._model_last, token
         if self._sym_state is not None and self._sym_state[0] == token:
             if not self._sym_state[1]:
                 return None
@@ -473,20 +479,31 @@ class KalmanFilter(object):
         if self._sym_pinned:
             self._sym_drop()
         with torch.cuda.device(self._device):
-            if self._sym_buf is None:
-                nb = self._lib.bke_kf_sym_models_bytes(self.n_filters)
-                self._sym_buf = torch.empty(nb // 4, dtype=torch.float32, device=self._device)
-                self._version += 1                          # the cached argument structs must keep the record alive
-            if self._sym_flag is None:
-                self._sym_flag = torch.empty(1, dtype=torch.int32, device=self._device)
-            rc = self._lib.bke_kf_pack_sym_models(self.n_filters, 4, 2, _lib.BKE_F32, ptr(Q), ptr(R), ptr(self._sym_buf),
-                                                  ptr(self._sym_flag), stream_ptr(self._device))
+            s = stream_ptr(self._device)
+            if self._sym_map is None:
+                self._sym_map = torch.empty(ctypes.sizeof(_lib.KfModelMap), dtype=torch.uint8, device=self._device)
+            rc = self._lib.bke_kf_scan_models(self.n_filters, 4, 2, _lib.BKE_F32, ptr(F), ptr(Q), ptr(H), ptr(R),
+                                              ptr(self._sym_map), s)
             if rc == _lib.BKE_ERR_UNSUPPORTED:
                 self._sym_ok = False
                 self._sym_drop()
                 return None
             _lib.check(rc)
-            usable = int(self._sym_flag.item()) == 0
+            hmap = _lib.KfModelMap.from_buffer_copy(self._sym_map.cpu().numpy().tobytes())     # the one host sync
+            usable = hmap.asymmetric == 0
+            if usable:
+                nb = self._lib.bke_kf_packed_models_bytes(self.n_filters, hmap.varying)
+                if self._sym_buf is None or self._sym_buf.numel() * 4 != nb:
+                    self._sym_buf = torch.empty(nb // 4, dtype=torch.float32, device=self._device)
+                    self._version += 1                      # the cached argument structs must keep the record alive
+                rc = self._lib.bke_kf_pack_models(self.n_filters, 4, 2, _lib.BKE_F32, ptr(F), ptr(Q), ptr(H), ptr(R),
+                                                  hmap.varying, ptr(self._sym_buf) if nb else None, s)
+                if rc == _lib.BKE_ERR_UNSUPPORTED:
+                    self._sym_ok = False
+                    self._sym_drop()
+                    return None
+                _lib.check(rc)
+                self._sym_host_map = hmap
         self._sym_state = (token, usable)
         return self._sym_buf if usable else None
 
@@ -574,10 +591,11 @@ class KalmanFilter(object):
         state is NOT rolled back after the warm-up / capture runs: set ``x`` / ``P`` afterwards.
 
         A 4/2 float32 bank whose models are all per filter and whose Q and R are exactly symmetric
-        steps from a packed copy of Q and R (DESIGN.md §2): the graph reads the copy taken before
-        the capture, so Q and R are frozen into it.  Re-capture after changing Q or R, whether by
-        assignment or in place; refilling z, x or P (or F, H) in place between replays works as for
-        any graph."""
+        steps from a packed copy of its model words (DESIGN.md §2): the graph reads the copy taken
+        before the capture, and the words every filter shares are baked into its launch parameters,
+        so F, Q, H and R are all frozen into it.  Re-capture after changing any of them, whether by
+        assignment or in place; refilling z, x or P in place between replays works as for any
+        graph."""
         self._flush()
         return StepGraph(fn, self._device, warmup)
 

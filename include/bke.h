@@ -137,6 +137,46 @@ int bke_kf_pack_sym_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int3
                            const void *R, void *record, int32_t *asymmetric, void *stream);
 int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream);
 
+/* Packed model words of a dim_x = 4, dim_z = 2, BKE_F32 bank whose F, Q, H and R are all per filter.
+ * Banks built from a template and a few per-filter parameters (dt, q, r) repeat most model words bit for
+ * bit in every filter; a step then only needs the words that differ, and the others ride in the launch
+ * parameters (40 instead of 148 B of models per filter for a constant-velocity bank with per-filter dt,
+ * q and r).  A filter's models are 37 words, in this order (word e = bit e of `varying`):
+ *   F 0..15 (row-major) | Q 16..25 (upper triangle: Q00 Q01 Q02 Q03 Q11 Q12 Q13 Q22 Q23 Q33) |
+ *   H 26..33 (row-major) | R 34..36 (R00 R01 R11).
+ *   bke_kf_scan_models          fills the map (DEVICE memory, 16-byte aligned) from the dense F[N,4,4],
+ *                               Q[N,4,4], H[N,2,4], R[N,2,2]: bit e of `varying` is set when word e of
+ *                               some filter differs from filter 0's in any bit (-0.0 against +0.0 and two
+ *                               NaN payloads differ), `words` are filter 0's, `asymmetric` is 1 when a
+ *                               filter's Q or R differs from its transpose in any bit (the record may only
+ *                               be used when it is 0);
+ *   bke_kf_packed_models_bytes  the size of the record of n_filters filters for a `varying` mask (0 for a
+ *                               mask with bits above 36); the caller allocates it, 16-byte aligned;
+ *   bke_kf_pack_models          fills the record: one tile of 128 filters after the other, each tile
+ *                               k = popcount(varying) planes of 128 floats, plane s holding the s-th
+ *                               varying word (in the order above) of each filter of the tile, padded with
+ *                               zeros to a whole last tile;
+ *   bke_kf_step_packed          bke_kf_step with the record and a HOST copy of the map standing in for
+ *                               args->F, Q, H and R (which must still be the per-filter arrays they were
+ *                               scanned and packed from, unchanged since); the results are bit-identical
+ *                               to bke_kf_step's.  The record may be NULL when no word varies.
+ * The calls return BKE_ERR_UNSUPPORTED for other shapes, dtypes, shared models, an asymmetric map,
+ * misaligned pointers, and when the environment sets BKE_KF_SYM=0; bke_kf_step is then the call to make. */
+#define BKE_KF42_MODEL_WORDS 37
+typedef struct bke_kf_model_map {
+    uint64_t varying;                       /* bit e: word e differs between filters */
+    int32_t asymmetric;                     /* 1: some Q or R is not exactly symmetric */
+    int32_t reserved;
+    float words[BKE_KF42_MODEL_WORDS];      /* filter 0's words */
+} bke_kf_model_map;
+
+int bke_kf_scan_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *F, const void *Q,
+                       const void *H, const void *R, bke_kf_model_map *map, void *stream);
+size_t bke_kf_packed_models_bytes(int64_t n_filters, uint64_t varying);
+int bke_kf_pack_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *F, const void *Q,
+                       const void *H, const void *R, uint64_t varying, void *record, void *stream);
+int bke_kf_step_packed(const bke_kf_args *args, const void *record, const bke_kf_model_map *host_map, void *stream);
+
 /* KalmanFilter.batch_filter over T epochs for a bank (kalman_filter.py:826-993; procedural
  * twin :1664-1788): the time loop runs inside one kernel with the models resident on chip.
  *   zs[T,N,m], zs_valid[T,N] (or NULL)

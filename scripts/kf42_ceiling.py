@@ -11,10 +11,13 @@ Prints JSON lines (and writes them to DIR/kf42_ceiling.jsonl with --out):
              filters; GB/s and its share of the data sheet's 3.35 TB/s
   ceiling_sym  the same twin with Q and R replaced by the packed 52 B-per-filter stream a symmetric
              bank's step reads instead (bke_kf_pack_sym_models): 316 B per filter
+  ceiling_words  the same twin with F, Q, H and R replaced by one 40 B-per-filter stream, the 10 model
+             words that differ between the filters of the bench bank (bke_kf_pack_models): 208 B
   step       the shipped step (KalmanFilter.predict + update, per-filter F/H/Q/R) replayed as CUDA
              graphs of 4 steps like bench.py, at N = 2^19 .. 2^22 (all above the bound under which
              the L2 hints are used); per-step time and GB/s for every N, counted with the bytes the
-             step moves (316 when it reads the packed Q / R, 344 with BKE_KF_SYM=0)
+             step moves (4 * popcount(varying) + 168 when it reads the packed model words, 208 for
+             the bench bank; 344 with BKE_KF_SYM=0)
   fit        t(N) = a + b N over those sizes: a is the fixed cost of a step, bytes / b its
              streaming rate
   shared     the same graph of 4 steps for a 2^20-filter bank whose F/H/Q/R are shared (one model
@@ -41,6 +44,7 @@ SRC = os.path.join(HERE, "kf42_ceiling.cu")
 LIB = os.path.join(HERE, "kf42_ceiling.so")
 BYTES = 344                 # per filter-step: x, P, F, Q, H, R, z read (264 B), x, P written (80 B)
 BYTES_SYM = 316             # the same with Q and R read as their packed upper triangles (52 B instead of 80)
+BYTES_WORDS = 208           # the same with F, Q, H, R read as the 10 varying words of the bench bank (40 B instead of 176)
 PEAK_GBS = 3350.0           # H100 SXM data sheet, HBM3
 RING = 4                    # steps per graph replay, as in bench.py
 
@@ -80,7 +84,7 @@ def reps_for(n_filters, seconds=0.3):
     return max(8, int(seconds / (n_filters * BYTES / 2.5e12)))
 
 
-def ceiling(torch, rounds, sym=False):
+def ceiling(torch, rounds, mode=0):
     lib = ctypes.CDLL(build_lib())
     lib.kf42_traffic.restype = ctypes.c_int
     lib.kf42_traffic.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
@@ -89,7 +93,7 @@ def ceiling(torch, rounds, sym=False):
     g = torch.Generator(device=dev).manual_seed(5)
     arr = {k: torch.randn(N * e, device=dev, generator=g) for k, e in
            (("x", 4), ("P", 16), ("F", 16), ("Q", 16), ("H", 8), ("R", 4), ("z", 2))}
-    nbytes = BYTES_SYM if sym else BYTES
+    nbytes = (BYTES, BYTES_SYM, BYTES_WORDS)[mode]
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
     stream = torch.cuda.current_stream().cuda_stream
     out = {}
@@ -97,7 +101,7 @@ def ceiling(torch, rounds, sym=False):
         grid = sms * per_sm
 
         def run():
-            rc = lib.kf42_traffic(*[arr[k].data_ptr() for k in "xPFQHRz"], N, grid, int(sym), stream)
+            rc = lib.kf42_traffic(*[arr[k].data_ptr() for k in "xPFQHRz"], N, grid, mode, stream)
             assert rc == 0, rc
         for _ in range(5):
             run()
@@ -106,7 +110,7 @@ def ceiling(torch, rounds, sym=False):
         gbs = nbytes * N / (ms * 1e-3) / 1e9
         out["ctas_per_sm_%d" % per_sm] = {"ms": ms, "GBps": gbs, "frac_of_3350": gbs / PEAK_GBS}
     best = max(out.values(), key=lambda v: v["GBps"])
-    return {"what": "ceiling_sym" if sym else "ceiling", "n_filters": N, "bytes_per_filter": nbytes, "ms": best["ms"],
+    return {"what": ("ceiling", "ceiling_sym", "ceiling_words")[mode], "n_filters": N, "bytes_per_filter": nbytes, "ms": best["ms"],
             "GBps": best["GBps"],
             "frac_of_3350": best["frac_of_3350"], "by_grid": out}
 
@@ -148,7 +152,8 @@ def main():
     assert torch.cuda.is_available(), "kf42_ceiling.py measures on a GPU"
     lines = [dict(what="card", **card()), dict(what="library", path=os.environ.get("BKE_LIB_PATH") or "in-tree")]
     lines.append(ceiling(torch, args.rounds))
-    lines.append(ceiling(torch, args.rounds, sym=True))
+    lines.append(ceiling(torch, args.rounds, mode=1))
+    lines.append(ceiling(torch, args.rounds, mode=2))
     sizes, times = [], []
     moved = BYTES
     for lg in (19, 20, 21, 22):
@@ -158,8 +163,8 @@ def main():
         ms = float(np.median(t))
         sizes.append(N); times.append(ms)
         packed = kf._sym_state is not None and kf._sym_state[1]
-        moved = BYTES_SYM if packed else BYTES
-        lines.append({"what": "step", "n_filters": N, "packed_QR": packed, "bytes_per_filter": moved, "ms": ms,
+        moved = 168 + 4 * bin(kf._sym_host_map.varying).count("1") if packed else BYTES
+        lines.append({"what": "step", "n_filters": N, "packed_words": packed, "bytes_per_filter": moved, "ms": ms,
                       "ms_rounds": t, "GBps": moved * N / (ms * 1e-3) / 1e9})
         del kf, graph
         torch.cuda.empty_cache()

@@ -1,5 +1,6 @@
-"""A/B of the 4/2 fp32 bank step with Q and R read dense (344 B per filter-step) or as the packed
-upper triangles of a symmetric bank (316 B), and the one-time cost of packing them.
+"""A/B of the 4/2 fp32 bank step with its models read dense (344 B per filter-step) or as the packed
+model words that differ between the filters (208 B on the bench bank), against the parent's packed
+upper triangles of Q and R (316 B), and the one-time cost of scanning and packing the models.
 
     python scripts/kf42_sym_ab.py [--out DIR] [--rounds R] [--steps 400,50] [--diag-rounds D]
                                   [--baseline-tree DIR]
@@ -7,9 +8,11 @@ upper triangles of a symmetric bank (316 B), and the one-time cost of packing th
 Prints JSON lines (and writes them to DIR/kf42_sym_ab.jsonl with --out):
 
   card     name, power limit and maximum SM clock (read-only nvidia-smi query)
-  pack     device time of bke_kf_pack_sym_models for the 2^20-filter bench bank (CUDA events, median of
-           rounds of 20 calls), with the bytes it moves (80 B read, 52 B written per filter) and the
-           number of steps the saving of 28 B per step takes to repay it
+  pack     device time of bke_kf_scan_models + bke_kf_pack_models for the 2^20-filter bench bank (CUDA
+           events, median of rounds of 20 calls), with the bytes they move (176 B read twice, 40 B
+           written per filter)
+  all_words  device time of one step of a 2^20-filter bank whose 37 model words all vary (316 B either
+           way): bke_kf_step_packed against bke_kf_step_sym, alternated (the cost of the per-word select)
   run      one `bench.py --no-cpu --no-extra --no-resample --steps K` per arm and round: ms_per_step
            and the kernel time of the headline
   diag     one `bench.py --no-cpu --no-resample --steps 50` per arm and round: the ms_per_step of the
@@ -18,7 +21,8 @@ Prints JSON lines (and writes them to DIR/kf42_sym_ab.jsonl with --out):
 
 Arms, alternated inside every round, each in its own process: `dense` (BKE_KF_SYM=0) and `packed`
 (the default) of this tree, and `baseline` (bench.py of another checkout, e.g. the parent commit
-built in place) when --baseline-tree is given.
+built in place) when --baseline-tree is given.  The summary's `repay_steps` is the scan + pack time
+over the per-step saving against the baseline at 400 steps.
 """
 import argparse
 import importlib.util
@@ -44,21 +48,30 @@ def card():
     return mod.card()
 
 
+def _dev(w):
+    import torch
+    return {k: torch.from_numpy(np.ascontiguousarray(w[k])).cuda() for k in "FQHR"}
+
+
 def pack_cost(rounds):
+    import ctypes
     import torch
     from filterpy_b200 import _lib
     from filterpy_b200.common import workloads as wl
     lib = _lib.load()
     w = wl.kf_bank_cv2d(N, seed=1234, steps=1, dtype=np.float32)
-    Q = torch.from_numpy(w["Q"]).cuda()
-    R = torch.from_numpy(w["R"]).cuda()
-    rec = torch.empty(lib.bke_kf_sym_models_bytes(N) // 4, dtype=torch.float32, device="cuda")
-    flag = torch.empty(1, dtype=torch.int32, device="cuda")
+    d = _dev(w)
+    dmap = torch.empty(ctypes.sizeof(_lib.KfModelMap), dtype=torch.uint8, device="cuda")
     s = torch.cuda.current_stream().cuda_stream
+    m = [ptr.data_ptr() for ptr in (d["F"], d["Q"], d["H"], d["R"])]
+    _lib.check(lib.bke_kf_scan_models(N, 4, 2, _lib.BKE_F32, *m, dmap.data_ptr(), s))
+    hmap = _lib.KfModelMap.from_buffer_copy(dmap.cpu().numpy().tobytes())
+    k = bin(hmap.varying).count("1")
+    rec = torch.empty(lib.bke_kf_packed_models_bytes(N, hmap.varying) // 4, dtype=torch.float32, device="cuda")
 
     def pack():
-        _lib.check(lib.bke_kf_pack_sym_models(N, 4, 2, _lib.BKE_F32, Q.data_ptr(), R.data_ptr(), rec.data_ptr(),
-                                              flag.data_ptr(), s))
+        _lib.check(lib.bke_kf_scan_models(N, 4, 2, _lib.BKE_F32, *m, dmap.data_ptr(), s))
+        _lib.check(lib.bke_kf_pack_models(N, 4, 2, _lib.BKE_F32, *m, hmap.varying, rec.data_ptr(), s))
     for _ in range(3):
         pack()
     torch.cuda.synchronize()
@@ -72,9 +85,61 @@ def pack_cost(rounds):
         torch.cuda.synchronize()
         ms.append(e0.elapsed_time(e1) / reps)
     med = float(np.median(ms))
-    moved = N * (80 + 52)
-    return {"what": "pack", "n_filters": N, "symmetric": int(flag.item()) == 0, "ms": med, "ms_rounds": ms,
-            "bytes": moved, "GBps": moved / (med * 1e-3) / 1e9}
+    moved = N * (2 * 176 + 4 * k)
+    return {"what": "pack", "n_filters": N, "varying_words": k, "symmetric": hmap.asymmetric == 0, "ms": med,
+            "ms_rounds": ms, "bytes": moved, "GBps": moved / (med * 1e-3) / 1e9}
+
+
+def all_words(rounds):
+    """One step of a bank whose 37 model words all vary: the packed words (bke_kf_step_packed, k = 37)
+    against the packed Q / R (bke_kf_step_sym); both move 316 B per filter."""
+    import ctypes
+    import torch
+    from filterpy_b200 import _lib
+    from filterpy_b200.common import workloads as wl
+    lib = _lib.load()
+    w = wl.kf_bank_cv2d(N, seed=1234, steps=1, dtype=np.float32)
+    rng = np.random.default_rng(5)
+    for k, n in (("F", (4, 4)), ("H", (2, 4)), ("Q", (4, 4)), ("R", (2, 2))):
+        a = w[k] + np.float32(1e-3) * rng.standard_normal((N,) + n).astype(np.float32)
+        if k in "QR":
+            a = np.triu(a) + np.swapaxes(np.triu(a, 1), 1, 2)
+        w[k] = np.ascontiguousarray(a)
+    d = _dev(w)
+    m = [d[k].data_ptr() for k in "FQHR"]
+    s = torch.cuda.current_stream().cuda_stream
+    dmap = torch.empty(ctypes.sizeof(_lib.KfModelMap), dtype=torch.uint8, device="cuda")
+    _lib.check(lib.bke_kf_scan_models(N, 4, 2, _lib.BKE_F32, *m, dmap.data_ptr(), s))
+    hmap = _lib.KfModelMap.from_buffer_copy(dmap.cpu().numpy().tobytes())
+    assert bin(hmap.varying).count("1") == 37 and hmap.asymmetric == 0
+    rec = torch.empty(lib.bke_kf_packed_models_bytes(N, hmap.varying) // 4, dtype=torch.float32, device="cuda")
+    _lib.check(lib.bke_kf_pack_models(N, 4, 2, _lib.BKE_F32, *m, hmap.varying, rec.data_ptr(), s))
+    srec = torch.empty(lib.bke_kf_sym_models_bytes(N) // 4, dtype=torch.float32, device="cuda")
+    flag = torch.empty(1, dtype=torch.int32, device="cuda")
+    _lib.check(lib.bke_kf_pack_sym_models(N, 4, 2, _lib.BKE_F32, m[1], m[3], srec.data_ptr(), flag.data_ptr(), s))
+    x = torch.from_numpy(w["x"]).cuda(); P = torch.from_numpy(w["P"]).cuda(); z = torch.from_numpy(w["zs"][0]).cuda()
+    a = _lib.KfArgs()
+    a.n_filters, a.dim_x, a.dim_z, a.dtype, a.flags, a.alpha_sq = N, 4, 2, _lib.BKE_F32, 3, 1.0
+    a.x = a.x_out = x.data_ptr(); a.P = a.P_out = P.data_ptr()
+    a.F, a.F_stride, a.Q, a.Q_stride = m[0], 16, m[1], 16
+    a.H, a.H_stride, a.R, a.R_stride = m[2], 8, m[3], 4
+    a.z = z.data_ptr()
+    calls = {"packed_words": lambda: lib.bke_kf_step_packed(a, rec.data_ptr(), hmap, s),
+             "packed_QR": lambda: lib.bke_kf_step_sym(a, srec.data_ptr(), s)}
+    reps, ms = 100, {k: [] for k in calls}
+    for r in range(2 * rounds):
+        for name in (list(calls) if r % 2 == 0 else list(calls)[::-1]):
+            for _ in range(10):
+                _lib.check(calls[name]())
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(reps):
+                calls[name]()
+            e1.record()
+            torch.cuda.synchronize()
+            ms[name].append(e0.elapsed_time(e1) / reps)
+    return {"what": "all_words", "n_filters": N, "bytes_per_filter": 316,
+            **{k: {"median_ms": float(np.median(v)), "ms_rounds": v} for k, v in ms.items()}}
 
 
 def bench(cwd, env_extra, argv):
@@ -108,7 +173,10 @@ def main():
         if out_f:
             out_f.write(line + "\n"); out_f.flush()
     emit(dict(what="card", **card()))
-    emit(pack_cost(args.rounds))
+    pack = pack_cost(args.rounds)
+    emit(pack)
+    torch.cuda.empty_cache()
+    emit(all_words(args.rounds))
     torch.cuda.empty_cache()
     arms = [("dense", ROOT, {"BKE_KF_SYM": "0"}), ("packed", ROOT, {})]
     if args.baseline_tree:
@@ -135,6 +203,9 @@ def main():
         dense = float(np.median(res[("dense", K)]))
         summary["%s_%d" % (name, K)] = {"median_ms": med, "min_ms": min(v), "max_ms": max(v),
                                         "gain_vs_dense": dense / med - 1.0}
+    if ("baseline", 400) in res:
+        saved = float(np.median(res[("baseline", 400)])) - float(np.median(res[("packed", 400)]))
+        summary["repay_steps"] = pack["ms"] / saved if saved > 0 else None
     for name, v in diag.items():
         summary["diag_%s" % name] = {"median_ms": float(np.median(v)), "all_ms": v}
     emit({"what": "summary", **summary})
