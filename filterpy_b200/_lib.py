@@ -30,6 +30,7 @@ EXPORTED_SYMBOLS = [
     "bke_merwe_sigma_points", "bke_unscented_transform",
     "bke_ukf_model_compile", "bke_ukf_model_log", "bke_ukf_model_registers", "bke_ukf_model_free", "bke_ukf_step_model",
     "bke_debug_ukf_model_cubin_bytes", "bke_ukf_rts_smoother_model",
+    "bke_ckf_step", "bke_ckf_model_compile", "bke_ckf_step_model", "bke_debug_ckf_model_cubin_bytes",
     "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
     "bke_residual_workspace_bytes", "bke_residual_prepare", "bke_searchsorted_bracket_sweep",
 ]
@@ -99,6 +100,28 @@ class UkfArgs(ctypes.Structure):
         ("K", c_void_p), ("y", c_void_p), ("S", c_void_p), ("SI", c_void_p),
         ("log_likelihood", c_void_p),
         ("status", c_void_p),
+    ]
+
+
+class CkfArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_filters", c_int64),
+        ("dim_x", c_int32), ("dim_z", c_int32),
+        ("dtype", c_int32), ("flags", c_uint32),
+        ("fx_model", c_int32), ("hx_model", c_int32),
+        ("dt", c_double),
+        ("x", c_void_p), ("P", c_void_p),
+        ("x_out", c_void_p), ("P_out", c_void_p),
+        ("Q", c_void_p), ("Q_stride", c_int64),
+        ("R", c_void_p), ("R_stride", c_int64),
+        ("F", c_void_p), ("F_stride", c_int64),
+        ("H", c_void_p), ("H_stride", c_int64),
+        ("z", c_void_p), ("z_valid", c_void_p),
+        ("x_prior", c_void_p), ("P_prior", c_void_p),
+        ("K", c_void_p), ("y", c_void_p), ("S", c_void_p), ("SI", c_void_p),
+        ("log_likelihood", c_void_p),
+        ("status", c_void_p),
+        ("sigmas_f", c_void_p),
     ]
 
 
@@ -259,6 +282,15 @@ def load():
     lib.bke_ukf_rts_smoother_model.restype = ctypes.c_int
     lib.bke_debug_ukf_model_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p]
     lib.bke_debug_ukf_model_cubin_bytes.restype = c_size_t
+    lib.bke_ckf_step.argtypes = [ctypes.POINTER(CkfArgs), c_void_p]
+    lib.bke_ckf_step.restype = ctypes.c_int
+    lib.bke_ckf_model_compile.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p,
+                                          ctypes.POINTER(c_void_p)]
+    lib.bke_ckf_model_compile.restype = ctypes.c_int
+    lib.bke_ckf_step_model.argtypes = [ctypes.POINTER(CkfArgs), c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]
+    lib.bke_ckf_step_model.restype = ctypes.c_int
+    lib.bke_debug_ckf_model_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p]
+    lib.bke_debug_ckf_model_cubin_bytes.restype = c_size_t
     lib.bke_resample_workspace_bytes.argtypes = [c_int64]
     lib.bke_resample_workspace_bytes.restype = c_size_t
     lib.bke_systematic_resample.argtypes = [c_int64, c_void_p, c_double, c_void_p, c_void_p, c_size_t,

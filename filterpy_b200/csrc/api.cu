@@ -243,4 +243,20 @@ int bke_ukf_step(const bke_ukf_args *args, void *stream)
     return launch_ukf(a, (cudaStream_t)stream);
 }
 
+int bke_ckf_step(const bke_ckf_args *args, void *stream)
+{
+    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    const bke_ckf_args &a = *args;
+    int rc = validate_ckf(a);
+    if (rc) return rc;
+    if (a.hx_model == BKE_HX_RANGE_AZ_EL && !(a.dim_x == 6 && a.dim_z == 3)) { set_error("BKE_HX_RANGE_AZ_EL needs dim_x=6, dim_z=3"); return BKE_ERR_BAD_ARG; }
+    if (a.hx_model == BKE_HX_RANGE_BEARING && !(a.dim_x == 4 && a.dim_z == 2)) { set_error("BKE_HX_RANGE_BEARING needs dim_x=4, dim_z=2"); return BKE_ERR_BAD_ARG; }
+    if (a.fx_model < 0 || a.fx_model > BKE_FX_CONST_VEL || a.hx_model < 0 || a.hx_model > BKE_HX_RANGE_BEARING) {
+        set_error("unknown fx/hx model id"); return BKE_ERR_BAD_ARG;
+    }
+    if ((rc = require_device())) return rc;
+    if (a.n_filters == 0) return BKE_OK;
+    return launch_ckf(a, (cudaStream_t)stream);
+}
+
 }  // extern "C"

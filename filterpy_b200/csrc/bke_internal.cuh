@@ -50,6 +50,8 @@ int launch_kf_tc(const bke_kf_args &a, cudaStream_t s);
 int launch_kf_any(const bke_kf_args &a, cudaStream_t s);
 int launch_kf_batch(const bke_kf_batch_args &a, cudaStream_t s);
 int launch_ukf(const bke_ukf_args &a, cudaStream_t s);
+int validate_ckf(const bke_ckf_args &a);
+int launch_ckf(const bke_ckf_args &a, cudaStream_t s);
 #endif
 
 }  // namespace bke

@@ -1,4 +1,4 @@
-// ukf_rtc.cu — UKF instances around USER-SUPPLIED process / measurement functions.
+// ukf_rtc.cu — UKF and CKF instances around USER-SUPPLIED process / measurement functions.
 //
 // The reference takes fx(x, dt, **args) and hx(x, **args) as Python callables (filterpy/kalman/UKF.py:
 // 284-288, called at :521-522 and :463-464).  A device cannot call back into Python, so the drop-in
@@ -6,6 +6,8 @@
 // kernel the pre-built instances use (ukf_kernel.cuh, model ids BKE_FX_USER / BKE_HX_USER), compiles it
 // for sm_90a with NVRTC (libnvrtc is dlopen'ed: libbke.so does not link it), loads the cubin with
 // cudaLibraryLoadData and launches the resulting cudaKernel_t like any other kernel.  No CPU path.
+// bke_ckf_model_compile does the same around the cubature kernel (ckf_kernel.cuh, CubatureKalmanFilter.py:
+// 314-321, 354-363); the handle records its family and each step entry point refuses the other's.
 //
 // Program text handed to NVRTC (the user's part between the markers):
 //     typedef double real;                       // or float
@@ -20,10 +22,15 @@
 #include <string.h>
 #include <string>
 #include <vector>
+#include "ckf_launch.cuh"
 #include "ukf_launch.cuh"
 #include "ukf_rts_launch.cuh"
 
+// the filter family a compiled model's kernels belong to
+enum { BKE_FAMILY_UKF = 0, BKE_FAMILY_CKF = 1 };
+
 struct bke_ukf_model {
+    int family;
     int n, m, dtype, fx_model, hx_model;
     cudaLibrary_t lib;
     cudaKernel_t kern[2];          // [0] plain, [1] with the optional outputs
@@ -79,8 +86,8 @@ Nvrtc *nvrtc()
 std::string kernel_name(const bke_ukf_model &m, int occ, bool extras)
 {
     char buf[256];
-    snprintf(buf, sizeof buf, "bke::ukfk::ukf_kernel<real, %d, %d, %d, %d, %d, %s>", m.n, m.m, m.fx_model, m.hx_model, occ,
-             extras ? "true" : "false");
+    snprintf(buf, sizeof buf, "%s<real, %d, %d, %d, %d, %d, %s>", m.family == BKE_FAMILY_CKF ? "bke::ckfk::ckf_kernel" : "bke::ukfk::ukf_kernel",
+             m.n, m.m, m.fx_model, m.hx_model, occ, extras ? "true" : "false");
     return buf;
 }
 
@@ -102,6 +109,23 @@ int launch_model(const bke_ukf_args &a, const bke_ukf_model &m, const void *fx_a
     return BKE_OK;
 }
 
+template <typename T>
+int launch_ckf_model(const bke_ckf_args &a, const bke_ukf_model &m, const void *fx_args, int64_t s_fx, const void *hx_args, int64_t s_hx,
+                     cudaStream_t s)
+{
+    ckfk::CkfP<T> p;
+    ckf_fill_params<T>(a, p);
+    p.fx_args = (const T *)fx_args; p.s_fx_args = s_fx;
+    p.hx_args = (const T *)hx_args; p.s_hx_args = s_hx;
+    const size_t smem = ckf_smem_bytes<T>(m.n, m.m, m.fx_model == BKE_FX_LINEAR, a.F_stride == 0, m.hx_model == BKE_HX_LINEAR, a.H_stride == 0);
+    const void *kern = (const void *)m.kern[ckf_has_extras(a) ? 1 : 0];
+    if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
+    const int64_t grid = (p.N + ukfk::UB - 1) / ukfk::UB;
+    void *params[] = {&p};
+    if (check_cuda(cudaLaunchKernel(kern, dim3((unsigned)grid), dim3(ukfk::UB), params, smem, s), "ckf model launch")) return BKE_ERR_CUDA;
+    return BKE_OK;
+}
+
 }  // namespace
 }  // namespace bke
 
@@ -109,17 +133,20 @@ using namespace bke;
 
 extern "C" {
 
-// NVRTC half of bke_ukf_model_compile (needs no GPU): program text -> sm_90a cubin + the lowered names
-// of the two kernel instances
-static int compile_cubin(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+// NVRTC half of bke_ukf_model_compile / bke_ckf_model_compile (needs no GPU): program text -> sm_90a cubin
+// + the lowered names of the kernel instances of the family (the step with / without the optional outputs
+// and, for a UKF around a user fx, the RTS smoother)
+static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
                          const char *include_dirs, std::vector<char> &cubin, std::string (&lowered)[3], std::string &log)
 {
-    if (dim_x < 1 || dim_x > 16 || dim_z < 1 || dim_z > dim_x + 8) { set_error("bke_ukf_model_compile: 1 <= dim_x <= 16, 1 <= dim_z"); return BKE_ERR_BAD_ARG; }
+    const bool ckf = family == BKE_FAMILY_CKF;
+    const char *fn = ckf ? "bke_ckf_model_compile" : "bke_ukf_model_compile";
+    if (dim_x < 1 || dim_x > 16 || dim_z < 1 || dim_z > dim_x + 8) { set_error("%s: 1 <= dim_x <= 16, 1 <= dim_z", fn); return BKE_ERR_BAD_ARG; }
     if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
     const bool ufx = fx_model == BKE_FX_USER, uhx = hx_model == BKE_HX_USER;
-    if (!ufx && !uhx) { set_error("bke_ukf_model_compile: neither fx nor hx is BKE_*_USER (use bke_ukf_step)"); return BKE_ERR_BAD_ARG; }
+    if (!ufx && !uhx) { set_error("%s: neither fx nor hx is BKE_*_USER (use %s)", fn, ckf ? "bke_ckf_step" : "bke_ukf_step"); return BKE_ERR_BAD_ARG; }
     if ((!ufx && fx_model != BKE_FX_LINEAR && fx_model != BKE_FX_CONST_VEL) || (!uhx && hx_model != BKE_HX_LINEAR)) {
-        set_error("bke_ukf_model_compile: the built-in partner of a user function must be BKE_FX_LINEAR / BKE_FX_CONST_VEL / BKE_HX_LINEAR");
+        set_error("%s: the built-in partner of a user function must be BKE_FX_LINEAR / BKE_FX_CONST_VEL / BKE_HX_LINEAR", fn);
         return BKE_ERR_BAD_ARG;
     }
     if (!ufx && fx_model == BKE_FX_CONST_VEL && (dim_x & 1)) { set_error("BKE_FX_CONST_VEL needs an even dim_x"); return BKE_ERR_BAD_ARG; }
@@ -130,7 +157,7 @@ static int compile_cubin(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx
     std::string text;
     text += dtype == BKE_F64 ? "typedef double real;\n" : "typedef float real;\n";
     text += "#define BKE_DIM_X " + std::to_string(dim_x) + "\n#define BKE_DIM_Z " + std::to_string(dim_z) + "\n";
-    text += "#include \"ukf_kernel.cuh\"\n#include \"ukf_rts_kernel.cuh\"\n";
+    text += ckf ? "#include \"ckf_kernel.cuh\"\n" : "#include \"ukf_kernel.cuh\"\n#include \"ukf_rts_kernel.cuh\"\n";
     text += "#line 1 \"user_model.cu\"\n";
     text += source;
     text += "\n#line 1 \"bke_glue.cu\"\nnamespace bke { namespace ukfk {\n";
@@ -138,11 +165,11 @@ static int compile_cubin(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx
     if (uhx) text += "template <> __device__ __forceinline__ void bke_user_hx<real>(const real *x, real *z, const real *args) { ::hx(x, z, args); }\n";
     text += "} }\n";
 
-    const int occ = ukf_occupancy(dim_x, dtype == BKE_F64);
+    const int occ = ckf ? ckf_occupancy(dim_x, dtype == BKE_F64) : ukf_occupancy(dim_x, dtype == BKE_F64);
     bke_ukf_model tmp;
-    tmp.n = dim_x; tmp.m = dim_z; tmp.fx_model = fx_model; tmp.hx_model = hx_model;
+    tmp.family = family; tmp.n = dim_x; tmp.m = dim_z; tmp.fx_model = fx_model; tmp.hx_model = hx_model;
     nvrtcProgram prog;
-    nvrtcResult r = rt->create(&prog, text.c_str(), "bke_ukf_user.cu", 0, nullptr, nullptr);
+    nvrtcResult r = rt->create(&prog, text.c_str(), ckf ? "bke_ckf_user.cu" : "bke_ukf_user.cu", 0, nullptr, nullptr);
     if (r != NVRTC_SUCCESS) { set_error("nvrtcCreateProgram: %s", rt->errstr(r)); return BKE_ERR_CUDA; }
     std::vector<std::string> opts = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "-default-device"};     // (bke.h declares the host C-ABI)
     {
@@ -158,7 +185,7 @@ static int compile_cubin(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx
     std::vector<const char *> copts;
     for (auto &o : opts) copts.push_back(o.c_str());
     // the step kernel with / without the optional outputs and, around a user fx, the RTS smoother
-    const bool with_rts = ufx && dim_x <= UR_MAXN;
+    const bool with_rts = !ckf && ufx && dim_x <= UR_MAXN;
     const int n_names = with_rts ? 3 : 2;
     const std::string names[3] = {kernel_name(tmp, occ, false), kernel_name(tmp, occ, true), "bke::ukf_rts_kernel<real, true>"};
     for (int i = 0; i < n_names; i++) rt->add_name(prog, names[i].c_str());
@@ -168,7 +195,7 @@ static int compile_cubin(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx
     log.clear();
     if (lsz > 1) { log.resize(lsz); rt->log(prog, &log[0]); }
     if (r != NVRTC_SUCCESS) {
-        set_error("NVRTC could not compile the UKF model: %s\n%s", rt->errstr(r), log.c_str());
+        set_error("NVRTC could not compile the %s model: %s\n%s", ckf ? "CKF" : "UKF", rt->errstr(r), log.c_str());
         rt->destroy(&prog);
         return BKE_ERR_BAD_ARG;
     }
@@ -190,17 +217,17 @@ static int compile_cubin(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx
     return BKE_OK;
 }
 
-int bke_ukf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
-                          const char *include_dirs, bke_ukf_model **out)
+static int model_compile(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+                         const char *include_dirs, bke_ukf_model **out)
 {
     if (!out) { set_error("out is NULL"); return BKE_ERR_BAD_ARG; }
     *out = nullptr;
     std::vector<char> cubin;
     std::string lowered[3], log;
-    int rc = compile_cubin(dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, cubin, lowered, log);
+    int rc = compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, cubin, lowered, log);
     if (rc != BKE_OK) return rc;
     bke_ukf_model *m = new bke_ukf_model();
-    m->n = dim_x; m->m = dim_z; m->dtype = dtype; m->fx_model = fx_model; m->hx_model = hx_model; m->lib = nullptr; m->log = log;
+    m->family = family; m->n = dim_x; m->m = dim_z; m->dtype = dtype; m->fx_model = fx_model; m->hx_model = hx_model; m->lib = nullptr; m->log = log;
     m->kern_rts = nullptr;
     if (check_cuda(cudaLibraryLoadData(&m->lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0), "cudaLibraryLoadData")) { delete m; return BKE_ERR_CUDA; }
     for (int i = 0; i < 2; i++) {
@@ -220,14 +247,38 @@ int bke_ukf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t f
     return BKE_OK;
 }
 
+int bke_ukf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+                          const char *include_dirs, bke_ukf_model **out)
+{
+    return model_compile(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, out);
+}
+
+int bke_ckf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+                          const char *include_dirs, bke_ukf_model **out)
+{
+    return model_compile(BKE_FAMILY_CKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, out);
+}
+
 // the NVRTC half alone (CPU-only check that a model's text compiles for sm_90a): cubin size or 0
-size_t bke_debug_ukf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
-                                       const char *include_dirs)
+static size_t cubin_bytes(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+                          const char *include_dirs)
 {
     std::vector<char> cubin;
     std::string lowered[3], log;
-    if (compile_cubin(dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, cubin, lowered, log) != BKE_OK) return 0;
+    if (compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, cubin, lowered, log) != BKE_OK) return 0;
     return cubin.size();
+}
+
+size_t bke_debug_ukf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+                                       const char *include_dirs)
+{
+    return cubin_bytes(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs);
+}
+
+size_t bke_debug_ckf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+                                       const char *include_dirs)
+{
+    return cubin_bytes(BKE_FAMILY_CKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs);
 }
 
 const char *bke_ukf_model_log(const bke_ukf_model *m) { return m ? m->log.c_str() : ""; }
@@ -246,6 +297,7 @@ int bke_ukf_step_model(const bke_ukf_args *args, const bke_ukf_model *model, con
 {
     if (!args || !model) { set_error("args / model is NULL"); return BKE_ERR_BAD_ARG; }
     const bke_ukf_args &a = *args;
+    if (model->family != BKE_FAMILY_UKF) { set_error("bke_ukf_step_model: the model was compiled for the CKF (bke_ckf_model_compile)"); return BKE_ERR_BAD_ARG; }
     if (a.dim_x != model->n || a.dim_z != model->m || a.dtype != model->dtype || a.fx_model != model->fx_model || a.hx_model != model->hx_model) {
         set_error("bke_ukf_step_model: args (dim_x=%d dim_z=%d dtype=%d fx=%d hx=%d) do not match the compiled model (%d %d %d %d %d)",
                   a.dim_x, a.dim_z, a.dtype, a.fx_model, a.hx_model, model->n, model->m, model->dtype, model->fx_model, model->hx_model);
@@ -272,6 +324,7 @@ int bke_ukf_rts_smoother_model(const bke_ukf_rts_args *args, const bke_ukf_model
 {
     if (!args || !model) { set_error("args / model is NULL"); return BKE_ERR_BAD_ARG; }
     const bke_ukf_rts_args &a = *args;
+    if (model->family != BKE_FAMILY_UKF) { set_error("bke_ukf_rts_smoother_model: the model was compiled for the CKF (bke_ckf_model_compile)"); return BKE_ERR_BAD_ARG; }
     if (!model->kern_rts) { set_error("bke_ukf_rts_smoother_model: the model has no user fx (use bke_ukf_rts_smoother) or dim_x > %d", UR_MAXN); return BKE_ERR_UNSUPPORTED; }
     if (a.dim_x != model->n || a.dtype != model->dtype || a.fx_model != BKE_FX_USER) { set_error("bke_ukf_rts_smoother_model: args do not match the compiled model"); return BKE_ERR_BAD_ARG; }
     if (a.n_filters < 0 || a.n_steps < 0 || fx_args_stride < 0 || a.Q_stride < 0) { set_error("negative sizes"); return BKE_ERR_BAD_ARG; }
@@ -284,6 +337,25 @@ int bke_ukf_rts_smoother_model(const bke_ukf_rts_args *args, const bke_ukf_model
     if (check_cuda(cudaLaunchKernel((const void *)model->kern_rts, dim3((unsigned)((a.n_filters + 63) / 64)), dim3(64), params, 0, (cudaStream_t)stream),
                    "ukf rts model launch")) return BKE_ERR_CUDA;
     return BKE_OK;
+}
+
+int bke_ckf_step_model(const bke_ckf_args *args, const bke_ukf_model *model, const void *fx_args, int64_t fx_args_stride,
+                       const void *hx_args, int64_t hx_args_stride, void *stream)
+{
+    if (!args || !model) { set_error("args / model is NULL"); return BKE_ERR_BAD_ARG; }
+    const bke_ckf_args &a = *args;
+    if (model->family != BKE_FAMILY_CKF) { set_error("bke_ckf_step_model: the model was compiled for the UKF (bke_ukf_model_compile)"); return BKE_ERR_BAD_ARG; }
+    if (a.dim_x != model->n || a.dim_z != model->m || a.dtype != model->dtype || a.fx_model != model->fx_model || a.hx_model != model->hx_model) {
+        set_error("bke_ckf_step_model: args (dim_x=%d dim_z=%d dtype=%d fx=%d hx=%d) do not match the compiled model (%d %d %d %d %d)",
+                  a.dim_x, a.dim_z, a.dtype, a.fx_model, a.hx_model, model->n, model->m, model->dtype, model->fx_model, model->hx_model);
+        return BKE_ERR_BAD_ARG;
+    }
+    int rc = validate_ckf(a);
+    if (rc) return rc;
+    if (fx_args_stride < 0 || hx_args_stride < 0) { set_error("negative args stride"); return BKE_ERR_BAD_ARG; }
+    if (a.n_filters == 0) return BKE_OK;
+    return a.dtype == BKE_F32 ? launch_ckf_model<float>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream)
+                              : launch_ckf_model<double>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -121,15 +121,16 @@ class DeviceHx(_DeviceModel):
 _compiled_models = {}
 
 
-def _compile_model(lib, dim_x, dim_z, dtype_id, fx, hx):
-    """One NVRTC build per (shape, dtype, source); shared by every filter object that uses it."""
+def _compile_model(lib, dim_x, dim_z, dtype_id, fx, hx, entry="bke_ukf_model_compile"):
+    """One NVRTC build per (filter family, shape, dtype, source); shared by every filter object that uses it.
+    ``entry`` names the family's compile call (bke_ukf_model_compile / bke_ckf_model_compile)."""
     src = "\n".join(m.source for m in (fx, hx) if isinstance(m, _DeviceModel))
-    key = (dim_x, dim_z, dtype_id, fx.model, hx.model, src)
+    key = (entry, dim_x, dim_z, dtype_id, fx.model, hx.model, src)
     h = _compiled_models.get(key)
     if h is None:
         out = ctypes.c_void_p()
-        _lib.check(lib.bke_ukf_model_compile(dim_x, dim_z, dtype_id, fx.model, hx.model, src.encode(),
-                                             _lib.kernel_include_dirs().encode(), ctypes.byref(out)))
+        _lib.check(getattr(lib, entry)(dim_x, dim_z, dtype_id, fx.model, hx.model, src.encode(),
+                                       _lib.kernel_include_dirs().encode(), ctypes.byref(out)))
         h = _compiled_models[key] = out
     return h
 
@@ -141,31 +142,21 @@ def _no_hook(name, v):
             "has no CPU fallback (see filterpy_b200/kalman/UKF.py)" % name)
 
 
-class UnscentedKalmanFilter(object):
-    def __init__(self, dim_x, dim_z, dt, hx, fx, points, sqrt_fn=None, x_mean_fn=None, z_mean_fn=None,
-                 residual_x=None, residual_z=None, state_add=None,
-                 n_filters=None, dtype=np.float64, device=None, diagnostics=True):
-        for nm, v in (("sqrt_fn", sqrt_fn), ("x_mean_fn", x_mean_fn), ("z_mean_fn", z_mean_fn),
-                      ("residual_x", residual_x), ("residual_z", residual_z), ("state_add", state_add)):
-            _no_hook(nm, v)
-        if not hasattr(fx, "model") or not hasattr(hx, "model"):
-            raise NotImplementedError(
-                "fx / hx must be device-side models (LinearFx, ConstVelFx, LinearHx, RangeAzElHx, "
-                "RangeBearingHx, or DeviceFx / DeviceHx around CUDA source text): Python callables cannot "
-                "run inside the CUDA kernel and there is no CPU fallback")
-        if points.n != dim_x:
-            raise ValueError("expected size(x) {}, but size is {}".format(points.n, dim_x))   # sigma_points.py:153
+class _SigmaPointBank(object):
+    """What the UKF and CKF mirrors share: the bank's state, models and diagnostics, their NumPy views in
+    single-filter mode, and the deferred predict (``_pending`` / ``_flush``)."""
+    _compile_model = staticmethod(_compile_model)
+
+    def _init_bank(self, dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics):
+        """The state, models, compiled user model and diagnostic buffers of a bank (the reference's
+        __init__ defaults: x = 0, P = I, Q = I, R = I)."""
         self._dim_x, self._dim_z = int(dim_x), int(dim_z)
         self._single = n_filters is None
         self.n_filters = 1 if self._single else int(n_filters)
         self._dtype = resolve_dtype(dtype)
         self._device = require_cuda(device)
         self._lib = _lib.load()
-        self.points_fn = points
-        self._dt = dt
-        self._num_sigmas = points.num_sigmas()
         self.fx, self.hx = fx, hx
-        self.Wm, self.Wc = points.Wm, points.Wc
         self.diagnostics = bool(diagnostics)
         N, n, m = self.n_filters, self._dim_x, self._dim_z
         kw = dict(dtype=self._dtype, device=self._device)
@@ -181,7 +172,7 @@ class UnscentedKalmanFilter(object):
         self._fx_args = self._hx_args = (None, 0)
         if isinstance(fx, _DeviceModel) or isinstance(hx, _DeviceModel):
             with torch.cuda.device(self._device):
-                self._user_model = _compile_model(self._lib, n, m, bke_dtype(self._dtype), fx, hx)
+                self._user_model = self._compile_model(self._lib, n, m, bke_dtype(self._dtype), fx, hx)
             if isinstance(fx, _DeviceModel):
                 self._fx_args = fx.pack({}, N, self._dtype, self._device) if all(k in fx.values for k in fx.arg_names) else (None, 0)
             if isinstance(hx, _DeviceModel):
@@ -307,6 +298,27 @@ class UnscentedKalmanFilter(object):
         if bad:
             raise np.linalg.LinAlgError("%d of %d filters: matrix not positive definite / singular"
                                         % (bad, self.n_filters))
+
+
+class UnscentedKalmanFilter(_SigmaPointBank):
+    def __init__(self, dim_x, dim_z, dt, hx, fx, points, sqrt_fn=None, x_mean_fn=None, z_mean_fn=None,
+                 residual_x=None, residual_z=None, state_add=None,
+                 n_filters=None, dtype=np.float64, device=None, diagnostics=True):
+        for nm, v in (("sqrt_fn", sqrt_fn), ("x_mean_fn", x_mean_fn), ("z_mean_fn", z_mean_fn),
+                      ("residual_x", residual_x), ("residual_z", residual_z), ("state_add", state_add)):
+            _no_hook(nm, v)
+        if not hasattr(fx, "model") or not hasattr(hx, "model"):
+            raise NotImplementedError(
+                "fx / hx must be device-side models (LinearFx, ConstVelFx, LinearHx, RangeAzElHx, "
+                "RangeBearingHx, or DeviceFx / DeviceHx around CUDA source text): Python callables cannot "
+                "run inside the CUDA kernel and there is no CPU fallback")
+        if points.n != dim_x:
+            raise ValueError("expected size(x) {}, but size is {}".format(points.n, dim_x))   # sigma_points.py:153
+        self._init_bank(dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics)
+        self.points_fn = points
+        self._dt = dt
+        self._num_sigmas = points.num_sigmas()
+        self.Wm, self.Wc = points.Wm, points.Wc
 
     # ------------------------------------------------------------------ predict / update
     def predict(self, dt=None, UT=None, fx=None, **fx_args):

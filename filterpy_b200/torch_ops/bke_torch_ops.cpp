@@ -4,6 +4,7 @@
 //   bke::kf_step              bke_kf_step              KalmanFilter.predict + update, kalman_filter.py:437-561
 //   bke::kf_predict           bke_kf_step (predict)    kalman_filter.py:437-482
 //   bke::ukf_step             bke_ukf_step             UnscentedKalmanFilter.predict + update, UKF.py:364-491
+//   bke::ckf_step             bke_ckf_step             CubatureKalmanFilter.predict + update, CubatureKalmanFilter.py:292-389
 //   bke::systematic_resample  bke_systematic_resample  monte_carlo/resampling.py:117-150
 //   bke::stratified_resample  bke_stratified_resample  monte_carlo/resampling.py:80-114
 #include <ATen/ATen.h>
@@ -104,6 +105,30 @@ std::tuple<at::Tensor, at::Tensor> ukf_step(const at::Tensor &x, const at::Tenso
     return std::make_tuple(x_out, P_out);
 }
 
+std::tuple<at::Tensor, at::Tensor> ckf_step(const at::Tensor &x, const at::Tensor &P, const at::Tensor &Q, const at::Tensor &R,
+                                            const at::Tensor &z, double dt, int64_t fx_model, int64_t hx_model,
+                                            const c10::optional<at::Tensor> &F, const c10::optional<at::Tensor> &H)
+{
+    TORCH_CHECK(x.is_cuda() && P.is_cuda() && x.is_contiguous() && P.is_contiguous() && x.dim() == 2 && P.dim() == 3, "bke: x is [N, n], P is [N, n, n] on the GPU");
+    c10::cuda::CUDAGuard guard(x.device());
+    const int64_t N = x.size(0), n = x.size(1), m = z.size(1);
+    bke_ckf_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_filters = N; a.dim_x = (int32_t)n; a.dim_z = (int32_t)m; a.dtype = dtype_of(x);
+    a.flags = BKE_DO_PREDICT | BKE_DO_UPDATE; a.fx_model = (int32_t)fx_model; a.hx_model = (int32_t)hx_model;
+    a.dt = dt;
+    at::Tensor x_out = at::empty_like(x), P_out = at::empty_like(P);
+    a.x = x.data_ptr(); a.P = P.data_ptr(); a.x_out = x_out.data_ptr(); a.P_out = P_out.data_ptr();
+    a.Q = model(Q, N, n, n, &a.Q_stride, x, "Q");
+    a.R = model(R, N, m, m, &a.R_stride, x, "R");
+    if (F.has_value()) a.F = model(*F, N, n, n, &a.F_stride, x, "F");
+    if (H.has_value()) a.H = model(*H, N, m, n, &a.H_stride, x, "H");
+    TORCH_CHECK(z.is_cuda() && z.is_contiguous() && z.scalar_type() == x.scalar_type() && z.dim() == 2 && z.size(0) == N, "bke: z is [N, m]");
+    a.z = z.data_ptr();
+    check_rc(bke_ckf_step(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_ckf_step");
+    return std::make_tuple(x_out, P_out);
+}
+
 at::Tensor resample(const at::Tensor &w, double u, const c10::optional<at::Tensor> &U)
 {
     TORCH_CHECK(w.is_cuda() && w.is_contiguous() && w.scalar_type() == at::kDouble && w.dim() == 1, "bke: weights must be a contiguous 1-D float64 CUDA tensor");
@@ -142,6 +167,8 @@ TORCH_LIBRARY(bke, m)
     m.def("kf_predict(Tensor x, Tensor P, Tensor F, Tensor Q, float alpha_sq=1.0) -> (Tensor, Tensor)");
     m.def("ukf_step(Tensor x, Tensor P, Tensor Q, Tensor R, Tensor z, float dt, float alpha, float beta, float kappa, "
           "int fx_model, int hx_model, Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor)");
+    m.def("ckf_step(Tensor x, Tensor P, Tensor Q, Tensor R, Tensor z, float dt, int fx_model, int hx_model, "
+          "Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor)");
     m.def("systematic_resample(Tensor weights, float u) -> Tensor");
     m.def("stratified_resample(Tensor weights, Tensor uniforms) -> Tensor");
 }
@@ -151,6 +178,7 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("kf_step", &kf_step);
     m.impl("kf_predict", &kf_predict);
     m.impl("ukf_step", &ukf_step);
+    m.impl("ckf_step", &ckf_step);
     m.impl("systematic_resample", &systematic_resample);
     m.impl("stratified_resample", &stratified_resample);
 }

@@ -260,6 +260,59 @@ int bke_ukf_step_model(const bke_ukf_args *args, const bke_ukf_model *model, con
 size_t bke_debug_ukf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
                                        const char *source, const char *include_dirs);
 
+/* ------------------------------------------------------------------------------------------
+ * Cubature Kalman filter bank.
+ * Replaces CubatureKalmanFilter.predict / update (filterpy/kalman/CubatureKalmanFilter.py:292-327,
+ * 329-389; spherical_radial_sigmas :52-61, ckf_transform :87-98) for N filters at once, with the fx / hx
+ * models of the UKF above (the closed set, or user source through bke_ckf_model_compile below).
+ * Per filter, m = 2n points, no centre point:
+ *   U = cholesky(P) * sqrt(n) (upper);  points x + U[k,:], x - U[k,:];  f_k = fx(point_k)   (:56-59, :320-321)
+ *   x- = sum f_k / m;  P- = sum (f_k - x-)(f_k - x-)' / m + Q                              [x_prior, P_prior]
+ *   Z_k = hx(f_k) (the propagated points, not redrawn, :362-363);  z^ = sum Z_k / m;
+ *   S = sum (Z_k - z^)(..)' / m + R;  Pxz = sum (f_k - x)(Z_k - z^)' / m  (:366-373);
+ *   K = Pxz S^-1;  y = z - z^;  x <- x + K y;  P <- P - K S K'                               (:375-379)
+ * The covariances are formed centred; the reference's ckf_transform forms them as raw second moments
+ * (sum f f' - m x x'), the same mathematics with more cancellation.
+ * sigmas_f[N,2n,n] (may be NULL) holds the propagated points, the reference's self.sigmas_f: a call with
+ * BKE_DO_PREDICT writes them when it is non-NULL, an update-only call reads them (and needs it non-NULL:
+ * the reference's update without predict reuses the points of the last predict).  z_valid, the optional
+ * outputs and status[N] behave as in bke_ukf_args. */
+typedef struct bke_ckf_args {
+    int64_t n_filters;
+    int32_t dim_x, dim_z;
+    int32_t dtype;
+    uint32_t flags;                  /* BKE_DO_PREDICT | BKE_DO_UPDATE */
+    int32_t fx_model, hx_model;
+    double dt;
+    const void *x, *P;
+    void *x_out, *P_out;
+    const void *Q; int64_t Q_stride;
+    const void *R; int64_t R_stride;
+    const void *F; int64_t F_stride; /* BKE_FX_LINEAR only */
+    const void *H; int64_t H_stride; /* BKE_HX_LINEAR only */
+    const void *z;
+    const uint8_t *z_valid;
+    void *x_prior, *P_prior;
+    void *K, *y, *S, *SI, *log_likelihood;
+    int32_t *status;
+    void *sigmas_f;                  /* [N,2n,n] or NULL */
+} bke_ckf_args;
+
+int bke_ckf_step(const bke_ckf_args *args, void *stream);
+
+/* User-supplied fx / hx for the CKF: the reference calls fx(x, dt, *fx_args) and hx(x, *hx_args)
+ * (CubatureKalmanFilter.py:314-321, :354-363).  Source text, include_dirs and the args vectors follow
+ * bke_ukf_model_compile / bke_ukf_step_model; the positional arguments are args[0..] in order.  The handle
+ * is a bke_ukf_model built for the CKF kernel (bke_ukf_model_log / _registers / _free apply to it);
+ * bke_ckf_step_model refuses a UKF handle and bke_ukf_step_model a CKF handle (BKE_ERR_BAD_ARG). */
+int bke_ckf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+                          const char *include_dirs, bke_ukf_model **out);
+int bke_ckf_step_model(const bke_ckf_args *args, const bke_ukf_model *model, const void *fx_args, int64_t fx_args_stride,
+                       const void *hx_args, int64_t hx_args_stride, void *stream);
+/* the NVRTC half alone (needs no GPU): size of the sm_90a cubin, 0 on failure (log in bke_last_error()) */
+size_t bke_debug_ckf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
+                                       const char *source, const char *include_dirs);
+
 /* Stand-alone pieces of the unscented path for callers that use them directly:
  *   MerweScaledSigmaPoints.sigma_points(x, P)   filterpy/kalman/sigma_points.py:124-177
  *       x[N,n], P[N,n,n] -> sigmas[N,2n+1,n]; status[N] = BKE_STATUS_NOT_PD where scipy's cholesky
