@@ -31,6 +31,7 @@ EXPORTED_SYMBOLS = [
     "bke_ukf_model_compile", "bke_ukf_model_log", "bke_ukf_model_registers", "bke_ukf_model_free", "bke_ukf_step_model",
     "bke_debug_ukf_model_cubin_bytes", "bke_ukf_rts_smoother_model",
     "bke_ckf_step", "bke_ckf_model_compile", "bke_ckf_step_model", "bke_debug_ckf_model_cubin_bytes",
+    "bke_srkf_step", "bke_cholesky_lower",
     "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
     "bke_residual_workspace_bytes", "bke_residual_prepare", "bke_searchsorted_bracket_sweep",
 ]
@@ -123,6 +124,30 @@ class CkfArgs(ctypes.Structure):
         ("status", c_void_p),
         ("sigmas_f", c_void_p),
     ]
+
+
+class SrkfArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_filters", c_int64),
+        ("dim_x", c_int32), ("dim_z", c_int32), ("dim_u", c_int32),
+        ("dtype", c_int32),
+        ("flags", c_uint32), ("reserved", c_uint32),
+        ("x", c_void_p), ("L", c_void_p),
+        ("x_out", c_void_p), ("L_out", c_void_p),
+        ("F", c_void_p), ("F_stride", c_int64),
+        ("H", c_void_p), ("H_stride", c_int64),
+        ("Lq", c_void_p), ("Lq_stride", c_int64),
+        ("Lr", c_void_p), ("Lr_stride", c_int64),
+        ("B", c_void_p), ("B_stride", c_int64),
+        ("u", c_void_p), ("u_stride", c_int64),
+        ("z", c_void_p), ("z_valid", c_void_p),
+        ("x_prior", c_void_p), ("L_prior", c_void_p),
+        ("K", c_void_p), ("y", c_void_p), ("S1_2", c_void_p), ("SI1_2", c_void_p),
+        ("status", c_void_p),
+    ]
+
+
+BKE_CHOLESKY_MAX_DIM = 16
 
 
 class ResampleShardArgs(ctypes.Structure):
@@ -291,6 +316,10 @@ def load():
     lib.bke_ckf_step_model.restype = ctypes.c_int
     lib.bke_debug_ckf_model_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p]
     lib.bke_debug_ckf_model_cubin_bytes.restype = c_size_t
+    lib.bke_srkf_step.argtypes = [ctypes.POINTER(SrkfArgs), c_void_p]
+    lib.bke_srkf_step.restype = ctypes.c_int
+    lib.bke_cholesky_lower.argtypes = [c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
+    lib.bke_cholesky_lower.restype = ctypes.c_int
     lib.bke_resample_workspace_bytes.argtypes = [c_int64]
     lib.bke_resample_workspace_bytes.restype = c_size_t
     lib.bke_systematic_resample.argtypes = [c_int64, c_void_p, c_double, c_void_p, c_void_p, c_size_t,

@@ -76,6 +76,33 @@ static int validate_kf(const bke_kf_args *a, bool need_z)
     return BKE_OK;
 }
 
+static int validate_srkf(const bke_srkf_args *a)
+{
+    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    if (a->n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    if (a->dim_x < 1) { set_error("dim_x must be 1 or greater"); return BKE_ERR_BAD_ARG; }   // square_root.py:128-133
+    if (a->dim_z < 1) { set_error("dim_z must be 1 or greater"); return BKE_ERR_BAD_ARG; }
+    if (a->dim_u < 0) { set_error("dim_u must be 0 or greater"); return BKE_ERR_BAD_ARG; }
+    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (!(a->flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
+    if (a->flags & ~(BKE_DO_PREDICT | BKE_DO_UPDATE)) { set_error("flags may only hold BKE_DO_PREDICT and BKE_DO_UPDATE"); return BKE_ERR_BAD_ARG; }
+    if (!a->x || !a->L || !a->x_out || !a->L_out) { set_error("x, L, x_out, L_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if ((a->flags & BKE_DO_PREDICT) && (!a->F || !a->Lq)) { set_error("predict needs F and Lq"); return BKE_ERR_BAD_ARG; }   // :240-243
+    if ((a->flags & BKE_DO_UPDATE) && (!a->H || !a->Lr || !a->z)) { set_error("update needs H, Lr and z"); return BKE_ERR_BAD_ARG; }   // :204-215
+    if ((a->B != nullptr || a->u != nullptr) && (!a->B || !a->u || a->dim_u < 1)) {
+        set_error("a control input needs B, u and dim_u >= 1");                                       // :240
+        return BKE_ERR_BAD_ARG;
+    }
+    const int64_t n = a->dim_x, m = a->dim_z, du = a->dim_u;
+    auto bad_stride = [](int64_t s, int64_t full) { return s != 0 && s != full; };
+    if (bad_stride(a->F_stride, n * n) || bad_stride(a->Lq_stride, n * n) || bad_stride(a->H_stride, m * n) ||
+        bad_stride(a->Lr_stride, m * m) || bad_stride(a->B_stride, n * du) || bad_stride(a->u_stride, du)) {
+        set_error("model strides must be 0 (shared) or the dense per-filter size");
+        return BKE_ERR_BAD_ARG;
+    }
+    return BKE_OK;
+}
+
 }  // namespace bke
 
 using namespace bke;
@@ -257,6 +284,33 @@ int bke_ckf_step(const bke_ckf_args *args, void *stream)
     if ((rc = require_device())) return rc;
     if (a.n_filters == 0) return BKE_OK;
     return launch_ckf(a, (cudaStream_t)stream);
+}
+
+int bke_srkf_step(const bke_srkf_args *args, void *stream)
+{
+    int rc = validate_srkf(args);
+    if (rc) return rc;
+    if ((rc = require_device())) return rc;
+    if (args->n_filters == 0) return BKE_OK;
+    return launch_srkf(*args, (cudaStream_t)stream);
+}
+
+int bke_cholesky_lower(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *L,
+                       int32_t *status, void *stream)
+{
+    if (n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    if (k < 1) { set_error("k must be 1 or greater"); return BKE_ERR_BAD_ARG; }
+    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (stride != 0 && stride != (int64_t)k * k) { set_error("stride must be 0 (shared) or k*k"); return BKE_ERR_BAD_ARG; }
+    if (n_filters > 0 && (!A || !L)) { set_error("A and L must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if (k > BKE_CHOLESKY_MAX_DIM) {
+        set_error("bke_cholesky_lower: k=%d is above BKE_CHOLESKY_MAX_DIM=%d", k, BKE_CHOLESKY_MAX_DIM);
+        return BKE_ERR_UNSUPPORTED;
+    }
+    int rc = require_device();
+    if (rc) return rc;
+    if (n_filters == 0) return BKE_OK;
+    return launch_cholesky_lower(n_filters, k, dtype, A, stride, L, status, (cudaStream_t)stream);
 }
 
 }  // extern "C"

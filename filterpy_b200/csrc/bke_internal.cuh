@@ -52,6 +52,9 @@ int launch_kf_batch(const bke_kf_batch_args &a, cudaStream_t s);
 int launch_ukf(const bke_ukf_args &a, cudaStream_t s);
 int validate_ckf(const bke_ckf_args &a);
 int launch_ckf(const bke_ckf_args &a, cudaStream_t s);
+int launch_srkf(const bke_srkf_args &a, cudaStream_t s);
+int launch_cholesky_lower(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *L,
+                          int32_t *status, cudaStream_t s);
 #endif
 
 }  // namespace bke

@@ -9,9 +9,9 @@
 // Shared (stride 0) models are read through the same pointers (all threads hit one line).
 // Optional outputs, z_valid and the three predict/update modes are supported; a control input
 // (B, u) and update-first go to the catch-all kernel.
-#include <type_traits>
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
+#include "kf_rowio.cuh"
 
 namespace bke {
 namespace {
@@ -27,48 +27,6 @@ struct DirP {
     T *x_out, *P_out, *x_prior, *P_prior, *K, *y, *S, *SI, *ll;
     int32_t *status;
 };
-
-template <typename T, int CNT>
-__device__ __forceinline__ void ldv(T *dst, const T *src)
-{
-    constexpr int VEC = 16 / sizeof(T);
-    if constexpr (CNT % VEC == 0) {
-        using V = typename std::conditional<sizeof(T) == 4, float4, double2>::type;
-#pragma unroll
-        for (int i = 0; i < CNT / VEC; i++) *reinterpret_cast<V *>(dst + i * VEC) = __ldg(reinterpret_cast<const V *>(src) + i);
-    } else {
-#pragma unroll
-        for (int i = 0; i < CNT; i++) dst[i] = __ldg(src + i);
-    }
-}
-// plain (coherent) loads: for x and P, which alias x_out / P_out in the in-place call — ld.global.nc
-// requires memory that nobody writes during the kernel
-template <typename T, int CNT>
-__device__ __forceinline__ void ldv_rw(T *dst, const T *src)
-{
-    constexpr int VEC = 16 / sizeof(T);
-    if constexpr (CNT % VEC == 0) {
-        using V = typename std::conditional<sizeof(T) == 4, float4, double2>::type;
-#pragma unroll
-        for (int i = 0; i < CNT / VEC; i++) *reinterpret_cast<V *>(dst + i * VEC) = reinterpret_cast<const V *>(src)[i];
-    } else {
-#pragma unroll
-        for (int i = 0; i < CNT; i++) dst[i] = src[i];
-    }
-}
-template <typename T, int CNT>
-__device__ __forceinline__ void stv(T *dst, const T *src)
-{
-    constexpr int VEC = 16 / sizeof(T);
-    if constexpr (CNT % VEC == 0) {
-        using V = typename std::conditional<sizeof(T) == 4, float4, double2>::type;
-#pragma unroll
-        for (int i = 0; i < CNT / VEC; i++) reinterpret_cast<V *>(dst)[i] = *reinterpret_cast<const V *>(src + i * VEC);
-    } else {
-#pragma unroll
-        for (int i = 0; i < CNT; i++) dst[i] = src[i];
-    }
-}
 
 // EX: the optional outputs are compiled in (a separate instantiation keeps their tests and live
 // ranges out of the plain kernel)
@@ -124,16 +82,6 @@ __global__ void __launch_bounds__(128) kf_direct_kernel(DirP<T> p)
     stv<T, N>(p.x_out + f * N, x);
     stv<T, N * N>(p.P_out + f * N * N, &P[0][0]);
     if (p.status && (st != BKE_STATUS_OK || !(p.flags & BKE_STATUS_STICKY))) p.status[f] = st;
-}
-
-// 16-byte vector accesses are used for the arrays whose row is a multiple of 16 bytes: their base
-// pointers and per-filter strides must be 16-byte aligned (otherwise the catch-all kernel runs)
-template <typename T, int CNT>
-bool vec_ok(const void *p, int64_t stride_elems = CNT)
-{
-    constexpr int VEC = 16 / sizeof(T);
-    if (CNT % VEC != 0 || p == nullptr) return true;
-    return (reinterpret_cast<uintptr_t>(p) & 15u) == 0 && (stride_elems * (int64_t)sizeof(T)) % 16 == 0;
 }
 
 template <typename T, int N, int M>

@@ -12,6 +12,7 @@
 //                       P = (I-KH) P (I-KH)' + K R K'      (Joseph form)
 //   z is None:515-520   posterior := prior
 #include "bke_internal.cuh"
+#include "kf_warp.cuh"
 
 namespace bke {
 namespace {
@@ -31,24 +32,6 @@ struct KfP {
     int32_t *status;
     int sticky;                       // BKE_STATUS_STICKY: write status only on failure
 };
-
-// C[r,c] = A[r,k] * B (B is [k,c], or [c,k] when TB), result handed to epi(e, i, j, value)
-template <bool TB, typename T, typename Epi>
-__device__ __forceinline__ void warp_mm(const T *A, const T *B, int r, int k, int c, int lane, Epi epi)
-{
-    for (int e = lane; e < r * c; e += 32) {
-        int i = e / c, j = e - i * c;
-        T s = T(0);
-        for (int q = 0; q < k; q++) s += A[i * k + q] * (TB ? B[j * k + q] : B[q * c + j]);
-        epi(e, i, j, s);
-    }
-}
-
-template <typename T>
-__device__ __forceinline__ void warp_copy_in(T *dst, const T *src, int cnt, int lane)
-{
-    for (int e = lane; e < cnt; e += 32) dst[e] = src[e];
-}
 
 // Gauss-Jordan inverse with partial pivoting of the m x m matrix A (destroyed) into Ai.
 // Returns false when a pivot is exactly zero (np.linalg.inv raises LinAlgError).

@@ -8,6 +8,7 @@ The same symbols exposed as torch.ops.* via a C++ extension for zero-copy CUDA t
     x, P = torch.ops.bke.kf_predict(x, P, F, Q)                    # :437-482
     x, P = torch.ops.bke.ukf_step(x, P, Q, R, z, dt, alpha, beta, kappa, fx_model, hx_model)   # UKF.py:364-491
     x, P = torch.ops.bke.ckf_step(x, P, Q, R, z, dt, fx_model, hx_model)   # CubatureKalmanFilter.py:292-389
+    x, L = torch.ops.bke.srkf_step(x, L, F, H, Lq, Lr, z)          # square_root.py:172-248 (L = P1_2)
     idx  = torch.ops.bke.systematic_resample(weights, u)           # resampling.py:117-150 (int32, bit-exact)
     idx  = torch.ops.bke.stratified_resample(weights, uniforms)    # resampling.py:80-114
 

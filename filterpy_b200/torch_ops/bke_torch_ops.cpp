@@ -5,6 +5,7 @@
 //   bke::kf_predict           bke_kf_step (predict)    kalman_filter.py:437-482
 //   bke::ukf_step             bke_ukf_step             UnscentedKalmanFilter.predict + update, UKF.py:364-491
 //   bke::ckf_step             bke_ckf_step             CubatureKalmanFilter.predict + update, CubatureKalmanFilter.py:292-389
+//   bke::srkf_step            bke_srkf_step            SquareRootKalmanFilter.predict + update, square_root.py:172-248
 //   bke::systematic_resample  bke_systematic_resample  monte_carlo/resampling.py:117-150
 //   bke::stratified_resample  bke_stratified_resample  monte_carlo/resampling.py:80-114
 #include <ATen/ATen.h>
@@ -129,6 +130,30 @@ std::tuple<at::Tensor, at::Tensor> ckf_step(const at::Tensor &x, const at::Tenso
     return std::make_tuple(x_out, P_out);
 }
 
+std::tuple<at::Tensor, at::Tensor> srkf_step(const at::Tensor &x, const at::Tensor &L, const at::Tensor &F, const at::Tensor &H,
+                                             const at::Tensor &Lq, const at::Tensor &Lr, const at::Tensor &z)
+{
+    TORCH_CHECK(x.is_cuda() && L.is_cuda() && x.is_contiguous() && L.is_contiguous(), "bke: x and L must be contiguous CUDA tensors");
+    TORCH_CHECK(x.dim() == 2 && L.dim() == 3 && L.size(0) == x.size(0) && L.size(1) == x.size(1) && L.size(2) == x.size(1), "bke: x is [N, n], L is [N, n, n]");
+    TORCH_CHECK(L.scalar_type() == x.scalar_type(), "bke: x and L must share a dtype");
+    c10::cuda::CUDAGuard guard(x.device());
+    const int64_t N = x.size(0), n = x.size(1), m = H.size(-2);
+    bke_srkf_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_filters = N; a.dim_x = (int32_t)n; a.dim_z = (int32_t)m; a.dtype = dtype_of(x);
+    a.flags = BKE_DO_PREDICT | BKE_DO_UPDATE;
+    at::Tensor x_out = at::empty_like(x), L_out = at::empty_like(L);
+    a.x = x.data_ptr(); a.L = L.data_ptr(); a.x_out = x_out.data_ptr(); a.L_out = L_out.data_ptr();
+    a.F = model(F, N, n, n, &a.F_stride, x, "F");
+    a.H = model(H, N, m, n, &a.H_stride, x, "H");
+    a.Lq = model(Lq, N, n, n, &a.Lq_stride, x, "Lq");
+    a.Lr = model(Lr, N, m, m, &a.Lr_stride, x, "Lr");
+    TORCH_CHECK(z.is_cuda() && z.is_contiguous() && z.scalar_type() == x.scalar_type() && z.dim() == 2 && z.size(0) == N && z.size(1) == m, "bke: z is [N, m]");
+    a.z = z.data_ptr();
+    check_rc(bke_srkf_step(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_srkf_step");
+    return std::make_tuple(x_out, L_out);
+}
+
 at::Tensor resample(const at::Tensor &w, double u, const c10::optional<at::Tensor> &U)
 {
     TORCH_CHECK(w.is_cuda() && w.is_contiguous() && w.scalar_type() == at::kDouble && w.dim() == 1, "bke: weights must be a contiguous 1-D float64 CUDA tensor");
@@ -169,6 +194,7 @@ TORCH_LIBRARY(bke, m)
           "int fx_model, int hx_model, Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor)");
     m.def("ckf_step(Tensor x, Tensor P, Tensor Q, Tensor R, Tensor z, float dt, int fx_model, int hx_model, "
           "Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor)");
+    m.def("srkf_step(Tensor x, Tensor L, Tensor F, Tensor H, Tensor Lq, Tensor Lr, Tensor z) -> (Tensor, Tensor)");
     m.def("systematic_resample(Tensor weights, float u) -> Tensor");
     m.def("stratified_resample(Tensor weights, Tensor uniforms) -> Tensor");
 }
@@ -179,6 +205,7 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("kf_predict", &kf_predict);
     m.impl("ukf_step", &ukf_step);
     m.impl("ckf_step", &ckf_step);
+    m.impl("srkf_step", &srkf_step);
     m.impl("systematic_resample", &systematic_resample);
     m.impl("stratified_resample", &stratified_resample);
 }

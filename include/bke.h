@@ -313,6 +313,59 @@ int bke_ckf_step_model(const bke_ckf_args *args, const bke_ukf_model *model, con
 size_t bke_debug_ckf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
                                        const char *source, const char *include_dirs);
 
+/* ------------------------------------------------------------------------------------------
+ * Square-root Kalman filter bank.
+ * Replaces SquareRootKalmanFilter.predict / update (filterpy/kalman/square_root.py:226-248, 172-224) for N
+ * filters at once.  The state is x[N,n] and the lower-triangular factor L[N,n,n] of P = L L' (P1_2), stored
+ * dense with explicit zeros above the diagonal; Lq[N,n,n] and Lr[N,m,m] are the factors of Q and R (Q1_2,
+ * R1_2).  Per filter, in this order (flags = BKE_DO_PREDICT | BKE_DO_UPDATE):
+ *   x <- F x (+ B u);  R~ = qr([F L | Lq]')[1] (2n x n);  L <- R~[:n,:n]'                   [x_prior, L_prior]
+ *   M = [[Lr', 0], [(H L)', L']];  r = qr(M)[1];  S1_2 = r[:m,:m]';  SI1_2 = S1_2^-1;
+ *   K = r[:m,m:]' SI1_2;  y = z - H x;  x <- x + K y;  L <- r[m:,m:]'
+ * The QR is LAPACK's dgeqr2 (what scipy.linalg.qr runs at these sizes), with its signs: a column whose
+ * sub-column is exactly zero is left as it is (tau = 0), otherwise its diagonal becomes
+ * -copysign(norm, alpha).  So L itself, not only L L', is the reference's.  Lr is read as the full matrix
+ * (update(z, R2) passes any square root); L and Lq as well.
+ * Deviation: the reference inverts S1_2 with pinv.  Here a zero diagonal entry of S1_2 sets status[f] =
+ * BKE_STATUS_SINGULAR_S, K = 0, SI1_2 = 0, and the posterior is the prior.  For S1_2 = 0 (e.g. H = 0 with
+ * Lr = 0) that is the reference's result; for a partially singular S1_2 pinv would give a non-zero gain.
+ * z_valid[i] == 0 means "z is None" for filter i (:189-193): x and L are not changed and the optional update
+ * outputs of that filter are not written.  Optional outputs (NULL = not wanted): x_prior, L_prior (written by
+ * a predict), K[N,n,m], y[N,m], S1_2[N,m,m], SI1_2[N,m,m], status[N].  x_out / L_out may alias x / L.
+ * Kernels (picked by shape, DESIGN.md §3.5c): a register tile per thread for 1/1, 2/2, 3/1, 4/1 and 4/2
+ * without control input, a warp per filter for every other shape. */
+typedef struct bke_srkf_args {
+    int64_t n_filters;
+    int32_t dim_x, dim_z, dim_u;     /* dim_u may be 0 */
+    int32_t dtype;
+    uint32_t flags;                  /* BKE_DO_PREDICT | BKE_DO_UPDATE */
+    uint32_t reserved;
+    const void *x, *L;               /* in  */
+    void *x_out, *L_out;             /* out */
+    const void *F; int64_t F_stride;
+    const void *H; int64_t H_stride;
+    const void *Lq; int64_t Lq_stride;
+    const void *Lr; int64_t Lr_stride;
+    const void *B; int64_t B_stride; /* [N,n,dim_u] or NULL */
+    const void *u; int64_t u_stride; /* [N,dim_u]   or NULL */
+    const void *z;                   /* [N,m]; may be NULL when BKE_DO_UPDATE is not set */
+    const uint8_t *z_valid;          /* [N] or NULL */
+    void *x_prior, *L_prior;
+    void *K, *y, *S1_2, *SI1_2;
+    int32_t *status;
+} bke_srkf_args;
+
+int bke_srkf_step(const bke_srkf_args *args, void *stream);
+
+/* The setters' factorisation: L[N,k,k] = scipy.linalg.cholesky(A, lower=True) per filter
+ * (square_root.py:288, :314, :330).  Only the lower triangle of A is read; L is written dense with zeros
+ * above the diagonal.  A[f] is at A + f * stride (stride 0: one matrix for every filter, k*k: per filter).
+ * status[N] (may be NULL) = BKE_STATUS_NOT_PD where cholesky would raise LinAlgError.
+ * k = 1 .. BKE_CHOLESKY_MAX_DIM (BKE_ERR_UNSUPPORTED above). */
+#define BKE_CHOLESKY_MAX_DIM 16
+int bke_cholesky_lower(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *L,
+                       int32_t *status, void *stream);
+
 /* Stand-alone pieces of the unscented path for callers that use them directly:
  *   MerweScaledSigmaPoints.sigma_points(x, P)   filterpy/kalman/sigma_points.py:124-177
  *       x[N,n], P[N,n,n] -> sigmas[N,2n+1,n]; status[N] = BKE_STATUS_NOT_PD where scipy's cholesky
