@@ -2,7 +2,8 @@
 // in ukf.cu does both on chip; these entry points serve callers of
 // MerweScaledSigmaPoints.sigma_points (filterpy/kalman/sigma_points.py:124-177) and
 // unscented_transform (filterpy/kalman/unscented_transform.py:22-128) themselves).
-// One warp per filter, matrices in the warp's slice of shared memory, any n <= 32.
+// One warp per filter, matrices in the warp's slice of shared memory: sigma points for any n <= 32, the
+// transform for any k <= 256 points of n <= 64 (up to 4 warps per block, fewer when their slices do not fit).
 #include "bke_internal.cuh"
 
 namespace bke {
@@ -92,13 +93,22 @@ template <typename T>
 int ut_t(int64_t N, int ns, int n, const void *sig, const void *Wm, const void *Wc, const void *noise, int64_t nstride,
          void *x_out, void *P_out, cudaStream_t s)
 {
-    const size_t smem = 4 * sizeof(T) * (size_t)(ns * n + n);
+    // 4 warps per block, or 2 / 1 when their slices exceed the device's opt-in shared memory per block:
+    // one warp's slice (at most 8 * (256 * 64 + 64) B = 131,584 B) always fits an H100's 227 KB
+    const size_t per_warp = sizeof(T) * (size_t)(ns * n + n);
+    int dev = 0, optin = 0;
+    if (check_cuda(cudaGetDevice(&dev), "cudaGetDevice") ||
+        check_cuda(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev), "cudaDeviceGetAttribute"))
+        return BKE_ERR_CUDA;
+    int wpb = 4;
+    while (wpb > 1 && per_warp * wpb > (size_t)optin) wpb >>= 1;
+    const size_t smem = per_warp * wpb;
     if (smem > 48 * 1024) {
         if (check_cuda(cudaFuncSetAttribute(k_unscented_transform<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
     }
-    int64_t grid = (N + 3) / 4, cap = (int64_t)sm_count() * 16;
-    k_unscented_transform<T><<<(unsigned)(grid < cap ? grid : cap), 128, smem, s>>>(N, ns, n, (const T *)sig, (const T *)Wm, (const T *)Wc,
-                                                                                  (const T *)noise, nstride, (T *)x_out, (T *)P_out);
+    int64_t grid = (N + wpb - 1) / wpb, cap = (int64_t)sm_count() * 16;
+    k_unscented_transform<T><<<(unsigned)(grid < cap ? grid : cap), 32 * wpb, smem, s>>>(N, ns, n, (const T *)sig, (const T *)Wm, (const T *)Wc,
+                                                                                       (const T *)noise, nstride, (T *)x_out, (T *)P_out);
     return check_cuda(cudaGetLastError(), "k_unscented_transform launch");
 }
 

@@ -238,36 +238,3 @@ def test_sigma_points_and_unscented_transform_standalone(golden):
         pts.sigma_points(np.zeros(6), -np.eye(6))
     with pytest.raises(NotImplementedError):
         unscented_transform(sig, pts.Wm, pts.Wc, mean_fn=lambda s, w: s[0])
-
-
-@pytest.mark.parametrize("case", ["azimuth_cut", "close_range"])
-def test_ukf_range_az_el_angle_paths_vs_oracle(case):
-    """The kernel evaluates the angles of the sigma points relative to the mean point (a short
-    series for small angular offsets, the library atan2 otherwise) and wraps into (-pi, pi].
-    Both paths and the wrap against the oracle's plain np.arctan2: targets straddling the +-pi
-    azimuth cut, and targets so close that the sigma points span wide angles."""
-    from filterpy_b200.kalman import UnscentedKalmanFilter, MerweScaledSigmaPoints, ConstVelFx, RangeAzElHx
-    from filterpy_b200.common import workloads as wl
-    from oracle import ukf as oukf
-    N = 3000
-    w = wl.ukf_bank_cv3d(N, seed=77, steps=1)
-    rng = np.random.default_rng(5)
-    x = w["x"].copy()
-    if case == "azimuth_cut":
-        x[:, 0] = -rng.uniform(300, 900, N); x[:, 2] = rng.uniform(-1.5, 1.5, N); x[:, 4] = rng.uniform(-50, 50, N)
-    else:
-        x[:, 0] = rng.uniform(2, 6, N) * rng.choice([-1, 1], N); x[:, 2] = rng.uniform(2, 6, N) * rng.choice([-1, 1], N)
-        x[:, 4] = rng.uniform(-4, 4, N)
-    px, py, pz = x[:, 0], x[:, 2], x[:, 4]
-    z = np.stack([np.sqrt(px * px + py * py + pz * pz), np.arctan2(py, px), np.arctan2(pz, np.sqrt(px * px + py * py))], 1)
-    z = z + rng.normal(size=z.shape) * np.array([0.5, 0.002, 0.002])
-    u = UnscentedKalmanFilter(6, 3, 0.1, RangeAzElHx(), ConstVelFx(), MerweScaledSigmaPoints(6, .5, 2., 0.),
-                              n_filters=N, dtype=np.float64)
-    u.x = x; u.P = w["P"]; u.Q = w["Q"]; u.R = w["R"]
-    u.predict(); u.update(z)
-    o = oukf.ukf_step_bank(x, w["P"], z, w["Q"], w["R"], 0.1, .5, 2., 0., oukf.FX_CONST_VEL, oukf.HX_RANGE_AZ_EL)
-    ok = np.isfinite(o["x"]).all(axis=1) & (u.status.cpu().numpy() == 0)
-    assert ok.mean() > 0.95
-    rel_close(u.x.cpu().numpy()[ok], o["x"][ok], 1e-6, "x " + case)
-    rel_close(u.P.cpu().numpy()[ok], o["P"][ok], 1e-6, "P " + case)
-    rel_close(u.S.cpu().numpy()[ok], o["S"][ok], 1e-6, "S " + case)
