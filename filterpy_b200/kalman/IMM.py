@@ -113,10 +113,12 @@ class IMMEstimator(object):
         with torch.cuda.device(self._device):
             _lib.check(fn(ctypes.byref(a), stream_ptr(self._device)))
 
-    def update(self, z):
-        """IMM.py:160-184: update every model, then mode probabilities and the combined estimate."""
+    def update(self, z, valid=None):
+        """IMM.py:160-184: update every model, then mode probabilities and the combined estimate.
+        ``z=None`` is a missed measurement for every track; ``valid`` (bool[N]) marks the tracks that
+        have one, the others behave as the reference's ``update(None)``."""
         for f in self.filters:
-            f.update(z)
+            f.update(z, valid=valid)
         a = _mm_args(self.filters)
         a.mu, a.cbar, a.omega, a.trans = ptr(self._mu), ptr(self._cbar), ptr(self._omega), ptr(self._M)
         self._call(self._lib.bke_mm_probabilities, a)

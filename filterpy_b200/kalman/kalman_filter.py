@@ -373,7 +373,10 @@ class KalmanFilter(object):
     def update(self, z, R=None, H=None, valid=None):
         """kalman_filter.py:485-561.  ``z`` is ``(N, dim_z)`` in bank mode (``valid`` — bool[N] —
         marks the filters that have a measurement; the others behave as ``z=None``); in single
-        mode anything the reference accepts.  ``z=None`` skips the update for the whole bank."""
+        mode anything the reference accepts.  ``z=None`` skips the update for the whole bank.
+
+        A filter without a measurement keeps K, S and SI, and its log-likelihood becomes the
+        reference's ``logpdf(y = 0, S)`` of the kept S (see ``_missed_log_likelihood``)."""
         pend, self._pending = self._pending, None
         if z is None:                                       # :515-520
             if pend is not None:
@@ -382,6 +385,7 @@ class KalmanFilter(object):
             if self.diagnostics:
                 self._post_alias = True
                 self._y.zero_()
+                self._ll.copy_(_missed_log_likelihood(self._S))
             return
         m = self.dim_z
         if self._single:
@@ -408,6 +412,9 @@ class KalmanFilter(object):
                 raise ValueError("valid must have shape (%d,)" % self.n_filters)
         flags = _lib.BKE_DO_UPDATE | (_lib.BKE_DO_PREDICT if pend is not None else 0)
         self._launch(flags, pend, zt, vt, R, H)
+        if vt is not None and self.diagnostics:
+            # the kernels leave log_likelihood untouched where z_valid == 0
+            self._ll.copy_(torch.where(vt.bool(), self._ll, _missed_log_likelihood(self._S)))
         self._z = zt
 
     def _call(self, a, rec=None):
@@ -706,6 +713,18 @@ class KalmanFilter(object):
     def __repr__(self):
         return "KalmanFilter bank (H100): n_filters=%d dim_x=%d dim_z=%d dtype=%s device=%s" % (
             self.n_filters, self.dim_x, self.dim_z, self._dtype, self._device)
+
+
+def _missed_log_likelihood(S):
+    """log N(0; 0, S) for each filter: what the reference's ``log_likelihood`` returns after
+    ``update(None)``, which clears the cached value and leaves y = 0 and the last S
+    (kalman_filter.py:511-520, :1203-1210).  -inf where det S <= 0: a filter that has never had a
+    measurement still has S = 0, where scipy's logpdf gives -inf (``likelihood`` then floors it at
+    float min).  Evaluated in fp64 with torch ops that do not synchronise the host, so a CUDA graph
+    can capture it."""
+    sign, logdet = torch.linalg.slogdet(S.double())
+    ll = -0.5 * (logdet + S.shape[-1] * math.log(2.0 * math.pi))
+    return torch.where(sign > 0, ll, -math.inf).to(S.dtype)
 
 
 def _rts(kf, Xs, Ps, Fs, Qs, shift, single, N, n):

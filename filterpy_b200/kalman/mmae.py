@@ -65,12 +65,13 @@ class MMAEFilterBank(object):
             f.predict(None if (np.isscalar(u) and u == 0) else u)
         self._x_prior.copy_(self._x); self._P_prior.copy_(self._P)
 
-    def update(self, z, R=None, H=None):
-        """mmae.py:155-206."""
+    def update(self, z, R=None, H=None, valid=None):
+        """mmae.py:155-206.  ``valid`` (bool[N]) marks the tracks that have a measurement; the
+        others behave as the reference's ``update(None)``."""
         if H is None:
             H = self.H
         for f in self.filters:
-            f.update(z, R, H)
+            f.update(z, R, H, valid=valid)
         a = _mm_args(self.filters, flags=_lib.BKE_MM_MMAE)
         a.mu = ptr(self._p)
         a.weights_stride = len(self.filters)

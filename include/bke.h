@@ -77,6 +77,9 @@ int bke_device_count(void);
  *   P <- (I - K H) P (I - K H)' + K R K'                                  (Joseph form, :555-556)
  * z_valid[i] == 0 means "z is None" for filter i: the update is skipped and the posterior is
  * the prior (kalman_filter.py:515-520).  z_valid == NULL means every filter has a measurement.
+ * For such a filter the step writes y = 0 and leaves K, S, SI and log_likelihood unchanged.  The
+ * reference's log-likelihood is then log N(0; 0, S) of the kept S (-inf while S is still zero);
+ * the caller computes it (KalmanFilter.update does).
  * Optional outputs (NULL = not wanted): x_prior, P_prior, K[N,n,m], y[N,m], S[N,m,m],
  * SI[N,m,m], log_likelihood[N] (log N(y; 0, S), kalman_filter.py:1203-1210), status[N].
  * x_out/P_out may alias x/P (in-place update).

@@ -153,6 +153,17 @@ def log_likelihood_bank(y, S):
     return -0.5 * (q + logdet + m * np.log(2.0 * np.pi))
 
 
+def missed_log_likelihood_bank(S):
+    """log N(0; 0, S) per filter: ``KalmanFilter.log_likelihood`` after ``update(None)``, which keeps the
+    last S and sets y = 0 (kalman_filter.py:511-520).  -inf where det S <= 0 (the S = 0 of a filter that
+    has never had a measurement: scipy's logpdf with allow_singular gives -inf there)."""
+    S = np.asarray(S, float)
+    sign, logdet = np.linalg.slogdet(S)
+    with np.errstate(invalid="ignore"):
+        ll = -0.5 * (logdet + S.shape[-1] * np.log(2.0 * np.pi))
+    return np.where(sign > 0, ll, -np.inf)
+
+
 def rts_smoother(Xs, Ps, Fs, Qs, shift=1):
     """kalman_filter.py:1056-1074 (method, step k uses Fs[k+1]: shift=1) and :1840-1858 (procedural,
     Fs[k]: shift=0), literal; Xs (T,n) or (T,n,1), Ps (T,n,n), Fs/Qs lists of length T."""

@@ -83,7 +83,8 @@ def run_kf_bank(w, steps, alpha=1.0, none_frac=0.0, seed=5, with_control=False):
             rec["x_prior"].append(kf.x_prior.copy()); rec["P_prior"].append(kf.P_prior.copy())
             rec["y"].append(np.asarray(kf.y, float).reshape(m))
             rec["K"].append(kf.K.copy()); rec["S"].append(kf.S.copy()); rec["SI"].append(kf.SI.copy())
-            rec["loglik"].append(kf.log_likelihood if z is not None else np.nan)
+            # after update(None) the reference evaluates logpdf(0, S) of the kept S (-inf while S is zero)
+            rec["loglik"].append(kf.log_likelihood)
         for k in keys:
             out[k].append(np.array(rec[k]))
     res = {"ref_" + k: np.array(v) for k, v in out.items()}
@@ -94,11 +95,25 @@ def run_kf_bank(w, steps, alpha=1.0, none_frac=0.0, seed=5, with_control=False):
     return res
 
 
+def save_same_inputs(name, changed, **arrs):
+    """``save``, after asserting that every array except those named in ``changed`` equals the committed
+    file's bit for bit: regenerating a golden must not move what it already pins."""
+    path = os.path.join(HERE, name + ".npz")
+    if os.path.exists(path):
+        old = np.load(path, allow_pickle=False)
+        assert set(old.files) == set(arrs) | {"reference_version"}, (name, sorted(set(old.files) ^ set(arrs)))
+        for k, v in arrs.items():
+            if k not in changed:
+                assert np.array_equal(old[k], np.asarray(v)), (name, k)
+    save(name, **arrs)
+
+
 def gen_kf_banks():
+    # ref_loglik holds the reference's log_likelihood at every epoch, a missed one included
     w = wl.kf_bank_cv2d(48, seed=1234, steps=5)
-    save("kf_bank_4_2", **w, **run_kf_bank(w, 5, none_frac=0.15))
+    save_same_inputs("kf_bank_4_2", ["ref_loglik"], **w, **run_kf_bank(w, 5, none_frac=0.15))
     w = wl.kf_bank_ca3d(24, seed=4321, steps=3)
-    save("kf_bank_9_3", **w, **run_kf_bank(w, 3, alpha=1.02))
+    save_same_inputs("kf_bank_9_3", ["ref_loglik"], **w, **run_kf_bank(w, 3, alpha=1.02))
     # odd little shapes: random well-conditioned dense models
     rng = np.random.default_rng(99)
     for (n, m) in [(1, 1), (2, 1), (3, 2), (6, 3), (5, 5)]:
@@ -111,7 +126,7 @@ def gen_kf_banks():
                  Q=0.01 * np.eye(n) + np.zeros((N, n, n)),
                  R=np.eye(m) * rng.uniform(0.2, 1.0, (N, 1, 1)),
                  zs=rng.standard_normal((steps, N, m)))
-        save("kf_bank_%d_%d" % (n, m), **w, **run_kf_bank(w, steps, with_control=(n == 3)))
+        save_same_inputs("kf_bank_%d_%d" % (n, m), ["ref_loglik"], **w, **run_kf_bank(w, steps, with_control=(n == 3)))
 
 
 # ----------------------------------------------------------------------------- UKF
@@ -453,6 +468,98 @@ def gen_mm():
     save("mm", **out)
 
 
+# (name, number of models, dim_x, dim_z): 4/2, 2/1 and 6/3 have row-parallel mixing kernels, 3/1 has not; M is
+# below, equal to and above dim_x for the MMAE zip.  "man" is one track that manoeuvres and then misses.
+MM_MISSING_CASES = [("a", 2, 4, 2), ("b", 3, 4, 2), ("c", 4, 4, 2), ("d", 2, 2, 1), ("e", 4, 2, 1),
+                    ("f", 3, 6, 3), ("g", 2, 3, 1), ("h", 4, 3, 1), ("man", 2, 4, 2)]
+
+
+def mm_missing_models(nm, n, m, n_tracks, seed, qs):
+    """nm models per track that differ in process noise: constant velocity on n/2 axes (H picks the
+    positions) for even n, constant acceleration on one axis for n = 3."""
+    rng = np.random.default_rng(seed)
+    dt = 1.0
+    if n % 2 == 0:
+        F = np.kron(np.eye(m), np.array([[1.0, dt], [0.0, 1.0]]))
+        H = np.kron(np.eye(m), np.array([[1.0, 0.0]]))
+        Q1 = np.kron(np.eye(m), np.array([[dt ** 3 / 3, dt ** 2 / 2], [dt ** 2 / 2, dt]]))
+    else:
+        F = np.array([[1.0, dt, dt * dt / 2], [0.0, 1.0, dt], [0.0, 0.0, 1.0]])
+        H = np.array([[1.0, 0.0, 0.0]])
+        Q1 = np.array([[dt ** 5 / 20, dt ** 4 / 8, dt ** 3 / 6], [dt ** 4 / 8, dt ** 3 / 3, dt ** 2 / 2],
+                       [dt ** 3 / 6, dt ** 2 / 2, dt]])
+    R = np.eye(m) * 0.5
+    x0 = rng.normal(size=(n_tracks, n)) * 3
+    P0 = np.array([np.diag(rng.uniform(1, 5, n)) for _ in range(n_tracks)])
+    return dict(F=F, H=H, R=R, Qs=np.array([Q1 * q for q in qs[:nm]]), x0=x0, P0=P0)
+
+
+def gen_mm_missing():
+    """IMMEstimator and MMAEFilterBank with missed measurements (update(None)): ~20 % of the tracks miss at
+    random epochs, every track misses at epoch 3, track 0 misses at epoch 0 (its filters' S is still zero),
+    and in case "man" one track takes four on-track measurements, a manoeuvre to z = (12, -6), then a miss."""
+    from filterpy.kalman import IMMEstimator, MMAEFilterBank
+    out = {}
+    T = 8
+    for ci, (name, nm, n, m) in enumerate(MM_MISSING_CASES):
+        rng = np.random.default_rng(500 + ci)
+        if name == "man":
+            NT, T_ = 1, 6
+            mdl = mm_missing_models(nm, n, m, NT, 600, [0.05, 8.0])
+            mdl["x0"][:] = 0.0; mdl["P0"][:] = np.eye(n)
+            zs = np.zeros((T_, NT, m))
+            zs[4, 0] = (12.0, -6.0)
+            valid = np.ones((T_, NT), bool); valid[5] = False
+            trans = np.array([[0.97, 0.03], [0.03, 0.97]])
+            mu0 = np.array([0.5, 0.5])
+        else:
+            NT, T_ = 9, T
+            mdl = mm_missing_models(nm, n, m, NT, 600 + ci, [0.05, 1.0, 8.0, 0.3])
+            zs = rng.normal(size=(T_, NT, m)) * 2 + np.cumsum(rng.normal(size=(T_, NT, m)), axis=0)
+            valid = rng.random((T_, NT)) >= 0.2
+            valid[3] = False
+            valid[0, 0] = False
+            trans = np.full((nm, nm), 0.1 / (nm - 1)) + np.eye(nm) * (0.9 - 0.1 / (nm - 1))
+            mu0 = np.arange(nm, 0, -1.0) / np.sum(np.arange(nm, 0, -1.0))
+        shp = dict(x=(n,), P=(n, n), xp=(n,), Pp=(n, n), mu=(nm,), cbar=(nm,), omega=(nm, nm),
+                   fx=(nm, n), fP=(nm, n, n), lik=(nm,))
+        rec = {k: np.zeros((T_, NT) + s) for k, s in shp.items()}
+        mrec = {k: np.zeros((T_, NT) + shp[k]) for k in ("x", "P", "fx", "fP", "lik")}
+        mrec["p"] = np.zeros((T_, NT, nm))
+        for t_ in range(NT):
+            def mk():
+                fs = []
+                for j in range(nm):
+                    f = KalmanFilter(n, m)
+                    f.x = mdl["x0"][t_].copy() + j; f.P = mdl["P0"][t_].copy()
+                    f.F, f.H, f.R, f.Q = mdl["F"], mdl["H"], mdl["R"], mdl["Qs"][j]
+                    fs.append(f)
+                return fs
+            imm = IMMEstimator(mk(), mu0, trans)
+            bank = MMAEFilterBank(mk(), list(mu0), dim_x=n)
+            for k in range(T_):
+                z = zs[k, t_] if valid[k, t_] else None
+                imm.predict()
+                rec["xp"][k, t_] = imm.x; rec["Pp"][k, t_] = imm.P
+                imm.update(z)
+                rec["x"][k, t_] = imm.x; rec["P"][k, t_] = imm.P; rec["mu"][k, t_] = imm.mu
+                rec["cbar"][k, t_] = imm.cbar; rec["omega"][k, t_] = imm.omega; rec["lik"][k, t_] = imm.likelihood
+                for j, f in enumerate(imm.filters):
+                    rec["fx"][k, t_, j] = f.x; rec["fP"][k, t_, j] = f.P
+                bank.predict()
+                bank.update(z)
+                mrec["x"][k, t_] = bank.x; mrec["P"][k, t_] = bank.P; mrec["p"][k, t_] = bank.p
+                for j, f in enumerate(bank.filters):
+                    mrec["fx"][k, t_, j] = f.x; mrec["fP"][k, t_, j] = f.P; mrec["lik"][k, t_, j] = f.likelihood
+        p = name + "_"
+        out.update({p + "zs": zs, p + "valid": valid, p + "trans": trans, p + "mu0": mu0, p + "F": mdl["F"],
+                    p + "H": mdl["H"], p + "R": mdl["R"], p + "Qs": mdl["Qs"], p + "x0": mdl["x0"], p + "P0": mdl["P0"]})
+        out.update({p + "imm_" + k: v for k, v in rec.items()})
+        out.update({p + "mmae_" + k: v for k, v in mrec.items()})
+    save("mm_missing", cases=np.array([c[0] for c in MM_MISSING_CASES]),
+         shapes=np.array([c[1:] for c in MM_MISSING_CASES]), **out)
+
+
 # ----------------------------------------------------------------------------- direct calls of the reference
 def gen_live():
     """What tests/test_oracle_golden.py compares the oracle with, taken from direct calls of the reference's
@@ -505,6 +612,7 @@ if __name__ == "__main__":
     gen_rts()
     gen_ukf_rts()
     gen_mm()
+    gen_mm_missing()
     gen_ukf_julier()
     gen_ukf_user()
     gen_live()

@@ -285,73 +285,125 @@ def test_rts_after_batch_filter_bank_vs_oracle():
 
 
 # ------------------------------------------------------------------ IMM / MMAE banks
-def mm_filters(g, nm, dtype, single_track=None):
+MM_MISSING = ["a", "b", "c", "d", "e", "f", "g", "h", "man"]
+
+
+def mm_case(golden, nm):
+    """One IMM / MMAE golden case: nm = 2 or 3 is mm.npz (4/2, every track measured at every epoch); a name of
+    MM_MISSING is a case of mm_missing.npz (4/2, 2/1, 6/3, 3/1 with 2..4 models and missed measurements)."""
+    if isinstance(nm, str):
+        g = golden("mm_missing")
+        return {k[len(nm) + 1:]: v for k, v in g.items() if k.startswith(nm + "_")}
+    g = golden("mm")
+    c = {k: g["m%d_%s" % (nm, k)] for k in ("zs", "trans", "mu0", "F", "H", "R", "Qs", "x0", "P0")}
+    c["valid"] = np.ones(c["zs"].shape[:2], bool)
+    for k in ("x", "P", "xp", "Pp", "mu", "fx", "fP", "init_x", "init_P", "init_omega", "init_cbar"):
+        c["imm_" + k] = g["imm%d_%s" % (nm, k)]
+    for k in ("x", "P", "p"):
+        c["mmae_" + k] = g["mmae%d_%s" % (nm, k)]
+    return c
+
+
+def mm_filters(c, dtype, single_track=None):
     from filterpy_b200.kalman import KalmanFilter
-    NT = g["m%d_x0" % nm].shape[0]
+    nm, n, m = c["Qs"].shape[0], c["F"].shape[0], c["H"].shape[0]
+    NT = c["x0"].shape[0]
     fs = []
     for j in range(nm):
         if single_track is None:
-            f = KalmanFilter(4, 2, n_filters=NT, dtype=dtype)
-            f.x = g["m%d_x0" % nm] + j; f.P = g["m%d_P0" % nm]
+            f = KalmanFilter(n, m, n_filters=NT, dtype=dtype)
+            f.x = c["x0"] + j; f.P = c["P0"]
         else:
-            f = KalmanFilter(4, 2, dtype=dtype)
-            f.x = g["m%d_x0" % nm][single_track] + j; f.P = g["m%d_P0" % nm][single_track]
-        f.F, f.H, f.R, f.Q = g["m%d_F" % nm], g["m%d_H" % nm], g["m%d_R" % nm], g["m%d_Qs" % nm][j]
+            f = KalmanFilter(n, m, dtype=dtype)
+            f.x = c["x0"][single_track] + j; f.P = c["P0"][single_track]
+        f.F, f.H, f.R, f.Q = c["F"], c["H"], c["R"], c["Qs"][j]
         fs.append(f)
     return fs
 
 
-@pytest.mark.parametrize("nm", [2, 3])
+def mm_update(est, c, k):
+    """Epoch k's measurements: update(z), update(None) when every track misses, else update(z, valid=...)."""
+    import torch
+    v = c["valid"][k]
+    z = torch.from_numpy(c["zs"][k])
+    if v.all():
+        est.update(z)
+    elif not v.any():
+        est.update(None)
+    else:
+        est.update(z, valid=torch.from_numpy(v))
+
+
+@pytest.mark.parametrize("nm", [2, 3] + MM_MISSING)
 @pytest.mark.parametrize("dtype,tol", [(np.float64, 1e-6), (np.float32, 2e-3)])
 def test_imm_bank_golden(golden, nm, dtype, tol):
-    import torch
     from filterpy_b200.kalman import IMMEstimator
-    g = golden("mm")
-    zs = g["m%d_zs" % nm]
-    T = zs.shape[0] if dtype == np.float64 else 8          # fp32 drifts with the recursion length
-    imm = IMMEstimator(mm_filters(g, nm, dtype), g["m%d_mu0" % nm], g["m%d_trans" % nm])
-    rel_close(imm.x[0].cpu().numpy(), g["imm%d_init_x" % nm], tol)
-    rel_close(imm.P[0].cpu().numpy(), g["imm%d_init_P" % nm], tol)
-    rel_close(imm.omega[0].cpu().numpy(), g["imm%d_init_omega" % nm], 1e-12)
-    rel_close(imm.cbar[0].cpu().numpy(), g["imm%d_init_cbar" % nm], 1e-12)
+    c = mm_case(golden, nm)
+    zs = c["zs"]
+    T = zs.shape[0] if dtype == np.float64 else min(8, zs.shape[0])      # fp32 drifts with the recursion length
+    imm = IMMEstimator(mm_filters(c, dtype), c["mu0"], c["trans"])
+    if "imm_init_x" in c:
+        rel_close(imm.x[0].cpu().numpy(), c["imm_init_x"], tol)
+        rel_close(imm.P[0].cpu().numpy(), c["imm_init_P"], tol)
+        rel_close(imm.omega[0].cpu().numpy(), c["imm_init_omega"], 1e-12)
+        rel_close(imm.cbar[0].cpu().numpy(), c["imm_init_cbar"], 1e-12)
     for k in range(T):
         imm.predict()
-        rel_close(imm.x.cpu().numpy(), g["imm%d_xp" % nm][k], tol); rel_close(imm.P.cpu().numpy(), g["imm%d_Pp" % nm][k], tol)
-        rel_close(imm.x_prior.cpu().numpy(), g["imm%d_xp" % nm][k], tol)
-        imm.update(torch.from_numpy(zs[k]))
-        rel_close(imm.x.cpu().numpy(), g["imm%d_x" % nm][k], tol); rel_close(imm.P.cpu().numpy(), g["imm%d_P" % nm][k], tol)
-        rel_close(imm.mu.cpu().numpy(), g["imm%d_mu" % nm][k], tol * 10)
+        rel_close(imm.x.cpu().numpy(), c["imm_xp"][k], tol); rel_close(imm.P.cpu().numpy(), c["imm_Pp"][k], tol)
+        rel_close(imm.x_prior.cpu().numpy(), c["imm_xp"][k], tol)
+        mm_update(imm, c, k)
+        rel_close(imm.x.cpu().numpy(), c["imm_x"][k], tol); rel_close(imm.P.cpu().numpy(), c["imm_P"][k], tol)
+        rel_close(imm.mu.cpu().numpy(), c["imm_mu"][k], tol * 10)
+        if "imm_omega" in c:
+            rel_close(imm.cbar.cpu().numpy(), c["imm_cbar"][k], tol * 10)
+            rel_close(imm.omega.cpu().numpy(), c["imm_omega"][k], tol * 10)
+            if dtype == np.float64:
+                np.testing.assert_allclose(imm.likelihood.cpu().numpy(), c["imm_lik"][k], rtol=1e-6, atol=0)
         for j, f in enumerate(imm.filters):
-            rel_close(f.x.cpu().numpy(), g["imm%d_fx" % nm][k][:, j], tol)
-            rel_close(f.P.cpu().numpy(), g["imm%d_fP" % nm][k][:, j], tol)
+            rel_close(f.x.cpu().numpy(), c["imm_fx"][k][:, j], tol)
+            rel_close(f.P.cpu().numpy(), c["imm_fP"][k][:, j], tol)
     assert abs(float(imm.mu.sum(dim=1).mean().item()) - 1.0) < 1e-12
 
 
-@pytest.mark.parametrize("nm", [2, 3])
+@pytest.mark.parametrize("nm", [2, 3] + MM_MISSING)
 def test_mmae_bank_golden(golden, nm):
-    import torch
     from filterpy_b200.kalman import MMAEFilterBank
-    g = golden("mm")
-    zs = g["m%d_zs" % nm]
-    bank = MMAEFilterBank(mm_filters(g, nm, np.float64), list(g["m%d_mu0" % nm]), dim_x=4)
+    c = mm_case(golden, nm)
+    zs = c["zs"]
+    bank = MMAEFilterBank(mm_filters(c, np.float64), list(c["mu0"]), dim_x=c["F"].shape[0])
     for k in range(zs.shape[0]):
         bank.predict()
-        bank.update(torch.from_numpy(zs[k]))
-        rel_close(bank.x.cpu().numpy(), g["mmae%d_x" % nm][k], 1e-6)
-        rel_close(bank.P.cpu().numpy(), g["mmae%d_P" % nm][k], 1e-6)
-        np.testing.assert_allclose(bank.p.cpu().numpy(), g["mmae%d_p" % nm][k], rtol=1e-5, atol=1e-300)
+        mm_update(bank, c, k)
+        rel_close(bank.x.cpu().numpy(), c["mmae_x"][k], 1e-6)
+        rel_close(bank.P.cpu().numpy(), c["mmae_P"][k], 1e-6)
+        np.testing.assert_allclose(bank.p.cpu().numpy(), c["mmae_p"][k], rtol=1e-5, atol=1e-300)
+        if "mmae_fx" in c:
+            for j, f in enumerate(bank.filters):
+                rel_close(f.x.cpu().numpy(), c["mmae_fx"][k][:, j], 1e-6)
+                rel_close(f.P.cpu().numpy(), c["mmae_fP"][k][:, j], 1e-6)
+                np.testing.assert_allclose(f.likelihood.cpu().numpy(), c["mmae_lik"][k][:, j], rtol=1e-6, atol=0)
 
 
 def test_imm_single_track_drop_in_and_errors(golden):
     from filterpy_b200.kalman import IMMEstimator, KalmanFilter, MMAEFilterBank
-    g = golden("mm")
-    zs = g["m2_zs"]
-    imm = IMMEstimator(mm_filters(g, 2, np.float64, single_track=3), g["m2_mu0"], g["m2_trans"])
+    c = mm_case(golden, 2)
+    zs = c["zs"]
+    imm = IMMEstimator(mm_filters(c, np.float64, single_track=3), c["mu0"], c["trans"])
     for k in range(6):
         imm.predict(); imm.update(zs[k, 3])
         assert imm.x.shape == (4,) and imm.P.shape == (4, 4) and imm.mu.shape == (2,)
-        rel_close(imm.x, g["imm2_x"][k, 3], 1e-6); rel_close(imm.P, g["imm2_P"][k, 3], 1e-6)
-        rel_close(imm.mu, g["imm2_mu"][k, 3], 1e-5)
+        rel_close(imm.x, c["imm_x"][k, 3], 1e-6); rel_close(imm.P, c["imm_P"][k, 3], 1e-6)
+        rel_close(imm.mu, c["imm_mu"][k, 3], 1e-5)
+    # a manoeuvre to z = (12, -6), then update(None): the reference re-evaluates each model's likelihood as
+    # logpdf(0, S) of the kept S, and the mode probabilities move back towards the low-noise model
+    c = mm_case(golden, "man")
+    imm = IMMEstimator(mm_filters(c, np.float64, single_track=0), c["mu0"], c["trans"])
+    for k in range(c["zs"].shape[0]):
+        imm.predict(); imm.update(c["zs"][k, 0] if c["valid"][k, 0] else None)
+        rel_close(imm.x, c["imm_x"][k, 0], 1e-6); rel_close(imm.P, c["imm_P"][k, 0], 1e-6)
+        rel_close(imm.mu, c["imm_mu"][k, 0], 1e-5)
+        np.testing.assert_allclose(imm.likelihood, c["imm_lik"][k, 0], rtol=1e-6, atol=0)
+    assert not c["valid"][-1, 0] and imm.mu[0] > 0.1
     with pytest.raises(ValueError):
         IMMEstimator([KalmanFilter(4, 2)], [1.0], np.eye(1))
     with pytest.raises(ValueError):
@@ -399,11 +451,11 @@ def test_imm_cuda_graph_of_three_steps_equals_direct_steps(golden):
     replay expects them."""
     import torch
     from filterpy_b200.kalman import IMMEstimator
-    g = golden("mm")
-    z = torch.from_numpy(g["m3_zs"][0]).cuda()
+    c = mm_case(golden, 3)
+    z = torch.from_numpy(c["zs"][0]).cuda()
 
     def make():
-        return IMMEstimator(mm_filters(g, 3, np.float64), g["m3_mu0"], g["m3_trans"])
+        return IMMEstimator(mm_filters(c, np.float64), c["mu0"], c["trans"])
     a, b = make(), make()
 
     def step(imm):
@@ -416,3 +468,30 @@ def test_imm_cuda_graph_of_three_steps_equals_direct_steps(golden):
     assert torch.equal(a.x, b.x) and torch.equal(a.P, b.P) and torch.equal(a.mu, b.mu)
     for fa, fb in zip(a.filters, b.filters):
         assert torch.equal(fa.x, fb.x) and torch.equal(fa.x_post, fb.x_post)
+
+
+def test_imm_cuda_graph_with_missed_measurements_equals_direct_steps(golden):
+    """A captured IMM step list with update(None) and update(z, valid=mask): the log-likelihood of a missed
+    measurement is computed on the device without a host synchronisation, so it replays like the rest."""
+    import torch
+    from filterpy_b200.kalman import IMMEstimator
+    c = mm_case(golden, "b")
+    z = torch.from_numpy(c["zs"][1]).cuda()
+    valid = torch.from_numpy(c["valid"][1]).cuda()
+
+    def make():
+        return IMMEstimator(mm_filters(c, np.float64), c["mu0"], c["trans"])
+    a, b = make(), make()
+
+    def steps(imm):
+        imm.predict(); imm.update(z)
+        imm.predict(); imm.update(None)
+        imm.predict(); imm.update(z, valid=valid)
+    graph = b.capture(lambda: steps(b), warmup=2)
+    graph.replay(); graph.replay()
+    for _ in range(4):
+        steps(a)
+    torch.cuda.synchronize()
+    assert torch.equal(a.x, b.x) and torch.equal(a.P, b.P) and torch.equal(a.mu, b.mu)
+    for fa, fb in zip(a.filters, b.filters):
+        assert torch.equal(fa.x, fb.x) and torch.equal(fa.log_likelihood, fb.log_likelihood)

@@ -34,6 +34,7 @@ def test_kf_bank_vs_reference(golden, name):
     g = golden(name)
     x, P = g["x"], g["P"]
     alpha_sq = float(g["alpha"]) ** 2
+    S_kept = np.zeros(g["R"].shape)                  # the reference's S before any update
     for t in range(g["zs"].shape[0]):
         if "B" in g:
             xp, Pp = okf.kf_predict_bank(x, P, g["F"], g["Q"], alpha_sq, g["B"], g["us"][t])
@@ -48,8 +49,12 @@ def test_kf_bank_vs_reference(golden, name):
         for k in ["K", "S", "SI"]:
             close(o[k][v], g["ref_" + k][t][v])
         close(o["y"], g["ref_y"][t])
-        ll = okf.log_likelihood_bank(o["y"], o["S"])
-        close(ll[v], g["ref_loglik"][t][v], rtol=1e-9, atol=1e-9)
+        # a missed measurement keeps S and evaluates logpdf(0, S) of it (-inf while S is still zero)
+        S_kept = np.where(v[:, None, None], o["S"], S_kept)
+        ll = np.where(v, okf.log_likelihood_bank(o["y"], o["S"]), okf.missed_log_likelihood_bank(S_kept))
+        assert np.array_equal(np.isneginf(ll), np.isneginf(g["ref_loglik"][t]))
+        fin = np.isfinite(g["ref_loglik"][t])
+        close(ll[fin], g["ref_loglik"][t][fin], rtol=1e-9, atol=1e-9)
 
 
 def test_kf_c_port_matches(golden):
@@ -311,6 +316,90 @@ def test_imm_and_mmae_oracle_vs_reference_vectors(golden, nm):
             bank.predict(); bank.update(zs[k, t_])
             close(bank.x, g["mmae%d_x" % nm][k, t_]); close(bank.P, g["mmae%d_P" % nm][k, t_])
             close(bank.p, g["mmae%d_p" % nm][k, t_], rtol=1e-8, atol=1e-300)
+
+
+def mm_missing_filters(g, c, t_):
+    nm = g[c + "_Qs"].shape[0]
+    return [dict(x=g[c + "_x0"][t_].copy() + j, P=g[c + "_P0"][t_].copy(), F=g[c + "_F"], H=g[c + "_H"],
+                 R=g[c + "_R"], Q=g[c + "_Qs"][j]) for j in range(nm)]
+
+
+MM_MISSING = ["a", "b", "c", "d", "e", "f", "g", "h", "man"]
+
+
+@pytest.mark.parametrize("c", MM_MISSING)
+def test_imm_and_mmae_oracle_with_missed_measurements(golden, c):
+    """The per-track oracle classes against the reference's IMMEstimator / MMAEFilterBank with update(None)
+    (tests/golden/mm_missing.npz), and the bank forms of oracle.imm — the arithmetic of each csrc/mix.cu
+    launch — against the classes, track by track."""
+    from oracle import imm as oimm
+    g = golden("mm_missing")
+    assert list(g["cases"]) == MM_MISSING
+    zs, valid, trans, mu0 = g[c + "_zs"], g[c + "_valid"], g[c + "_trans"], g[c + "_mu0"]
+    F, H, R, Qs = g[c + "_F"], g[c + "_H"], g[c + "_R"], g[c + "_Qs"]
+    T, NT, m = zs.shape
+    nm, n = Qs.shape[0], F.shape[0]
+    imms = [oimm.Imm(mm_missing_filters(g, c, t_), mu0, trans) for t_ in range(NT)]
+    banks = [oimm.Mmae(mm_missing_filters(g, c, t_), mu0) for t_ in range(NT)]
+    # bank pipeline: model j's states are xs[j] (NT, n), Ps[j]; S the kept innovation covariances
+    xs = np.array([[g[c + "_x0"][t_] + j for t_ in range(NT)] for j in range(nm)])
+    Ps = np.array([g[c + "_P0"]] * nm)
+    S = np.zeros((nm, NT, m, m))
+    mu, cbar, omega = oimm.mm_probabilities_bank(np.broadcast_to(mu0, (NT, nm)), trans=trans)
+    mxs, mPs, mS, p = xs.copy(), Ps.copy(), S.copy(), np.broadcast_to(mu0, (NT, nm)).copy()
+
+    def update(xs, Ps, S, k):
+        ll = np.zeros((NT, nm))
+        for j in range(nm):
+            o = okf.kf_update_bank(xs[j], Ps[j], zs[k], H, R, valid[k])
+            xs[j], Ps[j] = o["x"], o["P"]
+            S[j] = np.where(valid[k][:, None, None], o["S"], S[j])
+            ll[:, j] = np.where(valid[k], okf.log_likelihood_bank(o["y"], o["S"]), okf.missed_log_likelihood_bank(S[j]))
+        return ll
+
+    for k in range(T):
+        x0, P0 = oimm.mm_mix_bank(xs, Ps, omega)
+        for j in range(nm):
+            xs[j], Ps[j] = okf.kf_predict_bank(x0[j], P0[j], F, Qs[j])
+            mxs[j], mPs[j] = okf.kf_predict_bank(mxs[j], mPs[j], F, Qs[j])
+        xp, Pp = oimm.mm_estimate_bank(xs, Ps, mu)
+        ll = update(xs, Ps, S, k)
+        mu, cbar, omega = oimm.mm_probabilities_bank(mu, ll, cbar, trans)
+        x, P = oimm.mm_estimate_bank(xs, Ps, mu)
+        mll = update(mxs, mPs, mS, k)
+        p = oimm.mm_probabilities_bank(p, mll, mmae=True)
+        mx, mP = oimm.mm_estimate_bank(mxs, mPs, p, mmae=True)
+        for t_ in range(NT):
+            z = zs[k, t_] if valid[k, t_] else None
+            imm, bank = imms[t_], banks[t_]
+            imm.predict()
+            close(imm.x, g[c + "_imm_xp"][k, t_]); close(imm.P, g[c + "_imm_Pp"][k, t_])
+            close(xp[t_], imm.x, 1e-12, 1e-13); close(Pp[t_], imm.P, 1e-12, 1e-13)
+            imm.update(z)
+            close(imm.likelihood, g[c + "_imm_lik"][k, t_], rtol=1e-8, atol=0)
+            for key, want in (("x", imm.x), ("P", imm.P), ("cbar", imm.cbar), ("omega", imm.omega)):
+                close(want, g[c + "_imm_" + key][k, t_])
+            close(imm.mu, g[c + "_imm_mu"][k, t_], rtol=1e-8, atol=1e-300)
+            close(mu[t_], imm.mu, 1e-12, 1e-300); close(cbar[t_], imm.cbar, 1e-12, 1e-300)
+            close(omega[t_], imm.omega, 1e-12, 1e-300)
+            close(x[t_], imm.x, 1e-12, 1e-13); close(P[t_], imm.P, 1e-12, 1e-13)
+            for j, f in enumerate(imm.filters):
+                close(f["x"], g[c + "_imm_fx"][k, t_, j]); close(f["P"], g[c + "_imm_fP"][k, t_, j])
+                close(xs[j, t_], f["x"], 1e-12, 1e-13); close(Ps[j, t_], f["P"], 1e-12, 1e-13)
+            bank.predict(); bank.update(z)
+            close(bank.likelihood, g[c + "_mmae_lik"][k, t_], rtol=1e-8, atol=0)
+            close(bank.x, g[c + "_mmae_x"][k, t_]); close(bank.P, g[c + "_mmae_P"][k, t_])
+            close(bank.p, g[c + "_mmae_p"][k, t_], rtol=1e-8, atol=1e-300)
+            close(p[t_], bank.p, 1e-12, 1e-300)
+            close(mx[t_], bank.x, 1e-12, 1e-13); close(mP[t_], bank.P, 1e-12, 1e-13)
+            for j, f in enumerate(bank.filters):
+                close(f["x"], g[c + "_mmae_fx"][k, t_, j]); close(f["P"], g[c + "_mmae_fP"][k, t_, j])
+    # weights shared by the bank (weights_stride = 0) are the per-track forms with the weights repeated
+    for got, want in zip(oimm.mm_mix_bank(xs, Ps, omega[0]), oimm.mm_mix_bank(xs, Ps, np.broadcast_to(omega[0], omega.shape))):
+        assert np.array_equal(got, want)
+    for mmae in (False, True):
+        for got, want in zip(oimm.mm_estimate_bank(xs, Ps, mu[0], mmae), oimm.mm_estimate_bank(xs, Ps, np.broadcast_to(mu[0], mu.shape), mmae)):
+            assert np.array_equal(got, want)
 
 
 def test_ukf_rts_oracle_vs_reference_vectors(golden):
