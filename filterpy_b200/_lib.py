@@ -22,6 +22,7 @@ BKE_FX_USER = BKE_HX_USER = 100
 EXPORTED_SYMBOLS = [
     "bke_abi_version", "bke_last_error", "bke_device_count",
     "bke_kf_step", "bke_kf_batch_filter", "bke_ukf_step",
+    "bke_fls_workspace_bytes", "bke_fls_smooth",
     "bke_kf_sym_models_bytes", "bke_kf_pack_sym_models", "bke_kf_step_sym",
     "bke_kf_scan_models", "bke_kf_packed_models_bytes", "bke_kf_pack_models", "bke_kf_step_packed",
     "bke_resample_workspace_bytes", "bke_systematic_resample", "bke_stratified_resample",
@@ -79,6 +80,19 @@ class KfBatchArgs(ctypes.Structure):
         ("zs", c_void_p), ("zs_valid", c_void_p),
         ("means", c_void_p), ("covariances", c_void_p),
         ("means_p", c_void_p), ("covariances_p", c_void_p),
+    ]
+
+
+BKE_FLS_FUSED_MAX_LAG = 16
+
+
+class FlsArgs(ctypes.Structure):
+    _fields_ = [
+        ("step", KfArgs),
+        ("n_steps", c_int64), ("lag", c_int64), ("count", c_int64),
+        ("zs", c_void_p), ("us", c_void_p),
+        ("xs_smooth", c_void_p), ("xhat", c_void_p),
+        ("workspace", c_void_p), ("workspace_bytes", c_size_t),
     ]
 
 
@@ -290,6 +304,10 @@ def load():
     lib.bke_kf_step_packed.restype = ctypes.c_int
     lib.bke_kf_batch_filter.argtypes = [ctypes.POINTER(KfBatchArgs), c_void_p]
     lib.bke_kf_batch_filter.restype = ctypes.c_int
+    lib.bke_fls_workspace_bytes.argtypes = [c_int64, c_int32, c_int32, c_int32, c_int32, c_int64]
+    lib.bke_fls_workspace_bytes.restype = c_size_t
+    lib.bke_fls_smooth.argtypes = [ctypes.POINTER(FlsArgs), c_void_p]
+    lib.bke_fls_smooth.restype = ctypes.c_int
     lib.bke_ukf_step.argtypes = [ctypes.POINTER(UkfArgs), c_void_p]
     lib.bke_ukf_step.restype = ctypes.c_int
     lib.bke_ukf_model_compile.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p,

@@ -244,6 +244,31 @@ int bke_kf_batch_filter(const bke_kf_batch_args *args, void *stream)
     return launch_kf_batch(a, (cudaStream_t)stream);
 }
 
+size_t bke_fls_workspace_bytes(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dim_u, int32_t dtype, int64_t lag)
+{
+    return fls_workspace_bytes(n_filters, dim_x, dim_z, dim_u, dtype, lag);
+}
+
+int bke_fls_smooth(const bke_fls_args *args, void *stream)
+{
+    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    bke_kf_args st = args->step;
+    st.flags = BKE_DO_PREDICT | BKE_DO_UPDATE;
+    int rc = validate_kf(&st, false);
+    if (rc) return rc;
+    if (args->n_steps < 1) { set_error("n_steps must be 1 or greater"); return BKE_ERR_BAD_ARG; }
+    if (args->lag < 0) { set_error("lag < 0"); return BKE_ERR_BAD_ARG; }
+    if (args->count < 0) { set_error("count < 0"); return BKE_ERR_BAD_ARG; }
+    if (!args->zs) { set_error("zs is NULL"); return BKE_ERR_BAD_ARG; }
+    if (!args->xs_smooth) { set_error("xs_smooth (the history) is NULL"); return BKE_ERR_BAD_ARG; }
+    if (args->us && (!st.B || st.dim_u < 1)) { set_error("a control input needs us, step.B and dim_u >= 1"); return BKE_ERR_BAD_ARG; }
+    if ((rc = require_device())) return rc;
+    if (st.n_filters == 0) return BKE_OK;
+    bke_fls_args a = *args;
+    a.step = st;
+    return launch_fls(a, (cudaStream_t)stream);
+}
+
 int bke_ukf_step(const bke_ukf_args *args, void *stream)
 {
     if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }

@@ -49,6 +49,8 @@ int launch_kf_tc(const bke_kf_args &a, cudaStream_t s);
 // register tile with direct loads -> row-block -> catch-all
 int launch_kf_any(const bke_kf_args &a, cudaStream_t s);
 int launch_kf_batch(const bke_kf_batch_args &a, cudaStream_t s);
+size_t fls_workspace_bytes(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dim_u, int32_t dtype, int64_t lag);
+int launch_fls(const bke_fls_args &a, cudaStream_t s);
 int launch_ukf(const bke_ukf_args &a, cudaStream_t s);
 int validate_ckf(const bke_ckf_args &a);
 int launch_ckf(const bke_ckf_args &a, cudaStream_t s);

@@ -5,6 +5,7 @@ from .UKF import (UnscentedKalmanFilter, LinearFx, ConstVelFx, LinearHx, RangeAz
                   RangeBearingHx, DeviceFx, DeviceHx)
 from .CubatureKalmanFilter import CubatureKalmanFilter  # noqa: F401
 from .square_root import SquareRootKalmanFilter  # noqa: F401
+from .fixed_lag_smoother import FixedLagSmoother  # noqa: F401
 from .unscented_transform import unscented_transform  # noqa: F401
 from .IMM import IMMEstimator  # noqa: F401
 from .mmae import MMAEFilterBank  # noqa: F401

@@ -6,6 +6,7 @@
 //   bke::ukf_step             bke_ukf_step             UnscentedKalmanFilter.predict + update, UKF.py:364-491
 //   bke::ckf_step             bke_ckf_step             CubatureKalmanFilter.predict + update, CubatureKalmanFilter.py:292-389
 //   bke::srkf_step            bke_srkf_step            SquareRootKalmanFilter.predict + update, square_root.py:172-248
+//   bke::fls_smooth_batch     bke_fls_smooth           FixedLagSmoother.smooth_batch, fixed_lag_smoother.py:217-311
 //   bke::systematic_resample  bke_systematic_resample  monte_carlo/resampling.py:117-150
 //   bke::stratified_resample  bke_stratified_resample  monte_carlo/resampling.py:80-114
 #include <ATen/ATen.h>
@@ -154,6 +155,42 @@ std::tuple<at::Tensor, at::Tensor> srkf_step(const at::Tensor &x, const at::Tens
     return std::make_tuple(x_out, L_out);
 }
 
+// smooth_batch(zs, N) from (x, P): returns (xSmooth [T, N, n], xhat [T, N, n]); x and P are not changed
+std::tuple<at::Tensor, at::Tensor> fls_smooth_batch(const at::Tensor &x, const at::Tensor &P, const at::Tensor &F, const at::Tensor &H,
+                                                    const at::Tensor &Q, const at::Tensor &R, const at::Tensor &zs, int64_t lag)
+{
+    TORCH_CHECK(x.is_cuda() && P.is_cuda() && x.is_contiguous() && P.is_contiguous(), "bke: x and P must be contiguous CUDA tensors");
+    TORCH_CHECK(x.dim() == 2 && P.dim() == 3 && P.size(0) == x.size(0) && P.size(1) == x.size(1) && P.size(2) == x.size(1), "bke: x is [N, n], P is [N, n, n]");
+    TORCH_CHECK(P.scalar_type() == x.scalar_type(), "bke: x and P must share a dtype");
+    c10::cuda::CUDAGuard guard(x.device());
+    const int64_t N = x.size(0), n = x.size(1), m = H.size(-2);
+    TORCH_CHECK(zs.is_cuda() && zs.is_contiguous() && zs.scalar_type() == x.scalar_type() && zs.dim() == 3 && zs.size(1) == N && zs.size(2) == m,
+                "bke: zs is [T, N, m]");
+    const int64_t T = zs.size(0);
+    at::Tensor xs = at::empty({T, N, n}, x.options()), xhat = at::empty({T, N, n}, x.options());
+    if (T == 0 || N == 0) return std::make_tuple(xs, xhat);
+    bke_fls_args a;
+    std::memset(&a, 0, sizeof(a));
+    bke_kf_args &k = a.step;
+    k.n_filters = N; k.dim_x = (int32_t)n; k.dim_z = (int32_t)m; k.dtype = dtype_of(x); k.alpha_sq = 1.0;
+    at::Tensor x_out = at::empty_like(x), P_out = at::empty_like(P);
+    k.x = x.data_ptr(); k.P = P.data_ptr(); k.x_out = x_out.data_ptr(); k.P_out = P_out.data_ptr();
+    k.F = model(F, N, n, n, &k.F_stride, x, "F");
+    k.H = model(H, N, m, n, &k.H_stride, x, "H");
+    k.Q = model(Q, N, n, n, &k.Q_stride, x, "Q");
+    k.R = model(R, N, m, m, &k.R_stride, x, "R");
+    a.n_steps = T; a.lag = lag; a.count = 0;
+    a.zs = zs.data_ptr(); a.xs_smooth = xs.data_ptr(); a.xhat = xhat.data_ptr();
+    const size_t wsb = bke_fls_workspace_bytes(N, k.dim_x, k.dim_z, 0, k.dtype, lag);
+    at::Tensor ws;
+    if (wsb) {
+        ws = at::empty({(int64_t)wsb}, x.options().dtype(at::kByte));      // the caching allocator aligns to 512 B
+        a.workspace = ws.data_ptr(); a.workspace_bytes = wsb;
+    }
+    check_rc(bke_fls_smooth(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_fls_smooth");
+    return std::make_tuple(xs, xhat);
+}
+
 at::Tensor resample(const at::Tensor &w, double u, const c10::optional<at::Tensor> &U)
 {
     TORCH_CHECK(w.is_cuda() && w.is_contiguous() && w.scalar_type() == at::kDouble && w.dim() == 1, "bke: weights must be a contiguous 1-D float64 CUDA tensor");
@@ -195,6 +232,7 @@ TORCH_LIBRARY(bke, m)
     m.def("ckf_step(Tensor x, Tensor P, Tensor Q, Tensor R, Tensor z, float dt, int fx_model, int hx_model, "
           "Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor)");
     m.def("srkf_step(Tensor x, Tensor L, Tensor F, Tensor H, Tensor Lq, Tensor Lr, Tensor z) -> (Tensor, Tensor)");
+    m.def("fls_smooth_batch(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor zs, int N) -> (Tensor, Tensor)");
     m.def("systematic_resample(Tensor weights, float u) -> Tensor");
     m.def("stratified_resample(Tensor weights, Tensor uniforms) -> Tensor");
 }
@@ -206,6 +244,7 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("ukf_step", &ukf_step);
     m.impl("ckf_step", &ckf_step);
     m.impl("srkf_step", &srkf_step);
+    m.impl("fls_smooth_batch", &fls_smooth_batch);
     m.impl("systematic_resample", &systematic_resample);
     m.impl("stratified_resample", &stratified_resample);
 }

@@ -197,6 +197,45 @@ typedef struct bke_kf_batch_args {
 
 int bke_kf_batch_filter(const bke_kf_batch_args *args, void *stream);
 
+/* FixedLagSmoother.smooth / smooth_batch for a bank (filterpy/kalman/fixed_lag_smoother.py:133-215 /
+ * :217-311): T epochs of fixed-lag smoothing with lag N, continuing a run that has taken `count` epochs.
+ * Per filter, epoch k = count + t:
+ *   x_pre = F x (+ B u);  P = F P F' + Q;  y = z - H x_pre;  S = H P H' + R;  SI = S^-1;  K = P H' SI;
+ *   x = x_pre + K y;  P = (I - K H) P (I - K H)' + K R K'   (no fading factor)          [xhat[t] = x]
+ *   row k of the history = x_pre;  if k < N: row k = x;  else, with g = H' SI y and A = (F - K H)':
+ *   row k - i += P A^i g  for i = 0 .. N-1      (the reference's P (F - K H)'^i H' SI y, reassociated)
+ * After epoch k, rows k-N+2 .. k can still change; every row <= k-N+1 is final.
+ *   xs_smooth   the history, row r at r * n_filters * dim_x: the call reads the live rows count-N+1 ..
+ *               count-1 and writes rows up to count+T-1 (the caller provides room for them);
+ *   zs[T,N,m], us[T,N,dim_u] (NULL: no control input; else step.B and dim_u >= 1), xhat[T,N,n] (or NULL);
+ *   step        n_filters, dims, dtype, x / P, the models and strides, B, x_out / P_out (the state after the
+ *               last epoch; may alias x / P) and the optional status[N], y[N,m] and S[N,m,m] of the last
+ *               epoch.  Its flags, alpha_sq, z, z_valid, u, x_prior, P_prior, K, SI, log_likelihood are ignored.
+ * Every measurement is present (the reference has no missing-measurement rule: z = None raises TypeError).
+ * Where the reference's inv(S) raises LinAlgError, status[f] = BKE_STATUS_SINGULAR_S (sticky over the call's
+ * epochs), that filter keeps its prior for the epoch (x = x_pre, P = the predicted P), its row k is x_pre
+ * and no row is corrected.
+ * The workspace (bke_fls_workspace_bytes, 16-byte aligned) is only needed when the call runs the per-epoch
+ * path: the size is 0 when the fused kernel covers the shape.  Fused (DESIGN.md §3.4b): 1/1, 2/1 and 4/2,
+ * fp32 and fp64, without control input, lag <= BKE_FLS_FUSED_MAX_LAG; the lag window stays in shared memory
+ * and each history row is stored once.  Every other call runs bke_kf_step's kernels once per epoch and a
+ * lag-correction kernel on the history in HBM. */
+#define BKE_FLS_FUSED_MAX_LAG 16
+typedef struct bke_fls_args {
+    bke_kf_args step;
+    int64_t n_steps;                 /* T >= 1 */
+    int64_t lag;                     /* N >= 0 */
+    int64_t count;                   /* epochs already taken (>= 0) */
+    const void *zs;
+    const void *us;
+    void *xs_smooth;
+    void *xhat;
+    void *workspace; size_t workspace_bytes;
+} bke_fls_args;
+
+size_t bke_fls_workspace_bytes(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dim_u, int32_t dtype, int64_t lag);
+int bke_fls_smooth(const bke_fls_args *args, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * Unscented Kalman filter bank (Merwe scaled sigma points).
  * Replaces UnscentedKalmanFilter.predict / update (filterpy/kalman/UKF.py:364-411, 413-491),
