@@ -81,25 +81,16 @@ class IMMEstimator(object):
         self._x_post = self._x.clone(); self._P_post = self._P.clone()
 
     # ------------------------------------------------------------------ outputs
-    def _vec(self, t):
-        if not self._single:
-            return t
-        v = t[0].cpu().numpy()
-        return v.reshape(-1, 1) if self.filters[0]._x_col else v
-
-    def _mat(self, t):
-        return t if not self._single else t[0].cpu().numpy()
-
-    x = property(lambda self: self._vec(self._x))
-    P = property(lambda self: self._mat(self._P))
-    x_prior = property(lambda self: self._vec(self._x_prior))
-    P_prior = property(lambda self: self._mat(self._P_prior))
-    x_post = property(lambda self: self._vec(self._x_post))
-    P_post = property(lambda self: self._mat(self._P_post))
-    mu = property(lambda self: self._mat(self._mu))
+    x = property(lambda self: self.filters[0]._vec_out(self._x))
+    P = property(lambda self: self.filters[0]._out(self._P))
+    x_prior = property(lambda self: self.filters[0]._vec_out(self._x_prior))
+    P_prior = property(lambda self: self.filters[0]._out(self._P_prior))
+    x_post = property(lambda self: self.filters[0]._vec_out(self._x_post))
+    P_post = property(lambda self: self.filters[0]._out(self._P_post))
+    mu = property(lambda self: self.filters[0]._out(self._mu))
     M = property(lambda self: self._M.cpu().numpy())
-    cbar = property(lambda self: self._mat(self._cbar))
-    omega = property(lambda self: self._mat(self._omega))
+    cbar = property(lambda self: self.filters[0]._out(self._cbar))
+    omega = property(lambda self: self.filters[0]._out(self._omega))
 
     @property
     def likelihood(self):

@@ -18,15 +18,13 @@ CPU fallback.  As for the linear filter, ``n_filters=None`` gives a single-filte
 attributes are NumPy arrays (``x`` is 1-D, UKF.py:298).
 """
 import ctypes
-import math
-import sys
 
 import numpy as np
 import torch
 
 from .. import _lib
-from .._dev import bke_dtype, ptr, require_cuda, resolve_dtype, stream_ptr, to_dev
-from .kalman_filter import _Linked
+from .._dev import bke_dtype, ptr, stream_ptr
+from ._bank import _BankMirror, _model_prop
 
 __all__ = ["UnscentedKalmanFilter", "LinearFx", "ConstVelFx", "LinearHx", "RangeAzElHx", "RangeBearingHx",
            "DeviceFx", "DeviceHx"]
@@ -142,23 +140,28 @@ def _no_hook(name, v):
             "has no CPU fallback (see filterpy_b200/kalman/UKF.py)" % name)
 
 
-class _SigmaPointBank(object):
-    """What the UKF and CKF mirrors share: the bank's state, models and diagnostics, their NumPy views in
-    single-filter mode, and the deferred predict (``_pending`` / ``_flush``)."""
+def _require_device_models(fx, hx):
+    if not hasattr(fx, "model") or not hasattr(hx, "model"):
+        raise NotImplementedError(
+            "fx / hx must be device-side models (LinearFx, ConstVelFx, LinearHx, RangeAzElHx, "
+            "RangeBearingHx, or DeviceFx / DeviceHx around CUDA source text): Python callables cannot "
+            "run inside the CUDA kernel and there is no CPU fallback")
+
+
+class _SigmaPointBank(_BankMirror):
+    """What the UKF and CKF mirrors share on top of ``_BankMirror``: the device-side fx / hx models (and a
+    compiled user model), the reference's Q and R, the deferred predict (``_pending`` holds its dt) and the
+    fields and launch of their argument structs."""
     _compile_model = staticmethod(_compile_model)
+    _COLUMN_X = False                                   # x is 1-D (UKF.py:298)
+    _FAILURE = "matrix not positive definite / singular"
 
     def _init_bank(self, dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics):
         """The state, models, compiled user model and diagnostic buffers of a bank (the reference's
         __init__ defaults: x = 0, P = I, Q = I, R = I)."""
-        self._dim_x, self._dim_z = int(dim_x), int(dim_z)
-        self._single = n_filters is None
-        self.n_filters = 1 if self._single else int(n_filters)
-        self._dtype = resolve_dtype(dtype)
-        self._device = require_cuda(device)
-        self._lib = _lib.load()
+        _BankMirror._init_bank(self, dim_x, dim_z, n_filters, dtype, device, diagnostics)
         self.fx, self.hx = fx, hx
-        self.diagnostics = bool(diagnostics)
-        N, n, m = self.n_filters, self._dim_x, self._dim_z
+        N, n, m = self.n_filters, self.dim_x, self.dim_z
         kw = dict(dtype=self._dtype, device=self._device)
         self._x = torch.zeros(N, n, **kw)
         self._P = torch.eye(n, **kw).repeat(N, 1, 1)
@@ -178,126 +181,67 @@ class _SigmaPointBank(object):
             if isinstance(hx, _DeviceModel):
                 self._hx_args = hx.pack({}, N, self._dtype, self._device) if all(k in hx.values for k in hx.arg_names) else (None, 0)
         if self.diagnostics:
-            self._x_prior = self._x.clone(); self._P_prior = self._P.clone()
-            self._x_post = self._x.clone(); self._P_post = self._P.clone()
-            self._K = torch.zeros(N, n, m, **kw); self._y = torch.zeros(N, m, **kw)
-            self._S = torch.zeros(N, m, m, **kw); self._SI = torch.zeros(N, m, m, **kw)
-            self._ll = torch.full((N,), math.log(sys.float_info.min), **kw)
-            self._status = torch.zeros(N, dtype=torch.int32, device=self._device)
+            self._alloc_diagnostics()
 
-    # ------------------------------------------------------------------ plumbing (as KalmanFilter)
-    def _model(self, a, rows, cols, name):
-        if np.isscalar(a):
-            return torch.eye(rows, dtype=self._dtype, device=self._device) * float(a)
-        t = to_dev(a, self._dtype, self._device)
-        if tuple(t.shape) == (rows, cols) or tuple(t.shape) == (self.n_filters, rows, cols):
-            return t
-        raise ValueError("%s must have shape (%d,%d) or (%d,%d,%d), got %s"
-                         % (name, rows, cols, self.n_filters, rows, cols, tuple(t.shape)))
+    _dim_x = property(lambda self: self.dim_x)          # the reference's names
+    _dim_z = property(lambda self: self.dim_z)
+    Q = _model_prop("Q", "dim_x", "dim_x")
+    R = _model_prop("R", "dim_z", "dim_z")
 
-    @staticmethod
-    def _stride(t):
-        return 0 if t.dim() == 2 else t.shape[1] * t.shape[2]
+    def _flush(self):
+        if self._pending is not None:
+            dt, self._pending = self._pending, None
+            self._launch(_lib.BKE_DO_PREDICT, dt, None, None, None)
 
-    def _out(self, t):
-        return t if not self._single else t[0].cpu().numpy()
+    def _skip_update(self, dt):
+        """``update(None)``: run a pending predict, and the posterior is the prior."""
+        if dt is not None:
+            self._launch(_lib.BKE_DO_PREDICT, dt, None, None, None)
+        self._z = None
+        if self.diagnostics:
+            self._x_post.copy_(self._x); self._P_post.copy_(self._P)
 
-    @property
-    def x(self):
-        self._flush()
-        return self._x if not self._single else _Linked(self._x[0].cpu().numpy(), self, "x")
+    def _fill(self, a, flags, dt, zt, vt, R):
+        """The fields the UKF and CKF argument structs share."""
+        N, n, m = self.n_filters, self.dim_x, self.dim_z
+        a.n_filters, a.dim_x, a.dim_z = N, n, m
+        a.dtype = bke_dtype(self._dtype)
+        a.flags = flags
+        a.fx_model, a.hx_model = self.fx.model, self.hx.model
+        a.dt = float(dt)
+        a.x = a.x_out = ptr(self._x)
+        a.P = a.P_out = ptr(self._P)
+        a.Q, a.Q_stride = ptr(self._Q), self._stride(self._Q)
+        Rm = self._R if R is None else self._model(R, m, m, "R")          # scalar R -> R*I (UKF.py:456-457)
+        a.R, a.R_stride = ptr(Rm), self._stride(Rm)
+        if self._F is not None:
+            a.F, a.F_stride = ptr(self._F), self._stride(self._F)
+        if self._H is not None:
+            a.H, a.H_stride = ptr(self._H), self._stride(self._H)
+        a.z, a.z_valid = ptr(zt), ptr(vt)
+        if self.diagnostics:
+            if flags & _lib.BKE_DO_PREDICT:
+                a.x_prior, a.P_prior = ptr(self._x_prior), ptr(self._P_prior)
+            if flags & _lib.BKE_DO_UPDATE:
+                a.K, a.y, a.S, a.SI = ptr(self._K), ptr(self._y), ptr(self._S), ptr(self._SI)
+                a.log_likelihood = ptr(self._ll)
+            a.status = ptr(self._status)
+        return a
 
-    @x.setter
-    def x(self, v):
-        self._flush()
-        t = to_dev(v, self._dtype, self._device)
-        if tuple(t.shape) == (self._dim_x,):
-            t = t.expand(self.n_filters, self._dim_x)
-        if tuple(t.shape) != (self.n_filters, self._dim_x):
-            raise ValueError("x must have shape (%d,) or (%d,%d)" % (self._dim_x, self.n_filters, self._dim_x))
-        self._x = t.contiguous().clone()
-
-    @property
-    def P(self):
-        self._flush()
-        return self._P if not self._single else _Linked(self._P[0].cpu().numpy(), self, "P")
-
-    @P.setter
-    def P(self, v):
-        self._flush()
-        n = self._dim_x
-        if np.isscalar(v):
-            v = np.eye(n) * v
-        t = to_dev(v, self._dtype, self._device)
-        if tuple(t.shape) == (n, n):
-            t = t.expand(self.n_filters, n, n)
-        if tuple(t.shape) != (self.n_filters, n, n):
-            raise ValueError("P must have shape (%d,%d) or (%d,%d,%d)" % (n, n, self.n_filters, n, n))
-        self._P = t.contiguous().clone()
-
-    # A deferred predict() must run with the Q it was issued with (the reference's predict has
-    # already happened): the setters, and the bank-mode getters that hand out the live tensor,
-    # flush it first.  Single mode returns write-back arrays so that ``ukf.P[2, 2] = 100`` /
-    # ``ukf.Q[0, 0] = q`` reach the filter as they do in the reference.
-    def _get_model(self, name):
-        t = getattr(self, "_" + name)
-        if self._single:
-            return _Linked(t.cpu().numpy(), self, name)
-        self._flush()
-        return t
-
-    def _set_model(self, name, v, dim):
-        self._flush()
-        setattr(self, "_" + name, self._model(v, dim, dim, name))
-
-    Q = property(lambda self: self._get_model("Q"), lambda self, v: self._set_model("Q", v, self._dim_x))
-    R = property(lambda self: self._get_model("R"), lambda self, v: self._set_model("R", v, self._dim_z))
-
-    def _diag(self, name):
-        if not self.diagnostics:
-            raise AttributeError("%s is only kept when the filter is built with diagnostics=True" % name)
-        self._flush()
-        return getattr(self, "_" + name)
-
-    x_prior = property(lambda self: self._out(self._diag("x_prior")))
-    P_prior = property(lambda self: self._out(self._diag("P_prior")))
-    x_post = property(lambda self: self._out(self._diag("x_post")))
-    P_post = property(lambda self: self._out(self._diag("P_post")))
-    K = property(lambda self: self._out(self._diag("K")))
-    y = property(lambda self: self._out(self._diag("y")))
-    S = property(lambda self: self._out(self._diag("S")))
-    SI = property(lambda self: self._out(self._diag("SI")))
-    status = property(lambda self: self._diag("status"))
-
-    @property
-    def z(self):
-        if self._z is None:
-            return np.array([[None] * self._dim_z]).T
-        return self._out(self._z)
-
-    @property
-    def log_likelihood(self):
-        ll = self._diag("ll")
-        return float(ll[0].item()) if self._single else ll
-
-    @property
-    def likelihood(self):
-        lk = torch.exp(self._diag("ll")).clamp_min(sys.float_info.min)
-        return float(lk[0].item()) if self._single else lk
-
-    @property
-    def mahalanobis(self):
-        y, SI = self._diag("y"), self._diag("SI")
-        d = torch.sqrt(torch.einsum("ni,nij,nj->n", y, SI, y))
-        return float(d[0].item()) if self._single else d
-
-    def check(self):
-        """Raise LinAlgError where the reference would (non-PD P in cholesky, singular S)."""
-        st = self._diag("status")
-        bad = int((st != 0).sum().item())
-        if bad:
-            raise np.linalg.LinAlgError("%d of %d filters: matrix not positive definite / singular"
-                                        % (bad, self.n_filters))
+    def _step(self, a, step, step_model):
+        """Launch a filled struct on the built-in models (``step``) or the compiled user model (``step_model``)."""
+        if self._user_model is None:
+            self._run(step, a, stream_ptr(self._device))
+        else:
+            for nm, mdl, (t, _) in (("fx", self.fx, self._fx_args), ("hx", self.hx, self._hx_args)):
+                if isinstance(mdl, _DeviceModel) and mdl.arg_names and t is None:
+                    raise TypeError("%s needs values for its arguments %s" % (nm, list(mdl.arg_names)))
+            self._run(step_model, a, self._user_model, ptr(self._fx_args[0]), self._fx_args[1],
+                      ptr(self._hx_args[0]), self._hx_args[1], stream_ptr(self._device))
+        if self.diagnostics and (a.flags & _lib.BKE_DO_UPDATE):
+            self._x_post.copy_(self._x); self._P_post.copy_(self._P)
+        if self.diagnostics and self._single:
+            self.check()
 
 
 class UnscentedKalmanFilter(_SigmaPointBank):
@@ -307,11 +251,7 @@ class UnscentedKalmanFilter(_SigmaPointBank):
         for nm, v in (("sqrt_fn", sqrt_fn), ("x_mean_fn", x_mean_fn), ("z_mean_fn", z_mean_fn),
                       ("residual_x", residual_x), ("residual_z", residual_z), ("state_add", state_add)):
             _no_hook(nm, v)
-        if not hasattr(fx, "model") or not hasattr(hx, "model"):
-            raise NotImplementedError(
-                "fx / hx must be device-side models (LinearFx, ConstVelFx, LinearHx, RangeAzElHx, "
-                "RangeBearingHx, or DeviceFx / DeviceHx around CUDA source text): Python callables cannot "
-                "run inside the CUDA kernel and there is no CPU fallback")
+        _require_device_models(fx, hx)
         if points.n != dim_x:
             raise ValueError("expected size(x) {}, but size is {}".format(points.n, dim_x))   # sigma_points.py:153
         self._init_bank(dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics)
@@ -332,11 +272,6 @@ class UnscentedKalmanFilter(_SigmaPointBank):
             self._fx_args = self.fx.pack(fx_args, self.n_filters, self._dtype, self._device)
         self._pending = self._dt if dt is None else dt
 
-    def _flush(self):
-        if self._pending is not None:
-            dt, self._pending = self._pending, None
-            self._launch(_lib.BKE_DO_PREDICT, dt, None, None, None)
-
     def update(self, z, R=None, UT=None, hx=None, valid=None, **hx_args):
         """UKF.py:413-491.  ``z`` is ``(N, dim_z)`` in bank mode; ``z=None`` skips the update.
 
@@ -351,62 +286,18 @@ class UnscentedKalmanFilter(_SigmaPointBank):
             self._hx_args = self.hx.pack(hx_args, self.n_filters, self._dtype, self._device)
         dt, self._pending = self._pending, None
         if z is None:                                            # UKF.py:442-446
-            if dt is not None:
-                self._launch(_lib.BKE_DO_PREDICT, dt, None, None, None)
-            self._z = None
-            if self.diagnostics:
-                self._x_post.copy_(self._x); self._P_post.copy_(self._P)
+            self._skip_update(dt)
             return
-        m = self._dim_z
-        zt = to_dev(np.asarray(z, dtype=np.float64).reshape(1, -1) if self._single else z, self._dtype, self._device)
-        if tuple(zt.shape) != (self.n_filters, m):
-            raise ValueError("z must have shape (%d,%d), got %s" % (self.n_filters, m, tuple(zt.shape)))
-        vt = None
-        if valid is not None:
-            vt = torch.as_tensor(valid, device=self._device).to(torch.uint8).contiguous()
+        zt = self._z_rows(z)
+        vt = self._valid_mask(valid)
         flags = _lib.BKE_DO_UPDATE | (_lib.BKE_DO_PREDICT if dt is not None else 0)
-        self._launch(flags, self._dt if dt is None else dt, zt.contiguous(), vt, R)
+        self._launch(flags, self._dt if dt is None else dt, zt, vt, R)
         self._z = zt
 
     def _launch(self, flags, dt, zt, vt, R):
-        a = _lib.UkfArgs()
-        N, n, m = self.n_filters, self._dim_x, self._dim_z
-        a.n_filters, a.dim_x, a.dim_z = N, n, m
-        a.dtype = bke_dtype(self._dtype)
-        a.flags = flags
-        a.fx_model, a.hx_model = self.fx.model, self.hx.model
-        a.dt = float(dt)
+        a = self._fill(_lib.UkfArgs(), flags, dt, zt, vt, R)
         a.alpha, a.beta, a.kappa = self.points_fn.alpha, self.points_fn.beta, self.points_fn.kappa
-        a.x = a.x_out = ptr(self._x)
-        a.P = a.P_out = ptr(self._P)
-        a.Q, a.Q_stride = ptr(self._Q), self._stride(self._Q)
-        Rm = self._R if R is None else self._model(R, m, m, "R")          # scalar R -> R*I (UKF.py:456-457)
-        a.R, a.R_stride = ptr(Rm), self._stride(Rm)
-        if self._F is not None:
-            a.F, a.F_stride = ptr(self._F), self._stride(self._F)
-        if self._H is not None:
-            a.H, a.H_stride = ptr(self._H), self._stride(self._H)
-        a.z, a.z_valid = ptr(zt), ptr(vt)
-        if self.diagnostics:
-            if flags & _lib.BKE_DO_PREDICT:
-                a.x_prior, a.P_prior = ptr(self._x_prior), ptr(self._P_prior)
-            if flags & _lib.BKE_DO_UPDATE:
-                a.K, a.y, a.S, a.SI = ptr(self._K), ptr(self._y), ptr(self._S), ptr(self._SI)
-                a.log_likelihood = ptr(self._ll)
-            a.status = ptr(self._status)
-        with torch.cuda.device(self._device):
-            if self._user_model is not None:
-                for nm, mdl, (t, _) in (("fx", self.fx, self._fx_args), ("hx", self.hx, self._hx_args)):
-                    if isinstance(mdl, _DeviceModel) and mdl.arg_names and t is None:
-                        raise TypeError("%s needs values for its arguments %s" % (nm, list(mdl.arg_names)))
-                _lib.check(self._lib.bke_ukf_step_model(a, self._user_model, ptr(self._fx_args[0]), self._fx_args[1],
-                                                        ptr(self._hx_args[0]), self._hx_args[1], stream_ptr(self._device)))
-            else:
-                _lib.check(self._lib.bke_ukf_step(a, stream_ptr(self._device)))
-        if self.diagnostics and (flags & _lib.BKE_DO_UPDATE):
-            self._x_post.copy_(self._x); self._P_post.copy_(self._P)
-        if self.diagnostics and self._single:
-            self.check()
+        self._step(a, self._lib.bke_ukf_step, self._lib.bke_ukf_step_model)
 
     def rts_smoother(self, Xs, Ps, Qs=None, dts=None, UT=None):
         """UKF.py:634-739 on the GPU.  Bank mode: ``Xs[T,N,n]``, ``Ps[T,N,n,n]`` (what
@@ -417,16 +308,10 @@ class UnscentedKalmanFilter(_SigmaPointBank):
         if len(Xs) != len(Ps):
             raise ValueError('Xs and Ps must have the same length')
         self._flush()
-        N, n = self.n_filters, self._dim_x
+        N, n = self.n_filters, self.dim_x
         is_np = not isinstance(Xs, torch.Tensor)
-        Xt = to_dev(Xs, self._dtype, self._device)
-        Pt = to_dev(Ps, self._dtype, self._device)
+        Xt, Pt, _ = self._history(Xs, Ps)
         T = Xt.shape[0]
-        if self._single:
-            Xt = Xt.reshape(T, 1, n); Pt = Pt.reshape(T, 1, n, n)
-        if tuple(Xt.shape) != (T, N, n) or tuple(Pt.shape) != (T, N, n, n):
-            raise ValueError("Xs / Ps must have shapes (T,%d,%d) / (T,%d,%d,%d)" % (N, n, N, n, n))
-        Xt = Xt.contiguous(); Pt = Pt.contiguous()
         kw = dict(dtype=self._dtype, device=self._device)
         xs = torch.empty(T, N, n, **kw); Pso = torch.empty(T, N, n, n, **kw); Ks = torch.empty(T, N, n, n, **kw)
         status = torch.zeros(N, dtype=torch.int32, device=self._device)
@@ -451,16 +336,15 @@ class UnscentedKalmanFilter(_SigmaPointBank):
             a.F, a.F_stride = ptr(self._F), self._stride(self._F)
         a.x_out, a.P_out, a.K = ptr(xs), ptr(Pso), ptr(Ks)
         a.status = ptr(status)
-        with torch.cuda.device(self._device):
-            if isinstance(self.fx, _DeviceModel):
-                # the reference calls self.fx(sigma, dt) without keyword arguments here (UKF.py:712): the model's
-                # current argument values stand in for the defaults of its callable
-                if self.fx.arg_names and self._fx_args[0] is None:
-                    raise TypeError("fx needs values for its arguments %s" % list(self.fx.arg_names))
-                _lib.check(self._lib.bke_ukf_rts_smoother_model(ctypes.byref(a), self._user_model, ptr(self._fx_args[0]),
-                                                                self._fx_args[1], stream_ptr(self._device)))
-            else:
-                _lib.check(self._lib.bke_ukf_rts_smoother(ctypes.byref(a), stream_ptr(self._device)))
+        if isinstance(self.fx, _DeviceModel):
+            # the reference calls self.fx(sigma, dt) without keyword arguments here (UKF.py:712): the model's
+            # current argument values stand in for the defaults of its callable
+            if self.fx.arg_names and self._fx_args[0] is None:
+                raise TypeError("fx needs values for its arguments %s" % list(self.fx.arg_names))
+            self._run(self._lib.bke_ukf_rts_smoother_model, ctypes.byref(a), self._user_model, ptr(self._fx_args[0]),
+                      self._fx_args[1], stream_ptr(self._device))
+        else:
+            self._run(self._lib.bke_ukf_rts_smoother, ctypes.byref(a), stream_ptr(self._device))
         if not self._single:
             return xs, Pso, Ks
         if int(status[0].item()) != 0:
@@ -476,7 +360,7 @@ class UnscentedKalmanFilter(_SigmaPointBank):
             z0 = zs[0]
         except TypeError:
             raise TypeError('zs must be list-like')                       # UKF.py:593-596
-        m = self._dim_z
+        m = self.dim_z
         if self._single:
             if m == 1:
                 if not (np.isscalar(z0) or (np.ndim(z0) == 1 and len(z0) == 1)):
@@ -484,7 +368,7 @@ class UnscentedKalmanFilter(_SigmaPointBank):
             elif z0 is not None and len(z0) != m:
                 raise TypeError('each element in zs must be a 1D array of length {}'.format(m))
         T = len(zs)
-        N, n = self.n_filters, self._dim_x
+        N, n = self.n_filters, self.dim_x
         kw = dict(dtype=self._dtype, device=self._device)
         means = torch.empty(T, N, n, **kw); covs = torch.empty(T, N, n, n, **kw)
         for i in range(T):

@@ -15,15 +15,15 @@ import numpy as np
 import torch
 
 from .. import _lib
-from .._dev import bke_dtype, ptr, require_cuda, resolve_dtype, stream_ptr, to_dev
-from .kalman_filter import _Linked
+from .._dev import bke_dtype, ptr, stream_ptr, to_dev
+from ._bank import _BankMirror, _model_prop
 
 __all__ = ["FixedLagSmoother"]
 
 _HISTORY_CAPACITY = 64          # rows of the first history buffer (bank mode); doubled when full
 
 
-class FixedLagSmoother(object):
+class FixedLagSmoother(_BankMirror):
     """``FixedLagSmoother(dim_x, dim_z, N=None)`` for ``n_filters`` filters at once.
 
     Attributes as in the reference: ``x``, ``P``, ``F``, ``Q``, ``H``, ``R``, ``B``, ``K``, ``y``, ``S``, ``x_s``,
@@ -38,24 +38,13 @@ class FixedLagSmoother(object):
 
     def __init__(self, dim_x, dim_z, N=None, *, dim_u=0, n_filters=None, dtype=np.float64, device=None,
                  diagnostics=True):
-        if dim_x < 1:
-            raise ValueError('dim_x must be 1 or greater')
-        if dim_z < 1:
-            raise ValueError('dim_z must be 1 or greater')
         if dim_u < 0:
             raise ValueError('dim_u must be 0 or greater')
         if N is not None and int(N) < 0:
             raise ValueError('N must be 0 or greater')
-        self.dim_x, self.dim_z, self.dim_u = int(dim_x), int(dim_z), int(dim_u)
+        self._init_bank(dim_x, dim_z, n_filters, dtype, device, diagnostics)
+        self.dim_u = int(dim_u)
         self.N = None if N is None else int(N)
-        self._single = n_filters is None
-        self.n_filters = 1 if self._single else int(n_filters)
-        if self.n_filters < 0:
-            raise ValueError('n_filters must be 0 or greater')
-        self._dtype = resolve_dtype(dtype)
-        self._device = require_cuda(device)
-        self._lib = _lib.load()
-        self.diagnostics = bool(diagnostics)
         Nf, n, m = self.n_filters, self.dim_x, self.dim_z
         kw = dict(dtype=self._dtype, device=self._device)
         self._x = torch.zeros(Nf, n, **kw)                   # :113-123
@@ -65,7 +54,6 @@ class FixedLagSmoother(object):
         self._H = torch.eye(m, n, **kw)
         self._R = torch.eye(m, **kw)
         self._B = None                                        # the reference's B = 0.
-        self._x_col = True
         self._y = torch.zeros(Nf, m, **kw)
         self._S = torch.zeros(Nf, m, m, **kw)
         self._y_set = False
@@ -76,25 +64,6 @@ class FixedLagSmoother(object):
         self._ws = None
 
     # ------------------------------------------------------------------ plumbing
-    def _model(self, a, rows, cols, name):
-        """(rows,cols) -> shared; (N,rows,cols) -> per filter; a scalar -> scalar * I."""
-        if np.isscalar(a):
-            if rows != cols:
-                raise ValueError("%s: a scalar needs a square matrix" % name)
-            return torch.eye(rows, dtype=self._dtype, device=self._device) * float(a)
-        t = to_dev(a, self._dtype, self._device)
-        if tuple(t.shape) == (rows, cols) or tuple(t.shape) == (self.n_filters, rows, cols):
-            return t.contiguous()
-        raise ValueError("%s must have shape (%d,%d) or (%d,%d,%d), got %s"
-                         % (name, rows, cols, self.n_filters, rows, cols, tuple(t.shape)))
-
-    @staticmethod
-    def _stride(t):
-        return 0 if t.dim() == 2 else t.shape[1] * t.shape[2]
-
-    def _out(self, t):
-        return t if not self._single else t[0].cpu().numpy()
-
     def _workspace(self, du, lag):
         nb = self._lib.bke_fls_workspace_bytes(self.n_filters, self.dim_x, self.dim_z, du, bke_dtype(self._dtype), lag)
         if nb == 0:
@@ -157,83 +126,13 @@ class FixedLagSmoother(object):
         a.zs, a.xs_smooth, a.xhat = ptr(zt), ptr(xs), ptr(xhat)
         ws, nb = self._workspace(du, lag)
         a.workspace, a.workspace_bytes = ptr(ws), nb
-        with torch.cuda.device(self._device):
-            _lib.check(self._lib.bke_fls_smooth(a, stream_ptr(self._device)))
+        self._run(self._lib.bke_fls_smooth, a, stream_ptr(self._device))
 
     # ------------------------------------------------------------------ state
-    @property
-    def x(self):
-        if not self._single:
-            return self._x
-        v = self._x[0].cpu().numpy()
-        return _Linked(v.reshape(-1, 1) if self._x_col else v, self, "x")
-
-    @x.setter
-    def x(self, v):
-        n = self.dim_x
-        t = to_dev(v, self._dtype, self._device)
-        if self._single:
-            if tuple(t.shape) not in ((n, 1), (n,)):
-                raise ValueError("x must have shape (%d,1) or (%d,), got %s" % (n, n, tuple(t.shape)))
-            self._x_col = t.dim() == 2
-            self._x = t.reshape(1, n).clone()
-            return
-        if t.dim() == 3 and t.shape[-1] == 1:
-            t = t[..., 0]
-        if tuple(t.shape) == (n,):
-            t = t.expand(self.n_filters, n)
-        if tuple(t.shape) != (self.n_filters, n):
-            raise ValueError("x must have shape (%d,) or (%d,%d), got %s" % (n, self.n_filters, n, tuple(t.shape)))
-        self._x = t.contiguous().clone()
-
-    @property
-    def P(self):
-        return self._P if not self._single else _Linked(self._P[0].cpu().numpy(), self, "P")
-
-    @P.setter
-    def P(self, v):
-        n = self.dim_x
-        if np.isscalar(v):
-            v = np.eye(n) * v
-        t = to_dev(v, self._dtype, self._device)
-        if tuple(t.shape) == (n, n):
-            t = t.expand(self.n_filters, n, n)
-        if tuple(t.shape) != (self.n_filters, n, n):
-            raise ValueError("P must have shape (%d,%d) or (%d,%d,%d)" % (n, n, self.n_filters, n, n))
-        self._P = t.contiguous().clone()
-
-    def _matrix_prop(name, rows_attr, cols_attr):  # noqa: N805
-        priv = "_" + name
-
-        def get(self):
-            t = getattr(self, priv)
-            return _Linked(t.cpu().numpy(), self, name) if self._single else t
-
-        def set_(self, v):
-            setattr(self, priv, self._model(v, getattr(self, rows_attr), getattr(self, cols_attr), name))
-        return property(get, set_)
-
-    F = _matrix_prop("F", "dim_x", "dim_x")
-    Q = _matrix_prop("Q", "dim_x", "dim_x")
-    H = _matrix_prop("H", "dim_z", "dim_x")
-    R = _matrix_prop("R", "dim_z", "dim_z")
-    del _matrix_prop
-
-    @property
-    def B(self):
-        if self._B is None:
-            return 0.
-        return _Linked(self._B.cpu().numpy(), self, "B") if self._single else self._B
-
-    @B.setter
-    def B(self, v):
-        if v is None or (np.isscalar(v) and v == 0):
-            self._B = None
-            return
-        if np.isscalar(v):
-            raise NotImplementedError("B must be a (dim_x, dim_u) matrix (or 0): a scalar B is not supported")
-        shp = np.shape(v) if not isinstance(v, torch.Tensor) else tuple(v.shape)
-        self._B = self._model(v, self.dim_x, int(shp[-1]), "B")
+    F = _model_prop("F", "dim_x", "dim_x")
+    Q = _model_prop("Q", "dim_x", "dim_x")
+    H = _model_prop("H", "dim_z", "dim_x")
+    R = _model_prop("R", "dim_z", "dim_z")
 
     @property
     def K(self):
@@ -246,11 +145,6 @@ class FixedLagSmoother(object):
         """the reference's initial zeros((dim_x, 1)): never written (:114)"""
         return self.K
 
-    def _diag(self, name):
-        if not self.diagnostics:
-            raise AttributeError("%s is only kept when the smoother is built with diagnostics=True" % name)
-        return getattr(self, "_" + name)
-
     @property
     def y(self):
         t = self._diag("y")
@@ -259,15 +153,8 @@ class FixedLagSmoother(object):
         v = t[0].cpu().numpy()
         return v.reshape(-1, 1) if (self._x_col or not self._y_set) else v
 
-    S = property(lambda self: self._out(self._diag("S")))
     status = property(lambda self: self._status,
                       doc="int32[N]: 1 where the last smooth() call met a singular S (the reference raises LinAlgError)")
-
-    def check(self):
-        """Raise ``np.linalg.LinAlgError`` if the last ``smooth()`` met a singular S in any filter."""
-        bad = int((self._status != 0).sum().item())
-        if bad:
-            raise np.linalg.LinAlgError("Singular matrix in %d of %d filters" % (bad, self.n_filters))
 
     @property
     def xSmooth(self):

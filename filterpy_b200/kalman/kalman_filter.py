@@ -21,7 +21,6 @@ until the next ``update`` or until somebody looks at the state).
 """
 import ctypes
 import math
-import sys
 
 import numpy as np
 import torch
@@ -29,62 +28,18 @@ import torch
 from .. import _lib
 from .._dev import StepGraph, bke_dtype, ptr, require_cuda, resolve_dtype, stream_ptr, to_dev
 from ..common.helpers import reshape_z
+from ._bank import _BankMirror, _model_prop
 
 __all__ = ["KalmanFilter", "predict", "update", "batch_filter", "rts_smoother"]
 
 
-class _Linked(np.ndarray):
-    """What the single-mode attribute getters hand out: a host copy of a device array that WRITES
-    BACK.  The reference's attributes are the live arrays, so the usual idioms ``kf.P[2, 2] = 100``,
-    ``kf.x[0] = z``, ``kf.F[0, 1] = dt``, ``kf.P *= 10`` must reach the filter; here they re-assign
-    the attribute (which uploads it).  Views derived from it (``kf.P[2]``) do not write back."""
-
-    def __new__(cls, arr, owner, name):
-        obj = np.array(arr, copy=True).view(cls)
-        obj._owner, obj._name = owner, name
-        return obj
-
-    def __array_finalize__(self, obj):
-        self._owner, self._name = None, None
-
-    def _push(self):
-        if self._owner is not None:
-            setattr(self._owner, self._name, np.array(self, copy=True).view(np.ndarray))
-
-    def __setitem__(self, key, value):
-        np.ndarray.__setitem__(self, key, value)
-        self._push()
-
-    def _inplace(self, op, other):
-        res = op(self.view(np.ndarray), other)
-        np.ndarray.__setitem__(self, Ellipsis, res)
-        self._push()
-        return self
-
-    def __iadd__(self, o): return self._inplace(np.add, o)
-    def __isub__(self, o): return self._inplace(np.subtract, o)
-    def __imul__(self, o): return self._inplace(np.multiply, o)
-    def __itruediv__(self, o): return self._inplace(np.true_divide, o)
-
-
-class KalmanFilter(object):
+class KalmanFilter(_BankMirror):
     def __init__(self, dim_x, dim_z, dim_u=0, n_filters=None, dtype=np.float64, device=None,
                  diagnostics=True):
-        if dim_x < 1:
-            raise ValueError('dim_x must be 1 or greater')      # kalman_filter.py:388-393
-        if dim_z < 1:
-            raise ValueError('dim_z must be 1 or greater')
         if dim_u < 0:
             raise ValueError('dim_u must be 0 or greater')
-        self.dim_x, self.dim_z, self.dim_u = int(dim_x), int(dim_z), int(dim_u)
-        self._single = n_filters is None
-        self.n_filters = 1 if self._single else int(n_filters)
-        if self.n_filters < 0:
-            raise ValueError('n_filters must be 0 or greater')
-        self._dtype = resolve_dtype(dtype)
-        self._device = require_cuda(device)
-        self._lib = _lib.load()
-        self.diagnostics = bool(diagnostics)
+        self._init_bank(dim_x, dim_z, n_filters, dtype, device, diagnostics)
+        self.dim_u = int(dim_u)
         N, n, m = self.n_filters, self.dim_x, self.dim_z
         kw = dict(dtype=self._dtype, device=self._device)
         self._x = torch.zeros(N, n, **kw)
@@ -95,19 +50,11 @@ class KalmanFilter(object):
         self._R = torch.eye(m, **kw)
         self._B = None
         self._alpha_sq = 1.0
-        self._x_col = True            # single mode: x is (n,1) like the reference default
         self._pending = None          # deferred predict: dict(u,B,F,Q)
         self._z = None
         self.inv = np.linalg.inv      # kept for API parity; only the default is supported
         if self.diagnostics:
-            self._x_prior = self._x.clone(); self._P_prior = self._P.clone()
-            self._x_post = self._x.clone(); self._P_post = self._P.clone()
-            self._K = torch.zeros(N, n, m, **kw)
-            self._y = torch.zeros(N, m, **kw)
-            self._S = torch.zeros(N, m, m, **kw)
-            self._SI = torch.zeros(N, m, m, **kw)
-            self._ll = torch.full((N,), math.log(sys.float_info.min), **kw)
-            self._status = torch.zeros(N, dtype=torch.int32, device=self._device)
+            self._alloc_diagnostics()
         self._host = {k: np.ascontiguousarray(getattr(self, "_" + k).cpu().numpy()) for k in "FQHR"}
         self._has_update = False
         self._post_alias = False      # True: x_post / P_post are the live x / P (nothing has moved them since the update)
@@ -127,88 +74,25 @@ class KalmanFilter(object):
         self._model_version = 0
         self._model_last = None       # the token of the previous launch
 
-    # ------------------------------------------------------------------ helpers
-    def _model(self, a, rows, cols, name):
-        """(rows,cols) -> shared; (N,rows,cols) -> per filter.  Returns a device tensor."""
-        if np.isscalar(a):
-            if rows != cols:
-                raise ValueError("%s: a scalar needs a square matrix" % name)
-            return torch.eye(rows, dtype=self._dtype, device=self._device) * float(a)
-        t = to_dev(a, self._dtype, self._device)
-        if t.dim() == 2 and tuple(t.shape) == (rows, cols):
-            return t
-        if t.dim() == 3 and tuple(t.shape) == (self.n_filters, rows, cols):
-            return t
-        if t.dim() == 1 and rows == 1 and t.shape[0] == cols:
-            return t.reshape(1, cols)
-        raise ValueError("%s must have shape (%d,%d) or (%d,%d,%d), got %s"
-                         % (name, rows, cols, self.n_filters, rows, cols, tuple(t.shape)))
-
-    @staticmethod
-    def _stride(t):
-        return 0 if t.dim() == 2 else t.shape[1] * t.shape[2]
-
-    def _out(self, t):
-        """bank mode: the device tensor; single mode: NumPy with the bank axis dropped."""
-        if not self._single:
-            return t
-        return t[0].cpu().numpy()
-
-    # ------------------------------------------------------------------ state attributes
-    @property
-    def x(self):
-        self._flush()
-        if not self._single:
-            return self._x
-        v = self._x[0].cpu().numpy()
-        return _Linked(v.reshape(-1, 1) if self._x_col else v, self, "x")
-
-    @x.setter
-    def x(self, v):
-        self._flush()
-        n = self.dim_x
-        t = to_dev(v, self._dtype, self._device)
-        if self._single:
-            if tuple(t.shape) == (n, 1):
-                self._x_col = True
-            elif tuple(t.shape) == (n,):
-                self._x_col = False
-            else:
-                raise ValueError("x must have shape (%d,1) or (%d,), got %s" % (n, n, tuple(t.shape)))
-            self._snapshot_post()
-            self._x = t.reshape(1, n).clone()
-            self._version += 1
-        else:
-            if t.dim() == 3 and t.shape[-1] == 1:
-                t = t[..., 0]
-            if tuple(t.shape) == (n,):
-                t = t.expand(self.n_filters, n)
-            if tuple(t.shape) != (self.n_filters, n):
-                raise ValueError("x must have shape (%d,%d), got %s" % (self.n_filters, n, tuple(t.shape)))
-            self._snapshot_post()
-            self._x = t.contiguous().clone()
-            self._version += 1
-
-    @property
-    def P(self):
-        self._flush()
-        return self._P if not self._single else _Linked(self._P[0].cpu().numpy(), self, "P")
-
-    @P.setter
-    def P(self, v):
-        self._flush()
-        n = self.dim_x
-        if np.isscalar(v):
-            v = np.eye(n) * v
-        t = to_dev(v, self._dtype, self._device)
-        if tuple(t.shape) == (n, n):
-            t = t.expand(self.n_filters, n, n)
-        if tuple(t.shape) != (self.n_filters, n, n):
-            raise ValueError("P must have shape (%d,%d) or (%d,%d,%d)" % (n, n, self.n_filters, n, n))
+    # ------------------------------------------------------------------ hooks of _BankMirror
+    def _state_rebound(self):
         self._snapshot_post()
-        self._P = t.contiguous().clone()
         self._version += 1
 
+    def _model_hook(self, name, assigned):
+        # a new or handed-out model invalidates the cached argument structs that carry its host copy, and
+        # (F, Q, H, R) the packed model words
+        if self._host.pop(name, None) is not None or assigned:
+            self._version += 1
+        if name in ("F", "Q", "H", "R"):
+            self._model_version += 1
+            t = getattr(self, "_" + name)
+            if assigned and t is not None and t.dim() == 2:
+                # host copy of a model shared by the bank: lets the kernels carry it in their launch
+                # parameters (bke_kf_args.*_host)
+                self._host[name] = np.ascontiguousarray(t.cpu().numpy())
+
+    # ------------------------------------------------------------------ state attributes
     def _adopt_state(self, x_t, P_t):
         """Re-bind the state to caller-owned device tensors (no copy) and hand back a spare pair, so
         that a caller (IMMEstimator's mixing step) can double-buffer.  When x_post / P_post are
@@ -225,53 +109,23 @@ class KalmanFilter(object):
         self._version += 1
         return spare
 
-    def _mk_model_prop(name, rows_attr, cols_attr):  # noqa: N805
-        priv = "_" + name
+    F = _model_prop("F", "dim_x", "dim_x")
+    Q = _model_prop("Q", "dim_x", "dim_x")
+    H = _model_prop("H", "dim_z", "dim_x")
+    R = _model_prop("R", "dim_z", "dim_z")
 
-        def get(self):
-            t = getattr(self, priv)
-            if t is None:
-                return None
-            if self._single:
-                return _Linked(t.cpu().numpy(), self, name)
-            # the caller may edit the live tensor in place: a deferred predict must run with the
-            # model it was issued with (the reference's predict has already happened), and the
-            # host copy can no longer be trusted, nor can the packed model words
-            self._flush()
-            if self._host.pop(name, None) is not None:
-                self._version += 1
-            if name in "FQHR":
-                self._model_version += 1
-            return t
+    @property
+    def B(self):
+        return self._get_model("B")
 
-        def set_(self, v):
-            self._flush()                                   # predict(); kf.F = F2; update(): the predict used the OLD F
-            self._version += 1
-            self._host.pop(name, None)
-            if name in "FQHR":
-                self._model_version += 1
-            if v is None:
-                setattr(self, priv, None)
-                return
-            cols = getattr(self, cols_attr)
-            if name == "B" and cols == 0 and not np.isscalar(v):
-                cols = int(np.shape(v)[-1]) if np.ndim(v) >= 1 else 1     # the reference never checks B against dim_u
-                if np.ndim(v) == 1:
-                    v = np.asarray(v).reshape(-1, 1); cols = 1
-            t = self._model(v, getattr(self, rows_attr), cols, name)
-            setattr(self, priv, t)
-            if t.dim() == 2 and name in "FQHR":
-                # host copy of a model shared by the bank: lets the kernels carry it in their launch
-                # parameters (bke_kf_args.*_host)
-                self._host[name] = np.ascontiguousarray(t.cpu().numpy())
-        return property(get, set_)
-
-    F = _mk_model_prop("F", "dim_x", "dim_x")
-    Q = _mk_model_prop("Q", "dim_x", "dim_x")
-    H = _mk_model_prop("H", "dim_z", "dim_x")
-    R = _mk_model_prop("R", "dim_z", "dim_z")
-    B = _mk_model_prop("B", "dim_x", "dim_u")
-    del _mk_model_prop
+    @B.setter
+    def B(self, v):
+        cols = self.dim_u
+        if cols == 0 and v is not None and not np.isscalar(v):
+            cols = int(np.shape(v)[-1]) if np.ndim(v) >= 1 else 1     # the reference never checks B against dim_u
+            if np.ndim(v) == 1:
+                v = np.asarray(v).reshape(-1, 1); cols = 1
+        self._set_model("B", v, self.dim_x, cols)
 
     @property
     def alpha(self):
@@ -286,21 +140,6 @@ class KalmanFilter(object):
         self._alpha_sq = float(value) ** 2
         self._version += 1
 
-    def _diag(self, name):
-        if not self.diagnostics:
-            raise AttributeError("%s is only kept when the filter is built with diagnostics=True" % name)
-        self._flush()
-        return getattr(self, "_" + name)
-
-    def _vec_out(self, t):
-        """x-like vectors follow the shape of x in single mode."""
-        if not self._single:
-            return t
-        v = t[0].cpu().numpy()
-        return v.reshape(-1, 1) if self._x_col else v
-
-    x_prior = property(lambda self: self._vec_out(self._diag("x_prior")))
-    P_prior = property(lambda self: self._out(self._diag("P_prior")))
     # x_post / P_post (kalman_filter.py:560-561) equal x / P until the next predict runs: they are
     # the live tensors until then, and are snapshotted only when a predict is launched on its own
     x_post = property(lambda self: self._vec_out(self._diag("x" if self._post_alias_now() else "x_post")))
@@ -316,48 +155,6 @@ class KalmanFilter(object):
         if self.diagnostics and self._post_alias:
             self._x_post.copy_(self._x); self._P_post.copy_(self._P)
         self._post_alias = False
-    K = property(lambda self: self._out(self._diag("K")))
-    y = property(lambda self: self._vec_out(self._diag("y")))
-    S = property(lambda self: self._out(self._diag("S")))
-    SI = property(lambda self: self._out(self._diag("SI")))
-
-    @property
-    def z(self):
-        if self._z is None:
-            return np.array([[None] * self.dim_z]).T
-        return self._vec_out(self._z)
-
-    @property
-    def status(self):
-        """int32[N]: 0 ok, 1 = S was singular (the reference raises LinAlgError there)."""
-        return self._diag("status")
-
-    def check(self):
-        """Raise ``np.linalg.LinAlgError`` if any filter hit a singular S (kalman_filter.py:541)."""
-        st = self._diag("status")
-        bad = int((st != 0).sum().item())
-        if bad:
-            raise np.linalg.LinAlgError("Singular matrix in %d of %d filters" % (bad, self.n_filters))
-
-    @property
-    def log_likelihood(self):
-        """log-likelihood of the last measurement (kalman_filter.py:1203-1210)."""
-        ll = self._diag("ll")
-        return float(ll[0].item()) if self._single else ll
-
-    @property
-    def likelihood(self):
-        """kalman_filter.py:1213-1223 (exp of the log-likelihood, floored at float min)."""
-        ll = self._diag("ll")
-        lk = torch.exp(ll).clamp_min(sys.float_info.min)
-        return float(lk[0].item()) if self._single else lk
-
-    @property
-    def mahalanobis(self):
-        """sqrt(y' SI y) (kalman_filter.py:1226-1239)."""
-        y, SI = self._diag("y"), self._diag("SI")
-        d = torch.sqrt(torch.einsum("ni,nij,nj->n", y, SI, y))
-        return float(d[0].item()) if self._single else d
 
     # ------------------------------------------------------------------ predict / update
     def predict(self, u=None, B=None, F=None, Q=None):
@@ -387,29 +184,10 @@ class KalmanFilter(object):
                 self._y.zero_()
                 self._ll.copy_(_missed_log_likelihood(self._S))
             return
-        m = self.dim_z
-        if self._single:
-            if H is None:
-                z = reshape_z(z, m, 2 if self._x_col else 1)        # :527-529
-            zt = to_dev(np.asarray(z, dtype=np.float64).reshape(-1), self._dtype, self._device)
-            if zt.numel() != m:
-                raise ValueError("z (shape %s) must be convertible to shape (%d, 1)" % (np.shape(z), m))
-            zt = zt.reshape(1, m)
-        elif (isinstance(z, torch.Tensor) and z.device == self._device and z.dtype == self._dtype
-              and z.dim() == 2 and z.shape[0] == self.n_filters and z.shape[1] == m and z.is_contiguous()):
-            zt = z                                              # already where the kernel wants it
-        else:
-            zt = to_dev(z, self._dtype, self._device)
-            if zt.dim() == 3 and zt.shape[-1] == 1:
-                zt = zt[..., 0]
-            if tuple(zt.shape) != (self.n_filters, m):
-                raise ValueError("z must have shape (%d,%d), got %s" % (self.n_filters, m, tuple(zt.shape)))
-            zt = zt.contiguous()
-        vt = None
-        if valid is not None:
-            vt = torch.as_tensor(valid, device=self._device).to(torch.uint8).contiguous()
-            if tuple(vt.shape) != (self.n_filters,):
-                raise ValueError("valid must have shape (%d,)" % self.n_filters)
+        if self._single and H is None:
+            z = reshape_z(z, self.dim_z, 2 if self._x_col else 1)        # :527-529
+        zt = self._z_rows(z)
+        vt = self._valid_mask(valid)
         flags = _lib.BKE_DO_UPDATE | (_lib.BKE_DO_PREDICT if pend is not None else 0)
         self._launch(flags, pend, zt, vt, R, H)
         if vt is not None and self.diagnostics:
@@ -417,25 +195,17 @@ class KalmanFilter(object):
             self._ll.copy_(torch.where(vt.bool(), self._ll, _missed_log_likelihood(self._S)))
         self._z = zt
 
-    def _call(self, a, rec=None):
-        if torch.cuda.current_device() == self._device.index:
-            self._step(a, rec)
-        else:
-            with torch.cuda.device(self._device):
-                self._step(a, rec)
-
     def _step(self, a, rec):
         s = stream_ptr(self._device)
         if rec is not None:
             rc = self._lib.bke_kf_step_packed(a, ptr(rec) if rec.numel() else None, self._sym_host_map, s)
             if rc != _lib.BKE_ERR_UNSUPPORTED:
-                _lib.check(rc)
-                return
+                return rc
             # BKE_KF_SYM=0, or arrays the packed kernel does not take (not 16-byte aligned): the dense
             # models from now on
             self._sym_ok = False
             self._sym_drop()
-        _lib.check(self._lib.bke_kf_step(a, s))
+        return self._lib.bke_kf_step(a, s)
 
     def _capturing(self):
         if torch.cuda.current_device() == self._device.index:
@@ -527,7 +297,7 @@ class KalmanFilter(object):
                 a.z = ptr(zt); a.z_valid = ptr(vt)
                 if not (flags & _lib.BKE_DO_UPDATE):
                     self._snapshot_post()                   # a predict on its own is about to move x, P
-                self._call(a, rec)
+                self._run(self._step, a, rec)
                 if self.diagnostics and (flags & _lib.BKE_DO_UPDATE):
                     self._post_alias = True
                     if self._single:
@@ -584,7 +354,7 @@ class KalmanFilter(object):
                 a.status = ptr(self._status)
         if not (flags & _lib.BKE_DO_UPDATE):
             self._snapshot_post()                           # a predict on its own is about to move x, P
-        self._call(a, rec)
+        self._run(self._step, a, rec)
         if plain:
             self._args_cache[flags] = (self._version, a, keep)      # keep: the tensors `a` points into
         if self.diagnostics and (flags & _lib.BKE_DO_UPDATE):
@@ -707,8 +477,7 @@ class KalmanFilter(object):
         if len(Xs) != len(Ps):
             raise ValueError('length of Xs and Ps must be the same')
         self._flush()
-        n, N = self.dim_x, self.n_filters
-        return _rts(self, Xs, Ps, Fs, Qs, 1, self._single, N, n)
+        return _rts(self, Xs, Ps, Fs, Qs, 1)
 
     def __repr__(self):
         return "KalmanFilter bank (H100): n_filters=%d dim_x=%d dim_z=%d dtype=%s device=%s" % (
@@ -727,22 +496,12 @@ def _missed_log_likelihood(S):
     return torch.where(sign > 0, ll, -math.inf).to(S.dtype)
 
 
-def _rts(kf, Xs, Ps, Fs, Qs, shift, single, N, n):
+def _rts(kf, Xs, Ps, Fs, Qs, shift):
     """Shared body of the two rts_smoother forms: fills bke_rts_args and launches."""
-    dtype, device = kf._dtype, kf._device
+    dtype, device, single, N, n = kf._dtype, kf._device, kf._single, kf.n_filters, kf.dim_x
     is_np = not isinstance(Xs, torch.Tensor)
-    Xt = to_dev(Xs, dtype, device)
-    Pt = to_dev(Ps, dtype, device)
+    Xt, Pt, col = kf._history(Xs, Ps)
     T = Xt.shape[0]
-    col = False
-    if single:
-        col = Xt.dim() == 3 and Xt.shape[-1] == 1
-        Xt = Xt.reshape(T, 1, n)
-        Pt = Pt.reshape(T, 1, n, n)
-    if tuple(Xt.shape) != (T, N, n) or tuple(Pt.shape) != (T, N, n, n):
-        raise ValueError("Xs / Ps must have shapes (T,%d,%d) / (T,%d,%d,%d), got %s / %s"
-                         % (N, n, N, n, n, tuple(Xt.shape), tuple(Pt.shape)))
-    Xt = Xt.contiguous(); Pt = Pt.contiguous()
 
     def model(lst, default, name):
         """-> (tensor, per-filter stride, per-epoch stride)"""
@@ -774,8 +533,7 @@ def _rts(kf, Xs, Ps, Fs, Qs, shift, single, N, n):
     a.Q, a.Q_stride, a.Q_step_stride = ptr(Qt), sQ, tQ
     a.x_out, a.P_out, a.K, a.Pp = ptr(x), ptr(P), ptr(K), ptr(Pp)
     a.status = ptr(status)
-    with torch.cuda.device(device):
-        _lib.check(_lib.load().bke_kf_rts_smoother(a, stream_ptr(device)))
+    kf._run(kf._lib.bke_kf_rts_smoother, a, stream_ptr(device))
     if not single:
         return x, P, K, Pp
     if int(status[0].item()) != 0:
@@ -896,4 +654,4 @@ def rts_smoother(Xs, Ps, Fs, Qs, dtype=np.float64, device=None):
     def per_epoch(m):
         a = np.asarray(m, dtype=np.float64)
         return [a] * T if a.ndim == 2 else list(m)
-    return _rts(kf, Xa, np.asarray(Ps, dtype=np.float64), per_epoch(Fs), per_epoch(Qs), 0, True, 1, n)
+    return _rts(kf, Xa, np.asarray(Ps, dtype=np.float64), per_epoch(Fs), per_epoch(Qs), 0)

@@ -42,22 +42,13 @@ class MMAEFilterBank(object):
         self._x_prior = self._x.clone(); self._P_prior = self._P.clone()
         self._x_post = self._x.clone(); self._P_post = self._P.clone()
 
-    def _vec(self, t):
-        if not self._single:
-            return t
-        v = t[0].cpu().numpy()
-        return v.reshape(-1, 1) if self.filters[0]._x_col else v
-
-    def _mat(self, t):
-        return t if not self._single else t[0].cpu().numpy()
-
-    x = property(lambda self: self._vec(self._x))
-    P = property(lambda self: self._mat(self._P))
-    x_prior = property(lambda self: self._vec(self._x_prior))
-    P_prior = property(lambda self: self._mat(self._P_prior))
-    x_post = property(lambda self: self._vec(self._x_post))
-    P_post = property(lambda self: self._mat(self._P_post))
-    p = property(lambda self: self._mat(self._p))
+    x = property(lambda self: self.filters[0]._vec_out(self._x))
+    P = property(lambda self: self.filters[0]._out(self._P))
+    x_prior = property(lambda self: self.filters[0]._vec_out(self._x_prior))
+    P_prior = property(lambda self: self.filters[0]._out(self._P_prior))
+    x_post = property(lambda self: self.filters[0]._vec_out(self._x_post))
+    P_post = property(lambda self: self.filters[0]._out(self._P_post))
+    p = property(lambda self: self.filters[0]._out(self._p))
 
     def predict(self, u=0):
         """mmae.py:134-153."""

@@ -16,8 +16,8 @@ import numpy as np
 import torch
 
 from .. import _lib
-from .._dev import bke_dtype, ptr, require_cuda, resolve_dtype, stream_ptr, to_dev
-from .kalman_filter import _Linked
+from .._dev import bke_dtype, ptr, stream_ptr, to_dev
+from ._bank import _BankMirror, _model_prop
 
 __all__ = ["SquareRootKalmanFilter"]
 
@@ -26,7 +26,7 @@ def _is_zero_scalar(v):
     return np.isscalar(v) and v == 0
 
 
-class SquareRootKalmanFilter(object):
+class SquareRootKalmanFilter(_BankMirror):
     """``SquareRootKalmanFilter(dim_x, dim_z, dim_u=0)`` for ``n_filters`` filters at once.
 
     Attributes as in the reference: ``x``, ``P``, ``P1_2``, ``Q``, ``Q1_2``, ``R``, ``R1_2``, ``F``, ``H``,
@@ -46,21 +46,10 @@ class SquareRootKalmanFilter(object):
     """
 
     def __init__(self, dim_x, dim_z, dim_u=0, n_filters=None, dtype=np.float64, device=None, diagnostics=True):
-        if dim_x < 1:
-            raise ValueError('dim_x must be 1 or greater')          # square_root.py:128-133
-        if dim_z < 1:
-            raise ValueError('dim_z must be 1 or greater')
         if dim_u < 0:
-            raise ValueError('dim_u must be 0 or greater')
-        self.dim_x, self.dim_z, self.dim_u = int(dim_x), int(dim_z), int(dim_u)
-        self._single = n_filters is None
-        self.n_filters = 1 if self._single else int(n_filters)
-        if self.n_filters < 0:
-            raise ValueError('n_filters must be 0 or greater')
-        self._dtype = resolve_dtype(dtype)
-        self._device = require_cuda(device)
-        self._lib = _lib.load()
-        self.diagnostics = bool(diagnostics)
+            raise ValueError('dim_u must be 0 or greater')          # square_root.py:128-133
+        self._init_bank(dim_x, dim_z, n_filters, dtype, device, diagnostics)
+        self.dim_u = int(dim_u)
         N, n, m = self.n_filters, self.dim_x, self.dim_z
         kw = dict(dtype=self._dtype, device=self._device)
         self._x = torch.zeros(N, n, **kw)
@@ -70,7 +59,6 @@ class SquareRootKalmanFilter(object):
         self._F = torch.eye(n, **kw)
         self._H = torch.zeros(m, n, **kw)
         self._B = None                    # the reference's B = 0.
-        self._x_col = True
         self._pending = None              # the u of a deferred predict
         self._z = None
         if self.diagnostics:
@@ -81,31 +69,6 @@ class SquareRootKalmanFilter(object):
             self._status = torch.zeros(N, dtype=torch.int32, device=self._device)
 
     # ------------------------------------------------------------------ plumbing
-    def _model(self, a, rows, cols, name):
-        """(rows,cols) -> shared; (N,rows,cols) -> per filter; a scalar -> scalar * I."""
-        if np.isscalar(a):
-            if rows != cols:
-                raise ValueError("%s: a scalar needs a square matrix" % name)
-            return torch.eye(rows, dtype=self._dtype, device=self._device) * float(a)
-        t = to_dev(a, self._dtype, self._device)
-        if tuple(t.shape) == (rows, cols) or tuple(t.shape) == (self.n_filters, rows, cols):
-            return t.contiguous()
-        raise ValueError("%s must have shape (%d,%d) or (%d,%d,%d), got %s"
-                         % (name, rows, cols, self.n_filters, rows, cols, tuple(t.shape)))
-
-    @staticmethod
-    def _stride(t):
-        return 0 if t.dim() == 2 else t.shape[1] * t.shape[2]
-
-    def _out(self, t):
-        return t if not self._single else t[0].cpu().numpy()
-
-    def _vec_out(self, t):
-        if not self._single:
-            return t
-        v = t[0].cpu().numpy()
-        return v.reshape(-1, 1) if self._x_col else v
-
     def _cholesky(self, v, k, name):
         """scipy.linalg.cholesky(v, lower=True) of a (k,k) or (N,k,k) value on the device (square_root.py:288,
         :314, :330); raises LinAlgError when a matrix is not positive definite."""
@@ -113,9 +76,8 @@ class SquareRootKalmanFilter(object):
         cnt = 1 if t.dim() == 2 else t.shape[0]
         L = torch.empty_like(t)
         st = torch.zeros(cnt, dtype=torch.int32, device=self._device)
-        with torch.cuda.device(self._device):
-            _lib.check(self._lib.bke_cholesky_lower(cnt, k, bke_dtype(self._dtype), ptr(t), self._stride(t), ptr(L),
-                                                    ptr(st), stream_ptr(self._device)))
+        self._run(self._lib.bke_cholesky_lower, cnt, k, bke_dtype(self._dtype), ptr(t), self._stride(t), ptr(L),
+                  ptr(st), stream_ptr(self._device))
         bad = int((st != 0).sum().item())
         if bad:
             raise np.linalg.LinAlgError("%s: %d of %d matrices are not positive definite" % (name, bad, cnt))
@@ -126,31 +88,6 @@ class SquareRootKalmanFilter(object):
         return torch.matmul(L, L.transpose(-1, -2))
 
     # ------------------------------------------------------------------ state
-    @property
-    def x(self):
-        self._flush()
-        if not self._single:
-            return self._x
-        v = self._x[0].cpu().numpy()
-        return _Linked(v.reshape(-1, 1) if self._x_col else v, self, "x")
-
-    @x.setter
-    def x(self, v):
-        self._flush()
-        n = self.dim_x
-        t = to_dev(v, self._dtype, self._device)
-        if self._single:
-            if tuple(t.shape) not in ((n, 1), (n,)):
-                raise ValueError("x must have shape (%d,1) or (%d,), got %s" % (n, n, tuple(t.shape)))
-            self._x_col = t.dim() == 2
-            self._x = t.reshape(1, n).clone()
-            return
-        if tuple(t.shape) == (n,):
-            t = t.expand(self.n_filters, n)
-        if tuple(t.shape) != (self.n_filters, n):
-            raise ValueError("x must have shape (%d,) or (%d,%d), got %s" % (n, self.n_filters, n, tuple(t.shape)))
-        self._x = t.contiguous().clone()
-
     @property
     def P(self):
         """covariance matrix L L' (square_root.py:290-293)"""
@@ -193,41 +130,8 @@ class SquareRootKalmanFilter(object):
     R1_2 = property(lambda self: self._Lr if not self._single else self._Lr.cpu().numpy(),
                     doc="the lower Cholesky factor of R (read-only)")
 
-    def _matrix_prop(name, rows_attr, cols_attr):  # noqa: N805
-        priv = "_" + name
-
-        def get(self):
-            t = getattr(self, priv)
-            if self._single:
-                return _Linked(t.cpu().numpy(), self, name)
-            self._flush()          # the caller may edit the live tensor: a deferred predict runs with the old one
-            return t
-
-        def set_(self, v):
-            self._flush()
-            setattr(self, priv, self._model(v, getattr(self, rows_attr), getattr(self, cols_attr), name))
-        return property(get, set_)
-
-    F = _matrix_prop("F", "dim_x", "dim_x")
-    H = _matrix_prop("H", "dim_z", "dim_x")
-    del _matrix_prop
-
-    @property
-    def B(self):
-        if self._B is None:
-            return 0.
-        return _Linked(self._B.cpu().numpy(), self, "B") if self._single else self._B
-
-    @B.setter
-    def B(self, v):
-        self._flush()
-        if v is None or _is_zero_scalar(v):
-            self._B = None
-            return
-        if np.isscalar(v):
-            raise NotImplementedError("B must be a (dim_x, dim_u) matrix (or 0): a scalar B is not supported")
-        shp = np.shape(v) if not isinstance(v, torch.Tensor) else tuple(v.shape)
-        self._B = self._model(v, self.dim_x, int(shp[-1]), "B")
+    F = _model_prop("F", "dim_x", "dim_x")
+    H = _model_prop("H", "dim_z", "dim_x")
 
     # ------------------------------------------------------------------ predict / update
     def predict(self, u=0):
@@ -255,16 +159,10 @@ class SquareRootKalmanFilter(object):
             return
         m = self.dim_z
         Lr = self._Lr if R2 is None else self._model(R2, m, m, "R2")
-        zt = to_dev(np.asarray(z, dtype=np.float64).reshape(1, -1) if self._single else z, self._dtype, self._device)
-        if tuple(zt.shape) != (self.n_filters, m):
-            raise ValueError("z must have shape (%d,%d), got %s" % (self.n_filters, m, tuple(zt.shape)))
-        vt = None
-        if valid is not None:
-            vt = torch.as_tensor(valid, device=self._device).to(torch.uint8).contiguous()
-            if tuple(vt.shape) != (self.n_filters,):
-                raise ValueError("valid must have shape (%d,)" % self.n_filters)
+        zt = self._z_rows(z)
+        vt = self._valid_mask(valid)
         flags = _lib.BKE_DO_UPDATE | (_lib.BKE_DO_PREDICT if u is not None else 0)
-        self._launch(flags, u, zt.contiguous(), vt, Lr)
+        self._launch(flags, u, zt, vt, Lr)
         self._z = zt
         if self.diagnostics:
             self._x_post.copy_(self._x)
@@ -301,27 +199,16 @@ class SquareRootKalmanFilter(object):
             if flags & _lib.BKE_DO_UPDATE:
                 a.K, a.y, a.S1_2, a.SI1_2 = ptr(self._K), ptr(self._y), ptr(self._S1_2), ptr(self._SI1_2)
                 a.status = ptr(self._status)
-        with torch.cuda.device(self._device):
-            _lib.check(self._lib.bke_srkf_step(a, stream_ptr(self._device)))
+        self._run(self._lib.bke_srkf_step, a, stream_ptr(self._device))
 
     # ------------------------------------------------------------------ diagnostics
-    def _diag(self, name):
-        if not self.diagnostics:
-            raise AttributeError("%s is only kept when the filter is built with diagnostics=True" % name)
-        self._flush()
-        return getattr(self, "_" + name)
-
-    x_prior = property(lambda self: self._vec_out(self._diag("x_prior")))
-    x_post = property(lambda self: self._vec_out(self._diag("x_post")))
     P_prior = property(lambda self: self._out(self._product(self._diag("L_prior"))))
     P_post = property(lambda self: self._out(self._product(self._diag("L_prior"))),
                       doc="the PRIOR factor's product, as the reference's property returns (square_root.py:300-303)")
-    K = property(lambda self: self._out(self._diag("K")))
     S1_2 = property(lambda self: self._out(self._diag("S1_2")))
     SI1_2 = property(lambda self: self._out(self._diag("SI1_2")))
     S = property(lambda self: self._out(self._product(self._diag("S1_2"))))
     SI = property(lambda self: self._out(torch.matmul(self._diag("SI1_2").transpose(-1, -2), self._SI1_2)))
-    status = property(lambda self: self._diag("status"))
 
     @property
     def y(self):
