@@ -68,7 +68,7 @@ BKE_KF42_MODEL_WORDS = 37
 class KfModelMap(ctypes.Structure):
     _fields_ = [
         ("varying", c_uint64),
-        ("asymmetric", c_int32), ("reserved", c_int32),
+        ("asymmetric", c_int32), ("duplicate", c_uint32),
         ("words", ctypes.c_float * BKE_KF42_MODEL_WORDS),
     ]
 

@@ -218,6 +218,8 @@ int bke_kf_step_packed(const bke_kf_args *args, const void *record, const bke_kf
     if (!host_map) { set_error("host_map is NULL"); return BKE_ERR_BAD_ARG; }
     if (bad_mask(host_map->varying)) { set_error("varying has bits above word %d", BKE_KF42_MODEL_WORDS - 1); return BKE_ERR_BAD_ARG; }
     if (host_map->varying && !record) { set_error("record is NULL"); return BKE_ERR_BAD_ARG; }
+    int plane[BKE_KF42_MODEL_WORDS];
+    if ((rc = kf_model_planes(*host_map, plane))) return rc;
     if ((rc = require_device())) return rc;
     if (args->n_filters == 0) return BKE_OK;
     g_err[0] = '\0';

@@ -40,6 +40,10 @@ int launch_kf_scan_models(int64_t n_filters, const void *F, const void *Q, const
                           bke_kf_model_map *map, cudaStream_t s);
 int launch_kf_pack_models(int64_t n_filters, const void *F, const void *Q, const void *H, const void *R, uint64_t varying,
                           void *record, cudaStream_t s);
+// the record plane each model word of a (host) map is read from: its own slot, or the representative slot of
+// a copy flagged in map.duplicate (plane[e] = -1 for a shared word); BKE_ERR_BAD_ARG (with the error set) when
+// a flagged bit has no representative or lies at or above popcount(varying)
+int kf_model_planes(const bke_kf_model_map &map, int (&plane)[BKE_KF42_MODEL_WORDS]);
 int launch_kf_rowblock(const bke_kf_args &a, cudaStream_t s);
 int launch_kf_direct(const bke_kf_args &a, cudaStream_t s);
 // wgmma covariance propagation for shared-model fp32 banks with dim_x = 16 / 32 (kf_tc.cu); a fused step runs

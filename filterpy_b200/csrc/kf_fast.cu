@@ -21,7 +21,10 @@
 // Such a bank may go further and hand over only the model words that differ between its filters
 // (bke_kf_scan_models + bke_kf_pack_models, REC == 2): one bulk copy per tile brings those planes,
 // and every word the whole bank shares rides in the launch parameters (40 instead of 148 B of
-// models per filter for the kf_bank_cv2d template).
+// models per filter for the kf_bank_cv2d template).  A plane the scan found to be a copy of an earlier
+// plane in every filter (map.duplicate) is not copied: the step reads the earlier plane in its place,
+// so a tile's record comes in one bulk copy per run of consecutive planes the launch reads (20 B per
+// filter for the kf_bank_cv2d template, whose two axes share dt, q and r).
 //
 // Reference arithmetic: filterpy/kalman/kalman_filter.py:471-478, 533-556 (see kf_regtile.cuh).
 #include <stdlib.h>
@@ -56,9 +59,11 @@ constexpr int SYM_Q_PLANES = 10, SYM_PLANES = 13;
 // (bit e of a map's `varying` stands for word e):
 //   F 0..15 (row-major) | Q 16..25 (upper triangle, as above) | H 26..33 (row-major) | R 34..36 (R00 R01 R11).
 // The record holds only the words that differ between filters, tile-major like the one above with
-// k = popcount(varying) planes per tile, so predict reads a prefix of a tile (F, Q) and update a suffix (H, R).
+// k = popcount(varying) planes per tile.  A launch copies only the planes it reads (those of its MODE's words,
+// a copy replaced by its representative) into the same place of the stage, in at most REC_RUNS bulk copies.
 constexpr int WORDS = BKE_KF42_MODEL_WORDS, W_F = 0, W_Q = 16, W_H = 26, W_R = 34;
 constexpr uint64_t PREDICT_WORDS = (1ull << W_H) - 1;      // F and Q
+constexpr int REC_RUNS = (WORDS + 1) / 2;                  // runs of consecutive planes, at most every other one
 
 // REC: 0 = dense models, 1 = the packed Q / R record, 2 = the packed model words (stage sized for all 37)
 template <typename T, int N, int M, bool SHARED = false, int REC = 0>
@@ -140,7 +145,9 @@ struct FastP {
     uint64_t varying;               // REC == 2: bit e set = word e is read from the record...
     int slot_off[WORDS];            // ...at this byte offset into a tile's record (its plane * TILE * 4)
     int rec_planes;                 // REC == 2: planes per tile of the record,
-    int rec_first, rec_copy;        // the first plane this MODE reads and how many it reads
+    int rec_copy;                   // how many of them this launch copies,
+    int rec_runs;                   // in this many runs of consecutive planes:
+    int run_first[REC_RUNS], run_len[REC_RUNS];
 };
 
 // MODE: 3 = predict+update, 1 = predict only, 2 = update only
@@ -204,8 +211,10 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
             if (!REC) load(St::OR_, p.R, M * M, nf * M * M * 4, pol_first);
         }
         if (REC == 1) load(St::OQ + SYM_FIRST * TILE * 4, p.rec + SYM_FIRST * TILE, SYM_PLANES, SYM_BYTES, pol_first);
-        if (REC == 2 && p.rec_copy)
-            load(St::OQ + p.rec_first * TILE * 4, p.rec + p.rec_first * TILE, p.rec_planes, p.rec_copy * TILE * 4, pol_first);
+        if (REC == 2)
+            for (int r = 0; r < p.rec_runs; r++)
+                load(St::OQ + p.run_first[r] * TILE * 4, p.rec + p.run_first[r] * TILE, p.rec_planes,
+                     p.run_len[r] * TILE * 4, pol_first);
         if (DO_U && zb) load(St::OZ, p.z, M, zb, pol_first);
     };
 
@@ -586,6 +595,62 @@ kf42_scan_models_kernel(int64_t n_filters, const float4 *__restrict__ F, const f
     }
 }
 
+// Second scan pass, after kf42_scan_models_kernel on the same stream (which wrote map->varying and
+// map->words): AND into map->duplicate, which the caller set to all ones, the slots s < 32 that have a
+// candidate c(s) (the rule at bke_kf_model_map) and whose word equals the candidate's, as bits, in every
+// filter the block covers.  Each thread keeps its filter's words in its own column of shared memory, so
+// the candidate pairs are read at run-time indices without a local-memory array.
+__global__ void __launch_bounds__(256)
+kf42_scan_duplicates_kernel(int64_t n_filters, const float4 *__restrict__ F, const float4 *__restrict__ Q,
+                            const float4 *__restrict__ H, const float4 *__restrict__ R, bke_kf_model_map *map)
+{
+    __shared__ float col[WORDS][256];
+    __shared__ uint8_t pair_e[32], pair_c[32], pair_s[32];
+    __shared__ int n_pairs;
+    __shared__ uint32_t cand;
+    __shared__ uint32_t red[8];
+    const int tid = threadIdx.x;
+    if (tid == 0) {
+        const uint64_t v = map->varying;
+        int slot_word[32], n = 0;
+        uint32_t c = 0;
+        for (int e = 0, s = 0; e < WORDS && s < 32; e++) {
+            if (!((v >> e) & 1)) continue;
+            slot_word[s] = e;
+            for (int t = 0; t < s; t++)
+                if (__float_as_uint(map->words[slot_word[t]]) == __float_as_uint(map->words[e])) {
+                    pair_e[n] = e; pair_c[n] = slot_word[t]; pair_s[n] = s; n++;
+                    c |= 1u << s;
+                    break;
+                }
+            s++;
+        }
+        n_pairs = n;
+        cand = c;
+    }
+    __syncthreads();
+    const int n = n_pairs;
+    uint32_t differs = 0;
+    if (n) {
+        for (int64_t f = blockIdx.x * (int64_t)blockDim.x + tid; f < n_filters; f += (int64_t)gridDim.x * blockDim.x) {
+            float w[WORDS];
+            bool a;
+            kf42_model_words(F, Q, H, R, f, w, a);
+#pragma unroll
+            for (int e = 0; e < WORDS; e++) col[e][tid] = w[e];
+            for (int i = 0; i < n; i++)
+                differs |= (uint32_t)(__float_as_uint(col[pair_e[i]][tid]) != __float_as_uint(col[pair_c[i]][tid])) << pair_s[i];
+        }
+    }
+    differs = __reduce_or_sync(FULL, differs);
+    if (tid % 32 == 0) red[tid / 32] = differs;
+    __syncthreads();
+    if (tid == 0) {
+        for (int i = 1; i < (int)blockDim.x / 32; i++) differs |= red[i];
+        atomicAnd(&map->duplicate, cand & ~differs);
+    }
+}
+
 // Pack pass: the words in `varying` of every filter slot into the record described at WORDS (the
 // padding of the last tile is written with zeros), one thread per slot.
 __global__ void __launch_bounds__(256)
@@ -668,12 +733,50 @@ int launch_kf_scan_models(int64_t n_filters, const void *F, const void *Q, const
 {
     int rc = check_models(n_filters, F, Q, H, R, map);
     if (rc) return rc;
-    // varying and asymmetric start at zero; filter 0's words are written by the kernel
+    // varying and asymmetric start at zero, duplicate (for a bank of filters) at all ones; filter 0's words
+    // are written by the first kernel
     if (check_cuda(cudaMemsetAsync(map, 0, sizeof(bke_kf_model_map), s), "cudaMemsetAsync")) return BKE_ERR_CUDA;
     if (n_filters == 0) return BKE_OK;
-    kf42_scan_models_kernel<<<(int)pass_grid(n_filters), 256, 0, s>>>(n_filters, (const float4 *)F, (const float4 *)Q,
-                                                                      (const float4 *)H, (const float4 *)R, map);
-    return check_cuda(cudaGetLastError(), "kf42_scan_models_kernel launch");
+    if (check_cuda(cudaMemsetAsync(&map->duplicate, 0xff, sizeof(map->duplicate), s), "cudaMemsetAsync")) return BKE_ERR_CUDA;
+    const int grid = (int)pass_grid(n_filters);
+    kf42_scan_models_kernel<<<grid, 256, 0, s>>>(n_filters, (const float4 *)F, (const float4 *)Q, (const float4 *)H,
+                                                 (const float4 *)R, map);
+    if (check_cuda(cudaGetLastError(), "kf42_scan_models_kernel launch")) return BKE_ERR_CUDA;
+    kf42_scan_duplicates_kernel<<<grid, 256, 0, s>>>(n_filters, (const float4 *)F, (const float4 *)Q, (const float4 *)H,
+                                                     (const float4 *)R, map);
+    return check_cuda(cudaGetLastError(), "kf42_scan_duplicates_kernel launch");
+}
+
+int kf_model_planes(const bke_kf_model_map &map, int (&plane)[WORDS])
+{
+    const int k = __builtin_popcountll(map.varying);
+    if (k < 32 && (map.duplicate >> k) != 0) {
+        set_error("duplicate flags slot %d, but only %d words vary", 31 - __builtin_clz(map.duplicate), k);
+        return BKE_ERR_BAD_ARG;
+    }
+    int slot_word[WORDS];
+    for (int e = 0, s = 0; e < WORDS; e++) {
+        plane[e] = -1;
+        if (!((map.varying >> e) & 1)) continue;
+        slot_word[s] = e;
+        plane[e] = s;
+        if (s < 32 && ((map.duplicate >> s) & 1)) {
+            uint32_t we, wt;
+            memcpy(&we, &map.words[e], 4);
+            int t = 0;
+            for (; t < s; t++) {
+                memcpy(&wt, &map.words[slot_word[t]], 4);
+                if (wt == we) break;
+            }
+            if (t == s) {
+                set_error("duplicate flags slot %d (word %d), but no earlier slot has the same filter-0 word", s, e);
+                return BKE_ERR_BAD_ARG;
+            }
+            plane[e] = t;
+        }
+        s++;
+    }
+    return BKE_OK;
 }
 
 int launch_kf_pack_models(int64_t n_filters, const void *F, const void *Q, const void *H, const void *R, uint64_t varying,
@@ -750,14 +853,26 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const 
             for (int j = i; j < 4; j++, k++) p.Qh[i * 4 + j] = p.Qh[j * 4 + i] = w[k];
         p.Rh[0] = w[W_R]; p.Rh[1] = p.Rh[2] = w[W_R + 1]; p.Rh[3] = w[W_R + 2];
         p.varying = map->varying;
-        for (int e = 0, k = 0; e < WORDS; e++) {
-            p.slot_off[e] = k * TILE * 4;
-            k += (map->varying >> e) & 1;
+        int plane[WORDS];
+        if (int rc = kf_model_planes(*map, plane)) return rc;
+        // the planes this MODE reads, copied in runs of consecutive planes
+        const uint64_t words = map->varying & ((dp ? PREDICT_WORDS : 0) | (du ? ~PREDICT_WORDS : 0));
+        uint64_t read = 0;
+        for (int e = 0; e < WORDS; e++) {
+            p.slot_off[e] = plane[e] < 0 ? 0 : plane[e] * TILE * 4;
+            if ((words >> e) & 1) read |= 1ull << plane[e];
         }
-        const int k_all = __builtin_popcountll(map->varying), k_p = __builtin_popcountll(map->varying & PREDICT_WORDS);
-        p.rec_planes = k_all;
-        p.rec_first = dp ? 0 : k_p;
-        p.rec_copy = (du ? k_all : k_p) - p.rec_first;
+        p.rec_planes = __builtin_popcountll(map->varying);
+        p.rec_copy = __builtin_popcountll(read);
+        p.rec_runs = 0;
+        for (int k = 0; k < p.rec_planes; k++) {
+            if (!((read >> k) & 1)) continue;
+            if (k == 0 || !((read >> (k - 1)) & 1)) {
+                p.run_first[p.rec_runs] = k;
+                p.run_len[p.rec_runs++] = 0;
+            }
+            p.run_len[p.rec_runs - 1]++;
+        }
     }
     const bool extras = a.x_prior || a.P_prior || a.K || a.y || a.S || a.SI || a.log_likelihood || a.status;
 

@@ -152,7 +152,13 @@ int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream);
  *                               some filter differs from filter 0's in any bit (-0.0 against +0.0 and two
  *                               NaN payloads differ), `words` are filter 0's, `asymmetric` is 1 when a
  *                               filter's Q or R differs from its transpose in any bit (the record may only
- *                               be used when it is 0);
+ *                               be used when it is 0).  With v_0 < v_1 < ... the varying words (slot s
+ *                               of the record holds word v_s), let c(s) be the lowest slot t < s whose
+ *                               filter-0 word has the same bits as v_s's; bit s (s < 32) of `duplicate`
+ *                               is set when c(s) exists and word v_s equals word v_c(s) bit for bit in
+ *                               every filter, so plane s is a copy of plane c(s) (which is never flagged
+ *                               itself).  The rule is conservative: a copy it misses is read from its own
+ *                               plane.  A zero `duplicate` means "no copies";
  *   bke_kf_packed_models_bytes  the size of the record of n_filters filters for a `varying` mask (0 for a
  *                               mask with bits above 36); the caller allocates it, 16-byte aligned;
  *   bke_kf_pack_models          fills the record: one tile of 128 filters after the other, each tile
@@ -162,14 +168,19 @@ int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream);
  *   bke_kf_step_packed          bke_kf_step with the record and a HOST copy of the map standing in for
  *                               args->F, Q, H and R (which must still be the per-filter arrays they were
  *                               scanned and packed from, unchanged since); the results are bit-identical
- *                               to bke_kf_step's.  The record may be NULL when no word varies.
+ *                               to bke_kf_step's.  The record may be NULL when no word varies.  A plane
+ *                               flagged in the map's `duplicate` is not read: the step reads its
+ *                               representative plane c(s) instead (40 -> 20 B of models per filter for the
+ *                               constant-velocity bank above, which has the same dt, q and r on both
+ *                               axes).  A `duplicate` bit at or above popcount(varying), or whose slot has
+ *                               no c(s), is refused with BKE_ERR_BAD_ARG.
  * The calls return BKE_ERR_UNSUPPORTED for other shapes, dtypes, shared models, an asymmetric map,
  * misaligned pointers, and when the environment sets BKE_KF_SYM=0; bke_kf_step is then the call to make. */
 #define BKE_KF42_MODEL_WORDS 37
 typedef struct bke_kf_model_map {
     uint64_t varying;                       /* bit e: word e differs between filters */
     int32_t asymmetric;                     /* 1: some Q or R is not exactly symmetric */
-    int32_t reserved;
+    uint32_t duplicate;                     /* bit s: plane s is a copy of plane c(s) in every filter */
     float words[BKE_KF42_MODEL_WORDS];      /* filter 0's words */
 } bke_kf_model_map;
 

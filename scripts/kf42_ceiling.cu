@@ -5,7 +5,9 @@
 // written.  With mode 1, Q and R are replaced by one stream of 52 B per filter (the packed upper
 // triangles a symmetric bank's step reads, bke_kf_pack_sym_models): 236 B read, 316 B in all.  With
 // mode 2, F, Q, H and R are replaced by one stream of 40 B per filter (the 10 model words that differ
-// between the filters of the bench bank, bke_kf_pack_models): 128 B read, 208 B in all.
+// between the filters of the bench bank, bke_kf_pack_models): 128 B read, 208 B in all.  With mode 3,
+// that stream is 20 B per filter (the 5 distinct planes among those 10 words, the planes the step reads
+// when the scan has flagged the copies): 108 B read, 188 B in all.
 // Every array is read and written with flat, fully coalesced 16-byte accesses.  A CTA of
 // 256 threads covers 64 filters: every thread moves one 16-byte chunk of P, F, Q, the first 128
 // threads one of H, the first 64 one of x and R, the first 32 one of z, so the read/write mix is the
@@ -21,6 +23,7 @@ constexpr int CHUNK = 64;           // filters per CTA iteration
 constexpr int THREADS = 256;        // = CHUNK * 64 B / 16 B
 constexpr int SYM_CHUNKS = CHUNK * 52 / 16;     // 16-byte chunks of the packed Q / R stream per CTA iteration
 constexpr int WORD_CHUNKS = CHUNK * 40 / 16;    // 16-byte chunks of the packed model-word stream per CTA iteration
+constexpr int DISTINCT_CHUNKS = CHUNK * 20 / 16;    // the same for its distinct planes only
 
 __global__ void __launch_bounds__(THREADS)
 kf42_traffic_kernel(float4 *x, float4 *P, const float4 *F, const float4 *Q, const float4 *H, const float4 *R,
@@ -33,6 +36,8 @@ kf42_traffic_kernel(float4 *x, float4 *P, const float4 *F, const float4 *Q, cons
         float4 vh = make_float4(0.f, 0.f, 0.f, 0.f), vf = vh, vq = vh, vx = vh, vr = vh, vz = vh;
         if (mode == 2) {
             if (t < WORD_CHUNKS) vq = __ldg(Q + c * WORD_CHUNKS + t);
+        } else if (mode == 3) {
+            if (t < DISTINCT_CHUNKS) vq = __ldg(Q + c * DISTINCT_CHUNKS + t);
         } else {
             vf = __ldg(F + p16);
             if (mode == 1) {
@@ -62,7 +67,7 @@ kf42_traffic_kernel(float4 *x, float4 *P, const float4 *F, const float4 *Q, cons
 extern "C" {
 
 // One launch over n_filters (a multiple of 64); returns a cudaError_t.  mode 1: Q is the 52 B-per-filter
-// stream and R is not read; mode 2: Q is the 40 B-per-filter stream and F, H, R are not read.
+// stream and R is not read; mode 2 (3): Q is the 40 (20) B-per-filter stream and F, H, R are not read.
 int kf42_traffic(void *x, void *P, const void *F, const void *Q, const void *H, const void *R, const void *z,
                  int64_t n_filters, int grid, int mode, void *stream)
 {

@@ -13,11 +13,13 @@ Prints JSON lines (and writes them to DIR/kf42_ceiling.jsonl with --out):
              bank's step reads instead (bke_kf_pack_sym_models): 316 B per filter
   ceiling_words  the same twin with F, Q, H and R replaced by one 40 B-per-filter stream, the 10 model
              words that differ between the filters of the bench bank (bke_kf_pack_models): 208 B
+  ceiling_distinct  the same twin with that stream cut to 20 B per filter, the 5 distinct planes
+             among those 10 words (the step does not read a plane the scan flags as a copy): 188 B
   step       the shipped step (KalmanFilter.predict + update, per-filter F/H/Q/R) replayed as CUDA
              graphs of 4 steps like bench.py, at N = 2^19 .. 2^22 (all above the bound under which
              the L2 hints are used); per-step time and GB/s for every N, counted with the bytes the
-             step moves (4 * popcount(varying) + 168 when it reads the packed model words, 208 for
-             the bench bank; 344 with BKE_KF_SYM=0)
+             step moves (168 + 4 per distinct plane of the packed model words, i.e. per varying word
+             not flagged in the map's `duplicate`: 188 for the bench bank; 344 with BKE_KF_SYM=0)
   fit        t(N) = a + b N over those sizes: a is the fixed cost of a step, bytes / b its
              streaming rate
   shared     the same graph of 4 steps for a 2^20-filter bank whose F/H/Q/R are shared (one model
@@ -45,6 +47,7 @@ LIB = os.path.join(HERE, "kf42_ceiling.so")
 BYTES = 344                 # per filter-step: x, P, F, Q, H, R, z read (264 B), x, P written (80 B)
 BYTES_SYM = 316             # the same with Q and R read as their packed upper triangles (52 B instead of 80)
 BYTES_WORDS = 208           # the same with F, Q, H, R read as the 10 varying words of the bench bank (40 B instead of 176)
+BYTES_DISTINCT = 188        # the same with only the 5 distinct planes among those words read (20 B)
 PEAK_GBS = 3350.0           # H100 SXM data sheet, HBM3
 RING = 4                    # steps per graph replay, as in bench.py
 
@@ -93,7 +96,7 @@ def ceiling(torch, rounds, mode=0):
     g = torch.Generator(device=dev).manual_seed(5)
     arr = {k: torch.randn(N * e, device=dev, generator=g) for k, e in
            (("x", 4), ("P", 16), ("F", 16), ("Q", 16), ("H", 8), ("R", 4), ("z", 2))}
-    nbytes = (BYTES, BYTES_SYM, BYTES_WORDS)[mode]
+    nbytes = (BYTES, BYTES_SYM, BYTES_WORDS, BYTES_DISTINCT)[mode]
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
     stream = torch.cuda.current_stream().cuda_stream
     out = {}
@@ -110,7 +113,7 @@ def ceiling(torch, rounds, mode=0):
         gbs = nbytes * N / (ms * 1e-3) / 1e9
         out["ctas_per_sm_%d" % per_sm] = {"ms": ms, "GBps": gbs, "frac_of_3350": gbs / PEAK_GBS}
     best = max(out.values(), key=lambda v: v["GBps"])
-    return {"what": ("ceiling", "ceiling_sym", "ceiling_words")[mode], "n_filters": N, "bytes_per_filter": nbytes, "ms": best["ms"],
+    return {"what": ("ceiling", "ceiling_sym", "ceiling_words", "ceiling_distinct")[mode], "n_filters": N, "bytes_per_filter": nbytes, "ms": best["ms"],
             "GBps": best["GBps"],
             "frac_of_3350": best["frac_of_3350"], "by_grid": out}
 
@@ -154,6 +157,7 @@ def main():
     lines.append(ceiling(torch, args.rounds))
     lines.append(ceiling(torch, args.rounds, mode=1))
     lines.append(ceiling(torch, args.rounds, mode=2))
+    lines.append(ceiling(torch, args.rounds, mode=3))
     sizes, times = [], []
     moved = BYTES
     for lg in (19, 20, 21, 22):
@@ -163,7 +167,11 @@ def main():
         ms = float(np.median(t))
         sizes.append(N); times.append(ms)
         packed = kf._sym_state is not None and kf._sym_state[1]
-        moved = 168 + 4 * bin(kf._sym_host_map.varying).count("1") if packed else BYTES
+        if packed:
+            hm = kf._sym_host_map
+            moved = 168 + 4 * (bin(hm.varying).count("1") - bin(hm.duplicate).count("1"))
+        else:
+            moved = BYTES
         lines.append({"what": "step", "n_filters": N, "packed_words": packed, "bytes_per_filter": moved, "ms": ms,
                       "ms_rounds": t, "GBps": moved * N / (ms * 1e-3) / 1e9})
         del kf, graph

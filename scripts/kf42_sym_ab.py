@@ -1,6 +1,7 @@
 """A/B of the 4/2 fp32 bank step with its models read dense (344 B per filter-step) or as the packed
-model words that differ between the filters (208 B on the bench bank), against the parent's packed
-upper triangles of Q and R (316 B), and the one-time cost of scanning and packing the models.
+model words that differ between the filters, each distinct plane read once (188 B on the bench bank,
+whose 10 varying words hold 5 distinct planes), against another checkout (e.g. the parent commit), and
+the one-time cost of scanning and packing the models.
 
     python scripts/kf42_sym_ab.py [--out DIR] [--rounds R] [--steps 400,50] [--diag-rounds D]
                                   [--baseline-tree DIR]
@@ -9,8 +10,8 @@ Prints JSON lines (and writes them to DIR/kf42_sym_ab.jsonl with --out):
 
   card     name, power limit and maximum SM clock (read-only nvidia-smi query)
   pack     device time of bke_kf_scan_models + bke_kf_pack_models for the 2^20-filter bench bank (CUDA
-           events, median of rounds of 20 calls), with the bytes they move (176 B read twice, 40 B
-           written per filter)
+           events, median of rounds of 20 calls), with the bytes they move (176 B read three times:
+           the two scan passes and the pack; 40 B written per filter)
   all_words  device time of one step of a 2^20-filter bank whose 37 model words all vary (316 B either
            way): bke_kf_step_packed against bke_kf_step_sym, alternated (the cost of the per-word select)
   run      one `bench.py --no-cpu --no-extra --no-resample --steps K` per arm and round: ms_per_step
@@ -85,7 +86,7 @@ def pack_cost(rounds):
         torch.cuda.synchronize()
         ms.append(e0.elapsed_time(e1) / reps)
     med = float(np.median(ms))
-    moved = N * (2 * 176 + 4 * k)
+    moved = N * (3 * 176 + 4 * k)
     return {"what": "pack", "n_filters": N, "varying_words": k, "symmetric": hmap.asymmetric == 0, "ms": med,
             "ms_rounds": ms, "bytes": moved, "GBps": moved / (med * 1e-3) / 1e9}
 
