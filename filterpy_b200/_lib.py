@@ -32,6 +32,7 @@ EXPORTED_SYMBOLS = [
     "bke_ukf_model_compile", "bke_ukf_model_log", "bke_ukf_model_registers", "bke_ukf_model_free", "bke_ukf_step_model",
     "bke_debug_ukf_model_cubin_bytes", "bke_ukf_rts_smoother_model",
     "bke_ckf_step", "bke_ckf_model_compile", "bke_ckf_step_model", "bke_debug_ckf_model_cubin_bytes",
+    "bke_enkf_initialize", "bke_enkf_step", "bke_enkf_model_compile", "bke_enkf_step_model", "bke_debug_enkf_model_cubin_bytes",
     "bke_srkf_step", "bke_cholesky_lower",
     "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
     "bke_residual_workspace_bytes", "bke_residual_prepare", "bke_searchsorted_bracket_sweep",
@@ -137,6 +138,29 @@ class CkfArgs(ctypes.Structure):
         ("log_likelihood", c_void_p),
         ("status", c_void_p),
         ("sigmas_f", c_void_p),
+    ]
+
+
+class EnkfArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_filters", c_int64),
+        ("dim_x", c_int32), ("dim_z", c_int32),
+        ("n_members", c_int32),
+        ("dtype", c_int32), ("flags", c_uint32),
+        ("fx_model", c_int32), ("hx_model", c_int32),
+        ("seed", c_uint32), ("counter", c_uint32), ("reserved", c_uint32),
+        ("dt", c_double),
+        ("x", c_void_p), ("P", c_void_p),
+        ("x_out", c_void_p), ("P_out", c_void_p),
+        ("sigmas", c_void_p), ("sigmas_out", c_void_p),
+        ("Q", c_void_p), ("Q_stride", c_int64),
+        ("R", c_void_p), ("R_stride", c_int64),
+        ("F", c_void_p), ("F_stride", c_int64),
+        ("H", c_void_p), ("H_stride", c_int64),
+        ("z", c_void_p), ("z_valid", c_void_p),
+        ("x_prior", c_void_p), ("P_prior", c_void_p),
+        ("K", c_void_p), ("S", c_void_p), ("SI", c_void_p),
+        ("status", c_void_p),
     ]
 
 
@@ -334,6 +358,18 @@ def load():
     lib.bke_ckf_step_model.restype = ctypes.c_int
     lib.bke_debug_ckf_model_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p]
     lib.bke_debug_ckf_model_cubin_bytes.restype = c_size_t
+    lib.bke_enkf_initialize.argtypes = [c_int64, c_int32, c_int32, c_int32, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p]
+    lib.bke_enkf_initialize.restype = ctypes.c_int
+    lib.bke_enkf_step.argtypes = [ctypes.POINTER(EnkfArgs), c_void_p]
+    lib.bke_enkf_step.restype = ctypes.c_int
+    lib.bke_enkf_model_compile.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p,
+                                           ctypes.POINTER(c_void_p)]
+    lib.bke_enkf_model_compile.restype = ctypes.c_int
+    lib.bke_enkf_step_model.argtypes = [ctypes.POINTER(EnkfArgs), c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]
+    lib.bke_enkf_step_model.restype = ctypes.c_int
+    lib.bke_debug_enkf_model_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p]
+    lib.bke_debug_enkf_model_cubin_bytes.restype = c_size_t
     lib.bke_srkf_step.argtypes = [ctypes.POINTER(SrkfArgs), c_void_p]
     lib.bke_srkf_step.restype = ctypes.c_int
     lib.bke_cholesky_lower.argtypes = [c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]

@@ -313,6 +313,35 @@ int bke_ckf_step(const bke_ckf_args *args, void *stream)
     return launch_ckf(a, (cudaStream_t)stream);
 }
 
+int bke_enkf_step(const bke_enkf_args *args, void *stream)
+{
+    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    const bke_enkf_args &a = *args;
+    int rc = validate_enkf(a);
+    if (rc) return rc;
+    if (a.hx_model == BKE_HX_RANGE_AZ_EL && !(a.dim_x == 6 && a.dim_z == 3)) { set_error("BKE_HX_RANGE_AZ_EL needs dim_x=6, dim_z=3"); return BKE_ERR_BAD_ARG; }
+    if (a.hx_model == BKE_HX_RANGE_BEARING && !(a.dim_x == 4 && a.dim_z == 2)) { set_error("BKE_HX_RANGE_BEARING needs dim_x=4, dim_z=2"); return BKE_ERR_BAD_ARG; }
+    if (a.fx_model < 0 || a.fx_model > BKE_FX_CONST_VEL || a.hx_model < 0 || a.hx_model > BKE_HX_RANGE_BEARING) {
+        set_error("unknown fx/hx model id"); return BKE_ERR_BAD_ARG;
+    }
+    if ((rc = require_device())) return rc;
+    if (a.n_filters == 0) return BKE_OK;
+    return launch_enkf(a, (cudaStream_t)stream);
+}
+
+int bke_enkf_initialize(int64_t n_filters, int32_t dim_x, int32_t n_members, int32_t dtype, uint32_t seed, uint32_t counter,
+                        const void *x, const void *P, void *sigmas, int32_t *status, void *stream)
+{
+    if (n_filters < 0 || dim_x < 1 || dim_x > 16) { set_error("bke_enkf_initialize: n_filters >= 0 and 1 <= dim_x <= 16"); return BKE_ERR_BAD_ARG; }
+    if (n_members < 2 || n_members > (1 << 24)) { set_error("bke_enkf_initialize: 2 <= n_members <= 2^24"); return BKE_ERR_BAD_ARG; }
+    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (!x || !P || !sigmas) { set_error("x, P and sigmas must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    int rc = require_device();
+    if (rc) return rc;
+    if (n_filters == 0) return BKE_OK;
+    return launch_enkf_init(n_filters, dim_x, n_members, dtype, seed, counter, x, P, sigmas, status, (cudaStream_t)stream);
+}
+
 int bke_srkf_step(const bke_srkf_args *args, void *stream)
 {
     int rc = validate_srkf(args);

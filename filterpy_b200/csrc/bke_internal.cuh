@@ -58,6 +58,10 @@ int launch_fls(const bke_fls_args &a, cudaStream_t s);
 int launch_ukf(const bke_ukf_args &a, cudaStream_t s);
 int validate_ckf(const bke_ckf_args &a);
 int launch_ckf(const bke_ckf_args &a, cudaStream_t s);
+int validate_enkf(const bke_enkf_args &a);
+int launch_enkf(const bke_enkf_args &a, cudaStream_t s);
+int launch_enkf_init(int64_t n_filters, int32_t dim_x, int32_t n_members, int32_t dtype, uint32_t seed, uint32_t counter,
+                     const void *x, const void *P, void *sigmas, int32_t *status, cudaStream_t s);
 int launch_srkf(const bke_srkf_args &a, cudaStream_t s);
 int launch_cholesky_lower(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *L,
                           int32_t *status, cudaStream_t s);

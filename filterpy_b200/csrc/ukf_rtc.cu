@@ -7,7 +7,9 @@
 // for sm_90a with NVRTC (libnvrtc is dlopen'ed: libbke.so does not link it), loads the cubin with
 // cudaLibraryLoadData and launches the resulting cudaKernel_t like any other kernel.  No CPU path.
 // bke_ckf_model_compile does the same around the cubature kernel (ckf_kernel.cuh, CubatureKalmanFilter.py:
-// 314-321, 354-363); the handle records its family and each step entry point refuses the other's.
+// 314-321, 354-363), and bke_enkf_model_compile around the ensemble kernel (enkf_kernel.cuh,
+// ensemble_kalman_filter.py:250-251, 279-280); the handle records its family and each step entry point
+// refuses the others'.
 //
 // Program text handed to NVRTC (the user's part between the markers):
 //     typedef double real;                       // or float
@@ -23,11 +25,12 @@
 #include <string>
 #include <vector>
 #include "ckf_launch.cuh"
+#include "enkf_launch.cuh"
 #include "ukf_launch.cuh"
 #include "ukf_rts_launch.cuh"
 
 // the filter family a compiled model's kernels belong to
-enum { BKE_FAMILY_UKF = 0, BKE_FAMILY_CKF = 1 };
+enum { BKE_FAMILY_UKF = 0, BKE_FAMILY_CKF = 1, BKE_FAMILY_ENKF = 2 };
 
 struct bke_ukf_model {
     int family;
@@ -86,6 +89,11 @@ Nvrtc *nvrtc()
 std::string kernel_name(const bke_ukf_model &m, int occ, bool extras)
 {
     char buf[256];
+    if (m.family == BKE_FAMILY_ENKF) {        // no occupancy parameter: one warp per filter
+        snprintf(buf, sizeof buf, "bke::enkfk::enkf_kernel<real, %d, %d, %d, %d, %s>", m.n, m.m, m.fx_model, m.hx_model,
+                 extras ? "true" : "false");
+        return buf;
+    }
     snprintf(buf, sizeof buf, "%s<real, %d, %d, %d, %d, %d, %s>", m.family == BKE_FAMILY_CKF ? "bke::ckfk::ckf_kernel" : "bke::ukfk::ukf_kernel",
              m.n, m.m, m.fx_model, m.hx_model, occ, extras ? "true" : "false");
     return buf;
@@ -126,6 +134,22 @@ int launch_ckf_model(const bke_ckf_args &a, const bke_ukf_model &m, const void *
     return BKE_OK;
 }
 
+template <typename T>
+int launch_enkf_model(const bke_enkf_args &a, const bke_ukf_model &m, const void *fx_args, int64_t s_fx, const void *hx_args, int64_t s_hx,
+                      cudaStream_t s)
+{
+    enkfk::EnkfP<T> p;
+    enkf_fill_params<T>(a, p);
+    p.fx_args = (const T *)fx_args; p.s_fx_args = s_fx;
+    p.hx_args = (const T *)hx_args; p.s_hx_args = s_hx;
+    const size_t smem = enkf_smem_bytes(m.n, a.n_members, sizeof(T));
+    const void *kern = (const void *)m.kern[enkf_has_extras(a) ? 1 : 0];
+    if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
+    void *params[] = {&p};
+    if (check_cuda(cudaLaunchKernel(kern, dim3(enkf_grid(p.N)), dim3(enkfk::EB), params, smem, s), "enkf model launch")) return BKE_ERR_CUDA;
+    return BKE_OK;
+}
+
 }  // namespace
 }  // namespace bke
 
@@ -139,12 +163,12 @@ extern "C" {
 static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
                          const char *include_dirs, std::vector<char> &cubin, std::string (&lowered)[3], std::string &log)
 {
-    const bool ckf = family == BKE_FAMILY_CKF;
-    const char *fn = ckf ? "bke_ckf_model_compile" : "bke_ukf_model_compile";
+    const bool ckf = family == BKE_FAMILY_CKF, enkf = family == BKE_FAMILY_ENKF;
+    const char *fn = enkf ? "bke_enkf_model_compile" : ckf ? "bke_ckf_model_compile" : "bke_ukf_model_compile";
     if (dim_x < 1 || dim_x > 16 || dim_z < 1 || dim_z > dim_x + 8) { set_error("%s: 1 <= dim_x <= 16, 1 <= dim_z", fn); return BKE_ERR_BAD_ARG; }
     if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
     const bool ufx = fx_model == BKE_FX_USER, uhx = hx_model == BKE_HX_USER;
-    if (!ufx && !uhx) { set_error("%s: neither fx nor hx is BKE_*_USER (use %s)", fn, ckf ? "bke_ckf_step" : "bke_ukf_step"); return BKE_ERR_BAD_ARG; }
+    if (!ufx && !uhx) { set_error("%s: neither fx nor hx is BKE_*_USER (use %s)", fn, enkf ? "bke_enkf_step" : ckf ? "bke_ckf_step" : "bke_ukf_step"); return BKE_ERR_BAD_ARG; }
     if ((!ufx && fx_model != BKE_FX_LINEAR && fx_model != BKE_FX_CONST_VEL) || (!uhx && hx_model != BKE_HX_LINEAR)) {
         set_error("%s: the built-in partner of a user function must be BKE_FX_LINEAR / BKE_FX_CONST_VEL / BKE_HX_LINEAR", fn);
         return BKE_ERR_BAD_ARG;
@@ -157,7 +181,7 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     std::string text;
     text += dtype == BKE_F64 ? "typedef double real;\n" : "typedef float real;\n";
     text += "#define BKE_DIM_X " + std::to_string(dim_x) + "\n#define BKE_DIM_Z " + std::to_string(dim_z) + "\n";
-    text += ckf ? "#include \"ckf_kernel.cuh\"\n" : "#include \"ukf_kernel.cuh\"\n#include \"ukf_rts_kernel.cuh\"\n";
+    text += enkf ? "#include \"enkf_kernel.cuh\"\n" : ckf ? "#include \"ckf_kernel.cuh\"\n" : "#include \"ukf_kernel.cuh\"\n#include \"ukf_rts_kernel.cuh\"\n";
     text += "#line 1 \"user_model.cu\"\n";
     text += source;
     text += "\n#line 1 \"bke_glue.cu\"\nnamespace bke { namespace ukfk {\n";
@@ -165,11 +189,11 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     if (uhx) text += "template <> __device__ __forceinline__ void bke_user_hx<real>(const real *x, real *z, const real *args) { ::hx(x, z, args); }\n";
     text += "} }\n";
 
-    const int occ = ckf ? ckf_occupancy(dim_x, dtype == BKE_F64) : ukf_occupancy(dim_x, dtype == BKE_F64);
+    const int occ = enkf ? 0 : ckf ? ckf_occupancy(dim_x, dtype == BKE_F64) : ukf_occupancy(dim_x, dtype == BKE_F64);
     bke_ukf_model tmp;
     tmp.family = family; tmp.n = dim_x; tmp.m = dim_z; tmp.fx_model = fx_model; tmp.hx_model = hx_model;
     nvrtcProgram prog;
-    nvrtcResult r = rt->create(&prog, text.c_str(), ckf ? "bke_ckf_user.cu" : "bke_ukf_user.cu", 0, nullptr, nullptr);
+    nvrtcResult r = rt->create(&prog, text.c_str(), enkf ? "bke_enkf_user.cu" : ckf ? "bke_ckf_user.cu" : "bke_ukf_user.cu", 0, nullptr, nullptr);
     if (r != NVRTC_SUCCESS) { set_error("nvrtcCreateProgram: %s", rt->errstr(r)); return BKE_ERR_CUDA; }
     std::vector<std::string> opts = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "-default-device"};     // (bke.h declares the host C-ABI)
     {
@@ -185,7 +209,7 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     std::vector<const char *> copts;
     for (auto &o : opts) copts.push_back(o.c_str());
     // the step kernel with / without the optional outputs and, around a user fx, the RTS smoother
-    const bool with_rts = !ckf && ufx && dim_x <= UR_MAXN;
+    const bool with_rts = !ckf && !enkf && ufx && dim_x <= UR_MAXN;
     const int n_names = with_rts ? 3 : 2;
     const std::string names[3] = {kernel_name(tmp, occ, false), kernel_name(tmp, occ, true), "bke::ukf_rts_kernel<real, true>"};
     for (int i = 0; i < n_names; i++) rt->add_name(prog, names[i].c_str());
@@ -195,7 +219,7 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     log.clear();
     if (lsz > 1) { log.resize(lsz); rt->log(prog, &log[0]); }
     if (r != NVRTC_SUCCESS) {
-        set_error("NVRTC could not compile the %s model: %s\n%s", ckf ? "CKF" : "UKF", rt->errstr(r), log.c_str());
+        set_error("NVRTC could not compile the %s model: %s\n%s", enkf ? "EnKF" : ckf ? "CKF" : "UKF", rt->errstr(r), log.c_str());
         rt->destroy(&prog);
         return BKE_ERR_BAD_ARG;
     }
@@ -253,6 +277,12 @@ int bke_ukf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t f
     return model_compile(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, out);
 }
 
+int bke_enkf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+                           const char *include_dirs, bke_ukf_model **out)
+{
+    return model_compile(BKE_FAMILY_ENKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, out);
+}
+
 int bke_ckf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
                           const char *include_dirs, bke_ukf_model **out)
 {
@@ -279,6 +309,12 @@ size_t bke_debug_ckf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dty
                                        const char *include_dirs)
 {
     return cubin_bytes(BKE_FAMILY_CKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs);
+}
+
+size_t bke_debug_enkf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+                                        const char *include_dirs)
+{
+    return cubin_bytes(BKE_FAMILY_ENKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs);
 }
 
 const char *bke_ukf_model_log(const bke_ukf_model *m) { return m ? m->log.c_str() : ""; }
@@ -356,6 +392,25 @@ int bke_ckf_step_model(const bke_ckf_args *args, const bke_ukf_model *model, con
     if (a.n_filters == 0) return BKE_OK;
     return a.dtype == BKE_F32 ? launch_ckf_model<float>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream)
                               : launch_ckf_model<double>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream);
+}
+
+int bke_enkf_step_model(const bke_enkf_args *args, const bke_ukf_model *model, const void *fx_args, int64_t fx_args_stride,
+                        const void *hx_args, int64_t hx_args_stride, void *stream)
+{
+    if (!args || !model) { set_error("args / model is NULL"); return BKE_ERR_BAD_ARG; }
+    const bke_enkf_args &a = *args;
+    if (model->family != BKE_FAMILY_ENKF) { set_error("bke_enkf_step_model: the model was not compiled for the EnKF (bke_enkf_model_compile)"); return BKE_ERR_BAD_ARG; }
+    if (a.dim_x != model->n || a.dim_z != model->m || a.dtype != model->dtype || a.fx_model != model->fx_model || a.hx_model != model->hx_model) {
+        set_error("bke_enkf_step_model: args (dim_x=%d dim_z=%d dtype=%d fx=%d hx=%d) do not match the compiled model (%d %d %d %d %d)",
+                  a.dim_x, a.dim_z, a.dtype, a.fx_model, a.hx_model, model->n, model->m, model->dtype, model->fx_model, model->hx_model);
+        return BKE_ERR_BAD_ARG;
+    }
+    int rc = validate_enkf(a);
+    if (rc) return rc;
+    if (fx_args_stride < 0 || hx_args_stride < 0) { set_error("negative args stride"); return BKE_ERR_BAD_ARG; }
+    if (a.n_filters == 0) return BKE_OK;
+    return a.dtype == BKE_F32 ? launch_enkf_model<float>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream)
+                              : launch_enkf_model<double>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream);
 }
 
 }  // extern "C"

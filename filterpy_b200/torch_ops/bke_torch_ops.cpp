@@ -5,6 +5,7 @@
 //   bke::kf_predict           bke_kf_step (predict)    kalman_filter.py:437-482
 //   bke::ukf_step             bke_ukf_step             UnscentedKalmanFilter.predict + update, UKF.py:364-491
 //   bke::ckf_step             bke_ckf_step             CubatureKalmanFilter.predict + update, CubatureKalmanFilter.py:292-389
+//   bke::enkf_step            bke_enkf_step            EnsembleKalmanFilter.predict + update, ensemble_kalman_filter.py:218-290
 //   bke::srkf_step            bke_srkf_step            SquareRootKalmanFilter.predict + update, square_root.py:172-248
 //   bke::fls_smooth_batch     bke_fls_smooth           FixedLagSmoother.smooth_batch, fixed_lag_smoother.py:217-311
 //   bke::systematic_resample  bke_systematic_resample  monte_carlo/resampling.py:117-150
@@ -131,6 +132,38 @@ std::tuple<at::Tensor, at::Tensor> ckf_step(const at::Tensor &x, const at::Tenso
     return std::make_tuple(x_out, P_out);
 }
 
+// one fused EnKF epoch on sigmas[N, members, n]; the caller owns the noise stream's (seed, counter) and
+// advances counter by 2 per call (a predict and an update draw)
+std::tuple<at::Tensor, at::Tensor, at::Tensor> enkf_step(const at::Tensor &x, const at::Tensor &P, const at::Tensor &sigmas,
+                                                         const at::Tensor &Q, const at::Tensor &R, const at::Tensor &z, double dt,
+                                                         int64_t fx_model, int64_t hx_model, int64_t seed, int64_t counter,
+                                                         const c10::optional<at::Tensor> &F, const c10::optional<at::Tensor> &H)
+{
+    TORCH_CHECK(x.is_cuda() && P.is_cuda() && x.is_contiguous() && P.is_contiguous() && x.dim() == 2 && P.dim() == 3, "bke: x is [N, n], P is [N, n, n] on the GPU");
+    TORCH_CHECK(sigmas.is_cuda() && sigmas.is_contiguous() && sigmas.dim() == 3 && sigmas.size(0) == x.size(0) && sigmas.size(2) == x.size(1)
+                && sigmas.scalar_type() == x.scalar_type(), "bke: sigmas is [N, members, n] of the state's dtype");
+    TORCH_CHECK(seed >= 0 && seed <= 0xffffffffLL && counter >= 0 && counter <= 0xffffffffLL, "bke: seed and counter are uint32");
+    c10::cuda::CUDAGuard guard(x.device());
+    const int64_t N = x.size(0), n = x.size(1), m = z.size(1);
+    bke_enkf_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_filters = N; a.dim_x = (int32_t)n; a.dim_z = (int32_t)m; a.n_members = (int32_t)sigmas.size(1); a.dtype = dtype_of(x);
+    a.flags = BKE_DO_PREDICT | BKE_DO_UPDATE; a.fx_model = (int32_t)fx_model; a.hx_model = (int32_t)hx_model;
+    a.seed = (uint32_t)seed; a.counter = (uint32_t)counter;
+    a.dt = dt;
+    at::Tensor x_out = at::empty_like(x), P_out = at::empty_like(P), s_out = at::empty_like(sigmas);
+    a.x = x.data_ptr(); a.P = P.data_ptr(); a.x_out = x_out.data_ptr(); a.P_out = P_out.data_ptr();
+    a.sigmas = sigmas.data_ptr(); a.sigmas_out = s_out.data_ptr();
+    a.Q = model(Q, N, n, n, &a.Q_stride, x, "Q");
+    a.R = model(R, N, m, m, &a.R_stride, x, "R");
+    if (F.has_value()) a.F = model(*F, N, n, n, &a.F_stride, x, "F");
+    if (H.has_value()) a.H = model(*H, N, m, n, &a.H_stride, x, "H");
+    TORCH_CHECK(z.is_cuda() && z.is_contiguous() && z.scalar_type() == x.scalar_type() && z.dim() == 2 && z.size(0) == N, "bke: z is [N, m]");
+    a.z = z.data_ptr();
+    check_rc(bke_enkf_step(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_enkf_step");
+    return std::make_tuple(x_out, P_out, s_out);
+}
+
 std::tuple<at::Tensor, at::Tensor> srkf_step(const at::Tensor &x, const at::Tensor &L, const at::Tensor &F, const at::Tensor &H,
                                              const at::Tensor &Lq, const at::Tensor &Lr, const at::Tensor &z)
 {
@@ -231,6 +264,8 @@ TORCH_LIBRARY(bke, m)
           "int fx_model, int hx_model, Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor)");
     m.def("ckf_step(Tensor x, Tensor P, Tensor Q, Tensor R, Tensor z, float dt, int fx_model, int hx_model, "
           "Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor)");
+    m.def("enkf_step(Tensor x, Tensor P, Tensor sigmas, Tensor Q, Tensor R, Tensor z, float dt, int fx_model, int hx_model, "
+          "int seed, int counter, Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor, Tensor)");
     m.def("srkf_step(Tensor x, Tensor L, Tensor F, Tensor H, Tensor Lq, Tensor Lr, Tensor z) -> (Tensor, Tensor)");
     m.def("fls_smooth_batch(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor zs, int N) -> (Tensor, Tensor)");
     m.def("systematic_resample(Tensor weights, float u) -> Tensor");
@@ -243,6 +278,7 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("kf_predict", &kf_predict);
     m.impl("ukf_step", &ukf_step);
     m.impl("ckf_step", &ckf_step);
+    m.impl("enkf_step", &enkf_step);
     m.impl("srkf_step", &srkf_step);
     m.impl("fls_smooth_batch", &fls_smooth_batch);
     m.impl("systematic_resample", &systematic_resample);

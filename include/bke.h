@@ -367,6 +367,71 @@ size_t bke_debug_ckf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dty
                                        const char *source, const char *include_dirs);
 
 /* ------------------------------------------------------------------------------------------
+ * Ensemble Kalman filter bank.
+ * Replaces EnsembleKalmanFilter.initialize / predict / update (filterpy/kalman/ensemble_kalman_filter.py:
+ * 187-215, 275-290, 218-273) for N filters of n_members members each, with the fx / hx models of the UKF
+ * above (the closed set, or user source through bke_enkf_model_compile below).  sigmas[N, n_members, n].
+ * Per filter (flags = BKE_DO_PREDICT | BKE_DO_UPDATE; a fused call runs the predict first):
+ *   predict:  s_i <- fx(s_i, dt) + e_i, e_i ~ N(0, Q);  x <- mean(s);  P <- sum (s_i - x)(..)' / (n_members - 1)
+ *             [x_prior, P_prior]
+ *   update:   h_i = hx(s_i);  z^ = mean(h);  S = sum (h_i - z^)(..)' / (n_members - 1) + R;
+ *             Pxz = sum (s_i - x)(h_i - z^)' / (n_members - 1) with the x held before the update (:256-257);
+ *             SI = S^-1;  K = Pxz SI;  s_i <- s_i + K (z + r_i - h_i), r_i ~ N(0, R);  x <- mean(s);
+ *             P <- P - K S K'  (not the ensemble covariance, as in the reference, :268)      [K, S, SI]
+ * Noise: standard normals xi from Philox4x32-10 keyed with (seed, filter index) and counted with
+ * (component / 2, member, draw call, filter index >> 32); Box-Muller on uniforms in (0, 1] (DESIGN.md §3.5d).
+ * Each of initialize, predict and update is one draw call: a predict draws with call index `counter`, the
+ * update of the same launch with counter + 1, an update-only launch with `counter`.  The caller advances
+ * the counter by the number of draws of each launch.  A correlated draw is L xi with L L' = C lower, C's
+ * Cholesky factor in which a pivot <= 16 n eps max(diag C) zeroes its column (rank-deficient C, C = 0).
+ * status[f] = BKE_STATUS_NOT_PD when Q, R or the P of initialize is clearly indefinite (the reference's
+ * multivariate_normal only warns) and BKE_STATUS_SINGULAR_S when S is singular; the filter then keeps the
+ * state it had before the failing half.  z_valid[f] == 0 skips the update of filter f (no draws, members,
+ * x and P unchanged).  x_out / P_out may alias x / P and sigmas_out may alias sigmas. */
+typedef struct bke_enkf_args {
+    int64_t n_filters;
+    int32_t dim_x, dim_z;            /* dim_x <= 16 */
+    int32_t n_members;               /* >= 2 */
+    int32_t dtype;
+    uint32_t flags;                  /* BKE_DO_PREDICT | BKE_DO_UPDATE */
+    int32_t fx_model, hx_model;
+    uint32_t seed, counter;          /* noise key and the draw-call index of the launch's first draw */
+    uint32_t reserved;
+    double dt;
+    const void *x, *P;
+    void *x_out, *P_out;
+    const void *sigmas;              /* [N,n_members,n] in */
+    void *sigmas_out;                /* [N,n_members,n] out */
+    const void *Q; int64_t Q_stride;
+    const void *R; int64_t R_stride;
+    const void *F; int64_t F_stride; /* BKE_FX_LINEAR only */
+    const void *H; int64_t H_stride; /* BKE_HX_LINEAR only */
+    const void *z;
+    const uint8_t *z_valid;
+    void *x_prior, *P_prior;
+    void *K, *S, *SI;
+    int32_t *status;
+} bke_enkf_args;
+
+/* initialize (:206): sigmas[f, i] = x[f] + L_P xi_i with draw call `counter`; x and P are not changed.
+ * 1 <= dim_x <= 16.  status[N] (may be NULL): BKE_STATUS_NOT_PD for a clearly indefinite P, whose members
+ * are then all x[f]. */
+int bke_enkf_initialize(int64_t n_filters, int32_t dim_x, int32_t n_members, int32_t dtype, uint32_t seed, uint32_t counter,
+                        const void *x, const void *P, void *sigmas, int32_t *status, void *stream);
+int bke_enkf_step(const bke_enkf_args *args, void *stream);
+
+/* User-supplied fx / hx for the EnKF (the reference calls fx(s, dt) and hx(s), :251, :280): source text,
+ * include_dirs and args vectors as for bke_ukf_model_compile / bke_ukf_step_model.  The handle is a
+ * bke_ukf_model built for the EnKF kernel; the UKF and CKF step calls refuse it and bke_enkf_step_model
+ * refuses theirs (BKE_ERR_BAD_ARG). */
+int bke_enkf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
+                           const char *include_dirs, bke_ukf_model **out);
+int bke_enkf_step_model(const bke_enkf_args *args, const bke_ukf_model *model, const void *fx_args, int64_t fx_args_stride,
+                        const void *hx_args, int64_t hx_args_stride, void *stream);
+size_t bke_debug_enkf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
+                                        const char *source, const char *include_dirs);
+
+/* ------------------------------------------------------------------------------------------
  * Square-root Kalman filter bank.
  * Replaces SquareRootKalmanFilter.predict / update (filterpy/kalman/square_root.py:226-248, 172-224) for N
  * filters at once.  The state is x[N,n] and the lower-triangular factor L[N,n,n] of P = L L' (P1_2), stored
