@@ -14,6 +14,7 @@ BKE_F32, BKE_F64 = 0, 1
 BKE_OK, BKE_ERR_BAD_ARG, BKE_ERR_UNSUPPORTED, BKE_ERR_CUDA = 0, 1, 2, 3
 BKE_STATUS_OK, BKE_STATUS_SINGULAR_S, BKE_STATUS_NOT_PD = 0, 1, 2
 BKE_DO_PREDICT, BKE_DO_UPDATE, BKE_UPDATE_FIRST = 1, 2, 4
+BKE_REVERSE_TILES = 16
 BKE_FX_LINEAR, BKE_FX_CONST_VEL = 0, 1
 BKE_HX_LINEAR, BKE_HX_RANGE_AZ_EL, BKE_HX_RANGE_BEARING = 0, 1, 2
 BKE_FX_USER = BKE_HX_USER = 100

@@ -13,7 +13,10 @@
 //     stores;
 //   * consecutive launches overlap at their edges (programmatic dependent launch): a CTA's
 //     prologue runs before griddepcontrol.wait, every global access after it, and a CTA releases
-//     the next launch once it has issued the loads of its last tile.
+//     the next launch once it has issued the loads of its last tile;
+//   * the CTAs walk the tiles in a launch order (tile = blockIdx.x + k gridDim.x) that maps to the bank
+//     first to last, or last to first with BKE_REVERSE_TILES: a caller that alternates the two starts
+//     every step on the tiles the previous step finished, whose state and models are still in L2.
 // Shared models (stride 0) are read once per thread through the read-only path instead of TMA.
 // A bank whose per-filter Q and R are exactly symmetric may instead hand over a packed copy of their
 // upper triangles (bke_kf_pack_sym_models, REC == 1): one bulk copy per tile replaces the two of
@@ -130,6 +133,7 @@ struct FastP {
     int64_t N_filters;
     int num_tiles;
     int l2_hints;                   // 1: keep x, P in L2 between steps (evict_last), stream the rest (evict_first)
+    int reverse;                    // 1: the launch's tile t is the bank's tile num_tiles - 1 - t
     float alpha_sq;
     const float *x, *P, *z;         // the prior state and the measurements (dense AoS)
     const float *F, *Q, *H, *R;     // per-filter models (SHARED == 0) or the bank's one model (SHARED == 1)
@@ -181,6 +185,7 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
     const uint64_t pol_first = policy_evict_first(), pol_last = policy_evict_last();
     // the tile's blocks are contiguous byte ranges; a ragged last tile copies only its own filters
     // (z: 8 B per filter, rounded down to the 16-byte granule; an odd last filter reads its own z)
+    // (tile: the bank's tile, not the position in the launch order)
     auto issue = [&](int tile, int stage) {
         unsigned char *sb = smem + stage * St::BYTES;
         uint64_t *bar = &full[stage];
@@ -242,10 +247,13 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
     // griddepcontrol.wait makes those writes visible.
     griddep_wait();
     __syncthreads();
+    // Launch-order tile t stands for the bank's tile base + sign t; both are formed once from the
+    // parameters, so that the per-tile address arithmetic stays uniform.
+    const int base = p.reverse ? p.num_tiles - 1 : 0, sign = p.reverse ? -1 : 1;
     if (tid == 0) {
         for (int s = 0; s < STAGES; s++) {
             int tile = blockIdx.x + s * gridDim.x;
-            if (tile < p.num_tiles) issue(tile, s);
+            if (tile < p.num_tiles) issue(base + sign * tile, s);
         }
     }
     if (SHARED == 1) {
@@ -325,7 +333,7 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
                 R[0][0] = r.x; R[0][1] = r.y; R[1][0] = r.z; R[1][1] = r.w;
             }
         }
-        const int64_t f = (int64_t)tile * TILE + tid;
+        const int64_t f = (int64_t)(base + sign * tile) * TILE + tid;
         const bool live = f < p.N_filters;
         if (DO_U) {
             // the stage holds z up to the last whole 16 bytes: only an odd last filter misses its own
@@ -375,7 +383,7 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
         if (never && p.num_tiles < 0) p.x_out[0] = 0.f;              // keeps `acc` alive; cannot happen
         const int nt = tile + STAGES * gridDim.x;
         if (nt < p.num_tiles) {
-            if (tid == 0) issue(nt, stage);
+            if (tid == 0) issue(base + sign * nt, stage);
         } else {
             // this CTA has issued the loads of its last tile: the next launch on the stream may
             // take the SM slots this grid frees and run its prologue (it waits before touching memory)
@@ -448,7 +456,8 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 
 // ---------------------------------------------------------------------------- host side
 // switches (environment, read once): BKE_KF_L2 = 0 disables the L2 eviction-priority hints,
-// BKE_KF_SYM = 0 both packed records, BKE_KF_HOST_MODELS = 0 the shared models in the launch parameters
+// BKE_KF_SYM = 0 both packed records, BKE_KF_HOST_MODELS = 0 the shared models in the launch parameters,
+// BKE_KF_ORDER = 0 the reversed tile order (every launch walks the bank first to last)
 int env_int(const char *name, int dflt)
 {
     const char *v = getenv(name);
@@ -828,6 +837,10 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const 
         static const int l2_env = env_int("BKE_KF_L2", 1);
         p.l2_hints = l2_env && (N * 80 <= (int64_t)38 << 20) && a.x_out == a.x && a.P_out == a.P;
     }
+    // a bank whose state stays in L2 between steps (l2_hints) has nothing to gain from the order: it
+    // keeps walking first to last
+    static const int order_env = env_int("BKE_KF_ORDER", 1);
+    p.reverse = order_env && (a.flags & BKE_REVERSE_TILES) && !p.l2_hints;
     p.x = (const float *)a.x; p.P = (const float *)a.P; p.z = (const float *)a.z;
     p.F = (const float *)a.F; p.Q = (const float *)a.Q; p.H = (const float *)a.H; p.R = (const float *)a.R;
     p.rec = (const float *)rec;

@@ -60,6 +60,9 @@ class KalmanFilter(_BankMirror):
         self._post_alias = False      # True: x_post / P_post are the live x / P (nothing has moved them since the update)
         self._version = 0            # bumped whenever a tensor the kernels read is re-bound
         self._args_cache = {}
+        # Every other launch that steps x, P walks the bank's tiles last to first (BKE_REVERSE_TILES): it
+        # starts on the filters the previous launch finished, while their state and models are still in L2.
+        self._reverse = False
         # Packed copy of the per-filter model words that differ between filters (bke_kf_scan_models,
         # bke_kf_pack_models): derived data, valid for one state of F, Q, H and R.  _model_version counts
         # re-bindings of F / Q / H / R and hand-outs of the live tensors; together with the tensors' own
@@ -285,6 +288,9 @@ class KalmanFilter(_BankMirror):
         return self._sym_buf if usable else None
 
     def _launch(self, flags, pend, zt, vt, R, H):
+        if self._reverse:
+            flags |= _lib.BKE_REVERSE_TILES
+        self._reverse = not self._reverse
         # steady state of a filter loop: nothing but z changed since the last identical call ->
         # reuse the argument struct (the Python side of a launch drops to a few microseconds)
         plain = R is None and H is None and (pend is None or (pend.get("u") is None and pend.get("B") is None
@@ -372,7 +378,13 @@ class KalmanFilter(_BankMirror):
         before the capture, and the words every filter shares are baked into its launch parameters,
         so F, Q, H and R are all frozen into it.  Re-capture after changing any of them, whether by
         assignment or in place; refilling z, x or P in place between replays works as for any
-        graph."""
+        graph.
+
+        Consecutive launches walk the bank in alternating tile order (``BKE_REVERSE_TILES``, a
+        scheduling hint: the results are the same either way), and each captured launch keeps the
+        order it was captured with.  A graph with an even number of launches therefore alternates
+        across replays too; with an odd number, the first launch of a replay runs in the same order as
+        the last launch of the previous one, which costs that step the L2 reuse but nothing else."""
         self._flush()
         return StepGraph(fn, self._device, warmup)
 
@@ -384,7 +396,9 @@ class KalmanFilter(_BankMirror):
         ``zs`` as in the reference (entries may be None), NumPy outputs with its shapes.
 
         With time-constant models the whole T-epoch loop is ONE kernel (bke_kf_batch_filter);
-        per-epoch ``Fs/Qs/Hs/Rs/Bs/us`` or a ``saver`` run one fused launch per epoch."""
+        per-epoch ``Fs/Qs/Hs/Rs/Bs/us`` or a ``saver`` run one fused launch per epoch.  Those launches
+        step the bank like ``predict`` / ``update`` and alternate its tile order the same way (see
+        ``capture``; the results do not depend on it)."""
         self._flush()
         N, n, m = self.n_filters, self.dim_x, self.dim_z
         # (the reference's np.size(zs, 0), kalman_filter.py:951; a list that mixes None with arrays is

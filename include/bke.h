@@ -59,6 +59,14 @@ extern "C" {
 #define BKE_STATUS_STICKY 8u         /* status[f] is only written when the step FAILS (the caller zeroed it): an
                                         error of an earlier step survives.  bke_kf_batch_filter's status is
                                         sticky over all epochs on every path. */
+#define BKE_REVERSE_TILES 16u        /* scheduling hint, no result depends on it: the 4/2 fp32 step (bke_kf_step,
+                                        bke_kf_step_sym, bke_kf_step_packed) walks the bank last tile to first.
+                                        A caller stepping a bank larger than L2 in place sets it on every other
+                                        step, so that each step starts on the filters the previous one finished
+                                        while their x, P and models are still in L2.  Other kernels ignore it,
+                                        and so does the 4/2 step of a bank whose state fits L2 anyway (at
+                                        most 38 MiB of x, P, stepped in place); BKE_KF_ORDER=0 in the
+                                        environment makes the 4/2 step ignore it always. */
 
 int bke_abi_version(void);
 const char *bke_last_error(void);

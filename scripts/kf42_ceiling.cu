@@ -25,39 +25,76 @@ constexpr int SYM_CHUNKS = CHUNK * 52 / 16;     // 16-byte chunks of the packed 
 constexpr int WORD_CHUNKS = CHUNK * 40 / 16;    // 16-byte chunks of the packed model-word stream per CTA iteration
 constexpr int DISTINCT_CHUNKS = CHUNK * 20 / 16;    // the same for its distinct planes only
 
+// L2 cache-policy loads and stores (the accesses of the hinted variant below)
+__device__ __forceinline__ float4 ld_hint(const float4 *a, uint64_t pol)
+{
+    float4 v;
+    asm volatile("ld.global.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(a), "l"(pol) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_hint(float4 *a, float4 v, uint64_t pol)
+{
+    asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;"
+                 ::"l"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
+}
+
+// Order and L2 policy of one launch.  The CTAs walk the chunks in launch order c = blockIdx.x + k gridDim.x;
+// chunk c is the bank's chunk c (forward) or n_chunks - 1 - c (reverse).  With HINTS: z is read with
+// evict_first when z_first is set, the first `head` chunks of the launch order are read and written with
+// evict_first (they are the previous launch's tail, demoted), the last `tail` chunks with evict_last (kept
+// for the next launch, which walks the other way and starts on them); the rest with the default policy.
+struct Order {
+    int reverse, z_first;
+    int64_t head, tail;
+};
+
+template <bool HINTS>
 __global__ void __launch_bounds__(THREADS)
 kf42_traffic_kernel(float4 *x, float4 *P, const float4 *F, const float4 *Q, const float4 *H, const float4 *R,
-                    const float4 *z, int64_t n_chunks, int mode)
+                    const float4 *z, int64_t n_chunks, int mode, Order o)
 {
     const int t = threadIdx.x;
-    for (int64_t c = blockIdx.x; c < n_chunks; c += gridDim.x) {
+    uint64_t pol_first = 0, pol_last = 0, pol_normal = 0;
+    if (HINTS) {
+        asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_first));
+        asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_last));
+        asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol_normal));
+    }
+    for (int64_t k = blockIdx.x; k < n_chunks; k += gridDim.x) {
+        const int64_t c = o.reverse ? n_chunks - 1 - k : k;
+        const uint64_t pol = k < o.head ? pol_first : k >= n_chunks - o.tail ? pol_last : pol_normal;
+        const uint64_t pol_z = o.z_first ? pol_first : pol;
+        auto ld = [&](const float4 *a, uint64_t pl) { return HINTS ? ld_hint(a, pl) : __ldg(a); };
         const int64_t p16 = c * THREADS + t;            // 16-byte chunk of P, F, Q (4 per filter)
-        float4 vp = P[p16];
+        float4 vp = HINTS ? ld_hint(P + p16, pol) : P[p16];
         float4 vh = make_float4(0.f, 0.f, 0.f, 0.f), vf = vh, vq = vh, vx = vh, vr = vh, vz = vh;
         if (mode == 2) {
-            if (t < WORD_CHUNKS) vq = __ldg(Q + c * WORD_CHUNKS + t);
+            if (t < WORD_CHUNKS) vq = ld(Q + c * WORD_CHUNKS + t, pol);
         } else if (mode == 3) {
-            if (t < DISTINCT_CHUNKS) vq = __ldg(Q + c * DISTINCT_CHUNKS + t);
+            if (t < DISTINCT_CHUNKS) vq = ld(Q + c * DISTINCT_CHUNKS + t, pol);
         } else {
-            vf = __ldg(F + p16);
+            vf = ld(F + p16, pol);
             if (mode == 1) {
-                if (t < SYM_CHUNKS) vq = __ldg(Q + c * SYM_CHUNKS + t);
+                if (t < SYM_CHUNKS) vq = ld(Q + c * SYM_CHUNKS + t, pol);
             } else {
-                vq = __ldg(Q + p16);
-                if (t < THREADS / 4) vr = __ldg(R + c * (THREADS / 4) + t);
+                vq = ld(Q + p16, pol);
+                if (t < THREADS / 4) vr = ld(R + c * (THREADS / 4) + t, pol);
             }
-            if (t < THREADS / 2) vh = __ldg(H + c * (THREADS / 2) + t);
+            if (t < THREADS / 2) vh = ld(H + c * (THREADS / 2) + t, pol);
         }
-        if (t < THREADS / 4) vx = x[c * (THREADS / 4) + t];
-        if (t < THREADS / 8) vz = __ldg(z + c * (THREADS / 8) + t);
+        if (t < THREADS / 4) vx = HINTS ? ld_hint(x + c * (THREADS / 4) + t, pol) : x[c * (THREADS / 4) + t];
+        if (t < THREADS / 8) vz = ld(z + c * (THREADS / 8) + t, pol_z);
         // the stores depend on every load (bit-wise, no floating-point work), so none is dropped
-        const uint32_t k = __float_as_uint(vf.x) | __float_as_uint(vq.y) | __float_as_uint(vh.z) |
-                           __float_as_uint(vr.w) | __float_as_uint(vz.x);
-        vp.x = __uint_as_float(__float_as_uint(vp.x) | k);
-        P[p16] = vp;
+        const uint32_t kk = __float_as_uint(vf.x) | __float_as_uint(vq.y) | __float_as_uint(vh.z) |
+                            __float_as_uint(vr.w) | __float_as_uint(vz.x);
+        vp.x = __uint_as_float(__float_as_uint(vp.x) | kk);
+        if (HINTS) st_hint(P + p16, vp, pol);
+        else P[p16] = vp;
         if (t < THREADS / 4) {
-            vx.x = __uint_as_float(__float_as_uint(vx.x) | k);
-            x[c * (THREADS / 4) + t] = vx;
+            vx.x = __uint_as_float(__float_as_uint(vx.x) | kk);
+            if (HINTS) st_hint(x + c * (THREADS / 4) + t, vx, pol);
+            else x[c * (THREADS / 4) + t] = vx;
         }
     }
 }
@@ -68,12 +105,22 @@ extern "C" {
 
 // One launch over n_filters (a multiple of 64); returns a cudaError_t.  mode 1: Q is the 52 B-per-filter
 // stream and R is not read; mode 2 (3): Q is the 40 (20) B-per-filter stream and F, H, R are not read.
+// reverse: walk the chunks last to first.  z_first, head_filters, tail_filters: the L2 policy of the
+// hinted variant (Order above; head and tail in filters, rounded down to whole chunks); all zero and
+// hints == 0: plain accesses with the default policy.
 int kf42_traffic(void *x, void *P, const void *F, const void *Q, const void *H, const void *R, const void *z,
-                 int64_t n_filters, int grid, int mode, void *stream)
+                 int64_t n_filters, int grid, int mode, void *stream, int reverse, int hints, int z_first,
+                 int64_t head_filters, int64_t tail_filters)
 {
-    kf42_traffic_kernel<<<grid, THREADS, 0, (cudaStream_t)stream>>>(
-        (float4 *)x, (float4 *)P, (const float4 *)F, (const float4 *)Q, (const float4 *)H, (const float4 *)R,
-        (const float4 *)z, n_filters / CHUNK, mode);
+    const Order o = {reverse, z_first, head_filters / CHUNK, tail_filters / CHUNK};
+    if (hints)
+        kf42_traffic_kernel<true><<<grid, THREADS, 0, (cudaStream_t)stream>>>(
+            (float4 *)x, (float4 *)P, (const float4 *)F, (const float4 *)Q, (const float4 *)H, (const float4 *)R,
+            (const float4 *)z, n_filters / CHUNK, mode, o);
+    else
+        kf42_traffic_kernel<false><<<grid, THREADS, 0, (cudaStream_t)stream>>>(
+            (float4 *)x, (float4 *)P, (const float4 *)F, (const float4 *)Q, (const float4 *)H, (const float4 *)R,
+            (const float4 *)z, n_filters / CHUNK, mode, o);
     return (int)cudaGetLastError();
 }
 

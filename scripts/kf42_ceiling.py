@@ -15,6 +15,14 @@ Prints JSON lines (and writes them to DIR/kf42_ceiling.jsonl with --out):
              words that differ between the filters of the bench bank (bke_kf_pack_models): 208 B
   ceiling_distinct  the same twin with that stream cut to 20 B per filter, the 5 distinct planes
              among those 10 words (the step does not read a plane the scan flags as a copy): 188 B
+  ceiling_alternating  the 188 B twin at N = 2^19 .. 2^22, with a ring of 4 measurement buffers (z is
+             a different buffer every step, as in bench.py): `forward` launches every step in the same
+             tile order (as the shipped step did), the other arms in forward / reverse pairs, so that a
+             launch starts on the tiles the previous one finished: `alt` with the default L2 policy,
+             `alt_zfirst` with z read evict_first, `alt_tail_<W>MB` with, on top, the last W MB of a
+             launch's order (100 B per filter: x, P and the model planes) read and written evict_last
+             and demoted (evict_first) by the next launch.  ms per launch (best grid of 4 or 8 CTAs per
+             SM, median of rounds, the arms alternated inside every round) and the gain over `forward`
   step       the shipped step (KalmanFilter.predict + update, per-filter F/H/Q/R) replayed as CUDA
              graphs of 4 steps like bench.py, at N = 2^19 .. 2^22 (all above the bound under which
              the L2 hints are used); per-step time and GB/s for every N, counted with the bytes the
@@ -62,6 +70,15 @@ def build_lib():
     return LIB
 
 
+def traffic_lib():
+    lib = ctypes.CDLL(build_lib())
+    lib.kf42_traffic.restype = ctypes.c_int
+    lib.kf42_traffic.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int64,
+                                                         ctypes.c_int64]
+    return lib
+
+
 def card():
     try:
         r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -88,9 +105,7 @@ def reps_for(n_filters, seconds=0.3):
 
 
 def ceiling(torch, rounds, mode=0):
-    lib = ctypes.CDLL(build_lib())
-    lib.kf42_traffic.restype = ctypes.c_int
-    lib.kf42_traffic.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
+    lib = traffic_lib()
     N = 1 << 20
     dev = torch.device("cuda")
     g = torch.Generator(device=dev).manual_seed(5)
@@ -104,7 +119,7 @@ def ceiling(torch, rounds, mode=0):
         grid = sms * per_sm
 
         def run():
-            rc = lib.kf42_traffic(*[arr[k].data_ptr() for k in "xPFQHRz"], N, grid, mode, stream)
+            rc = lib.kf42_traffic(*[arr[k].data_ptr() for k in "xPFQHRz"], N, grid, mode, stream, 0, 0, 0, 0, 0)
             assert rc == 0, rc
         for _ in range(5):
             run()
@@ -116,6 +131,67 @@ def ceiling(torch, rounds, mode=0):
     return {"what": ("ceiling", "ceiling_sym", "ceiling_words", "ceiling_distinct")[mode], "n_filters": N, "bytes_per_filter": nbytes, "ms": best["ms"],
             "GBps": best["GBps"],
             "frac_of_3350": best["frac_of_3350"], "by_grid": out}
+
+
+TAIL_MB = (8, 16, 24, 32)   # the tail windows of the alternating sweep
+REUSED = 100                # bytes per filter a launch can take over from the previous one: x, P, the model planes
+
+
+def alternating(torch, rounds):
+    """The 188 B twin launched every step in one tile order, or in forward / reverse pairs (with and
+    without L2 hints); one line per bank size."""
+    lib = traffic_lib()
+    dev = torch.device("cuda")
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    stream = torch.cuda.current_stream().cuda_stream
+    arms = [("forward", False, 0, 0, 0), ("alt", True, 0, 0, 0), ("alt_zfirst", True, 1, 1, 0)]
+    arms += [("alt_tail_%dMB" % w, True, 1, 1, (w << 20) // REUSED) for w in TAIL_MB]
+    lines = []
+    for lg in (19, 20, 21, 22):
+        N = 1 << lg
+        g = torch.Generator(device=dev).manual_seed(5)
+        arr = {k: torch.randn(N * e, device=dev, generator=g) for k, e in
+               (("x", 4), ("P", 16), ("Q", 5), ("z", 2 * RING))}
+        ptr = {k: v.data_ptr() for k, v in arr.items()}
+        reps = reps_for(N) // 2 * 2
+        res = {}
+        ms = {}
+        for r in range(rounds):
+            for per_sm in (4, 8):
+                grid = sms * per_sm
+                for name, alt, hints, z_first, tail in (arms if r % 2 == 0 else arms[::-1]):
+                    state = {"i": 0}
+
+                    def run(alt=alt, hints=hints, z_first=z_first, tail=tail, grid=grid):
+                        i = state["i"]
+                        state["i"] = i + 1
+                        rc = lib.kf42_traffic(ptr["x"], ptr["P"], None, ptr["Q"], None, None,
+                                              ptr["z"] + (i % RING) * N * 8, N, grid, 3, stream,
+                                              i % 2 if alt else 0, hints, z_first, tail, tail)
+                        assert rc == 0, rc
+                    for _ in range(4):
+                        run()
+                    ms.setdefault((name, per_sm), []).append(time_ms(run, reps, torch))
+                    if tail:
+                        # one more launch (untimed) demotes the last launch's evict_last tail, so no line
+                        # keeps that priority once the sequence stops
+                        i = state["i"]
+                        rc = lib.kf42_traffic(ptr["x"], ptr["P"], None, ptr["Q"], None, None,
+                                              ptr["z"] + (i % RING) * N * 8, N, grid, 3, stream,
+                                              i % 2, hints, z_first, tail, 0)
+                        assert rc == 0, rc
+        for name, *_ in arms:
+            best = min((float(np.median(ms[(name, s)])), s) for s in (4, 8))
+            res[name] = {"ms": best[0], "ctas_per_sm": best[1],
+                         "GBps": BYTES_DISTINCT * N / (best[0] * 1e-3) / 1e9}
+        fwd = res["forward"]["ms"]
+        for v in res.values():
+            v["gain_vs_forward"] = fwd / v["ms"] - 1.0
+        lines.append({"what": "ceiling_alternating", "n_filters": N, "bytes_per_filter": BYTES_DISTINCT,
+                      "tail_filters_per_MB": (1 << 20) // REUSED, "arms": res})
+        del arr
+        torch.cuda.empty_cache()
+    return lines
 
 
 def bank(torch, N, shared=False):
@@ -158,6 +234,7 @@ def main():
     lines.append(ceiling(torch, args.rounds, mode=1))
     lines.append(ceiling(torch, args.rounds, mode=2))
     lines.append(ceiling(torch, args.rounds, mode=3))
+    lines += alternating(torch, args.rounds)
     sizes, times = [], []
     moved = BYTES
     for lg in (19, 20, 21, 22):
