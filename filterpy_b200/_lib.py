@@ -18,6 +18,8 @@ BKE_REVERSE_TILES = 16
 BKE_FX_LINEAR, BKE_FX_CONST_VEL = 0, 1
 BKE_HX_LINEAR, BKE_HX_RANGE_AZ_EL, BKE_HX_RANGE_BEARING = 0, 1, 2
 BKE_FX_USER = BKE_HX_USER = 100
+# the UKF / CKF hooks compiled from source text (bke_ukf_model_compile_hooks)
+BKE_HOOK_X_MEAN, BKE_HOOK_Z_MEAN, BKE_HOOK_RESIDUAL_X, BKE_HOOK_RESIDUAL_Z, BKE_HOOK_STATE_ADD = 1, 2, 4, 8, 16
 
 # every symbol include/bke.h declares (tests check that the library exports all of them)
 EXPORTED_SYMBOLS = [
@@ -33,6 +35,8 @@ EXPORTED_SYMBOLS = [
     "bke_ukf_model_compile", "bke_ukf_model_log", "bke_ukf_model_registers", "bke_ukf_model_free", "bke_ukf_step_model",
     "bke_debug_ukf_model_cubin_bytes", "bke_ukf_rts_smoother_model",
     "bke_ckf_step", "bke_ckf_model_compile", "bke_ckf_step_model", "bke_debug_ckf_model_cubin_bytes",
+    "bke_ukf_model_compile_hooks", "bke_debug_ukf_model_hooks_cubin_bytes",
+    "bke_ckf_model_compile_hooks", "bke_debug_ckf_model_hooks_cubin_bytes",
     "bke_enkf_initialize", "bke_enkf_step", "bke_enkf_model_compile", "bke_enkf_step_model", "bke_debug_enkf_model_cubin_bytes",
     "bke_srkf_step", "bke_cholesky_lower",
     "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
@@ -350,6 +354,14 @@ def load():
     lib.bke_ukf_rts_smoother_model.restype = ctypes.c_int
     lib.bke_debug_ukf_model_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p]
     lib.bke_debug_ukf_model_cubin_bytes.restype = c_size_t
+    for fam in ("ukf", "ckf"):
+        f = getattr(lib, "bke_%s_model_compile_hooks" % fam)
+        f.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_uint32, ctypes.c_char_p, ctypes.c_char_p,
+                      ctypes.POINTER(c_void_p)]
+        f.restype = ctypes.c_int
+        f = getattr(lib, "bke_debug_%s_model_hooks_cubin_bytes" % fam)
+        f.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_uint32, ctypes.c_char_p, ctypes.c_char_p]
+        f.restype = c_size_t
     lib.bke_ckf_step.argtypes = [ctypes.POINTER(CkfArgs), c_void_p]
     lib.bke_ckf_step.restype = ctypes.c_int
     lib.bke_ckf_model_compile.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p,

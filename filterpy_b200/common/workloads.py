@@ -245,3 +245,188 @@ def resample_weights(N, kind="heavy", seed=97):
         raise ValueError(kind)
     w /= w.sum()
     return w
+
+
+# ----------------------------------------------------------------------------- angle hooks (UKF.py:97-140)
+# Trackers whose angles cross +-pi: the reference's recipe passes residual / mean / state-add callables that
+# wrap the angle and take circular means.  Each function is given as CUDA source text (DeviceFn, DeviceFx,
+# DeviceHx) and as the Python callable the reference takes (tests/golden/make_golden_ukf_hooks.py).
+RB_HOOKS_SOURCE = """
+// (range, bearing) measurements: the bearing difference wrapped into (-pi, pi], the circular mean of the bearing
+__device__ real rb_wrap(real a)
+{
+    const real pi = 3.14159265358979323846;
+    if (a > pi) a -= 2 * pi; else if (a <= -pi) a += 2 * pi;
+    return a;
+}
+__device__ void residual_z(const real *a, const real *b, real *out) { out[0] = a[0] - b[0]; out[1] = rb_wrap(a[1] - b[1]); }
+__device__ void z_mean_fn(const real *sigmas, const real *Wm, real *out)
+{
+    real r = 0, s = 0, c = 0;
+    for (int i = 0; i < BKE_N_SIGMAS; i++) {
+        r += Wm[i] * sigmas[2 * i];
+        s += Wm[i] * sin(sigmas[2 * i + 1]);
+        c += Wm[i] * cos(sigmas[2 * i + 1]);
+    }
+    out[0] = r;
+    out[1] = atan2(s, c);
+}
+"""
+CTRV_FX_SOURCE = """
+// constant turn rate and velocity, state (px, py, heading, speed, yaw rate); the heading stays in (-pi, pi]
+__device__ void fx(const real *x, real *out, real dt, const real *args)
+{
+    const real pi = 3.14159265358979323846;
+    const real psi = x[2], v = x[3], w = x[4];
+    if (fabs(w) > real(1e-4)) {
+        out[0] = x[0] + v / w * (sin(psi + w * dt) - sin(psi));
+        out[1] = x[1] + v / w * (cos(psi) - cos(psi + w * dt));
+    } else {
+        out[0] = x[0] + v * cos(psi) * dt;
+        out[1] = x[1] + v * sin(psi) * dt;
+    }
+    real h = psi + w * dt;
+    if (h > pi) h -= 2 * pi; else if (h <= -pi) h += 2 * pi;
+    out[2] = h; out[3] = v; out[4] = w;
+}
+"""
+CTRV_RB_HX_SOURCE = """
+// range and bearing of (px, py) from a sensor at (args[0], args[1])
+__device__ void hx(const real *x, real *z, const real *args)
+{
+    const real dx = x[0] - args[0], dy = x[1] - args[1];
+    z[0] = sqrt(dx * dx + dy * dy);
+    z[1] = atan2(dy, dx);
+}
+"""
+CTRV_X_HOOKS_SOURCE = """
+// CTRV state: the heading (x[2]) is an angle
+__device__ real ctrv_wrap(real a)
+{
+    const real pi = 3.14159265358979323846;
+    if (a > pi) a -= 2 * pi; else if (a <= -pi) a += 2 * pi;
+    return a;
+}
+__device__ void residual_x(const real *a, const real *b, real *out)
+{
+    for (int i = 0; i < BKE_DIM_X; i++) out[i] = a[i] - b[i];
+    out[2] = ctrv_wrap(out[2]);
+}
+__device__ void state_add(const real *a, const real *b, real *out)
+{
+    for (int i = 0; i < BKE_DIM_X; i++) out[i] = a[i] + b[i];
+    out[2] = ctrv_wrap(out[2]);
+}
+__device__ void x_mean_fn(const real *sigmas, const real *Wm, real *out)
+{
+    real s = 0, c = 0;
+    for (int i = 0; i < BKE_DIM_X; i++) out[i] = 0;
+    for (int k = 0; k < BKE_N_SIGMAS; k++) {
+        for (int i = 0; i < BKE_DIM_X; i++) if (i != 2) out[i] += Wm[k] * sigmas[k * BKE_DIM_X + i];
+        s += Wm[k] * sin(sigmas[k * BKE_DIM_X + 2]);
+        c += Wm[k] * cos(sigmas[k * BKE_DIM_X + 2]);
+    }
+    out[2] = atan2(s, c);
+}
+"""
+
+
+def wrap_angle(a):
+    """Into (-pi, pi] for differences of two angles in (-pi, pi] (the CUDA text's rb_wrap / ctrv_wrap)."""
+    a = np.asarray(a, float)
+    return np.where(a > np.pi, a - 2 * np.pi, np.where(a <= -np.pi, a + 2 * np.pi, a))
+
+
+def rb_residual_z(a, b):
+    d = np.array(a - b, float)          # 1-D, or the CKF's (2, 1) columns: row 1 is the bearing either way
+    d[1] = wrap_angle(d[1])
+    return d
+
+
+def rb_z_mean(sigmas, Wm):
+    return np.array([np.dot(Wm, sigmas[:, 0]), np.arctan2(np.dot(Wm, np.sin(sigmas[:, 1])), np.dot(Wm, np.cos(sigmas[:, 1])))])
+
+
+def ctrv_fx(x, dt):
+    psi, v, w = x[2], x[3], x[4]
+    if abs(w) > 1e-4:
+        px = x[0] + v / w * (np.sin(psi + w * dt) - np.sin(psi))
+        py = x[1] + v / w * (np.cos(psi) - np.cos(psi + w * dt))
+    else:
+        px = x[0] + v * np.cos(psi) * dt
+        py = x[1] + v * np.sin(psi) * dt
+    return np.array([px, py, float(wrap_angle(psi + w * dt)), v, w])
+
+
+def ctrv_rb_hx(x, sx, sy):
+    dx, dy = x[0] - sx, x[1] - sy
+    return np.array([np.sqrt(dx * dx + dy * dy), np.arctan2(dy, dx)])
+
+
+def ctrv_residual_x(a, b):
+    d = np.array(a - b, float)
+    d[2] = wrap_angle(d[2])
+    return d
+
+
+def ctrv_state_add(a, b):
+    s = np.array(a + b, float)
+    s[2] = wrap_angle(s[2])
+    return s
+
+
+def ctrv_x_mean(sigmas, Wm):
+    x = np.dot(Wm, sigmas)
+    x[2] = np.arctan2(np.dot(Wm, np.sin(sigmas[:, 2])), np.dot(Wm, np.cos(sigmas[:, 2])))
+    return x
+
+
+def ukf_bank_rb_behind(N, seed=8080, steps=1, dt=1.0, dtype=np.float64):
+    """(a) N constant-velocity targets (x, vx, y, vy) BEHIND a range / bearing sensor at the origin, each
+    crossing the x axis (bearing +-pi) within ten steps."""
+    rng = np.random.default_rng(seed)
+    py = rng.uniform(-60, 60, N)
+    vy = -np.sign(py) * rng.uniform(6, 14, N)
+    xt = np.stack([rng.uniform(-400, -150, N), rng.uniform(-3, 3, N), py, vy], 1)
+    x0 = xt + rng.standard_normal((N, 4)) * np.array([2, .5, 2, .5])
+    P0 = np.zeros((N, 4, 4))
+    P0[:, np.arange(4), np.arange(4)] = rng.uniform(1.0, 9.0, (N, 4))
+    q = np.exp(rng.uniform(np.log(1e-3), np.log(1e-1), N))
+    qb = q_white_noise_block(2, np.full(N, dt), q)
+    Q = _block_diag([qb, qb])
+    sig = np.array([1.0, 0.01])
+    R = np.broadcast_to(np.diag(sig ** 2), (N, 2, 2)).copy()
+    zs = np.zeros((steps, N, 2))
+    for t in range(steps):
+        xt = xt.copy()
+        xt[:, 0::2] += dt * xt[:, 1::2]
+        px, pyt = xt[:, 0], xt[:, 2]
+        h = np.stack([np.sqrt(px * px + pyt * pyt), np.arctan2(pyt, px)], 1) + sig * rng.standard_normal((N, 2))
+        h[:, 1] = wrap_angle(h[:, 1])
+        zs[t] = h
+    out = dict(x=x0, P=P0, Q=Q, R=R, zs=zs)
+    return {k: np.ascontiguousarray(v, dtype=dtype) for k, v in out.items()}
+
+
+def ukf_bank_ctrv(N, seed=6060, steps=1, dt=0.5, dtype=np.float64):
+    """(b) N CTRV targets (px, py, heading, speed, yaw rate) whose heading crosses +-pi, seen by a range /
+    bearing sensor at ``sensor``."""
+    rng = np.random.default_rng(seed)
+    sensor = np.array([-50.0, 20.0])
+    xt = np.stack([rng.uniform(200, 600, N), rng.uniform(-200, 200, N), wrap_angle(np.pi + rng.uniform(-0.4, 0.4, N)),
+                   rng.uniform(5, 15, N), rng.uniform(0.15, 0.35, N) * rng.choice([-1.0, 1.0], N)], 1)
+    x0 = xt + rng.standard_normal((N, 5)) * np.array([2, 2, .05, .5, .02])
+    x0[:, 2] = wrap_angle(x0[:, 2])
+    P0 = np.zeros((N, 5, 5))
+    P0[:, np.arange(5), np.arange(5)] = np.array([4, 4, .01, .25, .001]) * rng.uniform(1.0, 2.0, (N, 5))
+    q = rng.uniform(0.5, 2.0, N)
+    Q = np.zeros((N, 5, 5))
+    Q[:, np.arange(5), np.arange(5)] = q[:, None] * np.array([.01, .01, 1e-4, .01, 1e-4]) * dt
+    sig = np.array([1.5, 0.004])
+    R = np.broadcast_to(np.diag(sig ** 2), (N, 2, 2)).copy()
+    zs = np.zeros((steps, N, 2))
+    for t in range(steps):
+        xt = np.stack([ctrv_fx(xt[f], dt) for f in range(N)])
+        zs[t] = np.stack([ctrv_rb_hx(xt[f], *sensor) for f in range(N)]) + sig * rng.standard_normal((N, 2))
+    out = dict(x=x0, P=P0, Q=Q, R=R, zs=zs, sensor=sensor)
+    return {k: np.ascontiguousarray(v, dtype=dtype) for k, v in out.items()}

@@ -86,8 +86,12 @@ __device__ __forceinline__ void gain_update(const Prm &p, int64_t f, bool live, 
             for (int b = 1; b < M; b++) s += Pxz[i][b] * o.SI[b][a];
             o.K[i][a] = s;
         }
+    if constexpr (ukfk::HOOKS & BKE_HOOK_RESIDUAL_Z) {
+        ukfk::bke_hook_residual_z<T>(zv, zm, o.y);                // the only hook the CKF calls (:376)
+    } else {
 #pragma unroll
-    for (int a = 0; a < M; a++) o.y[a] = zv[a] - zm[a];
+        for (int a = 0; a < M; a++) o.y[a] = zv[a] - zm[a];
+    }
 #pragma unroll
     for (int i = 0; i < N; i++) {
         T s = x[i];

@@ -51,6 +51,20 @@ struct UkfP {
 template <typename T> __device__ void bke_user_fx(const T *x, T *out, T dt, const T *args);
 template <typename T> __device__ void bke_user_hx(const T *x, T *z, const T *args);
 
+// The reference's mean / residual / state-add hooks (UKF.py:97-140; x_mean_fn, z_mean_fn, residual_x,
+// residual_z, state_add): BKE_UKF_HOOKS is the BKE_HOOK_* mask of the user functions the program text
+// supplies.  Only run-time compiled instances define it (ukf_rtc.cu), so every hook below sits behind
+// `if constexpr` and the pre-built instances compile to the code they had without hooks.
+#ifndef BKE_UKF_HOOKS
+#define BKE_UKF_HOOKS 0u
+#endif
+constexpr unsigned HOOKS = BKE_UKF_HOOKS;
+template <typename T> __device__ void bke_hook_x_mean(const T *sigmas, const T *Wm, T *out);     // sigmas [2n+1][n]
+template <typename T> __device__ void bke_hook_z_mean(const T *sigmas, const T *Wm, T *out);     // sigmas [2n+1][m]
+template <typename T> __device__ void bke_hook_residual_x(const T *a, const T *b, T *out);
+template <typename T> __device__ void bke_hook_residual_z(const T *a, const T *b, T *out);
+template <typename T> __device__ void bke_hook_state_add(const T *a, const T *b, T *out);
+
 template <int S> struct IntC { static constexpr int value = S; };
 
 // upper Cholesky factor of A (upper triangle of A is read, like scipy.linalg.cholesky):
@@ -344,15 +358,29 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
         T xm[N];
 #pragma unroll
         for (int i = 0; i < N; i++) xm[i] = T(0);
-        for_sigma<0, NS>([&](auto sc) {
-            constexpr int S = decltype(sc)::value;
-            T sp[N], fs[N];
-            sigma_point<T, N, S>(x, U, sp);
-            apply_fx<T, N, FX>(sp, fs, p.dt, Fp, fstride, fxa);
-            const T w = (S == 0) ? p.wm0 : p.wi;
+        // x_mean_fn sees every propagated point at once (UKF.py:403): only that instance stages them
+        T sf[(HOOKS & BKE_HOOK_X_MEAN) ? NS : 1][N];
+        if constexpr (HOOKS & BKE_HOOK_X_MEAN) {
+            T Wm[NS];
+            for_sigma<0, NS>([&](auto sc) {
+                constexpr int S = decltype(sc)::value;
+                T sp[N];
+                sigma_point<T, N, S>(x, U, sp);
+                apply_fx<T, N, FX>(sp, sf[S], p.dt, Fp, fstride, fxa);
+                Wm[S] = (S == 0) ? p.wm0 : p.wi;
+            });
+            bke_hook_x_mean<T>(&sf[0][0], Wm, xm);
+        } else {
+            for_sigma<0, NS>([&](auto sc) {
+                constexpr int S = decltype(sc)::value;
+                T sp[N], fs[N];
+                sigma_point<T, N, S>(x, U, sp);
+                apply_fx<T, N, FX>(sp, fs, p.dt, Fp, fstride, fxa);
+                const T w = (S == 0) ? p.wm0 : p.wi;
 #pragma unroll
-            for (int i = 0; i < N; i++) xm[i] += w * fs[i];
-        });
+                for (int i = 0; i < N; i++) xm[i] += w * fs[i];
+            });
+        }
         // pass 2: covariance (upper triangle; mirrored when Q is added)
         T Pm[N][N];
 #pragma unroll
@@ -362,12 +390,21 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
         for_sigma<0, NS>([&](auto sc) {
             constexpr int S = decltype(sc)::value;
             T sp[N], fs[N];
-            sigma_point<T, N, S>(x, U, sp);
-            apply_fx<T, N, FX>(sp, fs, p.dt, Fp, fstride, fxa);
+            if constexpr (HOOKS & BKE_HOOK_X_MEAN) {
+#pragma unroll
+                for (int i = 0; i < N; i++) fs[i] = sf[S][i];
+            } else {
+                sigma_point<T, N, S>(x, U, sp);
+                apply_fx<T, N, FX>(sp, fs, p.dt, Fp, fstride, fxa);
+            }
             const T w = (S == 0) ? p.wc0 : p.wi;
             T d[N];
+            if constexpr (HOOKS & BKE_HOOK_RESIDUAL_X) {
+                bke_hook_residual_x<T>(fs, xm, d);
+            } else {
 #pragma unroll
-            for (int i = 0; i < N; i++) d[i] = fs[i] - xm[i];
+                for (int i = 0; i < N; i++) d[i] = fs[i] - xm[i];
+            }
 #pragma unroll
             for (int i = 0; i < N; i++) {
                 T wd = w * d[i];
@@ -475,6 +512,16 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
                     }
                 }
             }
+            if constexpr (HOOKS & BKE_HOOK_Z_MEAN) {                // z_mean_fn(sigmas_h, Wm) (UKF.py:469)
+                T sh[NS * M], Wm[NS];
+#pragma unroll
+                for (int s = 0; s < NS; s++) {
+                    Wm[s] = (s == 0) ? p.wm0 : p.wi;
+#pragma unroll
+                    for (int a = 0; a < M; a++) sh[s * M + a] = zs[(s * M + a) * UB + tid];
+                }
+                bke_hook_z_mean<T>(sh, Wm, zm);
+            }
             KfUpdateOut<T, N, M> o;
             T Pxz[N][M];
             // R and z are needed after the covariance pass below: fetch them now so that their latency
@@ -500,8 +547,15 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
             for_sigma<0, NS>([&](auto sc) {
                 constexpr int S = decltype(sc)::value;
                 T dz[M];
+                if constexpr (HOOKS & BKE_HOOK_RESIDUAL_Z) {
+                    T h[M];
 #pragma unroll
-                for (int a = 0; a < M; a++) dz[a] = zs[(S * M + a) * UB + tid] - zm[a];
+                    for (int a = 0; a < M; a++) h[a] = zs[(S * M + a) * UB + tid];
+                    bke_hook_residual_z<T>(h, zm, dz);
+                } else {
+#pragma unroll
+                    for (int a = 0; a < M; a++) dz[a] = zs[(S * M + a) * UB + tid] - zm[a];
+                }
                 const T w = (S == 0) ? p.wc0 : p.wi;
 #pragma unroll
                 for (int a = 0; a < M; a++) {
@@ -509,8 +563,19 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
 #pragma unroll
                     for (int b = a; b < M; b++) o.S[a][b] += wd * dz[b];
                 }
-                // dx = sigma - x is the sigma offset itself: row k of +-U, zero left of the diagonal
-                if constexpr (S > 0) {
+                if constexpr (HOOKS & BKE_HOOK_RESIDUAL_X) {
+                    // dx = residual_x(sigma, x) (UKF.py:501): the point itself, not the offset row
+                    T sp[N], dx[N];
+                    sigma_point<T, N, S>(x, U, sp);
+                    bke_hook_residual_x<T>(sp, x, dx);
+#pragma unroll
+                    for (int i = 0; i < N; i++) {
+                        T wd = w * dx[i];
+#pragma unroll
+                        for (int a = 0; a < M; a++) Pxz[i][a] += wd * dz[a];
+                    }
+                } else if constexpr (S > 0) {
+                    // dx = sigma - x is the sigma offset itself: row k of +-U, zero left of the diagonal
                     constexpr int k = (S - 1) % N;
                     const T ws = (S <= N) ? w : -w;
 #pragma unroll
@@ -543,14 +608,32 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
                         for (int b = 1; b < M; b++) s += Pxz[i][b] * o.SI[b][a];
                         o.K[i][a] = s;
                     }
+                if constexpr (HOOKS & BKE_HOOK_RESIDUAL_Z) {
+                    bke_hook_residual_z<T>(zv, zm, o.y);                  // UKF.py:477
+                } else {
 #pragma unroll
-                for (int a = 0; a < M; a++) o.y[a] = zv[a] - zm[a];
+                    for (int a = 0; a < M; a++) o.y[a] = zv[a] - zm[a];
+                }
+                if constexpr (HOOKS & BKE_HOOK_STATE_ADD) {
+                    T ky[N], xn[N];                                        // state_add(x, K y) (UKF.py:480)
 #pragma unroll
-                for (int i = 0; i < N; i++) {
-                    T s = x[i];
+                    for (int i = 0; i < N; i++) {
+                        T s = o.K[i][0] * o.y[0];
 #pragma unroll
-                    for (int a = 0; a < M; a++) s += o.K[i][a] * o.y[a];
-                    x[i] = s;
+                        for (int a = 1; a < M; a++) s += o.K[i][a] * o.y[a];
+                        ky[i] = s;
+                    }
+                    bke_hook_state_add<T>(x, ky, xn);
+#pragma unroll
+                    for (int i = 0; i < N; i++) x[i] = xn[i];
+                } else {
+#pragma unroll
+                    for (int i = 0; i < N; i++) {
+                        T s = x[i];
+#pragma unroll
+                        for (int a = 0; a < M; a++) s += o.K[i][a] * o.y[a];
+                        x[i] = s;
+                    }
                 }
                 // optional outputs leave now, while S, SI, y are still in registers
                 if (UKF_EXTRAS && live) {

@@ -37,7 +37,8 @@ struct bke_ukf_model {
     int n, m, dtype, fx_model, hx_model;
     cudaLibrary_t lib;
     cudaKernel_t kern[2];          // [0] plain, [1] with the optional outputs
-    cudaKernel_t kern_rts;         // RTS smoother around the user's fx (NULL: fx is built in, or dim_x > UR_MAXN)
+    cudaKernel_t kern_rts;         // RTS smoother around the user's fx or hooks (NULL: neither, or dim_x > UR_MAXN)
+    unsigned hooks;                // BKE_HOOK_* mask the program was compiled with
     int regs[2];
     std::string log;
 };
@@ -159,19 +160,37 @@ extern "C" {
 
 // NVRTC half of bke_ukf_model_compile / bke_ckf_model_compile (needs no GPU): program text -> sm_90a cubin
 // + the lowered names of the kernel instances of the family (the step with / without the optional outputs
-// and, for a UKF around a user fx, the RTS smoother)
-static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
-                         const char *include_dirs, std::vector<char> &cubin, std::string (&lowered)[3], std::string &log)
+// and, for a UKF around a user fx or hooks, the RTS smoother)
+static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, unsigned hooks,
+                         const char *source, const char *include_dirs, std::vector<char> &cubin, std::string (&lowered)[3], std::string &log)
 {
     const bool ckf = family == BKE_FAMILY_CKF, enkf = family == BKE_FAMILY_ENKF;
-    const char *fn = enkf ? "bke_enkf_model_compile" : ckf ? "bke_ckf_model_compile" : "bke_ukf_model_compile";
+    const char *fn = hooks ? (ckf ? "bke_ckf_model_compile_hooks" : "bke_ukf_model_compile_hooks")
+                           : enkf ? "bke_enkf_model_compile" : ckf ? "bke_ckf_model_compile" : "bke_ukf_model_compile";
     if (dim_x < 1 || dim_x > 16 || dim_z < 1 || dim_z > dim_x + 8) { set_error("%s: 1 <= dim_x <= 16, 1 <= dim_z", fn); return BKE_ERR_BAD_ARG; }
     if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
     const bool ufx = fx_model == BKE_FX_USER, uhx = hx_model == BKE_HX_USER;
-    if (!ufx && !uhx) { set_error("%s: neither fx nor hx is BKE_*_USER (use %s)", fn, enkf ? "bke_enkf_step" : ckf ? "bke_ckf_step" : "bke_ukf_step"); return BKE_ERR_BAD_ARG; }
-    if ((!ufx && fx_model != BKE_FX_LINEAR && fx_model != BKE_FX_CONST_VEL) || (!uhx && hx_model != BKE_HX_LINEAR)) {
-        set_error("%s: the built-in partner of a user function must be BKE_FX_LINEAR / BKE_FX_CONST_VEL / BKE_HX_LINEAR", fn);
-        return BKE_ERR_BAD_ARG;
+    const unsigned all_hooks = BKE_HOOK_X_MEAN | BKE_HOOK_Z_MEAN | BKE_HOOK_RESIDUAL_X | BKE_HOOK_RESIDUAL_Z | BKE_HOOK_STATE_ADD;
+    if (hooks) {
+        if ((hooks & ~all_hooks) || enkf) { set_error("%s: unknown hook bits 0x%x", fn, hooks); return BKE_ERR_BAD_ARG; }
+        if (ckf && hooks != BKE_HOOK_RESIDUAL_Z) {
+            set_error("%s: the CKF calls residual_z only (CubatureKalmanFilter.py:376); hooks must be BKE_HOOK_RESIDUAL_Z", fn);
+            return BKE_ERR_BAD_ARG;
+        }
+        if (dim_x > UR_MAXN) { set_error("%s: hooks are supported up to dim_x = %d (got %d)", fn, UR_MAXN, dim_x); return BKE_ERR_UNSUPPORTED; }
+        // any model may go with hooks: the built-in transcendental ones read the positions at 0, 2 (, 4)
+        if ((!ufx && fx_model != BKE_FX_LINEAR && fx_model != BKE_FX_CONST_VEL) ||
+            (!uhx && hx_model != BKE_HX_LINEAR && !(hx_model == BKE_HX_RANGE_BEARING && dim_z == 2 && dim_x >= 3) &&
+             !(hx_model == BKE_HX_RANGE_AZ_EL && dim_z == 3 && dim_x >= 5))) {
+            set_error("%s: unknown fx / hx model, or a range model whose dim_x / dim_z it cannot serve", fn);
+            return BKE_ERR_BAD_ARG;
+        }
+    } else {
+        if (!ufx && !uhx) { set_error("%s: neither fx nor hx is BKE_*_USER (use %s)", fn, enkf ? "bke_enkf_step" : ckf ? "bke_ckf_step" : "bke_ukf_step"); return BKE_ERR_BAD_ARG; }
+        if ((!ufx && fx_model != BKE_FX_LINEAR && fx_model != BKE_FX_CONST_VEL) || (!uhx && hx_model != BKE_HX_LINEAR)) {
+            set_error("%s: the built-in partner of a user function must be BKE_FX_LINEAR / BKE_FX_CONST_VEL / BKE_HX_LINEAR", fn);
+            return BKE_ERR_BAD_ARG;
+        }
     }
     if (!ufx && fx_model == BKE_FX_CONST_VEL && (dim_x & 1)) { set_error("BKE_FX_CONST_VEL needs an even dim_x"); return BKE_ERR_BAD_ARG; }
     if (!source || !include_dirs) { set_error("source and include_dirs must be non-NULL"); return BKE_ERR_BAD_ARG; }
@@ -181,12 +200,19 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     std::string text;
     text += dtype == BKE_F64 ? "typedef double real;\n" : "typedef float real;\n";
     text += "#define BKE_DIM_X " + std::to_string(dim_x) + "\n#define BKE_DIM_Z " + std::to_string(dim_z) + "\n";
+    if (hooks)       // the hook-free text stays byte-identical
+        text += "#define BKE_UKF_HOOKS " + std::to_string(hooks) + "u\n#define BKE_N_SIGMAS " + std::to_string(ckf ? 2 * dim_x : 2 * dim_x + 1) + "\n";
     text += enkf ? "#include \"enkf_kernel.cuh\"\n" : ckf ? "#include \"ckf_kernel.cuh\"\n" : "#include \"ukf_kernel.cuh\"\n#include \"ukf_rts_kernel.cuh\"\n";
     text += "#line 1 \"user_model.cu\"\n";
     text += source;
     text += "\n#line 1 \"bke_glue.cu\"\nnamespace bke { namespace ukfk {\n";
     if (ufx) text += "template <> __device__ __forceinline__ void bke_user_fx<real>(const real *x, real *out, real dt, const real *args) { ::fx(x, out, dt, args); }\n";
     if (uhx) text += "template <> __device__ __forceinline__ void bke_user_hx<real>(const real *x, real *z, const real *args) { ::hx(x, z, args); }\n";
+    if (hooks & BKE_HOOK_X_MEAN) text += "template <> __device__ __forceinline__ void bke_hook_x_mean<real>(const real *s, const real *w, real *o) { ::x_mean_fn(s, w, o); }\n";
+    if (hooks & BKE_HOOK_Z_MEAN) text += "template <> __device__ __forceinline__ void bke_hook_z_mean<real>(const real *s, const real *w, real *o) { ::z_mean_fn(s, w, o); }\n";
+    if (hooks & BKE_HOOK_RESIDUAL_X) text += "template <> __device__ __forceinline__ void bke_hook_residual_x<real>(const real *a, const real *b, real *o) { ::residual_x(a, b, o); }\n";
+    if (hooks & BKE_HOOK_RESIDUAL_Z) text += "template <> __device__ __forceinline__ void bke_hook_residual_z<real>(const real *a, const real *b, real *o) { ::residual_z(a, b, o); }\n";
+    if (hooks & BKE_HOOK_STATE_ADD) text += "template <> __device__ __forceinline__ void bke_hook_state_add<real>(const real *a, const real *b, real *o) { ::state_add(a, b, o); }\n";
     text += "} }\n";
 
     const int occ = enkf ? 0 : ckf ? ckf_occupancy(dim_x, dtype == BKE_F64) : ukf_occupancy(dim_x, dtype == BKE_F64);
@@ -208,10 +234,11 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     }
     std::vector<const char *> copts;
     for (auto &o : opts) copts.push_back(o.c_str());
-    // the step kernel with / without the optional outputs and, around a user fx, the RTS smoother
-    const bool with_rts = !ckf && !enkf && ufx && dim_x <= UR_MAXN;
+    // the step kernel with / without the optional outputs and, around a user fx or hooks, the RTS smoother
+    const bool with_rts = !ckf && !enkf && (ufx || hooks) && dim_x <= UR_MAXN;
     const int n_names = with_rts ? 3 : 2;
-    const std::string names[3] = {kernel_name(tmp, occ, false), kernel_name(tmp, occ, true), "bke::ukf_rts_kernel<real, true>"};
+    const std::string names[3] = {kernel_name(tmp, occ, false), kernel_name(tmp, occ, true),
+                                  ufx ? "bke::ukf_rts_kernel<real, true>" : "bke::ukf_rts_kernel<real, false>"};
     for (int i = 0; i < n_names; i++) rt->add_name(prog, names[i].c_str());
     r = rt->compile(prog, (int)copts.size(), copts.data());
     size_t lsz = 0;
@@ -241,17 +268,18 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     return BKE_OK;
 }
 
-static int model_compile(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
-                         const char *include_dirs, bke_ukf_model **out)
+static int model_compile(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, unsigned hooks,
+                         const char *source, const char *include_dirs, bke_ukf_model **out)
 {
     if (!out) { set_error("out is NULL"); return BKE_ERR_BAD_ARG; }
     *out = nullptr;
     std::vector<char> cubin;
     std::string lowered[3], log;
-    int rc = compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, cubin, lowered, log);
+    int rc = compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs, cubin, lowered, log);
     if (rc != BKE_OK) return rc;
     bke_ukf_model *m = new bke_ukf_model();
     m->family = family; m->n = dim_x; m->m = dim_z; m->dtype = dtype; m->fx_model = fx_model; m->hx_model = hx_model; m->lib = nullptr; m->log = log;
+    m->hooks = hooks;
     m->kern_rts = nullptr;
     if (check_cuda(cudaLibraryLoadData(&m->lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0), "cudaLibraryLoadData")) { delete m; return BKE_ERR_CUDA; }
     for (int i = 0; i < 2; i++) {
@@ -274,47 +302,71 @@ static int model_compile(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
 int bke_ukf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
                           const char *include_dirs, bke_ukf_model **out)
 {
-    return model_compile(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, out);
+    return model_compile(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, 0u, source, include_dirs, out);
 }
 
 int bke_enkf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
                            const char *include_dirs, bke_ukf_model **out)
 {
-    return model_compile(BKE_FAMILY_ENKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, out);
+    return model_compile(BKE_FAMILY_ENKF, dim_x, dim_z, dtype, fx_model, hx_model, 0u, source, include_dirs, out);
 }
 
 int bke_ckf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
                           const char *include_dirs, bke_ukf_model **out)
 {
-    return model_compile(BKE_FAMILY_CKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, out);
+    return model_compile(BKE_FAMILY_CKF, dim_x, dim_z, dtype, fx_model, hx_model, 0u, source, include_dirs, out);
+}
+
+int bke_ukf_model_compile_hooks(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, uint32_t hooks,
+                                const char *source, const char *include_dirs, bke_ukf_model **out)
+{
+    return model_compile(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs, out);
+}
+
+int bke_ckf_model_compile_hooks(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, uint32_t hooks,
+                                const char *source, const char *include_dirs, bke_ukf_model **out)
+{
+    return model_compile(BKE_FAMILY_CKF, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs, out);
 }
 
 // the NVRTC half alone (CPU-only check that a model's text compiles for sm_90a): cubin size or 0
-static size_t cubin_bytes(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
-                          const char *include_dirs)
+static size_t cubin_bytes(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, unsigned hooks,
+                          const char *source, const char *include_dirs)
 {
     std::vector<char> cubin;
     std::string lowered[3], log;
-    if (compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs, cubin, lowered, log) != BKE_OK) return 0;
+    if (compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs, cubin, lowered, log) != BKE_OK) return 0;
     return cubin.size();
 }
 
 size_t bke_debug_ukf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
                                        const char *include_dirs)
 {
-    return cubin_bytes(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs);
+    return cubin_bytes(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, 0u, source, include_dirs);
 }
 
 size_t bke_debug_ckf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
                                        const char *include_dirs)
 {
-    return cubin_bytes(BKE_FAMILY_CKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs);
+    return cubin_bytes(BKE_FAMILY_CKF, dim_x, dim_z, dtype, fx_model, hx_model, 0u, source, include_dirs);
 }
 
 size_t bke_debug_enkf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
                                         const char *include_dirs)
 {
-    return cubin_bytes(BKE_FAMILY_ENKF, dim_x, dim_z, dtype, fx_model, hx_model, source, include_dirs);
+    return cubin_bytes(BKE_FAMILY_ENKF, dim_x, dim_z, dtype, fx_model, hx_model, 0u, source, include_dirs);
+}
+
+size_t bke_debug_ukf_model_hooks_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
+                                             uint32_t hooks, const char *source, const char *include_dirs)
+{
+    return cubin_bytes(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs);
+}
+
+size_t bke_debug_ckf_model_hooks_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
+                                             uint32_t hooks, const char *source, const char *include_dirs)
+{
+    return cubin_bytes(BKE_FAMILY_CKF, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs);
 }
 
 const char *bke_ukf_model_log(const bke_ukf_model *m) { return m ? m->log.c_str() : ""; }
@@ -361,8 +413,10 @@ int bke_ukf_rts_smoother_model(const bke_ukf_rts_args *args, const bke_ukf_model
     if (!args || !model) { set_error("args / model is NULL"); return BKE_ERR_BAD_ARG; }
     const bke_ukf_rts_args &a = *args;
     if (model->family != BKE_FAMILY_UKF) { set_error("bke_ukf_rts_smoother_model: the model was compiled for the CKF (bke_ckf_model_compile)"); return BKE_ERR_BAD_ARG; }
-    if (!model->kern_rts) { set_error("bke_ukf_rts_smoother_model: the model has no user fx (use bke_ukf_rts_smoother) or dim_x > %d", UR_MAXN); return BKE_ERR_UNSUPPORTED; }
-    if (a.dim_x != model->n || a.dtype != model->dtype || a.fx_model != BKE_FX_USER) { set_error("bke_ukf_rts_smoother_model: args do not match the compiled model"); return BKE_ERR_BAD_ARG; }
+    if (!model->kern_rts) { set_error("bke_ukf_rts_smoother_model: the model has neither a user fx nor hooks (use bke_ukf_rts_smoother) or dim_x > %d", UR_MAXN); return BKE_ERR_UNSUPPORTED; }
+    if (a.dim_x != model->n || a.dtype != model->dtype || a.fx_model != model->fx_model) { set_error("bke_ukf_rts_smoother_model: args do not match the compiled model"); return BKE_ERR_BAD_ARG; }
+    if (a.fx_model == BKE_FX_CONST_VEL && (a.dim_x & 1)) { set_error("BKE_FX_CONST_VEL needs an even dim_x"); return BKE_ERR_BAD_ARG; }
+    if (a.fx_model == BKE_FX_LINEAR && (!a.F || a.F_stride < 0)) { set_error("BKE_FX_LINEAR needs F"); return BKE_ERR_BAD_ARG; }
     if (a.n_filters < 0 || a.n_steps < 0 || fx_args_stride < 0 || a.Q_stride < 0) { set_error("negative sizes"); return BKE_ERR_BAD_ARG; }
     if (a.n_filters == 0 || a.n_steps == 0) return BKE_OK;
     if (!a.Xs || !a.Ps || !a.Q || !a.x_out || !a.P_out) { set_error("NULL argument"); return BKE_ERR_BAD_ARG; }

@@ -99,6 +99,11 @@ __global__ void __launch_bounds__(64) ukf_rts_kernel(UrP<T> p)
                 const T w = s == 0 ? p.wm0 : p.wi;
                 for (int i = 0; i < n; i++) xb[i] += w * fo[i];
             }
+            if constexpr (ukfk::HOOKS & BKE_HOOK_X_MEAN) {            // xb = x_mean_fn(sigmas_f, Wm) (:720-722)
+                T Wm[2 * UR_MAXN + 1];
+                for (int s = 0; s < ns; s++) Wm[s] = s == 0 ? p.wm0 : p.wi;
+                ukfk::bke_hook_x_mean<T>(sf, Wm, xb);
+            }
             // Pb = sum Wc y y' + Q ;  Pxb = sum Wc z y'   (z = sigma - Xs[k] = +-U row, y = f(sigma) - xb)
             for (int i = 0; i < n * n; i++) { Pb[i] = T(0); Pxb[i] = T(0); }
             for (int s = 0; s < ns; s++) {
@@ -106,6 +111,18 @@ __global__ void __launch_bounds__(64) ukf_rts_kernel(UrP<T> p)
                 const int row = s == 0 ? 0 : (s - 1) % n;
                 const T sign = s == 0 ? T(0) : (s <= n ? T(1) : T(-1));
                 T y[UR_MAXN];
+                if constexpr (ukfk::HOOKS & BKE_HOOK_RESIDUAL_X) {
+                    // y = residual_x(sigmas_f[i], xb), z = residual_x(sigmas[i], Xs[k]) (:727-728)
+                    T sp[UR_MAXN], z[UR_MAXN];
+                    ukfk::bke_hook_residual_x<T>(sf + s * n, xb, y);
+                    for (int i = 0; i < n; i++) sp[i] = (s == 0) ? xk[i] : xk[i] + sign * U[row * n + i];
+                    ukfk::bke_hook_residual_x<T>(sp, xk, z);
+                    for (int i = 0; i < n; i++) {
+                        const T wy = w * y[i], wz = w * z[i];
+                        for (int j = 0; j < n; j++) { Pb[i * n + j] += wy * y[j]; Pxb[i * n + j] += wz * y[j]; }
+                    }
+                    continue;
+                }
                 for (int i = 0; i < n; i++) y[i] = sf[s * n + i] - xb[i];
                 for (int i = 0; i < n; i++) {
                     const T wy = w * y[i];
@@ -148,10 +165,20 @@ __global__ void __launch_bounds__(64) ukf_rts_kernel(UrP<T> p)
                     for (int q = 0; q < n; q++) s += Pxb[i * n + q] * PbI[q * n + j];
                     Kk[i * n + j] = s;
                 }
-            for (int i = 0; i < n; i++) {
-                T s = T(0);
-                for (int q = 0; q < n; q++) s += Kk[i * n + q] * (xs[q] - xb[q]);
-                xk[i] += s;
+            if constexpr (ukfk::HOOKS & BKE_HOOK_RESIDUAL_X) {
+                T r[UR_MAXN];                                      // residual_x(xs[k+1], xb) (:735; no state_add)
+                ukfk::bke_hook_residual_x<T>(xs, xb, r);
+                for (int i = 0; i < n; i++) {
+                    T s = T(0);
+                    for (int q = 0; q < n; q++) s += Kk[i * n + q] * r[q];
+                    xk[i] += s;
+                }
+            } else {
+                for (int i = 0; i < n; i++) {
+                    T s = T(0);
+                    for (int q = 0; q < n; q++) s += Kk[i * n + q] * (xs[q] - xb[q]);
+                    xk[i] += s;
+                }
             }
             for (int i = 0; i < n; i++)
                 for (int j = 0; j < n; j++) {

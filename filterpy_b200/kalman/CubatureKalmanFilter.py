@@ -10,7 +10,7 @@ import torch
 
 from .. import _lib
 from .._dev import ptr
-from .UKF import _DeviceModel, _SigmaPointBank, _compile_model, _no_hook, _require_device_models
+from .UKF import _DeviceModel, _SigmaPointBank, _compile_model, _device_hooks, _no_hook, _require_device_models
 
 __all__ = ["CubatureKalmanFilter"]
 
@@ -46,15 +46,17 @@ class CubatureKalmanFilter(_SigmaPointBank):
     reading ``x`` or by ``update(None)``) still writes them.
     """
 
-    _compile_model = staticmethod(lambda *a: _compile_model(*a, entry="bke_ckf_model_compile"))
+    _compile_model = staticmethod(lambda *a, **k: _compile_model(*a, entry="bke_ckf_model_compile", **k))
 
     def __init__(self, dim_x, dim_z, dt, hx, fx, x_mean_fn=None, z_mean_fn=None, residual_x=None,
                  residual_z=None, n_filters=None, dtype=np.float64, device=None, diagnostics=True):
-        for nm, v in (("x_mean_fn", x_mean_fn), ("z_mean_fn", z_mean_fn), ("residual_x", residual_x),
-                      ("residual_z", residual_z)):
+        # the reference stores x_mean_fn, z_mean_fn and residual_x but never calls them; residual_z forms
+        # y = residual_z(z, z^) (:376) and may be a DeviceFn
+        for nm, v in (("x_mean_fn", x_mean_fn), ("z_mean_fn", z_mean_fn), ("residual_x", residual_x)):
             _no_hook(nm, v)
+        hooks = _device_hooks(residual_z=residual_z)
         _require_device_models(fx, hx)
-        self._init_bank(dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics)
+        self._init_bank(dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics, hooks)
         self._dt = dt
         self._num_sigmas = 2 * self.dim_x
         shape = (self.n_filters, self._num_sigmas, self.dim_x)

@@ -12,9 +12,10 @@ closed set of include/bke.h instead:
     hx = RangeAzElHx()      n=6 (x,vx,y,vy,z,vz) -> (range, azimuth, elevation)
     hx = RangeBearingHx()   n=4 (x,vx,y,vy)      -> (range, bearing)
 
-Passing a Python callable, or any of the hook arguments (sqrt_fn, x_mean_fn, z_mean_fn,
-residual_x, residual_z, state_add, per-call UT / fx / hx), raises NotImplementedError: there is no
-CPU fallback.  As for the linear filter, ``n_filters=None`` gives a single-filter drop-in whose
+The mean / residual / state-add hooks (x_mean_fn, z_mean_fn, residual_x, residual_z, state_add,
+UKF.py:97-140), with which the reference wraps angles and takes circular means, are accepted as
+``DeviceFn`` source text and compiled into the kernels.  Passing a Python callable for any hook or
+model, sqrt_fn, or a per-call UT / fx / hx raises NotImplementedError: there is no CPU fallback.  As for the linear filter, ``n_filters=None`` gives a single-filter drop-in whose
 attributes are NumPy arrays (``x`` is 1-D, UKF.py:298).
 """
 import ctypes
@@ -27,7 +28,7 @@ from .._dev import bke_dtype, ptr, stream_ptr
 from ._bank import _BankMirror, _model_prop
 
 __all__ = ["UnscentedKalmanFilter", "LinearFx", "ConstVelFx", "LinearHx", "RangeAzElHx", "RangeBearingHx",
-           "DeviceFx", "DeviceHx"]
+           "DeviceFx", "DeviceHx", "DeviceFn"]
 
 
 class LinearFx(object):
@@ -116,19 +117,64 @@ class DeviceHx(_DeviceModel):
     model = _lib.BKE_HX_USER
 
 
+class DeviceFn(object):
+    """One of the reference's hooks (UKF.py:97-140) as CUDA C++ source text.  The keyword it is passed as
+    names the ``__device__`` function the text defines, for the element type ``real`` (n = ``BKE_DIM_X``,
+    m = ``BKE_DIM_Z``, ``BKE_N_SIGMAS`` points)::
+
+        __device__ void residual_x(const real *a, const real *b, real *out);        # out = a - b, n
+        __device__ void residual_z(const real *a, const real *b, real *out);        # out = a - b, m
+        __device__ void state_add(const real *a, const real *b, real *out);         # out = a + b, n
+        __device__ void x_mean_fn(const real *sigmas, const real *Wm, real *out);   # sigmas [BKE_N_SIGMAS][n]
+        __device__ void z_mean_fn(const real *sigmas, const real *Wm, real *out);   # sigmas [BKE_N_SIGMAS][m]
+
+    One object may define several of them and be passed for each: its text is included once."""
+
+    def __init__(self, source):
+        self.source = str(source)
+
+
+_HOOK_BITS = (("x_mean_fn", _lib.BKE_HOOK_X_MEAN), ("z_mean_fn", _lib.BKE_HOOK_Z_MEAN),
+              ("residual_x", _lib.BKE_HOOK_RESIDUAL_X), ("residual_z", _lib.BKE_HOOK_RESIDUAL_Z),
+              ("state_add", _lib.BKE_HOOK_STATE_ADD))
+
+
+def _device_hooks(**given):
+    """The ``BKE_HOOK_*`` mask of the hooks given as ``DeviceFn`` and their distinct objects in keyword order;
+    a Python callable raises NotImplementedError."""
+    mask, fns = 0, []
+    for nm, bit in _HOOK_BITS:
+        v = given.get(nm)
+        if v is None:
+            continue
+        if not isinstance(v, DeviceFn):
+            _no_hook(nm, v)
+        mask |= bit
+        if not any(v is f for f in fns):
+            fns.append(v)
+    return mask, tuple(fns)
+
+
 _compiled_models = {}
 
 
-def _compile_model(lib, dim_x, dim_z, dtype_id, fx, hx, entry="bke_ukf_model_compile"):
-    """One NVRTC build per (filter family, shape, dtype, source); shared by every filter object that uses it.
-    ``entry`` names the family's compile call (bke_ukf_model_compile / bke_ckf_model_compile)."""
-    src = "\n".join(m.source for m in (fx, hx) if isinstance(m, _DeviceModel))
-    key = (entry, dim_x, dim_z, dtype_id, fx.model, hx.model, src)
+def _compile_model(lib, dim_x, dim_z, dtype_id, fx, hx, entry="bke_ukf_model_compile", hooks=(0, ())):
+    """One NVRTC build per (filter family, shape, dtype, hooks, source); shared by every filter object that
+    uses it.  ``entry`` names the family's compile call (bke_ukf_model_compile / bke_ckf_model_compile);
+    ``hooks`` is what ``_device_hooks`` returns."""
+    mask, fns = hooks
+    src = "\n".join([m.source for m in (fx, hx) if isinstance(m, _DeviceModel)] + [f.source for f in fns])
+    key = (entry, dim_x, dim_z, dtype_id, fx.model, hx.model, mask, src)
     h = _compiled_models.get(key)
     if h is None:
         out = ctypes.c_void_p()
-        _lib.check(getattr(lib, entry)(dim_x, dim_z, dtype_id, fx.model, hx.model, src.encode(),
-                                       _lib.kernel_include_dirs().encode(), ctypes.byref(out)))
+        inc = _lib.kernel_include_dirs().encode()
+        if mask:
+            rc = getattr(lib, entry + "_hooks")(dim_x, dim_z, dtype_id, fx.model, hx.model, mask, src.encode(), inc,
+                                                 ctypes.byref(out))
+        else:
+            rc = getattr(lib, entry)(dim_x, dim_z, dtype_id, fx.model, hx.model, src.encode(), inc, ctypes.byref(out))
+        _lib.check(rc)
         h = _compiled_models[key] = out
     return h
 
@@ -156,9 +202,9 @@ class _SigmaPointBank(_BankMirror):
     _COLUMN_X = False                                   # x is 1-D (UKF.py:298)
     _FAILURE = "matrix not positive definite / singular"
 
-    def _init_bank(self, dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics):
-        """The state, models, compiled user model and diagnostic buffers of a bank (the reference's
-        __init__ defaults: x = 0, P = I, Q = I, R = I)."""
+    def _init_bank(self, dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics, hooks=(0, ())):
+        """The state, models, compiled user model (around DeviceFx / DeviceHx or ``hooks``) and diagnostic
+        buffers of a bank (the reference's __init__ defaults: x = 0, P = I, Q = I, R = I)."""
         _BankMirror._init_bank(self, dim_x, dim_z, n_filters, dtype, device, diagnostics)
         self.fx, self.hx = fx, hx
         N, n, m = self.n_filters, self.dim_x, self.dim_z
@@ -173,9 +219,10 @@ class _SigmaPointBank(_BankMirror):
         self._z = None
         self._user_model = None
         self._fx_args = self._hx_args = (None, 0)
-        if isinstance(fx, _DeviceModel) or isinstance(hx, _DeviceModel):
+        self._hooks = hooks[0]
+        if isinstance(fx, _DeviceModel) or isinstance(hx, _DeviceModel) or self._hooks:
             with torch.cuda.device(self._device):
-                self._user_model = self._compile_model(self._lib, n, m, bke_dtype(self._dtype), fx, hx)
+                self._user_model = self._compile_model(self._lib, n, m, bke_dtype(self._dtype), fx, hx, hooks=hooks)
             if isinstance(fx, _DeviceModel):
                 self._fx_args = fx.pack({}, N, self._dtype, self._device) if all(k in fx.values for k in fx.arg_names) else (None, 0)
             if isinstance(hx, _DeviceModel):
@@ -248,13 +295,13 @@ class UnscentedKalmanFilter(_SigmaPointBank):
     def __init__(self, dim_x, dim_z, dt, hx, fx, points, sqrt_fn=None, x_mean_fn=None, z_mean_fn=None,
                  residual_x=None, residual_z=None, state_add=None,
                  n_filters=None, dtype=np.float64, device=None, diagnostics=True):
-        for nm, v in (("sqrt_fn", sqrt_fn), ("x_mean_fn", x_mean_fn), ("z_mean_fn", z_mean_fn),
-                      ("residual_x", residual_x), ("residual_z", residual_z), ("state_add", state_add)):
-            _no_hook(nm, v)
+        _no_hook("sqrt_fn", sqrt_fn)
+        hooks = _device_hooks(x_mean_fn=x_mean_fn, z_mean_fn=z_mean_fn, residual_x=residual_x,
+                              residual_z=residual_z, state_add=state_add)
         _require_device_models(fx, hx)
         if points.n != dim_x:
             raise ValueError("expected size(x) {}, but size is {}".format(points.n, dim_x))   # sigma_points.py:153
-        self._init_bank(dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics)
+        self._init_bank(dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics, hooks)
         self.points_fn = points
         self._dt = dt
         self._num_sigmas = points.num_sigmas()
@@ -336,10 +383,10 @@ class UnscentedKalmanFilter(_SigmaPointBank):
             a.F, a.F_stride = ptr(self._F), self._stride(self._F)
         a.x_out, a.P_out, a.K = ptr(xs), ptr(Pso), ptr(Ks)
         a.status = ptr(status)
-        if isinstance(self.fx, _DeviceModel):
+        if isinstance(self.fx, _DeviceModel) or self._hooks:
             # the reference calls self.fx(sigma, dt) without keyword arguments here (UKF.py:712): the model's
             # current argument values stand in for the defaults of its callable
-            if self.fx.arg_names and self._fx_args[0] is None:
+            if isinstance(self.fx, _DeviceModel) and self.fx.arg_names and self._fx_args[0] is None:
                 raise TypeError("fx needs values for its arguments %s" % list(self.fx.arg_names))
             self._run(self._lib.bke_ukf_rts_smoother_model, ctypes.byref(a), self._user_model, ptr(self._fx_args[0]),
                       self._fx_args[1], stream_ptr(self._device))

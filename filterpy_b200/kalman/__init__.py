@@ -2,7 +2,7 @@
 from .kalman_filter import KalmanFilter, predict, update, batch_filter, rts_smoother  # noqa: F401
 from .sigma_points import MerweScaledSigmaPoints, JulierSigmaPoints  # noqa: F401
 from .UKF import (UnscentedKalmanFilter, LinearFx, ConstVelFx, LinearHx, RangeAzElHx,  # noqa: F401
-                  RangeBearingHx, DeviceFx, DeviceHx)
+                  RangeBearingHx, DeviceFx, DeviceHx, DeviceFn)
 from .CubatureKalmanFilter import CubatureKalmanFilter  # noqa: F401
 from .ensemble_kalman_filter import EnsembleKalmanFilter  # noqa: F401
 from .square_root import SquareRootKalmanFilter  # noqa: F401

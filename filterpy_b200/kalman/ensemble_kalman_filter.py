@@ -47,7 +47,7 @@ class EnsembleKalmanFilter(_SigmaPointBank):
     (0 = no measurement) skips the update of single filters, as ``z=None`` does for the whole bank.
     """
 
-    _compile_model = staticmethod(lambda *a: _compile_model(*a, entry="bke_enkf_model_compile"))
+    _compile_model = staticmethod(lambda *a, **k: _compile_model(*a, entry="bke_enkf_model_compile", **k))
     _FAILURE = "covariance not positive semi-definite / singular S"
 
     def __init__(self, x, P, dim_z, dt, N, hx, fx, n_filters=None, dtype=np.float64, device=None,

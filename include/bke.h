@@ -321,6 +321,28 @@ int bke_ukf_step_model(const bke_ukf_args *args, const bke_ukf_model *model, con
 size_t bke_debug_ukf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
                                        const char *source, const char *include_dirs);
 
+/* The reference's mean / residual / state-add hooks (UKF.py:97-140: x_mean_fn, z_mean_fn, residual_x,
+ * residual_z, state_add), e.g. to wrap angles and take circular means, cross as source text too.  `hooks`
+ * is a mask of the functions `source` defines (n = BKE_DIM_X, m = BKE_DIM_Z, BKE_N_SIGMAS = 2n + 1):
+ *     __device__ void x_mean_fn(const real *sigmas, const real *Wm, real *out);   sigmas[BKE_N_SIGMAS][n]  BKE_HOOK_X_MEAN
+ *     __device__ void z_mean_fn(const real *sigmas, const real *Wm, real *out);   sigmas[BKE_N_SIGMAS][m]  BKE_HOOK_Z_MEAN
+ *     __device__ void residual_x(const real *a, const real *b, real *out);        out = a - b, n           BKE_HOOK_RESIDUAL_X
+ *     __device__ void residual_z(const real *a, const real *b, real *out);        out = a - b, m           BKE_HOOK_RESIDUAL_Z
+ *     __device__ void state_add(const real *a, const real *b, real *out);         out = a + b, n           BKE_HOOK_STATE_ADD
+ * With hooks != 0 any fx / hx model may be compiled, built-in or user; the handle also carries the RTS
+ * smoother (bke_ukf_rts_smoother_model), which calls x_mean_fn and residual_x as UKF.py:720-735 does.
+ * Hooks need dim_x <= 8 (BKE_ERR_UNSUPPORTED otherwise).  hooks == 0 is bke_ukf_model_compile exactly.
+ * The handle is launched with bke_ukf_step_model. */
+#define BKE_HOOK_X_MEAN 1u
+#define BKE_HOOK_Z_MEAN 2u
+#define BKE_HOOK_RESIDUAL_X 4u
+#define BKE_HOOK_RESIDUAL_Z 8u
+#define BKE_HOOK_STATE_ADD 16u
+int bke_ukf_model_compile_hooks(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, uint32_t hooks,
+                                const char *source, const char *include_dirs, bke_ukf_model **out);
+size_t bke_debug_ukf_model_hooks_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
+                                             uint32_t hooks, const char *source, const char *include_dirs);
+
 /* ------------------------------------------------------------------------------------------
  * Cubature Kalman filter bank.
  * Replaces CubatureKalmanFilter.predict / update (filterpy/kalman/CubatureKalmanFilter.py:292-327,
@@ -373,6 +395,12 @@ int bke_ckf_step_model(const bke_ckf_args *args, const bke_ukf_model *model, con
 /* the NVRTC half alone (needs no GPU): size of the sm_90a cubin, 0 on failure (log in bke_last_error()) */
 size_t bke_debug_ckf_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
                                        const char *source, const char *include_dirs);
+/* The CKF with hooks: the reference's CKF calls residual_z only (y = residual_z(z, z^), :376), so `hooks`
+ * is 0 or BKE_HOOK_RESIDUAL_Z; otherwise as bke_ukf_model_compile_hooks. */
+int bke_ckf_model_compile_hooks(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, uint32_t hooks,
+                                const char *source, const char *include_dirs, bke_ukf_model **out);
+size_t bke_debug_ckf_model_hooks_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
+                                             uint32_t hooks, const char *source, const char *include_dirs);
 
 /* ------------------------------------------------------------------------------------------
  * Ensemble Kalman filter bank.
@@ -661,7 +689,8 @@ typedef struct {
 } bke_ukf_rts_args;
 
 int bke_ukf_rts_smoother(const bke_ukf_rts_args *args, void *stream);
-/* the same around a user-supplied fx (fx_model = BKE_FX_USER, a model from bke_ukf_model_compile; dim_x <= 8).  The
+/* the same around a user-supplied fx (fx_model = BKE_FX_USER, a model from bke_ukf_model_compile; dim_x <= 8), or
+ * around any fx of a model from bke_ukf_model_compile_hooks (x_mean_fn / residual_x as UKF.py:720-735).  The
  * reference calls self.fx(sigma, dts[k]) WITHOUT keyword arguments here (UKF.py:712): fx_args are the values its
  * callable would default to. */
 int bke_ukf_rts_smoother_model(const bke_ukf_rts_args *args, const bke_ukf_model *model, const void *fx_args,
