@@ -1,5 +1,7 @@
 """Device-memory plumbing shared by the host-side mirrors (torch is used for allocation, streams
 and host<->device copies only; all arithmetic happens in libbke.so)."""
+import ctypes
+
 import numpy as np
 import torch
 
@@ -51,6 +53,12 @@ def stream_ptr(device):
     return torch.cuda.current_stream(device).cuda_stream
 
 
+def _capture_nodes(stream):
+    n = ctypes.c_int64()
+    _lib.check(_lib.load().bke_capture_node_count(stream.cuda_stream, ctypes.byref(n)))
+    return n.value
+
+
 class StepGraph(object):
     """A CUDA graph of a fixed sequence of engine calls (e.g. ``kf.predict(); kf.update(z_buf)`` for a
     ring of measurement buffers).  Replaying it re-runs exactly those kernels on the same device
@@ -59,7 +67,14 @@ class StepGraph(object):
     built with ``diagnostics=False`` and device-resident inputs.  One exception to "the same device
     buffers": a 4/2 float32 bank with symmetric per-filter Q and R is captured reading a packed copy
     of them, so its Q and R are frozen at capture (``KalmanFilter.capture``); re-capture after
-    changing them."""
+    changing them.
+
+    ``nodes`` is the number of graph nodes ``fn`` recorded.  ``launches`` and ``fused_steps`` are set by
+    ``KalmanFilter.capture``: the bank's kernel launches per replay, and how many predict+update steps
+    those launches run as fused rings (0: one launch per step)."""
+
+    launches = None
+    fused_steps = 0
 
     def __init__(self, fn, device, warmup=2):
         side = torch.cuda.Stream(device)
@@ -71,7 +86,9 @@ class StepGraph(object):
         torch.cuda.synchronize(device)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph, stream=side):
+            before = _capture_nodes(side)
             fn()
+            self.nodes = _capture_nodes(side) - before
 
     def replay(self):
         self.graph.replay()

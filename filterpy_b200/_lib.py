@@ -28,6 +28,7 @@ EXPORTED_SYMBOLS = [
     "bke_fls_workspace_bytes", "bke_fls_smooth",
     "bke_kf_sym_models_bytes", "bke_kf_pack_sym_models", "bke_kf_step_sym",
     "bke_kf_scan_models", "bke_kf_packed_models_bytes", "bke_kf_pack_models", "bke_kf_step_packed",
+    "bke_kf_steps_packed", "bke_capture_node_count",
     "bke_resample_workspace_bytes", "bke_systematic_resample", "bke_stratified_resample",
     "bke_weights_sum", "bke_weights_scale", "bke_resample_shard", "bke_resample_normalized",
     "bke_resample_composite_bytes", "bke_resample_shard_compose", "bke_resample_compose_carry", "bke_resample_shard_stage",
@@ -69,6 +70,7 @@ class KfArgs(ctypes.Structure):
 
 
 BKE_KF42_MODEL_WORDS = 37
+BKE_KF42_MAX_RING = 8
 
 
 class KfModelMap(ctypes.Structure):
@@ -331,6 +333,11 @@ def load():
     lib.bke_kf_pack_models.restype = ctypes.c_int
     lib.bke_kf_step_packed.argtypes = [ctypes.POINTER(KfArgs), c_void_p, ctypes.POINTER(KfModelMap), c_void_p]
     lib.bke_kf_step_packed.restype = ctypes.c_int
+    lib.bke_kf_steps_packed.argtypes = [ctypes.POINTER(KfArgs), c_void_p, ctypes.POINTER(KfModelMap),
+                                        ctypes.POINTER(c_void_p), c_int32, c_void_p]
+    lib.bke_kf_steps_packed.restype = ctypes.c_int
+    lib.bke_capture_node_count.argtypes = [c_void_p, ctypes.POINTER(c_int64)]
+    lib.bke_capture_node_count.restype = ctypes.c_int
     lib.bke_kf_batch_filter.argtypes = [ctypes.POINTER(KfBatchArgs), c_void_p]
     lib.bke_kf_batch_filter.restype = ctypes.c_int
     lib.bke_fls_workspace_bytes.argtypes = [c_int64, c_int32, c_int32, c_int32, c_int32, c_int64]

@@ -211,15 +211,20 @@ int bke_kf_pack_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t 
     return launch_kf_pack_models(n_filters, F, Q, H, R, varying, record, (cudaStream_t)stream);
 }
 
-int bke_kf_step_packed(const bke_kf_args *args, const void *record, const bke_kf_model_map *host_map, void *stream)
+static int validate_packed(const void *record, const bke_kf_model_map *host_map)
 {
-    int rc = validate_kf(args, true);
-    if (rc) return rc;
     if (!host_map) { set_error("host_map is NULL"); return BKE_ERR_BAD_ARG; }
     if (bad_mask(host_map->varying)) { set_error("varying has bits above word %d", BKE_KF42_MODEL_WORDS - 1); return BKE_ERR_BAD_ARG; }
     if (host_map->varying && !record) { set_error("record is NULL"); return BKE_ERR_BAD_ARG; }
     int plane[BKE_KF42_MODEL_WORDS];
-    if ((rc = kf_model_planes(*host_map, plane))) return rc;
+    return kf_model_planes(*host_map, plane);
+}
+
+int bke_kf_step_packed(const bke_kf_args *args, const void *record, const bke_kf_model_map *host_map, void *stream)
+{
+    int rc = validate_kf(args, true);
+    if (rc) return rc;
+    if ((rc = validate_packed(record, host_map))) return rc;
     if ((rc = require_device())) return rc;
     if (args->n_filters == 0) return BKE_OK;
     g_err[0] = '\0';
@@ -228,6 +233,58 @@ int bke_kf_step_packed(const bke_kf_args *args, const void *record, const bke_kf
         set_error("the packed models cover per-filter models of dim_x = 4, dim_z = 2, BKE_F32 banks without "
                   "control input, on 16-byte aligned arrays");
     return rc;
+}
+
+int bke_kf_steps_packed(const bke_kf_args *args, const void *record, const bke_kf_model_map *host_map,
+                        const void *const *zs, int32_t n_steps, void *stream)
+{
+    int rc = validate_kf(args, false);
+    if (rc) return rc;
+    if ((rc = validate_packed(record, host_map))) return rc;
+    if (!zs) { set_error("zs is NULL"); return BKE_ERR_BAD_ARG; }
+    // what only the fused ring refuses (launch_kf_fast refuses the rest), before anything is launched
+    const bke_kf_args &a = *args;
+    auto refuse = [](const char *why) { set_error("bke_kf_steps_packed: %s", why); return BKE_ERR_UNSUPPORTED; };
+    if (n_steps < 1 || n_steps > BKE_KF42_MAX_RING) return refuse("n_steps must be 1 .. BKE_KF42_MAX_RING");
+    if ((a.flags & ~BKE_REVERSE_TILES) != (BKE_DO_PREDICT | BKE_DO_UPDATE)) return refuse("flags must be BKE_DO_PREDICT | BKE_DO_UPDATE");
+    if (a.z_valid) return refuse("z_valid is not taken");
+    if (a.B || a.u) return refuse("a control input is not taken");
+    if (a.x_prior || a.P_prior || a.K || a.y || a.S || a.SI || a.log_likelihood || a.status)
+        return refuse("status and the optional outputs are not written");
+    if (a.x_out != a.x || a.P_out != a.P) return refuse("the state is stepped in place (x_out = x, P_out = P)");
+    const char *x0 = (const char *)a.x, *P0 = (const char *)a.P;
+    for (int k = 0; k < n_steps; k++) {
+        const char *z = (const char *)zs[k];
+        if (!z) { set_error("zs[%d] is NULL", k); return BKE_ERR_BAD_ARG; }
+        if (reinterpret_cast<uintptr_t>(z) & 15u) return refuse("every z must be 16-byte aligned");
+        if ((z < x0 + a.n_filters * 16 && x0 < z + a.n_filters * 8) || (z < P0 + a.n_filters * 64 && P0 < z + a.n_filters * 8))
+            return refuse("a z overlaps x or P");
+    }
+    if ((rc = require_device())) return rc;
+    if (a.n_filters == 0) return BKE_OK;
+    bke_kf_args st = a;
+    st.z = zs[0];
+    g_err[0] = '\0';
+    rc = launch_kf_fast(st, (cudaStream_t)stream, record, host_map, zs, n_steps);
+    if (rc == BKE_ERR_UNSUPPORTED && g_err[0] == '\0')     // (launch_kf_fast names some causes itself)
+        set_error("the fused ring covers per-filter models of dim_x = 4, dim_z = 2, BKE_F32 banks on 16-byte aligned arrays");
+    return rc;
+}
+
+int bke_capture_node_count(void *stream, int64_t *n_nodes)
+{
+    if (!n_nodes) { set_error("n_nodes is NULL"); return BKE_ERR_BAD_ARG; }
+    int rc = require_device();
+    if (rc) return rc;
+    cudaStreamCaptureStatus status = cudaStreamCaptureStatusNone;
+    cudaGraph_t graph = nullptr;
+    if (check_cuda(cudaStreamGetCaptureInfo((cudaStream_t)stream, &status, nullptr, &graph, nullptr, nullptr),
+                   "cudaStreamGetCaptureInfo")) return BKE_ERR_CUDA;
+    if (status != cudaStreamCaptureStatusActive || !graph) { set_error("the stream is not capturing"); return BKE_ERR_BAD_ARG; }
+    size_t n = 0;
+    if (check_cuda(cudaGraphGetNodes(graph, nullptr, &n), "cudaGraphGetNodes")) return BKE_ERR_CUDA;
+    *n_nodes = (int64_t)n;
+    return BKE_OK;
 }
 
 int bke_kf_batch_filter(const bke_kf_batch_args *args, void *stream)

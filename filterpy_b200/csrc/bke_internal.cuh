@@ -31,8 +31,11 @@ constexpr double LOG_2PI = 1.8378770664093454835606594728112;
 int launch_kf_generic(const bke_kf_args &a, cudaStream_t s);
 // returns BKE_ERR_UNSUPPORTED when the specialised kernel does not cover the call.  Optional: `rec` alone is a
 // record filled by launch_kf_pack_sym that replaces the per-filter Q and R; `rec` with the HOST copy of a map
-// filled by launch_kf_scan_models is a record filled by launch_kf_pack_models that replaces F, Q, H and R
-int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec = nullptr, const bke_kf_model_map *map = nullptr);
+// filled by launch_kf_scan_models is a record filled by launch_kf_pack_models that replaces F, Q, H and R;
+// with `zs` on top, the launch runs n_steps (1 .. BKE_KF42_MAX_RING) predict+update pairs on the measurements
+// zs[k] in turn (a.z is not read)
+int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec = nullptr, const bke_kf_model_map *map = nullptr,
+                   const void *const *zs = nullptr, int n_steps = 0);
 size_t kf_sym_models_bytes(int64_t n_filters);
 int launch_kf_pack_sym(int64_t n_filters, const void *Q, const void *R, void *record, int32_t *asym, cudaStream_t s);
 size_t kf_packed_models_bytes(int64_t n_filters, uint64_t varying);

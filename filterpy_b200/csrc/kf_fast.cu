@@ -69,7 +69,8 @@ constexpr uint64_t PREDICT_WORDS = (1ull << W_H) - 1;      // F and Q
 constexpr int REC_RUNS = (WORDS + 1) / 2;                  // runs of consecutive planes, at most every other one
 
 // REC: 0 = dense models, 1 = the packed Q / R record, 2 = the packed model words (stage sized for all 37)
-template <typename T, int N, int M, bool SHARED = false, int REC = 0>
+// ZS: measurement blocks per stage (the fused ring stages one per step)
+template <typename T, int N, int M, bool SHARED = false, int REC = 0, int ZS = 1>
 struct Stage {
     // byte sizes of one tile of each array
     static constexpr int XB = TILE * N * sizeof(T);
@@ -88,7 +89,7 @@ struct Stage {
     static constexpr int OX = OH + (SHARED || REC == 2 ? 0 : align_up(HB));
     static constexpr int OR_ = OX + align_up(XB);
     static constexpr int OZ = OR_ + (SHARED || REC ? 0 : align_up(RB));
-    static constexpr int BYTES = OZ + align_up(ZB);
+    static constexpr int BYTES = OZ + ZS * align_up(ZB);
 };
 
 // read the 16-byte chunk c of row `row` (ROWB bytes per row) from a linear tile
@@ -152,6 +153,8 @@ struct FastP {
     int rec_copy;                   // how many of them this launch copies,
     int rec_runs;                   // in this many runs of consecutive planes:
     int run_first[REC_RUNS], run_len[REC_RUNS];
+    const float *zs[BKE_KF42_MAX_RING];     // RING: the measurements of step k (p.z is not read),
+    int n_steps;                            // for k < n_steps
 };
 
 // MODE: 3 = predict+update, 1 = predict only, 2 = update only
@@ -162,16 +165,22 @@ struct FastP {
 // Each CTA keeps STAGES tiles in flight.  Resident CTAs per SM: 3 with per-filter models (33 KB per
 // stage, 29.5 KB with either record), 4 with one shared model (11 KB per stage), 5 when that model
 // rides in the launch parameters.
+// RING (MODE 3, REC 2, no EXTRAS): 0 = one step; BKE_KF42_MAX_RING = the fused ring: each thread loads x, P and
+// the model words once, runs p.n_steps predict+update pairs on the measurements p.zs[0 .. n_steps) back to
+// back in registers and stores x, P once.  A stage then holds one 1 KB measurement block per step
+// (36.5 KB per stage: 2 stages x 3 CTAs = 219 KB of the SM's 227 KB).
 constexpr int STAGES = 2;
 constexpr int kf42_ctas_per_sm(int shared) { return shared == 2 ? 5 : (shared ? 4 : 3); }
 
-template <int MODE, int SHARED, bool EXTRAS, int REC = 0>
+template <int MODE, int SHARED, bool EXTRAS, int REC = 0, int RING = 0>
 __global__ void __launch_bounds__(TILE, kf42_ctas_per_sm(SHARED))
 kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 {
     constexpr int N = 4, M = 2;
     static_assert(!(REC && SHARED), "the packed records hold per-filter models");
-    using St = Stage<float, N, M, SHARED != 0, REC>;
+    static_assert(!RING || (MODE == 3 && REC == 2 && !EXTRAS), "the fused ring steps the packed model words");
+    constexpr int ZS = RING ? RING : 1;
+    using St = Stage<float, N, M, SHARED != 0, REC, ZS>;
     // REC == 1: the part of a tile's record this MODE reads (the Q planes, the R planes or both)
     constexpr int SYM_FIRST = (MODE & 1) ? 0 : SYM_Q_PLANES;
     constexpr int SYM_LAST = (MODE & 2) ? SYM_PLANES : SYM_Q_PLANES;
@@ -199,7 +208,7 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
         // the records are padded to whole tiles: always the full planes
         if (REC == 1) tx += SYM_BYTES;
         if (REC == 2) tx += (uint32_t)p.rec_copy * TILE * 4;
-        if (DO_U) tx += zb;
+        if (DO_U) tx += RING ? p.n_steps * zb : zb;
         mbar_expect_tx(bar, tx);
         auto load = [&](int off, const float *src, int per_filter, uint32_t bytes, uint64_t pol) {
             if (p.l2_hints) bulk_load_hint(sb + off, src + f0 * per_filter, bytes, bar, pol);
@@ -220,7 +229,9 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
             for (int r = 0; r < p.rec_runs; r++)
                 load(St::OQ + p.run_first[r] * TILE * 4, p.rec + p.run_first[r] * TILE, p.rec_planes,
                      p.run_len[r] * TILE * 4, pol_first);
-        if (DO_U && zb) load(St::OZ, p.z, M, zb, pol_first);
+        if (!RING && DO_U && zb) load(St::OZ, p.z, M, zb, pol_first);
+        if (RING && zb)
+            for (int k = 0; k < p.n_steps; k++) load(St::OZ + k * St::align_up(St::ZB), p.zs[k], M, zb, pol_first);
     };
 
     // prologue: nothing here touches global memory, so it may overlap the previous launch
@@ -281,7 +292,7 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
         const unsigned char *sb = smem + stage * St::BYTES;
         mbar_wait(&full[stage], parity);
 
-        float x[N], P[N][N], z[M];
+        float x[N], P[N][N], z[ZS][M];
         {
             float4 v = lds_chunk<16>(sb + St::OX, tid, 0);
             x[0] = v.x; x[1] = v.y; x[2] = v.z; x[3] = v.w;
@@ -338,9 +349,22 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
         if (DO_U) {
             // the stage holds z up to the last whole 16 bytes: only an odd last filter misses its own
             const bool own = live && (p.N_filters & 1) && f == p.N_filters - 1;
-            float2 v = own ? *reinterpret_cast<const float2 *>(p.z + f * M)
-                           : *reinterpret_cast<const float2 *>(sb + St::OZ + tid * 8);
-            z[0] = v.x; z[1] = v.y;
+            if (!RING) {
+                float2 v = own ? *reinterpret_cast<const float2 *>(p.z + f * M)
+                               : *reinterpret_cast<const float2 *>(sb + St::OZ + tid * 8);
+                z[0][0] = v.x; z[0][1] = v.y;
+            }
+            // the ring: every step's measurement into registers now, so that nothing reads the stage after
+            // the barrier below (unrolled to the longest ring under a uniform guard: no run-time index
+            // into z[][])
+#pragma unroll
+            for (int k = 0; k < RING; k++) {
+                float2 v = make_float2(0.f, 0.f);
+                if (k < p.n_steps)
+                    v = own ? *reinterpret_cast<const float2 *>(p.zs[k] + f * M)
+                            : *reinterpret_cast<const float2 *>(sb + St::OZ + k * St::align_up(St::ZB) + tid * 8);
+                z[k][0] = v.x; z[k][1] = v.y;
+            }
         }
         // The stage is about to be handed back to the TMA engine (async proxy).  A plain barrier
         // does not order the generic-proxy LDS above against that: the loads may still sit in the
@@ -378,7 +402,10 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
                     if (!REC || b >= a) acc ^= __float_as_uint(R[a][b]);
             }
         }
-        if (DO_U) acc ^= __float_as_uint(z[0]) ^ __float_as_uint(z[1]);
+        if (DO_U) {
+#pragma unroll
+            for (int k = 0; k < ZS; k++) acc ^= __float_as_uint(z[k][0]) ^ __float_as_uint(z[k][1]);
+        }
         const int never = __syncthreads_and(acc == 0x7fc0beefu);     // every thread has drained the stage
         if (never && p.num_tiles < 0) p.x_out[0] = 0.f;              // keeps `acc` alive; cannot happen
         const int nt = tile + STAGES * gridDim.x;
@@ -391,7 +418,19 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
         }
 
         int st = BKE_STATUS_OK;
-        if (DO_P) {
+        if (RING) {
+            // the steps of the ring, back to back on the registers; the loop stays rolled and the
+            // measurements rotate through z[0] instead of being indexed
+#pragma unroll 1
+            for (int k = 0; k < p.n_steps; k++) {
+                reg_predict<float, N>(x, P, F, Q, p.alpha_sq);
+                KfUpdateOut<float, N, M> o;
+                reg_update<float, N, M>(x, P, H, R, z[0], o);
+#pragma unroll
+                for (int j = 0; j + 1 < ZS; j++) { z[j][0] = z[j + 1][0]; z[j][1] = z[j + 1][1]; }
+            }
+        }
+        if (!RING && DO_P) {
             reg_predict<float, N>(x, P, F, Q, p.alpha_sq);
             if (EXTRAS && live) {
                 if (p.x_prior) *reinterpret_cast<float4 *>(p.x_prior + f * N) = make_float4(x[0], x[1], x[2], x[3]);
@@ -402,12 +441,12 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
                 }
             }
         }
-        if (DO_U) {
+        if (!RING && DO_U) {
             bool has_z = true;
             if (p.valid != nullptr && live) has_z = p.valid[f] != 0;
             KfUpdateOut<float, N, M> o;
             if (has_z) {
-                reg_update<float, N, M>(x, P, H, R, z, o);
+                reg_update<float, N, M>(x, P, H, R, z[0], o);
                 if (!o.ok) st = BKE_STATUS_SINGULAR_S;
             }
             if (EXTRAS && live) {
@@ -457,18 +496,19 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 // ---------------------------------------------------------------------------- host side
 // switches (environment, read once): BKE_KF_L2 = 0 disables the L2 eviction-priority hints,
 // BKE_KF_SYM = 0 both packed records, BKE_KF_HOST_MODELS = 0 the shared models in the launch parameters,
-// BKE_KF_ORDER = 0 the reversed tile order (every launch walks the bank first to last)
+// BKE_KF_ORDER = 0 the reversed tile order (every launch walks the bank first to last),
+// BKE_KF_RING = 0 the fused ring (bke_kf_steps_packed reports BKE_ERR_UNSUPPORTED)
 int env_int(const char *name, int dflt)
 {
     const char *v = getenv(name);
     return v ? atoi(v) : dflt;
 }
 
-template <int MODE, int SHARED, bool EXTRAS, int REC = 0>
+template <int MODE, int SHARED, bool EXTRAS, int REC = 0, int RING = 0>
 int launch_variant(const FastP<4, 2> &p, cudaStream_t s)
 {
-    using St = Stage<float, 4, 2, SHARED != 0, REC>;
-    auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, REC>;
+    using St = Stage<float, 4, 2, SHARED != 0, REC, RING ? RING : 1>;
+    auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, REC, RING>;
     const int smem = STAGES * St::BYTES;
     static bool configured[64] = {false};
     int dev = 0;
@@ -801,9 +841,11 @@ int launch_kf_pack_models(int64_t n_filters, const void *F, const void *Q, const
     return check_cuda(cudaGetLastError(), "kf42_pack_models_kernel launch");
 }
 
-int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const bke_kf_model_map *map)
+int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const bke_kf_model_map *map,
+                   const void *const *zs, int n_steps)
 {
     const bool packed = map != nullptr, sym = rec != nullptr && !packed;
+    const bool ring = zs != nullptr;        // bke_kf_steps_packed, which has checked what only the ring refuses
     if ((sym || packed) && !sym_enabled()) {
         set_error(sym ? "the packed symmetric models are disabled (BKE_KF_SYM=0)" : "the packed models are disabled (BKE_KF_SYM=0)");
         return BKE_ERR_UNSUPPORTED;
@@ -888,6 +930,14 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const 
         }
     }
     const bool extras = a.x_prior || a.P_prior || a.K || a.y || a.S || a.SI || a.log_likelihood || a.status;
+    if (ring) {
+        static const int ring_env = env_int("BKE_KF_RING", 1);
+        if (!ring_env) { set_error("the fused ring is disabled (BKE_KF_RING=0)"); return BKE_ERR_UNSUPPORTED; }
+        if (!packed || !all_dense || !(dp && du) || extras || a.z_valid) return BKE_ERR_UNSUPPORTED;
+        for (int k = 0; k < n_steps; k++) p.zs[k] = (const float *)zs[k];
+        p.n_steps = n_steps;
+        return launch_variant<3, 0, false, 2, BKE_KF42_MAX_RING>(p, s);
+    }
 
 #define BKE_DISPATCH(MODE)                                                                   \
     do {                                                                                     \

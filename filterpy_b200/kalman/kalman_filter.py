@@ -76,6 +76,7 @@ class KalmanFilter(_BankMirror):
         self._sym_state = None        # (token, usable) of _sym_buf's pack
         self._model_version = 0
         self._model_last = None       # the token of the previous launch
+        self._ring_notes = None       # capture(): what each launch of the capture pass was (see _fuse_ring)
 
     # ------------------------------------------------------------------ hooks of _BankMirror
     def _state_rebound(self):
@@ -296,6 +297,8 @@ class KalmanFilter(_BankMirror):
         plain = R is None and H is None and (pend is None or (pend.get("u") is None and pend.get("B") is None
                                                                and pend.get("F") is None and pend.get("Q") is None))
         rec = self._sym_record() if plain else None
+        if self._ring_notes is not None and self._capturing():
+            self._ring_notes.append((flags & ~_lib.BKE_REVERSE_TILES, plain and vt is None, rec, zt))
         if plain:
             hit = self._args_cache.get(flags)
             if hit is not None and hit[0] == self._version:
@@ -384,9 +387,65 @@ class KalmanFilter(_BankMirror):
         scheduling hint: the results are the same either way), and each captured launch keeps the
         order it was captured with.  A graph with an even number of launches therefore alternates
         across replays too; with an odd number, the first launch of a replay runs in the same order as
-        the last launch of the previous one, which costs that step the L2 reuse but nothing else."""
+        the last launch of the previous one, which costs that step the L2 reuse but nothing else.
+
+        A ring of K plain ``predict(); update(z_i)`` pairs of such a bank (``diagnostics=False``, no
+        ``valid``, no per-call model, and nothing else in ``fn``: no torch op, no other bank) is returned
+        as a graph of ``ceil(K / 8)`` launches of ``bke_kf_steps_packed`` instead: each runs up to 8 of
+        the steps back to back with x and P in registers, so the state crosses HBM once per launch and
+        not once per step.  Inside a fused ring x and P exist in HBM only between replays; the results
+        are bit for bit those of the separate steps.  The returned graph's ``launches`` and
+        ``fused_steps`` say which of the two it is; ``BKE_KF_RING=0`` keeps the graph of separate steps."""
         self._flush()
-        return StepGraph(fn, self._device, warmup)
+        self._ring_notes = []
+        try:
+            graph = StepGraph(fn, self._device, warmup)
+        finally:
+            notes, self._ring_notes = self._ring_notes, None
+        graph.launches = len(notes)
+        return self._fuse_ring(notes, graph) or graph
+
+    def _fuse_ring(self, notes, graph):
+        """The fused form of a captured ring, or None when the capture is anything but plain fused
+        predict+update steps of this bank on one packed record: decided on the finished capture, from
+        what ``_launch`` noted of each launch, and from the graph's node count, which tells whether
+        ``fn`` recorded anything besides those launches."""
+        step = _lib.BKE_DO_PREDICT | _lib.BKE_DO_UPDATE
+        rec = notes[0][2] if notes else None
+        if (rec is None or self.diagnostics or graph.nodes != len(notes) or rec is not self._sym_buf
+                or any(n[0] != step or not n[1] or n[2] is not rec for n in notes)):
+            return None
+        # (the argument structs are cached under the flags of their launch, tile order included)
+        hit = self._args_cache.get(step) or self._args_cache[step | _lib.BKE_REVERSE_TILES]
+        a = _lib.KfArgs.from_buffer_copy(hit[1])
+        a.z_valid = None
+        zs = [n[3] for n in notes]
+        M = _lib.BKE_KF42_MAX_RING
+        rings = [(ctypes.c_void_p * len(c))(*[ptr(z) for z in c]) for c in (zs[i:i + M] for i in range(0, len(zs), M))]
+        # consecutive launches of a replay alternate the tile order, like consecutive steps
+        order = {id(r): (_lib.BKE_REVERSE_TILES if j % 2 else 0) for j, r in enumerate(rings)}
+        hmap, recp = self._sym_host_map, ptr(rec) if rec.numel() else None
+
+        def call(ring):
+            a.flags = step | order[id(ring)]
+            return self._lib.bke_kf_steps_packed(a, recp, hmap, ring, len(ring), stream_ptr(self._device))
+
+        def fused():
+            for ring in rings:
+                self._run(call, ring)
+        # once outside capture: the kernel's one-time function attribute must not be set under capture,
+        # and a refusal (BKE_KF_RING=0, a z the ring does not take) leaves the graph of separate steps
+        with torch.cuda.device(self._device):
+            rc = call(rings[0])
+        if rc == _lib.BKE_ERR_UNSUPPORTED:
+            return None
+        _lib.check(rc)
+        for ring in rings[1:]:
+            self._run(call, ring)
+        ring_graph = StepGraph(fused, self._device, warmup=0)
+        ring_graph.launches, ring_graph.fused_steps = len(rings), len(zs)
+        ring_graph._keep = (a, rec, hmap, rings, zs)        # what the captured launches point into
+        return ring_graph
 
     # ------------------------------------------------------------------ batch_filter
     def batch_filter(self, zs, Fs=None, Qs=None, Hs=None, Rs=None, Bs=None, us=None,

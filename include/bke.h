@@ -181,10 +181,24 @@ int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream);
  *                               representative plane c(s) instead (40 -> 20 B of models per filter for the
  *                               constant-velocity bank above, which has the same dt, q and r on both
  *                               axes).  A `duplicate` bit at or above popcount(varying), or whose slot has
- *                               no c(s), is refused with BKE_ERR_BAD_ARG.
+ *                               no c(s), is refused with BKE_ERR_BAD_ARG;
+ *   bke_kf_steps_packed         n_steps consecutive predict+update steps in ONE launch: the same x_out and
+ *                               P_out, bit for bit, as n_steps calls of bke_kf_step_packed with args->z =
+ *                               zs[k] in turn (args->z itself is ignored).  Every thread keeps its filter's x
+ *                               and P in registers between the steps, so the state is read and written once
+ *                               per call instead of once per step (212 B per filter and call with 4 steps
+ *                               of the constant-velocity bank above, against 4 x 188); between the steps
+ *                               x and P exist nowhere in memory.  zs is a HOST array of n_steps device
+ *                               pointers, each [N,2], 16-byte aligned and clear of x and P; the same pointer
+ *                               may appear more than once.  It takes flags = BKE_DO_PREDICT | BKE_DO_UPDATE
+ *                               (BKE_REVERSE_TILES is honoured as in a single step), an in-place state
+ *                               (x_out = x, P_out = P), 1 <= n_steps <= BKE_KF42_MAX_RING, and neither
+ *                               z_valid, B / u, status nor any optional output: anything else returns
+ *                               BKE_ERR_UNSUPPORTED, and so does BKE_KF_RING=0 in the environment.
  * The calls return BKE_ERR_UNSUPPORTED for other shapes, dtypes, shared models, an asymmetric map,
  * misaligned pointers, and when the environment sets BKE_KF_SYM=0; bke_kf_step is then the call to make. */
 #define BKE_KF42_MODEL_WORDS 37
+#define BKE_KF42_MAX_RING 8
 typedef struct bke_kf_model_map {
     uint64_t varying;                       /* bit e: word e differs between filters */
     int32_t asymmetric;                     /* 1: some Q or R is not exactly symmetric */
@@ -198,6 +212,13 @@ size_t bke_kf_packed_models_bytes(int64_t n_filters, uint64_t varying);
 int bke_kf_pack_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *F, const void *Q,
                        const void *H, const void *R, uint64_t varying, void *record, void *stream);
 int bke_kf_step_packed(const bke_kf_args *args, const void *record, const bke_kf_model_map *host_map, void *stream);
+int bke_kf_steps_packed(const bke_kf_args *args, const void *record, const bke_kf_model_map *host_map,
+                        const void *const *zs, int32_t n_steps, void *stream);
+
+/* The number of nodes of the graph `stream` is capturing into (*n_nodes; HOST).  A caller that captures its own
+ * launches can tell from it whether anything else went into the graph.  BKE_ERR_BAD_ARG when the stream is not
+ * capturing. */
+int bke_capture_node_count(void *stream, int64_t *n_nodes);
 
 /* KalmanFilter.batch_filter over T epochs for a bank (kalman_filter.py:826-993; procedural
  * twin :1664-1788): the time loop runs inside one kernel with the models resident on chip.

@@ -7,7 +7,9 @@
 // mode 2, F, Q, H and R are replaced by one stream of 40 B per filter (the 10 model words that differ
 // between the filters of the bench bank, bke_kf_pack_models): 128 B read, 208 B in all.  With mode 3,
 // that stream is 20 B per filter (the 5 distinct planes among those 10 words, the planes the step reads
-// when the scan has flagged the copies): 108 B read, 188 B in all.
+// when the scan has flagged the copies): 108 B read, 188 B in all.  The twin of the fused ring
+// (bke_kf_steps_packed, kf42_ring_traffic below) is mode 3 with n_z measurement streams instead of one: the
+// state and the 20 B of models once, 8 B of z per fused step, 180 + 8 n_z B per filter and launch.
 // Every array is read and written with flat, fully coalesced 16-byte accesses.  A CTA of
 // 256 threads covers 64 filters: every thread moves one 16-byte chunk of P, F, Q, the first 128
 // threads one of H, the first 64 one of x and R, the first 32 one of z, so the read/write mix is the
@@ -52,7 +54,7 @@ struct Order {
 template <bool HINTS>
 __global__ void __launch_bounds__(THREADS)
 kf42_traffic_kernel(float4 *x, float4 *P, const float4 *F, const float4 *Q, const float4 *H, const float4 *R,
-                    const float4 *z, int64_t n_chunks, int mode, Order o)
+                    const float4 *z, int64_t n_chunks, int mode, Order o, int n_z)
 {
     const int t = threadIdx.x;
     uint64_t pol_first = 0, pol_last = 0, pol_normal = 0;
@@ -84,7 +86,13 @@ kf42_traffic_kernel(float4 *x, float4 *P, const float4 *F, const float4 *Q, cons
             if (t < THREADS / 2) vh = ld(H + c * (THREADS / 2) + t, pol);
         }
         if (t < THREADS / 4) vx = HINTS ? ld_hint(x + c * (THREADS / 4) + t, pol) : x[c * (THREADS / 4) + t];
-        if (t < THREADS / 8) vz = ld(z + c * (THREADS / 8) + t, pol_z);
+        if (t < THREADS / 8) {
+            // (stream j of the ring's twin is the j-th [N,2] array behind z)
+            for (int j = 0; j < n_z; j++) {
+                const float4 v = ld(z + (j * n_chunks + c) * (THREADS / 8) + t, pol_z);
+                vz.x = __uint_as_float(__float_as_uint(vz.x) | __float_as_uint(v.x) | __float_as_uint(v.w));
+            }
+        }
         // the stores depend on every load (bit-wise, no floating-point work), so none is dropped
         const uint32_t kk = __float_as_uint(vf.x) | __float_as_uint(vq.y) | __float_as_uint(vh.z) |
                             __float_as_uint(vr.w) | __float_as_uint(vz.x);
@@ -116,11 +124,21 @@ int kf42_traffic(void *x, void *P, const void *F, const void *Q, const void *H, 
     if (hints)
         kf42_traffic_kernel<true><<<grid, THREADS, 0, (cudaStream_t)stream>>>(
             (float4 *)x, (float4 *)P, (const float4 *)F, (const float4 *)Q, (const float4 *)H, (const float4 *)R,
-            (const float4 *)z, n_filters / CHUNK, mode, o);
+            (const float4 *)z, n_filters / CHUNK, mode, o, 1);
     else
         kf42_traffic_kernel<false><<<grid, THREADS, 0, (cudaStream_t)stream>>>(
             (float4 *)x, (float4 *)P, (const float4 *)F, (const float4 *)Q, (const float4 *)H, (const float4 *)R,
-            (const float4 *)z, n_filters / CHUNK, mode, o);
+            (const float4 *)z, n_filters / CHUNK, mode, o, 1);
+    return (int)cudaGetLastError();
+}
+
+// The twin of one fused ring of n_z steps: x, P read and written in place, Q the 20 B-per-filter stream,
+// z the n_z consecutive [n_filters, 2] measurement arrays.
+int kf42_ring_traffic(void *x, void *P, const void *Q, const void *z, int64_t n_filters, int grid, int n_z, void *stream)
+{
+    kf42_traffic_kernel<false><<<grid, THREADS, 0, (cudaStream_t)stream>>>(
+        (float4 *)x, (float4 *)P, nullptr, (const float4 *)Q, nullptr, nullptr, (const float4 *)z, n_filters / CHUNK, 3,
+        Order{0, 0, 0, 0}, n_z);
     return (int)cudaGetLastError();
 }
 

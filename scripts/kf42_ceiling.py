@@ -1,7 +1,7 @@
 """Where the time of the 4/2 fp32 bank step goes: the card's ceiling for its traffic, and the step's
 fixed cost and streaming rate.
 
-    python scripts/kf42_ceiling.py [--out DIR] [--rounds R]
+    python scripts/kf42_ceiling.py [--out DIR] [--rounds R] [--ring]
 
 Prints JSON lines (and writes them to DIR/kf42_ceiling.jsonl with --out):
 
@@ -24,7 +24,7 @@ Prints JSON lines (and writes them to DIR/kf42_ceiling.jsonl with --out):
              and demoted (evict_first) by the next launch.  ms per launch (best grid of 4 or 8 CTAs per
              SM, median of rounds, the arms alternated inside every round) and the gain over `forward`
   step       the shipped step (KalmanFilter.predict + update, per-filter F/H/Q/R) replayed as CUDA
-             graphs of 4 steps like bench.py, at N = 2^19 .. 2^22 (all above the bound under which
+             graphs of 4 separate steps, at N = 2^19 .. 2^22 (all above the bound under which
              the L2 hints are used); per-step time and GB/s for every N, counted with the bytes the
              step moves (168 + 4 per distinct plane of the packed model words, i.e. per varying word
              not flagged in the map's `duplicate`: 188 for the bench bank; 344 with BKE_KF_SYM=0)
@@ -32,6 +32,12 @@ Prints JSON lines (and writes them to DIR/kf42_ceiling.jsonl with --out):
              streaming rate
   shared     the same graph of 4 steps for a 2^20-filter bank whose F/H/Q/R are shared (one model
              for the bank, carried in the launch parameters)
+  ring       the fused ring (bke_kf_steps_packed, what KalmanFilter.capture returns for a ring of plain
+             steps) at N = 2^19 .. 2^22 and K = 2, 4, 8 steps per launch, the arms alternated inside every
+             round: `twin`, the memory-only kernel moving the ring's 180 + 8 K B per filter; `steps`, the
+             graph of K separate steps; `fused`, a graph of one fused launch; `fused_alt`, two such graphs
+             in forward and reversed tile order replayed in turn.  ms per step (median of rounds) and, for
+             twin and fused, GB/s of the ring's bytes.  --ring prints only the card and these lines.
 
 The ceiling kernel is compiled with nvcc into scripts/kf42_ceiling.so (git-ignored) when that file
 is missing or older than its source.  BKE_LIB_PATH selects the engine library as everywhere else.
@@ -72,6 +78,8 @@ def build_lib():
 
 def traffic_lib():
     lib = ctypes.CDLL(build_lib())
+    lib.kf42_ring_traffic.restype = ctypes.c_int
+    lib.kf42_ring_traffic.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     lib.kf42_traffic.restype = ctypes.c_int
     lib.kf42_traffic.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                          ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int64,
@@ -211,7 +219,75 @@ def bank(torch, N, shared=False):
         for i in range(RING):
             kf.predict()
             kf.update(zs[i])
-    return kf, kf.capture(ring)
+    # the graph of separate steps: kf.capture would return this ring fused (the `ring` lines measure that)
+    from filterpy_b200._dev import StepGraph
+    return kf, StepGraph(ring, kf._device)
+
+
+def ring(torch, rounds):
+    """The fused ring against its memory-only twin and against the graph of separate steps."""
+    from filterpy_b200 import _lib
+    from filterpy_b200._dev import StepGraph
+    lib, tlib = _lib.load(), traffic_lib()
+    dev = torch.device("cuda")
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    lines = []
+    for lg in (19, 20, 21, 22):
+        N = 1 << lg
+        kf, _ = bank(torch, N)
+        assert kf._sym_buf is not None, "the bank does not step from the packed model words"
+        zs = torch.randn(8, N, 2, device=dev)
+        tw = {k: torch.randn(N * e, device=dev) for k, e in (("x", 4), ("P", 16), ("Q", 5))}
+        a = _lib.KfArgs.from_buffer_copy(next(iter(kf._args_cache.values()))[1])
+        a.z_valid = None
+        for K in (2, 4, 8):
+            arr = (ctypes.c_void_p * K)(*[zs[k].data_ptr() for k in range(K)])
+
+            def fused(flags):
+                a.flags = flags
+                _lib.check(lib.bke_kf_steps_packed(a, kf._sym_buf.data_ptr(), kf._sym_host_map, arr, K,
+                                                   torch.cuda.current_stream().cuda_stream))
+
+            def steps():
+                for k in range(K):
+                    kf.predict(); kf.update(zs[k])
+            fused(3)                                    # the one-time function attribute, outside capture
+            g_fwd = StepGraph(lambda: fused(3), dev, warmup=1)
+            g_rev = StepGraph(lambda: fused(3 | _lib.BKE_REVERSE_TILES), dev, warmup=1)
+            g_steps = StepGraph(steps, dev)
+            assert g_fwd.nodes == 1 and g_steps.nodes == K
+            flip = {"i": 0}
+
+            def alt():
+                flip["i"] ^= 1
+                (g_rev if flip["i"] else g_fwd).replay()
+
+            def twin(grid):
+                rc = tlib.kf42_ring_traffic(tw["x"].data_ptr(), tw["P"].data_ptr(), tw["Q"].data_ptr(), zs.data_ptr(), N,
+                                            grid, K, torch.cuda.current_stream().cuda_stream)
+                assert rc == 0, rc
+            arms = [("twin_4", lambda: twin(4 * sms)), ("twin_8", lambda: twin(8 * sms)), ("steps", g_steps.replay),
+                    ("fused", g_fwd.replay), ("fused_alt", alt)]
+            reps = max(4, reps_for(N) // K) // 2 * 2
+            ms = {}
+            for r in range(rounds):
+                for name, fn in (arms if r % 2 == 0 else arms[::-1]):
+                    for _ in range(4):
+                        fn()
+                    ms.setdefault(name, []).append(time_ms(fn, reps, torch) / K)
+            med = {k: float(np.median(v)) for k, v in ms.items()}
+            moved = 180 + 8 * K
+            twin_ms = min(med["twin_4"], med["twin_8"])
+            gbs = lambda t: moved * N / (t * K * 1e-3) / 1e9
+            lines.append({"what": "ring", "n_filters": N, "steps_per_launch": K, "bytes_per_filter_launch": moved,
+                          "ms_per_step": {"twin": twin_ms, "steps": med["steps"], "fused": med["fused"],
+                                          "fused_alt": med["fused_alt"]},
+                          "GBps": {"twin": gbs(twin_ms), "fused": gbs(med["fused"])},
+                          "fused_over_twin": med["fused"] / twin_ms, "steps_over_fused": med["steps"] / med["fused"],
+                          "alt_gain": med["fused"] / med["fused_alt"] - 1.0})
+        del kf, zs, tw
+        torch.cuda.empty_cache()
+    return lines
 
 
 def step_ms(torch, graph, N, rounds):
@@ -226,10 +302,13 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None, help="also write the JSON lines to OUT/kf42_ceiling.jsonl")
     ap.add_argument("--rounds", type=int, default=5, help="timed rounds per measurement (the median is reported)")
+    ap.add_argument("--ring", action="store_true", help="only the fused-ring lines")
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "kf42_ceiling.py measures on a GPU"
     lines = [dict(what="card", **card()), dict(what="library", path=os.environ.get("BKE_LIB_PATH") or "in-tree")]
+    if args.ring:
+        return emit(lines + ring(torch, args.rounds), args.out)
     lines.append(ceiling(torch, args.rounds))
     lines.append(ceiling(torch, args.rounds, mode=1))
     lines.append(ceiling(torch, args.rounds, mode=2))
@@ -262,11 +341,15 @@ def main():
     kf, graph = bank(torch, N, shared=True)
     t = step_ms(torch, graph, N, args.rounds)
     lines.append({"what": "shared", "n_filters": N, "ms": float(np.median(t)), "ms_rounds": t})
+    emit(lines + ring(torch, args.rounds), args.out)
+
+
+def emit(lines, out):
     text = "\n".join(json.dumps(l) for l in lines)
     print(text, flush=True)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "kf42_ceiling.jsonl"), "a") as f:
+    if out:
+        os.makedirs(out, exist_ok=True)
+        with open(os.path.join(out, "kf42_ceiling.jsonl"), "a") as f:
             f.write(text + "\n")
 
 
