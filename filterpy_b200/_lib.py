@@ -41,6 +41,7 @@ EXPORTED_SYMBOLS = [
     "bke_enkf_initialize", "bke_enkf_step", "bke_enkf_model_compile", "bke_enkf_step_model", "bke_debug_enkf_model_cubin_bytes",
     "bke_srkf_step", "bke_cholesky_lower",
     "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
+    "bke_resample_bank", "bke_gather_rows_bank",
     "bke_residual_workspace_bytes", "bke_residual_prepare", "bke_searchsorted_bracket_sweep",
 ]
 
@@ -215,6 +216,14 @@ class ResampleShardExt(ctypes.Structure):
         ("carry_approx_buf", c_void_p), ("carry_exact_buf", c_void_p),
         ("compose_status", c_void_p),
         ("shard_rank", c_int32), ("n_shards", c_int32),
+    ]
+
+
+class ResampleBankArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_sets", c_int64), ("n_particles", c_int64),
+        ("weights", c_void_p), ("u", c_void_p), ("uniforms", c_void_p),
+        ("indexes", c_void_p), ("status", c_void_p),
     ]
 
 
@@ -442,6 +451,11 @@ def load():
     lib.bke_gather_rows.argtypes = [c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
                                     c_void_p]
     lib.bke_gather_rows.restype = ctypes.c_int
+    lib.bke_gather_rows_bank.argtypes = [c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                                         c_void_p]
+    lib.bke_gather_rows_bank.restype = ctypes.c_int
+    lib.bke_resample_bank.argtypes = [ctypes.POINTER(ResampleBankArgs), c_void_p]
+    lib.bke_resample_bank.restype = ctypes.c_int
     lib.bke_residual_workspace_bytes.argtypes = [c_int64]
     lib.bke_residual_workspace_bytes.restype = c_size_t
     lib.bke_residual_prepare.argtypes = [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,

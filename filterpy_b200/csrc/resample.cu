@@ -1737,21 +1737,25 @@ __global__ void __launch_bounds__(256) k_searchsorted_lut(i64 n, const double *_
 
 // dst[r, :] = src[idx[r], :] for rows of `cpr` chunks of type V (the particle gather that follows a
 // resample, docs/monte_carlo/resampling.rst:4-8).  Consecutive threads move consecutive chunks of a row.
+// set_len > 0: a bank of sets of set_len rows each, indexes count within the set of the output row.
 template <typename V, typename I>
 __global__ void __launch_bounds__(256) k_gather_rows(i64 n_out, i64 n_src, i64 cpr, const V *__restrict__ src,
-                                                     const I *__restrict__ idx, V *__restrict__ dst, int *err)
+                                                     const I *__restrict__ idx, V *__restrict__ dst, int *err, i64 set_len)
 {
     const i64 total = n_out * cpr;
+    const i64 lim = set_len ? set_len : n_src;
     for (i64 c = (i64)blockIdx.x * blockDim.x + threadIdx.x; c < total; c += (i64)gridDim.x * blockDim.x) {
         const i64 r = c / cpr, within = c - r * cpr;
-        const i64 j = (i64)idx[r];
-        if (j < 0 || j >= n_src) { if (err) *err = 1; continue; }
+        i64 j = (i64)idx[r];
+        if (j < 0 || j >= lim) { if (err) *err = 1; continue; }
+        if (set_len) j += r - r % set_len;
         dst[c] = src[j * cpr + within];
     }
 }
 
 template <typename V, typename I>
-int launch_gather(i64 n_out, i64 n_src, i64 row_bytes, const void *src, const void *idx, void *dst, int *err, cudaStream_t s)
+int launch_gather(i64 n_out, i64 n_src, i64 row_bytes, const void *src, const void *idx, void *dst, int *err, cudaStream_t s,
+                  i64 set_len = 0)
 {
     const i64 cpr = row_bytes / (i64)sizeof(V);
     const i64 total = n_out * cpr;
@@ -1759,7 +1763,7 @@ int launch_gather(i64 n_out, i64 n_src, i64 row_bytes, const void *src, const vo
     const i64 cap = (i64)sm_count() * 16;
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
-    k_gather_rows<V, I><<<(unsigned)blocks, 256, 0, s>>>(n_out, n_src, cpr, (const V *)src, (const I *)idx, (V *)dst, err);
+    k_gather_rows<V, I><<<(unsigned)blocks, 256, 0, s>>>(n_out, n_src, cpr, (const V *)src, (const I *)idx, (V *)dst, err, set_len);
     return check_cuda(cudaGetLastError(), "gather launch");
 }
 
@@ -2111,8 +2115,8 @@ int bke_multinomial_resample(int64_t n, const double *weights, const double *uni
     return check_cuda(cudaGetLastError(), "multinomial launch");
 }
 
-int bke_gather_rows(int64_t n_out, int64_t n_src, int64_t row_bytes, const void *src, const void *indexes,
-                    int32_t index_is_64, void *dst, int32_t *err, void *stream)
+static int gather_rows(int64_t n_out, int64_t n_src, int64_t row_bytes, const void *src, const void *indexes,
+                       int32_t index_is_64, void *dst, int32_t *err, int64_t set_len, void *stream)
 {
     if (n_out < 0 || n_src < 0 || row_bytes <= 0) { set_error("bad sizes"); return BKE_ERR_BAD_ARG; }
     if (n_out == 0) return BKE_OK;
@@ -2120,13 +2124,28 @@ int bke_gather_rows(int64_t n_out, int64_t n_src, int64_t row_bytes, const void 
     if (src == dst) { set_error("gather cannot run in place"); return BKE_ERR_BAD_ARG; }
     cudaStream_t s = (cudaStream_t)stream;
     const uintptr_t al = reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst) | (uintptr_t)row_bytes;
-#define BKE_GATHER(V) (index_is_64 ? rs::launch_gather<V, long long>(n_out, n_src, row_bytes, src, indexes, dst, err, s) \
-                                   : rs::launch_gather<V, int>(n_out, n_src, row_bytes, src, indexes, dst, err, s))
+#define BKE_GATHER(V) (index_is_64 ? rs::launch_gather<V, long long>(n_out, n_src, row_bytes, src, indexes, dst, err, s, set_len) \
+                                   : rs::launch_gather<V, int>(n_out, n_src, row_bytes, src, indexes, dst, err, s, set_len))
     if ((al & 15) == 0) return BKE_GATHER(uint4);
     if ((al & 7) == 0) return BKE_GATHER(uint2);
     if ((al & 3) == 0) return BKE_GATHER(unsigned);
     return BKE_GATHER(unsigned char);
 #undef BKE_GATHER
+}
+
+int bke_gather_rows(int64_t n_out, int64_t n_src, int64_t row_bytes, const void *src, const void *indexes,
+                    int32_t index_is_64, void *dst, int32_t *err, void *stream)
+{
+    return gather_rows(n_out, n_src, row_bytes, src, indexes, index_is_64, dst, err, 0, stream);
+}
+
+int bke_gather_rows_bank(int64_t n_sets, int64_t set_len, int64_t row_bytes, const void *src, const void *indexes,
+                         int32_t index_is_64, void *dst, int32_t *err, void *stream)
+{
+    if (n_sets < 0 || set_len < 0) { set_error("bad sizes"); return BKE_ERR_BAD_ARG; }
+    if (set_len > 0 && n_sets > INT64_MAX / set_len) { set_error("n_sets * set_len overflows"); return BKE_ERR_BAD_ARG; }
+    const int64_t n = n_sets * set_len;
+    return gather_rows(n, n, row_bytes, src, indexes, index_is_64, dst, err, set_len, stream);
 }
 
 }  // extern "C"

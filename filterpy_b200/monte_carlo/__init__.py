@@ -1,4 +1,6 @@
 """GPU mirrors of ``filterpy.monte_carlo`` for the hot path."""
 from .resampling import (systematic_resample, stratified_resample, multinomial_resample, residual_resample,  # noqa: F401
                          residual_resample_with_uniforms,
-                         gather_particles, exact_cumsum, ResamplePlan, normalize_weights)
+                         gather_particles, exact_cumsum, ResamplePlan, normalize_weights,
+                         systematic_resample_bank, stratified_resample_bank, gather_particles_bank,
+                         BankResamplePlan)

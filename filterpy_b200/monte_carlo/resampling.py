@@ -19,7 +19,8 @@ from .._dev import require_cuda, stream_ptr
 
 __all__ = ["systematic_resample", "stratified_resample", "multinomial_resample", "residual_resample",
            "gather_particles", "exact_cumsum", "ResamplePlan", "normalize_weights",
-           "residual_resample_with_uniforms"]
+           "residual_resample_with_uniforms", "systematic_resample_bank", "stratified_resample_bank",
+           "gather_particles_bank", "BankResamplePlan"]
 
 
 class ResamplePlan(object):
@@ -303,3 +304,168 @@ def gather_particles(particles, indexes, out=None, check=True):
         if check and int(err.item()):
             raise IndexError("index out of bounds for axis 0 with size %d" % n_src)
     return out if (is_torch and particles.is_cuda) else out.cpu().numpy()
+
+
+# ------------------------------------------------------------------------------------------- banks
+def _bank_tensor_check(t, name, dtypes, shape, device):
+    if not (isinstance(t, torch.Tensor) and t.device == device and t.dtype in dtypes and t.is_contiguous()
+            and tuple(t.shape) == tuple(shape)):
+        raise ValueError("%s must be a contiguous %s tensor of shape %s on %s"
+                         % (name, " or ".join(str(d) for d in dtypes), tuple(shape), device))
+
+
+class BankResamplePlan(object):
+    """Output buffers for repeated resampling of a bank of ``n_sets`` particle sets of ``n_particles``
+    each on one GPU (``csrc/resample_bank.cu``): row ``b`` of the weights is one set, resampled as the
+    reference resamples one weight vector.  A call allocates nothing and does not synchronise the host,
+    so it can be captured in a CUDA graph.
+
+    ``status`` (int32 CUDA tensor [n_sets]) is 1 for a set whose positions ran past its cumulative sum
+    (the reference's ``IndexError``, resampling.py:145; that row's indexes are unspecified), else 0."""
+
+    def __init__(self, n_sets, n_particles, device=None):
+        self.n_sets = int(n_sets)
+        self.n_particles = int(n_particles)
+        if self.n_sets < 0 or self.n_particles < 0:
+            raise ValueError("n_sets and n_particles must be >= 0")
+        self.device = require_cuda(device)
+        self._lib = _lib.load()
+        self.indexes = torch.empty((self.n_sets, self.n_particles), dtype=torch.int32, device=self.device)
+        self.status = torch.zeros(self.n_sets, dtype=torch.int32, device=self.device)
+        self._err = torch.zeros(1, dtype=torch.int32, device=self.device)
+
+    def _run(self, weights, u, uniforms, out):
+        shape = (self.n_sets, self.n_particles)
+        _bank_tensor_check(weights, "weights", (torch.float64,), shape, self.device)
+        out = self.indexes if out is None else out
+        _bank_tensor_check(out, "out", (torch.int32,), shape, self.device)
+        a = _lib.ResampleBankArgs()
+        a.n_sets, a.n_particles = self.n_sets, self.n_particles
+        a.weights, a.indexes, a.status = weights.data_ptr(), out.data_ptr(), self.status.data_ptr()
+        a.u = u.data_ptr() if u is not None else None
+        a.uniforms = uniforms.data_ptr() if uniforms is not None else None
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.bke_resample_bank(ctypes.byref(a), stream_ptr(self.device)))
+        return out
+
+    def systematic(self, weights, u, out=None):
+        """indexes[b] for the offsets ``u[b]`` (float64 CUDA tensor [n_sets]; resampling.py:139:
+        positions = (u[b] + arange(M)) / M)."""
+        _bank_tensor_check(u, "u", (torch.float64,), (self.n_sets,), self.device)
+        return self._run(weights, u, None, out)
+
+    def stratified(self, weights, uniforms, out=None):
+        """indexes[b] for the per-particle uniforms ``uniforms[b]`` (float64 CUDA tensor [n_sets, M];
+        resampling.py:103: positions = (U[b] + arange(M)) / M)."""
+        _bank_tensor_check(uniforms, "uniforms", (torch.float64,), (self.n_sets, self.n_particles), self.device)
+        return self._run(weights, None, uniforms, out)
+
+    def gather(self, particles, indexes=None, out=None):
+        """``out[b] = particles[b][indexes[b]]`` (indexes default: the plan's last result).  No host
+        synchronisation: an index outside [0, n_particles) is reported by ``raise_if_bad_index``."""
+        indexes = self.indexes if indexes is None else indexes
+        if not (isinstance(particles, torch.Tensor) and particles.device == self.device
+                and tuple(particles.shape[:2]) == (self.n_sets, self.n_particles)):
+            raise ValueError("particles must be a CUDA tensor of shape (%d, %d, ...) on %s"
+                             % (self.n_sets, self.n_particles, self.device))
+        return _gather_bank(particles, indexes, out, self._err)
+
+    def raise_if_overflow(self):
+        """IndexError naming the first set whose positions ran past its cumulative sum (host sync)."""
+        _raise_first_overflow(self.status, self.n_particles)
+
+    def raise_if_bad_index(self):
+        """IndexError if a ``gather`` since the last check met an index outside [0, n_particles) (host sync)."""
+        if int(self._err.item()):
+            self._err.zero_()
+            raise IndexError("index out of bounds for axis 1 with size %d" % self.n_particles)
+
+
+def _raise_first_overflow(status, n_particles):
+    bad = torch.nonzero(status).flatten()
+    if bad.numel():
+        raise IndexError("set %d: index %d is out of bounds for axis 0 with size %d"
+                         % (int(bad[0]), n_particles, n_particles))
+
+
+def _run_bank(weights, stratified):
+    is_torch, w, dev = _weights_on_device(weights)
+    if w.dim() != 2:
+        raise ValueError("weights must be 2-D (n_sets, n_particles); got shape %s" % (tuple(w.shape),))
+    B, M = w.shape
+    # the reference's loop draws random() (random(M) stratified) once per row; random(B) and random((B, M))
+    # take the same values from the global stream in the same order
+    draw = random((B, M)) if stratified else random(B)
+    plan = BankResamplePlan(B, M, dev)
+    if B and M:
+        U = torch.from_numpy(np.ascontiguousarray(draw)).to(dev)
+        idx = plan.stratified(w, U) if stratified else plan.systematic(w, U)
+        plan.raise_if_overflow()                          # resampling.py:145 (IndexError), first failing row
+    else:
+        idx = plan.indexes
+    return idx if is_torch else idx.cpu().numpy()
+
+
+def systematic_resample_bank(weights):
+    """``systematic_resample`` (resampling.py:117-150) of every row of ``weights[B, M]`` in one launch:
+    returns int32 ``(B, M)``, an ndarray for array input, a CUDA tensor for a CUDA tensor.  Seeded with
+    ``np.random.seed``, the result and the stream position afterwards equal a Python loop of the
+    reference over the rows.  A failing row raises ``IndexError`` naming the first such row, where that
+    loop would have stopped; unlike the loop, the bank has by then drawn the uniforms of all B rows."""
+    return _run_bank(weights, False)
+
+
+def stratified_resample_bank(weights):
+    """``stratified_resample`` (resampling.py:80-114) of every row of ``weights[B, M]`` in one launch
+    (uniforms drawn as ``random((B, M))``); otherwise as ``systematic_resample_bank``."""
+    return _run_bank(weights, True)
+
+
+def _gather_bank(particles, indexes, out, err):
+    """particles (B, M, ...) and indexes (B, M) contiguous on one CUDA device; the kernel reads raw rows."""
+    if not (isinstance(particles, torch.Tensor) and particles.is_cuda and particles.is_contiguous()
+            and particles.dim() >= 2):
+        raise ValueError("particles must be a contiguous CUDA tensor of shape (n_sets, n_particles, ...)")
+    dev = particles.device
+    _bank_tensor_check(indexes, "indexes", (torch.int32, torch.int64), particles.shape[:2], dev)
+    B, M = indexes.shape
+    row_bytes = (particles.numel() // max(B * M, 1)) * particles.element_size()
+    if out is None:
+        out = torch.empty_like(particles)
+    else:
+        _bank_tensor_check(out, "out", (particles.dtype,), particles.shape, dev)
+    if B * M and row_bytes:
+        with torch.cuda.device(dev):
+            _lib.check(_lib.load().bke_gather_rows_bank(B, M, row_bytes, particles.data_ptr(), indexes.data_ptr(),
+                                                        1 if indexes.dtype == torch.int64 else 0, out.data_ptr(),
+                                                        err.data_ptr(), stream_ptr(dev)))
+    return out
+
+
+def gather_particles_bank(particles, indexes, out=None, check=True):
+    """``particles[b][indexes[b]]`` for every set b of a bank, on the GPU: ``particles`` is (B, M, ...) of
+    any dtype, ``indexes`` (B, M) int32 or int64 (what the bank resamplers return).  NumPy in -> NumPy out,
+    CUDA tensors in -> CUDA tensor out.  Raises IndexError for an index outside [0, M) like NumPy does
+    (negative indexes are not wrapped); ``check=False`` skips that test and the host synchronisation it
+    costs."""
+    is_torch = isinstance(particles, torch.Tensor) and particles.is_cuda
+    if is_torch:
+        dev = particles.device
+        src = particles.contiguous()
+    else:
+        dev = require_cuda(None)
+        src = torch.from_numpy(np.ascontiguousarray(np.asarray(particles))).to(dev)
+    if isinstance(indexes, torch.Tensor):
+        idx = indexes.to(dev)
+    else:
+        idx = torch.from_numpy(np.ascontiguousarray(np.asarray(indexes))).to(dev)
+    if idx.dtype not in (torch.int32, torch.int64):
+        raise IndexError("arrays used as indices must be of integer type")
+    if idx.dim() != 2 or src.dim() < 2:
+        raise ValueError("particles must be (n_sets, n_particles, ...) and indexes (n_sets, n_particles)")
+    idx = idx.contiguous()
+    err = torch.zeros(1, dtype=torch.int32, device=dev)
+    out = _gather_bank(src, idx, out, err)
+    if check and int(err.item()):
+        raise IndexError("index out of bounds for axis 1 with size %d" % idx.shape[1])
+    return out if is_torch else out.cpu().numpy()

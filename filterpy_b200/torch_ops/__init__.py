@@ -13,6 +13,8 @@ The same symbols exposed as torch.ops.* via a C++ extension for zero-copy CUDA t
     xs, xhat = torch.ops.bke.fls_smooth_batch(x, P, F, H, Q, R, zs, N)   # fixed_lag_smoother.py:217-311
     idx  = torch.ops.bke.systematic_resample(weights, u)           # resampling.py:117-150 (int32, bit-exact)
     idx  = torch.ops.bke.stratified_resample(weights, uniforms)    # resampling.py:80-114
+    idx  = torch.ops.bke.systematic_resample_bank(weights, u)      # every row of weights[B, M], u[B]
+    idx  = torch.ops.bke.stratified_resample_bank(weights, uniforms)   # uniforms[B, M]
 
 Models are shared by the bank when 2-D (stride 0) and per filter when 3-D.  Only the CUDA backend is
 registered: CPU tensors raise ``NotImplementedError`` (no CPU fallback).  The operators run on the

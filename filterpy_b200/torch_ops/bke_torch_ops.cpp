@@ -10,6 +10,8 @@
 //   bke::fls_smooth_batch     bke_fls_smooth           FixedLagSmoother.smooth_batch, fixed_lag_smoother.py:217-311
 //   bke::systematic_resample  bke_systematic_resample  monte_carlo/resampling.py:117-150
 //   bke::stratified_resample  bke_stratified_resample  monte_carlo/resampling.py:80-114
+//   bke::systematic_resample_bank  bke_resample_bank   resampling.py:117-150 on every row of weights[B, M]
+//   bke::stratified_resample_bank  bke_resample_bank   resampling.py:80-114 on every row of weights[B, M]
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
@@ -254,6 +256,37 @@ at::Tensor resample(const at::Tensor &w, double u, const c10::optional<at::Tenso
 at::Tensor systematic_resample(const at::Tensor &w, double u) { return resample(w, u, c10::nullopt); }
 at::Tensor stratified_resample(const at::Tensor &w, const at::Tensor &U) { return resample(w, 0.0, U); }
 
+at::Tensor resample_bank(const at::Tensor &w, const at::Tensor *u, const at::Tensor *U)
+{
+    TORCH_CHECK(w.is_cuda() && w.is_contiguous() && w.scalar_type() == at::kDouble && w.dim() == 2, "bke: weights must be a contiguous 2-D float64 CUDA tensor");
+    c10::cuda::CUDAGuard guard(w.device());
+    const int64_t B = w.size(0), M = w.size(1);
+    const at::Tensor &r = u ? *u : *U;
+    TORCH_CHECK(r.is_cuda() && r.is_contiguous() && r.scalar_type() == at::kDouble && r.device() == w.device(), "bke: uniforms must be a contiguous float64 CUDA tensor on the weights' device");
+    if (u) {
+        TORCH_CHECK(r.dim() == 1 && r.size(0) == B, "bke: u must be [n_sets]");
+    } else {
+        TORCH_CHECK(r.dim() == 2 && r.size(0) == B && r.size(1) == M, "bke: uniforms must be [n_sets, n_particles]");
+    }
+    at::Tensor idx = at::empty({B, M}, w.options().dtype(at::kInt));
+    if (B == 0 || M == 0) return idx;
+    at::Tensor status = at::empty({B}, w.options().dtype(at::kInt));
+    bke_resample_bank_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_sets = B; a.n_particles = M; a.weights = (const double *)w.data_ptr();
+    if (u) a.u = (const double *)r.data_ptr(); else a.uniforms = (const double *)r.data_ptr();
+    a.indexes = (int32_t *)idx.data_ptr(); a.status = (int32_t *)status.data_ptr();
+    check_rc(bke_resample_bank(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_resample_bank");
+    // resampling.py:145: the first row whose positions run past its cumsum is where the reference loop raises
+    const at::Tensor bad = status.nonzero();
+    TORCH_CHECK_INDEX(bad.numel() == 0, "set ", bad.numel() ? bad[0][0].item<int64_t>() : 0, ": index ", M,
+                      " is out of bounds for axis 0 with size ", M);
+    return idx;
+}
+
+at::Tensor systematic_resample_bank(const at::Tensor &w, const at::Tensor &u) { return resample_bank(w, &u, nullptr); }
+at::Tensor stratified_resample_bank(const at::Tensor &w, const at::Tensor &U) { return resample_bank(w, nullptr, &U); }
+
 }  // namespace
 
 TORCH_LIBRARY(bke, m)
@@ -270,6 +303,8 @@ TORCH_LIBRARY(bke, m)
     m.def("fls_smooth_batch(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor zs, int N) -> (Tensor, Tensor)");
     m.def("systematic_resample(Tensor weights, float u) -> Tensor");
     m.def("stratified_resample(Tensor weights, Tensor uniforms) -> Tensor");
+    m.def("systematic_resample_bank(Tensor weights, Tensor u) -> Tensor");
+    m.def("stratified_resample_bank(Tensor weights, Tensor uniforms) -> Tensor");
 }
 
 TORCH_LIBRARY_IMPL(bke, CUDA, m)
@@ -283,4 +318,6 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("fls_smooth_batch", &fls_smooth_batch);
     m.impl("systematic_resample", &systematic_resample);
     m.impl("stratified_resample", &stratified_resample);
+    m.impl("systematic_resample_bank", &systematic_resample_bank);
+    m.impl("stratified_resample_bank", &stratified_resample_bank);
 }

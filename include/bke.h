@@ -662,6 +662,28 @@ int bke_resample_shard_compose(const bke_resample_shard_args *args, void *compos
 int bke_resample_compose_carry(int32_t n_shards_before, const void *composites, double *carry_exact,
                                int32_t *status, void *stream);
 
+/* A BANK of independent particle sets in one launch: row b of weights[n_sets, n_particles] (fp64, dense)
+ * is one set, and row b of indexes[n_sets, n_particles] (int32) is, bit for bit, what the reference's
+ * systematic_resample / stratified_resample returns for that row (resampling.py:141-149 / :105-113,
+ * literally, for ANY values: negative, NaN, infinite, -0.0 and subnormal weights, and any u / uniforms,
+ * including values outside [0, 1) and out of order) with positions
+ *   (u[b] + arange(M)) / M          systematic, u[n_sets]               (:139)
+ *   (uniforms[b] + arange(M)) / M   stratified, uniforms[n_sets, M]     (:103)
+ * Give exactly one of u and uniforms.  status[b] (optional) = 1 where the positions run past
+ * cumsum(weights[b])[-1] (the reference's IndexError, :145; that row's indexes are unspecified), else 0.
+ * n_sets = 0 or n_particles = 0 does nothing; n_particles < 2^31.  No workspace, no allocation, no host
+ * sync: the call can be captured in a CUDA graph. */
+typedef struct bke_resample_bank_args {
+    int64_t n_sets, n_particles;
+    const double *weights;       /* [n_sets, n_particles] */
+    const double *u;             /* [n_sets] (systematic) or NULL */
+    const double *uniforms;      /* [n_sets, n_particles] (stratified) or NULL */
+    int32_t *indexes;            /* [n_sets, n_particles] */
+    int32_t *status;             /* [n_sets] or NULL */
+} bke_resample_bank_args;
+
+int bke_resample_bank(const bke_resample_bank_args *args, void *stream);
+
 /* sum of weights (fp64, deterministic tree order) — the quantity that is all-reduced across
  * GPUs before a distributed resample; also used to normalise: weights_out[i] = weights[i] / sum
  * (IEEE division, the same elementwise operation as NumPy's `w / w.sum()` given that sum). */
@@ -766,7 +788,10 @@ int bke_mm_estimate(const bke_mm_args *args, void *stream);
  * bke_gather_rows: dst[r, :] = src[indexes[r], :] for rows of row_bytes bytes — the
  *   `particles[:] = particles[indexes]` that follows every resample (docs/monte_carlo/resampling.rst:4-8);
  *   indexes int32 (systematic / stratified) or int64 (multinomial); *err is set to 1 if an index is
- *   outside [0, n_src) (that row is left untouched).  src and dst must not alias. */
+ *   outside [0, n_src) (that row is left untouched).  src and dst must not alias.
+ * bke_gather_rows_bank: the same per set of a bank, dst[b, i, :] = src[b, indexes[b, i], :] for
+ *   n_sets sets of set_len rows each (the gather after bke_resample_bank); *err is set to 1 if an index is
+ *   outside [0, set_len). */
 int bke_cumsum_exact(int64_t n, const double *weights, double *cumsum_out, int32_t last_one, void *workspace,
                      size_t workspace_bytes, int32_t *info, void *stream);
 int bke_searchsorted(int64_t n, const double *sorted, int64_t n_keys, const double *keys, int32_t side_right,
@@ -776,6 +801,8 @@ int bke_multinomial_resample(int64_t n, const double *weights, const double *uni
                              int32_t *info, void *stream);
 int bke_gather_rows(int64_t n_out, int64_t n_src, int64_t row_bytes, const void *src, const void *indexes,
                     int32_t index_is_64, void *dst, int32_t *err, void *stream);
+int bke_gather_rows_bank(int64_t n_sets, int64_t set_len, int64_t row_bytes, const void *src, const void *indexes,
+                         int32_t index_is_64, void *dst, int32_t *err, void *stream);
 
 /* ---- residual_resample (filterpy/monte_carlo/resampling.py:27-76) --------------------------------
  *
