@@ -42,6 +42,9 @@ EXPORTED_SYMBOLS = [
     "bke_srkf_step", "bke_cholesky_lower",
     "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
     "bke_resample_bank", "bke_gather_rows_bank",
+    "bke_multinomial_resample_bank_workspace_bytes", "bke_multinomial_resample_bank",
+    "bke_residual_resample_bank_workspace_bytes", "bke_residual_resample_bank_prepare",
+    "bke_residual_resample_bank_search",
     "bke_residual_workspace_bytes", "bke_residual_prepare", "bke_searchsorted_bracket_sweep",
 ]
 
@@ -224,6 +227,24 @@ class ResampleBankArgs(ctypes.Structure):
         ("n_sets", c_int64), ("n_particles", c_int64),
         ("weights", c_void_p), ("u", c_void_p), ("uniforms", c_void_p),
         ("indexes", c_void_p), ("status", c_void_p),
+    ]
+
+
+class MultinomialResampleBankArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_sets", c_int64), ("n_particles", c_int64),
+        ("weights", c_void_p), ("uniforms", c_void_p),
+        ("indexes", c_void_p), ("status", c_void_p),
+        ("workspace", c_void_p), ("workspace_bytes", c_size_t),
+    ]
+
+
+class ResidualResampleBankArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_sets", c_int64), ("n_particles", c_int64),
+        ("weights", c_void_p), ("uniforms", c_void_p),
+        ("indexes", c_void_p), ("n_copies", c_void_p), ("status", c_void_p),
+        ("workspace", c_void_p), ("workspace_bytes", c_size_t),
     ]
 
 
@@ -456,6 +477,14 @@ def load():
     lib.bke_gather_rows_bank.restype = ctypes.c_int
     lib.bke_resample_bank.argtypes = [ctypes.POINTER(ResampleBankArgs), c_void_p]
     lib.bke_resample_bank.restype = ctypes.c_int
+    for name in ("bke_multinomial_resample_bank_workspace_bytes", "bke_residual_resample_bank_workspace_bytes"):
+        getattr(lib, name).argtypes = [c_int64, c_int64]
+        getattr(lib, name).restype = c_size_t
+    lib.bke_multinomial_resample_bank.argtypes = [ctypes.POINTER(MultinomialResampleBankArgs), c_void_p]
+    lib.bke_multinomial_resample_bank.restype = ctypes.c_int
+    for name in ("bke_residual_resample_bank_prepare", "bke_residual_resample_bank_search"):
+        getattr(lib, name).argtypes = [ctypes.POINTER(ResidualResampleBankArgs), c_void_p]
+        getattr(lib, name).restype = ctypes.c_int
     lib.bke_residual_workspace_bytes.argtypes = [c_int64]
     lib.bke_residual_workspace_bytes.restype = c_size_t
     lib.bke_residual_prepare.argtypes = [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,

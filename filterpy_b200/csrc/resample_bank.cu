@@ -22,7 +22,26 @@
 // Each round consumes at least one window per unfinished set, so a set of M particles finishes in at
 // most 2M / COLS + 1 rounds.  Global traffic: weights (and uniforms) read once, indexes written once,
 // all as 256-byte / 128-byte row segments.
+//
+// Below k_resample_bank: multinomial (resampling.py:153-176) and residual (:27-76) resampling of a bank.
+// Both end in np.searchsorted(c, keys) (side='left') over a per-set array c, which NumPy bisects with a
+// bracket carried from key to key ([r[i-1], M) if key[i-1] < key[i], else [0, r[i-1] + 1), NaN last;
+// csrc/residual.cu).  One warp per set:
+//   k_prepare_bank   the strictly sequential parts literally: builtin sum(residual) and np.cumsum, one
+//                    __dadd_rn per element, the chain fed by a warp shuffle of 32 coalesced loads; c goes
+//                    to the workspace with c[-1] = 1.  Residual also writes the copies repeat(arange(M),
+//                    num_copies) as coalesced 32-wide segments, and k.  The set is marked for the exact
+//                    search unless c[0..M-2] is nondecreasing in NaN-last order and c[M-2] <= 1: then the
+//                    whole c is sorted, less(c[i], key) holds on a prefix for every key, any bracket NumPy
+//                    carries contains that prefix's end, and every key can be searched on its own.
+//   k_search_bank    32 keys per round, one per lane.  A sorted set takes one bisection per key.  Any other
+//                    set runs the carried-bracket recurrence as a fixed point inside the round: each lane
+//                    re-bisects from the bracket its left neighbour's current answer gives (lane 0: the
+//                    previous round's last key and answer, which are final), until a sweep changes no lane.
+//                    After t sweeps the first t lanes are final, so a round takes at most 33 sweeps; on
+//                    residual's sets two or three are typical.
 #include "bke_internal.cuh"
+#include "residual_rules.cuh"
 
 namespace bke {
 namespace rsb {
@@ -126,6 +145,173 @@ __global__ void __launch_bounds__(ROWS) k_resample_bank(i64 n_sets, i64 M, const
     }
 }
 
+// ---------------------------------------------------------------------- multinomial / residual
+constexpr int MR_WARPS = 8;                    // sets per CTA, one warp each
+constexpr int ST_FAIL = 1;                     // status bit: the reference raises IndexError (residual: k > M)
+constexpr int ST_EXACT = 2;                    // status bit: the set takes the carried-bracket search
+
+__device__ __forceinline__ int warp_incl_scan(int v, int lane)
+{
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(FULL, v, o); if (lane >= o) v += y; }
+    return v;
+}
+
+// c = np.cumsum(w) (multinomial, :173) or np.cumsum(residual / sum(residual)) (residual, :69-71), c[-1] = 1;
+// residual also writes indexes[b, :k] and k[b].  status[b] = ST_FAIL where k > M, else ST_EXACT or 0.
+template <bool RESIDUAL>
+__global__ void __launch_bounds__(32 * MR_WARPS) k_prepare_bank(i64 n_sets, int M, const double *__restrict__ w,
+                                                                 double *__restrict__ cws, int *__restrict__ idx,
+                                                                 i64 *__restrict__ k_out, int *__restrict__ status)
+{
+    const int lane = threadIdx.x & 31;
+    const i64 b = (i64)blockIdx.x * MR_WARPS + (threadIdx.x >> 5);
+    if (b >= n_sets) return;                                  // whole warps leave
+    const double *wr = w + b * M;
+    double *cr = cws + b * M;
+    const double Md = (double)M;
+    double s = 0.0;
+    if (RESIDUAL) {
+        // k (copies, saturated at M + 1) and s = 0 + r0 + r1 + ... (:70, the builtin sum)
+        i64 k = 0;
+        for (int j0 = 0; j0 < M; j0 += 32) {
+            const int j = j0 + lane, n = M - j0 < 32 ? M - j0 : 32;
+            const double x = j < M ? __ldg(wr + j) : 0.0;
+            const double r = rr::residual_of(Md, x);
+            i64 cnt = j < M ? rr::copies_made(Md, x) : 0;
+            cnt = cnt > (i64)M + 1 ? (i64)M + 1 : cnt;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(FULL, cnt, o);
+            k = k + cnt > (i64)M + 1 ? (i64)M + 1 : k + cnt;
+            for (int t = 0; t < n; t++) s = __dadd_rn(s, __shfl_sync(FULL, r, t));
+        }
+        if (lane == 0) k_out[b] = k;
+        if (k > M) {                                          // indexes[k] = i runs off the end (:61)
+            if (lane == 0) status[b] = ST_FAIL;
+            return;
+        }
+    }
+    double acc = 0.0;                                         // c[j0 - 1]
+    bool unsorted = false;
+    int off = 0;                                              // copies written so far
+    int *ir = RESIDUAL ? idx + b * M : nullptr;
+    for (int j0 = 0; j0 < M; j0 += 32) {
+        const int j = j0 + lane, n = M - j0 < 32 ? M - j0 : 32;
+        const double x = j < M ? __ldg(wr + j) : 0.0;
+        const double v = RESIDUAL ? __ddiv_rn(rr::residual_of(Md, x), s) : x;
+        const double before = acc;
+        double mine = 0.0;
+        for (int t = 0; t < n; t++) {                         // np.cumsum: c_0 = v_0, then one add per element
+            const double y = __shfl_sync(FULL, v, t);
+            acc = (j0 == 0 && t == 0) ? y : __dadd_rn(acc, y);
+            if (lane == t) mine = acc;
+        }
+        double left = __shfl_up_sync(FULL, mine, 1);
+        if (lane == 0) left = before;
+        if (j >= 1 && j <= M - 2 && rr::np_lt(mine, left)) unsorted = true;
+        if (j == M - 2 && rr::np_lt(1.0, mine)) unsorted = true;   // c[-1] = 1 would end the sort
+        if (j < M) cr[j] = j == M - 1 ? 1.0 : mine;                // :174 / :72
+        if (RESIDUAL) {                                       // repeat(arange(M), num_copies) (:58-62), in order
+            const int cnt = j < M ? (int)rr::copies_made(Md, x) : 0;
+            const int inc = warp_incl_scan(cnt, lane);
+            const int tot = __shfl_sync(FULL, inc, 31);
+            for (int q0 = 0; q0 < tot; q0 += 32) {
+                const int q = q0 + lane;
+                int lo = 0, hi = 31;                          // the first lane whose inclusive count exceeds q
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (__shfl_sync(FULL, inc, mid) > q) hi = mid; else lo = mid + 1;
+                }
+                if (q < tot) ir[off + q] = j0 + lo;
+            }
+            off += tot;
+        }
+    }
+    unsorted = __any_sync(FULL, unsorted);
+    if (lane == 0) status[b] = unsorted ? ST_EXACT : 0;
+}
+
+// np.searchsorted(c, key) over [lo, hi): NumPy's left bisection in NaN-last order
+__device__ __forceinline__ int bisect(const double *__restrict__ c, double key, int lo, int hi)
+{
+    while (lo < hi) {
+        const int mid = lo + ((hi - lo) >> 1);
+        if (rr::np_lt(__ldg(c + mid), key)) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+
+// indexes[b, k_b + q] = searchsorted(c_b, keys[b, q]) for q < M - k_b (multinomial: k_b = 0)
+template <bool RESIDUAL, typename I>
+__global__ void __launch_bounds__(32 * MR_WARPS) k_search_bank(i64 n_sets, int M, const double *__restrict__ cws,
+                                                                const double *__restrict__ U,
+                                                                const i64 *__restrict__ k_in,
+                                                                const int *__restrict__ status, I *__restrict__ idx)
+{
+    const int lane = threadIdx.x & 31;
+    const i64 b = (i64)blockIdx.x * MR_WARPS + (threadIdx.x >> 5);
+    if (b >= n_sets) return;
+    const int st = status[b];
+    if (st & ST_FAIL) return;
+    const int k = RESIDUAL ? (int)k_in[b] : 0;
+    const int n = M - k;
+    const double *c = cws + b * M, *keys = U + b * M;
+    I *out = idx + b * M + k;
+    const bool exact = st & ST_EXACT;
+    double ck = 0.0;                                          // the previous round's last key and answer
+    int cr = 0;
+    for (int q0 = 0; q0 < n; q0 += 32) {
+        const int q = q0 + lane;
+        const bool valid = q < n;
+        const double key = valid ? __ldg(keys + q) : 0.0;
+        int r = bisect(c, key, 0, M);
+        if (exact) {
+            for (;;) {
+                double pk = __shfl_up_sync(FULL, key, 1);
+                int pr = __shfl_up_sync(FULL, r, 1);
+                if (lane == 0) { pk = ck; pr = cr; }
+                int lo = 0, hi = M;                           // the first key: [0, M)
+                if (q > 0) {
+                    if (rr::np_lt(pk, key)) lo = pr;
+                    else hi = pr < M ? pr + 1 : M;
+                }
+                const int nr = bisect(c, key, lo, hi);
+                const bool changed = valid && nr != r;
+                r = nr;
+                if (!__any_sync(FULL, changed)) break;
+            }
+            const int last = n - q0 < 32 ? n - q0 - 1 : 31;
+            ck = __shfl_sync(FULL, key, last);
+            cr = __shfl_sync(FULL, r, last);
+        }
+        if (valid) out[q] = (I)r;
+    }
+}
+
+static size_t mr_ws_bytes(i64 B, i64 M)
+{
+    if (B <= 0 || M <= 0) return 0;
+    if (B > (i64)(SIZE_MAX / 8) / M) return SIZE_MAX;
+    return (size_t)B * (size_t)M * sizeof(double);
+}
+
+// the checks every multinomial / residual bank call shares; *done = 1: nothing to compute
+static int mr_check(i64 B, i64 M, const void *ws, size_t ws_bytes, int *done)
+{
+    *done = 0;
+    if (B < 0 || M < 0) { set_error("n_sets and n_particles must be >= 0"); return BKE_ERR_BAD_ARG; }
+    if (M >= ((i64)1 << 31)) { set_error("n_particles must be < 2^31"); return BKE_ERR_BAD_ARG; }
+    if (B == 0 || M == 0) { *done = 1; return BKE_OK; }
+    if ((B + MR_WARPS - 1) / MR_WARPS >= ((i64)1 << 31) || mr_ws_bytes(B, M) == SIZE_MAX) {
+        set_error("n_sets too large"); return BKE_ERR_BAD_ARG;
+    }
+    if (!ws || (reinterpret_cast<uintptr_t>(ws) & 7)) { set_error("workspace must be non-NULL and 8-byte aligned"); return BKE_ERR_BAD_ARG; }
+    if (ws_bytes < mr_ws_bytes(B, M)) {
+        set_error("workspace too small: %zu < %zu", ws_bytes, mr_ws_bytes(B, M)); return BKE_ERR_BAD_ARG;
+    }
+    return BKE_OK;
+}
+
 }  // namespace rsb
 }  // namespace bke
 
@@ -151,6 +337,65 @@ int bke_resample_bank(const bke_resample_bank_args *a, void *stream)
         rsb::k_resample_bank<false><<<(unsigned)blocks, rsb::ROWS, 0, s>>>(a->n_sets, a->n_particles, a->weights, a->u,
                                                                           nullptr, a->indexes, a->status);
     return check_cuda(cudaGetLastError(), "resample bank launch");
+}
+
+size_t bke_multinomial_resample_bank_workspace_bytes(int64_t n_sets, int64_t n_particles)
+{
+    return rsb::mr_ws_bytes(n_sets, n_particles);
+}
+
+size_t bke_residual_resample_bank_workspace_bytes(int64_t n_sets, int64_t n_particles)
+{
+    return rsb::mr_ws_bytes(n_sets, n_particles);
+}
+
+int bke_multinomial_resample_bank(const bke_multinomial_resample_bank_args *a, void *stream)
+{
+    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    int done, rc = rsb::mr_check(a->n_sets, a->n_particles, a->workspace, a->workspace_bytes, &done);
+    if (rc != BKE_OK || done) return rc;
+    if (!a->weights || !a->uniforms || !a->indexes || !a->status) {
+        set_error("weights, uniforms, indexes and status must be non-NULL"); return BKE_ERR_BAD_ARG;
+    }
+    const unsigned blocks = (unsigned)((a->n_sets + rsb::MR_WARPS - 1) / rsb::MR_WARPS);
+    const int M = (int)a->n_particles;
+    double *c = (double *)a->workspace;
+    cudaStream_t s = (cudaStream_t)stream;
+    rsb::k_prepare_bank<false><<<blocks, 32 * rsb::MR_WARPS, 0, s>>>(a->n_sets, M, a->weights, c, nullptr, nullptr,
+                                                                     a->status);
+    rsb::k_search_bank<false, long long><<<blocks, 32 * rsb::MR_WARPS, 0, s>>>(
+        a->n_sets, M, c, a->uniforms, nullptr, a->status, (long long *)a->indexes);
+    return check_cuda(cudaGetLastError(), "multinomial bank launch");
+}
+
+int bke_residual_resample_bank_prepare(const bke_residual_resample_bank_args *a, void *stream)
+{
+    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    int done, rc = rsb::mr_check(a->n_sets, a->n_particles, a->workspace, a->workspace_bytes, &done);
+    if (rc != BKE_OK || done) return rc;
+    if (!a->weights || !a->indexes || !a->n_copies || !a->status) {
+        set_error("weights, indexes, n_copies and status must be non-NULL"); return BKE_ERR_BAD_ARG;
+    }
+    const unsigned blocks = (unsigned)((a->n_sets + rsb::MR_WARPS - 1) / rsb::MR_WARPS);
+    rsb::k_prepare_bank<true><<<blocks, 32 * rsb::MR_WARPS, 0, (cudaStream_t)stream>>>(
+        a->n_sets, (int)a->n_particles, a->weights, (double *)a->workspace, a->indexes, (rsb::i64 *)a->n_copies,
+        a->status);
+    return check_cuda(cudaGetLastError(), "residual bank prepare launch");
+}
+
+int bke_residual_resample_bank_search(const bke_residual_resample_bank_args *a, void *stream)
+{
+    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    int done, rc = rsb::mr_check(a->n_sets, a->n_particles, a->workspace, a->workspace_bytes, &done);
+    if (rc != BKE_OK || done) return rc;
+    if (!a->uniforms || !a->indexes || !a->n_copies || !a->status) {
+        set_error("uniforms, indexes, n_copies and status must be non-NULL"); return BKE_ERR_BAD_ARG;
+    }
+    const unsigned blocks = (unsigned)((a->n_sets + rsb::MR_WARPS - 1) / rsb::MR_WARPS);
+    rsb::k_search_bank<true, int><<<blocks, 32 * rsb::MR_WARPS, 0, (cudaStream_t)stream>>>(
+        a->n_sets, (int)a->n_particles, (const double *)a->workspace, a->uniforms, (const rsb::i64 *)a->n_copies,
+        a->status, a->indexes);
+    return check_cuda(cudaGetLastError(), "residual bank search launch");
 }
 
 }  // extern "C"

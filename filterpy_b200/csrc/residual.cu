@@ -20,12 +20,11 @@
 //    previous sweep's values; after t sweeps the first t+1 answers are final, and a sweep that changes
 //    nothing proves the whole array (the brackets only differ where the array is locally non-monotone,
 //    so two or three sweeps are typical).  The host repeats sweeps until `changed` stays 0.
-#include "bke_internal.cuh"
+#include "residual_rules.cuh"
 
 namespace bke {
 namespace rr {
 
-typedef long long i64;
 constexpr int RB = 256;                 // threads per CTA
 constexpr int RIPT = 8;                 // particles per thread
 constexpr int RTILE = RB * RIPT;        // 2048 particles per tile
@@ -53,13 +52,6 @@ static void carve(i64 n, unsigned char *base, RWs *ws)
     ws->tile_off = reinterpret_cast<i64 *>(p);
     ws->T = (int)T;
 }
-
-// resampling.py:57 — floor(N * w) as int64 (N * w is one fp64 multiply of float(N) and w)
-__device__ __forceinline__ i64 num_copies(double Nd, double w) { return __double2ll_rz(floor(__dmul_rn(Nd, w))); }
-// resampling.py:69 — w - num_copies (int64 -> fp64 is exact below 2^53)
-__device__ __forceinline__ double residual_of(double Nd, double w) { return __dsub_rn(w, (double)num_copies(Nd, w)); }
-// range(num_copies[i]) is empty for a negative count (resampling.py:60)
-__device__ __forceinline__ i64 copies_made(double Nd, double w) { const i64 c = num_copies(Nd, w); return c > 0 ? c : 0; }
 
 __device__ __forceinline__ i64 block_sum_i64(i64 v, i64 *sh)
 {
@@ -213,9 +205,6 @@ __global__ void __launch_bounds__(32, 1) k_residual_seq(i64 n, const double *__r
         __syncwarp();
     }
 }
-
-// NumPy's ordering of doubles in searchsorted (NaN sorts last): npy_sort.h DOUBLE_LT
-__device__ __forceinline__ bool np_lt(double a, double b) { return a < b || (b != b && a == a); }
 
 // one sweep of the bracket recurrence (see the header of this file); prev == nullptr: every key over [0, n)
 __global__ void __launch_bounds__(256) k_bisect_sweep(i64 n, const double *__restrict__ arr, i64 m, const double *__restrict__ keys,

@@ -20,7 +20,7 @@ from .._dev import require_cuda, stream_ptr
 __all__ = ["systematic_resample", "stratified_resample", "multinomial_resample", "residual_resample",
            "gather_particles", "exact_cumsum", "ResamplePlan", "normalize_weights",
            "residual_resample_with_uniforms", "systematic_resample_bank", "stratified_resample_bank",
-           "gather_particles_bank", "BankResamplePlan"]
+           "gather_particles_bank", "BankResamplePlan", "multinomial_resample_bank", "residual_resample_bank"]
 
 
 class ResamplePlan(object):
@@ -321,7 +321,13 @@ class BankResamplePlan(object):
     so it can be captured in a CUDA graph.
 
     ``status`` (int32 CUDA tensor [n_sets]) is 1 for a set whose positions ran past its cumulative sum
-    (the reference's ``IndexError``, resampling.py:145; that row's indexes are unspecified), else 0."""
+    (the reference's ``IndexError``, resampling.py:145; that row's indexes are unspecified), else 0.
+
+    ``multinomial`` and ``residual`` run the reference's ``multinomial_resample`` / ``residual_resample``
+    per row for caller-supplied uniforms.  Their first call allocates the plan's workspace (n_sets *
+    n_particles doubles for the per-set cumulative sums), so make one call before capturing a graph.
+    After them ``status`` has bit 0 set where the reference raises (residual: k > M) and bit 1 (value 2)
+    where the set took NumPy's carried-bracket search because its cumulative sum is not sorted."""
 
     def __init__(self, n_sets, n_particles, device=None):
         self.n_sets = int(n_sets)
@@ -333,6 +339,72 @@ class BankResamplePlan(object):
         self.indexes = torch.empty((self.n_sets, self.n_particles), dtype=torch.int32, device=self.device)
         self.status = torch.zeros(self.n_sets, dtype=torch.int32, device=self.device)
         self._err = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self.n_copies = torch.zeros(self.n_sets, dtype=torch.int64, device=self.device)
+        self._ws = None
+        self._idx64 = None
+
+    def _workspace(self):
+        if self._ws is None:
+            nbytes = int(self._lib.bke_residual_resample_bank_workspace_bytes(self.n_sets, self.n_particles))
+            self._ws = torch.empty(max(nbytes // 8, 1), dtype=torch.float64, device=self.device)
+        return self._ws
+
+    def multinomial(self, weights, uniforms, out=None):
+        """indexes[b] = ``searchsorted(cumsum(weights[b]) with [-1] = 1, uniforms[b])`` (resampling.py:173-176),
+        int64 (B, M) like ``np.searchsorted``; ``uniforms`` float64 CUDA tensor [n_sets, M]."""
+        shape = (self.n_sets, self.n_particles)
+        _bank_tensor_check(weights, "weights", (torch.float64,), shape, self.device)
+        _bank_tensor_check(uniforms, "uniforms", (torch.float64,), shape, self.device)
+        if out is None:
+            if self._idx64 is None:
+                self._idx64 = torch.empty(shape, dtype=torch.int64, device=self.device)
+            out = self._idx64
+        _bank_tensor_check(out, "out", (torch.int64,), shape, self.device)
+        ws = self._workspace()
+        a = _lib.MultinomialResampleBankArgs()
+        a.n_sets, a.n_particles = self.n_sets, self.n_particles
+        a.weights, a.uniforms, a.indexes, a.status = (weights.data_ptr(), uniforms.data_ptr(), out.data_ptr(),
+                                                      self.status.data_ptr())
+        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel() * 8
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.bke_multinomial_resample_bank(ctypes.byref(a), stream_ptr(self.device)))
+        return out
+
+    def _residual_args(self, weights, uniforms, out):
+        out = self.indexes if out is None else out
+        _bank_tensor_check(out, "out", (torch.int32,), (self.n_sets, self.n_particles), self.device)
+        ws = self._workspace()
+        a = _lib.ResidualResampleBankArgs()
+        a.n_sets, a.n_particles = self.n_sets, self.n_particles
+        a.weights = weights.data_ptr() if weights is not None else None
+        a.uniforms = uniforms.data_ptr() if uniforms is not None else None
+        a.indexes, a.n_copies, a.status = out.data_ptr(), self.n_copies.data_ptr(), self.status.data_ptr()
+        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel() * 8
+        return a, out
+
+    def residual_prepare(self, weights, out=None):
+        """The deterministic part of residual_resample (resampling.py:52-72) for every row: ``out[b, :k_b]``
+        (default: ``indexes``), ``n_copies[b] = k_b`` and the per-set cumulative sums in the workspace."""
+        _bank_tensor_check(weights, "weights", (torch.float64,), (self.n_sets, self.n_particles), self.device)
+        a, out = self._residual_args(weights, None, out)
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.bke_residual_resample_bank_prepare(ctypes.byref(a), stream_ptr(self.device)))
+        return out
+
+    def residual_search(self, uniforms, out=None):
+        """``out[b, k_b:] = searchsorted(cumulative_sum_b, uniforms[b, :M - k_b])`` (resampling.py:74) after
+        ``residual_prepare`` on the same plan and ``out``; the rest of each row of ``uniforms`` is not read."""
+        _bank_tensor_check(uniforms, "uniforms", (torch.float64,), (self.n_sets, self.n_particles), self.device)
+        a, out = self._residual_args(None, uniforms, out)
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.bke_residual_resample_bank_search(ctypes.byref(a), stream_ptr(self.device)))
+        return out
+
+    def residual(self, weights, uniforms, out=None):
+        """residual_resample (resampling.py:27-76) of every row for caller-supplied uniforms: row b uses
+        ``uniforms[b, :M - k_b]``.  int32 (B, M); ``raise_if_overflow`` reports a row with k > M."""
+        out = self.residual_prepare(weights, out)
+        return self.residual_search(uniforms, out)
 
     def _run(self, weights, u, uniforms, out):
         shape = (self.n_sets, self.n_particles)
@@ -382,7 +454,7 @@ class BankResamplePlan(object):
 
 
 def _raise_first_overflow(status, n_particles):
-    bad = torch.nonzero(status).flatten()
+    bad = torch.nonzero(status & 1).flatten()
     if bad.numel():
         raise IndexError("set %d: index %d is out of bounds for axis 0 with size %d"
                          % (int(bad[0]), n_particles, n_particles))
@@ -419,6 +491,57 @@ def stratified_resample_bank(weights):
     """``stratified_resample`` (resampling.py:80-114) of every row of ``weights[B, M]`` in one launch
     (uniforms drawn as ``random((B, M))``); otherwise as ``systematic_resample_bank``."""
     return _run_bank(weights, True)
+
+
+def _bank_2d(weights):
+    is_torch, w, dev = _weights_on_device(weights)
+    if w.dim() != 2:
+        raise ValueError("weights must be 2-D (n_sets, n_particles); got shape %s" % (tuple(w.shape),))
+    B, M = w.shape
+    if B and not M:                                       # cumulative_sum[-1] = 1. of row 0, before any draw
+        raise IndexError("set 0: index -1 is out of bounds for axis 0 with size 0")
+    return is_torch, w, dev, B, M
+
+
+def multinomial_resample_bank(weights):
+    """``multinomial_resample`` (resampling.py:153-176) of every row of ``weights[B, M]``: int64 ``(B, M)``,
+    an ndarray for array input, a CUDA tensor for a CUDA tensor.  Draws ``random((B, M))``, the values and
+    stream position of a Python loop of the reference over the rows, and returns that loop's result bit
+    for bit, NumPy's bracket-carrying ``searchsorted`` included (csrc/resample_bank.cu)."""
+    is_torch, w, dev, B, M = _bank_2d(weights)
+    draw = random((B, M))
+    plan = BankResamplePlan(B, M, dev)
+    if B:
+        idx = plan.multinomial(w, torch.from_numpy(np.ascontiguousarray(draw)).to(dev))
+    else:
+        idx = torch.zeros((0, M), dtype=torch.int64, device=dev)
+    return idx if is_torch else idx.cpu().numpy()
+
+
+def residual_resample_bank(weights):
+    """``residual_resample`` (resampling.py:27-76) of every row of ``weights[B, M]``: int32 ``(B, M)``, ndarray
+    or CUDA tensor like the input.  The deterministic copies and cumulative sums run first on the GPU; the
+    copy counts k_b are then read back (one host synchronisation) to draw ``random(M - k_b)`` for every row
+    in row order as one draw, which are the values and the stream position of the reference's loop.  A row
+    with k_b > M raises ``IndexError`` naming it, after drawing only for the rows before it, as the loop
+    does."""
+    is_torch, w, dev, B, M = _bank_2d(weights)
+    if not B:
+        idx = torch.zeros((0, M), dtype=torch.int32, device=dev)
+        return idx if is_torch else idx.cpu().numpy()
+    plan = BankResamplePlan(B, M, dev)
+    plan.residual_prepare(w)
+    k = plan.n_copies.cpu().numpy()
+    bad = np.flatnonzero(k > M)
+    first = int(bad[0]) if bad.size else B
+    draw = random(int((M - k[:first]).sum()))
+    if first < B:                                         # indexes[k] = i runs off the end (:61)
+        raise IndexError("set %d: index %d is out of bounds for axis 0 with size %d" % (first, M, M))
+    U = torch.zeros((B, M), dtype=torch.float64, device=dev)
+    keep = torch.arange(M, device=dev)[None, :] < torch.from_numpy(M - k).to(dev)[:, None]
+    U[keep] = torch.from_numpy(np.ascontiguousarray(draw)).to(dev)     # row b's M - k_b draws, in row order
+    idx = plan.residual_search(U)
+    return idx if is_torch else idx.cpu().numpy()
 
 
 def _gather_bank(particles, indexes, out, err):

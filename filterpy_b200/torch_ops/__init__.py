@@ -15,6 +15,8 @@ The same symbols exposed as torch.ops.* via a C++ extension for zero-copy CUDA t
     idx  = torch.ops.bke.stratified_resample(weights, uniforms)    # resampling.py:80-114
     idx  = torch.ops.bke.systematic_resample_bank(weights, u)      # every row of weights[B, M], u[B]
     idx  = torch.ops.bke.stratified_resample_bank(weights, uniforms)   # uniforms[B, M]
+    idx  = torch.ops.bke.multinomial_resample_bank(weights, uniforms)  # int64, resampling.py:153-176 per row
+    idx  = torch.ops.bke.residual_resample_bank(weights, uniforms)     # row b uses uniforms[b, :M - k_b]
 
 Models are shared by the bank when 2-D (stride 0) and per filter when 3-D.  Only the CUDA backend is
 registered: CPU tensors raise ``NotImplementedError`` (no CPU fallback).  The operators run on the

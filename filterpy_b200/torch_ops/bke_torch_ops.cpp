@@ -12,6 +12,8 @@
 //   bke::stratified_resample  bke_stratified_resample  monte_carlo/resampling.py:80-114
 //   bke::systematic_resample_bank  bke_resample_bank   resampling.py:117-150 on every row of weights[B, M]
 //   bke::stratified_resample_bank  bke_resample_bank   resampling.py:80-114 on every row of weights[B, M]
+//   bke::multinomial_resample_bank bke_multinomial_resample_bank       resampling.py:153-176 per row
+//   bke::residual_resample_bank    bke_residual_resample_bank_prepare / _search   resampling.py:27-76 per row
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
@@ -287,6 +289,62 @@ at::Tensor resample_bank(const at::Tensor &w, const at::Tensor *u, const at::Ten
 at::Tensor systematic_resample_bank(const at::Tensor &w, const at::Tensor &u) { return resample_bank(w, &u, nullptr); }
 at::Tensor stratified_resample_bank(const at::Tensor &w, const at::Tensor &U) { return resample_bank(w, nullptr, &U); }
 
+void check_bank_uniforms(const at::Tensor &w, const at::Tensor &U)
+{
+    TORCH_CHECK(w.is_cuda() && w.is_contiguous() && w.scalar_type() == at::kDouble && w.dim() == 2, "bke: weights must be a contiguous 2-D float64 CUDA tensor");
+    TORCH_CHECK(U.is_cuda() && U.is_contiguous() && U.scalar_type() == at::kDouble && U.device() == w.device(), "bke: uniforms must be a contiguous float64 CUDA tensor on the weights' device");
+    TORCH_CHECK(U.dim() == 2 && U.size(0) == w.size(0) && U.size(1) == w.size(1), "bke: uniforms must be [n_sets, n_particles]");
+}
+
+// resampling.py:173-176 on every row for the caller's uniforms[B, M]: int64 indexes
+at::Tensor multinomial_resample_bank(const at::Tensor &w, const at::Tensor &U)
+{
+    check_bank_uniforms(w, U);
+    c10::cuda::CUDAGuard guard(w.device());
+    const int64_t B = w.size(0), M = w.size(1);
+    TORCH_CHECK_INDEX(B == 0 || M > 0, "set 0: index -1 is out of bounds for axis 0 with size 0");
+    at::Tensor idx = at::empty({B, M}, w.options().dtype(at::kLong));
+    if (B == 0) return idx;
+    at::Tensor status = at::empty({B}, w.options().dtype(at::kInt));
+    const size_t wsb = bke_multinomial_resample_bank_workspace_bytes(B, M);
+    at::Tensor ws = at::empty({(int64_t)(wsb / 8)}, w.options());
+    bke_multinomial_resample_bank_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_sets = B; a.n_particles = M; a.weights = (const double *)w.data_ptr(); a.uniforms = (const double *)U.data_ptr();
+    a.indexes = (int64_t *)idx.data_ptr(); a.status = (int32_t *)status.data_ptr();
+    a.workspace = ws.data_ptr(); a.workspace_bytes = wsb;
+    check_rc(bke_multinomial_resample_bank(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_multinomial_resample_bank");
+    return idx;
+}
+
+// resampling.py:27-76 on every row; row b uses uniforms[b, :M - k_b]: int32 indexes
+at::Tensor residual_resample_bank(const at::Tensor &w, const at::Tensor &U)
+{
+    check_bank_uniforms(w, U);
+    c10::cuda::CUDAGuard guard(w.device());
+    const int64_t B = w.size(0), M = w.size(1);
+    TORCH_CHECK_INDEX(B == 0 || M > 0, "set 0: index -1 is out of bounds for axis 0 with size 0");
+    at::Tensor idx = at::zeros({B, M}, w.options().dtype(at::kInt));
+    if (B == 0) return idx;
+    at::Tensor status = at::empty({B}, w.options().dtype(at::kInt));
+    at::Tensor k = at::empty({B}, w.options().dtype(at::kLong));
+    const size_t wsb = bke_residual_resample_bank_workspace_bytes(B, M);
+    at::Tensor ws = at::empty({(int64_t)(wsb / 8)}, w.options());
+    bke_residual_resample_bank_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_sets = B; a.n_particles = M; a.weights = (const double *)w.data_ptr(); a.uniforms = (const double *)U.data_ptr();
+    a.indexes = (int32_t *)idx.data_ptr(); a.n_copies = (int64_t *)k.data_ptr(); a.status = (int32_t *)status.data_ptr();
+    a.workspace = ws.data_ptr(); a.workspace_bytes = wsb;
+    void *st = (void *)c10::cuda::getCurrentCUDAStream().stream();
+    check_rc(bke_residual_resample_bank_prepare(&a, st), "bke_residual_resample_bank_prepare");
+    check_rc(bke_residual_resample_bank_search(&a, st), "bke_residual_resample_bank_search");
+    // resampling.py:61: the first row with k > M is where the reference loop raises
+    const at::Tensor bad = status.bitwise_and(1).nonzero();
+    TORCH_CHECK_INDEX(bad.numel() == 0, "set ", bad.numel() ? bad[0][0].item<int64_t>() : 0, ": index ", M,
+                      " is out of bounds for axis 0 with size ", M);
+    return idx;
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bke, m)
@@ -305,6 +363,8 @@ TORCH_LIBRARY(bke, m)
     m.def("stratified_resample(Tensor weights, Tensor uniforms) -> Tensor");
     m.def("systematic_resample_bank(Tensor weights, Tensor u) -> Tensor");
     m.def("stratified_resample_bank(Tensor weights, Tensor uniforms) -> Tensor");
+    m.def("multinomial_resample_bank(Tensor weights, Tensor uniforms) -> Tensor");
+    m.def("residual_resample_bank(Tensor weights, Tensor uniforms) -> Tensor");
 }
 
 TORCH_LIBRARY_IMPL(bke, CUDA, m)
@@ -320,4 +380,6 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("stratified_resample", &stratified_resample);
     m.impl("systematic_resample_bank", &systematic_resample_bank);
     m.impl("stratified_resample_bank", &stratified_resample_bank);
+    m.impl("multinomial_resample_bank", &multinomial_resample_bank);
+    m.impl("residual_resample_bank", &residual_resample_bank);
 }

@@ -684,6 +684,55 @@ typedef struct bke_resample_bank_args {
 
 int bke_resample_bank(const bke_resample_bank_args *args, void *stream);
 
+/* multinomial_resample (resampling.py:153-176) of every row of weights[n_sets, n_particles] (fp64, dense):
+ *   indexes[b] = np.searchsorted(c_b, uniforms[b]),  c_b = np.cumsum(weights[b]), c_b[-1] = 1
+ * bit for bit for ANY values (negative, NaN, infinite, -0.0 and subnormal weights; uniforms outside [0, 1),
+ * NaN or out of order), NumPy's bracket-carrying bisection included.  indexes are int64 like
+ * np.searchsorted's.  status[b] = 0 where every key was bisected on its own (c_b is sorted), 2 where the set
+ * took the carried-bracket search; bit 0 is never set (multinomial cannot fail once n_particles > 0).
+ * workspace: bke_multinomial_resample_bank_workspace_bytes(n_sets, n_particles) bytes, 8-byte aligned (it
+ * holds c).  n_sets = 0 or n_particles = 0 does nothing; n_particles < 2^31.  No allocation, no host sync:
+ * the call can be captured in a CUDA graph. */
+typedef struct bke_multinomial_resample_bank_args {
+    int64_t n_sets, n_particles;
+    const double *weights;       /* [n_sets, n_particles] */
+    const double *uniforms;      /* [n_sets, n_particles] */
+    int64_t *indexes;            /* [n_sets, n_particles] */
+    int32_t *status;             /* [n_sets] */
+    void *workspace;
+    size_t workspace_bytes;
+} bke_multinomial_resample_bank_args;
+
+size_t bke_multinomial_resample_bank_workspace_bytes(int64_t n_sets, int64_t n_particles);
+int bke_multinomial_resample_bank(const bke_multinomial_resample_bank_args *args, void *stream);
+
+/* residual_resample (resampling.py:27-76) of every row of weights[n_sets, n_particles], in two stream-ordered
+ * calls on the same args, bit for bit for ANY weights (the sums in the reference's order, NumPy's
+ * bracket-carrying bisection over the non-monotone cumulative sum):
+ *   _prepare  reads weights; writes indexes[b, :k_b] = repeat(arange(M), max(floor(M w), 0)), n_copies[b] =
+ *             k_b, cumsum(residual / sum(residual)) with [-1] = 1 into the workspace, and status[b]: 1 where
+ *             k_b > M (the reference's IndexError, :61; that row's indexes are unspecified and n_copies[b] is
+ *             some value > M), else 0 or 2 (2: the set takes the carried-bracket search, the usual case).
+ *   _search   reads uniforms[b, :M - k_b] (the reference's random(M - k_b); the rest of the row is not
+ *             read), n_copies, status and the workspace; writes indexes[b, k_b:] (int32); skips status-1 rows.
+ * workspace: bke_residual_resample_bank_workspace_bytes(n_sets, n_particles) bytes, 8-byte aligned.  The
+ * caller can read n_copies between the calls to draw exactly M - k_b uniforms per row.  n_sets = 0 or
+ * n_particles = 0 does nothing; n_particles < 2^31.  No allocation, no host sync: graph-capturable. */
+typedef struct bke_residual_resample_bank_args {
+    int64_t n_sets, n_particles;
+    const double *weights;       /* [n_sets, n_particles] (_prepare) */
+    const double *uniforms;      /* [n_sets, n_particles] (_search) */
+    int32_t *indexes;            /* [n_sets, n_particles] */
+    int64_t *n_copies;           /* [n_sets]: k_b */
+    int32_t *status;             /* [n_sets] */
+    void *workspace;
+    size_t workspace_bytes;
+} bke_residual_resample_bank_args;
+
+size_t bke_residual_resample_bank_workspace_bytes(int64_t n_sets, int64_t n_particles);
+int bke_residual_resample_bank_prepare(const bke_residual_resample_bank_args *args, void *stream);
+int bke_residual_resample_bank_search(const bke_residual_resample_bank_args *args, void *stream);
+
 /* sum of weights (fp64, deterministic tree order) — the quantity that is all-reduced across
  * GPUs before a distributed resample; also used to normalise: weights_out[i] = weights[i] / sum
  * (IEEE division, the same elementwise operation as NumPy's `w / w.sum()` given that sum). */
