@@ -15,6 +15,7 @@ BKE_OK, BKE_ERR_BAD_ARG, BKE_ERR_UNSUPPORTED, BKE_ERR_CUDA = 0, 1, 2, 3
 BKE_STATUS_OK, BKE_STATUS_SINGULAR_S, BKE_STATUS_NOT_PD = 0, 1, 2
 BKE_DO_PREDICT, BKE_DO_UPDATE, BKE_UPDATE_FIRST = 1, 2, 4
 BKE_REVERSE_TILES = 16
+BKE_UKF_SIMPLEX = 32             # bke_ukf_args.flags / bke_ukf_rts_args.flags: SimplexSigmaPoints
 BKE_FX_LINEAR, BKE_FX_CONST_VEL = 0, 1
 BKE_HX_LINEAR, BKE_HX_RANGE_AZ_EL, BKE_HX_RANGE_BEARING = 0, 1, 2
 BKE_FX_USER = BKE_HX_USER = 100
@@ -32,7 +33,8 @@ EXPORTED_SYMBOLS = [
     "bke_resample_workspace_bytes", "bke_systematic_resample", "bke_stratified_resample",
     "bke_weights_sum", "bke_weights_scale", "bke_resample_shard", "bke_resample_normalized",
     "bke_resample_composite_bytes", "bke_resample_shard_compose", "bke_resample_compose_carry", "bke_resample_shard_stage",
-    "bke_merwe_sigma_points", "bke_unscented_transform",
+    "bke_merwe_sigma_points", "bke_simplex_sigma_points", "bke_unscented_transform",
+    "bke_ukf_model_compile_points", "bke_debug_ukf_model_points_cubin_bytes",
     "bke_ukf_model_compile", "bke_ukf_model_log", "bke_ukf_model_registers", "bke_ukf_model_free", "bke_ukf_step_model",
     "bke_debug_ukf_model_cubin_bytes", "bke_ukf_rts_smoother_model",
     "bke_ckf_step", "bke_ckf_model_compile", "bke_ckf_step_model", "bke_debug_ckf_model_cubin_bytes",
@@ -263,7 +265,7 @@ class RtsArgs(ctypes.Structure):
 class UkfRtsArgs(ctypes.Structure):
     _fields_ = [
         ("n_filters", c_int64), ("n_steps", c_int64),
-        ("dim_x", c_int32), ("dtype", c_int32), ("fx_model", c_int32), ("reserved", c_int32),
+        ("dim_x", c_int32), ("dtype", c_int32), ("fx_model", c_int32), ("flags", c_uint32),
         ("alpha", c_double), ("beta", c_double), ("kappa", c_double), ("dt", c_double),
         ("dts", c_void_p),
         ("Xs", c_void_p), ("Ps", c_void_p),
@@ -391,6 +393,12 @@ def load():
     lib.bke_ukf_rts_smoother_model.restype = ctypes.c_int
     lib.bke_debug_ukf_model_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p]
     lib.bke_debug_ukf_model_cubin_bytes.restype = c_size_t
+    lib.bke_ukf_model_compile_points.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_uint32, c_uint32,
+                                                 ctypes.c_char_p, ctypes.c_char_p, ctypes.POINTER(c_void_p)]
+    lib.bke_ukf_model_compile_points.restype = ctypes.c_int
+    lib.bke_debug_ukf_model_points_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_uint32, c_uint32,
+                                                           ctypes.c_char_p, ctypes.c_char_p]
+    lib.bke_debug_ukf_model_points_cubin_bytes.restype = c_size_t
     for fam in ("ukf", "ckf"):
         f = getattr(lib, "bke_%s_model_compile_hooks" % fam)
         f.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_uint32, ctypes.c_char_p, ctypes.c_char_p,
@@ -452,6 +460,8 @@ def load():
     lib.bke_merwe_sigma_points.argtypes = [c_int64, c_int32, c_int32, c_double, c_double, c_double,
                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.bke_merwe_sigma_points.restype = ctypes.c_int
+    lib.bke_simplex_sigma_points.argtypes = [c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.bke_simplex_sigma_points.restype = ctypes.c_int
     lib.bke_unscented_transform.argtypes = [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
     lib.bke_unscented_transform.restype = ctypes.c_int

@@ -347,7 +347,7 @@ int bke_ukf_step(const bke_ukf_args *args, void *stream)
         set_error("unknown fx/hx model id"); return BKE_ERR_BAD_ARG;
     }
     double lam_n = a.alpha * a.alpha * (a.dim_x + a.kappa);
-    if (!(lam_n != 0.0)) { set_error("alpha^2 (n + kappa) must be non-zero"); return BKE_ERR_BAD_ARG; }
+    if (!(a.flags & BKE_UKF_SIMPLEX) && !(lam_n != 0.0)) { set_error("alpha^2 (n + kappa) must be non-zero"); return BKE_ERR_BAD_ARG; }
     int rc = require_device();
     if (rc) return rc;
     if (a.n_filters == 0) return BKE_OK;

@@ -1,19 +1,25 @@
 // ukf.cu — host side of the unscented Kalman filter bank: the closed set of pre-built (dim_x, dim_z,
-// fx, hx) instances of the kernel in ukf_kernel.cuh and their launch.  (Instances around user-supplied
-// fx / hx are compiled at run time: ukf_rtc.cu.)
+// fx, hx) instances of the kernel in ukf_kernel.cuh and their launch (Merwe points here, the simplex set
+// in ukf_simplex.cu).  (Instances around user-supplied fx / hx are compiled at run time: ukf_rtc.cu.)
 #include "ukf_kernel.cuh"
 #include "ukf_launch.cuh"
 
 namespace bke {
+
+// the simplex instances of the same (dim_x, dim_z, fx, hx) set (ukf_simplex.cu)
+template <typename T, int N, int M, int FX, int HX>
+int launch_ukf_simplex(const bke_ukf_args &a, cudaStream_t s);
+
 namespace {
 using namespace ukfk;
 
 template <typename T, int N, int M, int FX, int HX>
 int launch_inst(const bke_ukf_args &a, cudaStream_t s)
 {
+    if (a.flags & BKE_UKF_SIMPLEX) return launch_ukf_simplex<T, N, M, FX, HX>(a, s);      // ukf_simplex.cu
     UkfP<T> p;
     ukf_fill_params<T>(a, N, p);
-    const size_t smem = ukf_smem_bytes<T>(N, M, FX == BKE_FX_LINEAR, a.F_stride == 0, HX == BKE_HX_LINEAR, a.H_stride == 0);
+    const size_t smem = ukf_smem_bytes<T>(N, M, 2 * N + 1, FX == BKE_FX_LINEAR, a.F_stride == 0, HX == BKE_HX_LINEAR, a.H_stride == 0);
     constexpr int OCC = ukf_occupancy(N, sizeof(T) == 8);
     const bool ex = a.x_prior || a.P_prior || a.K || a.y || a.S || a.SI || a.log_likelihood;
     auto kern = ex ? ukf_kernel<T, N, M, FX, HX, OCC, true> : ukf_kernel<T, N, M, FX, HX, OCC, false>;

@@ -68,9 +68,9 @@ template <typename T> __device__ void bke_hook_state_add(const T *a, const T *b,
 template <int S> struct IntC { static constexpr int value = S; };
 
 // upper Cholesky factor of A (upper triangle of A is read, like scipy.linalg.cholesky):
-// U'U = A, U upper triangular.  Returns false if A is not positive definite.
-template <typename T, int N>
-__device__ __forceinline__ bool chol_upper(const T (&A)[N][N], T (&U)[N][N])
+// U'U = A, U upper triangular (rows N.. of a taller U are left alone).  Returns false if A is not positive definite.
+template <typename T, int N, int NR = N>
+__device__ __forceinline__ bool chol_upper(const T (&A)[N][N], T (&U)[NR][N])
 {
     bool ok = true;
 #pragma unroll
@@ -110,6 +110,60 @@ __device__ __forceinline__ void sigma_point(const T (&x)[N], const T (&U)[N][N],
         constexpr int k = S - 1 - N;
 #pragma unroll
         for (int i = 0; i < N; i++) sp[i] = (i >= k) ? x[i] - U[k][i] : x[i];
+    }
+}
+
+// SimplexSigmaPoints (sigma_points.py:499-513): U = chol_upper(P) unscaled, Xi_j = x + D_j with
+// D = (U' sqrt(n) Istar)'.  In closed form, with c_d = sqrt(n / (lambda d (d+1))) = sqrt((n+1) / (d (d+1)))
+// and the suffix sums S_j = sum_{k >= j} c_{k+1} U[k,:]:
+//     D_0 = -c_1 U[0,:] + S_1,   D_1 = c_1 U[0,:] + S_1,   D_j = -j c_j U[j-1,:] + S_j  (j >= 2).
+// D_j (j >= 1) is zero left of column j-1, like row j-1 of U, and overwrites that row (j = n down to 1,
+// with a running S); D_0 is dense and goes to the extra row U[n].  No simplex point equals x.
+template <typename T>
+__device__ __forceinline__ T simplex_coef(int n, int d)
+{
+    return T(sqrt(double(n + 1) / double(d * (d + 1))));
+}
+
+template <typename T, int N>
+__device__ __forceinline__ void simplex_offsets(T (&U)[N + 1][N])
+{
+    T S[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) S[i] = T(0);
+#pragma unroll
+    for (int j = N; j >= 2; j--) {
+        const T c = simplex_coef<T>(N, j);
+#pragma unroll
+        for (int i = j - 1; i < N; i++) {
+            const T u = U[j - 1][i];
+            U[j - 1][i] = T(-j) * c * u + S[i];
+            S[i] += c * u;
+        }
+    }
+    const T c1 = simplex_coef<T>(N, 1);
+#pragma unroll
+    for (int i = 0; i < N; i++) {
+        const T u = U[0][i];
+        U[N][i] = S[i] - c1 * u;
+        U[0][i] = S[i] + c1 * u;
+    }
+}
+
+// sigma point S of the point set: Merwe's (U is [N][N]), or x + D_S of the simplex set (U is [N+1][N]: D_S in
+// row S-1, D_0 in row N)
+template <typename T, int N, int S, int NR>
+__device__ __forceinline__ void point(const T (&x)[N], const T (&U)[NR][N], T (&sp)[N])
+{
+    if constexpr (NR == N) {
+        sigma_point<T, N, S>(x, U, sp);
+    } else if constexpr (S == 0) {
+#pragma unroll
+        for (int i = 0; i < N; i++) sp[i] = x[i] + U[N][i];
+    } else {
+        constexpr int k = S - 1;
+#pragma unroll
+        for (int i = 0; i < N; i++) sp[i] = (i >= k) ? x[i] + U[k][i] : x[i];
     }
 }
 
@@ -287,12 +341,13 @@ __device__ __forceinline__ void slab_store(T *g, const T *slab, int cnt)
 }
 
 // UKF_EXTRAS: the optional outputs (priors, K, y, S, SI, log-likelihood) are compiled in; the plain
-// instantiation is 2-4 % faster without their tests and live ranges
-template <typename T, int N, int M, int FX, int HX, int OCC, bool UKF_EXTRAS>
+// instantiation is 2-4 % faster without their tests and live ranges.
+// SPX: the simplex point set (n + 1 points, p.scale = 1, every weight 1/(n+1)) instead of Merwe's.
+template <typename T, int N, int M, int FX, int HX, int OCC, bool UKF_EXTRAS, bool SPX = false>
 __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    constexpr int NS = 2 * N + 1;
+    constexpr int NS = SPX ? N + 1 : 2 * N + 1;
     constexpr int PADP = (N * N) | 1;                        // odd per-filter stride of the P / Q slab
     constexpr int NT = N * (N + 1) / 2;
     constexpr int SLAB = (NS * M + NT > PADP ? NS * M + NT : PADP) * UB;
@@ -345,7 +400,7 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
     if (q_dense) slab_load<T, N * N, PADP>(zs, p.Q + tile0 * N * N, cnt);     // parked until the end of predict
     __syncthreads();
     int st = BKE_STATUS_OK;
-    T U[N][N];
+    T U[SPX ? N + 1 : N][N];                                 // the simplex set keeps its offset D_0 in row N
 
     if (do_p) {
         T A[N][N];
@@ -354,6 +409,7 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
 #pragma unroll
             for (int j = 0; j < N; j++) A[i][j] = p.scale * P[i][j];
         if (!chol_upper<T, N>(A, U)) st = BKE_STATUS_NOT_PD;
+        if constexpr (SPX) simplex_offsets<T, N>(U);
         // pass 1: mean of the propagated points
         T xm[N];
 #pragma unroll
@@ -365,7 +421,7 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
             for_sigma<0, NS>([&](auto sc) {
                 constexpr int S = decltype(sc)::value;
                 T sp[N];
-                sigma_point<T, N, S>(x, U, sp);
+                point<T, N, S>(x, U, sp);
                 apply_fx<T, N, FX>(sp, sf[S], p.dt, Fp, fstride, fxa);
                 Wm[S] = (S == 0) ? p.wm0 : p.wi;
             });
@@ -374,7 +430,7 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
             for_sigma<0, NS>([&](auto sc) {
                 constexpr int S = decltype(sc)::value;
                 T sp[N], fs[N];
-                sigma_point<T, N, S>(x, U, sp);
+                point<T, N, S>(x, U, sp);
                 apply_fx<T, N, FX>(sp, fs, p.dt, Fp, fstride, fxa);
                 const T w = (S == 0) ? p.wm0 : p.wi;
 #pragma unroll
@@ -394,7 +450,7 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
 #pragma unroll
                 for (int i = 0; i < N; i++) fs[i] = sf[S][i];
             } else {
-                sigma_point<T, N, S>(x, U, sp);
+                point<T, N, S>(x, U, sp);
                 apply_fx<T, N, FX>(sp, fs, p.dt, Fp, fstride, fxa);
             }
             const T w = (S == 0) ? p.wc0 : p.wi;
@@ -439,6 +495,7 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
 #pragma unroll
                     for (int j = i; j < N; j++) A[i][j] = p.scale * P[i][j];
                 if (!chol_upper<T, N>(A, U)) st = BKE_STATUS_NOT_PD;
+                if constexpr (SPX) simplex_offsets<T, N>(U);
             }
             // P is not needed again until the posterior: park its upper triangle in shared memory and
             // free the registers.  A (never expected) non-symmetric P keeps its lower triangle in P_out.
@@ -463,12 +520,44 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
                 for_sigma<0, NS>([&](auto sc) {
                     constexpr int S = decltype(sc)::value;
                     T sp[N], h[M];
-                    sigma_point<T, N, S>(x, U, sp);
+                    point<T, N, S>(x, U, sp);
                     apply_hx<T, N, M, HX>(sp, h, Hp, hstride, hxa);
                     const T w = (S == 0) ? p.wm0 : p.wi;
 #pragma unroll
                     for (int a = 0; a < M; a++) { zm[a] += w * h[a]; zs[(S * M + a) * UB + tid] = h[a]; }
                 });
+            } else if constexpr (SPX) {
+                // The transcendental models on the simplex set: as below, the positions are parked and a
+                // run-time loop evaluates hx in place, but no point equals x, so hx(x) (weight 0) is the
+                // reference direction of the relative angles.  D_j with j - 1 past the last position
+                // component leaves the positions of x unchanged: that point's hx is hx(x).
+                for_sigma<0, NS>([&](auto sc) {
+                    constexpr int S = decltype(sc)::value;
+                    T sp[N];
+                    point<T, N, S>(x, U, sp);
+#pragma unroll
+                    for (int a = 0; a < M; a++) zs[(S * M + a) * UB + tid] = sp[2 * a];
+                });
+                T h0[M], pos0[M];
+#pragma unroll
+                for (int a = 0; a < M; a++) pos0[a] = x[2 * a];
+                hx_positions<T, M, HX>(pos0, h0);
+                const T rho0 = sqrt(pos0[0] * pos0[0] + pos0[1] * pos0[1]);
+#pragma unroll 1
+                for (int s = 0; s < NS; s++) {
+                    T h[M];
+                    if (s >= 2 && hx_ignores_row<HX, N>(s - 1)) {
+#pragma unroll
+                        for (int a = 0; a < M; a++) h[a] = h0[a];
+                    } else {
+                        T pa[M];
+#pragma unroll
+                        for (int a = 0; a < M; a++) pa[a] = zs[(s * M + a) * UB + tid];
+                        hx_positions_rel<T, M, HX>(pa, pos0, rho0, h0, h);
+                    }
+#pragma unroll
+                    for (int a = 0; a < M; a++) { zm[a] += p.wi * h[a]; zs[(s * M + a) * UB + tid] = h[a]; }
+                }
             } else {
                 // Transcendental measurement models: the inputs hx reads (M position components per
                 // sigma point) are parked in the slab first, then a run-time loop over the n offset
@@ -566,11 +655,20 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
                 if constexpr (HOOKS & BKE_HOOK_RESIDUAL_X) {
                     // dx = residual_x(sigma, x) (UKF.py:501): the point itself, not the offset row
                     T sp[N], dx[N];
-                    sigma_point<T, N, S>(x, U, sp);
+                    point<T, N, S>(x, U, sp);
                     bke_hook_residual_x<T>(sp, x, dx);
 #pragma unroll
                     for (int i = 0; i < N; i++) {
                         T wd = w * dx[i];
+#pragma unroll
+                        for (int a = 0; a < M; a++) Pxz[i][a] += wd * dz[a];
+                    }
+                } else if constexpr (SPX) {
+                    // dx = sigma - x = D_S: row N of U, or row S-1 (zero left of column S-1)
+                    constexpr int k = S == 0 ? 0 : S - 1, row = S == 0 ? N : S - 1;
+#pragma unroll
+                    for (int i = k; i < N; i++) {
+                        T wd = w * U[row][i];
 #pragma unroll
                         for (int a = 0; a < M; a++) Pxz[i][a] += wd * dz[a];
                     }

@@ -39,6 +39,7 @@ struct bke_ukf_model {
     cudaKernel_t kern[2];          // [0] plain, [1] with the optional outputs
     cudaKernel_t kern_rts;         // RTS smoother around the user's fx or hooks (NULL: neither, or dim_x > UR_MAXN)
     unsigned hooks;                // BKE_HOOK_* mask the program was compiled with
+    bool simplex;                  // UKF: compiled for the simplex point set (BKE_UKF_SIMPLEX)
     int regs[2];
     std::string log;
 };
@@ -95,8 +96,8 @@ std::string kernel_name(const bke_ukf_model &m, int occ, bool extras)
                  extras ? "true" : "false");
         return buf;
     }
-    snprintf(buf, sizeof buf, "%s<real, %d, %d, %d, %d, %d, %s>", m.family == BKE_FAMILY_CKF ? "bke::ckfk::ckf_kernel" : "bke::ukfk::ukf_kernel",
-             m.n, m.m, m.fx_model, m.hx_model, occ, extras ? "true" : "false");
+    snprintf(buf, sizeof buf, "%s<real, %d, %d, %d, %d, %d, %s%s>", m.family == BKE_FAMILY_CKF ? "bke::ckfk::ckf_kernel" : "bke::ukfk::ukf_kernel",
+             m.n, m.m, m.fx_model, m.hx_model, occ, extras ? "true" : "false", m.simplex ? ", true" : "");
     return buf;
 }
 
@@ -108,7 +109,8 @@ int launch_model(const bke_ukf_args &a, const bke_ukf_model &m, const void *fx_a
     ukf_fill_params<T>(a, m.n, p);
     p.fx_args = (const T *)fx_args; p.s_fx_args = s_fx;
     p.hx_args = (const T *)hx_args; p.s_hx_args = s_hx;
-    const size_t smem = ukf_smem_bytes<T>(m.n, m.m, m.fx_model == BKE_FX_LINEAR, a.F_stride == 0, m.hx_model == BKE_HX_LINEAR, a.H_stride == 0);
+    const size_t smem = ukf_smem_bytes<T>(m.n, m.m, m.simplex ? m.n + 1 : 2 * m.n + 1, m.fx_model == BKE_FX_LINEAR, a.F_stride == 0,
+                                          m.hx_model == BKE_HX_LINEAR, a.H_stride == 0);
     const bool ex = a.x_prior || a.P_prior || a.K || a.y || a.S || a.SI || a.log_likelihood;
     const void *kern = (const void *)m.kern[ex ? 1 : 0];
     if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
@@ -162,10 +164,12 @@ extern "C" {
 // + the lowered names of the kernel instances of the family (the step with / without the optional outputs
 // and, for a UKF around a user fx or hooks, the RTS smoother)
 static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, unsigned hooks,
-                         const char *source, const char *include_dirs, std::vector<char> &cubin, std::string (&lowered)[3], std::string &log)
+                         bool simplex, const char *source, const char *include_dirs, std::vector<char> &cubin, std::string (&lowered)[3],
+                         std::string &log)
 {
     const bool ckf = family == BKE_FAMILY_CKF, enkf = family == BKE_FAMILY_ENKF;
-    const char *fn = hooks ? (ckf ? "bke_ckf_model_compile_hooks" : "bke_ukf_model_compile_hooks")
+    const char *fn = simplex ? "bke_ukf_model_compile_points"
+                   : hooks ? (ckf ? "bke_ckf_model_compile_hooks" : "bke_ukf_model_compile_hooks")
                            : enkf ? "bke_enkf_model_compile" : ckf ? "bke_ckf_model_compile" : "bke_ukf_model_compile";
     if (dim_x < 1 || dim_x > 16 || dim_z < 1 || dim_z > dim_x + 8) { set_error("%s: 1 <= dim_x <= 16, 1 <= dim_z", fn); return BKE_ERR_BAD_ARG; }
     if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
@@ -200,8 +204,11 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     std::string text;
     text += dtype == BKE_F64 ? "typedef double real;\n" : "typedef float real;\n";
     text += "#define BKE_DIM_X " + std::to_string(dim_x) + "\n#define BKE_DIM_Z " + std::to_string(dim_z) + "\n";
-    if (hooks)       // the hook-free text stays byte-identical
-        text += "#define BKE_UKF_HOOKS " + std::to_string(hooks) + "u\n#define BKE_N_SIGMAS " + std::to_string(ckf ? 2 * dim_x : 2 * dim_x + 1) + "\n";
+    // the text of a Merwe model without hooks defines neither; with hooks both, in this order
+    if (hooks)
+        text += "#define BKE_UKF_HOOKS " + std::to_string(hooks) + "u\n";
+    if (hooks || simplex)
+        text += "#define BKE_N_SIGMAS " + std::to_string(ckf ? 2 * dim_x : simplex ? dim_x + 1 : 2 * dim_x + 1) + "\n";
     text += enkf ? "#include \"enkf_kernel.cuh\"\n" : ckf ? "#include \"ckf_kernel.cuh\"\n" : "#include \"ukf_kernel.cuh\"\n#include \"ukf_rts_kernel.cuh\"\n";
     text += "#line 1 \"user_model.cu\"\n";
     text += source;
@@ -215,9 +222,10 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     if (hooks & BKE_HOOK_STATE_ADD) text += "template <> __device__ __forceinline__ void bke_hook_state_add<real>(const real *a, const real *b, real *o) { ::state_add(a, b, o); }\n";
     text += "} }\n";
 
-    const int occ = enkf ? 0 : ckf ? ckf_occupancy(dim_x, dtype == BKE_F64) : ukf_occupancy(dim_x, dtype == BKE_F64);
+    const int occ = enkf ? 0 : ckf ? ckf_occupancy(dim_x, dtype == BKE_F64)
+                                   : ukf_occupancy(dim_x, dtype == BKE_F64, simplex, hx_model == BKE_HX_RANGE_AZ_EL || hx_model == BKE_HX_RANGE_BEARING);
     bke_ukf_model tmp;
-    tmp.family = family; tmp.n = dim_x; tmp.m = dim_z; tmp.fx_model = fx_model; tmp.hx_model = hx_model;
+    tmp.family = family; tmp.n = dim_x; tmp.m = dim_z; tmp.fx_model = fx_model; tmp.hx_model = hx_model; tmp.simplex = simplex;
     nvrtcProgram prog;
     nvrtcResult r = rt->create(&prog, text.c_str(), enkf ? "bke_enkf_user.cu" : ckf ? "bke_ckf_user.cu" : "bke_ukf_user.cu", 0, nullptr, nullptr);
     if (r != NVRTC_SUCCESS) { set_error("nvrtcCreateProgram: %s", rt->errstr(r)); return BKE_ERR_CUDA; }
@@ -238,7 +246,7 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     const bool with_rts = !ckf && !enkf && (ufx || hooks) && dim_x <= UR_MAXN;
     const int n_names = with_rts ? 3 : 2;
     const std::string names[3] = {kernel_name(tmp, occ, false), kernel_name(tmp, occ, true),
-                                  ufx ? "bke::ukf_rts_kernel<real, true>" : "bke::ukf_rts_kernel<real, false>"};
+                                  std::string("bke::ukf_rts_kernel<real, ") + (ufx ? "true" : "false") + (simplex ? ", true>" : ">")};
     for (int i = 0; i < n_names; i++) rt->add_name(prog, names[i].c_str());
     r = rt->compile(prog, (int)copts.size(), copts.data());
     size_t lsz = 0;
@@ -269,17 +277,18 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
 }
 
 static int model_compile(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, unsigned hooks,
-                         const char *source, const char *include_dirs, bke_ukf_model **out)
+                         const char *source, const char *include_dirs, bke_ukf_model **out, bool simplex = false)
 {
     if (!out) { set_error("out is NULL"); return BKE_ERR_BAD_ARG; }
     *out = nullptr;
     std::vector<char> cubin;
     std::string lowered[3], log;
-    int rc = compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs, cubin, lowered, log);
+    int rc = compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, hooks, simplex, source, include_dirs, cubin, lowered, log);
     if (rc != BKE_OK) return rc;
     bke_ukf_model *m = new bke_ukf_model();
     m->family = family; m->n = dim_x; m->m = dim_z; m->dtype = dtype; m->fx_model = fx_model; m->hx_model = hx_model; m->lib = nullptr; m->log = log;
     m->hooks = hooks;
+    m->simplex = simplex;
     m->kern_rts = nullptr;
     if (check_cuda(cudaLibraryLoadData(&m->lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0), "cudaLibraryLoadData")) { delete m; return BKE_ERR_CUDA; }
     for (int i = 0; i < 2; i++) {
@@ -303,6 +312,22 @@ int bke_ukf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t f
                           const char *include_dirs, bke_ukf_model **out)
 {
     return model_compile(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, 0u, source, include_dirs, out);
+}
+
+// the point set of a UKF model: 0 (MerweScaledSigmaPoints, as bke_ukf_model_compile[_hooks]) or BKE_UKF_SIMPLEX
+static int check_points(uint32_t points)
+{
+    if (points != 0u && points != BKE_UKF_SIMPLEX) { set_error("bke_ukf_model_compile_points: points must be 0 or BKE_UKF_SIMPLEX"); return BKE_ERR_BAD_ARG; }
+    return BKE_OK;
+}
+
+int bke_ukf_model_compile_points(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, uint32_t hooks,
+                                 uint32_t points, const char *source, const char *include_dirs, bke_ukf_model **out)
+{
+    if (out) *out = nullptr;
+    const int rc = check_points(points);
+    if (rc) return rc;
+    return model_compile(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs, out, points != 0u);
 }
 
 int bke_enkf_model_compile(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, const char *source,
@@ -331,11 +356,11 @@ int bke_ckf_model_compile_hooks(int32_t dim_x, int32_t dim_z, int32_t dtype, int
 
 // the NVRTC half alone (CPU-only check that a model's text compiles for sm_90a): cubin size or 0
 static size_t cubin_bytes(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, unsigned hooks,
-                          const char *source, const char *include_dirs)
+                          const char *source, const char *include_dirs, bool simplex = false)
 {
     std::vector<char> cubin;
     std::string lowered[3], log;
-    if (compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs, cubin, lowered, log) != BKE_OK) return 0;
+    if (compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, hooks, simplex, source, include_dirs, cubin, lowered, log) != BKE_OK) return 0;
     return cubin.size();
 }
 
@@ -369,6 +394,13 @@ size_t bke_debug_ckf_model_hooks_cubin_bytes(int32_t dim_x, int32_t dim_z, int32
     return cubin_bytes(BKE_FAMILY_CKF, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs);
 }
 
+size_t bke_debug_ukf_model_points_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
+                                              uint32_t hooks, uint32_t points, const char *source, const char *include_dirs)
+{
+    if (check_points(points)) return 0;
+    return cubin_bytes(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs, points != 0u);
+}
+
 const char *bke_ukf_model_log(const bke_ukf_model *m) { return m ? m->log.c_str() : ""; }
 
 int bke_ukf_model_registers(const bke_ukf_model *m, int32_t extras) { return m ? m->regs[extras ? 1 : 0] : -1; }
@@ -400,8 +432,14 @@ int bke_ukf_step_model(const bke_ukf_args *args, const bke_ukf_model *model, con
     if (a.hx_model == BKE_HX_LINEAR && (a.flags & BKE_DO_UPDATE) && !a.H) { set_error("BKE_HX_LINEAR needs H"); return BKE_ERR_BAD_ARG; }
     if (a.fx_model == BKE_FX_CONST_VEL && (a.dim_x & 1)) { set_error("BKE_FX_CONST_VEL needs an even dim_x"); return BKE_ERR_BAD_ARG; }
     if (fx_args_stride < 0 || hx_args_stride < 0) { set_error("negative args stride"); return BKE_ERR_BAD_ARG; }
+    const bool spx = (a.flags & BKE_UKF_SIMPLEX) != 0;
+    if (spx != model->simplex) {
+        set_error("bke_ukf_step_model: the model was compiled for the %s point set, the step asks for the %s set",
+                  model->simplex ? "simplex" : "Merwe", spx ? "simplex" : "Merwe");
+        return BKE_ERR_BAD_ARG;
+    }
     const double lam_n = a.alpha * a.alpha * (a.dim_x + a.kappa);
-    if (!(lam_n != 0.0)) { set_error("alpha^2 (n + kappa) must be non-zero"); return BKE_ERR_BAD_ARG; }
+    if (!spx && !(lam_n != 0.0)) { set_error("alpha^2 (n + kappa) must be non-zero"); return BKE_ERR_BAD_ARG; }
     if (a.n_filters == 0) return BKE_OK;
     return a.dtype == BKE_F32 ? launch_model<float>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream)
                               : launch_model<double>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream);
@@ -415,6 +453,11 @@ int bke_ukf_rts_smoother_model(const bke_ukf_rts_args *args, const bke_ukf_model
     if (model->family != BKE_FAMILY_UKF) { set_error("bke_ukf_rts_smoother_model: the model was compiled for the CKF (bke_ckf_model_compile)"); return BKE_ERR_BAD_ARG; }
     if (!model->kern_rts) { set_error("bke_ukf_rts_smoother_model: the model has neither a user fx nor hooks (use bke_ukf_rts_smoother) or dim_x > %d", UR_MAXN); return BKE_ERR_UNSUPPORTED; }
     if (a.dim_x != model->n || a.dtype != model->dtype || a.fx_model != model->fx_model) { set_error("bke_ukf_rts_smoother_model: args do not match the compiled model"); return BKE_ERR_BAD_ARG; }
+    if (((a.flags & BKE_UKF_SIMPLEX) != 0) != model->simplex) {
+        set_error("bke_ukf_rts_smoother_model: the model was compiled for the %s point set, the smoother asks for the %s set",
+                  model->simplex ? "simplex" : "Merwe", model->simplex ? "Merwe" : "simplex");
+        return BKE_ERR_BAD_ARG;
+    }
     if (a.fx_model == BKE_FX_CONST_VEL && (a.dim_x & 1)) { set_error("BKE_FX_CONST_VEL needs an even dim_x"); return BKE_ERR_BAD_ARG; }
     if (a.fx_model == BKE_FX_LINEAR && (!a.F || a.F_stride < 0)) { set_error("BKE_FX_LINEAR needs F"); return BKE_ERR_BAD_ARG; }
     if (a.n_filters < 0 || a.n_steps < 0 || fx_args_stride < 0 || a.Q_stride < 0) { set_error("negative sizes"); return BKE_ERR_BAD_ARG; }

@@ -10,7 +10,8 @@ int launch_t(const bke_ukf_rts_args &a, cudaStream_t s)
 {
     UrP<T> p;
     ukf_rts_fill_params<T>(a, p);
-    ukf_rts_kernel<T, false><<<(unsigned)((p.N + 63) / 64), 64, 0, s>>>(p);
+    auto kern = (a.flags & BKE_UKF_SIMPLEX) ? ukf_rts_kernel<T, false, true> : ukf_rts_kernel<T, false>;
+    kern<<<(unsigned)((p.N + 63) / 64), 64, 0, s>>>(p);
     return check_cuda(cudaGetLastError(), "ukf rts launch");
 }
 

@@ -33,17 +33,42 @@ struct UrP {
     int64_t s_fx_args;             // 0 = one vector for the bank, else elements per filter
 };
 
-// USER_FX: the process function is the user's (run-time compiled instance, ukf_rtc.cu); see ukf_kernel.cuh
-template <typename T, bool USER_FX>
+// the simplex offsets of ukfk::simplex_offsets for a run-time n: row j-1 of U (n x n, zero below the
+// diagonal) becomes D_j, D0 receives D_0
+template <typename T>
+__device__ __forceinline__ void simplex_offsets_rt(int n, T *U, T *D0)
+{
+    T S[UR_MAXN];
+    for (int i = 0; i < n; i++) S[i] = T(0);
+    for (int j = n; j >= 2; j--) {
+        const T c = ukfk::simplex_coef<T>(n, j);
+        for (int i = j - 1; i < n; i++) {
+            const T u = U[(j - 1) * n + i];
+            U[(j - 1) * n + i] = T(-j) * c * u + S[i];
+            S[i] += c * u;
+        }
+    }
+    const T c1 = ukfk::simplex_coef<T>(n, 1);
+    for (int i = 0; i < n; i++) {
+        const T u = U[i];
+        D0[i] = S[i] - c1 * u;
+        U[i] = S[i] + c1 * u;
+    }
+}
+
+// USER_FX: the process function is the user's (run-time compiled instance, ukf_rtc.cu); see ukf_kernel.cuh.
+// SPX: the simplex point set (n + 1 points x + D_s, p.scale = 1, every weight 1/(n+1)).
+template <typename T, bool USER_FX, bool SPX = false>
 __global__ void __launch_bounds__(64) ukf_rts_kernel(UrP<T> p)
 {
     const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= p.N) return;
-    const int n = p.n, ns = 2 * n + 1;
+    const int n = p.n, ns = SPX ? n + 1 : 2 * n + 1;
     T xs[UR_MAXN], Ps[UR_MAXN * UR_MAXN];                 // smoothed epoch k+1
     T xk[UR_MAXN], Pk[UR_MAXN * UR_MAXN];
     T U[UR_MAXN * UR_MAXN], Pb[UR_MAXN * UR_MAXN], Pxb[UR_MAXN * UR_MAXN], PbI[UR_MAXN * UR_MAXN], Kk[UR_MAXN * UR_MAXN];
     T sf[(2 * UR_MAXN + 1) * UR_MAXN], xb[UR_MAXN], tmp[UR_MAXN * UR_MAXN];
+    T D0[SPX ? UR_MAXN : 1];                              // the simplex offset D_0
     const T *Q = p.Q + f * p.sQ;
     const T *F = p.F ? p.F + f * p.sF : nullptr;
     int64_t tf = (p.Tn - 1) * p.N + f;
@@ -74,6 +99,9 @@ __global__ void __launch_bounds__(64) ukf_rts_kernel(UrP<T> p)
                     U[j * n + i] = s * inv;
                 }
             }
+            if constexpr (SPX) {
+                if (ok) simplex_offsets_rt<T>(n, U, D0);
+            }
         }
         if (ok) {
             const T dt = p.dts ? (T)p.dts[k] : p.dt;
@@ -83,7 +111,11 @@ __global__ void __launch_bounds__(64) ukf_rts_kernel(UrP<T> p)
                 T sp[UR_MAXN];
                 const int row = s == 0 ? 0 : (s - 1) % n;
                 const T sign = s == 0 ? T(0) : (s <= n ? T(1) : T(-1));
-                for (int i = 0; i < n; i++) sp[i] = (s == 0) ? xk[i] : xk[i] + sign * U[row * n + i];
+                if constexpr (SPX) {
+                    for (int i = 0; i < n; i++) sp[i] = xk[i] + (s == 0 ? D0[i] : U[(s - 1) * n + i]);
+                } else {
+                    for (int i = 0; i < n; i++) sp[i] = (s == 0) ? xk[i] : xk[i] + sign * U[row * n + i];
+                }
                 T *fo = sf + s * n;
                 if constexpr (USER_FX) {
                     ukfk::bke_user_fx<T>(sp, fo, dt, p.fx_args ? p.fx_args + f * p.s_fx_args : nullptr);
@@ -115,7 +147,11 @@ __global__ void __launch_bounds__(64) ukf_rts_kernel(UrP<T> p)
                     // y = residual_x(sigmas_f[i], xb), z = residual_x(sigmas[i], Xs[k]) (:727-728)
                     T sp[UR_MAXN], z[UR_MAXN];
                     ukfk::bke_hook_residual_x<T>(sf + s * n, xb, y);
-                    for (int i = 0; i < n; i++) sp[i] = (s == 0) ? xk[i] : xk[i] + sign * U[row * n + i];
+                    if constexpr (SPX) {
+                        for (int i = 0; i < n; i++) sp[i] = xk[i] + (s == 0 ? D0[i] : U[(s - 1) * n + i]);
+                    } else {
+                        for (int i = 0; i < n; i++) sp[i] = (s == 0) ? xk[i] : xk[i] + sign * U[row * n + i];
+                    }
                     ukfk::bke_hook_residual_x<T>(sp, xk, z);
                     for (int i = 0; i < n; i++) {
                         const T wy = w * y[i], wz = w * z[i];
@@ -127,7 +163,12 @@ __global__ void __launch_bounds__(64) ukf_rts_kernel(UrP<T> p)
                 for (int i = 0; i < n; i++) {
                     const T wy = w * y[i];
                     for (int j = 0; j < n; j++) Pb[i * n + j] += wy * y[j];
-                    if (s > 0) {
+                    if constexpr (SPX) {
+                        // every simplex point is off x: (x + D_s) - x, formed as the reference does (:722)
+                        const T z = (xk[i] + (s == 0 ? D0[i] : U[(s - 1) * n + i])) - xk[i];
+                        const T wz = w * z;
+                        for (int j = 0; j < n; j++) Pxb[i * n + j] += wz * y[j];
+                    } else if (s > 0) {
                         // the reference forms (x + U) - x in floating point (:722); so does this
                         const T z = (xk[i] + sign * U[row * n + i]) - xk[i];
                         const T wz = w * z;

@@ -1,22 +1,26 @@
 // ut.cu — stand-alone sigma-point generation and unscented transform for a bank (the fused UKF step
 // in ukf.cu does both on chip; these entry points serve callers of
-// MerweScaledSigmaPoints.sigma_points (filterpy/kalman/sigma_points.py:124-177) and
+// MerweScaledSigmaPoints.sigma_points (filterpy/kalman/sigma_points.py:124-177),
+// SimplexSigmaPoints.sigma_points (:454-513) and
 // unscented_transform (filterpy/kalman/unscented_transform.py:22-128) themselves).
 // One warp per filter, matrices in the warp's slice of shared memory: sigma points for any n <= 32, the
 // transform for any k <= 256 points of n <= 64 (up to 4 warps per block, fewer when their slices do not fit).
 #include "bke_internal.cuh"
+#include "ukf_kernel.cuh"
 
 namespace bke {
 namespace {
 
-template <typename T>
+// SPX: SimplexSigmaPoints (sigma_points.py:499-513, scale = 1): lane i forms column i of the offsets
+// D_n .. D_0 with the running suffix sum of ukf_kernel.cuh's simplex_offsets
+template <typename T, bool SPX = false>
 __global__ void __launch_bounds__(128) k_sigma_points(int64_t N, int n, T scale, const T *x, const T *P, T *sig, int32_t *status)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, wpb = blockDim.x >> 5;
     T *U = reinterpret_cast<T *>(smem_raw) + (size_t)wib * (n * n + n);
     T *xs = U + n * n;
-    const int ns = 2 * n + 1;
+    const int ns = SPX ? n + 1 : 2 * n + 1;
     for (int64_t f = (int64_t)blockIdx.x * wpb + wib; f < N; f += (int64_t)gridDim.x * wpb) {
         for (int e = lane; e < n * n; e += 32) U[e] = scale * P[f * n * n + e];
         for (int e = lane; e < n; e += 32) xs[e] = x[f * n + e];
@@ -38,6 +42,26 @@ __global__ void __launch_bounds__(128) k_sigma_points(int64_t N, int n, T scale,
             __syncwarp();
         }
         T *o = sig + f * (int64_t)ns * n;
+        if constexpr (SPX) {
+            for (int i = lane; i < n; i += 32) {
+                T S = T(0);
+                for (int j = n; j >= 2; j--) {
+                    T v = xs[i];
+                    if (i >= j - 1) {
+                        const T c = ukfk::simplex_coef<T>(n, j), u = U[(j - 1) * n + i];
+                        v = xs[i] + (T(-j) * c * u + S);
+                        S += c * u;
+                    }
+                    o[j * n + i] = v;
+                }
+                const T c1 = ukfk::simplex_coef<T>(n, 1), u = U[i];
+                o[i] = xs[i] + (S - c1 * u);
+                o[n + i] = xs[i] + (S + c1 * u);
+            }
+            if (status && lane == 0) status[f] = st;
+            __syncwarp();
+            continue;
+        }
         for (int e = lane; e < ns * n; e += 32) {
             const int s = e / n, i = e - s * n;
             T v = xs[i];
@@ -90,6 +114,15 @@ int sigma_t(int64_t N, int n, double alpha, double kappa, const void *x, const v
 }
 
 template <typename T>
+int simplex_t(int64_t N, int n, const void *x, const void *P, void *sig, int32_t *status, cudaStream_t s)
+{
+    const size_t smem = 4 * sizeof(T) * (size_t)(n * n + n);
+    int64_t grid = (N + 3) / 4, cap = (int64_t)sm_count() * 16;
+    k_sigma_points<T, true><<<(unsigned)(grid < cap ? grid : cap), 128, smem, s>>>(N, n, T(1), (const T *)x, (const T *)P, (T *)sig, status);
+    return check_cuda(cudaGetLastError(), "k_sigma_points launch");
+}
+
+template <typename T>
 int ut_t(int64_t N, int ns, int n, const void *sig, const void *Wm, const void *Wc, const void *noise, int64_t nstride,
          void *x_out, void *P_out, cudaStream_t s)
 {
@@ -130,6 +163,18 @@ int bke_merwe_sigma_points(int64_t n_filters, int32_t dim_x, int32_t dtype, doub
     if (bke_device_count() <= 0) { set_error("no CUDA device available; the engine has no CPU fallback"); return BKE_ERR_CUDA; }
     return dtype == BKE_F32 ? sigma_t<float>(n_filters, dim_x, alpha, kappa, x, P, sigmas, status, (cudaStream_t)stream)
                             : sigma_t<double>(n_filters, dim_x, alpha, kappa, x, P, sigmas, status, (cudaStream_t)stream);
+}
+
+int bke_simplex_sigma_points(int64_t n_filters, int32_t dim_x, int32_t dtype, const void *x, const void *P, void *sigmas,
+                             int32_t *status, void *stream)
+{
+    if (n_filters < 0 || dim_x < 1 || dim_x > 32) { set_error("bad dimensions (1 <= dim_x <= 32)"); return BKE_ERR_BAD_ARG; }
+    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (n_filters == 0) return BKE_OK;
+    if (!x || !P || !sigmas) { set_error("NULL argument"); return BKE_ERR_BAD_ARG; }
+    if (bke_device_count() <= 0) { set_error("no CUDA device available; the engine has no CPU fallback"); return BKE_ERR_CUDA; }
+    return dtype == BKE_F32 ? simplex_t<float>(n_filters, dim_x, x, P, sigmas, status, (cudaStream_t)stream)
+                            : simplex_t<double>(n_filters, dim_x, x, P, sigmas, status, (cudaStream_t)stream);
 }
 
 int bke_unscented_transform(int64_t n_filters, int32_t n_sigmas, int32_t dim, int32_t dtype, const void *sigmas,

@@ -26,6 +26,7 @@ import torch
 from .. import _lib
 from .._dev import bke_dtype, ptr, stream_ptr
 from ._bank import _BankMirror, _model_prop
+from .sigma_points import SimplexSigmaPoints
 
 __all__ = ["UnscentedKalmanFilter", "LinearFx", "ConstVelFx", "LinearHx", "RangeAzElHx", "RangeBearingHx",
            "DeviceFx", "DeviceHx", "DeviceFn"]
@@ -158,18 +159,21 @@ def _device_hooks(**given):
 _compiled_models = {}
 
 
-def _compile_model(lib, dim_x, dim_z, dtype_id, fx, hx, entry="bke_ukf_model_compile", hooks=(0, ())):
-    """One NVRTC build per (filter family, shape, dtype, hooks, source); shared by every filter object that
-    uses it.  ``entry`` names the family's compile call (bke_ukf_model_compile / bke_ckf_model_compile);
-    ``hooks`` is what ``_device_hooks`` returns."""
+def _compile_model(lib, dim_x, dim_z, dtype_id, fx, hx, entry="bke_ukf_model_compile", hooks=(0, ()), points=0):
+    """One NVRTC build per (filter family, shape, dtype, hooks, point set, source); shared by every filter object
+    that uses it.  ``entry`` names the family's compile call (bke_ukf_model_compile / bke_ckf_model_compile);
+    ``hooks`` is what ``_device_hooks`` returns; ``points`` is 0 or BKE_UKF_SIMPLEX (UKF only)."""
     mask, fns = hooks
     src = "\n".join([m.source for m in (fx, hx) if isinstance(m, _DeviceModel)] + [f.source for f in fns])
-    key = (entry, dim_x, dim_z, dtype_id, fx.model, hx.model, mask, src)
+    key = (entry, dim_x, dim_z, dtype_id, fx.model, hx.model, mask, points, src)
     h = _compiled_models.get(key)
     if h is None:
         out = ctypes.c_void_p()
         inc = _lib.kernel_include_dirs().encode()
-        if mask:
+        if points:
+            rc = lib.bke_ukf_model_compile_points(dim_x, dim_z, dtype_id, fx.model, hx.model, mask, points, src.encode(), inc,
+                                                  ctypes.byref(out))
+        elif mask:
             rc = getattr(lib, entry + "_hooks")(dim_x, dim_z, dtype_id, fx.model, hx.model, mask, src.encode(), inc,
                                                  ctypes.byref(out))
         else:
@@ -202,9 +206,9 @@ class _SigmaPointBank(_BankMirror):
     _COLUMN_X = False                                   # x is 1-D (UKF.py:298)
     _FAILURE = "matrix not positive definite / singular"
 
-    def _init_bank(self, dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics, hooks=(0, ())):
-        """The state, models, compiled user model (around DeviceFx / DeviceHx or ``hooks``) and diagnostic
-        buffers of a bank (the reference's __init__ defaults: x = 0, P = I, Q = I, R = I)."""
+    def _init_bank(self, dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics, hooks=(0, ()), points=0):
+        """The state, models, compiled user model (around DeviceFx / DeviceHx or ``hooks``, for the point set
+        ``points``) and diagnostic buffers of a bank (the reference's __init__ defaults: x = 0, P = I, Q = I, R = I)."""
         _BankMirror._init_bank(self, dim_x, dim_z, n_filters, dtype, device, diagnostics)
         self.fx, self.hx = fx, hx
         N, n, m = self.n_filters, self.dim_x, self.dim_z
@@ -222,7 +226,7 @@ class _SigmaPointBank(_BankMirror):
         self._hooks = hooks[0]
         if isinstance(fx, _DeviceModel) or isinstance(hx, _DeviceModel) or self._hooks:
             with torch.cuda.device(self._device):
-                self._user_model = self._compile_model(self._lib, n, m, bke_dtype(self._dtype), fx, hx, hooks=hooks)
+                self._user_model = self._compile_model(self._lib, n, m, bke_dtype(self._dtype), fx, hx, hooks=hooks, points=points)
             if isinstance(fx, _DeviceModel):
                 self._fx_args = fx.pack({}, N, self._dtype, self._device) if all(k in fx.values for k in fx.arg_names) else (None, 0)
             if isinstance(hx, _DeviceModel):
@@ -301,7 +305,9 @@ class UnscentedKalmanFilter(_SigmaPointBank):
         _require_device_models(fx, hx)
         if points.n != dim_x:
             raise ValueError("expected size(x) {}, but size is {}".format(points.n, dim_x))   # sigma_points.py:153
-        self._init_bank(dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics, hooks)
+        # the point set selects the kernel instances: SimplexSigmaPoints runs the simplex ones (n + 1 points)
+        self._point_flag = _lib.BKE_UKF_SIMPLEX if isinstance(points, SimplexSigmaPoints) else 0
+        self._init_bank(dim_x, dim_z, fx, hx, n_filters, dtype, device, diagnostics, hooks, self._point_flag)
         self.points_fn = points
         self._dt = dt
         self._num_sigmas = points.num_sigmas()
@@ -342,8 +348,9 @@ class UnscentedKalmanFilter(_SigmaPointBank):
         self._z = zt
 
     def _launch(self, flags, dt, zt, vt, R):
-        a = self._fill(_lib.UkfArgs(), flags, dt, zt, vt, R)
-        a.alpha, a.beta, a.kappa = self.points_fn.alpha, self.points_fn.beta, self.points_fn.kappa
+        a = self._fill(_lib.UkfArgs(), flags | self._point_flag, dt, zt, vt, R)
+        if not self._point_flag:
+            a.alpha, a.beta, a.kappa = self.points_fn.alpha, self.points_fn.beta, self.points_fn.kappa
         self._step(a, self._lib.bke_ukf_step, self._lib.bke_ukf_step_model)
 
     def rts_smoother(self, Xs, Ps, Qs=None, dts=None, UT=None):
@@ -365,7 +372,9 @@ class UnscentedKalmanFilter(_SigmaPointBank):
         a = _lib.UkfRtsArgs()
         a.n_filters, a.n_steps, a.dim_x, a.dtype = N, T, n, bke_dtype(self._dtype)
         a.fx_model = self.fx.model
-        a.alpha, a.beta, a.kappa = self.points_fn.alpha, self.points_fn.beta, self.points_fn.kappa
+        a.flags = self._point_flag
+        if not self._point_flag:
+            a.alpha, a.beta, a.kappa = self.points_fn.alpha, self.points_fn.beta, self.points_fn.kappa
         a.dt = float(self._dt)
         dts_t = None
         if dts is not None:

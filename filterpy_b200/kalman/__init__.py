@@ -1,6 +1,6 @@
 """GPU mirrors of ``filterpy.kalman`` for the hot path (see DESIGN.md for the scope)."""
 from .kalman_filter import KalmanFilter, predict, update, batch_filter, rts_smoother  # noqa: F401
-from .sigma_points import MerweScaledSigmaPoints, JulierSigmaPoints  # noqa: F401
+from .sigma_points import MerweScaledSigmaPoints, JulierSigmaPoints, SimplexSigmaPoints  # noqa: F401
 from .UKF import (UnscentedKalmanFilter, LinearFx, ConstVelFx, LinearHx, RangeAzElHx,  # noqa: F401
                   RangeBearingHx, DeviceFx, DeviceHx, DeviceFn)
 from .CubatureKalmanFilter import CubatureKalmanFilter  # noqa: F401

@@ -7,6 +7,7 @@ The same symbols exposed as torch.ops.* via a C++ extension for zero-copy CUDA t
     x, P = torch.ops.bke.kf_step(x, P, F, H, Q, R, z)              # kalman_filter.py:437-561 for a bank
     x, P = torch.ops.bke.kf_predict(x, P, F, Q)                    # :437-482
     x, P = torch.ops.bke.ukf_step(x, P, Q, R, z, dt, alpha, beta, kappa, fx_model, hx_model)   # UKF.py:364-491
+    x, P = torch.ops.bke.ukf_step(..., simplex=True)               # the same on SimplexSigmaPoints(n)
     x, P = torch.ops.bke.ckf_step(x, P, Q, R, z, dt, fx_model, hx_model)   # CubatureKalmanFilter.py:292-389
     x, P, s = torch.ops.bke.enkf_step(x, P, sigmas, Q, R, z, dt, fx_model, hx_model, seed, counter)   # ensemble_kalman_filter.py:218-290
     x, L = torch.ops.bke.srkf_step(x, L, F, H, Lq, Lr, z)          # square_root.py:172-248 (L = P1_2)

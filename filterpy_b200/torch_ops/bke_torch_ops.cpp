@@ -90,7 +90,7 @@ std::tuple<at::Tensor, at::Tensor> kf_predict(const at::Tensor &x, const at::Ten
 std::tuple<at::Tensor, at::Tensor> ukf_step(const at::Tensor &x, const at::Tensor &P, const at::Tensor &Q, const at::Tensor &R,
                                             const at::Tensor &z, double dt, double alpha, double beta, double kappa,
                                             int64_t fx_model, int64_t hx_model, const c10::optional<at::Tensor> &F,
-                                            const c10::optional<at::Tensor> &H)
+                                            const c10::optional<at::Tensor> &H, bool simplex)
 {
     TORCH_CHECK(x.is_cuda() && P.is_cuda() && x.is_contiguous() && P.is_contiguous() && x.dim() == 2 && P.dim() == 3, "bke: x is [N, n], P is [N, n, n] on the GPU");
     c10::cuda::CUDAGuard guard(x.device());
@@ -100,6 +100,7 @@ std::tuple<at::Tensor, at::Tensor> ukf_step(const at::Tensor &x, const at::Tenso
     a.n_filters = N; a.dim_x = (int32_t)n; a.dim_z = (int32_t)m; a.dtype = dtype_of(x);
     a.flags = BKE_DO_PREDICT | BKE_DO_UPDATE; a.fx_model = (int32_t)fx_model; a.hx_model = (int32_t)hx_model;
     a.dt = dt; a.alpha = alpha; a.beta = beta; a.kappa = kappa;
+    if (simplex) a.flags |= BKE_UKF_SIMPLEX;                   // SimplexSigmaPoints: alpha, beta, kappa ignored
     at::Tensor x_out = at::empty_like(x), P_out = at::empty_like(P);
     a.x = x.data_ptr(); a.P = P.data_ptr(); a.x_out = x_out.data_ptr(); a.P_out = P_out.data_ptr();
     a.Q = model(Q, N, n, n, &a.Q_stride, x, "Q");
@@ -352,7 +353,7 @@ TORCH_LIBRARY(bke, m)
     m.def("kf_step(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor z, float alpha_sq=1.0) -> (Tensor, Tensor)");
     m.def("kf_predict(Tensor x, Tensor P, Tensor F, Tensor Q, float alpha_sq=1.0) -> (Tensor, Tensor)");
     m.def("ukf_step(Tensor x, Tensor P, Tensor Q, Tensor R, Tensor z, float dt, float alpha, float beta, float kappa, "
-          "int fx_model, int hx_model, Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor)");
+          "int fx_model, int hx_model, Tensor? F=None, Tensor? H=None, bool simplex=False) -> (Tensor, Tensor)");
     m.def("ckf_step(Tensor x, Tensor P, Tensor Q, Tensor R, Tensor z, float dt, int fx_model, int hx_model, "
           "Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor)");
     m.def("enkf_step(Tensor x, Tensor P, Tensor sigmas, Tensor Q, Tensor R, Tensor z, float dt, int fx_model, int hx_model, "

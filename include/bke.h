@@ -292,12 +292,17 @@ int bke_fls_smooth(const bke_fls_args *args, void *stream);
 #define BKE_FX_USER 100          /* device function supplied as source text: bke_ukf_model_compile (below) */
 #define BKE_HX_USER 100
 
+/* flag of bke_ukf_args.flags and bke_ukf_rts_args.flags: SimplexSigmaPoints(n) (sigma_points.py:386-534) instead
+ * of MerweScaledSigmaPoints: n + 1 points x + D_j, D = (chol_upper(P)' sqrt(n) Istar)', Wm = Wc = 1/(n+1);
+ * alpha, beta and kappa are ignored */
+#define BKE_UKF_SIMPLEX 32u
+
 typedef struct bke_ukf_args {
     int64_t n_filters;
     int32_t dim_x, dim_z;
     int32_t dtype;
     uint32_t flags;                  /* BKE_DO_PREDICT | BKE_DO_UPDATE (update alone re-draws the
-                                        sigma points from (x,P), UKF.py:407) */
+                                        sigma points from (x,P), UKF.py:407), | BKE_UKF_SIMPLEX */
     int32_t fx_model, hx_model;
     double dt;
     double alpha, beta, kappa;       /* MerweScaledSigmaPoints(n, alpha, beta, kappa) */
@@ -363,6 +368,15 @@ int bke_ukf_model_compile_hooks(int32_t dim_x, int32_t dim_z, int32_t dtype, int
                                 const char *source, const char *include_dirs, bke_ukf_model **out);
 size_t bke_debug_ukf_model_hooks_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
                                              uint32_t hooks, const char *source, const char *include_dirs);
+
+/* The same for a chosen point set: points = 0 (MerweScaledSigmaPoints: bke_ukf_model_compile_hooks exactly) or
+ * BKE_UKF_SIMPLEX (SimplexSigmaPoints; the text sees BKE_N_SIGMAS = n + 1, hooks or not).  The handle remembers
+ * its point set: bke_ukf_step_model and bke_ukf_rts_smoother_model refuse args whose flags ask for the other
+ * set (BKE_ERR_BAD_ARG). */
+int bke_ukf_model_compile_points(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, uint32_t hooks,
+                                 uint32_t points, const char *source, const char *include_dirs, bke_ukf_model **out);
+size_t bke_debug_ukf_model_points_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
+                                              uint32_t hooks, uint32_t points, const char *source, const char *include_dirs);
 
 /* ------------------------------------------------------------------------------------------
  * Cubature Kalman filter bank.
@@ -550,6 +564,10 @@ int bke_cholesky_lower(int64_t n_filters, int32_t k, int32_t dtype, const void *
  *       -> x_out[N,n], P_out[N,n,n]   (default mean / residual functions). */
 int bke_merwe_sigma_points(int64_t n_filters, int32_t dim_x, int32_t dtype, double alpha, double beta, double kappa,
                            const void *x, const void *P, void *sigmas, int32_t *status, void *stream);
+/*   SimplexSigmaPoints.sigma_points(x, P)   filterpy/kalman/sigma_points.py:454-513
+ *       x[N,n], P[N,n,n] -> sigmas[N,n+1,n] (Xi_0 .. Xi_n); bounds and status as bke_merwe_sigma_points. */
+int bke_simplex_sigma_points(int64_t n_filters, int32_t dim_x, int32_t dtype, const void *x, const void *P, void *sigmas,
+                             int32_t *status, void *stream);
 int bke_unscented_transform(int64_t n_filters, int32_t n_sigmas, int32_t dim, int32_t dtype, const void *sigmas,
                             const void *Wm, const void *Wc, const void *noise_cov, int64_t noise_stride,
                             void *x_out, void *P_out, void *stream);
@@ -766,10 +784,12 @@ int bke_kf_rts_smoother(const bke_rts_args *args, void *stream);
 /* UnscentedKalmanFilter.rts_smoother filterpy/kalman/UKF.py:634-739 for a bank; same layout as
  * bke_kf_rts_smoother.  Q is the filter's own Q (the reference never reads its Qs argument, :715);
  * dts is a DEVICE array of n_steps doubles (step k uses dts[k], :712) or NULL = dt for every step;
- * fx_model / F as in bke_ukf_args.  K may be NULL. */
+ * fx_model / F as in bke_ukf_args.  K may be NULL.  flags: 0 (Merwe points from alpha, beta, kappa) or
+ * BKE_UKF_SIMPLEX (simplex points; alpha, beta, kappa ignored). */
 typedef struct {
     int64_t n_filters, n_steps;
-    int32_t dim_x, dtype, fx_model, reserved;
+    int32_t dim_x, dtype, fx_model;
+    uint32_t flags;
     double alpha, beta, kappa;
     double dt;
     const double *dts;
