@@ -23,6 +23,13 @@ int check_cuda(cudaError_t e, const char *what)
     return BKE_ERR_CUDA;
 }
 
+int launch_kernel(const void *kern, unsigned grid, unsigned block, size_t smem, void *params, cudaStream_t s, const char *what)
+{
+    if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
+    void *args[] = {params};
+    return check_cuda(cudaLaunchKernel(kern, dim3(grid), dim3(block), args, smem, s), what);
+}
+
 int sm_count()
 {
     static int cached[64] = {0};
@@ -101,6 +108,79 @@ static int validate_srkf(const bke_srkf_args *a)
         return BKE_ERR_BAD_ARG;
     }
     return BKE_OK;
+}
+
+// the checks every sigma-point step (UKF, CKF, EnKF; pre-built and run-time compiled) makes
+template <typename Args>
+static int validate_sigma(const Args &a)
+{
+    if (a.dtype != BKE_F32 && a.dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (!(a.flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
+    if (!a.x || !a.P || !a.x_out || !a.P_out) { set_error("x, P, x_out, P_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if ((a.flags & BKE_DO_PREDICT) && !a.Q) { set_error("predict needs Q"); return BKE_ERR_BAD_ARG; }
+    if ((a.flags & BKE_DO_UPDATE) && (!a.R || !a.z)) { set_error("update needs R and z"); return BKE_ERR_BAD_ARG; }
+    if (a.fx_model == BKE_FX_LINEAR && (a.flags & BKE_DO_PREDICT) && !a.F) { set_error("BKE_FX_LINEAR needs F"); return BKE_ERR_BAD_ARG; }
+    if (a.hx_model == BKE_HX_LINEAR && (a.flags & BKE_DO_UPDATE) && !a.H) { set_error("BKE_HX_LINEAR needs H"); return BKE_ERR_BAD_ARG; }
+    if (a.fx_model == BKE_FX_CONST_VEL && (a.dim_x & 1)) { set_error("BKE_FX_CONST_VEL needs an even dim_x"); return BKE_ERR_BAD_ARG; }
+    return BKE_OK;
+}
+
+// bke_ukf_step and bke_ukf_step_model (where the dimension and dtype checks cannot fail: the args matched
+// a compiled model)
+int validate_ukf(const bke_ukf_args &a)
+{
+    if (a.n_filters < 0 || a.dim_x < 1 || a.dim_z < 1) { set_error("bad dimensions"); return BKE_ERR_BAD_ARG; }
+    if (int rc = validate_sigma(a)) return rc;
+    const double lam_n = a.alpha * a.alpha * (a.dim_x + a.kappa);
+    if (!(a.flags & BKE_UKF_SIMPLEX) && !(lam_n != 0.0)) { set_error("alpha^2 (n + kappa) must be non-zero"); return BKE_ERR_BAD_ARG; }
+    return BKE_OK;
+}
+
+int validate_ckf(const bke_ckf_args &a)
+{
+    if (a.n_filters < 0 || a.dim_x < 1 || a.dim_z < 1) { set_error("bad dimensions"); return BKE_ERR_BAD_ARG; }
+    if (int rc = validate_sigma(a)) return rc;
+    if ((a.flags & BKE_DO_UPDATE) && !(a.flags & BKE_DO_PREDICT) && !a.sigmas_f) {
+        set_error("an update without predict reads the propagated points of the last predict: sigmas_f must be non-NULL");
+        return BKE_ERR_BAD_ARG;
+    }
+    return BKE_OK;
+}
+
+int validate_enkf(const bke_enkf_args &a)
+{
+    if (a.n_filters < 0 || a.dim_x < 1 || a.dim_x > 16 || a.dim_z < 1) { set_error("bad dimensions (1 <= dim_x <= 16, 1 <= dim_z)"); return BKE_ERR_BAD_ARG; }
+    if (a.n_members < 2) { set_error("n_members must be 2 or greater (the covariances divide by n_members - 1)"); return BKE_ERR_BAD_ARG; }
+    if (int rc = validate_sigma(a)) return rc;
+    if (a.flags & ~(BKE_DO_PREDICT | BKE_DO_UPDATE)) { set_error("flags: only BKE_DO_PREDICT and BKE_DO_UPDATE apply to the EnKF"); return BKE_ERR_BAD_ARG; }
+    if (!a.sigmas || !a.sigmas_out) { set_error("sigmas and sigmas_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if (a.Q_stride < 0 || a.R_stride < 0 || a.F_stride < 0 || a.H_stride < 0) { set_error("negative model stride"); return BKE_ERR_BAD_ARG; }
+    if (a.n_members > (1 << 24)) { set_error("n_members must be at most 2^24"); return BKE_ERR_BAD_ARG; }
+    return BKE_OK;
+}
+
+// the pre-built steps: a known model id, and a range model at the shape it is written for
+template <typename Args>
+static int validate_builtin_models(const Args &a)
+{
+    if (a.hx_model == BKE_HX_RANGE_AZ_EL && !(a.dim_x == 6 && a.dim_z == 3)) { set_error("BKE_HX_RANGE_AZ_EL needs dim_x=6, dim_z=3"); return BKE_ERR_BAD_ARG; }
+    if (a.hx_model == BKE_HX_RANGE_BEARING && !(a.dim_x == 4 && a.dim_z == 2)) { set_error("BKE_HX_RANGE_BEARING needs dim_x=4, dim_z=2"); return BKE_ERR_BAD_ARG; }
+    if (a.fx_model < 0 || a.fx_model > BKE_FX_CONST_VEL || a.hx_model < 0 || a.hx_model > BKE_HX_RANGE_BEARING) {
+        set_error("unknown fx/hx model id"); return BKE_ERR_BAD_ARG;
+    }
+    return BKE_OK;
+}
+
+// bke_ukf_step, bke_ckf_step, bke_enkf_step
+template <typename Args>
+static int sigma_step(const Args *args, int (*validate)(const Args &), int (*launch)(const Args &, cudaStream_t), void *stream)
+{
+    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    const Args &a = *args;
+    int rc = validate(a);
+    if (rc || (rc = validate_builtin_models(a)) || (rc = require_device())) return rc;
+    if (a.n_filters == 0) return BKE_OK;
+    return launch(a, (cudaStream_t)stream);
 }
 
 }  // namespace bke
@@ -328,63 +408,11 @@ int bke_fls_smooth(const bke_fls_args *args, void *stream)
     return launch_fls(a, (cudaStream_t)stream);
 }
 
-int bke_ukf_step(const bke_ukf_args *args, void *stream)
-{
-    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    const bke_ukf_args &a = *args;
-    if (a.n_filters < 0 || a.dim_x < 1 || a.dim_z < 1) { set_error("bad dimensions"); return BKE_ERR_BAD_ARG; }
-    if (a.dtype != BKE_F32 && a.dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
-    if (!(a.flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
-    if (!a.x || !a.P || !a.x_out || !a.P_out) { set_error("x, P, x_out, P_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    if ((a.flags & BKE_DO_PREDICT) && !a.Q) { set_error("predict needs Q"); return BKE_ERR_BAD_ARG; }
-    if ((a.flags & BKE_DO_UPDATE) && (!a.R || !a.z)) { set_error("update needs R and z"); return BKE_ERR_BAD_ARG; }
-    if (a.fx_model == BKE_FX_LINEAR && (a.flags & BKE_DO_PREDICT) && !a.F) { set_error("BKE_FX_LINEAR needs F"); return BKE_ERR_BAD_ARG; }
-    if (a.hx_model == BKE_HX_LINEAR && (a.flags & BKE_DO_UPDATE) && !a.H) { set_error("BKE_HX_LINEAR needs H"); return BKE_ERR_BAD_ARG; }
-    if (a.fx_model == BKE_FX_CONST_VEL && (a.dim_x & 1)) { set_error("BKE_FX_CONST_VEL needs an even dim_x"); return BKE_ERR_BAD_ARG; }
-    if (a.hx_model == BKE_HX_RANGE_AZ_EL && !(a.dim_x == 6 && a.dim_z == 3)) { set_error("BKE_HX_RANGE_AZ_EL needs dim_x=6, dim_z=3"); return BKE_ERR_BAD_ARG; }
-    if (a.hx_model == BKE_HX_RANGE_BEARING && !(a.dim_x == 4 && a.dim_z == 2)) { set_error("BKE_HX_RANGE_BEARING needs dim_x=4, dim_z=2"); return BKE_ERR_BAD_ARG; }
-    if (a.fx_model < 0 || a.fx_model > BKE_FX_CONST_VEL || a.hx_model < 0 || a.hx_model > BKE_HX_RANGE_BEARING) {
-        set_error("unknown fx/hx model id"); return BKE_ERR_BAD_ARG;
-    }
-    double lam_n = a.alpha * a.alpha * (a.dim_x + a.kappa);
-    if (!(a.flags & BKE_UKF_SIMPLEX) && !(lam_n != 0.0)) { set_error("alpha^2 (n + kappa) must be non-zero"); return BKE_ERR_BAD_ARG; }
-    int rc = require_device();
-    if (rc) return rc;
-    if (a.n_filters == 0) return BKE_OK;
-    return launch_ukf(a, (cudaStream_t)stream);
-}
+int bke_ukf_step(const bke_ukf_args *args, void *stream) { return sigma_step(args, validate_ukf, launch_ukf, stream); }
 
-int bke_ckf_step(const bke_ckf_args *args, void *stream)
-{
-    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    const bke_ckf_args &a = *args;
-    int rc = validate_ckf(a);
-    if (rc) return rc;
-    if (a.hx_model == BKE_HX_RANGE_AZ_EL && !(a.dim_x == 6 && a.dim_z == 3)) { set_error("BKE_HX_RANGE_AZ_EL needs dim_x=6, dim_z=3"); return BKE_ERR_BAD_ARG; }
-    if (a.hx_model == BKE_HX_RANGE_BEARING && !(a.dim_x == 4 && a.dim_z == 2)) { set_error("BKE_HX_RANGE_BEARING needs dim_x=4, dim_z=2"); return BKE_ERR_BAD_ARG; }
-    if (a.fx_model < 0 || a.fx_model > BKE_FX_CONST_VEL || a.hx_model < 0 || a.hx_model > BKE_HX_RANGE_BEARING) {
-        set_error("unknown fx/hx model id"); return BKE_ERR_BAD_ARG;
-    }
-    if ((rc = require_device())) return rc;
-    if (a.n_filters == 0) return BKE_OK;
-    return launch_ckf(a, (cudaStream_t)stream);
-}
+int bke_ckf_step(const bke_ckf_args *args, void *stream) { return sigma_step(args, validate_ckf, launch_ckf, stream); }
 
-int bke_enkf_step(const bke_enkf_args *args, void *stream)
-{
-    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    const bke_enkf_args &a = *args;
-    int rc = validate_enkf(a);
-    if (rc) return rc;
-    if (a.hx_model == BKE_HX_RANGE_AZ_EL && !(a.dim_x == 6 && a.dim_z == 3)) { set_error("BKE_HX_RANGE_AZ_EL needs dim_x=6, dim_z=3"); return BKE_ERR_BAD_ARG; }
-    if (a.hx_model == BKE_HX_RANGE_BEARING && !(a.dim_x == 4 && a.dim_z == 2)) { set_error("BKE_HX_RANGE_BEARING needs dim_x=4, dim_z=2"); return BKE_ERR_BAD_ARG; }
-    if (a.fx_model < 0 || a.fx_model > BKE_FX_CONST_VEL || a.hx_model < 0 || a.hx_model > BKE_HX_RANGE_BEARING) {
-        set_error("unknown fx/hx model id"); return BKE_ERR_BAD_ARG;
-    }
-    if ((rc = require_device())) return rc;
-    if (a.n_filters == 0) return BKE_OK;
-    return launch_enkf(a, (cudaStream_t)stream);
-}
+int bke_enkf_step(const bke_enkf_args *args, void *stream) { return sigma_step(args, validate_enkf, launch_enkf, stream); }
 
 int bke_enkf_initialize(int64_t n_filters, int32_t dim_x, int32_t n_members, int32_t dtype, uint32_t seed, uint32_t counter,
                         const void *x, const void *P, void *sigmas, int32_t *status, void *stream)

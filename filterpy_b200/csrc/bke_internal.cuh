@@ -12,6 +12,9 @@ namespace bke {
 #ifndef __CUDACC_RTC__
 void set_error(const char *fmt, ...);
 int check_cuda(cudaError_t e, const char *what);
+// sets the kernel's dynamic shared-memory limit to smem bytes and launches it on grid x block threads with
+// the one parameter block *params; `what` names the launch in the error
+int launch_kernel(const void *kern, unsigned grid, unsigned block, size_t smem, void *params, cudaStream_t s, const char *what);
 
 // Number of SMs of the current device (cached).
 int sm_count();
@@ -58,10 +61,12 @@ int launch_kf_any(const bke_kf_args &a, cudaStream_t s);
 int launch_kf_batch(const bke_kf_batch_args &a, cudaStream_t s);
 size_t fls_workspace_bytes(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dim_u, int32_t dtype, int64_t lag);
 int launch_fls(const bke_fls_args &a, cudaStream_t s);
-int launch_ukf(const bke_ukf_args &a, cudaStream_t s);
+// the argument checks of each sigma-point family's step, pre-built and run-time compiled (api.cu)
+int validate_ukf(const bke_ukf_args &a);
 int validate_ckf(const bke_ckf_args &a);
-int launch_ckf(const bke_ckf_args &a, cudaStream_t s);
 int validate_enkf(const bke_enkf_args &a);
+int launch_ukf(const bke_ukf_args &a, cudaStream_t s);
+int launch_ckf(const bke_ckf_args &a, cudaStream_t s);
 int launch_enkf(const bke_enkf_args &a, cudaStream_t s);
 int launch_enkf_init(int64_t n_filters, int32_t dim_x, int32_t n_members, int32_t dtype, uint32_t seed, uint32_t counter,
                      const void *x, const void *P, void *sigmas, int32_t *status, cudaStream_t s);

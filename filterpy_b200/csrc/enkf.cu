@@ -1,8 +1,7 @@
-// enkf.cu — host side of the ensemble Kalman filter bank: the closed set of pre-built (dim_x, dim_z, fx, hx)
-// instances of the kernel in enkf_kernel.cuh, the initialize kernel for every dim_x <= 16, their launch and
-// the argument checks shared by bke_enkf_step (api.cu) and bke_enkf_step_model (ukf_rtc.cu).
+// enkf.cu — host side of the ensemble Kalman filter bank: the pre-built instances (BKE_SIGMA_INSTANCES) of
+// the kernel in enkf_kernel.cuh, the initialize kernel for every dim_x <= 16 and their launch.
 // (Instances around user-supplied fx / hx are compiled at run time: ukf_rtc.cu.)
-#include "enkf_launch.cuh"
+#include "sigma_launch.cuh"
 
 namespace bke {
 namespace {
@@ -15,35 +14,14 @@ int launch_inst(const bke_enkf_args &a, cudaStream_t s)
     enkf_fill_params<T>(a, p);
     const size_t smem = enkf_smem_bytes(N, a.n_members, sizeof(T));
     auto kern = enkf_has_extras(a) ? enkf_kernel<T, N, M, FX, HX, true> : enkf_kernel<T, N, M, FX, HX, false>;
-    if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
-    kern<<<enkf_grid(p.N), EB, smem, s>>>(p);
-    return check_cuda(cudaGetLastError(), "enkf_kernel launch");
+    return launch_kernel((const void *)kern, enkf_grid(p.N), EB, smem, &p, s, "enkf_kernel launch");
 }
 
-// the same (dim_x, dim_z, fx, hx) set as the UKF's and the CKF's
 template <typename T>
 int dispatch(const bke_enkf_args &a, cudaStream_t s)
 {
-    const int n = a.dim_x, m = a.dim_z, fx = a.fx_model, hx = a.hx_model;
-#define BKE_ENKF(NN, MM, FXX, HXX) \
-    if (n == NN && m == MM && fx == FXX && hx == HXX) return launch_inst<T, NN, MM, FXX, HXX>(a, s);
-    BKE_ENKF(6, 3, BKE_FX_CONST_VEL, BKE_HX_RANGE_AZ_EL)
-    BKE_ENKF(6, 3, BKE_FX_CONST_VEL, BKE_HX_LINEAR)
-    BKE_ENKF(6, 3, BKE_FX_LINEAR, BKE_HX_LINEAR)
-    BKE_ENKF(6, 3, BKE_FX_LINEAR, BKE_HX_RANGE_AZ_EL)
-    BKE_ENKF(4, 2, BKE_FX_CONST_VEL, BKE_HX_RANGE_BEARING)
-    BKE_ENKF(4, 2, BKE_FX_LINEAR, BKE_HX_RANGE_BEARING)
-    BKE_ENKF(4, 2, BKE_FX_CONST_VEL, BKE_HX_LINEAR)
-    BKE_ENKF(4, 2, BKE_FX_LINEAR, BKE_HX_LINEAR)
-    BKE_ENKF(1, 1, BKE_FX_LINEAR, BKE_HX_LINEAR)
-    BKE_ENKF(2, 1, BKE_FX_LINEAR, BKE_HX_LINEAR)
-    BKE_ENKF(2, 1, BKE_FX_CONST_VEL, BKE_HX_LINEAR)
-    BKE_ENKF(2, 2, BKE_FX_LINEAR, BKE_HX_LINEAR)
-    BKE_ENKF(3, 1, BKE_FX_LINEAR, BKE_HX_LINEAR)
-    BKE_ENKF(3, 3, BKE_FX_LINEAR, BKE_HX_LINEAR)
-    BKE_ENKF(4, 4, BKE_FX_LINEAR, BKE_HX_LINEAR)
-#undef BKE_ENKF
-    set_error("bke_enkf_step: no kernel instance for dim_x=%d dim_z=%d fx_model=%d hx_model=%d", n, m, fx, hx);
+    BKE_SIGMA_INSTANCES(BKE_SIGMA_DISPATCH_ROW)
+    set_error("bke_enkf_step: no kernel instance for dim_x=%d dim_z=%d fx_model=%d hx_model=%d", a.dim_x, a.dim_z, a.fx_model, a.hx_model);
     return BKE_ERR_UNSUPPORTED;
 }
 
@@ -69,26 +47,6 @@ int init_dispatch(const EnkfInitP<T> &p, int n, cudaStream_t s)
 }
 
 }  // namespace
-
-// checks common to bke_enkf_step and bke_enkf_step_model
-int validate_enkf(const bke_enkf_args &a)
-{
-    if (a.n_filters < 0 || a.dim_x < 1 || a.dim_x > 16 || a.dim_z < 1) { set_error("bad dimensions (1 <= dim_x <= 16, 1 <= dim_z)"); return BKE_ERR_BAD_ARG; }
-    if (a.n_members < 2) { set_error("n_members must be 2 or greater (the covariances divide by n_members - 1)"); return BKE_ERR_BAD_ARG; }
-    if (a.dtype != BKE_F32 && a.dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
-    if (!(a.flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
-    if (a.flags & ~(BKE_DO_PREDICT | BKE_DO_UPDATE)) { set_error("flags: only BKE_DO_PREDICT and BKE_DO_UPDATE apply to the EnKF"); return BKE_ERR_BAD_ARG; }
-    if (!a.x || !a.P || !a.x_out || !a.P_out) { set_error("x, P, x_out, P_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    if (!a.sigmas || !a.sigmas_out) { set_error("sigmas and sigmas_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    if ((a.flags & BKE_DO_PREDICT) && !a.Q) { set_error("predict needs Q"); return BKE_ERR_BAD_ARG; }
-    if ((a.flags & BKE_DO_UPDATE) && (!a.R || !a.z)) { set_error("update needs R and z"); return BKE_ERR_BAD_ARG; }
-    if (a.Q_stride < 0 || a.R_stride < 0 || a.F_stride < 0 || a.H_stride < 0) { set_error("negative model stride"); return BKE_ERR_BAD_ARG; }
-    if (a.fx_model == BKE_FX_LINEAR && (a.flags & BKE_DO_PREDICT) && !a.F) { set_error("BKE_FX_LINEAR needs F"); return BKE_ERR_BAD_ARG; }
-    if (a.hx_model == BKE_HX_LINEAR && (a.flags & BKE_DO_UPDATE) && !a.H) { set_error("BKE_HX_LINEAR needs H"); return BKE_ERR_BAD_ARG; }
-    if (a.fx_model == BKE_FX_CONST_VEL && (a.dim_x & 1)) { set_error("BKE_FX_CONST_VEL needs an even dim_x"); return BKE_ERR_BAD_ARG; }
-    if (a.n_members > (1 << 24)) { set_error("n_members must be at most 2^24"); return BKE_ERR_BAD_ARG; }
-    return BKE_OK;
-}
 
 int launch_enkf(const bke_enkf_args &a, cudaStream_t s)
 {

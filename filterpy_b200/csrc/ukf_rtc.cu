@@ -24,9 +24,7 @@
 #include <string.h>
 #include <string>
 #include <vector>
-#include "ckf_launch.cuh"
-#include "enkf_launch.cuh"
-#include "ukf_launch.cuh"
+#include "sigma_launch.cuh"
 #include "ukf_rts_launch.cuh"
 
 // the filter family a compiled model's kernels belong to
@@ -107,17 +105,10 @@ int launch_model(const bke_ukf_args &a, const bke_ukf_model &m, const void *fx_a
 {
     ukfk::UkfP<T> p;
     ukf_fill_params<T>(a, m.n, p);
-    p.fx_args = (const T *)fx_args; p.s_fx_args = s_fx;
-    p.hx_args = (const T *)hx_args; p.s_hx_args = s_hx;
+    set_user_args<T>(p, fx_args, s_fx, hx_args, s_hx);
     const size_t smem = ukf_smem_bytes<T>(m.n, m.m, m.simplex ? m.n + 1 : 2 * m.n + 1, m.fx_model == BKE_FX_LINEAR, a.F_stride == 0,
                                           m.hx_model == BKE_HX_LINEAR, a.H_stride == 0);
-    const bool ex = a.x_prior || a.P_prior || a.K || a.y || a.S || a.SI || a.log_likelihood;
-    const void *kern = (const void *)m.kern[ex ? 1 : 0];
-    if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
-    const int64_t grid = (p.N + ukfk::UB - 1) / ukfk::UB;
-    void *params[] = {&p};
-    if (check_cuda(cudaLaunchKernel(kern, dim3((unsigned)grid), dim3(ukfk::UB), params, smem, s), "ukf model launch")) return BKE_ERR_CUDA;
-    return BKE_OK;
+    return launch_kernel((const void *)m.kern[has_extras(a)], ukf_grid(p.N), ukfk::UB, smem, &p, s, "ukf model launch");
 }
 
 template <typename T>
@@ -126,15 +117,10 @@ int launch_ckf_model(const bke_ckf_args &a, const bke_ukf_model &m, const void *
 {
     ckfk::CkfP<T> p;
     ckf_fill_params<T>(a, p);
-    p.fx_args = (const T *)fx_args; p.s_fx_args = s_fx;
-    p.hx_args = (const T *)hx_args; p.s_hx_args = s_hx;
-    const size_t smem = ckf_smem_bytes<T>(m.n, m.m, m.fx_model == BKE_FX_LINEAR, a.F_stride == 0, m.hx_model == BKE_HX_LINEAR, a.H_stride == 0);
-    const void *kern = (const void *)m.kern[ckf_has_extras(a) ? 1 : 0];
-    if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
-    const int64_t grid = (p.N + ukfk::UB - 1) / ukfk::UB;
-    void *params[] = {&p};
-    if (check_cuda(cudaLaunchKernel(kern, dim3((unsigned)grid), dim3(ukfk::UB), params, smem, s), "ckf model launch")) return BKE_ERR_CUDA;
-    return BKE_OK;
+    set_user_args<T>(p, fx_args, s_fx, hx_args, s_hx);
+    const size_t smem = ukf_smem_bytes<T>(m.n, m.m, 2 * m.n, m.fx_model == BKE_FX_LINEAR, a.F_stride == 0, m.hx_model == BKE_HX_LINEAR,
+                                          a.H_stride == 0);
+    return launch_kernel((const void *)m.kern[has_extras(a)], ukf_grid(p.N), ukfk::UB, smem, &p, s, "ckf model launch");
 }
 
 template <typename T>
@@ -143,14 +129,28 @@ int launch_enkf_model(const bke_enkf_args &a, const bke_ukf_model &m, const void
 {
     enkfk::EnkfP<T> p;
     enkf_fill_params<T>(a, p);
-    p.fx_args = (const T *)fx_args; p.s_fx_args = s_fx;
-    p.hx_args = (const T *)hx_args; p.s_hx_args = s_hx;
+    set_user_args<T>(p, fx_args, s_fx, hx_args, s_hx);
     const size_t smem = enkf_smem_bytes(m.n, a.n_members, sizeof(T));
-    const void *kern = (const void *)m.kern[enkf_has_extras(a) ? 1 : 0];
-    if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
-    void *params[] = {&p};
-    if (check_cuda(cudaLaunchKernel(kern, dim3(enkf_grid(p.N)), dim3(enkfk::EB), params, smem, s), "enkf model launch")) return BKE_ERR_CUDA;
-    return BKE_OK;
+    return launch_kernel((const void *)m.kern[enkf_has_extras(a)], enkf_grid(p.N), enkfk::EB, smem, &p, s, "enkf model launch");
+}
+
+// a *_model step refuses a handle compiled for another family, naming the one it was compiled for
+int check_family(const bke_ukf_model &m, int family, const char *fn)
+{
+    static const char *const name[] = {"UKF (bke_ukf_model_compile)", "CKF (bke_ckf_model_compile)", "EnKF (bke_enkf_model_compile)"};
+    if (m.family == family) return BKE_OK;
+    set_error("%s: the model was compiled for the %s", fn, name[m.family]);
+    return BKE_ERR_BAD_ARG;
+}
+
+// the compiled model's shape, element type and models against the step's args
+template <typename Args>
+int check_match(const Args &a, const bke_ukf_model &m, const char *fn)
+{
+    if (a.dim_x == m.n && a.dim_z == m.m && a.dtype == m.dtype && a.fx_model == m.fx_model && a.hx_model == m.hx_model) return BKE_OK;
+    set_error("%s: args (dim_x=%d dim_z=%d dtype=%d fx=%d hx=%d) do not match the compiled model (%d %d %d %d %d)", fn, a.dim_x, a.dim_z,
+              a.dtype, a.fx_model, a.hx_model, m.n, m.m, m.dtype, m.fx_model, m.hx_model);
+    return BKE_ERR_BAD_ARG;
 }
 
 }  // namespace
@@ -417,20 +417,10 @@ int bke_ukf_step_model(const bke_ukf_args *args, const bke_ukf_model *model, con
 {
     if (!args || !model) { set_error("args / model is NULL"); return BKE_ERR_BAD_ARG; }
     const bke_ukf_args &a = *args;
-    if (model->family != BKE_FAMILY_UKF) { set_error("bke_ukf_step_model: the model was compiled for the CKF (bke_ckf_model_compile)"); return BKE_ERR_BAD_ARG; }
-    if (a.dim_x != model->n || a.dim_z != model->m || a.dtype != model->dtype || a.fx_model != model->fx_model || a.hx_model != model->hx_model) {
-        set_error("bke_ukf_step_model: args (dim_x=%d dim_z=%d dtype=%d fx=%d hx=%d) do not match the compiled model (%d %d %d %d %d)",
-                  a.dim_x, a.dim_z, a.dtype, a.fx_model, a.hx_model, model->n, model->m, model->dtype, model->fx_model, model->hx_model);
-        return BKE_ERR_BAD_ARG;
-    }
-    if (a.n_filters < 0) { set_error("bad dimensions"); return BKE_ERR_BAD_ARG; }
-    if (!(a.flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
-    if (!a.x || !a.P || !a.x_out || !a.P_out) { set_error("x, P, x_out, P_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    if ((a.flags & BKE_DO_PREDICT) && !a.Q) { set_error("predict needs Q"); return BKE_ERR_BAD_ARG; }
-    if ((a.flags & BKE_DO_UPDATE) && (!a.R || !a.z)) { set_error("update needs R and z"); return BKE_ERR_BAD_ARG; }
-    if (a.fx_model == BKE_FX_LINEAR && (a.flags & BKE_DO_PREDICT) && !a.F) { set_error("BKE_FX_LINEAR needs F"); return BKE_ERR_BAD_ARG; }
-    if (a.hx_model == BKE_HX_LINEAR && (a.flags & BKE_DO_UPDATE) && !a.H) { set_error("BKE_HX_LINEAR needs H"); return BKE_ERR_BAD_ARG; }
-    if (a.fx_model == BKE_FX_CONST_VEL && (a.dim_x & 1)) { set_error("BKE_FX_CONST_VEL needs an even dim_x"); return BKE_ERR_BAD_ARG; }
+    int rc;
+    if ((rc = check_family(*model, BKE_FAMILY_UKF, "bke_ukf_step_model")) || (rc = check_match(a, *model, "bke_ukf_step_model")) ||
+        (rc = validate_ukf(a)))
+        return rc;
     if (fx_args_stride < 0 || hx_args_stride < 0) { set_error("negative args stride"); return BKE_ERR_BAD_ARG; }
     const bool spx = (a.flags & BKE_UKF_SIMPLEX) != 0;
     if (spx != model->simplex) {
@@ -438,8 +428,6 @@ int bke_ukf_step_model(const bke_ukf_args *args, const bke_ukf_model *model, con
                   model->simplex ? "simplex" : "Merwe", spx ? "simplex" : "Merwe");
         return BKE_ERR_BAD_ARG;
     }
-    const double lam_n = a.alpha * a.alpha * (a.dim_x + a.kappa);
-    if (!spx && !(lam_n != 0.0)) { set_error("alpha^2 (n + kappa) must be non-zero"); return BKE_ERR_BAD_ARG; }
     if (a.n_filters == 0) return BKE_OK;
     return a.dtype == BKE_F32 ? launch_model<float>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream)
                               : launch_model<double>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream);
@@ -450,7 +438,8 @@ int bke_ukf_rts_smoother_model(const bke_ukf_rts_args *args, const bke_ukf_model
 {
     if (!args || !model) { set_error("args / model is NULL"); return BKE_ERR_BAD_ARG; }
     const bke_ukf_rts_args &a = *args;
-    if (model->family != BKE_FAMILY_UKF) { set_error("bke_ukf_rts_smoother_model: the model was compiled for the CKF (bke_ckf_model_compile)"); return BKE_ERR_BAD_ARG; }
+    int rc = check_family(*model, BKE_FAMILY_UKF, "bke_ukf_rts_smoother_model");
+    if (rc) return rc;
     if (!model->kern_rts) { set_error("bke_ukf_rts_smoother_model: the model has neither a user fx nor hooks (use bke_ukf_rts_smoother) or dim_x > %d", UR_MAXN); return BKE_ERR_UNSUPPORTED; }
     if (a.dim_x != model->n || a.dtype != model->dtype || a.fx_model != model->fx_model) { set_error("bke_ukf_rts_smoother_model: args do not match the compiled model"); return BKE_ERR_BAD_ARG; }
     if (((a.flags & BKE_UKF_SIMPLEX) != 0) != model->simplex) {
@@ -477,14 +466,10 @@ int bke_ckf_step_model(const bke_ckf_args *args, const bke_ukf_model *model, con
 {
     if (!args || !model) { set_error("args / model is NULL"); return BKE_ERR_BAD_ARG; }
     const bke_ckf_args &a = *args;
-    if (model->family != BKE_FAMILY_CKF) { set_error("bke_ckf_step_model: the model was compiled for the UKF (bke_ukf_model_compile)"); return BKE_ERR_BAD_ARG; }
-    if (a.dim_x != model->n || a.dim_z != model->m || a.dtype != model->dtype || a.fx_model != model->fx_model || a.hx_model != model->hx_model) {
-        set_error("bke_ckf_step_model: args (dim_x=%d dim_z=%d dtype=%d fx=%d hx=%d) do not match the compiled model (%d %d %d %d %d)",
-                  a.dim_x, a.dim_z, a.dtype, a.fx_model, a.hx_model, model->n, model->m, model->dtype, model->fx_model, model->hx_model);
-        return BKE_ERR_BAD_ARG;
-    }
-    int rc = validate_ckf(a);
-    if (rc) return rc;
+    int rc;
+    if ((rc = check_family(*model, BKE_FAMILY_CKF, "bke_ckf_step_model")) || (rc = check_match(a, *model, "bke_ckf_step_model")) ||
+        (rc = validate_ckf(a)))
+        return rc;
     if (fx_args_stride < 0 || hx_args_stride < 0) { set_error("negative args stride"); return BKE_ERR_BAD_ARG; }
     if (a.n_filters == 0) return BKE_OK;
     return a.dtype == BKE_F32 ? launch_ckf_model<float>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream)
@@ -496,14 +481,10 @@ int bke_enkf_step_model(const bke_enkf_args *args, const bke_ukf_model *model, c
 {
     if (!args || !model) { set_error("args / model is NULL"); return BKE_ERR_BAD_ARG; }
     const bke_enkf_args &a = *args;
-    if (model->family != BKE_FAMILY_ENKF) { set_error("bke_enkf_step_model: the model was not compiled for the EnKF (bke_enkf_model_compile)"); return BKE_ERR_BAD_ARG; }
-    if (a.dim_x != model->n || a.dim_z != model->m || a.dtype != model->dtype || a.fx_model != model->fx_model || a.hx_model != model->hx_model) {
-        set_error("bke_enkf_step_model: args (dim_x=%d dim_z=%d dtype=%d fx=%d hx=%d) do not match the compiled model (%d %d %d %d %d)",
-                  a.dim_x, a.dim_z, a.dtype, a.fx_model, a.hx_model, model->n, model->m, model->dtype, model->fx_model, model->hx_model);
-        return BKE_ERR_BAD_ARG;
-    }
-    int rc = validate_enkf(a);
-    if (rc) return rc;
+    int rc;
+    if ((rc = check_family(*model, BKE_FAMILY_ENKF, "bke_enkf_step_model")) || (rc = check_match(a, *model, "bke_enkf_step_model")) ||
+        (rc = validate_enkf(a)))
+        return rc;
     if (fx_args_stride < 0 || hx_args_stride < 0) { set_error("negative args stride"); return BKE_ERR_BAD_ARG; }
     if (a.n_filters == 0) return BKE_OK;
     return a.dtype == BKE_F32 ? launch_enkf_model<float>(a, *model, fx_args, fx_args_stride, hx_args, hx_args_stride, (cudaStream_t)stream)

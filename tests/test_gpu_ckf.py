@@ -183,9 +183,10 @@ def test_ukf_and_ckf_handles_do_not_mix():
     from filterpy_b200.common import workloads as wl
     lib = _lib.load()
     inc = _lib.kernel_include_dirs().encode()
-    hu, hc = ctypes.c_void_p(), ctypes.c_void_p()
+    hu, hc, he = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
     _lib.check(lib.bke_ukf_model_compile(4, 2, 1, _lib.BKE_FX_USER, _lib.BKE_HX_LINEAR, wl.CT_FX_SOURCE.encode(), inc, ctypes.byref(hu)))
     _lib.check(lib.bke_ckf_model_compile(4, 2, 1, _lib.BKE_FX_USER, _lib.BKE_HX_LINEAR, wl.CT_FX_SOURCE.encode(), inc, ctypes.byref(hc)))
+    _lib.check(lib.bke_enkf_model_compile(4, 2, 1, _lib.BKE_FX_USER, _lib.BKE_HX_LINEAR, wl.CT_FX_SOURCE.encode(), inc, ctypes.byref(he)))
     N = 4
     t = {k: torch.zeros(s, dtype=torch.float64, device="cuda") for k, s in
          dict(x=(N, 4), P=(N, 4, 4), Q=(4, 4), R=(2, 2), H=(2, 4), z=(N, 2), sf=(N, 8, 4), args=(1,)).items()}
@@ -199,9 +200,13 @@ def test_ukf_and_ckf_handles_do_not_mix():
         if cls is _lib.UkfArgs:
             a.alpha, a.beta, a.kappa = 0.5, 2.0, 0.0
             rc = lib.bke_ukf_step_model(a, hc, t["args"].data_ptr(), 0, None, 0, None)
+            assert rc == _lib.BKE_ERR_BAD_ARG and b"compiled for the CKF" in lib.bke_last_error(), rc
+            rc = lib.bke_ukf_step_model(a, he, t["args"].data_ptr(), 0, None, 0, None)
+            assert b"compiled for the EnKF" in lib.bke_last_error()        # the family the handle was compiled for
         else:
             a.sigmas_f = t["sf"].data_ptr()
             rc = lib.bke_ckf_step_model(a, hu, t["args"].data_ptr(), 0, None, 0, None)
+            assert b"compiled for the UKF" in lib.bke_last_error()
         assert rc == _lib.BKE_ERR_BAD_ARG, rc
     a = _lib.CkfArgs()
     a.n_filters, a.dim_x, a.dim_z, a.dtype, a.flags = N, 4, 2, 1, _lib.BKE_DO_UPDATE
@@ -209,4 +214,4 @@ def test_ukf_and_ckf_handles_do_not_mix():
     a.x = a.x_out = t["x"].data_ptr(); a.P = a.P_out = t["P"].data_ptr()
     a.R, a.H, a.z = t["R"].data_ptr(), t["H"].data_ptr(), t["z"].data_ptr()
     assert lib.bke_ckf_step(a, None) == _lib.BKE_ERR_BAD_ARG             # update-only without sigmas_f
-    lib.bke_ukf_model_free(hu); lib.bke_ukf_model_free(hc)
+    lib.bke_ukf_model_free(hu); lib.bke_ukf_model_free(hc); lib.bke_ukf_model_free(he)

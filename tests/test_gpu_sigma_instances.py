@@ -41,16 +41,20 @@ INSTANCES = [
 INSTANCE_IDS = ["%d_%d_%s_%s" % (n, m, fx.lower(), hx.lower()) for n, m, fx, hx in INSTANCES]
 
 
-@pytest.mark.parametrize("src,macro", [("ukf.cu", "BKE_UKF"), ("ckf.cu", "BKE_CKF")])
-def test_instance_list_matches_dispatch_table(src, macro):
-    """INSTANCES is the dispatch table of ukf.cu / ckf.cu: an instance added there without being added to the
-    tests below fails here, on a machine without a GPU too."""
+@pytest.mark.parametrize("src", ["ukf.cu", "ukf_simplex.cu", "ckf.cu", "enkf.cu"])
+def test_instance_table_is_the_dispatch_table(src):
+    """INSTANCES is BKE_SIGMA_INSTANCES (sigma_launch.cuh), the one table from which ukf.cu, ckf.cu and enkf.cu
+    dispatch and ukf_simplex.cu instantiates: an instance added there without being added to the tests below
+    fails here, on a machine without a GPU too, and so does a row written into one of the four files by hand."""
+    with open(os.path.join(CSRC, "sigma_launch.cuh")) as fh:
+        table = re.search(r"#define BKE_SIGMA_INSTANCES\(X\)((?:.*\\\n)*.*)", fh.read()).group(1)
+    row = r"\w+\(\s*(\d+)\s*,\s*(\d+)\s*,\s*BKE_FX_(\w+)\s*,\s*BKE_HX_(\w+)\s*\)"
+    got = [(int(n), int(m), fx, hx) for n, m, fx, hx in re.findall(row, table)]
+    assert got == INSTANCES
     with open(os.path.join(CSRC, src)) as fh:
         text = fh.read()
-    pat = r"^\s*%s\(\s*(\d+)\s*,\s*(\d+)\s*,\s*BKE_FX_(\w+)\s*,\s*BKE_HX_(\w+)\s*\)" % macro
-    got = [(int(n), int(m), fx, hx) for n, m, fx, hx in re.findall(pat, text, re.M)]
-    assert got == INSTANCES
-    assert len(re.findall(r"\b%s\(" % macro, text)) == len(INSTANCES) + 1       # + the #define: no other form
+    assert re.search(r"^\s*BKE_SIGMA_INSTANCES\(\w+\)", text, re.M)
+    assert not re.findall(row, text)                 # no hand-written row next to the table
 
 
 # ----------------------------------------------------------------------------------------------- problems
