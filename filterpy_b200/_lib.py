@@ -47,6 +47,8 @@ EXPORTED_SYMBOLS = [
     "bke_multinomial_resample_bank_workspace_bytes", "bke_multinomial_resample_bank",
     "bke_residual_resample_bank_workspace_bytes", "bke_residual_resample_bank_prepare",
     "bke_residual_resample_bank_search",
+    "bke_resample_bank_gated_workspace_bytes", "bke_resample_bank_gated", "bke_resample_bank_gated_stats",
+    "bke_resample_bank_gated_apply",
     "bke_residual_workspace_bytes", "bke_residual_prepare", "bke_searchsorted_bracket_sweep",
 ]
 
@@ -229,6 +231,17 @@ class ResampleBankArgs(ctypes.Structure):
         ("n_sets", c_int64), ("n_particles", c_int64),
         ("weights", c_void_p), ("u", c_void_p), ("uniforms", c_void_p),
         ("indexes", c_void_p), ("status", c_void_p),
+    ]
+
+
+class ResampleBankGatedArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_sets", c_int64), ("n_particles", c_int64),
+        ("weights", c_void_p), ("u", c_void_p), ("uniforms", c_void_p),
+        ("threshold", ctypes.c_double),
+        ("particles", c_void_p), ("particle_bytes", c_int64),
+        ("indexes", c_void_p), ("neff", c_void_p), ("resampled", c_void_p), ("status", c_void_p),
+        ("workspace", c_void_p), ("workspace_bytes", c_size_t),
     ]
 
 
@@ -492,6 +505,11 @@ def load():
         getattr(lib, name).restype = c_size_t
     lib.bke_multinomial_resample_bank.argtypes = [ctypes.POINTER(MultinomialResampleBankArgs), c_void_p]
     lib.bke_multinomial_resample_bank.restype = ctypes.c_int
+    lib.bke_resample_bank_gated_workspace_bytes.argtypes = [c_int64]
+    lib.bke_resample_bank_gated_workspace_bytes.restype = c_size_t
+    for name in ("bke_resample_bank_gated", "bke_resample_bank_gated_stats", "bke_resample_bank_gated_apply"):
+        getattr(lib, name).argtypes = [ctypes.POINTER(ResampleBankGatedArgs), c_void_p]
+        getattr(lib, name).restype = ctypes.c_int
     for name in ("bke_residual_resample_bank_prepare", "bke_residual_resample_bank_search"):
         getattr(lib, name).argtypes = [ctypes.POINTER(ResidualResampleBankArgs), c_void_p]
         getattr(lib, name).restype = ctypes.c_int

@@ -40,6 +40,8 @@
 //                    previous round's last key and answer, which are final), until a sweep changes no lane.
 //                    After t sweeps the first t lanes are final, so a round takes at most 33 sweeps; on
 //                    residual's sets two or three are typical.
+#include <type_traits>
+
 #include "bke_internal.cuh"
 #include "residual_rules.cuh"
 
@@ -63,15 +65,26 @@ struct Shared {
     int load_w[ROWS], load_p[ROWS];
 };
 
-template <bool STRAT>
+// The CTA's sets are b0 .. b0 + ROWS - 1, or, with a RowList, list.rows[b0 ..] of the *list.count listed sets
+// (the gated epoch below resamples only those).  NoList is an empty trailing argument, so the plain
+// instances keep their parameter offsets and their code.
+struct NoList {};
+struct RowList { const int *rows; const int *count; };
+
+template <bool STRAT, typename L = NoList>
 __global__ void __launch_bounds__(ROWS) k_resample_bank(i64 n_sets, i64 M, const double *__restrict__ w,
                                                         const double *__restrict__ u, const double *__restrict__ U,
-                                                        int *__restrict__ idx, int *__restrict__ status)
+                                                        int *__restrict__ idx, int *__restrict__ status, L list = L())
 {
+    constexpr bool LISTED = std::is_same<L, RowList>::value;
     __shared__ Shared sh;
     const int r = threadIdx.x;
     const i64 b0 = (i64)blockIdx.x * ROWS;
-    const i64 rem = n_sets - b0;
+    i64 rem = n_sets - b0;
+    if constexpr (LISTED) {
+        rem = (i64)*list.count - b0;
+        if (rem <= 0) return;                     // the whole CTA: past the listed sets
+    }
     const int rows = rem < ROWS ? (int)rem : ROWS;
     const double Md = (double)M;
 
@@ -80,9 +93,11 @@ __global__ void __launch_bounds__(ROWS) k_resample_bank(i64 n_sets, i64 M, const
     int ii = 0, jj = 0;             // merge pointers within the windows: i = ki + ii, j = kj + jj
     double c = 0.0;                 // cumsum(w)[j]
     bool fresh_w = true;            // the weight window was just loaded: c still lacks w[kj]
+    i64 set = 0;                    // the listed set of this thread (plain instances: b0 + r)
+    if constexpr (LISTED) set = active ? (i64)list.rows[b0 + r] : 0;
     sh.kj[r] = 0; sh.ki[r] = 0; sh.fbase[r] = 0; sh.nflush[r] = 0;
     sh.load_w[r] = active; sh.load_p[r] = active;
-    sh.u[r] = (!STRAT && active) ? u[b0 + r] : 0.0;
+    sh.u[r] = (!STRAT && active) ? u[LISTED ? set : b0 + r] : 0.0;
     bool more = active;
 
     while (__syncthreads_or(more)) {
@@ -90,7 +105,9 @@ __global__ void __launch_bounds__(ROWS) k_resample_bank(i64 n_sets, i64 M, const
 #pragma unroll 4
         for (int e = r; e < ROWS * COLS; e += ROWS) {
             const int q = e / COLS, t = e % COLS;
-            const i64 row = (b0 + q) * M;
+            i64 qset = b0 + q;
+            if constexpr (LISTED) qset = q < rows ? (i64)list.rows[b0 + q] : 0;
+            const i64 row = qset * M;
             if (t < sh.nflush[q]) idx[row + (i64)sh.fbase[q] * COLS + t] = sh.out[q][t];
             if (sh.load_w[q]) {
                 const i64 k = (i64)sh.kj[q] * COLS + t;
@@ -130,18 +147,146 @@ __global__ void __launch_bounds__(ROWS) k_resample_bank(i64 n_sets, i64 M, const
                 nflush = ii;
                 if (ki + ii == M) {                           // every position placed
                     active = false;
-                    if (status) status[b0 + r] = 0;
+                    if (status) status[LISTED ? set : b0 + r] = 0;
                 } else { need_p = 1; ki += COLS; ii = 0; }
             } else if (kj + jj == M) {                        // j ran off the end: the reference's IndexError (:145)
                 nflush = ii;
                 active = false;
-                if (status) status[b0 + r] = 1;
+                if (status) status[LISTED ? set : b0 + r] = 1;
             } else { need_w = 1; kj += COLS; jj = 0; fresh_w = true; }
         }
         sh.nflush[r] = nflush; sh.fbase[r] = (int)(fbase / COLS);
         sh.load_w[r] = need_w; sh.kj[r] = (int)(kj / COLS);
         sh.load_p[r] = need_p; sh.ki[r] = (int)(ki / COLS);
         more = active || nflush > 0;
+    }
+}
+
+// ---------------------------------------------------------------------- gated epoch
+// A particle filter's epoch over a bank: normalise every row, take its effective sample size, and resample
+// and gather only the sets below the threshold.  Three launches:
+//   k_gated_stats      one warp per set: S = np.sum(w), w /= S in place, neff = 1 / np.sum(np.square(w)), the
+//                      gate; a gated set appends itself to the row list in the workspace;
+//   k_resample_bank    <STRAT, RowList>: the merge above on the listed sets only, so its rounds are paid per
+//                      resampled set and not per CTA of 64 sets of which a few are live;
+//   k_gather_reset     one CTA per listed set: particles[b] <- particles[b][indexes[b]] through shared
+//                      memory, weights[b] <- 1 / M.
+//
+// np.sum of a contiguous fp64 row is fl(+0.0 + pw(a)), pw NumPy's pairwise_sum (numpy/_core/src/umath/
+// loops_utils.h.src, PW_BLOCKSIZE = 128): n < 8 a sequential sum from 0; n <= 128 eight strided accumulators
+// r[k] += a[i + k], combined ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)), then the n % 8 rest in order; above 128 the
+// sum of the two halves split at n / 2 - (n / 2) % 8.  The tree depends only on M, so the warp walks it
+// uniformly: a leaf is staged in shared memory by coalesced loads, lane k (mod 8) runs accumulator k, a xor
+// butterfly over 1, 2, 4 forms the bracketing above (fp add commutes), and the pending right halves and left
+// sums of the path to the root sit one per lane (the tree is at most 25 deep for M < 2^31).
+constexpr int GW = 8;           // sets per CTA of k_gated_stats, one warp each
+constexpr int PW_BLOCK = 128;   // NumPy's PW_BLOCKSIZE
+
+__device__ __forceinline__ double pw_leaf(const double *s, int n, int lane)
+{
+    if (n < 8) {
+        double r = 0.0;
+        for (int i = 0; i < n; i++) r = __dadd_rn(r, s[i]);
+        return r;
+    }
+    const int k = lane & 7, n8 = n - (n & 7);
+    double r = s[k];
+    for (int i = 8; i < n8; i += 8) r = __dadd_rn(r, s[i + k]);
+    r = __dadd_rn(r, __shfl_xor_sync(FULL, r, 1));
+    r = __dadd_rn(r, __shfl_xor_sync(FULL, r, 2));
+    r = __dadd_rn(r, __shfl_xor_sync(FULL, r, 4));
+    for (int i = n8; i < n; i++) r = __dadd_rn(r, s[i]);
+    return r;
+}
+
+// NORMALISE = false: pw(row).  true: row <- row / S in place, and pw(square(row)).  Every lane returns it.
+template <bool NORMALISE>
+__device__ double pw_row(double *row, int M, double S, double *sm, int lane)
+{
+    int off = 0, n = M, sp = 0;
+    int st_off = 0, st_n = 0;             // stack level `lane`: the right half still to sum
+    bool st_left = false;                 // ... and whether its left half's sum is in st_sum
+    double st_sum = 0.0;
+    for (;;) {
+        while (n > PW_BLOCK) {
+            const int n2 = n / 2 - (n / 2) % 8;
+            if (lane == sp) { st_off = off + n2; st_n = n - n2; st_left = false; }
+            ++sp;
+            n = n2;
+        }
+        for (int i = lane; i < n; i += 32) {
+            double x = row[off + i];
+            if (NORMALISE) {
+                x = __ddiv_rn(x, S);
+                row[off + i] = x;
+                x = __dmul_rn(x, x);
+            }
+            sm[i] = x;
+        }
+        __syncwarp();
+        double v = pw_leaf(sm, n, lane);
+        __syncwarp();
+        for (;;) {
+            if (sp == 0) return v;
+            const int top = sp - 1;
+            if (!__shfl_sync(FULL, st_left, top)) {
+                if (lane == top) { st_left = true; st_sum = v; }
+                off = __shfl_sync(FULL, st_off, top);
+                n = __shfl_sync(FULL, st_n, top);
+                break;
+            }
+            v = __dadd_rn(__shfl_sync(FULL, st_sum, top), v);
+            --sp;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(32 * GW) k_gated_stats(i64 n_sets, int M, double *w, double threshold,
+                                                         double *__restrict__ neff, uint8_t *__restrict__ resampled,
+                                                         int *__restrict__ status, int *count, int *__restrict__ list)
+{
+    __shared__ double sm[GW][PW_BLOCK];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const i64 b = (i64)blockIdx.x * GW + wid;
+    if (b >= n_sets) return;                                  // whole warps leave
+    double *row = w + b * M;
+    const double S = __dadd_rn(0.0, pw_row<false>(row, M, 0.0, sm[wid], lane));
+    const double q = __dadd_rn(0.0, pw_row<true>(row, M, S, sm[wid], lane));
+    const double ne = __ddiv_rn(1.0, q);
+    const bool gate = ne < threshold;
+    if (lane == 0) {
+        neff[b] = ne;
+        resampled[b] = gate;
+        status[b] = 0;
+        if (gate) list[atomicAdd(count, 1)] = (int)b;        // the order only decides which sets share a CTA
+    }
+}
+
+// particles[b] <- particles[b][indexes[b]] and weights[b] <- 1 / M for the listed sets that did not fail; the
+// set's row of M * cpp chunks of V is staged in dynamic shared memory, so the gather runs in place.
+template <typename V>
+__global__ void __launch_bounds__(256) k_gather_reset(int M, int cpp, V *parts, const int *__restrict__ idx,
+                                                      double *w, const int *__restrict__ list, const int *count,
+                                                      const int *__restrict__ status)
+{
+    extern __shared__ uint4 stage_raw[];
+    V *stage = reinterpret_cast<V *>(stage_raw);
+    const int n = *count, total = M * cpp;
+    const double inv = __ddiv_rn(1.0, (double)M);
+    for (int t = blockIdx.x; t < n; t += gridDim.x) {
+        const i64 b = list[t];
+        if (status[b]) continue;                              // the reference raised: keep the row as it is
+        V *row = parts + b * (i64)total;
+        for (int e = threadIdx.x; e < total; e += blockDim.x) stage[e] = row[e];
+        __syncthreads();
+        const int *ir = idx + b * M;
+        for (int e = threadIdx.x; e < total; e += blockDim.x) {
+            const int i = e / cpp, c = e - i * cpp;
+            row[e] = stage[ir[i] * cpp + c];
+        }
+        double *wr = w + b * M;
+        for (int i = threadIdx.x; i < M; i += blockDim.x) wr[i] = inv;
+        __syncthreads();                                      // the next set overwrites the stage
     }
 }
 
@@ -337,6 +482,108 @@ int bke_resample_bank(const bke_resample_bank_args *a, void *stream)
         rsb::k_resample_bank<false><<<(unsigned)blocks, rsb::ROWS, 0, s>>>(a->n_sets, a->n_particles, a->weights, a->u,
                                                                           nullptr, a->indexes, a->status);
     return check_cuda(cudaGetLastError(), "resample bank launch");
+}
+
+size_t bke_resample_bank_gated_workspace_bytes(int64_t n_sets)
+{
+    return n_sets <= 0 ? 0 : 16 + (size_t)n_sets * sizeof(int32_t);      // the counter, padded, then the list
+}
+
+// the checks _stats and _apply share; *done = 1: nothing to compute
+static int gated_check(const bke_resample_bank_gated_args *a, int *done)
+{
+    *done = 0;
+    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    if (a->n_sets < 0 || a->n_particles < 0) { set_error("n_sets and n_particles must be >= 0"); return BKE_ERR_BAD_ARG; }
+    if (a->n_particles >= ((int64_t)1 << 31)) { set_error("n_particles must be < 2^31"); return BKE_ERR_BAD_ARG; }
+    if (a->n_sets >= ((int64_t)1 << 31)) { set_error("n_sets must be < 2^31"); return BKE_ERR_BAD_ARG; }
+    if (a->n_sets == 0 || a->n_particles == 0) { *done = 1; return BKE_OK; }
+    if (!a->weights || !a->neff || !a->resampled || !a->status) {
+        set_error("weights, neff, resampled and status must be non-NULL"); return BKE_ERR_BAD_ARG;
+    }
+    if (!a->workspace || (reinterpret_cast<uintptr_t>(a->workspace) & 3)) {
+        set_error("workspace must be non-NULL and 4-byte aligned"); return BKE_ERR_BAD_ARG;
+    }
+    const size_t need = bke_resample_bank_gated_workspace_bytes(a->n_sets);
+    if (a->workspace_bytes < need) { set_error("workspace too small: %zu < %zu", a->workspace_bytes, need); return BKE_ERR_BAD_ARG; }
+    return BKE_OK;
+}
+
+int bke_resample_bank_gated_stats(const bke_resample_bank_gated_args *a, void *stream)
+{
+    int done, rc = gated_check(a, &done);
+    if (rc != BKE_OK || done) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    int *count = (int *)a->workspace;
+    int *list = (int *)((char *)a->workspace + 16);
+    if (check_cuda(cudaMemsetAsync(count, 0, sizeof(int), s), "gated bank counter reset")) return BKE_ERR_CUDA;
+    const unsigned blocks = (unsigned)((a->n_sets + rsb::GW - 1) / rsb::GW);
+    rsb::k_gated_stats<<<blocks, 32 * rsb::GW, 0, s>>>(a->n_sets, (int)a->n_particles, a->weights, a->threshold,
+                                                       a->neff, a->resampled, a->status, count, list);
+    return check_cuda(cudaGetLastError(), "gated bank statistics launch");
+}
+
+// what _apply needs beyond gated_check, the shared-memory cap last (it asks the device)
+static int gated_apply_check(const bke_resample_bank_gated_args *a)
+{
+    if ((a->u == nullptr) == (a->uniforms == nullptr)) { set_error("give exactly one of u (systematic) and uniforms (stratified)"); return BKE_ERR_BAD_ARG; }
+    if (!a->particles || !a->indexes) { set_error("particles and indexes must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if (a->particle_bytes <= 0) { set_error("particle_bytes must be > 0"); return BKE_ERR_BAD_ARG; }
+    int dev = 0, cap = 0;
+    if (check_cuda(cudaGetDevice(&dev), "cudaGetDevice") ||
+        check_cuda(cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev), "cudaDeviceGetAttribute"))
+        return BKE_ERR_CUDA;
+    if (a->particle_bytes > cap || a->n_particles > cap / a->particle_bytes) {
+        set_error("a set's particle row of %lld x %lld bytes exceeds the %d bytes of shared memory one CTA can stage "
+                  "(the device's opt-in maximum per block)", (long long)a->n_particles, (long long)a->particle_bytes, cap);
+        return BKE_ERR_BAD_ARG;
+    }
+    return BKE_OK;
+}
+
+int bke_resample_bank_gated_apply(const bke_resample_bank_gated_args *a, void *stream)
+{
+    int done, rc = gated_check(a, &done);
+    if (rc != BKE_OK || done) return rc;
+    if ((rc = gated_apply_check(a)) != BKE_OK) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    const rsb::RowList rl{(const int *)((const char *)a->workspace + 16), (const int *)a->workspace};
+    const unsigned blocks = (unsigned)((a->n_sets + rsb::ROWS - 1) / rsb::ROWS);
+    if (a->uniforms)
+        rsb::k_resample_bank<true, rsb::RowList><<<blocks, rsb::ROWS, 0, s>>>(
+            a->n_sets, a->n_particles, a->weights, nullptr, a->uniforms, a->indexes, a->status, rl);
+    else
+        rsb::k_resample_bank<false, rsb::RowList><<<blocks, rsb::ROWS, 0, s>>>(
+            a->n_sets, a->n_particles, a->weights, a->u, nullptr, a->indexes, a->status, rl);
+    if (check_cuda(cudaGetLastError(), "gated bank resample launch")) return BKE_ERR_CUDA;
+
+    const int M = (int)a->n_particles;
+    const uintptr_t al = reinterpret_cast<uintptr_t>(a->particles) | (uintptr_t)a->particle_bytes;
+    const size_t smem = (size_t)a->n_particles * (size_t)a->particle_bytes;
+    const int64_t cap_blocks = (int64_t)sm_count() * 8;
+    const unsigned grid = (unsigned)(a->n_sets < cap_blocks ? a->n_sets : cap_blocks);
+#define BKE_GATHER_RESET(V) do {                                                                             \
+        auto kern = rsb::k_gather_reset<V>;                                                                  \
+        if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),   \
+                       "cudaFuncSetAttribute")) return BKE_ERR_CUDA;                                         \
+        kern<<<grid, 256, smem, s>>>(M, (int)(a->particle_bytes / (int64_t)sizeof(V)), (V *)a->particles,   \
+                                     a->indexes, a->weights, rl.rows, rl.count, a->status);                  \
+    } while (0)
+    if ((al & 15) == 0) BKE_GATHER_RESET(uint4);
+    else if ((al & 7) == 0) BKE_GATHER_RESET(uint2);
+    else if ((al & 3) == 0) BKE_GATHER_RESET(unsigned);
+    else BKE_GATHER_RESET(unsigned char);
+#undef BKE_GATHER_RESET
+    return check_cuda(cudaGetLastError(), "gated bank gather launch");
+}
+
+int bke_resample_bank_gated(const bke_resample_bank_gated_args *a, void *stream)
+{
+    int done, rc = gated_check(a, &done);
+    if (rc != BKE_OK || done) return rc;
+    if ((rc = gated_apply_check(a)) != BKE_OK) return rc;             // before the weights are normalised
+    rc = bke_resample_bank_gated_stats(a, stream);
+    return rc != BKE_OK ? rc : bke_resample_bank_gated_apply(a, stream);
 }
 
 size_t bke_multinomial_resample_bank_workspace_bytes(int64_t n_sets, int64_t n_particles)

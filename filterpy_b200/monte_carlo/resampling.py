@@ -20,7 +20,8 @@ from .._dev import require_cuda, stream_ptr
 __all__ = ["systematic_resample", "stratified_resample", "multinomial_resample", "residual_resample",
            "gather_particles", "exact_cumsum", "ResamplePlan", "normalize_weights",
            "residual_resample_with_uniforms", "systematic_resample_bank", "stratified_resample_bank",
-           "gather_particles_bank", "BankResamplePlan", "multinomial_resample_bank", "residual_resample_bank"]
+           "gather_particles_bank", "BankResamplePlan", "multinomial_resample_bank", "residual_resample_bank",
+           "systematic_resample_bank_if_degenerate", "stratified_resample_bank_if_degenerate"]
 
 
 class ResamplePlan(object):
@@ -342,6 +343,7 @@ class BankResamplePlan(object):
         self.n_copies = torch.zeros(self.n_sets, dtype=torch.int64, device=self.device)
         self._ws = None
         self._idx64 = None
+        self._neff = None                                 # resample_if_degenerate's buffers, made on first use
 
     def _workspace(self):
         if self._ws is None:
@@ -441,6 +443,67 @@ class BankResamplePlan(object):
             raise ValueError("particles must be a CUDA tensor of shape (%d, %d, ...) on %s"
                              % (self.n_sets, self.n_particles, self.device))
         return _gather_bank(particles, indexes, out, self._err)
+
+    def _gated(self, entry, weights, particles, u, uniforms, threshold):
+        shape = (self.n_sets, self.n_particles)
+        _bank_tensor_check(weights, "weights", (torch.float64,), shape, self.device)
+        if not (isinstance(particles, torch.Tensor) and particles.device == self.device and particles.is_contiguous()
+                and particles.dim() >= 2 and tuple(particles.shape[:2]) == shape):
+            raise ValueError("particles must be a contiguous tensor of shape (%d, %d, ...) on %s"
+                             % (self.n_sets, self.n_particles, self.device))
+        if self._neff is None:
+            nbytes = int(self._lib.bke_resample_bank_gated_workspace_bytes(self.n_sets))
+            self._gated_ws = torch.empty(max((nbytes + 3) // 4, 1), dtype=torch.int32, device=self.device)
+            self._neff = torch.empty(self.n_sets, dtype=torch.float64, device=self.device)
+            self._resampled = torch.zeros(self.n_sets, dtype=torch.bool, device=self.device)
+            if self.n_particles == 0:                     # 1. / np.sum(np.square([])) is inf: nothing resamples
+                self._neff.fill_(float("inf"))
+        a = _lib.ResampleBankGatedArgs()
+        a.n_sets, a.n_particles = self.n_sets, self.n_particles
+        a.weights = weights.data_ptr()
+        a.u = u.data_ptr() if u is not None else None
+        a.uniforms = uniforms.data_ptr() if uniforms is not None else None
+        a.threshold = float(self.n_particles / 2 if threshold is None else threshold)
+        a.particles = particles.data_ptr()
+        a.particle_bytes = (particles.numel() // max(self.n_sets * self.n_particles, 1)) * particles.element_size()
+        a.indexes, a.status = self.indexes.data_ptr(), self.status.data_ptr()
+        a.neff, a.resampled = self._neff.data_ptr(), self._resampled.data_ptr()
+        a.workspace, a.workspace_bytes = self._gated_ws.data_ptr(), self._gated_ws.numel() * 4
+        try:
+            with torch.cuda.device(self.device):
+                _lib.check(entry(ctypes.byref(a), stream_ptr(self.device)))
+        except ValueError as e:
+            if "shared memory" in str(e):
+                raise ValueError("%s; resample larger sets with systematic / stratified and gather_particles_bank"
+                                 % e) from None
+            raise
+        return self._resampled, self._neff
+
+    def resample_if_degenerate(self, weights, particles, u=None, uniforms=None, threshold=None):
+        """One particle-filter epoch of every set, resampling only the degenerate ones, in place:
+
+        ``w = w / np.sum(w)``; ``neff = 1. / np.sum(np.square(w))``; where ``neff < threshold`` (default
+        ``n_particles / 2``), ``particles[b] = particles[b][systematic_resample(w)]`` for the offset ``u[b]``
+        (``stratified_resample`` for ``uniforms[b]``) and ``w = 1 / n_particles``.  The sums are NumPy's
+        pairwise sums, so the weights, ``neff`` and the decisions are those of NumPy bit for bit.
+
+        ``weights`` float64 [n_sets, n_particles] and ``particles`` (n_sets, n_particles, ...) of any dtype
+        are updated in place; give exactly one of ``u`` float64 [n_sets] and ``uniforms`` float64
+        [n_sets, n_particles] (only the rows of resampled sets are read).  Returns the plan's
+        ``(resampled bool [n_sets], neff float64 [n_sets])``; ``indexes`` holds the resampled rows' indexes
+        and ``status`` is 1 where a resampled set's positions ran past its cumulative sum (the reference's
+        IndexError): that set keeps its particles and its normalised weights.
+
+        One set's particle row must fit in one CTA's shared memory (227 KB on the H100).  The first call
+        allocates the plan's buffers; later calls allocate nothing and do not synchronise the host, so they
+        can be captured in a CUDA graph."""
+        if u is not None:
+            _bank_tensor_check(u, "u", (torch.float64,), (self.n_sets,), self.device)
+        if uniforms is not None:
+            _bank_tensor_check(uniforms, "uniforms", (torch.float64,), (self.n_sets, self.n_particles), self.device)
+        if (u is None) == (uniforms is None):
+            raise ValueError("give exactly one of u (systematic) and uniforms (stratified)")
+        return self._gated(self._lib.bke_resample_bank_gated, weights, particles, u, uniforms, threshold)
 
     def raise_if_overflow(self):
         """IndexError naming the first set whose positions ran past its cumulative sum (host sync)."""
@@ -542,6 +605,73 @@ def residual_resample_bank(weights):
     U[keep] = torch.from_numpy(np.ascontiguousarray(draw)).to(dev)     # row b's M - k_b draws, in row order
     idx = plan.residual_search(U)
     return idx if is_torch else idx.cpu().numpy()
+
+
+def _run_bank_if_degenerate(weights, particles, threshold, stratified):
+    w_dev = isinstance(weights, torch.Tensor) and weights.is_cuda
+    p_dev = isinstance(particles, torch.Tensor) and particles.is_cuda
+    if w_dev != p_dev:
+        raise ValueError("weights and particles must both be CUDA tensors or both be arrays")
+    if w_dev:
+        w, p, dev = weights, particles, weights.device
+        if not (w.dtype == torch.float64 and w.is_contiguous() and p.is_contiguous() and p.device == dev):
+            raise ValueError("weights must be a contiguous float64 CUDA tensor and particles a contiguous tensor on "
+                             "its device (both are updated in place)")
+    else:
+        if not (isinstance(weights, np.ndarray) and weights.dtype == np.float64 and isinstance(particles, np.ndarray)):
+            raise ValueError("weights must be a float64 ndarray and particles an ndarray (both are updated in place)")
+        dev = require_cuda(None)
+        w = torch.from_numpy(np.ascontiguousarray(weights)).to(dev)
+        p = torch.from_numpy(np.ascontiguousarray(particles)).to(dev)
+    if w.dim() != 2 or p.dim() < 2 or tuple(p.shape[:2]) != tuple(w.shape):
+        raise ValueError("weights must be (n_sets, n_particles) and particles (n_sets, n_particles, ...)")
+    B, M = w.shape
+    plan = BankResamplePlan(B, M, dev)
+    resampled, neff = plan._gated(plan._lib.bke_resample_bank_gated_stats, w, p, None, None, threshold)
+    mask = resampled.cpu().numpy()
+    n_res = int(mask.sum())
+    # the loop draws random() (stratified: random(M)) for each set it resamples, in row order; one draw of
+    # random(n_res) (random((n_res, M))) takes the same values and leaves the stream in the same place
+    draw = random((n_res, M)) if stratified else random(n_res)
+    if n_res:
+        rows = torch.from_numpy(np.flatnonzero(mask)).to(dev)
+        U = torch.zeros((B, M) if stratified else (B,), dtype=torch.float64, device=dev)
+        U[rows] = torch.from_numpy(np.ascontiguousarray(draw)).to(dev)
+        plan._gated(plan._lib.bke_resample_bank_gated_apply, w, p, None if stratified else U,
+                    U if stratified else None, threshold)
+    if not w_dev:
+        np.copyto(weights, w.cpu().numpy())
+        np.copyto(particles, p.cpu().numpy())
+        resampled, neff = mask, neff.cpu().numpy()
+    if n_res:
+        _raise_first_overflow(plan.status, M)
+    return resampled, neff
+
+
+def systematic_resample_bank_if_degenerate(weights, particles, threshold=None):
+    """A particle filter's resampling step on every set of a bank, where it is due, in place::
+
+        w = w / np.sum(w); neff = 1. / np.sum(np.square(w))
+        if neff < threshold:                 # default n_particles / 2
+            particles[:] = particles[systematic_resample(w)]; w = np.full(M, 1. / M)
+
+    for each row of ``weights[B, M]`` (float64) and ``particles[B, M, ...]`` (any dtype): ndarrays, updated in
+    place, or CUDA tensors, updated in place.  Returns ``(resampled bool[B], neff[B])`` of the same kind.
+    The sums are NumPy's pairwise sums, so every result is that loop's bit for bit.  Seeded with
+    ``np.random.seed``, ``random()`` is drawn for the resampled sets in row order, the values and stream
+    position of the loop: the statistics run first and the mask is read back (one host synchronisation).
+
+    A set whose positions run past its cumulative sum keeps its particles and normalised weights, and
+    ``IndexError`` names the first such set.  By then every row has been processed and drawn for, where the
+    loop would have stopped at that set.  One set's particle row must fit in one CTA's shared memory
+    (227 KB on the H100); ``gather_particles_bank`` serves larger sets."""
+    return _run_bank_if_degenerate(weights, particles, threshold, False)
+
+
+def stratified_resample_bank_if_degenerate(weights, particles, threshold=None):
+    """As ``systematic_resample_bank_if_degenerate`` with ``stratified_resample``: each resampled set draws
+    ``random(M)``, taken for all of them as ``random((n_res, M))``."""
+    return _run_bank_if_degenerate(weights, particles, threshold, True)
 
 
 def _gather_bank(particles, indexes, out, err):

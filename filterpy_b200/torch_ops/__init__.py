@@ -18,6 +18,9 @@ The same symbols exposed as torch.ops.* via a C++ extension for zero-copy CUDA t
     idx  = torch.ops.bke.stratified_resample_bank(weights, uniforms)   # uniforms[B, M]
     idx  = torch.ops.bke.multinomial_resample_bank(weights, uniforms)  # int64, resampling.py:153-176 per row
     idx  = torch.ops.bke.residual_resample_bank(weights, uniforms)     # row b uses uniforms[b, :M - k_b]
+    res, neff = torch.ops.bke.systematic_resample_bank_if_degenerate(weights, particles, u, threshold)
+    res, neff = torch.ops.bke.stratified_resample_bank_if_degenerate(weights, particles, uniforms, threshold)
+                                     # normalise, neff, resample + gather the sets with neff < threshold, in place
 
 Models are shared by the bank when 2-D (stride 0) and per filter when 3-D.  Only the CUDA backend is
 registered: CPU tensors raise ``NotImplementedError`` (no CPU fallback).  The operators run on the

@@ -14,6 +14,10 @@
 //   bke::stratified_resample_bank  bke_resample_bank   resampling.py:80-114 on every row of weights[B, M]
 //   bke::multinomial_resample_bank bke_multinomial_resample_bank       resampling.py:153-176 per row
 //   bke::residual_resample_bank    bke_residual_resample_bank_prepare / _search   resampling.py:27-76 per row
+//   bke::systematic_resample_bank_if_degenerate  bke_resample_bank_gated   normalise, neff, resample + gather where
+//   bke::stratified_resample_bank_if_degenerate  bke_resample_bank_gated   neff < threshold, in place, per row
+#include <limits>
+
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
@@ -346,6 +350,58 @@ at::Tensor residual_resample_bank(const at::Tensor &w, const at::Tensor &U)
     return idx;
 }
 
+// w <- w / np.sum(w), neff = 1 / np.sum(np.square(w)), and where neff < threshold: particles[b] <- particles[b][idx],
+// w <- 1 / M (systematic for u[B], stratified for uniforms[B, M]); weights and particles in place
+std::tuple<at::Tensor, at::Tensor> resample_bank_if_degenerate(const at::Tensor &w, const at::Tensor &parts,
+                                                               const at::Tensor *u, const at::Tensor *U, double threshold)
+{
+    TORCH_CHECK(w.is_cuda() && w.is_contiguous() && w.scalar_type() == at::kDouble && w.dim() == 2, "bke: weights must be a contiguous 2-D float64 CUDA tensor");
+    c10::cuda::CUDAGuard guard(w.device());
+    const int64_t B = w.size(0), M = w.size(1);
+    TORCH_CHECK(parts.is_cuda() && parts.is_contiguous() && parts.device() == w.device() && parts.dim() >= 2 &&
+                parts.size(0) == B && parts.size(1) == M, "bke: particles must be a contiguous CUDA tensor [n_sets, n_particles, ...] on the weights' device");
+    const at::Tensor &r = u ? *u : *U;
+    TORCH_CHECK(r.is_cuda() && r.is_contiguous() && r.scalar_type() == at::kDouble && r.device() == w.device(), "bke: uniforms must be a contiguous float64 CUDA tensor on the weights' device");
+    if (u) {
+        TORCH_CHECK(r.dim() == 1 && r.size(0) == B, "bke: u must be [n_sets]");
+    } else {
+        TORCH_CHECK(r.dim() == 2 && r.size(0) == B && r.size(1) == M, "bke: uniforms must be [n_sets, n_particles]");
+    }
+    at::Tensor resampled = at::zeros({B}, w.options().dtype(at::kBool));
+    at::Tensor neff = at::full({B}, std::numeric_limits<double>::infinity(), w.options());   // M = 0: 1 / sum([]) = inf
+    if (B == 0 || M == 0) return {resampled, neff};
+    at::Tensor idx = at::empty({B, M}, w.options().dtype(at::kInt));
+    at::Tensor status = at::empty({B}, w.options().dtype(at::kInt));
+    const size_t wsb = bke_resample_bank_gated_workspace_bytes(B);
+    at::Tensor ws = at::empty({(int64_t)((wsb + 3) / 4)}, w.options().dtype(at::kInt));
+    bke_resample_bank_gated_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_sets = B; a.n_particles = M; a.weights = (double *)w.data_ptr(); a.threshold = threshold;
+    if (u) a.u = (const double *)r.data_ptr(); else a.uniforms = (const double *)r.data_ptr();
+    a.particles = parts.data_ptr(); a.particle_bytes = parts.numel() / (B * M) * (int64_t)parts.element_size();
+    a.indexes = (int32_t *)idx.data_ptr(); a.neff = (double *)neff.data_ptr();
+    a.resampled = (uint8_t *)resampled.data_ptr(); a.status = (int32_t *)status.data_ptr();
+    a.workspace = ws.data_ptr(); a.workspace_bytes = wsb;
+    check_rc(bke_resample_bank_gated(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_resample_bank_gated");
+    // resampling.py:145: the first resampled row whose positions run past its cumsum is where the loop raises
+    const at::Tensor bad = status.nonzero();
+    TORCH_CHECK_INDEX(bad.numel() == 0, "set ", bad.numel() ? bad[0][0].item<int64_t>() : 0, ": index ", M,
+                      " is out of bounds for axis 0 with size ", M);
+    return {resampled, neff};
+}
+
+std::tuple<at::Tensor, at::Tensor> systematic_resample_bank_if_degenerate(at::Tensor w, at::Tensor parts, const at::Tensor &u,
+                                                                          double threshold)
+{
+    return resample_bank_if_degenerate(w, parts, &u, nullptr, threshold);
+}
+
+std::tuple<at::Tensor, at::Tensor> stratified_resample_bank_if_degenerate(at::Tensor w, at::Tensor parts, const at::Tensor &U,
+                                                                          double threshold)
+{
+    return resample_bank_if_degenerate(w, parts, nullptr, &U, threshold);
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bke, m)
@@ -366,6 +422,10 @@ TORCH_LIBRARY(bke, m)
     m.def("stratified_resample_bank(Tensor weights, Tensor uniforms) -> Tensor");
     m.def("multinomial_resample_bank(Tensor weights, Tensor uniforms) -> Tensor");
     m.def("residual_resample_bank(Tensor weights, Tensor uniforms) -> Tensor");
+    m.def("systematic_resample_bank_if_degenerate(Tensor(a!) weights, Tensor(b!) particles, Tensor u, float threshold) "
+          "-> (Tensor resampled, Tensor neff)");
+    m.def("stratified_resample_bank_if_degenerate(Tensor(a!) weights, Tensor(b!) particles, Tensor uniforms, "
+          "float threshold) -> (Tensor resampled, Tensor neff)");
 }
 
 TORCH_LIBRARY_IMPL(bke, CUDA, m)
@@ -383,4 +443,6 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("stratified_resample_bank", &stratified_resample_bank);
     m.impl("multinomial_resample_bank", &multinomial_resample_bank);
     m.impl("residual_resample_bank", &residual_resample_bank);
+    m.impl("systematic_resample_bank_if_degenerate", &systematic_resample_bank_if_degenerate);
+    m.impl("stratified_resample_bank_if_degenerate", &stratified_resample_bank_if_degenerate);
 }

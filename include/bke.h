@@ -702,6 +702,50 @@ typedef struct bke_resample_bank_args {
 
 int bke_resample_bank(const bke_resample_bank_args *args, void *stream);
 
+/* One particle-filter epoch of a bank, resampling only the sets that degenerated.  For every row b of
+ * weights[n_sets, n_particles] (fp64, dense), independently:
+ *   1. w_b <- w_b / np.sum(w_b), in place, with NumPy's pairwise summation order;
+ *   2. neff[b] = 1. / np.sum(np.square(w_b)) over the normalised row (pairwise again);
+ *   3. resampled[b] = neff[b] < threshold (strict; a NaN neff does not resample);
+ *   4. where resampled[b]: indexes[b] is systematic_resample(w_b) for u[b] or stratified_resample(w_b) for
+ *      uniforms[b], exactly as bke_resample_bank computes it; particles[b] <- particles[b][indexes[b]] in
+ *      place; weights[b] <- 1. / n_particles everywhere;
+ *   5. status[b] = 1 where the positions run past the normalised row's cumsum (the reference's IndexError,
+ *      resampling.py:145): that row keeps its particles and its normalised weights.  Otherwise 0.
+ * Rows that do not resample have their particles neither read nor written, and their indexes are
+ * unspecified.  Give exactly one of u and uniforms; only the rows of resampled sets are read.
+ *
+ * A particle is particle_bytes bytes of any type.  A set's particle row (n_particles * particle_bytes) is
+ * staged in one CTA's shared memory, so it must not exceed the device's opt-in shared memory per block
+ * (227 KB on the H100); a larger row returns BKE_ERR_BAD_ARG.  n_sets < 2^31, n_particles < 2^31;
+ * n_sets = 0 or n_particles = 0 does nothing.
+ *
+ * workspace: bke_resample_bank_gated_workspace_bytes(n_sets) bytes, 4-byte aligned; it holds the list of
+ * sets to resample and its counter.  Three launches and a memset, no allocation, no host sync: the call
+ * can be captured in a CUDA graph.  The two halves are callable on their own, in stream order on the same
+ * args: _stats runs steps 1-3 (u / uniforms are not read, and may both be NULL), _apply runs steps 4-5 on
+ * the sets _stats listed, so a caller can read `resampled` back and draw uniforms only for those sets. */
+typedef struct bke_resample_bank_gated_args {
+    int64_t n_sets, n_particles;
+    double *weights;             /* [n_sets, n_particles] in: raw weights; out: normalised, or 1/M where resampled */
+    const double *u;             /* [n_sets] (systematic) or NULL */
+    const double *uniforms;      /* [n_sets, n_particles] (stratified) or NULL */
+    double threshold;
+    void *particles;             /* [n_sets, n_particles] particles of particle_bytes each, any type; in place */
+    int64_t particle_bytes;
+    int32_t *indexes;            /* [n_sets, n_particles] */
+    double *neff;                /* [n_sets] */
+    uint8_t *resampled;          /* [n_sets], 0 or 1 */
+    int32_t *status;             /* [n_sets] */
+    void *workspace;
+    size_t workspace_bytes;
+} bke_resample_bank_gated_args;
+
+size_t bke_resample_bank_gated_workspace_bytes(int64_t n_sets);
+int bke_resample_bank_gated(const bke_resample_bank_gated_args *args, void *stream);
+int bke_resample_bank_gated_stats(const bke_resample_bank_gated_args *args, void *stream);
+int bke_resample_bank_gated_apply(const bke_resample_bank_gated_args *args, void *stream);
+
 /* multinomial_resample (resampling.py:153-176) of every row of weights[n_sets, n_particles] (fp64, dense):
  *   indexes[b] = np.searchsorted(c_b, uniforms[b]),  c_b = np.cumsum(weights[b]), c_b[-1] = 1
  * bit for bit for ANY values (negative, NaN, infinite, -0.0 and subnormal weights; uniforms outside [0, 1),
