@@ -155,6 +155,7 @@ struct FastP {
     int run_first[REC_RUNS], run_len[REC_RUNS];
     const float *zs[BKE_KF42_MAX_RING];     // RING: the measurements of step k (p.z is not read),
     int n_steps;                            // for k < n_steps
+    int ring_ox, ring_oz, ring_stage;       // RING: the stage laid out for this launch (ring_layout)
 };
 
 // MODE: 3 = predict+update, 1 = predict only, 2 = update only
@@ -167,13 +168,14 @@ struct FastP {
 // rides in the launch parameters.
 // RING (MODE 3, REC 2, no EXTRAS): 0 = one step; BKE_KF42_MAX_RING = the fused ring: each thread loads x, P and
 // the model words once, runs p.n_steps predict+update pairs on the measurements p.zs[0 .. n_steps) back to
-// back in registers and stores x, P once.  A stage then holds one 1 KB measurement block per step
-// (36.5 KB per stage: 2 stages x 3 CTAs = 219 KB of the SM's 227 KB).
+// back in registers and stores x, P once.  Its stage is laid out per launch (ring_layout): P, the record's
+// planes, x and one 1 KB measurement block per step, so a launch stages only what it reads (19 KB per
+// stage for the kf_bank_cv2d template at 4 steps) and up to 4 CTAs, the register limit, fit an SM.
 constexpr int STAGES = 2;
-constexpr int kf42_ctas_per_sm(int shared) { return shared == 2 ? 5 : (shared ? 4 : 3); }
+constexpr int kf42_ctas_per_sm(int shared, int ring = 0) { return ring ? 4 : shared == 2 ? 5 : (shared ? 4 : 3); }
 
 template <int MODE, int SHARED, bool EXTRAS, int REC = 0, int RING = 0>
-__global__ void __launch_bounds__(TILE, kf42_ctas_per_sm(SHARED))
+__global__ void __launch_bounds__(TILE, kf42_ctas_per_sm(SHARED, RING))
 kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 {
     constexpr int N = 4, M = 2;
@@ -190,13 +192,15 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
     __shared__ __align__(8) uint64_t full[STAGES];
 
     const int tid = threadIdx.x;
+    const int stage_bytes = RING ? p.ring_stage : St::BYTES, off_x = RING ? p.ring_ox : St::OX,
+              off_z = RING ? p.ring_oz : St::OZ;
 
     const uint64_t pol_first = policy_evict_first(), pol_last = policy_evict_last();
     // the tile's blocks are contiguous byte ranges; a ragged last tile copies only its own filters
     // (z: 8 B per filter, rounded down to the 16-byte granule; an odd last filter reads its own z)
     // (tile: the bank's tile, not the position in the launch order)
     auto issue = [&](int tile, int stage) {
-        unsigned char *sb = smem + stage * St::BYTES;
+        unsigned char *sb = smem + stage * stage_bytes;
         uint64_t *bar = &full[stage];
         const int64_t f0 = (int64_t)tile * TILE;
         const int64_t left = p.N_filters - f0;
@@ -215,7 +219,7 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
             else bulk_load(sb + off, src + f0 * per_filter, bytes, bar);
         };
         load(St::OP, p.P, N * N, nf * N * N * 4, pol_last);
-        load(St::OX, p.x, N, nf * N * 4, pol_last);
+        load(off_x, p.x, N, nf * N * 4, pol_last);
         if (!SHARED && REC != 2 && DO_P) {
             load(St::OF, p.F, N * N, nf * N * N * 4, pol_first);
             if (!REC) load(St::OQ, p.Q, N * N, nf * N * N * 4, pol_first);
@@ -231,7 +235,7 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
                      p.run_len[r] * TILE * 4, pol_first);
         if (!RING && DO_U && zb) load(St::OZ, p.z, M, zb, pol_first);
         if (RING && zb)
-            for (int k = 0; k < p.n_steps; k++) load(St::OZ + k * St::align_up(St::ZB), p.zs[k], M, zb, pol_first);
+            for (int k = 0; k < p.n_steps; k++) load(off_z + k * St::align_up(St::ZB), p.zs[k], M, zb, pol_first);
     };
 
     // prologue: nothing here touches global memory, so it may overlap the previous launch
@@ -289,12 +293,12 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, it++) {
         const int stage = it % STAGES;
         const uint32_t parity = (it / STAGES) & 1;
-        const unsigned char *sb = smem + stage * St::BYTES;
+        const unsigned char *sb = smem + stage * stage_bytes;
         mbar_wait(&full[stage], parity);
 
         float x[N], P[N][N], z[ZS][M];
         {
-            float4 v = lds_chunk<16>(sb + St::OX, tid, 0);
+            float4 v = lds_chunk<16>(sb + off_x, tid, 0);
             x[0] = v.x; x[1] = v.y; x[2] = v.z; x[3] = v.w;
         }
         lds_row<N>(sb + St::OP, tid, P);
@@ -362,7 +366,7 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
                 float2 v = make_float2(0.f, 0.f);
                 if (k < p.n_steps)
                     v = own ? *reinterpret_cast<const float2 *>(p.zs[k] + f * M)
-                            : *reinterpret_cast<const float2 *>(sb + St::OZ + k * St::align_up(St::ZB) + tid * 8);
+                            : *reinterpret_cast<const float2 *>(sb + off_z + k * St::align_up(St::ZB) + tid * 8);
                 z[k][0] = v.x; z[k][1] = v.y;
             }
         }
@@ -509,15 +513,36 @@ int launch_variant(const FastP<4, 2> &p, cudaStream_t s)
 {
     using St = Stage<float, 4, 2, SHARED != 0, REC, RING ? RING : 1>;
     auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, REC, RING>;
-    const int smem = STAGES * St::BYTES;
+    // (the ring's stage is laid out per launch and never exceeds St::BYTES)
+    const int smem = STAGES * (RING ? p.ring_stage : St::BYTES);
     static bool configured[64] = {false};
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64 || !configured[dev]) {
-        if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
+        if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGES * St::BYTES),
+                       "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
         if (dev >= 0 && dev < 64) configured[dev] = true;
     }
-    int grid = sm_count() * kf42_ctas_per_sm(SHARED);
+    int ctas = kf42_ctas_per_sm(SHARED, RING);
+    if (RING) {
+        // the resident CTAs at this launch's shared memory, per device and stage size (a stage is a whole
+        // number of 512 B units); the first launch of a shape queries it, so a captured launch finds it
+        constexpr int UNITS = STAGES * St::BYTES / 512 + 1;
+        static int resident[64][UNITS] = {};
+        const int unit = smem / 512;
+        int *r = dev >= 0 && dev < 64 && unit < UNITS ? &resident[dev][unit] : nullptr;
+        if (!r || *r == 0) {
+            int n = 0;
+            if (check_cuda(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, TILE, smem), "cudaOccupancyMaxActiveBlocksPerMultiprocessor"))
+                return BKE_ERR_CUDA;
+            if (n < 1) n = 1;
+            if (r) *r = n;
+            ctas = n;
+        } else {
+            ctas = *r;
+        }
+    }
+    int grid = sm_count() * ctas;
     if (grid > p.num_tiles) grid = p.num_tiles;
     // programmatic stream serialization: this launch may start while the previous kernel on the
     // stream drains (the kernel waits with griddepcontrol.wait before it touches memory); under
@@ -936,6 +961,12 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const 
         if (!packed || !all_dense || !(dp && du) || extras || a.z_valid) return BKE_ERR_UNSUPPORTED;
         for (int k = 0; k < n_steps; k++) p.zs[k] = (const float *)zs[k];
         p.n_steps = n_steps;
+        // the stage: P, the record's planes (each copied plane sits at its place in the record), x, and
+        // one measurement block per step
+        using St = Stage<float, 4, 2, false, 2, BKE_KF42_MAX_RING>;
+        p.ring_ox = St::OQ + p.rec_planes * TILE * 4;
+        p.ring_oz = p.ring_ox + St::align_up(St::XB);
+        p.ring_stage = p.ring_oz + n_steps * St::align_up(St::ZB);
         return launch_variant<3, 0, false, 2, BKE_KF42_MAX_RING>(p, s);
     }
 
