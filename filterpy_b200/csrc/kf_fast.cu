@@ -67,6 +67,40 @@ constexpr int SYM_Q_PLANES = 10, SYM_PLANES = 13;
 constexpr int WORDS = BKE_KF42_MODEL_WORDS, W_F = 0, W_Q = 16, W_H = 26, W_R = 34;
 constexpr uint64_t PREDICT_WORDS = (1ull << W_H) - 1;      // F and Q
 constexpr int REC_RUNS = (WORDS + 1) / 2;                  // runs of consecutive planes, at most every other one
+// the word of Q[i][j] (upper triangle, row by row)
+constexpr int q_word(int i, int j)
+{
+    const int r = i < j ? i : j, c = i < j ? j : i;
+    return W_Q + r * 4 - r * (r - 1) / 2 + (c - r);
+}
+
+// The structural words an instance of the fused ring is built for: bit e of ZERO = word e is +0 (bit pattern 0)
+// in every filter, of ONE = word e is 1.0f in every filter.  The ring takes them as constants and drops or
+// folds the products with them (reg_predict_pat, reg_update_pat; F0 .. R0 are those functions' view).
+template <uint64_t Z, uint64_t O>
+struct WordPattern {
+    static constexpr uint64_t ZERO = Z, ONE = O;
+    static constexpr bool any = (ZERO | ONE) != 0;
+    static constexpr bool structural(int e) { return ((Z | O) >> e) & 1; }
+    static constexpr uint32_t F0(int i) { return (uint32_t)(Z >> (W_F + 4 * i)) & 15u; }
+    static constexpr uint32_t F1(int i) { return (uint32_t)(O >> (W_F + 4 * i)) & 15u; }
+    static constexpr uint32_t H0(int a) { return (uint32_t)(Z >> (W_H + 4 * a)) & 15u; }
+    static constexpr uint32_t H1(int a) { return (uint32_t)(O >> (W_H + 4 * a)) & 15u; }
+    static constexpr bool Q0(int i, int j) { return (Z >> q_word(i, j)) & 1; }
+    static constexpr bool R0(int a, int b) { return (Z >> (W_R + a + b)) & 1; }
+};
+// every word as it comes: the generic kernels
+struct NoPattern : WordPattern<0, 0> {};
+// the constant-velocity 2-D model of kf_bank_cv2d: F = I + dt (E01 + E23) (ten +0, four 1 on the diagonal),
+// Q block-diagonal (Q02 Q03 Q12 Q13 +0), H = [e0; e2] (six +0, two 1), R diagonal (R01 +0)
+struct Cv2dPattern : WordPattern<
+    // F 2 3 4 6 7 8 9 12 13 14 | Q02 Q03 Q12 Q13 | H 27 28 29 30 31 33 | R01
+    (1ull << 2) | (1ull << 3) | (1ull << 4) | (1ull << 6) | (1ull << 7) | (1ull << 8) | (1ull << 9) | (1ull << 12) |
+        (1ull << 13) | (1ull << 14) | (1ull << q_word(0, 2)) | (1ull << q_word(0, 3)) | (1ull << q_word(1, 2)) |
+        (1ull << q_word(1, 3)) | (1ull << 27) | (1ull << 28) | (1ull << 29) | (1ull << 30) | (1ull << 31) |
+        (1ull << 33) | (1ull << (W_R + 1)),
+    // F 0 5 10 15 | H 26 32
+    (1ull << 0) | (1ull << 5) | (1ull << 10) | (1ull << 15) | (1ull << 26) | (1ull << 32)> {};
 
 // REC: 0 = dense models, 1 = the packed Q / R record, 2 = the packed model words (stage sized for all 37)
 // ZS: measurement blocks per stage (the fused ring stages one per step)
@@ -174,13 +208,15 @@ struct FastP {
 constexpr int STAGES = 2;
 constexpr int kf42_ctas_per_sm(int shared, int ring = 0) { return ring ? 4 : shared == 2 ? 5 : (shared ? 4 : 3); }
 
-template <int MODE, int SHARED, bool EXTRAS, int REC = 0, int RING = 0>
+// PAT (the fused ring only): the structural words the instance takes as constants (WordPattern)
+template <int MODE, int SHARED, bool EXTRAS, int REC = 0, int RING = 0, class PAT = NoPattern>
 __global__ void __launch_bounds__(TILE, kf42_ctas_per_sm(SHARED, RING))
 kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 {
     constexpr int N = 4, M = 2;
     static_assert(!(REC && SHARED), "the packed records hold per-filter models");
     static_assert(!RING || (MODE == 3 && REC == 2 && !EXTRAS), "the fused ring steps the packed model words");
+    static_assert(!PAT::any || RING, "a pattern instance is a fused ring");
     constexpr int ZS = RING ? RING : 1;
     using St = Stage<float, N, M, SHARED != 0, REC, ZS>;
     // REC == 1: the part of a tile's record this MODE reads (the Q planes, the R planes or both)
@@ -305,9 +341,11 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
         // REC: word `tid` of a plane of the record (no bank conflicts); the lower triangles are the same
         // registers.  REC == 1 holds all 13 Q / R words, in order; REC == 2 the words in p.varying, and
         // the others are the bank's shared values.  (The shared values are run-time parameters, so the
-        // arithmetic is the same instructions as with a dense model: nothing is folded away.)
+        // arithmetic is the same instructions as with a dense model: nothing is folded away.  A pattern
+        // instance's structural words are constants instead, and its arithmetic drops or folds them.)
         const unsigned char *rec = sb + St::OQ + tid * 4;
         auto word = [&](int e, float shared) -> float {
+            if (PAT::structural(e)) return (PAT::ONE >> e) & 1 ? 1.f : 0.f;
             if (REC == 1) return *reinterpret_cast<const float *>(rec + (e < W_H ? e - W_Q : e - W_R + SYM_Q_PLANES) * TILE * 4);
             return (p.varying >> e) & 1 ? *reinterpret_cast<const float *>(rec + p.slot_off[e]) : shared;
         };
@@ -386,24 +424,26 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
             for (int j = 0; j < N; j++) acc ^= __float_as_uint(P[i][j]);
         }
         // (REC: each loaded word once; folding a mirrored pair would cancel it out of the predicate.
-        // REC == 2 folds every model word: a shared one is a launch parameter and harmless in it)
+        // REC == 2 folds every model word: a shared one is a launch parameter and harmless in it; a
+        // structural word of PAT is a constant and is left out)
         if (!SHARED && DO_P) {
 #pragma unroll
             for (int i = 0; i < N; i++)
 #pragma unroll
                 for (int j = 0; j < N; j++) {
-                    acc ^= __float_as_uint(F[i][j]);
-                    if (!REC || j >= i) acc ^= __float_as_uint(Q[i][j]);
+                    if (!PAT::structural(W_F + i * N + j)) acc ^= __float_as_uint(F[i][j]);
+                    if ((!REC || j >= i) && !PAT::structural(q_word(i, j))) acc ^= __float_as_uint(Q[i][j]);
                 }
         }
         if (!SHARED && DO_U) {
 #pragma unroll
             for (int a = 0; a < M; a++) {
 #pragma unroll
-                for (int j = 0; j < N; j++) acc ^= __float_as_uint(H[a][j]);
+                for (int j = 0; j < N; j++)
+                    if (!PAT::structural(W_H + a * N + j)) acc ^= __float_as_uint(H[a][j]);
 #pragma unroll
                 for (int b = 0; b < M; b++)
-                    if (!REC || b >= a) acc ^= __float_as_uint(R[a][b]);
+                    if ((!REC || b >= a) && !PAT::structural(W_R + a + b)) acc ^= __float_as_uint(R[a][b]);
             }
         }
         if (DO_U) {
@@ -423,15 +463,97 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 
         int st = BKE_STATUS_OK;
         if (RING) {
+            // PAT: the structural words' products are dropped, which is exact for finite operands only
+            // (0 Inf is NaN).  nf = the sum of 0 v over every word v the ring reads and every word it writes
+            // is NaN when any of them is not finite; such a filter runs the dense ring again (below).
+            float nf = 0.f;
+            auto check = [&](float v) { nf = __fmaf_rn(0.f, v, nf); };
+            if (PAT::any) {
+                check(p.alpha_sq);
+#pragma unroll
+                for (int i = 0; i < N; i++) {
+                    check(x[i]);
+#pragma unroll
+                    for (int j = 0; j < N; j++) {
+                        check(P[i][j]);
+                        if (!PAT::structural(W_F + i * N + j)) check(F[i][j]);
+                        if (j >= i && !PAT::structural(q_word(i, j))) check(Q[i][j]);
+                    }
+                }
+#pragma unroll
+                for (int a = 0; a < M; a++) {
+#pragma unroll
+                    for (int j = 0; j < N; j++)
+                        if (!PAT::structural(W_H + a * N + j)) check(H[a][j]);
+#pragma unroll
+                    for (int b = a; b < M; b++)
+                        if (!PAT::structural(W_R + a + b)) check(R[a][b]);
+                }
+#pragma unroll
+                for (int k = 0; k < ZS; k++) { check(z[k][0]); check(z[k][1]); }
+            }
             // the steps of the ring, back to back on the registers; the loop stays rolled and the
             // measurements rotate through z[0] instead of being indexed
 #pragma unroll 1
             for (int k = 0; k < p.n_steps; k++) {
-                reg_predict<float, N>(x, P, F, Q, p.alpha_sq);
-                KfUpdateOut<float, N, M> o;
-                reg_update<float, N, M>(x, P, H, R, z[0], o);
+                if (PAT::any) {
+                    reg_predict_pat<PAT, N>(x, P, F, Q, p.alpha_sq);
+                    reg_update_pat<PAT, N, M>(x, P, H, R, z[0]);
+                } else {
+                    reg_predict<float, N>(x, P, F, Q, p.alpha_sq);
+                    KfUpdateOut<float, N, M> o;
+                    reg_update<float, N, M>(x, P, H, R, z[0], o);
+                }
 #pragma unroll
                 for (int j = 0; j + 1 < ZS; j++) { z[j][0] = z[j + 1][0]; z[j][1] = z[j + 1][1]; }
+            }
+            if (PAT::any) {
+#pragma unroll
+                for (int i = 0; i < N; i++) {
+                    check(x[i]);
+#pragma unroll
+                    for (int j = 0; j < N; j++) check(P[i][j]);
+                }
+            }
+            if (PAT::any && live && nf != 0.f) {
+                // The dense ring on this filter's inputs, as the generic instance runs it.  They are still in
+                // global memory: the ring steps in place, only this thread writes filter f (below), and no z
+                // overlaps the state.  A structural word is the bank's shared value (a launch parameter).
+                const float *rec = p.rec + (int64_t)(base + sign * tile) * p.rec_planes * TILE + tid;
+                auto gword = [&](int e, float shared) -> float {
+                    if (PAT::structural(e)) return shared;
+                    return (p.varying >> e) & 1 ? rec[p.slot_off[e] / 4] : shared;
+                };
+                float Fd[N][N], Qd[N][N], Hd[M][N], Rd[M][M];
+#pragma unroll
+                for (int i = 0, e = W_Q; i < N; i++) {
+#pragma unroll
+                    for (int j = 0; j < N; j++) Fd[i][j] = gword(W_F + i * N + j, p.Fh[i * N + j]);
+#pragma unroll
+                    for (int j = i; j < N; j++, e++) Qd[i][j] = Qd[j][i] = gword(e, p.Qh[i * N + j]);
+                }
+#pragma unroll
+                for (int a = 0; a < M; a++)
+#pragma unroll
+                    for (int j = 0; j < N; j++) Hd[a][j] = gword(W_H + a * N + j, p.Hh[a * N + j]);
+                Rd[0][0] = gword(W_R, p.Rh[0]);
+                Rd[0][1] = Rd[1][0] = gword(W_R + 1, p.Rh[1]);
+                Rd[1][1] = gword(W_R + 2, p.Rh[3]);
+                const float4 vx = *reinterpret_cast<const float4 *>(p.x + f * N);
+                x[0] = vx.x; x[1] = vx.y; x[2] = vx.z; x[3] = vx.w;
+#pragma unroll
+                for (int i = 0; i < N; i++) {
+                    const float4 v = *reinterpret_cast<const float4 *>(p.P + f * N * N + i * N);
+                    P[i][0] = v.x; P[i][1] = v.y; P[i][2] = v.z; P[i][3] = v.w;
+                }
+#pragma unroll 1
+                for (int k = 0; k < p.n_steps; k++) {
+                    const float2 v = *reinterpret_cast<const float2 *>(p.zs[k] + f * M);
+                    const float zk[M] = {v.x, v.y};
+                    reg_predict<float, N>(x, P, Fd, Qd, p.alpha_sq);
+                    KfUpdateOut<float, N, M> o;
+                    reg_update<float, N, M>(x, P, Hd, Rd, zk, o);
+                }
             }
         }
         if (!RING && DO_P) {
@@ -508,11 +630,11 @@ int env_int(const char *name, int dflt)
     return v ? atoi(v) : dflt;
 }
 
-template <int MODE, int SHARED, bool EXTRAS, int REC = 0, int RING = 0>
+template <int MODE, int SHARED, bool EXTRAS, int REC = 0, int RING = 0, class PAT = NoPattern>
 int launch_variant(const FastP<4, 2> &p, cudaStream_t s)
 {
     using St = Stage<float, 4, 2, SHARED != 0, REC, RING ? RING : 1>;
-    auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, REC, RING>;
+    auto kern = kf42_f32_kernel<MODE, SHARED, EXTRAS, REC, RING, PAT>;
     // (the ring's stage is laid out per launch and never exceeds St::BYTES)
     const int smem = STAGES * (RING ? p.ring_stage : St::BYTES);
     static bool configured[64] = {false};
@@ -967,6 +1089,18 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const 
         p.ring_ox = St::OQ + p.rec_planes * TILE * 4;
         p.ring_oz = p.ring_ox + St::align_up(St::XB);
         p.ring_stage = p.ring_oz + n_steps * St::align_up(St::ZB);
+        // the pattern instance when every one of its structural words is, in every filter, the same bits
+        // (+0, not -0; exactly 1) and so a word the scan found shared
+        uint64_t zero = 0, one = 0;
+        for (int e = 0; e < WORDS; e++) {
+            uint32_t v;
+            memcpy(&v, &map->words[e], 4);
+            if ((map->varying >> e) & 1) continue;
+            if (v == 0u) zero |= 1ull << e;
+            if (v == 0x3f800000u) one |= 1ull << e;
+        }
+        if ((zero & Cv2dPattern::ZERO) == Cv2dPattern::ZERO && (one & Cv2dPattern::ONE) == Cv2dPattern::ONE)
+            return launch_variant<3, 0, false, 2, BKE_KF42_MAX_RING, Cv2dPattern>(p, s);
         return launch_variant<3, 0, false, 2, BKE_KF42_MAX_RING>(p, s);
     }
 

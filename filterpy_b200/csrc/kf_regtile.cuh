@@ -216,4 +216,205 @@ __device__ __forceinline__ void reg_update(T (&x)[N], T (&P)[N][N], const T (&H)
         }
 }
 
+// ---------------------------------------------------------------------------- structural model words
+// reg_predict_pat / reg_update_pat: reg_predict / reg_update for a bank whose models hold structural words,
+// +0 (bit pattern 0) or 1 in every filter, named at compile time by PAT:
+//   PAT::F0(i), PAT::F1(i)   row i of F: bit k set = F[i][k] is +0 / is 1
+//   PAT::H0(a), PAT::H1(a)   row a of H, likewise
+//   PAT::Q0(i, j), PAT::R0(a, b)   Q[i][j], R[a][b] is +0
+// The structural entries of F, Q, H, R are not read.  For finite inputs whose arithmetic stays finite they
+// give the bits of the dense functions as compiled, with the products by a structural word dropped or folded.
+//
+// The dense chain  s = a0 b0;  s += a1 b1; ...  compiles to FMUL of product 1, FFMA of product 0 onto it, then
+// FFMA of products 2, 3, ... in order.  A product a b with a = +0 and b finite is a zero of b's sign, and
+// adding a zero changes only the sign of a zero partial sum: fma(+0, b, s) is s, or -0 when s is -0 and b's
+// sign bit is set.  So a run of dropped products adds the zero whose sign is the AND of the run's sign bits:
+// 0 * w, with w the AND of the run's bit patterns (finite, as every b is).  A run ahead of the first kept
+// product is the addend of its FFMA (the FMUL becomes an FFMA); a later run costs one FFMA(0, w, s),
+// since a kept product or partial sum may round to -0.  A run of one is the dense FFMA itself.
+// A factor 1: 1 b is b, fma(1, b, s) is s + b; a product 1 b ahead of every kept product is b, and the run
+// ahead of it is added together with the run after it (b + z1 + z2 = b + (z1 + z2) for any b).
+
+// the AND of the bit patterns of b[k], k in D (a finite float for finite b)
+template <int L>
+__device__ __forceinline__ float and_bits(const float (&b)[L], uint32_t D)
+{
+    uint32_t m = ~0u;
+#pragma unroll
+    for (int k = 0; k < L; k++)
+        if ((D >> k) & 1) m &= __float_as_uint(b[k]);
+    return __uint_as_float(m);
+}
+
+// sum_k a[k] b[k] in the dense chain's order and bits, for a[k] = +0 (bit k of Z) or 1 (bit k of O) in every
+// filter.  !SIGNED: the caller maps a zero result of either sign to the same value, so the zero's sign is
+// not tracked and the dropped products cost nothing.
+// (Z, O and SIGNED are constants wherever it is inlined: the loop unrolls to the kept instructions)
+template <int L>
+__device__ __forceinline__ float pat_chain(uint32_t Z, uint32_t O, bool SIGNED, const float (&a)[L], const float (&b)[L])
+{
+    float s = 0.f;
+    bool have = false;      // s holds a partial sum
+    uint32_t d = 0;         // dropped products not yet added
+#pragma unroll
+    for (int p = 0; p < L; p++) {
+        const int k = L > 1 && p < 2 ? 1 - p : p;       // the product evaluated p-th
+        if ((Z >> k) & 1) {
+            if (SIGNED) d |= 1u << k;
+            continue;
+        }
+        const bool one = (O >> k) & 1;
+        if (!have) {
+            have = true;
+            if (one) { s = b[k]; continue; }            // d is added with the next run
+            s = d ? __fmaf_rn(a[k], b[k], __fmul_rn(0.f, and_bits(b, d))) : __fmul_rn(a[k], b[k]);
+            d = 0;
+            continue;
+        }
+        if (d) { s = __fmaf_rn(0.f, and_bits(b, d), s); d = 0; }
+        s = one ? __fadd_rn(s, b[k]) : __fmaf_rn(a[k], b[k], s);
+    }
+    if (d) s = have ? __fmaf_rn(0.f, and_bits(b, d), s) : __fmul_rn(0.f, and_bits(b, d));
+    return s;
+}
+
+template <class PAT, int N>
+__device__ __forceinline__ void reg_predict_pat(float (&x)[N], float (&P)[N][N], const float (&F)[N][N],
+                                                const float (&Q)[N][N], float alpha_sq)
+{
+    float xn[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) xn[i] = pat_chain(PAT::F0(i), PAT::F1(i), true, F[i], x);
+    float FP[N][N];
+#pragma unroll
+    for (int j = 0; j < N; j++) {
+        float col[N];
+#pragma unroll
+        for (int k = 0; k < N; k++) col[k] = P[k][j];
+#pragma unroll
+        for (int i = 0; i < N; i++) FP[i][j] = pat_chain(PAT::F0(i), PAT::F1(i), true, F[i], col);
+    }
+    // alpha_sq s + (+0) is +0 for a zero s of either sign: those entries need no sign of s
+#pragma unroll
+    for (int i = 0; i < N; i++)
+#pragma unroll
+        for (int j = 0; j < N; j++)
+            P[i][j] = __fmaf_rn(alpha_sq, pat_chain(PAT::F0(j), PAT::F1(j), !PAT::Q0(i, j), F[j], FP[i]), Q[i][j]);
+#pragma unroll
+    for (int i = 0; i < N; i++) x[i] = xn[i];
+}
+
+// the columns of H whose entries are all structural (any), or all +0 (!any)
+template <class PAT, int M>
+__host__ __device__ constexpr uint32_t pat_cols(bool any)
+{
+    uint32_t c = ~0u;
+    for (int a = 0; a < M; a++) c &= any ? PAT::H0(a) | PAT::H1(a) : PAT::H0(a);
+    return c;
+}
+
+// false when S is singular (the state is left at the prior, as reg_update leaves it)
+template <class PAT, int N, int M>
+__device__ __forceinline__ bool reg_update_pat(float (&x)[N], float (&P)[N][N], const float (&H)[M][N],
+                                               const float (&R)[M][M], const float (&z)[M])
+{
+    float y[M];
+#pragma unroll
+    for (int a = 0; a < M; a++) y[a] = __fadd_rn(z[a], -pat_chain(PAT::H0(a), PAT::H1(a), true, H[a], x));
+    float PHT[N][M];
+#pragma unroll
+    for (int i = 0; i < N; i++)
+#pragma unroll
+        for (int a = 0; a < M; a++) PHT[i][a] = pat_chain(PAT::H0(a), PAT::H1(a), true, H[a], P[i]);
+    float S[M][M], SI[M][M], logdet;
+#pragma unroll
+    for (int b = 0; b < M; b++) {
+        float col[N];
+#pragma unroll
+        for (int k = 0; k < N; k++) col[k] = PHT[k][b];
+        // s + (+0) is +0 for a zero s of either sign
+#pragma unroll
+        for (int a = 0; a < M; a++) S[a][b] = __fadd_rn(pat_chain(PAT::H0(a), PAT::H1(a), !PAT::R0(a, b), H[a], col), R[a][b]);
+    }
+    if (!reg_inverse<float, M>(S, SI, logdet)) return false;
+    float K[N][M];
+#pragma unroll
+    for (int i = 0; i < N; i++)
+#pragma unroll
+        for (int a = 0; a < M; a++) {
+            float s = PHT[i][0] * SI[0][a];
+#pragma unroll
+            for (int b = 1; b < M; b++) s += PHT[i][b] * SI[b][a];
+            K[i][a] = s;
+        }
+#pragma unroll
+    for (int i = 0; i < N; i++) {
+        float s = x[i];
+#pragma unroll
+        for (int a = 0; a < M; a++) s += K[i][a] * y[a];
+        x[i] = s;
+    }
+    // IKH = I - K H.  A column j of H whose entries are all structural (HS): IKH[i][j] = delta_ij - K[i][a] over
+    // the a with H[a][j] = 1, in order (delta - K is never -0, and nor is a difference of it, so the dropped
+    // products change nothing); with none such (HZ), IKH[:, j] is the constant delta_ij, a structural word of T1
+    // and P.  A column with any other entry runs the dense chain.
+    constexpr uint32_t HS = pat_cols<PAT, M>(true), HZ = pat_cols<PAT, M>(false);
+    float IKH[N][N];
+#pragma unroll
+    for (int j = 0; j < N; j++) {
+#pragma unroll
+        for (int i = 0; i < N; i++) {
+            float s = i == j ? 1.f : 0.f;
+            if ((HS >> j) & 1) {
+#pragma unroll
+                for (int a = 0; a < M; a++)
+                    if ((PAT::H1(a) >> j) & 1) s = __fadd_rn(s, -K[i][a]);
+            } else {
+#pragma unroll
+                for (int a = 0; a < M; a++) s = __fmaf_rn(-K[i][a], H[a][j], s);
+            }
+            IKH[i][j] = s;
+        }
+    }
+    float T1[N][N];
+#pragma unroll
+    for (int j = 0; j < N; j++) {
+        float col[N];
+#pragma unroll
+        for (int k = 0; k < N; k++) col[k] = P[k][j];
+#pragma unroll
+        for (int i = 0; i < N; i++) T1[i][j] = pat_chain(HZ & ~(1u << i), HZ & (1u << i), true, IKH[i], col);
+    }
+    float KR[N][M];
+#pragma unroll
+    for (int b = 0; b < M; b++) {
+        float col[M];
+        uint32_t rz = 0;
+#pragma unroll
+        for (int a = 0; a < M; a++) { col[a] = R[a][b]; rz |= PAT::R0(a, b) ? 1u << a : 0u; }
+#pragma unroll
+        for (int i = 0; i < N; i++) KR[i][b] = pat_chain(rz, 0u, true, col, K[i]);
+    }
+    // P = T1 IKH' + KR K', one chain of N + M products per entry
+#pragma unroll
+    for (int j = 0; j < N; j++) {
+        float a[N + M];
+#pragma unroll
+        for (int k = 0; k < N; k++) a[k] = IKH[j][k];
+#pragma unroll
+        for (int k = 0; k < M; k++) a[N + k] = K[j][k];
+#pragma unroll
+        for (int i = 0; i < N; i++) {
+            float b[N + M];
+#pragma unroll
+            for (int k = 0; k < N; k++) b[k] = T1[i][k];
+#pragma unroll
+            for (int k = 0; k < M; k++) b[N + k] = KR[i][k];
+            P[i][j] = pat_chain(HZ & ~(1u << j), HZ & (1u << j), true, a, b);
+        }
+    }
+    return true;
+}
+
+
 }  // namespace bke
