@@ -128,8 +128,6 @@ int dispatch(const bke_kf_args &a, cudaStream_t s)
 
 int launch_kf_direct(const bke_kf_args &a, cudaStream_t s)
 {
-    static const int enabled = [] { const char *e = getenv("BKE_KF_DIRECT"); return e ? atoi(e) : 1; }();
-    if (!enabled) return BKE_ERR_UNSUPPORTED;
     if (a.B != nullptr && a.u != nullptr) return BKE_ERR_UNSUPPORTED;
     if (a.flags & BKE_UPDATE_FIRST) return BKE_ERR_UNSUPPORTED;
     return a.dtype == BKE_F32 ? dispatch<float>(a, s) : dispatch<double>(a, s);

@@ -30,7 +30,6 @@
 // filter for the kf_bank_cv2d template, whose two axes share dt, q and r).
 //
 // Reference arithmetic: filterpy/kalman/kalman_filter.py:471-478, 533-556 (see kf_regtile.cuh).
-#include <stdlib.h>
 #include <string.h>
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
@@ -620,16 +619,6 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
 }
 
 // ---------------------------------------------------------------------------- host side
-// switches (environment, read once): BKE_KF_L2 = 0 disables the L2 eviction-priority hints,
-// BKE_KF_SYM = 0 both packed records, BKE_KF_HOST_MODELS = 0 the shared models in the launch parameters,
-// BKE_KF_ORDER = 0 the reversed tile order (every launch walks the bank first to last),
-// BKE_KF_RING = 0 the fused ring (bke_kf_steps_packed reports BKE_ERR_UNSUPPORTED)
-int env_int(const char *name, int dflt)
-{
-    const char *v = getenv(name);
-    return v ? atoi(v) : dflt;
-}
-
 template <int MODE, int SHARED, bool EXTRAS, int REC = 0, int RING = 0, class PAT = NoPattern>
 int launch_variant(const FastP<4, 2> &p, cudaStream_t s)
 {
@@ -866,13 +855,6 @@ kf42_pack_models_kernel(int64_t n_filters, int64_t slots, const float4 *__restri
     }
 }
 
-// BKE_KF_SYM = 0 turns the packed records off (their entry points report BKE_ERR_UNSUPPORTED)
-bool sym_enabled()
-{
-    static const int env = env_int("BKE_KF_SYM", 1);
-    return env != 0;
-}
-
 bool misaligned16(const void *p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15u) != 0; }
 
 }  // namespace
@@ -885,7 +867,6 @@ size_t kf_sym_models_bytes(int64_t n_filters)
 
 int launch_kf_pack_sym(int64_t n_filters, const void *Q, const void *R, void *record, int32_t *asym, cudaStream_t s)
 {
-    if (!sym_enabled()) { set_error("the packed symmetric models are disabled (BKE_KF_SYM=0)"); return BKE_ERR_UNSUPPORTED; }
     if (n_filters >= (int64_t)1 << 30) { set_error("the packed symmetric models take at most 2^30 filters"); return BKE_ERR_UNSUPPORTED; }
     if (misaligned16(Q) || misaligned16(R) || misaligned16(record)) {
         set_error("Q, R and record must be 16-byte aligned");
@@ -909,7 +890,6 @@ size_t kf_packed_models_bytes(int64_t n_filters, uint64_t varying)
 
 static int check_models(int64_t n_filters, const void *F, const void *Q, const void *H, const void *R, const void *out)
 {
-    if (!sym_enabled()) { set_error("the packed models are disabled (BKE_KF_SYM=0)"); return BKE_ERR_UNSUPPORTED; }
     if (n_filters >= (int64_t)1 << 30) { set_error("the packed models take at most 2^30 filters"); return BKE_ERR_UNSUPPORTED; }
     if (misaligned16(F) || misaligned16(Q) || misaligned16(H) || misaligned16(R) || misaligned16(out)) {
         set_error("F, Q, H, R and the map or record must be 16-byte aligned");
@@ -993,10 +973,6 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const 
 {
     const bool packed = map != nullptr, sym = rec != nullptr && !packed;
     const bool ring = zs != nullptr;        // bke_kf_steps_packed, which has checked what only the ring refuses
-    if ((sym || packed) && !sym_enabled()) {
-        set_error(sym ? "the packed symmetric models are disabled (BKE_KF_SYM=0)" : "the packed models are disabled (BKE_KF_SYM=0)");
-        return BKE_ERR_UNSUPPORTED;
-    }
     if (misaligned16(rec)) { set_error("record must be 16-byte aligned"); return BKE_ERR_UNSUPPORTED; }
     if (packed && map->asymmetric) { set_error("the map reports an asymmetric Q or R: the bank runs on bke_kf_step"); return BKE_ERR_UNSUPPORTED; }
     if (!(a.dtype == BKE_F32 && a.dim_x == 4 && a.dim_z == 2)) return BKE_ERR_UNSUPPORTED;
@@ -1021,15 +997,11 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const 
     p.N_filters = N;
     p.num_tiles = (int)((N + TILE - 1) / TILE);
     p.alpha_sq = (float)a.alpha_sq;
-    {
-        // keep-the-state-in-L2 hints pay off when x, P fit the L2 together with the streaming traffic
-        static const int l2_env = env_int("BKE_KF_L2", 1);
-        p.l2_hints = l2_env && (N * 80 <= (int64_t)38 << 20) && a.x_out == a.x && a.P_out == a.P;
-    }
+    // keep-the-state-in-L2 hints pay off when x, P fit the L2 together with the streaming traffic
+    p.l2_hints = (N * 80 <= (int64_t)38 << 20) && a.x_out == a.x && a.P_out == a.P;
     // a bank whose state stays in L2 between steps (l2_hints) has nothing to gain from the order: it
     // keeps walking first to last
-    static const int order_env = env_int("BKE_KF_ORDER", 1);
-    p.reverse = order_env && (a.flags & BKE_REVERSE_TILES) && !p.l2_hints;
+    p.reverse = (a.flags & BKE_REVERSE_TILES) && !p.l2_hints;
     p.x = (const float *)a.x; p.P = (const float *)a.P; p.z = (const float *)a.z;
     p.F = (const float *)a.F; p.Q = (const float *)a.Q; p.H = (const float *)a.H; p.R = (const float *)a.R;
     p.rec = (const float *)rec;
@@ -1039,8 +1011,7 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const 
     p.S = (float *)a.S; p.SI = (float *)a.SI; p.ll = (float *)a.log_likelihood; p.status = a.status;
     p.sticky = (a.flags & BKE_STATUS_STICKY) ? 1 : 0;
     // host copies of the shared models (optional): carried in the launch parameters
-    static const int hostm_env = env_int("BKE_KF_HOST_MODELS", 1);
-    const bool host_models = hostm_env && all_shared && a.F_host && a.Q_host && a.H_host && a.R_host;
+    const bool host_models = all_shared && a.F_host && a.Q_host && a.H_host && a.R_host;
     if (host_models) {
         memcpy(p.Fh, a.F_host, sizeof(p.Fh)); memcpy(p.Qh, a.Q_host, sizeof(p.Qh));
         memcpy(p.Hh, a.H_host, sizeof(p.Hh)); memcpy(p.Rh, a.R_host, sizeof(p.Rh));
@@ -1078,8 +1049,6 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const 
     }
     const bool extras = a.x_prior || a.P_prior || a.K || a.y || a.S || a.SI || a.log_likelihood || a.status;
     if (ring) {
-        static const int ring_env = env_int("BKE_KF_RING", 1);
-        if (!ring_env) { set_error("the fused ring is disabled (BKE_KF_RING=0)"); return BKE_ERR_UNSUPPORTED; }
         if (!packed || !all_dense || !(dp && du) || extras || a.z_valid) return BKE_ERR_UNSUPPORTED;
         for (int k = 0; k < n_steps; k++) p.zs[k] = (const float *)zs[k];
         p.n_steps = n_steps;

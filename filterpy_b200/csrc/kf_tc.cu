@@ -28,7 +28,6 @@
 // distance between 8-row groups), so no tensor map is needed and the hi / lo split happens on the way in.
 // The accumulator fragment of the first product is written straight back as the (transposed, split)
 // A operand of the second; the second goes through a padded scratch so that thread t holds row t.
-#include <stdlib.h>
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
 #include "ptx.cuh"
@@ -460,23 +459,20 @@ int launch_m(const TcP &p, int m, cudaStream_t s)
 
 static bool al16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-// BKE_KF_TC=0 keeps the CUDA-core kernels for these shapes (A/B measurements).  Eligible: fp32, dim_x 16 / 32, F and Q
-// shared, no control input.  A fused predict+update whose H and R are shared too and whose dim_z <= 4 runs entirely in
-// this kernel (BKE_KF_TC_FUSED=0: predict here, update through the usual order); any other fused step runs its predict
-// here and its update through launch_kf_any on the prior left in x_out / P_out.
+// Eligible: fp32, dim_x 16 / 32, F and Q shared, no control input.  A fused predict+update whose H and R are shared too
+// and whose dim_z <= 4 runs entirely in this kernel; any other fused step runs its predict here and its update through
+// launch_kf_any on the prior left in x_out / P_out.
 int launch_kf_tc(const bke_kf_args &a, cudaStream_t s)
 {
-    static const int mode = [] { const char *e = getenv("BKE_KF_TC"); return e ? atoi(e) : 1; }();
-    static const bool fused_on = [] { const char *e = getenv("BKE_KF_TC_FUSED"); return !(e && e[0] == '0'); }();
-    if (mode == 0) return BKE_ERR_UNSUPPORTED;
     if (a.dtype != BKE_F32 || !(a.dim_x == 16 || a.dim_x == 32)) return BKE_ERR_UNSUPPORTED;
     if (!(a.flags & BKE_DO_PREDICT) || (a.flags & BKE_UPDATE_FIRST)) return BKE_ERR_UNSUPPORTED;
     if (a.F_stride != 0 || a.Q_stride != 0 || (a.B && a.u)) return BKE_ERR_UNSUPPORTED;
     if (!(al16(a.x) && al16(a.P) && al16(a.x_out) && al16(a.P_out) && al16(a.x_prior) && al16(a.P_prior))) return BKE_ERR_UNSUPPORTED;
     const bool fused = (a.flags & BKE_DO_UPDATE) != 0;
-    const bool fused_here = fused && fused_on && a.H_stride == 0 && a.R_stride == 0 && a.dim_z >= 1 && a.dim_z <= 4 && a.z;
-    // without the fused kernel the 16/4 and 16/2 fused steps are faster as ONE row-block launch than as predict-here + update-there
-    if (fused && !fused_here && mode == 1 && a.dim_x == 16 && (a.dim_z == 4 || a.dim_z == 2)) return BKE_ERR_UNSUPPORTED;
+    const bool fused_here = fused && a.H_stride == 0 && a.R_stride == 0 && a.dim_z >= 1 && a.dim_z <= 4 && a.z;
+    // a 16/4 or 16/2 fused step this kernel does not take whole is faster as ONE row-block launch than as
+    // predict-here + update-there
+    if (fused && !fused_here && a.dim_x == 16 && (a.dim_z == 4 || a.dim_z == 2)) return BKE_ERR_UNSUPPORTED;
     // x_out may alias x and P_out may alias P (each tile reads its rows before it writes them); nothing else may overlap
     tc::TcP p;
     p.N = a.n_filters; p.alpha_sq = (float)a.alpha_sq;

@@ -1,5 +1,5 @@
 // ptx.cuh — Hopper (sm_90a) PTX wrappers shared by the kernels: mbarriers, bulk and tensor copies
-// (cp.async.bulk), programmatic dependent launch, L2 cache policies and relaxed global loads / stores.
+// (cp.async.bulk), programmatic dependent launch and L2 cache policies.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -96,19 +96,6 @@ __device__ __forceinline__ uint64_t policy_evict_last()
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
     return p;
-}
-
-// ---------------------------------------------------------------------------- relaxed global accesses
-// (status words that other CTAs poll: never served from a stale L1 line)
-__device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long long *p)
-{
-    unsigned long long v;
-    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_relaxed_u64(unsigned long long *p, unsigned long long v)
-{
-    asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
 }  // namespace bke

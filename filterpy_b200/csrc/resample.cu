@@ -31,7 +31,6 @@
 //   G  sequential fallback (normally exits at once), info
 #include "resample_common.cuh"
 #include "ptx.cuh"
-#include <stdlib.h>
 
 namespace bke {
 namespace rs {
@@ -79,7 +78,6 @@ struct Ws {
     int *ord2tile;          // [UMAX+SEQMAX]
     Run *runs;              // [max_runs]
     int *slow_list;         // [T] tiles that did not qualify for the fast path (order irrelevant)
-    u64 *st1;               // [T] status words of k_front's look-back (directly after the header: one memset clears both)
     SM *ctot;               // [CHAIN_CTAS] composite of each chain CTA's tile range
     int max_runs;
     int T;
@@ -95,7 +93,6 @@ size_t carve(int64_t n, unsigned char *base, Ws *w)
     auto take = [&](size_t bytes) { size_t o = off; off += align256(bytes); return base ? base + o : nullptr; };
     unsigned char *p;
     p = take(sizeof(Header));                 if (w) w->hdr = (Header *)p;
-    p = take(sizeof(u64) * T);                if (w) w->st1 = (u64 *)p;
     p = take(sizeof(SM) * CHAIN_CTAS);        if (w) w->ctot = (SM *)p;
     p = take(sizeof(double) * T);             if (w) w->tile_sum = (double *)p;
     p = take(sizeof(double) * (T + 1));       if (w) w->tile_prefix = (double *)p;
@@ -423,153 +420,6 @@ __global__ void __launch_bounds__(BLOCK, 5) k_tile_maps_fast1(Params p)
         const int any_nz = __syncthreads_or(nz);
         if (threadIdx.x == 0) {
             p.ws.tile_k[t] = any_nz ? e0 : K_ID; p.ws.tile_d[t] = total; p.ws.tile_t[t] = 0;
-            p.ws.tile_slot[t] = SLOT_FAST;
-        }
-    } else if (threadIdx.x == 0) {
-        p.ws.slow_list[atomicAdd(&p.ws.hdr->n_slow, 1)] = t;
-    }
-}
-
-// ------------------------------------------------------------------ passes A + B + C in one launch
-// One CTA per tile, in blockIdx order.  The tile is read ONCE: its sum is published as a 64-bit status
-// word (value with the two low mantissa bits replaced by a flag: 1 = aggregate, 2 = inclusive prefix;
-// the perturbation is far inside the classification margin eb), warp 0 looks back over the earlier
-// tiles' words for the approximate exclusive prefix (decoupled look-back, one warp-wide window of 32
-// tiles per poll), and the fast-path map of k_tile_maps_fast1 is then computed from the registers the
-// loads landed in.  The approximate prefixes only have to be within eb of the exact running sum, which
-// holds for any summation order of non-negative terms.
-constexpr u64 ST_AGG = 1, ST_INCL = 2;
-constexpr int FRONT_SPINS = 1 << 20;      // polls of a blocked window before giving up (-> sequential fallback)
-constexpr int FRONT_LBK = 8;              // status words per lane and poll: a window of 256 tiles
-
-// named barrier 1 of the first NT threads (k_front: the data warps, k_emit2: the consumer warps; the
-// remaining warp never joins it)
-template <int NT> __device__ __forceinline__ void bar_sync()
-{
-    asm volatile("barrier.cta.sync 1, %0;" ::"n"(NT) : "memory");
-}
-template <int NT> __device__ __forceinline__ int bar_and(int pred)
-{
-    int out;
-    asm volatile("{\n.reg .pred p, q;\nsetp.ne.b32 p, %1, 0;\nbarrier.cta.red.and.pred q, 1, %2, p;\nselp.b32 %0, 1, 0, q;\n}\n"
-                 : "=r"(out) : "r"(pred), "n"(NT) : "memory");
-    return out;
-}
-
-// With ~600 tiles in flight and one tile retiring every ~6 ns the nearest tile that already owns an
-// inclusive prefix is ~200 tiles back (poll latency / tile period), so a 32-tile window would need
-// 6-7 dependent polls; eight independent loads per lane cover that distance in one round trip.
-__device__ __forceinline__ double front_lookback(const Params &p, int t, int lane)
-{
-    double part = 0.0;                                     // this lane's share, reduced at the end
-    int idx = t - 1 - lane;
-    int spins = 0;
-    bool done = false;
-    while (!done) {
-        u64 v[FRONT_LBK];
-#pragma unroll
-        for (int j = 0; j < FRONT_LBK; j++) {
-            const int i = idx - 32 * j;
-            v[j] = (i >= 0) ? ld_relaxed_u64(p.ws.st1 + i) : ST_INCL;           // before the first tile: 0.0, inclusive
-        }
-        bool blocked = false;
-#pragma unroll
-        for (int j = 0; j < FRONT_LBK; j++) {
-            if (!done && !blocked) {
-                const unsigned incl = __ballot_sync(FULL, (v[j] & 3) == ST_INCL);
-                const unsigned empty = __ballot_sync(FULL, (v[j] & 3) == 0);
-                const int first = incl ? __ffs(incl) - 1 : 32;        // nearest tile with an inclusive prefix
-                const unsigned closer = first >= 32 ? FULL : ((1u << first) - 1u);
-                if (empty & closer) blocked = true;                   // a word this side of it is not there yet
-                else {
-                    if (lane <= first) part += __longlong_as_double((i64)(v[j] & ~3ull));
-                    if (incl) done = true; else idx -= 32;
-                }
-            }
-        }
-        if (blocked) {
-            if (++spins > FRONT_SPINS) { if (lane == 0) p.ws.hdr->fallback = 1; break; }
-            __nanosleep(40);
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(FULL, part, o);
-    return part;
-}
-
-// Warps 0-7 own the tile's data; warp 8 starts the look-back the moment the CTA starts (it needs nothing
-// of this tile), so the prefix is usually there when the tile's own sum is.
-__global__ void __launch_bounds__(BLOCK + 32, 4) k_front(Params p)
-{
-    __shared__ double shd[BLOCK / 32];
-    __shared__ i64 shi[BLOCK / 32 + 1];
-    __shared__ double s_ex, s_tot;
-    const int t = blockIdx.x, T = p.ws.T;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (wid == BLOCK / 32) {
-        const double ex = front_lookback(p, t, lane);
-        if (lane == 0) s_ex = ex;
-        __syncthreads();
-        if (lane == 0) {
-            const double tot = s_tot;
-            st_relaxed_u64(p.ws.st1 + t, ((u64)__double_as_longlong(ex + tot) & ~3ull) | ST_INCL);
-            const double tp = (p.carry_approx ? *p.carry_approx : 0.0) + ex;
-            p.ws.tile_prefix[t] = tp;
-            if (t == T - 1) p.ws.tile_prefix[T] = tp + tot;
-        }
-        return;
-    }
-    double2 g[IPT / 2];
-    fetch_tile(p, t, g);
-    double s = 0.0;
-    bool bad = false;
-#pragma unroll
-    for (int i = 0; i < IPT / 2; i++) {
-        if (!(g[i].x >= 0.0) || !(g[i].y >= 0.0) || isinf(g[i].x) || isinf(g[i].y)) bad = true;
-        s += g[i].x + g[i].y;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(FULL, s, o);
-    if (lane == 0) shd[wid] = s;
-    if (threadIdx.x == 0) shi[BLOCK / 32] = 0;             // "some weight of the tile is non-zero"
-    if (bad) p.ws.hdr->fallback = 1;
-    bar_sync<BLOCK>();
-    if (wid == 0) {
-        double tot = 0.0;
-#pragma unroll
-        for (int i = 0; i < BLOCK / 32; i++) tot += shd[i];
-        if (lane == 0) { st_relaxed_u64(p.ws.st1 + t, ((u64)__double_as_longlong(tot) & ~3ull) | ST_AGG); p.ws.tile_sum[t] = tot; s_tot = tot; }
-    }
-    __syncthreads();
-    const double tp = (p.carry_approx ? *p.carry_approx : 0.0) + s_ex;
-    int e0;
-    const bool tile_clean = clean_add(tp, tp + s_tot, p.eb, &e0);      // the whole tile stays deep inside binade e0
-    const i64 base = (i64)e0 << 52;
-    const double B0 = __longlong_as_double(base), B1 = __longlong_as_double(base + 1);
-    i64 acc = 0;
-    bool ok = tile_clean, nz = false;
-#pragma unroll
-    for (int i = 0; i < IPT / 2; i++) {
-        const double w2[2] = {g[i].x, g[i].y};
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-            const i64 d0 = __double_as_longlong(__dadd_rn(B0, w2[h])) - base;
-            const i64 d1 = __double_as_longlong(__dadd_rn(B1, w2[h])) - (base + 1);
-            ok = ok && (d0 == d1);
-            nz = nz || (w2[h] != 0.0);
-            acc += d0;
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(FULL, acc, o);
-    nz = __any_sync(FULL, nz);
-    if (lane == 0) { shi[wid] = acc; if (nz) shi[BLOCK / 32] = 1; }
-    if (bar_and<BLOCK>(ok)) {
-        if (threadIdx.x == 0) {
-            i64 total = 0;
-#pragma unroll
-            for (int i = 0; i < BLOCK / 32; i++) total += shi[i];
-            p.ws.tile_k[t] = shi[BLOCK / 32] ? e0 : K_ID; p.ws.tile_d[t] = total; p.ws.tile_t[t] = 0;
             p.ws.tile_slot[t] = SLOT_FAST;
         }
     } else if (threadIdx.x == 0) {
@@ -1227,9 +1077,15 @@ __global__ void __launch_bounds__(BLOCK, 2) k_emit_fast(Params p)
 // conflict-free LDS.128) while the consumers work on the current one.  Expansion: every particle with
 // >= 1 copies stores (local index + 1) at its first output slot of a zeroed window, a max-scan over the
 // slots fills the runs (no divergent copy loop) and every thread leaves with 16-byte stores of 20
-// consecutive indexes.
-constexpr int E2_NW = 8, E2_NT = E2_NW * 32, E2_SPT = 20, E2_WIN = E2_NT * E2_SPT;
+// consecutive indexes.  Two 32 KB stages, 96 registers, two CTAs per SM.
+constexpr int E2_NW = 8, E2_NT = E2_NW * 32, E2_SPT = 20, E2_WIN = E2_NT * E2_SPT, E2_STAGES = 2, E2_CTAS = 2;
 static_assert(E2_NT * IPT == TILE, "the second-generation emit uses the tile size of passes A-D");
+
+// named barrier 1 of the first NT threads (the consumer warps; the loader warp never joins it)
+template <int NT> __device__ __forceinline__ void bar_sync()
+{
+    asm volatile("barrier.cta.sync 1, %0;" ::"n"(NT) : "memory");
+}
 
 // byte offset of weight (row r = owning thread, 16-byte chunk c) inside a swizzled stage
 __device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)r * 128u + (uint32_t)((c ^ (r & 7)) << 4); }
@@ -1288,7 +1144,6 @@ bool weights_map(const double *w, int64_t n, int box_rows, CUtensorMap *out)
 
 }  // namespace
 
-template <int E2_STAGES>
 struct Emit2Shared {
     double w[E2_STAGES][TILE];         // TMA destinations (128-byte swizzle): must stay first, 1024-aligned
     int win[E2_WIN];                   // output window (all zero between tiles)
@@ -1298,16 +1153,12 @@ struct Emit2Shared {
     int skip;
 };
 
-// <E2_STAGES, E2_CTAS>: <2, 2> two 32 KB stages, 96 registers; <1, 3> one stage (the next tile's TMA is
-// issued as soon as the warps hold the current one in registers and lands long before it is needed),
-// 72 registers, three CTAs per SM.  <2, 2> is the default; BKE_RS_E2=1 selects <1, 3>, which on the H100
-// is slower for systematic but about 17 % faster for stratified resampling (DESIGN.md §3.6)
-template <bool STRAT, int E2_STAGES, int E2_CTAS, bool NORM>
+template <bool STRAT, bool NORM>
 __global__ void __launch_bounds__(E2_NT + 32, E2_CTAS) k_emit2(const __grid_constant__ CUtensorMap wmap, Params p)
 {
     constexpr int NT = E2_NT, NW = E2_NW, WIN = E2_WIN, SPT = E2_SPT;
     extern __shared__ __align__(1024) unsigned char e2_smem[];
-    Emit2Shared<E2_STAGES> &sm = *reinterpret_cast<Emit2Shared<E2_STAGES> *>(e2_smem);
+    Emit2Shared &sm = *reinterpret_cast<Emit2Shared *>(e2_smem);
     const Ws &ws = p.ws;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     if (tid == 0) {
@@ -1783,8 +1634,7 @@ struct RunArgs {
     double *wnorm_out;   // with div, optional: receives w / *div
 };
 
-// The passes a.phase selects.  NORM (a normalised call) always runs passes A, B and C as separate launches
-// and the default second-generation emit: BKE_RS_FRONT and BKE_RS_E2 have no NORM instances.
+// The passes a.phase selects.
 template <bool NORM>
 int launch(const RunArgs &a, const Params &p, cudaStream_t s)
 {
@@ -1794,23 +1644,12 @@ int launch(const RunArgs &a, const Params &p, cudaStream_t s)
     const int sms = sm_count();
     const int slow_grid = T < sms * 2 ? T : sms * 2;
     if (a.phase & 1) {
-        // BKE_RS_FRONT=1: tile sums, their scan (decoupled look-back) and the fast maps in ONE pass over the
-        // weights.  Slower than the three launches it replaces on an earlier target (with hundreds of tiles in
-        // flight the nearest inclusive prefix is far back and the polling competes with the streaming loads);
-        // about 6 % faster on the H100 (DESIGN.md §3.6), not yet the default.
-        static const bool fused_front = [] { const char *e = getenv("BKE_RS_FRONT"); return e && e[0] == '1'; }();
-        if (!NORM && !(a.phase & 8) && fused_front) {
-            const size_t clr = (size_t)((unsigned char *)(p.ws.st1 + T) - (unsigned char *)p.ws.hdr);
-            if (check_cuda(cudaMemsetAsync(p.ws.hdr, 0, clr, s), "memset header + status words")) return BKE_ERR_CUDA;
-            k_front<<<T, BLOCK + 32, 0, s>>>(p);
-        } else {
-            if (!(a.phase & 8)) {                   // bit 8: the header reset and pass A have run already (bke_resample_shard_stage)
-                if (check_cuda(cudaMemsetAsync(p.ws.hdr, 0, sizeof(Header), s), "memset header")) return BKE_ERR_CUDA;
-                k_tile_sums<NORM><<<T, BLOCK, 0, s>>>(p);
-            }
-            k_scan_tiles<<<1, CHAIN_THREADS, 0, s>>>(p);
-            k_tile_maps_fast1<NORM><<<T, BLOCK, 0, s>>>(p);
+        if (!(a.phase & 8)) {                       // bit 8: the header reset and pass A have run already (bke_resample_shard_stage)
+            if (check_cuda(cudaMemsetAsync(p.ws.hdr, 0, sizeof(Header), s), "memset header")) return BKE_ERR_CUDA;
+            k_tile_sums<NORM><<<T, BLOCK, 0, s>>>(p);
         }
+        k_scan_tiles<<<1, CHAIN_THREADS, 0, s>>>(p);
+        k_tile_maps_fast1<NORM><<<T, BLOCK, 0, s>>>(p);
         k_tile_maps<NORM><<<slow_grid, BLOCK, 0, s>>>(p);
     }
     if (a.phase & 2) {
@@ -1828,17 +1667,11 @@ int launch(const RunArgs &a, const Params &p, cudaStream_t s)
         CUtensorMap wmap;
         const bool emit2 = !a.cumsum_out && (n % 16) == 0 && weights_map(a.w, n, E2_NT, &wmap);
         if (emit2) {
-            static const int e2_variant = [] { const char *e = getenv("BKE_RS_E2"); return e ? atoi(e) : 0; }();
-            auto launch2 = [&](auto kern, int smem2, int ctas) -> int {
-                if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
-                const int g = T < sms * ctas ? T : sms * ctas;
-                kern<<<g, E2_NT + 32, smem2, s>>>(wmap, p);
-                return BKE_OK;
-            };
-            int rc2;
-            if (!NORM && e2_variant == 1) rc2 = a.U ? launch2(k_emit2<true, 1, 3, false>, (int)sizeof(Emit2Shared<1>), 3) : launch2(k_emit2<false, 1, 3, false>, (int)sizeof(Emit2Shared<1>), 3);
-            else rc2 = a.U ? launch2(k_emit2<true, 2, 2, NORM>, (int)sizeof(Emit2Shared<2>), 2) : launch2(k_emit2<false, 2, 2, NORM>, (int)sizeof(Emit2Shared<2>), 2);
-            if (rc2 != BKE_OK) return rc2;
+            const auto kern = a.U ? k_emit2<true, NORM> : k_emit2<false, NORM>;
+            const int smem2 = (int)sizeof(Emit2Shared);
+            if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
+            const int g = T < sms * E2_CTAS ? T : sms * E2_CTAS;
+            kern<<<g, E2_NT + 32, smem2, s>>>(wmap, p);
             if (a.U) k_emit_slow<true, NORM><<<slow_grid, BLOCK, emit_smem, s>>>(p);
             else k_emit_slow<false, NORM><<<slow_grid, BLOCK, emit_smem, s>>>(p);
         } else if (a.U) {

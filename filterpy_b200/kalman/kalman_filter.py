@@ -205,8 +205,7 @@ class KalmanFilter(_BankMirror):
             rc = self._lib.bke_kf_step_packed(a, ptr(rec) if rec.numel() else None, self._sym_host_map, s)
             if rc != _lib.BKE_ERR_UNSUPPORTED:
                 return rc
-            # BKE_KF_SYM=0, or arrays the packed kernel does not take (not 16-byte aligned): the dense
-            # models from now on
+            # arrays the packed kernel does not take (not 16-byte aligned): the dense models from now on
             self._sym_ok = False
             self._sym_drop()
         return self._lib.bke_kf_step(a, s)
@@ -395,7 +394,7 @@ class KalmanFilter(_BankMirror):
         the steps back to back with x and P in registers, so the state crosses HBM once per launch and
         not once per step.  Inside a fused ring x and P exist in HBM only between replays; the results
         are bit for bit those of the separate steps.  The returned graph's ``launches`` and
-        ``fused_steps`` say which of the two it is; ``BKE_KF_RING=0`` keeps the graph of separate steps."""
+        ``fused_steps`` say which of the two it is."""
         self._flush()
         self._ring_notes = []
         try:
@@ -434,7 +433,8 @@ class KalmanFilter(_BankMirror):
             for ring in rings:
                 self._run(call, ring)
         # once outside capture: the kernel's one-time function attribute must not be set under capture,
-        # and a refusal (BKE_KF_RING=0, a z the ring does not take) leaves the graph of separate steps
+        # and a refusal (a z the ring does not take, such as one that overlaps x or P) leaves the graph of
+        # separate steps
         with torch.cuda.device(self._device):
             rc = call(rings[0])
         if rc == _lib.BKE_ERR_UNSUPPORTED:

@@ -65,8 +65,7 @@ extern "C" {
                                         step, so that each step starts on the filters the previous one finished
                                         while their x, P and models are still in L2.  Other kernels ignore it,
                                         and so does the 4/2 step of a bank whose state fits L2 anyway (at
-                                        most 38 MiB of x, P, stepped in place); BKE_KF_ORDER=0 in the
-                                        environment makes the 4/2 step ignore it always. */
+                                        most 38 MiB of x, P, stepped in place). */
 
 int bke_abi_version(void);
 const char *bke_last_error(void);
@@ -96,7 +95,6 @@ int bke_device_count(void);
  * shape, and — fp32 banks with dim_x = 16 or 32 whose F and Q are shared (stride 0) — the wgmma tile: F P F' as
  * three-term TF32 products accumulated in fp32 (everything else of the
  * step in plain fp32), the whole predict+update in one launch when H and R are shared too and dim_z <= 4.
- * Environment switches (measurements): BKE_KF_TC=0 keeps those banks on the CUDA cores.
  */
 typedef struct bke_kf_args {
     int64_t n_filters;
@@ -141,8 +139,8 @@ int bke_kf_step(const bke_kf_args *args, void *stream);
  *   bke_kf_step_sym          bke_kf_step with the record standing in for args->Q and args->R (which
  *                            must still be the per-filter arrays it was packed from, unchanged since);
  *                            the results are bit-identical to bke_kf_step's.
- * Both calls return BKE_ERR_UNSUPPORTED for other shapes, dtypes, shared models or misaligned pointers,
- * and when the environment sets BKE_KF_SYM=0; bke_kf_step is then the call to make. */
+ * Both calls return BKE_ERR_UNSUPPORTED for other shapes, dtypes, shared models or misaligned pointers;
+ * bke_kf_step is then the call to make. */
 size_t bke_kf_sym_models_bytes(int64_t n_filters);
 int bke_kf_pack_sym_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *Q,
                            const void *R, void *record, int32_t *asymmetric, void *stream);
@@ -194,9 +192,9 @@ int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream);
  *                               (BKE_REVERSE_TILES is honoured as in a single step), an in-place state
  *                               (x_out = x, P_out = P), 1 <= n_steps <= BKE_KF42_MAX_RING, and neither
  *                               z_valid, B / u, status nor any optional output: anything else returns
- *                               BKE_ERR_UNSUPPORTED, and so does BKE_KF_RING=0 in the environment.
- * The calls return BKE_ERR_UNSUPPORTED for other shapes, dtypes, shared models, an asymmetric map,
- * misaligned pointers, and when the environment sets BKE_KF_SYM=0; bke_kf_step is then the call to make. */
+ *                               BKE_ERR_UNSUPPORTED.
+ * The calls return BKE_ERR_UNSUPPORTED for other shapes, dtypes, shared models, an asymmetric map or
+ * misaligned pointers; bke_kf_step is then the call to make. */
 #define BKE_KF42_MODEL_WORDS 37
 #define BKE_KF42_MAX_RING 8
 typedef struct bke_kf_model_map {

@@ -27,7 +27,7 @@ Prints JSON lines (and writes them to DIR/kf42_ceiling.jsonl with --out):
              graphs of 4 separate steps, at N = 2^19 .. 2^22 (all above the bound under which
              the L2 hints are used); per-step time and GB/s for every N, counted with the bytes the
              step moves (168 + 4 per distinct plane of the packed model words, i.e. per varying word
-             not flagged in the map's `duplicate`: 188 for the bench bank; 344 with BKE_KF_SYM=0)
+             not flagged in the map's `duplicate`: 188 for the bench bank)
   fit        t(N) = a + b N over those sizes: a is the fixed cost of a step, bytes / b its
              streaming rate
   shared     the same graph of 4 steps for a 2^20-filter bank whose F/H/Q/R are shared (one model

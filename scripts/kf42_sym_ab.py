@@ -1,10 +1,10 @@
-"""A/B of the 4/2 fp32 bank step with its models read dense (344 B per filter-step) or as the packed
-model words that differ between the filters, each distinct plane read once (188 B on the bench bank,
-whose 10 varying words hold 5 distinct planes), against another checkout (e.g. the parent commit), and
-the one-time cost of scanning and packing the models.
+"""A/B of the 4/2 fp32 bank step, which reads the packed model words that differ between the filters,
+each distinct plane once (188 B per filter-step on the bench bank, whose 10 varying words hold 5
+distinct planes), against another checkout (e.g. the parent commit), and the one-time cost of scanning
+and packing the models.
 
-    python scripts/kf42_sym_ab.py [--out DIR] [--rounds R] [--steps 400,50] [--diag-rounds D]
-                                  [--baseline-tree DIR]
+    python scripts/kf42_sym_ab.py --baseline-tree DIR [--out DIR] [--rounds R] [--steps 400,50]
+                                  [--diag-rounds D]
 
 Prints JSON lines (and writes them to DIR/kf42_sym_ab.jsonl with --out):
 
@@ -18,12 +18,12 @@ Prints JSON lines (and writes them to DIR/kf42_sym_ab.jsonl with --out):
            and the kernel time of the headline
   diag     one `bench.py --no-cpu --no-resample --steps 50` per arm and round: the ms_per_step of the
            kf_c2_diagnostics leg (the same kernel with its optional outputs)
-  summary  per arm and step count: the median ms_per_step, and the change against the dense arm
+  summary  per arm and step count: the median ms_per_step, and the change against the baseline arm
 
-Arms, alternated inside every round, each in its own process: `dense` (BKE_KF_SYM=0) and `packed`
-(the default) of this tree, and `baseline` (bench.py of another checkout, e.g. the parent commit
-built in place) when --baseline-tree is given.  The summary's `repay_steps` is the scan + pack time
-over the per-step saving against the baseline at 400 steps.
+Arms, alternated inside every round, each in its own process: `tree` (bench.py of this tree) and
+`baseline` (bench.py of the checkout at --baseline-tree, e.g. the parent commit built in place).  The
+summary's `repay_steps` is the scan + pack time over the per-step saving against the baseline at 400
+steps.
 """
 import argparse
 import importlib.util
@@ -143,10 +143,8 @@ def all_words(rounds):
             **{k: {"median_ms": float(np.median(v)), "ms_rounds": v} for k, v in ms.items()}}
 
 
-def bench(cwd, env_extra, argv):
-    env = dict(os.environ)
-    env.update(env_extra)
-    r = subprocess.run([sys.executable, "bench.py", "--gpus", "1"] + argv, cwd=cwd, env=env,
+def bench(cwd, argv):
+    r = subprocess.run([sys.executable, "bench.py", "--gpus", "1"] + argv, cwd=cwd,
                        capture_output=True, text=True, timeout=1800)
     if r.returncode != 0:
         raise RuntimeError("bench.py failed in %s:\n%s\n%s" % (cwd, r.stdout[-3000:], r.stderr[-3000:]))
@@ -159,7 +157,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=5, help="rounds per step count (each runs every arm once)")
     ap.add_argument("--steps", default="400,50", help="comma-separated --steps values")
     ap.add_argument("--diag-rounds", type=int, default=2, help="rounds of the bench run with the diagnostics leg (0: none)")
-    ap.add_argument("--baseline-tree", default=None, help="a checkout whose bench.py is the third arm")
+    ap.add_argument("--baseline-tree", required=True, help="the checkout whose bench.py is the baseline arm")
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "kf42_sym_ab.py measures on a GPU"
@@ -179,33 +177,31 @@ def main():
     torch.cuda.empty_cache()
     emit(all_words(args.rounds))
     torch.cuda.empty_cache()
-    arms = [("dense", ROOT, {"BKE_KF_SYM": "0"}), ("packed", ROOT, {})]
-    if args.baseline_tree:
-        arms.append(("baseline", os.path.abspath(args.baseline_tree), {}))
+    arms = [("tree", ROOT), ("baseline", os.path.abspath(args.baseline_tree))]
     res = {}
     for K in [int(k) for k in args.steps.split(",")]:
         for r in range(args.rounds):
             order = arms if r % 2 == 0 else arms[::-1]
-            for name, cwd, env in order:
-                j = bench(cwd, env, ["--steps", str(K), "--warmup", "5", "--no-cpu", "--no-extra", "--no-resample"])
+            for name, cwd in order:
+                j = bench(cwd, ["--steps", str(K), "--warmup", "5", "--no-cpu", "--no-extra", "--no-resample"])
                 res.setdefault((name, K), []).append(j["ms_per_step"])
                 emit({"what": "run", "arm": name, "steps": K, "round": r, "ms_per_step": j["ms_per_step"],
                       "kernel_ms": j["roofline"]["kernel_ms"], "value": j["value"]})
     diag = {}
     for r in range(args.diag_rounds):
         order = arms if r % 2 == 0 else arms[::-1]
-        for name, cwd, env in order:
-            j = bench(cwd, env, ["--steps", "50", "--warmup", "5", "--no-cpu", "--no-resample"])
+        for name, cwd in order:
+            j = bench(cwd, ["--steps", "50", "--warmup", "5", "--no-cpu", "--no-resample"])
             diag.setdefault(name, []).append(j["kf_c2_diagnostics"]["ms_per_step"])
             emit({"what": "diag", "arm": name, "round": r, "kf_c2_diagnostics_ms": j["kf_c2_diagnostics"]["ms_per_step"]})
     summary = {}
     for (name, K), v in sorted(res.items()):
         med = float(np.median(v))
-        dense = float(np.median(res[("dense", K)]))
+        base = float(np.median(res[("baseline", K)]))
         summary["%s_%d" % (name, K)] = {"median_ms": med, "min_ms": min(v), "max_ms": max(v),
-                                        "gain_vs_dense": dense / med - 1.0}
+                                        "gain_vs_baseline": base / med - 1.0}
     if ("baseline", 400) in res:
-        saved = float(np.median(res[("baseline", 400)])) - float(np.median(res[("packed", 400)]))
+        saved = float(np.median(res[("baseline", 400)])) - float(np.median(res[("tree", 400)]))
         summary["repay_steps"] = pack["ms"] / saved if saved > 0 else None
     for name, v in diag.items():
         summary["diag_%s" % name] = {"median_ms": float(np.median(v)), "all_ms": v}

@@ -1,5 +1,5 @@
 """wgmma covariance propagation (csrc/kf_tc.cu) against NumPy fp64: errors and timings.
-python scripts/tc_check.py [check|time]   (BKE_KF_TC=0 selects the CUDA-core kernels for the same calls)"""
+python scripts/tc_check.py [check|time]"""
 import json
 import os
 import sys
@@ -70,14 +70,14 @@ def time_():
             kf.predict(); kf._flush()
         ms = timeit(pred)
         bpu = (2 * n + 2 * n * n) * 4
-        print(json.dumps({"case": "predict %d shared f32 N=%d tc=%s" % (n, N, os.environ.get("BKE_KF_TC", "1")), "ms": round(ms, 4),
+        print(json.dumps({"case": "predict %d shared f32 N=%d" % (n, N), "ms": round(ms, 4),
                           "GBps": round(N * bpu / ms / 1e6, 1), "frac": round(N * bpu / ms / 1e6 / PEAK, 4)}), flush=True)
 
         def step():
             kf.predict(); kf.update(zd)
         ms = timeit(step)
         bpu = (2 * n + 2 * n * n + m) * 4
-        print(json.dumps({"case": "predict+update %d/%d shared f32 N=%d tc=%s" % (n, m, N, os.environ.get("BKE_KF_TC", "1")), "ms": round(ms, 4),
+        print(json.dumps({"case": "predict+update %d/%d shared f32 N=%d" % (n, m, N), "ms": round(ms, 4),
                           "GBps": round(N * bpu / ms / 1e6, 1), "frac": round(N * bpu / ms / 1e6 / PEAK, 4)}), flush=True)
 
 
