@@ -74,6 +74,7 @@ class KfArgs(ctypes.Structure):
         ("log_likelihood", c_void_p),
         ("status", c_void_p),
         ("F_host", c_void_p), ("Q_host", c_void_p), ("H_host", c_void_p), ("R_host", c_void_p),
+        ("tile_order", c_void_p),
     ]
 
 

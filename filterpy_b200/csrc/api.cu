@@ -322,6 +322,7 @@ int bke_kf_steps_packed(const bke_kf_args *args, const void *record, const bke_k
     if (rc) return rc;
     if ((rc = validate_packed(record, host_map))) return rc;
     if (!zs) { set_error("zs is NULL"); return BKE_ERR_BAD_ARG; }
+    if (reinterpret_cast<uintptr_t>(args->tile_order) & 3u) { set_error("tile_order must be 4-byte aligned"); return BKE_ERR_BAD_ARG; }
     // what only the fused ring refuses (launch_kf_fast refuses the rest), before anything is launched
     const bke_kf_args &a = *args;
     auto refuse = [](const char *why) { set_error("bke_kf_steps_packed: %s", why); return BKE_ERR_UNSUPPORTED; };

@@ -17,6 +17,8 @@
 //   * the CTAs walk the tiles in a launch order (tile = blockIdx.x + k gridDim.x) that maps to the bank
 //     first to last, or last to first with BKE_REVERSE_TILES: a caller that alternates the two starts
 //     every step on the tiles the previous step finished, whose state and models are still in L2.
+//     The fused ring may take the order from a device word instead (bke_kf_args.tile_order): the parity
+//     of a launch count the kernel itself advances, so that one captured launch alternates across replays.
 // Shared models (stride 0) are read once per thread through the read-only path instead of TMA.
 // A bank whose per-filter Q and R are exactly symmetric may instead hand over a packed copy of their
 // upper triangles (bke_kf_pack_sym_models, REC == 1): one bulk copy per tile replaces the two of
@@ -46,6 +48,21 @@ __device__ __forceinline__ void st_hint(float *addr, float4 v, uint64_t pol)
 {
     asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;"
                  ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
+}
+
+// the tile-order word of the fused ring (FastP::order): a relaxed read at GPU scope (never a stale L1 line), and
+// the acq_rel arrival of a CTA
+__device__ __forceinline__ uint32_t ld_relaxed_gpu(const uint32_t *addr)
+{
+    uint32_t v;
+    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint32_t atom_add_acq_rel_gpu(uint32_t *addr, uint32_t v)
+{
+    uint32_t old;
+    asm volatile("atom.add.acq_rel.gpu.global.u32 %0, [%1], %2;" : "=r"(old) : "l"(addr), "r"(v) : "memory");
+    return old;
 }
 
 // ---------------------------------------------------------------------------- tile geometry
@@ -189,6 +206,8 @@ struct FastP {
     const float *zs[BKE_KF42_MAX_RING];     // RING: the measurements of step k (p.z is not read),
     int n_steps;                            // for k < n_steps
     int ring_ox, ring_oz, ring_stage;       // RING: the stage laid out for this launch (ring_layout)
+    uint32_t *order;                        // RING: the bank's tile-order word {epoch, arrived} (device), or
+                                            // NULL: `reverse` decides (last, so no other field moves)
 };
 
 // MODE: 3 = predict+update, 1 = predict only, 2 = update only
@@ -296,10 +315,16 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
     // stream (the previous step, or whatever produced z) may have written any of it, and only
     // griddepcontrol.wait makes those writes visible.
     griddep_wait();
+    // RING with an order word: the launch walks the bank last to first when the bank's count of such launches
+    // (epoch) is odd, so that consecutive launches alternate whether they come from one graph replay or from
+    // two.  Read once per CTA, after the wait (the previous launch may have advanced it), and shared.
+    __shared__ uint32_t order_epoch;
+    if (RING && p.order && tid == 0) order_epoch = ld_relaxed_gpu(p.order);
     __syncthreads();
     // Launch-order tile t stands for the bank's tile base + sign t; both are formed once from the
-    // parameters, so that the per-tile address arithmetic stays uniform.
-    const int base = p.reverse ? p.num_tiles - 1 : 0, sign = p.reverse ? -1 : 1;
+    // parameters (or the order word), so that the per-tile address arithmetic stays uniform.
+    const int reverse = RING && p.order ? (int)(order_epoch & 1u) : p.reverse;
+    const int base = reverse ? p.num_tiles - 1 : 0, sign = reverse ? -1 : 1;
     if (tid == 0) {
         for (int s = 0; s < STAGES; s++) {
             int tile = blockIdx.x + s * gridDim.x;
@@ -614,6 +639,15 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
                     *reinterpret_cast<float4 *>(p.P_out + f * N * N + i * N) = make_float4(P[i][0], P[i][1], P[i][2], P[i][3]);
             }
             if (EXTRAS && p.status && (st != BKE_STATUS_OK || !p.sticky)) p.status[f] = st;
+        }
+    }
+    // Advance the order word: every CTA arrives once, after its read of epoch; the last to arrive resets the
+    // count and bumps epoch.  No CTA of this launch reads epoch after that, and the next launch reads it only
+    // after its griddepcontrol.wait, which sees every write of this one.
+    if (RING && p.order && tid == 0) {
+        if (atom_add_acq_rel_gpu(p.order + 1, 1u) == gridDim.x - 1) {
+            p.order[1] = 0u;
+            p.order[0] = order_epoch + 1u;
         }
     }
 }
@@ -1000,8 +1034,9 @@ int launch_kf_fast(const bke_kf_args &a, cudaStream_t s, const void *rec, const 
     // keep-the-state-in-L2 hints pay off when x, P fit the L2 together with the streaming traffic
     p.l2_hints = (N * 80 <= (int64_t)38 << 20) && a.x_out == a.x && a.P_out == a.P;
     // a bank whose state stays in L2 between steps (l2_hints) has nothing to gain from the order: it
-    // keeps walking first to last
+    // keeps walking first to last (a ring given an order word follows the word, which is harmless there)
     p.reverse = (a.flags & BKE_REVERSE_TILES) && !p.l2_hints;
+    p.order = ring ? a.tile_order : nullptr;
     p.x = (const float *)a.x; p.P = (const float *)a.P; p.z = (const float *)a.z;
     p.F = (const float *)a.F; p.Q = (const float *)a.Q; p.H = (const float *)a.H; p.R = (const float *)a.R;
     p.rec = (const float *)rec;

@@ -77,6 +77,7 @@ class KalmanFilter(_BankMirror):
         self._model_version = 0
         self._model_last = None       # the token of the previous launch
         self._ring_notes = None       # capture(): what each launch of the capture pass was (see _fuse_ring)
+        self._tile_order = None       # the fused rings' tile-order word {epoch, arrived} (device, see _fuse_ring)
 
     # ------------------------------------------------------------------ hooks of _BankMirror
     def _state_rebound(self):
@@ -383,10 +384,13 @@ class KalmanFilter(_BankMirror):
         graph.
 
         Consecutive launches walk the bank in alternating tile order (``BKE_REVERSE_TILES``, a
-        scheduling hint: the results are the same either way), and each captured launch keeps the
-        order it was captured with.  A graph with an even number of launches therefore alternates
-        across replays too; with an odd number, the first launch of a replay runs in the same order as
-        the last launch of the previous one, which costs that step the L2 reuse but nothing else.
+        scheduling hint: the results are the same either way).  In a graph of separate steps each
+        captured launch keeps the order it was captured with: a graph with an even number of launches
+        therefore alternates across replays too; with an odd number, the first launch of a replay runs
+        in the same order as the last launch of the previous one, which costs that step the L2 reuse
+        but nothing else.  The launches of a fused ring (below) instead take their order from a word
+        the bank keeps on the device and each launch advances, so they alternate across replays
+        whatever their number, a ring of one launch included.
 
         A ring of K plain ``predict(); update(z_i)`` pairs of such a bank (``diagnostics=False``, no
         ``valid``, no per-call model, and nothing else in ``fn``: no torch op, no other bank) is returned
@@ -421,12 +425,17 @@ class KalmanFilter(_BankMirror):
         zs = [n[3] for n in notes]
         M = _lib.BKE_KF42_MAX_RING
         rings = [(ctypes.c_void_p * len(c))(*[ptr(z) for z in c]) for c in (zs[i:i + M] for i in range(0, len(zs), M))]
-        # consecutive launches of a replay alternate the tile order, like consecutive steps
-        order = {id(r): (_lib.BKE_REVERSE_TILES if j % 2 else 0) for j, r in enumerate(rings)}
+        # consecutive launches alternate the tile order, within a replay and across replays: each launch reads
+        # the parity of the bank's launch count from this word and advances it on the device (a flag would be
+        # frozen into the captured launch).  One word per bank, allocated here, outside any capture.
+        if self._tile_order is None:
+            self._tile_order = torch.zeros(2, dtype=torch.int32, device=self._device)
+        order = self._tile_order
+        a.flags = step
+        a.tile_order = ptr(order)
         hmap, recp = self._sym_host_map, ptr(rec) if rec.numel() else None
 
         def call(ring):
-            a.flags = step | order[id(ring)]
             return self._lib.bke_kf_steps_packed(a, recp, hmap, ring, len(ring), stream_ptr(self._device))
 
         def fused():
@@ -444,7 +453,7 @@ class KalmanFilter(_BankMirror):
             self._run(call, ring)
         ring_graph = StepGraph(fused, self._device, warmup=0)
         ring_graph.launches, ring_graph.fused_steps = len(rings), len(zs)
-        ring_graph._keep = (a, rec, hmap, rings, zs)        # what the captured launches point into
+        ring_graph._keep = (a, rec, hmap, rings, zs, order)     # what the captured launches point into
         return ring_graph
 
     # ------------------------------------------------------------------ batch_filter

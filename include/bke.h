@@ -65,7 +65,10 @@ extern "C" {
                                         step, so that each step starts on the filters the previous one finished
                                         while their x, P and models are still in L2.  Other kernels ignore it,
                                         and so does the 4/2 step of a bank whose state fits L2 anyway (at
-                                        most 38 MiB of x, P, stepped in place). */
+                                        most 38 MiB of x, P, stepped in place).  bke_kf_steps_packed given
+                                        a tile-order word (bke_kf_args.tile_order) ignores it too: the word
+                                        alternates the order across launches on the device, where a flag
+                                        frozen into a captured launch cannot. */
 
 int bke_abi_version(void);
 const char *bke_last_error(void);
@@ -120,6 +123,13 @@ typedef struct bke_kf_args {
      * four are given (and equal the device copies) a kernel may carry them in its launch parameters
      * instead of loading them from device memory.  NULL = not available. */
     const void *F_host, *Q_host, *H_host, *R_host;
+    /* Optional DEVICE tile-order word of the bank, two uint32 {epoch, arrived}, zeroed once by the caller,
+     * 4-byte aligned; read by bke_kf_steps_packed only (every other call ignores it).  A launch walks the
+     * bank last tile to first when epoch is odd (BKE_REVERSE_TILES is then ignored), and leaves epoch one
+     * higher and arrived at 0 when it ends, so consecutive launches on one word alternate, including the
+     * replays of a captured graph of one launch.  Launches that share a word must run in stream order.
+     * NULL = not used. */
+    uint32_t *tile_order;
 } bke_kf_args;
 
 int bke_kf_step(const bke_kf_args *args, void *stream);
@@ -189,7 +199,9 @@ int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream);
  *                               x and P exist nowhere in memory.  zs is a HOST array of n_steps device
  *                               pointers, each [N,2], 16-byte aligned and clear of x and P; the same pointer
  *                               may appear more than once.  It takes flags = BKE_DO_PREDICT | BKE_DO_UPDATE
- *                               (BKE_REVERSE_TILES is honoured as in a single step), an in-place state
+ *                               (BKE_REVERSE_TILES is honoured as in a single step when args->tile_order
+ *                               is NULL; with a tile-order word the word decides, and a word that is not
+ *                               4-byte aligned is refused with BKE_ERR_BAD_ARG), an in-place state
  *                               (x_out = x, P_out = P), 1 <= n_steps <= BKE_KF42_MAX_RING, and neither
  *                               z_valid, B / u, status nor any optional output: anything else returns
  *                               BKE_ERR_UNSUPPORTED.

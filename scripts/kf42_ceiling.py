@@ -35,9 +35,12 @@ Prints JSON lines (and writes them to DIR/kf42_ceiling.jsonl with --out):
   ring       the fused ring (bke_kf_steps_packed, what KalmanFilter.capture returns for a ring of plain
              steps) at N = 2^19 .. 2^22 and K = 2, 4, 8 steps per launch, the arms alternated inside every
              round: `twin`, the memory-only kernel moving the ring's 180 + 8 K B per filter; `steps`, the
-             graph of K separate steps; `fused`, a graph of one fused launch; `fused_alt`, two such graphs
-             in forward and reversed tile order replayed in turn.  ms per step (median of rounds) and, for
-             twin and fused, GB/s of the ring's bytes.  --ring prints only the card and these lines.
+             graph of K separate steps; `fused`, a graph of one fused launch that takes its tile order from
+             a bank-owned order word (bke_kf_args.tile_order), so consecutive replays alternate forward and
+             reverse, as KalmanFilter.capture runs it; `fused_forward`, the same graph with tile_order
+             cleared, so every replay walks the bank first to last.  ms per step (median of rounds), for twin
+             and fused GB/s of the ring's bytes, and alt_gain = fused_forward / fused - 1.  --ring prints
+             only the card and these lines.
 
 The ceiling kernel is compiled with nvcc into scripts/kf42_ceiling.so (git-ignored) when that file
 is missing or older than its source.  BKE_LIB_PATH selects the engine library as everywhere else.
@@ -238,36 +241,33 @@ def ring(torch, rounds):
         assert kf._sym_buf is not None, "the bank does not step from the packed model words"
         zs = torch.randn(8, N, 2, device=dev)
         tw = {k: torch.randn(N * e, device=dev) for k, e in (("x", 4), ("P", 16), ("Q", 5))}
-        a = _lib.KfArgs.from_buffer_copy(next(iter(kf._args_cache.values()))[1])
-        a.z_valid = None
+        a_fwd = _lib.KfArgs.from_buffer_copy(next(iter(kf._args_cache.values()))[1])
+        a_fwd.z_valid, a_fwd.flags, a_fwd.tile_order = None, 3, None
+        order = torch.zeros(2, dtype=torch.int32, device=dev)
+        a_word = _lib.KfArgs.from_buffer_copy(a_fwd)
+        a_word.tile_order = order.data_ptr()
         for K in (2, 4, 8):
             arr = (ctypes.c_void_p * K)(*[zs[k].data_ptr() for k in range(K)])
 
-            def fused(flags):
-                a.flags = flags
+            def fused(a):
                 _lib.check(lib.bke_kf_steps_packed(a, kf._sym_buf.data_ptr(), kf._sym_host_map, arr, K,
                                                    torch.cuda.current_stream().cuda_stream))
 
             def steps():
                 for k in range(K):
                     kf.predict(); kf.update(zs[k])
-            fused(3)                                    # the one-time function attribute, outside capture
-            g_fwd = StepGraph(lambda: fused(3), dev, warmup=1)
-            g_rev = StepGraph(lambda: fused(3 | _lib.BKE_REVERSE_TILES), dev, warmup=1)
+            fused(a_fwd)                                # the one-time function attribute, outside capture
+            g_word = StepGraph(lambda: fused(a_word), dev, warmup=1)
+            g_fwd = StepGraph(lambda: fused(a_fwd), dev, warmup=1)
             g_steps = StepGraph(steps, dev)
-            assert g_fwd.nodes == 1 and g_steps.nodes == K
-            flip = {"i": 0}
-
-            def alt():
-                flip["i"] ^= 1
-                (g_rev if flip["i"] else g_fwd).replay()
+            assert g_word.nodes == 1 and g_fwd.nodes == 1 and g_steps.nodes == K
 
             def twin(grid):
                 rc = tlib.kf42_ring_traffic(tw["x"].data_ptr(), tw["P"].data_ptr(), tw["Q"].data_ptr(), zs.data_ptr(), N,
                                             grid, K, torch.cuda.current_stream().cuda_stream)
                 assert rc == 0, rc
             arms = [("twin_4", lambda: twin(4 * sms)), ("twin_8", lambda: twin(8 * sms)), ("steps", g_steps.replay),
-                    ("fused", g_fwd.replay), ("fused_alt", alt)]
+                    ("fused", g_word.replay), ("fused_forward", g_fwd.replay)]
             reps = max(4, reps_for(N) // K) // 2 * 2
             ms = {}
             for r in range(rounds):
@@ -281,11 +281,11 @@ def ring(torch, rounds):
             gbs = lambda t: moved * N / (t * K * 1e-3) / 1e9
             lines.append({"what": "ring", "n_filters": N, "steps_per_launch": K, "bytes_per_filter_launch": moved,
                           "ms_per_step": {"twin": twin_ms, "steps": med["steps"], "fused": med["fused"],
-                                          "fused_alt": med["fused_alt"]},
+                                          "fused_forward": med["fused_forward"]},
                           "GBps": {"twin": gbs(twin_ms), "fused": gbs(med["fused"])},
                           "fused_over_twin": med["fused"] / twin_ms, "steps_over_fused": med["steps"] / med["fused"],
-                          "alt_gain": med["fused"] / med["fused_alt"] - 1.0})
-        del kf, zs, tw
+                          "alt_gain": med["fused_forward"] / med["fused"] - 1.0})
+        del kf, zs, tw, order
         torch.cuda.empty_cache()
     return lines
 
