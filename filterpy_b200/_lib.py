@@ -25,7 +25,7 @@ BKE_HOOK_X_MEAN, BKE_HOOK_Z_MEAN, BKE_HOOK_RESIDUAL_X, BKE_HOOK_RESIDUAL_Z, BKE_
 # every symbol include/bke.h declares (tests check that the library exports all of them)
 EXPORTED_SYMBOLS = [
     "bke_abi_version", "bke_last_error", "bke_device_count",
-    "bke_kf_step", "bke_kf_batch_filter", "bke_ukf_step",
+    "bke_kf_step", "bke_kf_step_correlated", "bke_kf_update_rows", "bke_kf_batch_filter", "bke_ukf_step",
     "bke_fls_workspace_bytes", "bke_fls_smooth",
     "bke_kf_sym_models_bytes", "bke_kf_pack_sym_models", "bke_kf_step_sym",
     "bke_kf_scan_models", "bke_kf_packed_models_bytes", "bke_kf_pack_models", "bke_kf_step_packed",
@@ -75,6 +75,16 @@ class KfArgs(ctypes.Structure):
         ("status", c_void_p),
         ("F_host", c_void_p), ("Q_host", c_void_p), ("H_host", c_void_p), ("R_host", c_void_p),
         ("tile_order", c_void_p),
+    ]
+
+
+class KfRowsArgs(ctypes.Structure):
+    _fields_ = [
+        ("step", KfArgs),
+        ("start", c_int32), ("rows", c_int32),
+        ("H_i", c_void_p), ("H_i_stride", c_int64),
+        ("R_i", c_void_p), ("R_i_stride", c_int64),
+        ("z_record", c_void_p),
     ]
 
 
@@ -362,6 +372,10 @@ def load():
     lib.bke_device_count.restype = ctypes.c_int
     lib.bke_kf_step.argtypes = [ctypes.POINTER(KfArgs), c_void_p]
     lib.bke_kf_step.restype = ctypes.c_int
+    lib.bke_kf_step_correlated.argtypes = [ctypes.POINTER(KfArgs), c_void_p, c_int64, c_void_p]
+    lib.bke_kf_step_correlated.restype = ctypes.c_int
+    lib.bke_kf_update_rows.argtypes = [ctypes.POINTER(KfRowsArgs), c_void_p]
+    lib.bke_kf_update_rows.restype = ctypes.c_int
     lib.bke_kf_sym_models_bytes.argtypes = [c_int64]
     lib.bke_kf_sym_models_bytes.restype = c_size_t
     lib.bke_kf_pack_sym_models.argtypes = [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -222,6 +222,68 @@ int bke_kf_step(const bke_kf_args *args, void *stream)
     return launch_kf_any(*args, s);
 }
 
+// the flags of the two other update forms: an update, optionally after a predict
+static int validate_update_form(const bke_kf_args *a)
+{
+    if (!(a->flags & BKE_DO_UPDATE) || (a->flags & ~(BKE_DO_PREDICT | BKE_DO_UPDATE | BKE_STATUS_STICKY | BKE_REVERSE_TILES))) {
+        set_error("flags must be BKE_DO_UPDATE, optionally with BKE_DO_PREDICT and BKE_STATUS_STICKY");
+        return BKE_ERR_BAD_ARG;
+    }
+    return BKE_OK;
+}
+
+int bke_kf_step_correlated(const bke_kf_args *args, const void *M, int64_t M_stride, void *stream)
+{
+    int rc = validate_kf(args, true);
+    if (rc || (rc = validate_update_form(args))) return rc;
+    if (!M) { set_error("M is NULL"); return BKE_ERR_BAD_ARG; }
+    if (M_stride != 0 && M_stride != (int64_t)args->dim_x * args->dim_z) {
+        set_error("M_stride must be 0 (shared) or dim_x * dim_z");
+        return BKE_ERR_BAD_ARG;
+    }
+    if ((rc = require_device())) return rc;
+    if (args->n_filters == 0) return BKE_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    rc = launch_kf_direct_correlated(*args, M, M_stride, s);
+    if (rc == BKE_ERR_UNSUPPORTED) rc = launch_kf_generic_correlated(*args, M, M_stride, s);
+    return rc;
+}
+
+int bke_kf_update_rows(const bke_kf_rows_args *args, void *stream)
+{
+    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    const bke_kf_args &a = args->step;
+    const int64_t n = a.dim_x, m = a.dim_z, L = args->rows, start = args->start;
+    if (L < 1 || start < 0 || start + L > m) {
+        set_error("the block of rows %lld .. %lld is not within the %lld rows of z", (long long)start, (long long)(start + L - 1), (long long)m);
+        return BKE_ERR_BAD_ARG;
+    }
+    if (args->H_i_stride != 0 && args->H_i_stride != L * n) { set_error("H_i_stride must be 0 (shared) or rows * dim_x"); return BKE_ERR_BAD_ARG; }
+    if (args->R_i_stride != 0 && args->R_i_stride != L * L) { set_error("R_i_stride must be 0 (shared) or rows * rows"); return BKE_ERR_BAD_ARG; }
+    if (a.S || a.SI || a.log_likelihood) { set_error("update_rows does not write S, SI or log_likelihood: they must be NULL"); return BKE_ERR_BAD_ARG; }
+    // the checks of bke_kf_step on the bank's arrays; a caller-supplied block stands in for H or R there
+    bke_kf_args chk = a;
+    if (args->H_i) { chk.H = args->H_i; chk.H_stride = 0; }
+    if (args->R_i) { chk.R = args->R_i; chk.R_stride = 0; }
+    int rc = validate_kf(&chk, true);
+    if (rc || (rc = validate_update_form(&a))) return rc;
+    if ((rc = require_device())) return rc;
+    if (a.n_filters == 0) return BKE_OK;
+    // the block as an update of L rows: H_i is contiguous in the bank's H, R_i has the row pitch m there
+    const size_t es = a.dtype == BKE_F32 ? 4 : 8;
+    bke_kf_args b = a;
+    b.dim_z = (int32_t)L;
+    if (args->H_i) { b.H = args->H_i; b.H_stride = args->H_i_stride; }
+    else b.H = (const char *)a.H + start * n * es;
+    int rpitch = (int)L;
+    if (args->R_i) { b.R = args->R_i; b.R_stride = args->R_i_stride; }
+    else { b.R = (const char *)a.R + (start * m + start) * es; rpitch = (int)m; }
+    cudaStream_t s = (cudaStream_t)stream;
+    rc = launch_kf_direct_rows(b, (int)m, (int)start, rpitch, args->z_record, s);
+    if (rc == BKE_ERR_UNSUPPORTED) rc = launch_kf_generic_rows(b, (int)m, (int)start, rpitch, args->z_record, s);
+    return rc;
+}
+
 size_t bke_kf_sym_models_bytes(int64_t n_filters) { return kf_sym_models_bytes(n_filters); }
 
 int bke_kf_pack_sym_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *Q,

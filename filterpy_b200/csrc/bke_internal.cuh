@@ -52,6 +52,13 @@ int launch_kf_pack_models(int64_t n_filters, const void *F, const void *Q, const
 int kf_model_planes(const bke_kf_model_map &map, int (&plane)[BKE_KF42_MODEL_WORDS]);
 int launch_kf_rowblock(const bke_kf_args &a, cudaStream_t s);
 int launch_kf_direct(const bke_kf_args &a, cudaStream_t s);
+// update_correlated and update_sequential's row block (bke_kf_step_correlated, bke_kf_update_rows): register tiles
+// for the shapes launch_kf_direct covers (BKE_ERR_UNSUPPORTED otherwise), the warp-per-filter kernel for any other.
+// The rows calls take `a` with dim_z = L and H, R, z at the block; m is the bank's dim_z, the pitch of y, K and zrec.
+int launch_kf_direct_correlated(const bke_kf_args &a, const void *M, int64_t M_stride, cudaStream_t s);
+int launch_kf_generic_correlated(const bke_kf_args &a, const void *M, int64_t M_stride, cudaStream_t s);
+int launch_kf_direct_rows(const bke_kf_args &a, int m, int start, int rpitch, void *zrec, cudaStream_t s);
+int launch_kf_generic_rows(const bke_kf_args &a, int m, int start, int rpitch, void *zrec, cudaStream_t s);
 // wgmma covariance propagation for shared-model fp32 banks with dim_x = 16 / 32 (kf_tc.cu); a fused step runs
 // its update through launch_kf_any afterwards
 int launch_kf_tc(const bke_kf_args &a, cudaStream_t s);

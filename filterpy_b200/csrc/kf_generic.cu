@@ -11,6 +11,10 @@
 //   update   :515-561   y = z - Hx; S = H P H' + R; SI = inv(S); K = P H' SI; x += K y;
 //                       P = (I-KH) P (I-KH)' + K R K'      (Joseph form)
 //   z is None:515-520   posterior := prior
+// and, with the update form a template parameter (DESIGN.md §3.10):
+//   update_correlated  :730-748   S = H P H' + H M + M' H' + R; K = (P H' + M) SI; P = P - K (H P + M')
+//   update_sequential  :778-824   the Joseph update of rows start .. start+L-1 (m = L here), K = P H' (1 / S)
+//                                 for L = 1; y, K and the z record are written in the block's rows / columns
 #include "bke_internal.cuh"
 #include "kf_warp.cuh"
 
@@ -31,7 +35,12 @@ struct KfP {
     T *x_prior, *P_prior, *K, *y, *S, *SI, *ll;
     int32_t *status;
     int sticky;                       // BKE_STATUS_STICKY: write status only on failure
+    const T *Mc; int64_t sM;          // FORM_CORRELATED: the cross-correlation M [N,n,m]
+    int mfull, start, rpitch;         // FORM_ROWS: the bank's dim_z, the block's first row, R's row pitch
+    T *zrec;                          // FORM_ROWS: the z record [N,mfull]
 };
+
+enum { FORM_PLAIN = 0, FORM_CORRELATED = 1, FORM_ROWS = 2 };
 
 // Gauss-Jordan inverse with partial pivoting of the m x m matrix A (destroyed) into Ai.
 // Returns false when a pivot is exactly zero (np.linalg.inv raises LinAlgError).
@@ -80,7 +89,7 @@ __device__ bool warp_inverse(T *A, T *Ai, T *col, int m, int lane, T &logdet)
     return true;
 }
 
-template <typename T>
+template <typename T, int FORM = FORM_PLAIN>
 __global__ void __launch_bounds__(128) kf_generic_kernel(KfP<T> p, int per_warp_elems)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -97,6 +106,8 @@ __global__ void __launch_bounds__(128) kf_generic_kernel(KfP<T> p, int per_warp_
     T *S = R + mm;       T *SI = S + mm;
     T *SA = SI + mm;     T *y = SA + mm;
     T *col = y + m;
+    T *Mc = col + m;     // FORM_CORRELATED only: M [n,m] and G = H P + M' [m,n]
+    T *G = Mc + nm;
 
     const bool do_predict = p.flags & BKE_DO_PREDICT;
     const bool do_update = p.flags & BKE_DO_UPDATE;
@@ -136,14 +147,81 @@ __global__ void __launch_bounds__(128) kf_generic_kernel(KfP<T> p, int per_warp_
             if (p.P_prior) for (int e = lane; e < nn; e += 32) p.P_prior[f * nn + e] = P[e];
         };
 
-        auto update = [&]() {
-            const bool has_z = (p.valid == nullptr) || (p.valid[f] != 0);
-            if (!has_z) {   // kalman_filter.py:515-520 — y = 0, posterior = prior
+        // kalman_filter.py:730-748
+        auto update_correlated = [&]() {
+            if (p.valid != nullptr && p.valid[f] == 0) {   // :705-710 — y = 0, posterior = prior
                 if (p.y) for (int a = lane; a < m; a += 32) p.y[f * m + a] = T(0);
                 return;
             }
             warp_copy_in(H, p.H + f * p.sH, nm, lane);
             warp_copy_in(R, p.R + f * p.sR, mm, lane);
+            warp_copy_in(Mc, p.Mc + f * p.sM, nm, lane);
+            __syncwarp();
+            for (int a = lane; a < m; a += 32) {
+                T s = T(0);
+                for (int q = 0; q < n; q++) s += H[a * n + q] * x[q];
+                y[a] = p.z[f * m + a] - s;
+            }
+            warp_mm<true>(P, H, n, n, m, lane, [&](int e, int, int, T s) { PHT[e] = s; });
+            __syncwarp();
+            // S = H PHT + H M + M' H' + R, with (M' H')[a][b] = (H M)[b][a]
+            for (int e = lane; e < mm; e += 32) {
+                const int a = e / m, b = e - a * m;
+                T s = T(0), hm = T(0), mh = T(0);
+                for (int q = 0; q < n; q++) {
+                    s += H[a * n + q] * PHT[q * m + b];
+                    hm += H[a * n + q] * Mc[q * m + b];
+                    mh += H[b * n + q] * Mc[q * m + a];
+                }
+                S[e] = s + hm + mh + R[e]; SA[e] = S[e];
+            }
+            __syncwarp();
+            if (p.S) for (int e = lane; e < mm; e += 32) p.S[f * mm + e] = S[e];
+            T logdet = T(0);
+            bool ok = warp_inverse(SA, SI, col, m, lane, logdet);
+            if (!ok) { st = BKE_STATUS_SINGULAR_S; return; }
+            for (int e = lane; e < nm; e += 32) PHT[e] += Mc[e];
+            __syncwarp();
+            warp_mm<false>(PHT, SI, n, m, m, lane, [&](int e, int, int, T s) { K[e] = s; });
+            __syncwarp();
+            for (int i = lane; i < n; i += 32) {
+                T s = T(0);
+                for (int q = 0; q < m; q++) s += K[i * m + q] * y[q];
+                xp[i] = x[i] + s;
+            }
+            warp_mm<false>(H, P, m, n, n, lane, [&](int e, int a, int j, T s) { G[e] = s + Mc[j * m + a]; });
+            __syncwarp();
+            for (int i = lane; i < n; i += 32) x[i] = xp[i];
+            warp_mm<false>(K, G, n, m, n, lane, [&](int e, int, int, T s) { F[e] = P[e] - s; });
+            __syncwarp();
+            for (int e = lane; e < nn; e += 32) P[e] = F[e];
+            if (p.K) for (int e = lane; e < nm; e += 32) p.K[f * nm + e] = K[e];
+            if (p.y) for (int a = lane; a < m; a += 32) p.y[f * m + a] = y[a];
+            if (p.SI) for (int e = lane; e < mm; e += 32) p.SI[f * mm + e] = SI[e];
+            if (p.ll && lane == 0) {
+                T q = T(0);
+                for (int a = 0; a < m; a++) {
+                    T s = T(0);
+                    for (int b = 0; b < m; b++) s += SI[a * m + b] * y[b];
+                    q += y[a] * s;
+                }
+                p.ll[f] = T(-0.5) * (q + logdet + T(m) * T(LOG_2PI));
+            }
+            __syncwarp();
+        };
+
+        auto update = [&]() {
+            const bool has_z = (p.valid == nullptr) || (p.valid[f] != 0);
+            if (!has_z) {   // kalman_filter.py:515-520 — y = 0, posterior = prior
+                if (FORM != FORM_ROWS && p.y) for (int a = lane; a < m; a += 32) p.y[f * m + a] = T(0);
+                return;
+            }
+            warp_copy_in(H, p.H + f * p.sH, nm, lane);
+            if constexpr (FORM == FORM_ROWS) {
+                for (int e = lane; e < mm; e += 32) R[e] = p.R[f * p.sR + (e / m) * p.rpitch + e % m];
+            } else {
+                warp_copy_in(R, p.R + f * p.sR, mm, lane);
+            }
             __syncwarp();
             for (int a = lane; a < m; a += 32) {
                 T s = T(0);
@@ -156,8 +234,13 @@ __global__ void __launch_bounds__(128) kf_generic_kernel(KfP<T> p, int per_warp_
             __syncwarp();
             if (p.S) for (int e = lane; e < mm; e += 32) p.S[f * mm + e] = S[e];
             T logdet = T(0);
-            bool ok = warp_inverse(SA, SI, col, m, lane, logdet);   // SA = scratch copy of S
-            if (!ok) { st = BKE_STATUS_SINGULAR_S; return; }
+            if (FORM == FORM_ROWS && m == 1) {
+                if (lane == 0) SI[0] = T(1) / SA[0];                 // PH' (1 / S): inf for S = 0, no LinAlgError
+                __syncwarp();
+            } else {
+                bool ok = warp_inverse(SA, SI, col, m, lane, logdet);   // SA = scratch copy of S
+                if (!ok) { st = BKE_STATUS_SINGULAR_S; return; }
+            }
             warp_mm<false>(PHT, SI, n, m, m, lane, [&](int e, int, int, T s) { K[e] = s; });
             __syncwarp();
             for (int i = lane; i < n; i += 32) {
@@ -183,6 +266,16 @@ __global__ void __launch_bounds__(128) kf_generic_kernel(KfP<T> p, int per_warp_
             }
             __syncwarp();
             for (int e = lane; e < nn; e += 32) P[e] = F[e];
+            if constexpr (FORM == FORM_ROWS) {
+                const int M = p.mfull;
+                if (p.K) for (int e = lane; e < nm; e += 32) p.K[(f * n + e / m) * M + p.start + e % m] = K[e];
+                for (int a = lane; a < m; a += 32) {
+                    if (p.y) p.y[f * M + p.start + a] = y[a];
+                    if (p.zrec) p.zrec[f * M + p.start + a] = p.z[f * m + a];
+                }
+                __syncwarp();
+                return;
+            }
             if (p.K) for (int e = lane; e < nm; e += 32) p.K[f * nm + e] = K[e];
             if (p.y) for (int a = lane; a < m; a += 32) p.y[f * m + a] = y[a];
             if (p.SI) for (int e = lane; e < mm; e += 32) p.SI[f * mm + e] = SI[e];
@@ -198,14 +291,18 @@ __global__ void __launch_bounds__(128) kf_generic_kernel(KfP<T> p, int per_warp_
             __syncwarp();
         };
 
+        auto run_update = [&]() {
+            if constexpr (FORM == FORM_CORRELATED) update_correlated();
+            else update();
+        };
         if (update_first) {
-            if (do_update) update();
+            if (do_update) run_update();
             __syncwarp();
             if (do_predict) predict();
         } else {
             if (do_predict) predict();
             __syncwarp();
-            if (do_update) update();
+            if (do_update) run_update();
         }
         __syncwarp();
         for (int i = lane; i < n; i += 32) p.x_out[f * n + i] = x[i];
@@ -215,10 +312,10 @@ __global__ void __launch_bounds__(128) kf_generic_kernel(KfP<T> p, int per_warp_
     }
 }
 
-template <typename T>
-int launch_t(const bke_kf_args &a, cudaStream_t s)
+template <typename T, int FORM = FORM_PLAIN>
+int launch_t(const bke_kf_args &a, cudaStream_t s, const KfP<T> *form = nullptr)
 {
-    KfP<T> p;
+    KfP<T> p = form ? *form : KfP<T>{};
     p.N = a.n_filters; p.n = a.dim_x; p.m = a.dim_z; p.du = a.dim_u; p.flags = a.flags;
     p.alpha_sq = (T)a.alpha_sq;
     p.x = (const T *)a.x; p.P = (const T *)a.P; p.x_out = (T *)a.x_out; p.P_out = (T *)a.P_out;
@@ -231,8 +328,8 @@ int launch_t(const bke_kf_args &a, cudaStream_t s)
     p.sticky = (a.flags & BKE_STATUS_STICKY) ? 1 : 0;
 
     const int n = p.n, m = p.m;
-    // layout must match the kernel: x, xp, P, F, T1, T2, H, PHT, K, R, S, SI, SA, y, col
-    int per_warp = 2 * n + 4 * (n * n) + 3 * (n * m) + 4 * (m * m) + 2 * m;
+    // layout must match the kernel: x, xp, P, F, T1, T2, H, PHT, K, R, S, SI, SA, y, col (, Mc, G)
+    int per_warp = 2 * n + 4 * (n * n) + 3 * (n * m) + 4 * (m * m) + 2 * m + (FORM == FORM_CORRELATED ? 2 * n * m : 0);
     per_warp = (per_warp + 3) & ~3;
     size_t bytes_per_warp = (size_t)per_warp * sizeof(T);
     int wpb = 4;
@@ -241,13 +338,13 @@ int launch_t(const bke_kf_args &a, cudaStream_t s)
     if (bytes_per_warp * wpb > budget) { set_error("bke_kf_step: dim_x=%d dim_z=%d needs %zu B of shared memory per filter (> %zu)", n, m, bytes_per_warp, budget); return BKE_ERR_UNSUPPORTED; }
     size_t smem = bytes_per_warp * wpb;
     if (smem > 48 * 1024) {
-        if (check_cuda(cudaFuncSetAttribute(kf_generic_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
+        if (check_cuda(cudaFuncSetAttribute(kf_generic_kernel<T, FORM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
     }
     int64_t want = (p.N + wpb - 1) / wpb;
     int64_t cap = (int64_t)sm_count() * 16;
     int grid = (int)(want < cap ? want : cap);
     if (grid < 1) grid = 1;
-    kf_generic_kernel<T><<<grid, wpb * 32, smem, s>>>(p, per_warp);
+    kf_generic_kernel<T, FORM><<<grid, wpb * 32, smem, s>>>(p, per_warp);
     return check_cuda(cudaGetLastError(), "kf_generic_kernel launch");
 }
 
@@ -256,6 +353,32 @@ int launch_t(const bke_kf_args &a, cudaStream_t s)
 int launch_kf_generic(const bke_kf_args &a, cudaStream_t s)
 {
     return a.dtype == BKE_F32 ? launch_t<float>(a, s) : launch_t<double>(a, s);
+}
+
+template <typename T>
+static int correlated_t(const bke_kf_args &a, const void *M, int64_t M_stride, cudaStream_t s)
+{
+    KfP<T> p{};
+    p.Mc = (const T *)M; p.sM = M_stride;
+    return launch_t<T, FORM_CORRELATED>(a, s, &p);
+}
+
+int launch_kf_generic_correlated(const bke_kf_args &a, const void *M, int64_t M_stride, cudaStream_t s)
+{
+    return a.dtype == BKE_F32 ? correlated_t<float>(a, M, M_stride, s) : correlated_t<double>(a, M, M_stride, s);
+}
+
+template <typename T>
+static int rows_t(const bke_kf_args &a, int m, int start, int rpitch, void *zrec, cudaStream_t s)
+{
+    KfP<T> p{};
+    p.mfull = m; p.start = start; p.rpitch = rpitch; p.zrec = (T *)zrec;
+    return launch_t<T, FORM_ROWS>(a, s, &p);
+}
+
+int launch_kf_generic_rows(const bke_kf_args &a, int m, int start, int rpitch, void *zrec, cudaStream_t s)
+{
+    return a.dtype == BKE_F32 ? rows_t<float>(a, m, start, rpitch, zrec, s) : rows_t<double>(a, m, start, rpitch, zrec, s);
 }
 
 }  // namespace bke

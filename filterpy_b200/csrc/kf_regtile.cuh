@@ -125,10 +125,13 @@ struct KfUpdateOut {
     bool ok;
 };
 
-template <typename T, int N, int M>
+// RECIP: the one-row block of update_sequential (kalman_filter.py:806-807), K = PH' (1 / S): a zero S gives
+// inf, never LinAlgError, so the update runs on (o.ok is still false for a zero S)
+template <typename T, int N, int M, bool RECIP = false>
 __device__ __forceinline__ void reg_update(T (&x)[N], T (&P)[N][N], const T (&H)[M][N], const T (&R)[M][M],
                                            const T (&z)[M], KfUpdateOut<T, N, M> &o)
 {
+    static_assert(!RECIP || M == 1, "the reciprocal gain is the one-row block's");
 #pragma unroll
     for (int a = 0; a < M; a++) {
         T s = H[a][0] * x[0];
@@ -156,7 +159,7 @@ __device__ __forceinline__ void reg_update(T (&x)[N], T (&P)[N][N], const T (&H)
             o.S[a][b] = s + R[a][b];
         }
     o.ok = reg_inverse<T, M>(o.S, o.SI, o.logdet);
-    if (!o.ok) return;      // np.linalg.inv would raise; state stays at the prior
+    if (!RECIP && !o.ok) return;      // np.linalg.inv would raise; state stays at the prior
 #pragma unroll
     for (int i = 0; i < N; i++)
 #pragma unroll
@@ -213,6 +216,87 @@ __device__ __forceinline__ void reg_update(T (&x)[N], T (&P)[N][N], const T (&H)
 #pragma unroll
             for (int a = 0; a < M; a++) s += KR[i][a] * o.K[j][a];
             P[i][j] = s;
+        }
+}
+
+// update_correlated (kalman_filter.py:730-748), process noise correlated with the measurement noise by Mc[N][M]:
+//   y = z - H x ; PHT = P H' ; S = H PHT + H Mc + Mc' H' + R ; SI = S^-1 ; K = (PHT + Mc) SI ; x = x + K y ;
+//   P = P - K (H P + Mc')          (not the Joseph form, and not symmetrised: the reference's arithmetic)
+template <typename T, int N, int M>
+__device__ __forceinline__ void reg_update_correlated(T (&x)[N], T (&P)[N][N], const T (&H)[M][N], const T (&R)[M][M],
+                                                      const T (&Mc)[N][M], const T (&z)[M], KfUpdateOut<T, N, M> &o)
+{
+#pragma unroll
+    for (int a = 0; a < M; a++) {
+        T s = H[a][0] * x[0];
+#pragma unroll
+        for (int k = 1; k < N; k++) s += H[a][k] * x[k];
+        o.y[a] = z[a] - s;
+    }
+    T PHT[N][M], HM[M][M];
+#pragma unroll
+    for (int i = 0; i < N; i++)
+#pragma unroll
+        for (int a = 0; a < M; a++) {
+            T s = P[i][0] * H[a][0];
+#pragma unroll
+            for (int k = 1; k < N; k++) s += P[i][k] * H[a][k];
+            PHT[i][a] = s;
+        }
+#pragma unroll
+    for (int a = 0; a < M; a++)
+#pragma unroll
+        for (int b = 0; b < M; b++) {
+            T s = H[a][0] * Mc[0][b];
+#pragma unroll
+            for (int k = 1; k < N; k++) s += H[a][k] * Mc[k][b];
+            HM[a][b] = s;
+        }
+#pragma unroll
+    for (int a = 0; a < M; a++)
+#pragma unroll
+        for (int b = 0; b < M; b++) {
+            T s = H[a][0] * PHT[0][b];
+#pragma unroll
+            for (int k = 1; k < N; k++) s += H[a][k] * PHT[k][b];
+            o.S[a][b] = s + HM[a][b] + HM[b][a] + R[a][b];      // (M' H')[a][b] = (H M)[b][a]
+        }
+    o.ok = reg_inverse<T, M>(o.S, o.SI, o.logdet);
+    if (!o.ok) return;
+#pragma unroll
+    for (int i = 0; i < N; i++)
+#pragma unroll
+        for (int a = 0; a < M; a++) {
+            T s = (PHT[i][0] + Mc[i][0]) * o.SI[0][a];
+#pragma unroll
+            for (int b = 1; b < M; b++) s += (PHT[i][b] + Mc[i][b]) * o.SI[b][a];
+            o.K[i][a] = s;
+        }
+#pragma unroll
+    for (int i = 0; i < N; i++) {
+        T s = x[i];
+#pragma unroll
+        for (int a = 0; a < M; a++) s += o.K[i][a] * o.y[a];
+        x[i] = s;
+    }
+    T G[M][N];      // H P + Mc'
+#pragma unroll
+    for (int a = 0; a < M; a++)
+#pragma unroll
+        for (int j = 0; j < N; j++) {
+            T s = H[a][0] * P[0][j];
+#pragma unroll
+            for (int k = 1; k < N; k++) s += H[a][k] * P[k][j];
+            G[a][j] = s + Mc[j][a];
+        }
+#pragma unroll
+    for (int i = 0; i < N; i++)
+#pragma unroll
+        for (int j = 0; j < N; j++) {
+            T s = o.K[i][0] * G[0][j];
+#pragma unroll
+            for (int a = 1; a < M; a++) s += o.K[i][a] * G[a][j];
+            P[i][j] -= s;
         }
 }
 

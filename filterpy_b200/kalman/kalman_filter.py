@@ -2,7 +2,7 @@
 
 Same names, argument meaning and error behaviour as the reference
 (``filterpy/kalman/kalman_filter.py``: ``__init__`` :387-434, ``predict`` :437-482, ``update``
-:485-561, ``batch_filter`` :826-993, ``rts_smoother`` :995-1074; procedural ``predict`` :1571,
+:485-561, ``update_correlated`` :670-752, ``update_sequential`` :754-824, ``batch_filter`` :826-993, ``rts_smoother`` :995-1074; procedural ``predict`` :1571,
 ``update`` :1401, ``batch_filter`` :1664, ``rts_smoother`` :1792), with one addition: a leading ``n_filters`` axis.  All arithmetic runs in
 the hand-written CUDA kernels behind the C-ABI (``include/bke.h``); this file only validates
 shapes, owns the device tensors and fills the argument structs.  There is no CPU fallback.
@@ -48,6 +48,8 @@ class KalmanFilter(_BankMirror):
         self._F = torch.eye(n, **kw)
         self._H = torch.zeros(m, n, **kw)
         self._R = torch.eye(m, **kw)
+        self._M = torch.zeros(n, m, **kw)   # process-measurement cross-correlation (:407), read by update_correlated
+        self._zrec = None                   # update_sequential's z record [N, m] (the blocks it has seen)
         self._B = None
         self._alpha_sq = 1.0
         self._pending = None          # deferred predict: dict(u,B,F,Q)
@@ -86,7 +88,9 @@ class KalmanFilter(_BankMirror):
 
     def _model_hook(self, name, assigned):
         # a new or handed-out model invalidates the cached argument structs that carry its host copy, and
-        # (F, Q, H, R) the packed model words
+        # (F, Q, H, R) the packed model words.  M is in neither: update_correlated fills its struct every call.
+        if name == "M":
+            return
         if self._host.pop(name, None) is not None or assigned:
             self._version += 1
         if name in ("F", "Q", "H", "R"):
@@ -118,6 +122,7 @@ class KalmanFilter(_BankMirror):
     Q = _model_prop("Q", "dim_x", "dim_x")
     H = _model_prop("H", "dim_z", "dim_x")
     R = _model_prop("R", "dim_z", "dim_z")
+    M = _model_prop("M", "dim_x", "dim_z")
 
     @property
     def B(self):
@@ -312,6 +317,26 @@ class KalmanFilter(_BankMirror):
                     if self._single:
                         self.check()
                 return
+        a, keep = self._args(flags, pend, zt, vt, R, H)
+        if plain and len(self._host) == 4:                  # every model shared and known on the host
+            hm = [self._host[k] for k in "FQHR"]
+            a.F_host, a.Q_host, a.H_host, a.R_host = (h.ctypes.data for h in hm)
+            keep += hm
+        if self._sym_buf is not None:
+            keep.append(self._sym_buf)
+        if not (flags & _lib.BKE_DO_UPDATE):
+            self._snapshot_post()                           # a predict on its own is about to move x, P
+        self._run(self._step, a, rec)
+        if plain:
+            self._args_cache[flags] = (self._version, a, keep)      # keep: the tensors `a` points into
+        if self.diagnostics and (flags & _lib.BKE_DO_UPDATE):
+            self._post_alias = True
+            if self._single:
+                self.check()
+
+    def _args(self, flags, pend, zt, vt, R, H):
+        """A fresh argument struct of a step with the pending predict ``pend`` and the update's ``z`` / ``valid``
+        tensors and per-call ``R`` / ``H``, and the tensors it points into."""
         a = _lib.KfArgs()
         N, n, m = self.n_filters, self.dim_x, self.dim_z
         a.n_filters, a.dim_x, a.dim_z, a.dim_u = N, n, m, 0
@@ -348,12 +373,6 @@ class KalmanFilter(_BankMirror):
             a.z = ptr(zt)
             a.z_valid = ptr(vt)
             keep += [Rm, Hm, zt, vt]
-        if plain and len(self._host) == 4:                  # every model shared and known on the host
-            hm = [self._host[k] for k in "FQHR"]
-            a.F_host, a.Q_host, a.H_host, a.R_host = (h.ctypes.data for h in hm)
-            keep += hm
-        if self._sym_buf is not None:
-            keep.append(self._sym_buf)
         if self.diagnostics:
             if flags & _lib.BKE_DO_PREDICT:
                 a.x_prior, a.P_prior = ptr(self._x_prior), ptr(self._P_prior)
@@ -361,15 +380,99 @@ class KalmanFilter(_BankMirror):
                 a.K, a.y, a.S, a.SI = ptr(self._K), ptr(self._y), ptr(self._S), ptr(self._SI)
                 a.log_likelihood = ptr(self._ll)
                 a.status = ptr(self._status)
-        if not (flags & _lib.BKE_DO_UPDATE):
-            self._snapshot_post()                           # a predict on its own is about to move x, P
-        self._run(self._step, a, rec)
-        if plain:
-            self._args_cache[flags] = (self._version, a, keep)      # keep: the tensors `a` points into
-        if self.diagnostics and (flags & _lib.BKE_DO_UPDATE):
+        return a, keep
+
+    # ------------------------------------------------------------------ the other update forms
+    def _form_launch(self, fn, *args):
+        """Run ``update_correlated`` / ``update_sequential``'s C-ABI call.  Their argument structs are built
+        per call and never cached, they leave the tile order and the packed model words alone, and a graph
+        captured over them stays a graph of separate launches (the note below is never fusable)."""
+        if self._ring_notes is not None and self._capturing():
+            self._ring_notes.append((_lib.BKE_DO_UPDATE, False, None, None))
+        self._run(fn, *args)
+        if self.diagnostics:
             self._post_alias = True
             if self._single:
                 self.check()
+
+    def update_correlated(self, z, R=None, H=None, valid=None):
+        """kalman_filter.py:670-752: ``update`` for process noise correlated with the measurement noise by
+        ``M`` (``(dim_x, dim_z)`` shared or ``(N, dim_x, dim_z)`` per filter; zeros by default)::
+
+            S = H P H' + H M + M' H' + R;  K = (P H' + M) S^-1;  x += K y;  P = P - K (H P + M')
+
+        (not the Joseph form, and not symmetrised).  Arguments, ``valid``, the fused pending predict,
+        ``z=None``, the diagnostics and the error behaviour are those of ``update``."""
+        if z is None:                                       # :705-710 is update(None)
+            return self.update(None)
+        pend, self._pending = self._pending, None
+        if self._single and H is None:
+            z = reshape_z(z, self.dim_z, 2 if self._x_col else 1)        # :718-719
+        zt = self._z_rows(z)
+        vt = self._valid_mask(valid)
+        flags = _lib.BKE_DO_UPDATE | (_lib.BKE_DO_PREDICT if pend is not None else 0)
+        a, keep = self._args(flags, pend, zt, vt, R, H)
+        Mt = self._M
+        self._form_launch(self._lib.bke_kf_step_correlated, a, ptr(Mt), self._stride(Mt), stream_ptr(self._device))
+        if vt is not None and self.diagnostics:
+            self._ll.copy_(torch.where(vt.bool(), self._ll, _missed_log_likelihood(self._S)))
+        self._z = zt
+
+    def update_sequential(self, start, z_i, R_i=None, H_i=None, valid=None):
+        """kalman_filter.py:754-824: the update with rows ``start .. start+L-1`` of the measurement alone.
+        ``R_i`` defaults to that block of ``R`` (a scalar is ``R_i * I``), ``H_i`` to those rows of ``H``; both
+        are read in place from the bank's ``R`` and ``H``.  ``K = P H_i' (1 / S_i)`` when ``L = 1`` (a zero
+        ``S_i`` gives inf, never ``LinAlgError``), ``P H_i' inv(S_i)`` otherwise; x and P take the Joseph
+        update with ``R_i``.
+
+        Bank mode: ``z_i`` is ``(N, L)``, ``R_i`` ``(L, L)`` or ``(N, L, L)``, ``H_i`` ``(L, dim_x)`` or
+        ``(N, L, dim_x)``, ``valid`` (bool[N]) as in ``update``.  Single mode: the reference's arguments.
+
+        Rows ``start .. start+L-1`` of ``y`` and ``z`` and the columns of ``K`` receive the block's values;
+        the others keep theirs (rows of ``z`` that no update has set read NaN, where the reference has None).
+        ``S``, ``SI`` and ``log_likelihood`` are left as they were: the reference computes its log-likelihood
+        lazily, so its value after this call depends on whether it was read before."""
+        pend, self._pending = self._pending, None
+        N, n, m = self.n_filters, self.dim_x, self.dim_z
+        if self._single:
+            L = 1 if np.isscalar(z_i) else len(z_i)
+            zt = to_dev(np.reshape(np.asarray(z_i, dtype=np.float64), (1, L)), self._dtype, self._device)   # :778-782
+        else:
+            zt = to_dev(z_i, self._dtype, self._device)
+            if zt.dim() == 3 and zt.shape[-1] == 1:
+                zt = zt[..., 0]
+            if zt.dim() == 1:
+                zt = zt.reshape(N, 1)
+            if zt.dim() != 2 or zt.shape[0] != N:
+                raise ValueError("z_i must have shape (%d, L), got %s" % (N, tuple(zt.shape)))
+            zt = zt.contiguous()
+            L = zt.shape[1]
+        start = int(start)
+        if start < 0 or L < 1 or start + L > m:
+            raise ValueError("rows %d .. %d are not within the %d rows of z" % (start, start + L - 1, m))
+        Rt = None if R_i is None else self._model(R_i, L, L, "R_i")           # scalar -> R_i * I (:787-788)
+        if H_i is not None and self._single:
+            H_i = np.reshape(np.asarray(H_i, dtype=np.float64), (L, n))       # :793
+        Ht = None if H_i is None else self._model(H_i, L, n, "H_i")
+        vt = self._valid_mask(valid)
+        flags = _lib.BKE_DO_UPDATE | (_lib.BKE_DO_PREDICT if pend is not None else 0)
+        a, keep = self._args(flags, pend, zt, vt, None, None)
+        a.S = a.SI = a.log_likelihood = None
+        if self._zrec is None:
+            self._zrec = torch.full((N, m), math.nan, dtype=self._dtype, device=self._device)
+        if self._z is not self._zrec:                       # the record starts from the last z
+            if self._z is None or tuple(self._z.shape) != (N, m):
+                self._zrec.fill_(math.nan)
+            else:
+                self._zrec.copy_(self._z)
+        ra = _lib.KfRowsArgs()
+        ra.step = a
+        ra.start, ra.rows = start, L
+        ra.H_i, ra.H_i_stride = (ptr(Ht), self._stride(Ht)) if Ht is not None else (None, 0)
+        ra.R_i, ra.R_i_stride = (ptr(Rt), self._stride(Rt)) if Rt is not None else (None, 0)
+        ra.z_record = ptr(self._zrec)
+        self._form_launch(self._lib.bke_kf_update_rows, ra, stream_ptr(self._device))
+        self._z = self._zrec
 
     def capture(self, fn, warmup=2):
         """Capture ``fn`` — a fixed sequence of ``predict()/update(z_buffer)`` calls on this bank —

@@ -6,6 +6,8 @@ The same symbols exposed as torch.ops.* via a C++ extension for zero-copy CUDA t
 
     x, P = torch.ops.bke.kf_step(x, P, F, H, Q, R, z)              # kalman_filter.py:437-561 for a bank
     x, P = torch.ops.bke.kf_predict(x, P, F, Q)                    # :437-482
+    x, P = torch.ops.bke.kf_step_correlated(x, P, F, H, Q, R, M, z)   # predict + update_correlated, :670-752
+    x, P = torch.ops.bke.kf_update_rows(x, P, F, H, Q, R, z_i, start)  # predict + update_sequential, :754-824
     x, P = torch.ops.bke.ukf_step(x, P, Q, R, z, dt, alpha, beta, kappa, fx_model, hx_model)   # UKF.py:364-491
     x, P = torch.ops.bke.ukf_step(..., simplex=True)               # the same on SimplexSigmaPoints(n)
     x, P = torch.ops.bke.ckf_step(x, P, Q, R, z, dt, fx_model, hx_model)   # CubatureKalmanFilter.py:292-389

@@ -3,6 +3,8 @@
 // asks for this twin of the ctypes binding: the same entry points, no arithmetic of its own.
 //   bke::kf_step              bke_kf_step              KalmanFilter.predict + update, kalman_filter.py:437-561
 //   bke::kf_predict           bke_kf_step (predict)    kalman_filter.py:437-482
+//   bke::kf_step_correlated   bke_kf_step_correlated   predict + update_correlated, kalman_filter.py:437-482, 670-752
+//   bke::kf_update_rows       bke_kf_update_rows       predict + update_sequential, kalman_filter.py:437-482, 754-824
 //   bke::ukf_step             bke_ukf_step             UnscentedKalmanFilter.predict + update, UKF.py:364-491
 //   bke::ckf_step             bke_ckf_step             CubatureKalmanFilter.predict + update, CubatureKalmanFilter.py:292-389
 //   bke::enkf_step            bke_enkf_step            EnsembleKalmanFilter.predict + update, ensemble_kalman_filter.py:218-290
@@ -48,9 +50,15 @@ const void *model(const at::Tensor &t, int64_t N, int64_t r, int64_t c, int64_t 
     return t.data_ptr();
 }
 
+// the form of update a kf_run call makes after its predict
+struct KfForm {
+    const at::Tensor *M = nullptr;          // update_correlated
+    int64_t start = -1, rows = 0;           // update_sequential's block (z is then [N, rows])
+};
+
 std::tuple<at::Tensor, at::Tensor> kf_run(const at::Tensor &x, const at::Tensor &P, const at::Tensor &F, const at::Tensor &H,
                                           const at::Tensor &Q, const at::Tensor &R, const c10::optional<at::Tensor> &z,
-                                          double alpha_sq, unsigned flags)
+                                          double alpha_sq, unsigned flags, const KfForm &form = KfForm())
 {
     TORCH_CHECK(x.is_cuda() && P.is_cuda() && x.is_contiguous() && P.is_contiguous(), "bke: x and P must be contiguous CUDA tensors");
     TORCH_CHECK(x.dim() == 2 && P.dim() == 3 && P.size(0) == x.size(0) && P.size(1) == x.size(1) && P.size(2) == x.size(1), "bke: x is [N, n], P is [N, n, n]");
@@ -71,10 +79,23 @@ std::tuple<at::Tensor, at::Tensor> kf_run(const at::Tensor &x, const at::Tensor 
     if (flags & BKE_DO_UPDATE) {
         TORCH_CHECK(z.has_value(), "bke: update needs z");
         const at::Tensor &zz = *z;
-        TORCH_CHECK(zz.is_cuda() && zz.is_contiguous() && zz.scalar_type() == x.scalar_type() && zz.dim() == 2 && zz.size(0) == N && zz.size(1) == m, "bke: z is [N, m]");
+        const int64_t zm = form.start >= 0 ? form.rows : m;
+        TORCH_CHECK(zz.is_cuda() && zz.is_contiguous() && zz.scalar_type() == x.scalar_type() && zz.dim() == 2 && zz.size(0) == N && zz.size(1) == zm, "bke: z is [N, m] (z_i [N, L] for a block)");
         a.z = zz.data_ptr();
     }
-    check_rc(bke_kf_step(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_kf_step");
+    void *stream = (void *)c10::cuda::getCurrentCUDAStream().stream();
+    if (form.M) {
+        int64_t sM = 0;
+        const void *Mp = model(*form.M, N, n, m, &sM, x, "M");
+        check_rc(bke_kf_step_correlated(&a, Mp, sM, stream), "bke_kf_step_correlated");
+    } else if (form.start >= 0) {
+        bke_kf_rows_args r;
+        std::memset(&r, 0, sizeof(r));
+        r.step = a; r.start = (int32_t)form.start; r.rows = (int32_t)form.rows;
+        check_rc(bke_kf_update_rows(&r, stream), "bke_kf_update_rows");
+    } else {
+        check_rc(bke_kf_step(&a, stream), "bke_kf_step");
+    }
     return std::make_tuple(x_out, P_out);
 }
 
@@ -82,6 +103,26 @@ std::tuple<at::Tensor, at::Tensor> kf_step(const at::Tensor &x, const at::Tensor
                                            const at::Tensor &Q, const at::Tensor &R, const at::Tensor &z, double alpha_sq)
 {
     return kf_run(x, P, F, H, Q, R, z, alpha_sq, BKE_DO_PREDICT | BKE_DO_UPDATE);
+}
+
+std::tuple<at::Tensor, at::Tensor> kf_step_correlated(const at::Tensor &x, const at::Tensor &P, const at::Tensor &F, const at::Tensor &H,
+                                                      const at::Tensor &Q, const at::Tensor &R, const at::Tensor &M, const at::Tensor &z,
+                                                      double alpha_sq)
+{
+    KfForm form;
+    form.M = &M;
+    return kf_run(x, P, F, H, Q, R, z, alpha_sq, BKE_DO_PREDICT | BKE_DO_UPDATE, form);
+}
+
+// H and R are the bank's full [.,m,n] / [.,m,m]: the block's rows are read in place
+std::tuple<at::Tensor, at::Tensor> kf_update_rows(const at::Tensor &x, const at::Tensor &P, const at::Tensor &F, const at::Tensor &H,
+                                                  const at::Tensor &Q, const at::Tensor &R, const at::Tensor &z_i, int64_t start,
+                                                  double alpha_sq)
+{
+    KfForm form;
+    form.start = start;
+    form.rows = z_i.dim() == 2 ? z_i.size(1) : 0;
+    return kf_run(x, P, F, H, Q, R, z_i, alpha_sq, BKE_DO_PREDICT | BKE_DO_UPDATE, form);
 }
 
 std::tuple<at::Tensor, at::Tensor> kf_predict(const at::Tensor &x, const at::Tensor &P, const at::Tensor &F, const at::Tensor &Q, double alpha_sq)
@@ -408,6 +449,10 @@ TORCH_LIBRARY(bke, m)
 {
     m.def("kf_step(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor z, float alpha_sq=1.0) -> (Tensor, Tensor)");
     m.def("kf_predict(Tensor x, Tensor P, Tensor F, Tensor Q, float alpha_sq=1.0) -> (Tensor, Tensor)");
+    m.def("kf_step_correlated(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor M, Tensor z, "
+          "float alpha_sq=1.0) -> (Tensor, Tensor)");
+    m.def("kf_update_rows(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor z_i, int start, "
+          "float alpha_sq=1.0) -> (Tensor, Tensor)");
     m.def("ukf_step(Tensor x, Tensor P, Tensor Q, Tensor R, Tensor z, float dt, float alpha, float beta, float kappa, "
           "int fx_model, int hx_model, Tensor? F=None, Tensor? H=None, bool simplex=False) -> (Tensor, Tensor)");
     m.def("ckf_step(Tensor x, Tensor P, Tensor Q, Tensor R, Tensor z, float dt, int fx_model, int hx_model, "
@@ -432,6 +477,8 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
 {
     m.impl("kf_step", &kf_step);
     m.impl("kf_predict", &kf_predict);
+    m.impl("kf_step_correlated", &kf_step_correlated);
+    m.impl("kf_update_rows", &kf_update_rows);
     m.impl("ukf_step", &ukf_step);
     m.impl("ckf_step", &ckf_step);
     m.impl("enkf_step", &enkf_step);

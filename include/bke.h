@@ -134,6 +134,41 @@ typedef struct bke_kf_args {
 
 int bke_kf_step(const bke_kf_args *args, void *stream);
 
+/* KalmanFilter.update_correlated(z, R, H)      filterpy/kalman/kalman_filter.py:670-752
+ * bke_kf_step with process noise correlated with the measurement noise by M [N,n,m] (M_stride = n*m) or
+ * [n,m] shared (M_stride = 0).  flags = BKE_DO_UPDATE, optionally | BKE_DO_PREDICT (the predict runs first,
+ * as in bke_kf_step) and BKE_STATUS_STICKY.  Per filter with a measurement:
+ *   y = z - H x;  S = H P H' + H M + M' H' + R;  SI = S^-1;  K = (P H' + M) SI;  x <- x + K y;
+ *   P <- P - K (H P + M')                       (not the Joseph form, and not symmetrised: :748)
+ * z_valid, status and the optional outputs are those of bke_kf_step (a filter without a measurement gets
+ * y = 0 and keeps K, S, SI and log_likelihood).  A NULL M, or a stride that is neither 0 nor n*m, is
+ * BKE_ERR_BAD_ARG. */
+int bke_kf_step_correlated(const bke_kf_args *args, const void *M, int64_t M_stride, void *stream);
+
+/* KalmanFilter.update_sequential(start, z_i, R_i, H_i)      filterpy/kalman/kalman_filter.py:754-824
+ * The update with the block of rows start .. start+rows-1 (L = rows) of z, H and R.  step.dim_z is the bank's
+ * full m, 1 <= L and start + L <= m.  step.z is z_i [N,L].  H_i [.,L,n] and R_i [.,L,L] are per filter
+ * (stride L*n, L*L) or shared (stride 0); a NULL one is read in place from the block of step.H / step.R (the
+ * bank's [.,m,n] / [.,m,m], strides as in bke_kf_step), without a copy.  Per filter with a measurement:
+ *   y_i = z_i - H_i x;  S_i = H_i P H_i' + R_i;  K_i = P H_i' S_i^-1, or P H_i' (1 / S_i) when L = 1;
+ *   x <- x + K_i y_i;  P <- (I - K_i H_i) P (I - K_i H_i)' + K_i R_i K_i'        (Joseph form, :819)
+ * and y[N,m] rows, K[N,n,m] columns and z_record[N,m] rows start .. start+L-1 receive y_i, K_i and z_i (each
+ * may be NULL); everything else of them keeps its value, and so does a filter with z_valid[f] = 0, which gets
+ * only the predict of BKE_DO_PREDICT.  For L = 1 a zero S_i gives inf (the reference's reciprocal): status
+ * stays BKE_STATUS_OK.  For L > 1 a singular S_i is BKE_STATUS_SINGULAR_S and the filter keeps the prior.
+ * flags, B / u, x_prior / P_prior and status are those of bke_kf_step; S, SI and log_likelihood are not
+ * written by this update (non-NULL is BKE_ERR_BAD_ARG).  A block outside 0 .. m-1 or a bad H_i / R_i stride is
+ * BKE_ERR_BAD_ARG. */
+typedef struct bke_kf_rows_args {
+    bke_kf_args step;
+    int32_t start, rows;
+    const void *H_i; int64_t H_i_stride;     /* [N,L,n] / [L,n], or NULL: rows of step.H */
+    const void *R_i; int64_t R_i_stride;     /* [N,L,L] / [L,L], or NULL: the block of step.R */
+    void *z_record;                          /* [N,m] or NULL */
+} bke_kf_rows_args;
+
+int bke_kf_update_rows(const bke_kf_rows_args *args, void *stream);
+
 /* Packed symmetric models of a dim_x = 4, dim_z = 2, BKE_F32 bank (per-filter Q and R).
  * Q and R are covariances: when every filter's Q and R equal their transposes bit for bit, a step
  * only needs their upper triangles, 52 instead of 80 B per filter.  The record holds them tile-major,
