@@ -42,6 +42,7 @@ EXPORTED_SYMBOLS = [
     "bke_ckf_model_compile_hooks", "bke_debug_ckf_model_hooks_cubin_bytes",
     "bke_enkf_initialize", "bke_enkf_step", "bke_enkf_model_compile", "bke_enkf_step_model", "bke_debug_enkf_model_cubin_bytes",
     "bke_srkf_step", "bke_cholesky_lower",
+    "bke_if_step", "bke_inverse",
     "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
     "bke_resample_bank", "bke_gather_rows_bank",
     "bke_multinomial_resample_bank_workspace_bytes", "bke_multinomial_resample_bank",
@@ -212,6 +213,32 @@ class SrkfArgs(ctypes.Structure):
 
 
 BKE_CHOLESKY_MAX_DIM = 16
+
+BKE_STATUS_STICKY = 8
+BKE_IF_LL_NONE, BKE_IF_LL_FULL, BKE_IF_LL_BROADCAST = 0, 1, 2
+
+
+class IfArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_filters", c_int64),
+        ("dim_x", c_int32), ("dim_z", c_int32), ("dim_u", c_int32),
+        ("dtype", c_int32),
+        ("flags", c_uint32), ("ll_mode", c_int32),
+        ("x", c_void_p), ("P_inv", c_void_p),
+        ("x_out", c_void_p), ("P_inv_out", c_void_p),
+        ("no_information", c_void_p),
+        ("F", c_void_p), ("F_stride", c_int64),
+        ("F_inv", c_void_p), ("F_inv_stride", c_int64),
+        ("Q", c_void_p), ("Q_stride", c_int64),
+        ("H", c_void_p), ("H_stride", c_int64),
+        ("R_inv", c_void_p), ("R_inv_stride", c_int64),
+        ("B", c_void_p), ("B_stride", c_int64),
+        ("u", c_void_p), ("u_stride", c_int64),
+        ("z", c_void_p), ("z_valid", c_void_p),
+        ("x_prior", c_void_p), ("P_inv_prior", c_void_p),
+        ("K", c_void_p), ("y", c_void_p), ("S", c_void_p), ("log_likelihood", c_void_p),
+        ("status", c_void_p),
+    ]
 
 
 class ResampleShardArgs(ctypes.Structure):
@@ -460,6 +487,10 @@ def load():
     lib.bke_srkf_step.restype = ctypes.c_int
     lib.bke_cholesky_lower.argtypes = [c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
     lib.bke_cholesky_lower.restype = ctypes.c_int
+    lib.bke_if_step.argtypes = [ctypes.POINTER(IfArgs), c_void_p]
+    lib.bke_if_step.restype = ctypes.c_int
+    lib.bke_inverse.argtypes = [c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
+    lib.bke_inverse.restype = ctypes.c_int
     lib.bke_resample_workspace_bytes.argtypes = [c_int64]
     lib.bke_resample_workspace_bytes.restype = c_size_t
     lib.bke_systematic_resample.argtypes = [c_int64, c_void_p, c_double, c_void_p, c_void_p, c_size_t,

@@ -110,6 +110,49 @@ static int validate_srkf(const bke_srkf_args *a)
     return BKE_OK;
 }
 
+// the checks of bke_if_step
+static int validate_if(const bke_if_args *a)
+{
+    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    if (a->n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    if (a->dim_x < 1) { set_error("dim_x must be 1 or greater"); return BKE_ERR_BAD_ARG; }   // information_filter.py:132-137
+    if (a->dim_z < 1) { set_error("dim_z must be 1 or greater"); return BKE_ERR_BAD_ARG; }
+    if (a->dim_u < 0) { set_error("dim_u must be 0 or greater"); return BKE_ERR_BAD_ARG; }
+    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (!(a->flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
+    if (a->flags & ~(BKE_DO_PREDICT | BKE_DO_UPDATE | BKE_STATUS_STICKY)) {
+        set_error("flags may only hold BKE_DO_PREDICT, BKE_DO_UPDATE and BKE_STATUS_STICKY");
+        return BKE_ERR_BAD_ARG;
+    }
+    if (!a->x || !a->P_inv || !a->x_out || !a->P_inv_out) { set_error("x, P_inv, x_out, P_inv_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if (!a->no_information) { set_error("no_information must be non-NULL (the per-filter flag is read and written)"); return BKE_ERR_BAD_ARG; }
+    if ((a->flags & BKE_DO_PREDICT) && (!a->F || !a->F_inv || !a->Q)) { set_error("predict needs F, F_inv and Q"); return BKE_ERR_BAD_ARG; }
+    if ((a->flags & BKE_DO_UPDATE) && (!a->H || !a->R_inv || !a->z)) { set_error("update needs H, R_inv and z"); return BKE_ERR_BAD_ARG; }
+    if ((a->B != nullptr || a->u != nullptr) && (!a->B || !a->u || a->dim_u < 1)) {
+        set_error("a control input needs B, u and dim_u >= 1");                                       // :274
+        return BKE_ERR_BAD_ARG;
+    }
+    const int64_t n = a->dim_x, m = a->dim_z, du = a->dim_u;
+    auto bad_stride = [](int64_t s, int64_t full) { return s != 0 && s != full; };
+    if (bad_stride(a->F_stride, n * n) || bad_stride(a->F_inv_stride, n * n) || bad_stride(a->Q_stride, n * n) ||
+        bad_stride(a->H_stride, m * n) || bad_stride(a->R_inv_stride, m * m) || bad_stride(a->B_stride, n * du) ||
+        bad_stride(a->u_stride, du)) {
+        set_error("model strides must be 0 (shared) or the dense per-filter size");
+        return BKE_ERR_BAD_ARG;
+    }
+    if (a->ll_mode != BKE_IF_LL_NONE && a->ll_mode != BKE_IF_LL_FULL && a->ll_mode != BKE_IF_LL_BROADCAST) {
+        set_error("ll_mode must be BKE_IF_LL_NONE, BKE_IF_LL_FULL or BKE_IF_LL_BROADCAST");
+        return BKE_ERR_BAD_ARG;
+    }
+    if ((a->ll_mode == BKE_IF_LL_FULL && m != n) || (a->ll_mode == BKE_IF_LL_BROADCAST && m != 1)) {
+        set_error("ll_mode %s needs %s", a->ll_mode == BKE_IF_LL_FULL ? "BKE_IF_LL_FULL" : "BKE_IF_LL_BROADCAST",
+                  a->ll_mode == BKE_IF_LL_FULL ? "dim_z == dim_x" : "dim_z == 1");
+        return BKE_ERR_BAD_ARG;
+    }
+    if (a->ll_mode != BKE_IF_LL_NONE && !a->log_likelihood) { set_error("ll_mode needs log_likelihood"); return BKE_ERR_BAD_ARG; }
+    return BKE_OK;
+}
+
 // the checks every sigma-point step (UKF, CKF, EnKF; pre-built and run-time compiled) makes
 template <typename Args>
 static int validate_sigma(const Args &a)
@@ -515,6 +558,29 @@ int bke_cholesky_lower(int64_t n_filters, int32_t k, int32_t dtype, const void *
     if (rc) return rc;
     if (n_filters == 0) return BKE_OK;
     return launch_cholesky_lower(n_filters, k, dtype, A, stride, L, status, (cudaStream_t)stream);
+}
+
+int bke_if_step(const bke_if_args *args, void *stream)
+{
+    int rc = validate_if(args);
+    if (rc) return rc;
+    if ((rc = require_device())) return rc;
+    if (args->n_filters == 0) return BKE_OK;
+    return launch_if(*args, (cudaStream_t)stream);
+}
+
+int bke_inverse(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *Ai, int32_t *status,
+                void *stream)
+{
+    if (n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    if (k < 1) { set_error("k must be 1 or greater"); return BKE_ERR_BAD_ARG; }
+    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (stride != 0 && stride != (int64_t)k * k) { set_error("stride must be 0 (shared) or k*k"); return BKE_ERR_BAD_ARG; }
+    if (n_filters > 0 && (!A || !Ai)) { set_error("A and Ai must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    int rc = require_device();
+    if (rc) return rc;
+    if (n_filters == 0) return BKE_OK;
+    return launch_inverse(n_filters, k, dtype, A, stride, Ai, status, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -80,6 +80,9 @@ int launch_enkf_init(int64_t n_filters, int32_t dim_x, int32_t n_members, int32_
 int launch_srkf(const bke_srkf_args &a, cudaStream_t s);
 int launch_cholesky_lower(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *L,
                           int32_t *status, cudaStream_t s);
+int launch_if(const bke_if_args &a, cudaStream_t s);
+int launch_inverse(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *Ai, int32_t *status,
+                   cudaStream_t s);
 #endif
 
 }  // namespace bke

@@ -42,53 +42,6 @@ struct KfP {
 
 enum { FORM_PLAIN = 0, FORM_CORRELATED = 1, FORM_ROWS = 2 };
 
-// Gauss-Jordan inverse with partial pivoting of the m x m matrix A (destroyed) into Ai.
-// Returns false when a pivot is exactly zero (np.linalg.inv raises LinAlgError).
-// logdet receives log|det A|.
-template <typename T>
-__device__ bool warp_inverse(T *A, T *Ai, T *col, int m, int lane, T &logdet)
-{
-    for (int e = lane; e < m * m; e += 32) Ai[e] = (e / m == e % m) ? T(1) : T(0);
-    __syncwarp();
-    T ld = T(0);
-    for (int c = 0; c < m; c++) {
-        // pivot search (every lane scans; m is tiny)
-        int p = c;
-        T best = fabs(A[c * m + c]);
-        for (int r = c + 1; r < m; r++) {
-            T v = fabs(A[r * m + c]);
-            if (v > best) { best = v; p = r; }
-        }
-        if (!(best > T(0))) return false;
-        __syncwarp();
-        if (p != c) {
-            for (int j = lane; j < m; j += 32) {
-                T t = A[c * m + j]; A[c * m + j] = A[p * m + j]; A[p * m + j] = t;
-                t = Ai[c * m + j]; Ai[c * m + j] = Ai[p * m + j]; Ai[p * m + j] = t;
-            }
-            __syncwarp();
-        }
-        T piv = A[c * m + c];
-        ld += log(fabs(piv));
-        T d = T(1) / piv;
-        __syncwarp();
-        for (int j = lane; j < m; j += 32) { A[c * m + j] *= d; Ai[c * m + j] *= d; }
-        for (int r = lane; r < m; r += 32) col[r] = A[r * m + c];
-        __syncwarp();
-        for (int e = lane; e < m * m; e += 32) {
-            int r = e / m, j = e - r * m;
-            if (r != c) {
-                T f = col[r];
-                A[e] -= f * A[c * m + j];
-                Ai[e] -= f * Ai[c * m + j];
-            }
-        }
-        __syncwarp();
-    }
-    logdet = ld;
-    return true;
-}
-
 template <typename T, int FORM = FORM_PLAIN>
 __global__ void __launch_bounds__(128) kf_generic_kernel(KfP<T> p, int per_warp_elems)
 {

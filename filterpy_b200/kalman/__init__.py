@@ -6,6 +6,7 @@ from .UKF import (UnscentedKalmanFilter, LinearFx, ConstVelFx, LinearHx, RangeAz
 from .CubatureKalmanFilter import CubatureKalmanFilter  # noqa: F401
 from .ensemble_kalman_filter import EnsembleKalmanFilter  # noqa: F401
 from .square_root import SquareRootKalmanFilter  # noqa: F401
+from .information_filter import InformationFilter  # noqa: F401
 from .fixed_lag_smoother import FixedLagSmoother  # noqa: F401
 from .unscented_transform import unscented_transform  # noqa: F401
 from .IMM import IMMEstimator  # noqa: F401

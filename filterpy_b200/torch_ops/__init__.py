@@ -13,6 +13,7 @@ The same symbols exposed as torch.ops.* via a C++ extension for zero-copy CUDA t
     x, P = torch.ops.bke.ckf_step(x, P, Q, R, z, dt, fx_model, hx_model)   # CubatureKalmanFilter.py:292-389
     x, P, s = torch.ops.bke.enkf_step(x, P, sigmas, Q, R, z, dt, fx_model, hx_model, seed, counter)   # ensemble_kalman_filter.py:218-290
     x, L = torch.ops.bke.srkf_step(x, L, F, H, Lq, Lr, z)          # square_root.py:172-248 (L = P1_2)
+    x, P_inv, ni, status = torch.ops.bke.if_step(x, P_inv, ni, F, F_inv, Q, H, R_inv, z)   # information_filter.py:178-289
     xs, xhat = torch.ops.bke.fls_smooth_batch(x, P, F, H, Q, R, zs, N)   # fixed_lag_smoother.py:217-311
     idx  = torch.ops.bke.systematic_resample(weights, u)           # resampling.py:117-150 (int32, bit-exact)
     idx  = torch.ops.bke.stratified_resample(weights, uniforms)    # resampling.py:80-114

@@ -9,6 +9,7 @@
 //   bke::ckf_step             bke_ckf_step             CubatureKalmanFilter.predict + update, CubatureKalmanFilter.py:292-389
 //   bke::enkf_step            bke_enkf_step            EnsembleKalmanFilter.predict + update, ensemble_kalman_filter.py:218-290
 //   bke::srkf_step            bke_srkf_step            SquareRootKalmanFilter.predict + update, square_root.py:172-248
+//   bke::if_step              bke_if_step              InformationFilter.predict + update, information_filter.py:178-289
 //   bke::fls_smooth_batch     bke_fls_smooth           FixedLagSmoother.smooth_batch, fixed_lag_smoother.py:217-311
 //   bke::systematic_resample  bke_systematic_resample  monte_carlo/resampling.py:117-150
 //   bke::stratified_resample  bke_stratified_resample  monte_carlo/resampling.py:80-114
@@ -238,6 +239,39 @@ std::tuple<at::Tensor, at::Tensor> srkf_step(const at::Tensor &x, const at::Tens
     return std::make_tuple(x_out, L_out);
 }
 
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> if_step(const at::Tensor &x, const at::Tensor &P_inv, const at::Tensor &no_information,
+                                                       const at::Tensor &F, const at::Tensor &F_inv, const at::Tensor &Q,
+                                                       const at::Tensor &H, const at::Tensor &R_inv, const at::Tensor &z)
+{
+    TORCH_CHECK(x.is_cuda() && P_inv.is_cuda() && x.is_contiguous() && P_inv.is_contiguous(), "bke: x and P_inv must be contiguous CUDA tensors");
+    TORCH_CHECK(x.dim() == 2 && P_inv.dim() == 3 && P_inv.size(0) == x.size(0) && P_inv.size(1) == x.size(1) && P_inv.size(2) == x.size(1),
+                "bke: x is [N, n], P_inv is [N, n, n]");
+    TORCH_CHECK(P_inv.scalar_type() == x.scalar_type(), "bke: x and P_inv must share a dtype");
+    TORCH_CHECK(no_information.is_cuda() && no_information.scalar_type() == at::kByte && no_information.dim() == 1 &&
+                no_information.size(0) == x.size(0), "bke: no_information is a uint8 CUDA tensor [N]");
+    c10::cuda::CUDAGuard guard(x.device());
+    const int64_t N = x.size(0), n = x.size(1), m = H.size(-2);
+    bke_if_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_filters = N; a.dim_x = (int32_t)n; a.dim_z = (int32_t)m; a.dtype = dtype_of(x);
+    a.flags = BKE_DO_PREDICT | BKE_DO_UPDATE;
+    a.ll_mode = BKE_IF_LL_NONE;
+    at::Tensor x_out = at::empty_like(x), P_out = at::empty_like(P_inv), ni_out = no_information.contiguous().clone();
+    at::Tensor status = at::empty({N}, x.options().dtype(at::kInt));   // BKE_STATUS_SINGULAR_S where an inv raises
+    a.x = x.data_ptr(); a.P_inv = P_inv.data_ptr(); a.x_out = x_out.data_ptr(); a.P_inv_out = P_out.data_ptr();
+    a.no_information = ni_out.data_ptr<uint8_t>();
+    a.status = status.data_ptr<int32_t>();
+    a.F = model(F, N, n, n, &a.F_stride, x, "F");
+    a.F_inv = model(F_inv, N, n, n, &a.F_inv_stride, x, "F_inv");
+    a.Q = model(Q, N, n, n, &a.Q_stride, x, "Q");
+    a.H = model(H, N, m, n, &a.H_stride, x, "H");
+    a.R_inv = model(R_inv, N, m, m, &a.R_inv_stride, x, "R_inv");
+    TORCH_CHECK(z.is_cuda() && z.is_contiguous() && z.scalar_type() == x.scalar_type() && z.dim() == 2 && z.size(0) == N && z.size(1) == m, "bke: z is [N, m]");
+    a.z = z.data_ptr();
+    check_rc(bke_if_step(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_if_step");
+    return std::make_tuple(x_out, P_out, ni_out, status);
+}
+
 // smooth_batch(zs, N) from (x, P): returns (xSmooth [T, N, n], xhat [T, N, n]); x and P are not changed
 std::tuple<at::Tensor, at::Tensor> fls_smooth_batch(const at::Tensor &x, const at::Tensor &P, const at::Tensor &F, const at::Tensor &H,
                                                     const at::Tensor &Q, const at::Tensor &R, const at::Tensor &zs, int64_t lag)
@@ -460,6 +494,8 @@ TORCH_LIBRARY(bke, m)
     m.def("enkf_step(Tensor x, Tensor P, Tensor sigmas, Tensor Q, Tensor R, Tensor z, float dt, int fx_model, int hx_model, "
           "int seed, int counter, Tensor? F=None, Tensor? H=None) -> (Tensor, Tensor, Tensor)");
     m.def("srkf_step(Tensor x, Tensor L, Tensor F, Tensor H, Tensor Lq, Tensor Lr, Tensor z) -> (Tensor, Tensor)");
+    m.def("if_step(Tensor x, Tensor P_inv, Tensor no_information, Tensor F, Tensor F_inv, Tensor Q, Tensor H, Tensor R_inv, "
+          "Tensor z) -> (Tensor, Tensor, Tensor, Tensor)");
     m.def("fls_smooth_batch(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor zs, int N) -> (Tensor, Tensor)");
     m.def("systematic_resample(Tensor weights, float u) -> Tensor");
     m.def("stratified_resample(Tensor weights, Tensor uniforms) -> Tensor");
@@ -483,6 +519,7 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("ckf_step", &ckf_step);
     m.impl("enkf_step", &enkf_step);
     m.impl("srkf_step", &srkf_step);
+    m.impl("if_step", &if_step);
     m.impl("fls_smooth_batch", &fls_smooth_batch);
     m.impl("systematic_resample", &systematic_resample);
     m.impl("stratified_resample", &stratified_resample);

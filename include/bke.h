@@ -600,6 +600,67 @@ int bke_srkf_step(const bke_srkf_args *args, void *stream);
 int bke_cholesky_lower(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *L,
                        int32_t *status, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Information filter bank.
+ * Replaces InformationFilter.predict / update (filterpy/kalman/information_filter.py:245-289, 178-243) for N
+ * filters at once.  The state is x[N,n], the information matrix P_inv[N,n,n] and the flag no_information[N]
+ * (uint8, read and written; 0 at construction).  The models are F, F_inv (inv(F) as the F setter last
+ * computed it: an in-place edit of F does not refresh it), Q[n,n], H[m,n], R_inv[m,m] and B / u, each per
+ * filter or shared (stride 0).  Per filter, in this order (flags = BKE_DO_PREDICT | BKE_DO_UPDATE):
+ *   predict  A = F_inv' P_inv F_inv.  A invertible:  if no_information: x <- inv(P_inv) x (0 x when P_inv is
+ *            singular), no_information <- 0;  x <- F x (+ B u);  P_inv <- inv(inv(A) + Q)     [x_prior, P_inv_prior]
+ *            A singular:  no_information <- 1;  FTI = inv(F');  AQI = inv(A + Q);
+ *            x <- FTI ((I - P_inv F_inv) AQI) (FTI x);  P_inv unchanged                 [x_prior, P_inv_prior = AQI]
+ *   update   no_information set:  x <- P_inv x + H' R_inv z;  P_inv <- P_inv + H' R_inv H;
+ *                                  log_likelihood = log(DBL_MIN); y, K, S unchanged
+ *            otherwise:  y = z - H x;  S = P_inv + H' R_inv H (n x n);  K = inv(S) H' R_inv;  x <- x + K y;
+ *                        P_inv <- S;  log_likelihood per ll_mode (BKE_IF_LL_*)
+ * "inv fails" is a pivot of the partially pivoted elimination that is exactly zero (LAPACK's dgetrf2
+ * decision for n = 2 in the register tile).  A singular A is a branch.  A singular inv(A) + Q, F', A + Q
+ * or S is where the reference's np.linalg.inv raises: status[f] = BKE_STATUS_SINGULAR_S and the filter stops there with what the
+ * reference has set by then (a failed predict keeps P_inv, skips the update and writes no prior; a failed
+ * update keeps x and P_inv and writes y and S but not K).
+ * z_valid[i] == 0 means "z is None" (:194-198): nothing of that filter changes in the update.  Optional
+ * outputs (NULL = not wanted): x_prior, P_inv_prior (written by a predict), K[N,n,m], y[N,m], S[N,n,n],
+ * log_likelihood[N], status[N] (only written on failure with BKE_STATUS_STICKY).  x_out / P_inv_out may
+ * alias x / P_inv.  ll_mode other than BKE_IF_LL_NONE needs log_likelihood and the m it names.
+ * Kernels (picked by shape, DESIGN.md §3.5e): a register tile per thread for 1/1, 2/1, 2/2, 3/1, 4/1, 4/2,
+ * 4/4 and (fp32) 6/3 without control input, a warp per filter for every other shape. */
+#define BKE_IF_LL_NONE 0             /* log_likelihood is not computed by an informed update */
+#define BKE_IF_LL_FULL 1             /* m == n: log N(y; 0, S) (stats.py logpdf, information_filter.py:235) */
+#define BKE_IF_LL_BROADCAST 2        /* m == 1: log N([y, .., y]; 0, S), scipy's broadcast of y over n */
+typedef struct bke_if_args {
+    int64_t n_filters;
+    int32_t dim_x, dim_z, dim_u;     /* dim_u may be 0 */
+    int32_t dtype;
+    uint32_t flags;                  /* BKE_DO_PREDICT | BKE_DO_UPDATE | BKE_STATUS_STICKY */
+    int32_t ll_mode;                 /* BKE_IF_LL_* */
+    const void *x, *P_inv;           /* in  */
+    void *x_out, *P_inv_out;         /* out */
+    uint8_t *no_information;         /* [N], read and written */
+    const void *F; int64_t F_stride;
+    const void *F_inv; int64_t F_inv_stride;
+    const void *Q; int64_t Q_stride;
+    const void *H; int64_t H_stride;
+    const void *R_inv; int64_t R_inv_stride;
+    const void *B; int64_t B_stride; /* [N,n,dim_u] or NULL */
+    const void *u; int64_t u_stride; /* [N,dim_u]   or NULL */
+    const void *z;                   /* [N,m]; may be NULL when BKE_DO_UPDATE is not set */
+    const uint8_t *z_valid;          /* [N] or NULL */
+    void *x_prior, *P_inv_prior;
+    void *K, *y, *S, *log_likelihood;
+    int32_t *status;
+} bke_if_args;
+
+int bke_if_step(const bke_if_args *args, void *stream);
+
+/* np.linalg.inv per filter, for the InformationFilter's F setter (F_inv) and P property:
+ * Ai[N,k,k] = inv(A[f]), A[f] at A + f * stride (stride 0: one matrix for every filter, k*k: per filter).
+ * status[N] (may be NULL) = BKE_STATUS_SINGULAR_S where a pivot is exactly zero (Ai is then undefined).
+ * k >= 1; BKE_ERR_UNSUPPORTED when a k x k pair does not fit a warp's shared memory. */
+int bke_inverse(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *Ai,
+                int32_t *status, void *stream);
+
 /* Stand-alone pieces of the unscented path for callers that use them directly:
  *   MerweScaledSigmaPoints.sigma_points(x, P)   filterpy/kalman/sigma_points.py:124-177
  *       x[N,n], P[N,n,n] -> sigmas[N,2n+1,n]; status[N] = BKE_STATUS_NOT_PD where scipy's cholesky
