@@ -43,6 +43,7 @@ EXPORTED_SYMBOLS = [
     "bke_enkf_initialize", "bke_enkf_step", "bke_enkf_model_compile", "bke_enkf_step_model", "bke_debug_enkf_model_cubin_bytes",
     "bke_srkf_step", "bke_cholesky_lower",
     "bke_if_step", "bke_inverse",
+    "bke_poly_filter",
     "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
     "bke_resample_bank", "bke_gather_rows_bank",
     "bke_multinomial_resample_bank_workspace_bytes", "bke_multinomial_resample_bank",
@@ -238,6 +239,28 @@ class IfArgs(ctypes.Structure):
         ("x_prior", c_void_p), ("P_inv_prior", c_void_p),
         ("K", c_void_p), ("y", c_void_p), ("S", c_void_p), ("log_likelihood", c_void_p),
         ("status", c_void_p),
+    ]
+
+BKE_POLY_GH, BKE_POLY_GHK, BKE_POLY_GH_ORDER, BKE_POLY_LSQ, BKE_POLY_FADING = 0, 1, 2, 3, 4
+BKE_POLY_UPDATE, BKE_POLY_BATCH = 0, 1
+
+
+class PolyArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_filters", c_int64), ("n_steps", c_int64),
+        ("family", c_int32), ("order", c_int32), ("dtype", c_int32), ("mode", c_int32),
+        ("x", c_void_p), ("dx", c_void_p), ("ddx", c_void_p),
+        ("g", c_void_p), ("g_stride", c_int64),
+        ("h", c_void_p), ("h_stride", c_int64),
+        ("k", c_void_p), ("k_stride", c_int64),
+        ("dt", c_void_p), ("dt_stride", c_int64),
+        ("dt2", c_void_p), ("dt2_stride", c_int64),
+        ("hdt2", c_void_p), ("hdt2_stride", c_int64),
+        ("n", c_void_p), ("n_max", c_int64),
+        ("z", c_void_p),
+        ("results", c_void_p), ("predictions", c_void_p), ("y", c_void_p),
+        ("x_prediction", c_void_p), ("dx_prediction", c_void_p), ("ddx_prediction", c_void_p),
+        ("K", c_void_p),
     ]
 
 
@@ -491,6 +514,8 @@ def load():
     lib.bke_if_step.restype = ctypes.c_int
     lib.bke_inverse.argtypes = [c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
     lib.bke_inverse.restype = ctypes.c_int
+    lib.bke_poly_filter.argtypes = [ctypes.POINTER(PolyArgs), c_void_p]
+    lib.bke_poly_filter.restype = ctypes.c_int
     lib.bke_resample_workspace_bytes.argtypes = [c_int64]
     lib.bke_resample_workspace_bytes.restype = c_size_t
     lib.bke_systematic_resample.argtypes = [c_int64, c_void_p, c_double, c_void_p, c_void_p, c_size_t,

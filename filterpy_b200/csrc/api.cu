@@ -153,6 +153,64 @@ static int validate_if(const bke_if_args *a)
     return BKE_OK;
 }
 
+// the checks of bke_poly_filter
+static int validate_poly(const bke_poly_args *a)
+{
+    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    if (a->n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    if (a->n_steps < 1) { set_error("n_steps must be 1 or greater"); return BKE_ERR_BAD_ARG; }
+    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    const int fam = a->family;
+    if (fam < BKE_POLY_GH || fam > BKE_POLY_FADING) { set_error("family must be one of BKE_POLY_*"); return BKE_ERR_BAD_ARG; }
+    const bool gh = fam == BKE_POLY_GH || fam == BKE_POLY_GHK;
+    if (!gh && (a->order < 0 || a->order > 2)) { set_error("order must be between 0 and 2"); return BKE_ERR_BAD_ARG; }
+    if (a->mode != BKE_POLY_UPDATE && a->mode != BKE_POLY_BATCH) { set_error("mode must be BKE_POLY_UPDATE or BKE_POLY_BATCH"); return BKE_ERR_BAD_ARG; }
+    const bool batch = a->mode == BKE_POLY_BATCH;
+    const int ord = fam == BKE_POLY_GH ? 1 : fam == BKE_POLY_GHK ? 2 : a->order;
+    if (a->n_filters == 0) return BKE_OK;
+    // what the instance reads
+    const bool need_dx = gh, need_ddx = fam == BKE_POLY_GHK && !batch;
+    const bool need_g = fam != BKE_POLY_LSQ;
+    const bool need_h = gh || (ord >= 1 && fam != BKE_POLY_LSQ);
+    const bool need_k = (fam == BKE_POLY_GHK && !batch) || (ord == 2 && (fam == BKE_POLY_GH_ORDER || fam == BKE_POLY_FADING));
+    const bool need_dt = ord >= 1;
+    const bool need_dt2 = (fam == BKE_POLY_GHK && !batch) || (!gh && ord == 2);
+    const bool need_hdt2 = fam == BKE_POLY_LSQ && ord == 2;
+    if (!a->x || !a->z || (need_dx && !a->dx) || (need_ddx && !a->ddx)) { set_error("the state and z must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if ((need_g && !a->g) || (need_h && !a->h) || (need_k && !a->k) || (need_dt && !a->dt) || (need_dt2 && !a->dt2) ||
+        (need_hdt2 && !a->hdt2)) {
+        set_error("a parameter this family and order read is NULL");
+        return BKE_ERR_BAD_ARG;
+    }
+    auto bad_stride = [](const void *p, int64_t s) { return p && s != 0 && s != 1; };
+    if (bad_stride(a->g, a->g_stride) || bad_stride(a->h, a->h_stride) || bad_stride(a->k, a->k_stride) ||
+        bad_stride(a->dt, a->dt_stride) || bad_stride(a->dt2, a->dt2_stride) || bad_stride(a->hdt2, a->hdt2_stride)) {
+        set_error("parameter strides must be 0 (shared) or 1 (per filter)");
+        return BKE_ERR_BAD_ARG;
+    }
+    // the outputs each family and mode have
+    if (a->predictions && !(gh && batch)) { set_error("predictions is an output of the GH / GHK batch_filter only"); return BKE_ERR_BAD_ARG; }
+    if (a->y && (batch || fam == BKE_POLY_LSQ || fam == BKE_POLY_FADING)) {
+        set_error("y is an output of the GH, GHK and GH_ORDER update only");      // least_squares.py:128 never stores y
+        return BKE_ERR_BAD_ARG;
+    }
+    if ((a->x_prediction || a->dx_prediction) && !(gh && !batch)) { set_error("x_prediction / dx_prediction are outputs of the GH / GHK update only"); return BKE_ERR_BAD_ARG; }
+    if (a->ddx_prediction && !(fam == BKE_POLY_GHK && !batch)) { set_error("ddx_prediction is an output of the GHK update only"); return BKE_ERR_BAD_ARG; }
+    if (a->K && !(fam == BKE_POLY_LSQ && !batch)) { set_error("K is an output of the LSQ update only"); return BKE_ERR_BAD_ARG; }
+    if (fam == BKE_POLY_LSQ) {
+        if (!a->n) { set_error("LSQ needs the counter n"); return BKE_ERR_BAD_ARG; }
+        // the largest counter the call reaches, and the product of it the order's gains form (least_squares.py:131-145)
+        int64_t top, p;
+        if (a->n_max < 0 || __builtin_add_overflow(a->n_max, a->n_steps, &top) ||
+            (ord >= 1 && __builtin_mul_overflow(top, top + 1, &p)) ||
+            (ord == 2 && (__builtin_mul_overflow(p, top + 2, &p) || __builtin_mul_overflow(top, 3 * top, &p)))) {
+            set_error("the LSQ counter n_max + n_steps overflows int64 in n(n+1)(n+2) (or the product its order forms)");
+            return BKE_ERR_BAD_ARG;
+        }
+    }
+    return BKE_OK;
+}
+
 // the checks every sigma-point step (UKF, CKF, EnKF; pre-built and run-time compiled) makes
 template <typename Args>
 static int validate_sigma(const Args &a)
@@ -581,6 +639,15 @@ int bke_inverse(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int6
     if (rc) return rc;
     if (n_filters == 0) return BKE_OK;
     return launch_inverse(n_filters, k, dtype, A, stride, Ai, status, (cudaStream_t)stream);
+}
+
+int bke_poly_filter(const bke_poly_args *args, void *stream)
+{
+    int rc = validate_poly(args);
+    if (rc) return rc;
+    if ((rc = require_device())) return rc;
+    if (args->n_filters == 0) return BKE_OK;
+    return launch_poly(*args, (cudaStream_t)stream);
 }
 
 }  // extern "C"

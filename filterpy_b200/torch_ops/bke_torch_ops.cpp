@@ -10,6 +10,8 @@
 //   bke::enkf_step            bke_enkf_step            EnsembleKalmanFilter.predict + update, ensemble_kalman_filter.py:218-290
 //   bke::srkf_step            bke_srkf_step            SquareRootKalmanFilter.predict + update, square_root.py:172-248
 //   bke::if_step              bke_if_step              InformationFilter.predict + update, information_filter.py:178-289
+//   bke::poly_filter          bke_poly_filter          GHFilter / GHKFilter / GHFilterOrder / LeastSquaresFilter / FadingMemoryFilter
+//                                                      update (T epochs) and the g-h batch_filter, gh_filter.py, least_squares.py, fading_memory.py
 //   bke::fls_smooth_batch     bke_fls_smooth           FixedLagSmoother.smooth_batch, fixed_lag_smoother.py:217-311
 //   bke::systematic_resample  bke_systematic_resample  monte_carlo/resampling.py:117-150
 //   bke::stratified_resample  bke_stratified_resample  monte_carlo/resampling.py:80-114
@@ -272,6 +274,80 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> if_step(const at::Ten
     return std::make_tuple(x_out, P_out, ni_out, status);
 }
 
+// a polynomial tracker parameter: 0-d (shared, stride 0) or [N] (per filter, stride 1); undefined = not given
+const void *poly_param(const c10::optional<at::Tensor> &t, int64_t N, int64_t *stride, const at::Tensor &like, const char *name)
+{
+    if (!t.has_value() || !t->defined()) return nullptr;
+    TORCH_CHECK(t->is_cuda() && t->device() == like.device() && t->is_contiguous() && t->scalar_type() == like.scalar_type(),
+                "bke: ", name, " must be a contiguous CUDA tensor of the state's dtype, on its device");
+    TORCH_CHECK(t->dim() == 0 || (t->dim() == 1 && t->size(0) == N), "bke: ", name, " is 0-d (shared) or [N]");
+    *stride = t->dim() == 0 ? 0 : 1;
+    return t->data_ptr();
+}
+
+// T epochs of update() (batch = false) or batch_filter (batch = true) on z[T, N].  Returns (x, dx, ddx, n, results,
+// predictions): the state after the call (the input state for batch), results[T+1, N, W] and, for the g-h batch,
+// predictions[T, N]; what the family does not have is an empty tensor.  The inputs are not modified.
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> poly_filter(
+    const at::Tensor &x, const c10::optional<at::Tensor> &dx, const c10::optional<at::Tensor> &ddx,
+    const c10::optional<at::Tensor> &n, const at::Tensor &z, const c10::optional<at::Tensor> &g,
+    const c10::optional<at::Tensor> &h, const c10::optional<at::Tensor> &k, const c10::optional<at::Tensor> &dt,
+    const c10::optional<at::Tensor> &dt2, const c10::optional<at::Tensor> &hdt2, int64_t family, int64_t order, bool batch)
+{
+    TORCH_CHECK(family >= BKE_POLY_GH && family <= BKE_POLY_FADING, "bke: family must be one of BKE_POLY_*");
+    const bool gh = family == BKE_POLY_GH || family == BKE_POLY_GHK;
+    TORCH_CHECK(gh || (order >= 0 && order <= 2), "bke: order must be between 0 and 2");
+    // the kernel indexes x as [N] (GH / GHK) or [N, order+1] and the call carries no size for it: check the shape here
+    TORCH_CHECK(x.is_cuda(), "bke: x must be a CUDA tensor");
+    if (gh) {
+        TORCH_CHECK(x.dim() == 1, "bke: x of GH / GHK is [N] (dx and ddx are separate tensors)");
+    } else {
+        TORCH_CHECK(x.dim() == 2 && x.size(1) == order + 1, "bke: x is [N, order+1] = [N, ", order + 1, "], got ", x.sizes());
+    }
+    c10::cuda::CUDAGuard guard(x.device());
+    const int64_t N = x.size(0);
+    TORCH_CHECK(z.is_cuda() && z.device() == x.device() && z.is_contiguous() && z.scalar_type() == x.scalar_type() &&
+                z.dim() == 2 && z.size(1) == N, "bke: z is [T, N] in the state's dtype, on x's device");
+    bke_poly_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_filters = N; a.n_steps = z.size(0); a.family = (int32_t)family; a.order = (int32_t)order; a.dtype = dtype_of(x);
+    a.mode = batch ? BKE_POLY_BATCH : BKE_POLY_UPDATE;
+    auto state = [&](const c10::optional<at::Tensor> &t, const char *name) {
+        if (!t.has_value() || !t->defined()) return at::Tensor();
+        TORCH_CHECK(t->is_cuda() && t->device() == x.device() && t->scalar_type() == x.scalar_type() && t->dim() == 1 &&
+                    t->size(0) == N, "bke: ", name, " is a CUDA tensor [N] of x's dtype, on x's device");
+        return t->contiguous().clone();
+    };
+    at::Tensor x_out = x.contiguous().clone(), dx_out = state(dx, "dx"), ddx_out = state(ddx, "ddx"), n_out;
+    a.x = x_out.data_ptr();
+    a.dx = dx_out.defined() ? dx_out.data_ptr() : nullptr;
+    a.ddx = ddx_out.defined() ? ddx_out.data_ptr() : nullptr;
+    if (family == BKE_POLY_LSQ) {
+        TORCH_CHECK(n.has_value() && n->is_cuda() && n->device() == x.device() && n->scalar_type() == at::kLong && n->dim() == 1 && n->size(0) == N,
+                    "bke: LSQ needs the counter n, an int64 CUDA tensor [N]");
+        n_out = n->contiguous().clone();
+        a.n = n_out.data_ptr<int64_t>();
+        a.n_max = N ? n_out.max().item<int64_t>() : 0;
+    }
+    a.g = poly_param(g, N, &a.g_stride, x, "g");
+    a.h = poly_param(h, N, &a.h_stride, x, "h");
+    a.k = poly_param(k, N, &a.k_stride, x, "k");
+    a.dt = poly_param(dt, N, &a.dt_stride, x, "dt");
+    a.dt2 = poly_param(dt2, N, &a.dt2_stride, x, "dt2");
+    a.hdt2 = poly_param(hdt2, N, &a.hdt2_stride, x, "hdt2");
+    a.z = z.data_ptr();
+    const int64_t W = gh ? 2 : order + 1;
+    at::Tensor results = at::empty({z.size(0) + 1, N, W}, x.options()), predictions;
+    a.results = results.data_ptr();
+    if (gh && batch) {
+        predictions = at::empty({z.size(0), N}, x.options());
+        a.predictions = predictions.data_ptr();
+    }
+    check_rc(bke_poly_filter(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_poly_filter");
+    auto or_empty = [&](const at::Tensor &t) { return t.defined() ? t : at::empty({0}, x.options()); };
+    return std::make_tuple(x_out, or_empty(dx_out), or_empty(ddx_out), or_empty(n_out), results, or_empty(predictions));
+}
+
 // smooth_batch(zs, N) from (x, P): returns (xSmooth [T, N, n], xhat [T, N, n]); x and P are not changed
 std::tuple<at::Tensor, at::Tensor> fls_smooth_batch(const at::Tensor &x, const at::Tensor &P, const at::Tensor &F, const at::Tensor &H,
                                                     const at::Tensor &Q, const at::Tensor &R, const at::Tensor &zs, int64_t lag)
@@ -496,6 +572,8 @@ TORCH_LIBRARY(bke, m)
     m.def("srkf_step(Tensor x, Tensor L, Tensor F, Tensor H, Tensor Lq, Tensor Lr, Tensor z) -> (Tensor, Tensor)");
     m.def("if_step(Tensor x, Tensor P_inv, Tensor no_information, Tensor F, Tensor F_inv, Tensor Q, Tensor H, Tensor R_inv, "
           "Tensor z) -> (Tensor, Tensor, Tensor, Tensor)");
+    m.def("poly_filter(Tensor x, Tensor? dx, Tensor? ddx, Tensor? n, Tensor z, Tensor? g, Tensor? h, Tensor? k, Tensor? dt, "
+          "Tensor? dt2, Tensor? hdt2, int family, int order, bool batch=False) -> (Tensor, Tensor, Tensor, Tensor, Tensor, Tensor)");
     m.def("fls_smooth_batch(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor zs, int N) -> (Tensor, Tensor)");
     m.def("systematic_resample(Tensor weights, float u) -> Tensor");
     m.def("stratified_resample(Tensor weights, Tensor uniforms) -> Tensor");
@@ -520,6 +598,7 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("enkf_step", &enkf_step);
     m.impl("srkf_step", &srkf_step);
     m.impl("if_step", &if_step);
+    m.impl("poly_filter", &poly_filter);
     m.impl("fls_smooth_batch", &fls_smooth_batch);
     m.impl("systematic_resample", &systematic_resample);
     m.impl("stratified_resample", &stratified_resample);

@@ -661,6 +661,68 @@ int bke_if_step(const bke_if_args *args, void *stream);
 int bke_inverse(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *Ai,
                 int32_t *status, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Polynomial tracker banks: the g-h family, the expanding-memory least-squares filter and the fading-memory
+ * filter, n_steps epochs of N filters in one launch (one thread per filter, the time loop inside the kernel).
+ *   BKE_POLY_GH        GHFilter.update / batch_filter        filterpy/gh/gh_filter.py:363-377, 421-455
+ *   BKE_POLY_GHK       GHKFilter.update / batch_filter       gh_filter.py:659-680, 717-748
+ *   BKE_POLY_GH_ORDER  GHFilterOrder.update, order 0..2      gh_filter.py:142-181
+ *   BKE_POLY_LSQ       LeastSquaresFilter.update, order 0..2 filterpy/leastsq/least_squares.py:122-155
+ *   BKE_POLY_FADING    FadingMemoryFilter.update, order 0..2 filterpy/memory/fading_memory.py:164-194
+ * State: GH / GHK keep x[N], dx[N] (and ddx[N] for GHK; order is ignored); the others keep x[N, order+1].
+ * mode BKE_POLY_UPDATE runs n_steps calls of update() on z[t, :] and writes the state back (LSQ: n[N] and K
+ * [N, order+1] too).  mode BKE_POLY_BATCH reads the state and leaves it alone: GH and GHK run batch_filter's
+ * recursion (GHKFilter.batch_filter is GHFilter's: k and ddx are not read), the others run update()'s.
+ * Parameters, each per filter (stride 1) or shared (stride 0), in the state's dtype.  Every constant the
+ * reference derives from its scalars is computed by the caller with the reference's expression:
+ *   g    GH, GHK, GH_ORDER: g                      FADING: G (1 - beta, 1 - beta**2, 1 - beta**3 by order)
+ *   h    GH, GHK, GH_ORDER 1-2 (update): h         GH, GHK (batch): h / dt      FADING 1-2: H / dt
+ *   k    GHK (update), GH_ORDER 2: k               FADING 2: 2*K / dt**2
+ *   dt   every family but the order-0 filters
+ *   dt2  dt**2: GHK (update), GH_ORDER 2, LSQ 2, FADING 2
+ *   hdt2 0.5 * dt**2: LSQ 2
+ * A parameter the instance does not read may be NULL.  LSQ reads and advances n[N] (int64; its gains come from
+ * the counter by exact int64 arithmetic and round-to-nearest conversions, as Python's do); n_max is an upper
+ * bound of n[] on entry, and the call is refused when the counter's products (n, n(n+1), n(n+1)(n+2) for
+ * order 0, 1, 2) could overflow int64 within n_steps.
+ * Optional outputs (NULL = not wanted):
+ *   results[T+1, N, W]   the state before the first and after every epoch: W = 2 (x, dx) for GH / GHK,
+ *                        order+1 otherwise
+ *   predictions[T, N]    batch_filter's x_est: GH / GHK batch only
+ *   y[N]                 the last residual: GH, GHK, GH_ORDER update only
+ *   x_prediction, dx_prediction [N]: GH / GHK update;  ddx_prediction[N]: GHK update
+ *   K[N, order+1]        the last gains: LSQ update only
+ * An output the family and mode do not have is refused with BKE_ERR_BAD_ARG. */
+#define BKE_POLY_GH 0
+#define BKE_POLY_GHK 1
+#define BKE_POLY_GH_ORDER 2
+#define BKE_POLY_LSQ 3
+#define BKE_POLY_FADING 4
+#define BKE_POLY_UPDATE 0
+#define BKE_POLY_BATCH 1
+typedef struct bke_poly_args {
+    int64_t n_filters;
+    int64_t n_steps;                 /* T >= 1 */
+    int32_t family, order;           /* BKE_POLY_*; order 0..2 (GH_ORDER, LSQ, FADING) */
+    int32_t dtype;
+    int32_t mode;                    /* BKE_POLY_UPDATE or BKE_POLY_BATCH */
+    void *x, *dx, *ddx;              /* read, and written by BKE_POLY_UPDATE */
+    const void *g; int64_t g_stride;
+    const void *h; int64_t h_stride;
+    const void *k; int64_t k_stride;
+    const void *dt; int64_t dt_stride;
+    const void *dt2; int64_t dt2_stride;
+    const void *hdt2; int64_t hdt2_stride;
+    int64_t *n;                      /* LSQ: [N] */
+    int64_t n_max;                   /* LSQ: max(n) on entry */
+    const void *z;                   /* [T, N] */
+    void *results, *predictions, *y;
+    void *x_prediction, *dx_prediction, *ddx_prediction;
+    void *K;
+} bke_poly_args;
+
+int bke_poly_filter(const bke_poly_args *args, void *stream);
+
 /* Stand-alone pieces of the unscented path for callers that use them directly:
  *   MerweScaledSigmaPoints.sigma_points(x, P)   filterpy/kalman/sigma_points.py:124-177
  *       x[N,n], P[N,n,n] -> sigmas[N,2n+1,n]; status[N] = BKE_STATUS_NOT_PD where scipy's cholesky
