@@ -44,6 +44,7 @@ EXPORTED_SYMBOLS = [
     "bke_srkf_step", "bke_cholesky_lower",
     "bke_if_step", "bke_inverse",
     "bke_poly_filter",
+    "bke_score_measurements",
     "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
     "bke_resample_bank", "bke_gather_rows_bank",
     "bke_multinomial_resample_bank_workspace_bytes", "bke_multinomial_resample_bank",
@@ -261,6 +262,22 @@ class PolyArgs(ctypes.Structure):
         ("results", c_void_p), ("predictions", c_void_p), ("y", c_void_p),
         ("x_prediction", c_void_p), ("dx_prediction", c_void_p), ("ddx_prediction", c_void_p),
         ("K", c_void_p),
+    ]
+
+
+class ScoreArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_tracks", c_int64), ("n_candidates", c_int64),
+        ("dim_x", c_int32), ("dim_z", c_int32), ("dtype", c_int32), ("reserved", c_int32),
+        ("x", c_void_p), ("mean", c_void_p), ("P", c_void_p),
+        ("S", c_void_p), ("S_stride", c_int64),
+        ("H", c_void_p), ("H_stride", c_int64),
+        ("R", c_void_p), ("R_stride", c_int64),
+        ("z", c_void_p), ("z_track_stride", c_int64), ("z_cand_stride", c_int64),
+        ("z_valid", c_void_p),
+        ("zhat", c_void_p), ("y", c_void_p), ("d2", c_void_p), ("mahalanobis", c_void_p),
+        ("log_likelihood", c_void_p), ("likelihood", c_void_p),
+        ("status", c_void_p),
     ]
 
 
@@ -516,6 +533,8 @@ def load():
     lib.bke_inverse.restype = ctypes.c_int
     lib.bke_poly_filter.argtypes = [ctypes.POINTER(PolyArgs), c_void_p]
     lib.bke_poly_filter.restype = ctypes.c_int
+    lib.bke_score_measurements.argtypes = [ctypes.POINTER(ScoreArgs), c_void_p]
+    lib.bke_score_measurements.restype = ctypes.c_int
     lib.bke_resample_workspace_bytes.argtypes = [c_int64]
     lib.bke_resample_workspace_bytes.restype = c_size_t
     lib.bke_systematic_resample.argtypes = [c_int64, c_void_p, c_double, c_void_p, c_void_p, c_size_t,

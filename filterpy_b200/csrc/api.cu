@@ -211,6 +211,47 @@ static int validate_poly(const bke_poly_args *a)
     return BKE_OK;
 }
 
+// the checks of bke_score_measurements
+static int validate_score(const bke_score_args *a)
+{
+    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    if (a->n_tracks < 0 || a->n_candidates < 0) { set_error("n_tracks and n_candidates must be 0 or greater"); return BKE_ERR_BAD_ARG; }
+    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    const bool uses_n = a->x || a->P;
+    if (a->dim_z < 1 || a->dim_z > 1024 || (uses_n && (a->dim_x < 1 || a->dim_x > 1024))) {
+        set_error("dim_z (and dim_x, when x or P is given) must be between 1 and 1024");
+        return BKE_ERR_BAD_ARG;
+    }
+    const int64_t n = a->dim_x, m = a->dim_z;
+    if (!a->x == !a->mean) { set_error("exactly one of x and mean must be given"); return BKE_ERR_BAD_ARG; }
+    if (a->P && a->S) { set_error("at most one of P and S may be given"); return BKE_ERR_BAD_ARG; }
+    if (a->H && !uses_n) { set_error("H maps x or P: it is read only with one of them"); return BKE_ERR_BAD_ARG; }
+    if (uses_n && !a->H && n != m) { set_error("without H (the identity) dim_x must equal dim_z"); return BKE_ERR_BAD_ARG; }
+    if (a->P && !a->R) { set_error("S = H P H' + R needs R"); return BKE_ERR_BAD_ARG; }
+    if (a->R && !a->P) { set_error("R is read only with P"); return BKE_ERR_BAD_ARG; }
+    if ((a->H && a->H_stride != 0 && a->H_stride != m * n) || (a->R && a->R_stride != 0 && a->R_stride != m * m) ||
+        (a->S && a->S_stride != 0 && a->S_stride != m * m)) {
+        set_error("H, R and S strides must be 0 (shared) or the dense per-track size");
+        return BKE_ERR_BAD_ARG;
+    }
+    const bool scores = a->d2 || a->mahalanobis || a->log_likelihood || a->likelihood;
+    if (!(a->zhat || a->y || scores || a->status)) { set_error("no output is requested"); return BKE_ERR_BAD_ARG; }
+    if ((scores || a->status) && !a->P && !a->S) { set_error("the scores and status need a covariance: P or S"); return BKE_ERR_BAD_ARG; }
+    if ((a->y || scores) && !a->z) { set_error("y and the scores need z"); return BKE_ERR_BAD_ARG; }
+    if (a->z_track_stride < 0 || a->z_cand_stride < 0) { set_error("z strides must be 0 or greater"); return BKE_ERR_BAD_ARG; }
+    // every offset the kernel forms fits int64: pair * m, and z's last element
+    int64_t pairs, t, u, last;
+    if (__builtin_mul_overflow(a->n_tracks, a->n_candidates, &pairs) || __builtin_mul_overflow(pairs, m, &t) ||
+        (a->n_tracks > 0 && __builtin_mul_overflow(a->n_tracks - 1, a->z_track_stride, &t)) ||
+        (a->n_candidates > 0 && __builtin_mul_overflow(a->n_candidates - 1, a->z_cand_stride, &u)) ||
+        (a->n_tracks > 0 && a->n_candidates > 0 && __builtin_add_overflow(t, u, &last)) ||
+        (a->n_tracks > 0 && a->n_candidates > 0 && __builtin_add_overflow(last, m, &last))) {
+        set_error("N * K * dim_z or the z offsets overflow int64");
+        return BKE_ERR_BAD_ARG;
+    }
+    return BKE_OK;
+}
+
 // the checks every sigma-point step (UKF, CKF, EnKF; pre-built and run-time compiled) makes
 template <typename Args>
 static int validate_sigma(const Args &a)
@@ -648,6 +689,15 @@ int bke_poly_filter(const bke_poly_args *args, void *stream)
     if ((rc = require_device())) return rc;
     if (args->n_filters == 0) return BKE_OK;
     return launch_poly(*args, (cudaStream_t)stream);
+}
+
+int bke_score_measurements(const bke_score_args *args, void *stream)
+{
+    int rc = validate_score(args);
+    if (rc) return rc;
+    if ((rc = require_device())) return rc;
+    if (args->n_tracks == 0 || args->n_candidates == 0) return BKE_OK;
+    return launch_score(*args, (cudaStream_t)stream);
 }
 
 }  // extern "C"

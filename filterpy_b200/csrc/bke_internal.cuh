@@ -84,6 +84,7 @@ int launch_if(const bke_if_args &a, cudaStream_t s);
 int launch_inverse(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *Ai, int32_t *status,
                    cudaStream_t s);
 int launch_poly(const bke_poly_args &a, cudaStream_t s);
+int launch_score(const bke_score_args &a, cudaStream_t s);
 #endif
 
 }  // namespace bke

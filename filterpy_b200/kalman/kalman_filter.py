@@ -2,7 +2,8 @@
 
 Same names, argument meaning and error behaviour as the reference
 (``filterpy/kalman/kalman_filter.py``: ``__init__`` :387-434, ``predict`` :437-482, ``update``
-:485-561, ``update_correlated`` :670-752, ``update_sequential`` :754-824, ``batch_filter`` :826-993, ``rts_smoother`` :995-1074; procedural ``predict`` :1571,
+:485-561, ``update_correlated`` :670-752, ``update_sequential`` :754-824, ``batch_filter`` :826-993, ``rts_smoother`` :995-1074,
+``residual_of`` / ``measurement_of_state`` / ``log_likelihood_of`` :1175-1201, 1252-1260; procedural ``predict`` :1571,
 ``update`` :1401, ``batch_filter`` :1664, ``rts_smoother`` :1792), with one addition: a leading ``n_filters`` axis.  All arithmetic runs in
 the hand-written CUDA kernels behind the C-ABI (``include/bke.h``); this file only validates
 shapes, owns the device tensors and fills the argument structs.  There is no CPU fallback.
@@ -28,6 +29,7 @@ import torch
 from .. import _lib
 from .._dev import StepGraph, bke_dtype, ptr, require_cuda, resolve_dtype, stream_ptr, to_dev
 from ..common.helpers import reshape_z
+from ..stats.stats import LOG_DBL_MIN, _candidates, _valid, score as _score
 from ._bank import _BankMirror, _model_prop
 
 __all__ = ["KalmanFilter", "predict", "update", "batch_filter", "rts_smoother"]
@@ -473,6 +475,74 @@ class KalmanFilter(_BankMirror):
         ra.z_record = ptr(self._zrec)
         self._form_launch(self._lib.bke_kf_update_rows, ra, stream_ptr(self._device))
         self._z = self._zrec
+
+    # ------------------------------------------------------------------ scores without a step
+    def _candidates(self, z):
+        """Bank-mode ``z`` of the scoring methods -> (``z[N or 1, K, m]``, whether it was ``[N, m]``)."""
+        return _candidates(z, self.n_filters, self.dim_z, self._dtype, self._device)
+
+    def log_likelihood_of(self, z, valid=None):
+        """kalman_filter.py:1252-1260: logpdf(z, H x, S) with the current x and the S stored by the last update,
+        not one formed from P (after ``predict`` the result mixes the prior x with the old S, as the reference's
+        docstring warns).  ``z=None`` is log(DBL_MIN).  Bank mode: ``z`` is ``[N, m]`` (results ``[N]``), ``[N, K, m]``
+        or ``[1, K, m]`` (one scan for the whole bank; results ``[N, K]``); ``valid`` (bool, one per pair) marks
+        missing candidates, which score log(DBL_MIN).  A singular S scores NaN (bank) or raises ``LinAlgError``
+        (single mode), where scipy would return -inf or a pseudo-determinant value."""
+        self._flush()
+        S = self._diag("S")
+        N = self.n_filters
+        if z is None:
+            return LOG_DBL_MIN if self._single else torch.full((N,), LOG_DBL_MIN, dtype=self._dtype, device=self._device)
+        if self._single:
+            zt, sq = to_dev(np.asarray(z, dtype=np.float64).reshape(1, 1, -1), self._dtype, self._device), True
+            if zt.shape[-1] != self.dim_z:
+                raise ValueError("z must hold %d values, got %d" % (self.dim_z, zt.shape[-1]))
+        else:
+            zt, sq = self._candidates(z)
+        vt = _valid(valid, N, zt.shape[1], self._device)
+        out = _score(zt, x=self._x, S=S, H=self._H, valid=vt, want=("log_likelihood", "status"))
+        ll = out["log_likelihood"]
+        if self._single:
+            if int(out["status"][0].item()) != 0:
+                raise np.linalg.LinAlgError("Singular matrix")
+            return float(ll[0, 0].item())
+        return ll[:, 0] if sq else ll
+
+    def residual_of(self, z):
+        """kalman_filter.py:1175-1181: z - H x_prior.  Bank mode: ``z`` as in ``log_likelihood_of``, the result
+        ``[N, m]`` or ``[N, K, m]``."""
+        self._flush()
+        xp = self._diag("x_prior")
+        m = self.dim_z
+        if self._single:
+            zr = reshape_z(z, m, 2 if self._x_col else 1)
+            zt = to_dev(np.asarray(zr, dtype=np.float64).reshape(1, 1, m), self._dtype, self._device)
+            y = _score(zt, x=xp, H=self._H, want=("y",))["y"][0, 0].cpu().numpy()
+            return y.reshape(m, 1) if self._x_col else y
+        zt, sq = self._candidates(z)
+        y = _score(zt, x=xp, H=self._H, want=("y",))["y"]
+        return y[:, 0] if sq else y
+
+    def measurement_of_state(self, x):
+        """kalman_filter.py:1183-1201: H x.  Bank mode: ``x[N, n]`` -> ``[N, m]``."""
+        self._flush()
+        n = self.dim_x
+        if self._single:
+            xa = np.asarray(x, dtype=np.float64)
+            if xa.size != n:
+                raise ValueError("x must hold %d values, got %d" % (n, xa.size))
+            xt = to_dev(xa.reshape(1, n), self._dtype, self._device)
+        else:
+            xt = to_dev(x, self._dtype, self._device)
+            if xt.dim() == 3 and xt.shape[-1] == 1:
+                xt = xt[..., 0]
+            if tuple(xt.shape) != (self.n_filters, n):
+                raise ValueError("x must have shape (%d, %d), got %s" % (self.n_filters, n, tuple(xt.shape)))
+        zh = _score(None, x=xt.contiguous(), H=self._H, want=("zhat",))["zhat"]
+        if not self._single:
+            return zh
+        zh = zh[0].cpu().numpy()
+        return zh.reshape(-1, 1) if xa.ndim == 2 else zh
 
     def capture(self, fn, warmup=2):
         """Capture ``fn`` — a fixed sequence of ``predict()/update(z_buffer)`` calls on this bank —

@@ -16,6 +16,8 @@ The same symbols exposed as torch.ops.* via a C++ extension for zero-copy CUDA t
     x, P_inv, ni, status = torch.ops.bke.if_step(x, P_inv, ni, F, F_inv, Q, H, R_inv, z)   # information_filter.py:178-289
     x, dx, ddx, n, res, pred = torch.ops.bke.poly_filter(x, dx, ddx, n, z, g, h, k, dt, dt2, hdt2, family, order, batch)
                                                                    # gh_filter.py, least_squares.py, fading_memory.py
+    ll, d = torch.ops.bke.score_measurements(z, x, None, P, None, H, R, None, ["log_likelihood", "mahalanobis"])
+                                                                   # stats.py:64-154, N tracks x K candidates z[N|1, K, m]
     xs, xhat = torch.ops.bke.fls_smooth_batch(x, P, F, H, Q, R, zs, N)   # fixed_lag_smoother.py:217-311
     idx  = torch.ops.bke.systematic_resample(weights, u)           # resampling.py:117-150 (int32, bit-exact)
     idx  = torch.ops.bke.stratified_resample(weights, uniforms)    # resampling.py:80-114

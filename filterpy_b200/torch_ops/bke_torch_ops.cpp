@@ -12,6 +12,8 @@
 //   bke::if_step              bke_if_step              InformationFilter.predict + update, information_filter.py:178-289
 //   bke::poly_filter          bke_poly_filter          GHFilter / GHKFilter / GHFilterOrder / LeastSquaresFilter / FadingMemoryFilter
 //                                                      update (T epochs) and the g-h batch_filter, gh_filter.py, least_squares.py, fading_memory.py
+//   bke::score_measurements   bke_score_measurements   stats.mahalanobis / log_likelihood / logpdf / NEES and
+//                                                      KalmanFilter.log_likelihood_of, N tracks x K candidates
 //   bke::fls_smooth_batch     bke_fls_smooth           FixedLagSmoother.smooth_batch, fixed_lag_smoother.py:217-311
 //   bke::systematic_resample  bke_systematic_resample  monte_carlo/resampling.py:117-150
 //   bke::stratified_resample  bke_stratified_resample  monte_carlo/resampling.py:80-114
@@ -29,6 +31,7 @@
 #include <torch/library.h>
 #include <cstring>
 #include <tuple>
+#include <vector>
 #include "../../include/bke.h"
 
 namespace {
@@ -272,6 +275,66 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> if_step(const at::Ten
     a.z = z.data_ptr();
     check_rc(bke_if_step(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_if_step");
     return std::make_tuple(x_out, P_out, ni_out, status);
+}
+
+// N tracks against K candidates (bke_score_measurements): z is [N, K, m] or [1, K, m] (one scan shared by every
+// track); exactly one of x [N, n] and mean [N, m]; P (with R) or S; H, R, S shared [r, c] or per track [N, r, c];
+// valid [N, K] uint8.  `outputs` names the outputs wanted, returned in that order: zhat, y, d2, mahalanobis,
+// log_likelihood, likelihood, status.  Every tensor must be on z's device.
+std::vector<at::Tensor> score_measurements(const at::Tensor &z, const c10::optional<at::Tensor> &x,
+                                           const c10::optional<at::Tensor> &mean, const c10::optional<at::Tensor> &P,
+                                           const c10::optional<at::Tensor> &S, const c10::optional<at::Tensor> &H,
+                                           const c10::optional<at::Tensor> &R, const c10::optional<at::Tensor> &valid,
+                                           c10::ArrayRef<c10::string_view> outputs)
+{
+    TORCH_CHECK(z.is_cuda() && z.is_contiguous() && z.dim() == 3, "bke: z is a contiguous CUDA tensor [N, K, m] or [1, K, m]");
+    const int dt = dtype_of(z);
+    auto given = [](const c10::optional<at::Tensor> &t) { return t.has_value() && t->defined(); };
+    auto check = [&](const c10::optional<at::Tensor> &t, const char *name) {
+        if (!given(t)) return (const void *)nullptr;
+        TORCH_CHECK(t->is_cuda() && t->device() == z.device() && t->is_contiguous() && t->scalar_type() == z.scalar_type(),
+                    "bke: ", name, " must be a contiguous CUDA tensor of z's dtype, on z's device");
+        return (const void *)t->data_ptr();
+    };
+    TORCH_CHECK(given(x) != given(mean), "bke: exactly one of x and mean");
+    const at::Tensor &src = given(x) ? *x : *mean;
+    TORCH_CHECK(src.dim() == 2, "bke: x is [N, n], mean is [N, m]");
+    const int64_t N = src.size(0), K = z.size(1), m = z.size(2);
+    TORCH_CHECK(z.size(0) == N || z.size(0) == 1, "bke: z is [N, K, m] or [1, K, m]");
+    const int64_t n = given(x) ? x->size(1) : (given(P) ? P->size(-1) : m);
+    c10::cuda::CUDAGuard guard(z.device());
+    bke_score_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_tracks = N; a.n_candidates = K; a.dim_x = (int32_t)n; a.dim_z = (int32_t)m; a.dtype = dt;
+    a.x = check(x, "x"); a.mean = check(mean, "mean");
+    if (given(mean)) TORCH_CHECK(mean->size(1) == m, "bke: mean is [N, m]");
+    a.P = check(P, "P");
+    if (given(P)) TORCH_CHECK(P->dim() == 3 && P->size(0) == N && P->size(1) == n && P->size(2) == n, "bke: P is [N, n, n]");
+    if (given(S)) { check(S, "S"); a.S = model(*S, N, m, m, &a.S_stride, z, "S"); }
+    if (given(H)) { check(H, "H"); a.H = model(*H, N, m, n, &a.H_stride, z, "H"); }
+    if (given(R)) { check(R, "R"); a.R = model(*R, N, m, m, &a.R_stride, z, "R"); }
+    a.z = z.data_ptr(); a.z_track_stride = z.size(0) == 1 ? 0 : K * m; a.z_cand_stride = m;
+    if (given(valid)) {
+        TORCH_CHECK(valid->is_cuda() && valid->device() == z.device() && valid->scalar_type() == at::kByte &&
+                    valid->is_contiguous() && valid->numel() == N * K, "bke: valid is a contiguous uint8 CUDA tensor [N, K] on z's device");
+        a.z_valid = valid->data_ptr<uint8_t>();
+    }
+    std::vector<at::Tensor> out;
+    for (const auto &name : outputs) {
+        at::Tensor t;
+        if (name == "zhat") { t = at::empty({N, m}, z.options()); a.zhat = t.data_ptr(); }
+        else if (name == "y") { t = at::empty({N, K, m}, z.options()); a.y = t.data_ptr(); }
+        else if (name == "d2") { t = at::empty({N, K}, z.options()); a.d2 = t.data_ptr(); }
+        else if (name == "mahalanobis") { t = at::empty({N, K}, z.options()); a.mahalanobis = t.data_ptr(); }
+        else if (name == "log_likelihood") { t = at::empty({N, K}, z.options()); a.log_likelihood = t.data_ptr(); }
+        else if (name == "likelihood") { t = at::empty({N, K}, z.options()); a.likelihood = t.data_ptr(); }
+        else if (name == "status") { t = at::empty({N}, z.options().dtype(at::kInt)); a.status = t.data_ptr<int32_t>(); }
+        else TORCH_CHECK(false, "bke: unknown output ", name);
+        out.push_back(t);
+    }
+    if (N > 0 && K > 0)     // an empty tensor has no data pointer to pass
+        check_rc(bke_score_measurements(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_score_measurements");
+    return out;
 }
 
 // a polynomial tracker parameter: 0-d (shared, stride 0) or [N] (per filter, stride 1); undefined = not given
@@ -574,6 +637,8 @@ TORCH_LIBRARY(bke, m)
           "Tensor z) -> (Tensor, Tensor, Tensor, Tensor)");
     m.def("poly_filter(Tensor x, Tensor? dx, Tensor? ddx, Tensor? n, Tensor z, Tensor? g, Tensor? h, Tensor? k, Tensor? dt, "
           "Tensor? dt2, Tensor? hdt2, int family, int order, bool batch=False) -> (Tensor, Tensor, Tensor, Tensor, Tensor, Tensor)");
+    m.def("score_measurements(Tensor z, Tensor? x, Tensor? mean, Tensor? P, Tensor? S, Tensor? H, Tensor? R, Tensor? valid, "
+          "str[] outputs) -> Tensor[]");
     m.def("fls_smooth_batch(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor zs, int N) -> (Tensor, Tensor)");
     m.def("systematic_resample(Tensor weights, float u) -> Tensor");
     m.def("stratified_resample(Tensor weights, Tensor uniforms) -> Tensor");
@@ -599,6 +664,7 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("srkf_step", &srkf_step);
     m.impl("if_step", &if_step);
     m.impl("poly_filter", &poly_filter);
+    m.impl("score_measurements", &score_measurements);
     m.impl("fls_smooth_batch", &fls_smooth_batch);
     m.impl("systematic_resample", &systematic_resample);
     m.impl("stratified_resample", &stratified_resample);

@@ -723,6 +723,51 @@ typedef struct bke_poly_args {
 
 int bke_poly_filter(const bke_poly_args *args, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Measurement scoring: N tracks against K candidates each, without stepping anything.  Replaces, per pair:
+ *   stats.mahalanobis(z, mean, S)                 filterpy/stats/stats.py:64-109
+ *   stats.log_likelihood / likelihood(z, x, P, H, R)   stats.py:112-128 (S = H P H' + R)
+ *   stats.logpdf(z, mean, S)                      stats.py:131-154
+ *   stats.NEES(xs, est_xs, ps)                    stats.py:1138-1179 (d2 with z = xs, mean = est_xs, S = ps)
+ *   KalmanFilter.log_likelihood_of / residual_of / measurement_of_state   kalman_filter.py:1252-1260, 1175-1201
+ * Per track i, once:  zhat = H x (x when H is NULL), or the given mean;  S = H P H' + R (P + R when H is NULL),
+ * or the given S;  SI = S^-1 and log|det S| by the step kernels' inverse (a zero pivot of the partially pivoted
+ * elimination is a singular S).  Per pair (i, k), with z_ik at z + i * z_track_stride + k * z_cand_stride:
+ *   y = z_ik - zhat;  d2 = y' SI y;  mahalanobis = sqrt(d2);  log_likelihood = -0.5 (d2 + log|det S| + m log 2pi);
+ *   likelihood = exp(log_likelihood) (no floor, as stats.likelihood)
+ * A pair with z_valid == 0 is "z is None": y = d2 = mahalanobis = 0, log_likelihood = log(DBL_MIN)
+ * (kalman_filter.py:1258-1259, 515-520), whatever S is.  Where S is singular, status[i] = BKE_STATUS_SINGULAR_S and
+ * the track's valid pairs get NaN in d2, mahalanobis, log_likelihood and likelihood (y is still written).
+ * Inputs: exactly one of x[N,n] and mean[N,m]; at most one of P[N,n,n] (with R) and S; H and R with x or P only.
+ * H, R and S are per track (stride m*n, m*m) or shared (stride 0); z's strides are any element strides >= 0
+ * ([N,K,m]: K*m and m;  one scan [K,m] shared by every track: 0 and m).  dim_x is not read when neither x nor P
+ * is given.  Outputs (NULL = not wanted, at least one): zhat[N,m], y[N,K,m], d2, mahalanobis, log_likelihood,
+ * likelihood [N,K], status[N].  The covariance is needed by every output but zhat and y, z by every output but
+ * zhat and status.  N = 0 or K = 0 launches nothing (zhat and status are then not written either).  The call allocates
+ * nothing, so it can be captured.
+ * Kernels (DESIGN.md §3.5g): a CTA per tile of tracks computes each track's zhat, SI and log|det S| into shared
+ * memory (a register tile per thread for the shapes 1/1, 2/1, 2/2, 3/1, 3/3, 4/1, 4/2, 4/4 and 6/3, a warp per
+ * track otherwise), then sweeps the tile's N_tile * K pairs with its threads in pair order. */
+typedef struct bke_score_args {
+    int64_t n_tracks;                /* N */
+    int64_t n_candidates;            /* K */
+    int32_t dim_x, dim_z;            /* n, m */
+    int32_t dtype;
+    int32_t reserved;
+    const void *x;                   /* [N,n] or NULL */
+    const void *mean;                /* [N,m] or NULL */
+    const void *P;                   /* [N,n,n] or NULL */
+    const void *S; int64_t S_stride; /* [N,m,m] or NULL */
+    const void *H; int64_t H_stride; /* [N,m,n] or NULL = identity (n == m) */
+    const void *R; int64_t R_stride; /* [N,m,m]; with P only */
+    const void *z; int64_t z_track_stride, z_cand_stride;
+    const uint8_t *z_valid;          /* [N,K] or NULL */
+    void *zhat, *y, *d2, *mahalanobis, *log_likelihood, *likelihood;
+    int32_t *status;
+} bke_score_args;
+
+int bke_score_measurements(const bke_score_args *args, void *stream);
+
 /* Stand-alone pieces of the unscented path for callers that use them directly:
  *   MerweScaledSigmaPoints.sigma_points(x, P)   filterpy/kalman/sigma_points.py:124-177
  *       x[N,n], P[N,n,n] -> sigmas[N,2n+1,n]; status[N] = BKE_STATUS_NOT_PD where scipy's cholesky
