@@ -44,6 +44,7 @@ EXPORTED_SYMBOLS = [
     "bke_srkf_step", "bke_cholesky_lower",
     "bke_if_step", "bke_inverse",
     "bke_poly_filter",
+    "bke_imm_batch_filter",
     "bke_score_measurements",
     "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
     "bke_resample_bank", "bke_gather_rows_bank",
@@ -384,6 +385,32 @@ class MmArgs(ctypes.Structure):
     ]
 
 
+_MM = BKE_MM_MAX_MODELS
+
+
+class ImmBatchArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_tracks", c_int64),
+        ("dim_x", c_int32), ("dim_z", c_int32), ("n_models", c_int32), ("dtype", c_int32),
+        ("n_steps", c_int64),
+        ("flags", c_uint32), ("reserved", c_uint32),
+        ("x", c_void_p * _MM), ("P", c_void_p * _MM),
+        ("F", c_void_p * _MM), ("F_stride", c_int64 * _MM),
+        ("Q", c_void_p * _MM), ("Q_stride", c_int64 * _MM),
+        ("H", c_void_p * _MM), ("H_stride", c_int64 * _MM),
+        ("R", c_void_p * _MM), ("R_stride", c_int64 * _MM),
+        ("alpha_sq", ctypes.c_double * _MM),
+        ("S", c_void_p * _MM), ("log_likelihood", c_void_p * _MM),
+        ("K", c_void_p * _MM), ("y", c_void_p * _MM), ("SI", c_void_p * _MM),
+        ("x_prior", c_void_p * _MM), ("P_prior", c_void_p * _MM),
+        ("status", c_void_p * _MM),
+        ("mu", c_void_p), ("cbar", c_void_p), ("omega", c_void_p), ("trans", c_void_p),
+        ("zs", c_void_p), ("zs_valid", c_void_p),
+        ("means", c_void_p), ("covariances", c_void_p), ("means_p", c_void_p), ("covariances_p", c_void_p),
+        ("mus", c_void_p),
+    ]
+
+
 class BkeError(RuntimeError):
     pass
 
@@ -572,6 +599,8 @@ def load():
     lib.bke_kf_rts_smoother.restype = ctypes.c_int
     lib.bke_ukf_rts_smoother.argtypes = [ctypes.POINTER(UkfRtsArgs), c_void_p]
     lib.bke_ukf_rts_smoother.restype = ctypes.c_int
+    lib.bke_imm_batch_filter.argtypes = [ctypes.POINTER(ImmBatchArgs), c_void_p]
+    lib.bke_imm_batch_filter.restype = ctypes.c_int
     for name in ("bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate"):
         getattr(lib, name).argtypes = [ctypes.POINTER(MmArgs), c_void_p]
         getattr(lib, name).restype = ctypes.c_int

@@ -211,6 +211,82 @@ static int validate_poly(const bke_poly_args *a)
     return BKE_OK;
 }
 
+// the checks of bke_imm_batch_filter; -1 = go
+static int validate_imm(const bke_imm_batch_args *a)
+{
+    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    if (a->n_tracks < 0) { set_error("n_tracks < 0"); return BKE_ERR_BAD_ARG; }
+    if (a->n_steps < 0) { set_error("n_steps < 0"); return BKE_ERR_BAD_ARG; }
+    if (a->dim_x < 1 || a->dim_z < 1) { set_error("dim_x and dim_z must be 1 or greater"); return BKE_ERR_BAD_ARG; }
+    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (a->n_models < 2 || a->n_models > BKE_MM_MAX_MODELS) { set_error("n_models must be in [2, %d]", BKE_MM_MAX_MODELS); return BKE_ERR_BAD_ARG; }
+    if (a->flags & ~BKE_STATUS_STICKY) { set_error("flags may only hold BKE_STATUS_STICKY"); return BKE_ERR_BAD_ARG; }
+    const int M = a->n_models;
+    const int64_t N = a->n_tracks, T = a->n_steps, n = a->dim_x, m = a->dim_z;
+    auto bad_stride = [](int64_t s, int64_t full) { return s != 0 && s != full; };
+    for (int j = 0; j < M; j++) {
+        if (bad_stride(a->F_stride[j], n * n) || bad_stride(a->Q_stride[j], n * n) || bad_stride(a->H_stride[j], m * n) ||
+            bad_stride(a->R_stride[j], m * m)) {
+            set_error("model %d: strides must be 0 (shared) or the dense per-track size", j);
+            return BKE_ERR_BAD_ARG;
+        }
+    }
+    if (N == 0 || T == 0) return BKE_OK;
+    for (int j = 0; j < M; j++) {
+        if (!a->x[j] || !a->P[j] || !a->F[j] || !a->Q[j] || !a->H[j] || !a->R[j] || !a->S[j] || !a->log_likelihood[j] ||
+            !a->K[j] || !a->y[j] || !a->SI[j] || !a->x_prior[j] || !a->P_prior[j] || !a->status[j]) {
+            set_error("model %d: an array the call reads or writes is NULL", j);
+            return BKE_ERR_BAD_ARG;
+        }
+    }
+    if (!a->mu || !a->cbar || !a->omega || !a->trans || !a->zs || !a->means || !a->covariances || !a->means_p ||
+        !a->covariances_p || !a->mus) {
+        set_error("mu, cbar, omega, trans, zs and the five outputs must be non-NULL");
+        return BKE_ERR_BAD_ARG;
+    }
+    // every array the call writes must be clear of every other array it touches
+    struct Span { const void *p; int64_t bytes; bool written; };
+    const int64_t es = a->dtype == BKE_F32 ? 4 : 8;
+    Span sp[14 * BKE_MM_MAX_MODELS + 10];
+    int ns = 0;
+    auto add = [&](const void *p, int64_t elems, bool written) { sp[ns++] = Span{p, elems, written}; };
+    for (int j = 0; j < M; j++) {
+        add(a->x[j], N * n * es, true); add(a->P[j], N * n * n * es, true);
+        add(a->F[j], (a->F_stride[j] ? N : 1) * n * n * es, false); add(a->Q[j], (a->Q_stride[j] ? N : 1) * n * n * es, false);
+        add(a->H[j], (a->H_stride[j] ? N : 1) * m * n * es, false); add(a->R[j], (a->R_stride[j] ? N : 1) * m * m * es, false);
+        add(a->S[j], N * m * m * es, true); add(a->log_likelihood[j], N * es, true); add(a->K[j], N * n * m * es, true);
+        add(a->y[j], N * m * es, true); add(a->SI[j], N * m * m * es, true); add(a->x_prior[j], N * n * es, true);
+        add(a->P_prior[j], N * n * n * es, true); add(a->status[j], N * 4, true);
+    }
+    add(a->mu, N * M * 8, true); add(a->cbar, N * M * 8, true); add(a->omega, N * M * M * 8, true);
+    add(a->trans, (int64_t)M * M * 8, false); add(a->zs, T * N * m * es, false);
+    if (a->zs_valid) add(a->zs_valid, T * N, false);
+    add(a->means, T * N * n * es, true); add(a->covariances, T * N * n * n * es, true);
+    add(a->means_p, T * N * n * es, true); add(a->covariances_p, T * N * n * n * es, true);
+    add(a->mus, T * N * M * 8, true);
+    for (int i = 0; i < ns; i++) {
+        for (int k = i + 1; k < ns; k++) {
+            if (!sp[i].written && !sp[k].written) continue;
+            const uintptr_t p0 = (uintptr_t)sp[i].p, p1 = (uintptr_t)sp[k].p;
+            if (p0 < p1 + (uintptr_t)sp[k].bytes && p1 < p0 + (uintptr_t)sp[i].bytes) {
+                set_error("an array bke_imm_batch_filter writes overlaps another of its arrays");
+                return BKE_ERR_BAD_ARG;
+            }
+        }
+    }
+    if (!imm_batch_has_instance(a->dim_x, a->dim_z, a->dtype)) {
+        set_error("bke_imm_batch_filter: no fused instance for dim_x=%d, dim_z=%d in this dtype", a->dim_x, a->dim_z);
+        return BKE_ERR_UNSUPPORTED;
+    }
+    auto al16 = [](const void *p) { return ((uintptr_t)p & 15u) == 0; };
+    bool al = al16(a->means) && al16(a->covariances) && al16(a->means_p) && al16(a->covariances_p);
+    for (int j = 0; j < M; j++)
+        al = al && al16(a->x[j]) && al16(a->P[j]) && al16(a->S[j]) && al16(a->log_likelihood[j]) && al16(a->K[j]) &&
+             al16(a->y[j]) && al16(a->SI[j]) && al16(a->x_prior[j]) && al16(a->P_prior[j]);
+    if (!al) { set_error("bke_imm_batch_filter: the state, diagnostic and output arrays must be 16-byte aligned"); return BKE_ERR_UNSUPPORTED; }
+    return -1;
+}
+
 // the checks of bke_score_measurements
 static int validate_score(const bke_score_args *a)
 {
@@ -689,6 +765,15 @@ int bke_poly_filter(const bke_poly_args *args, void *stream)
     if ((rc = require_device())) return rc;
     if (args->n_filters == 0) return BKE_OK;
     return launch_poly(*args, (cudaStream_t)stream);
+}
+
+int bke_imm_batch_filter(const bke_imm_batch_args *args, void *stream)
+{
+    const int v = validate_imm(args);
+    if (v >= 0) return v;
+    int rc = require_device();
+    if (rc) return rc;
+    return launch_imm_batch(*args, (cudaStream_t)stream);
 }
 
 int bke_score_measurements(const bke_score_args *args, void *stream)

@@ -85,6 +85,9 @@ int launch_inverse(int64_t n_filters, int32_t k, int32_t dtype, const void *A, i
                    cudaStream_t s);
 int launch_poly(const bke_poly_args &a, cudaStream_t s);
 int launch_score(const bke_score_args &a, cudaStream_t s);
+// the (dim_x, dim_z, dtype) combinations bke_imm_batch_filter has a fused kernel for
+bool imm_batch_has_instance(int dim_x, int dim_z, int dtype);
+int launch_imm_batch(const bke_imm_batch_args &a, cudaStream_t s);
 #endif
 
 }  // namespace bke

@@ -12,7 +12,8 @@ import numpy as np
 import torch
 
 from .. import _lib
-from .._dev import StepGraph, bke_dtype, ptr, stream_ptr
+from .._dev import StepGraph, bke_dtype, ptr, stream_ptr, to_dev
+from ..common.helpers import reshape_z
 
 __all__ = ["IMMEstimator"]
 
@@ -40,6 +41,12 @@ def _mm_args(filters, flags=0):
         a.x[j], a.P[j] = ptr(f._x), ptr(f._P)
         a.log_likelihood[j] = ptr(f._ll)
     return a
+
+
+def _set_model_ptr(a, name, j, p, stride):
+    """model ``name``'s pointer and stride of model j in an ImmBatchArgs."""
+    getattr(a, name)[j] = p
+    getattr(a, name + "_stride")[j] = stride
 
 
 class IMMEstimator(object):
@@ -141,6 +148,96 @@ class IMMEstimator(object):
         a = _mm_args(self.filters, flags=_lib.BKE_MM_FROM_MU)
         a.mu, a.cbar, a.omega, a.trans = ptr(self._mu), ptr(self._cbar), ptr(self._omega), ptr(self._M)
         self._call(self._lib.bke_mm_probabilities, a)
+
+    def batch_filter(self, zs, valid=None):
+        """T epochs of ``predict(); update(zs[k], valid=valid[k])`` — the reference has no IMM batch_filter.
+
+        Bank mode: ``zs[T,N,dim_z]`` (``valid[T,N]`` optional, False = that track misses the epoch) -> device
+        tensors ``means[T,N,n] covariances[T,N,n,n] means_p covariances_p`` (the combined posterior and prior
+        of each epoch) and ``mus[T,N,M]`` (fp64, the mode probabilities after each update).  Single mode: ``zs``
+        is a sequence whose entries may be None; NumPy outputs ``(T,n) (T,n,n) (T,n) (T,n,n) (T,M)``.
+
+        The estimator and its model filters are left as the loop leaves them.  Shapes with a fused instance
+        (bke_imm_batch_filter: 2/1, 3/1 in fp32 and fp64, 4/2 in fp32) run in ONE launch; any other runs the
+        loop of separate launches.  Neither synchronises the host in bank mode, so a graph can capture it."""
+        fs = self.filters
+        f0 = fs[0]
+        N, n, m, nm = self.n_tracks, f0.dim_x, f0.dim_z, self.N
+        if any(f.dim_z != m for f in fs):
+            raise ValueError("batch_filter: every model must have the same dim_z")
+        T = zs.shape[0] if isinstance(zs, torch.Tensor) else (len(zs) if isinstance(zs, (list, tuple)) else np.size(zs, 0))
+        if self._single:
+            zarr = np.zeros((T, 1, m))
+            vmask = np.ones((T, 1), dtype=bool)
+            for i, z in enumerate(zs):
+                if z is None:
+                    vmask[i, 0] = False
+                else:
+                    zarr[i, 0] = np.asarray(z, dtype=np.float64).reshape(-1)[:m] if np.size(z) == m else reshape_z(z, m, 1)
+            zt = to_dev(zarr, self._dtype, self._device)
+            vt = None if vmask.all() else torch.from_numpy(vmask.astype(np.uint8)).to(self._device)
+        else:
+            zt = to_dev(zs, self._dtype, self._device)
+            if zt.dim() == 4 and zt.shape[-1] == 1:
+                zt = zt[..., 0].contiguous()
+            if tuple(zt.shape) != (T, N, m):
+                raise ValueError("zs must have shape (T,%d,%d), got %s" % (N, m, tuple(zt.shape)))
+            vt = None
+            if valid is not None:
+                vt = torch.as_tensor(valid, device=self._device).to(torch.uint8).contiguous()
+                if tuple(vt.shape) != (T, N):
+                    raise ValueError("valid must have shape (%d,%d)" % (T, N))
+        kw = dict(dtype=self._dtype, device=self._device)
+        means = torch.empty(T, N, n, **kw); means_p = torch.empty(T, N, n, **kw)
+        covs = torch.empty(T, N, n, n, **kw); covs_p = torch.empty(T, N, n, n, **kw)
+        mus = torch.empty(T, N, nm, dtype=torch.float64, device=self._device)
+        for f in fs:
+            f._flush()
+        a = _lib.ImmBatchArgs()
+        a.n_tracks, a.dim_x, a.dim_z, a.n_models, a.dtype = N, n, m, nm, bke_dtype(self._dtype)
+        a.n_steps = T
+        a.flags = _lib.BKE_STATUS_STICKY if self._single else 0
+        keep = []
+        for j, f in enumerate(fs):
+            a.x[j], a.P[j] = ptr(f._x), ptr(f._P)
+            for name in "FQHR":
+                t = getattr(f, "_" + name)
+                _set_model_ptr(a, name, j, ptr(t), f._stride(t))
+            a.alpha_sq[j] = f._alpha_sq
+            a.S[j], a.log_likelihood[j], a.K[j], a.y[j], a.SI[j] = ptr(f._S), ptr(f._ll), ptr(f._K), ptr(f._y), ptr(f._SI)
+            a.x_prior[j], a.P_prior[j], a.status[j] = ptr(f._x_prior), ptr(f._P_prior), ptr(f._status)
+        a.mu, a.cbar, a.omega, a.trans = ptr(self._mu), ptr(self._cbar), ptr(self._omega), ptr(self._M)
+        a.zs, a.zs_valid = ptr(zt), ptr(vt)
+        a.means, a.covariances, a.means_p, a.covariances_p, a.mus = ptr(means), ptr(covs), ptr(means_p), ptr(covs_p), ptr(mus)
+        with torch.cuda.device(self._device):
+            rc = self._lib.bke_imm_batch_filter(ctypes.byref(a), stream_ptr(self._device))
+        if rc == _lib.BKE_ERR_UNSUPPORTED:
+            # no fused instance for this shape / dtype: the same epochs on the separate launches
+            for k in range(T):
+                self.predict()
+                means_p[k].copy_(self._x); covs_p[k].copy_(self._P)
+                if self._single:
+                    self.update(zarr[k, 0] if vmask[k, 0] else None)
+                else:
+                    self.update(zt[k], valid=None if vt is None else vt[k])
+                means[k].copy_(self._x); covs[k].copy_(self._P); mus[k].copy_(self._mu)
+        else:
+            _lib.check(rc)
+            if T > 0:
+                self._x.copy_(means[T - 1]); self._P.copy_(covs[T - 1])
+                self._x_prior.copy_(means_p[T - 1]); self._P_prior.copy_(covs_p[T - 1])
+                self._x_post.copy_(means[T - 1]); self._P_post.copy_(covs[T - 1])
+                last = None if (self._single and not vmask[T - 1, 0]) else zt[T - 1]
+                for f in fs:
+                    f._post_alias = True
+                    f._z = last
+                if self._single:
+                    for f in fs:
+                        f.check()
+        if not self._single:
+            return means, covs, means_p, covs_p, mus
+        return (means[:, 0].cpu().numpy(), covs[:, 0].cpu().numpy(), means_p[:, 0].cpu().numpy(),
+                covs_p[:, 0].cpu().numpy(), mus[:, 0].cpu().numpy())
 
     def capture(self, fn, warmup=2):
         """Capture ``fn`` — a fixed sequence of ``predict()`` / ``update(z_buffer)`` calls — into a CUDA

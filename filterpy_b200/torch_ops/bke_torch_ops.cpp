@@ -14,6 +14,7 @@
 //                                                      update (T epochs) and the g-h batch_filter, gh_filter.py, least_squares.py, fading_memory.py
 //   bke::score_measurements   bke_score_measurements   stats.mahalanobis / log_likelihood / logpdf / NEES and
 //                                                      KalmanFilter.log_likelihood_of, N tracks x K candidates
+//   bke::imm_batch_filter     bke_imm_batch_filter     IMMEstimator.batch_filter: T epochs of predict(); update(z), IMM.py:160-247
 //   bke::fls_smooth_batch     bke_fls_smooth           FixedLagSmoother.smooth_batch, fixed_lag_smoother.py:217-311
 //   bke::systematic_resample  bke_systematic_resample  monte_carlo/resampling.py:117-150
 //   bke::stratified_resample  bke_stratified_resample  monte_carlo/resampling.py:80-114
@@ -411,6 +412,75 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tenso
     return std::make_tuple(x_out, or_empty(dx_out), or_empty(ddx_out), or_empty(n_out), results, or_empty(predictions));
 }
 
+// T epochs of IMMEstimator predict(); update(z) for N tracks of M models (bke_imm_batch_filter).  x[j], P[j], S[j],
+// log_likelihood[j] (model j's state, kept S and log-likelihood), mu and cbar are read and updated in place;
+// the models' K, y, SI, x_prior, P_prior, status and omega are not returned.  Returns (means, covariances, means_p,
+// covariances_p, mus).
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> imm_batch_filter(
+    at::TensorList x, at::TensorList P, at::TensorList F, at::TensorList Q, at::TensorList H, at::TensorList R,
+    at::ArrayRef<double> alpha_sq, at::TensorList S, at::TensorList log_likelihood, at::Tensor mu, at::Tensor cbar,
+    const at::Tensor &trans, const at::Tensor &zs, const c10::optional<at::Tensor> &zs_valid)
+{
+    const int64_t M = (int64_t)x.size();
+    TORCH_CHECK(M >= 2 && M <= BKE_MM_MAX_MODELS, "bke: 2 .. ", BKE_MM_MAX_MODELS, " models");
+    TORCH_CHECK((int64_t)P.size() == M && (int64_t)F.size() == M && (int64_t)Q.size() == M && (int64_t)H.size() == M &&
+                (int64_t)R.size() == M && (int64_t)alpha_sq.size() == M && (int64_t)S.size() == M &&
+                (int64_t)log_likelihood.size() == M, "bke: one x, P, F, Q, H, R, alpha_sq, S and log_likelihood per model");
+    const at::Tensor &x0 = x[0];
+    TORCH_CHECK(x0.is_cuda() && x0.dim() == 2, "bke: x[j] is a CUDA tensor [N, n]");
+    c10::cuda::CUDAGuard guard(x0.device());
+    const int64_t N = x0.size(0), n = x0.size(1);
+    TORCH_CHECK(zs.is_cuda() && zs.device() == x0.device() && zs.is_contiguous() && zs.scalar_type() == x0.scalar_type() &&
+                zs.dim() == 3 && zs.size(1) == N, "bke: zs is [T, N, m] in the state's dtype, on x's device");
+    const int64_t T = zs.size(0), m = zs.size(2);
+    auto same = [&](const at::Tensor &t, std::vector<int64_t> shape, at::ScalarType st, const char *name) {
+        TORCH_CHECK(t.is_cuda() && t.device() == x0.device() && t.is_contiguous() && t.scalar_type() == st &&
+                    t.sizes().vec() == shape, "bke: ", name, " must be a contiguous CUDA tensor ", at::IntArrayRef(shape),
+                    " of the right dtype, on x's device");
+    };
+    const auto dt = x0.scalar_type();
+    bke_imm_batch_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_tracks = N; a.dim_x = (int32_t)n; a.dim_z = (int32_t)m; a.n_models = (int32_t)M; a.dtype = dtype_of(x0); a.n_steps = T;
+    std::vector<at::Tensor> scratch;
+    auto opts = x0.options();
+    for (int64_t j = 0; j < M; j++) {
+        same(x[j], {N, n}, dt, "x[j]"); same(P[j], {N, n, n}, dt, "P[j]");
+        same(S[j], {N, m, m}, dt, "S[j]"); same(log_likelihood[j], {N}, dt, "log_likelihood[j]");
+        a.x[j] = x[j].data_ptr(); a.P[j] = P[j].data_ptr(); a.S[j] = S[j].data_ptr(); a.log_likelihood[j] = log_likelihood[j].data_ptr();
+        TORCH_CHECK(F[j].device() == x0.device() && Q[j].device() == x0.device() && H[j].device() == x0.device() &&
+                    R[j].device() == x0.device(), "bke: the models must be on x's device");
+        a.F[j] = model(F[j], N, n, n, &a.F_stride[j], x0, "F[j]");
+        a.Q[j] = model(Q[j], N, n, n, &a.Q_stride[j], x0, "Q[j]");
+        a.H[j] = model(H[j], N, m, n, &a.H_stride[j], x0, "H[j]");
+        a.R[j] = model(R[j], N, m, m, &a.R_stride[j], x0, "R[j]");
+        a.alpha_sq[j] = alpha_sq[j];
+        scratch.push_back(at::zeros({N, n, m}, opts)); a.K[j] = scratch.back().data_ptr();
+        scratch.push_back(at::zeros({N, m}, opts)); a.y[j] = scratch.back().data_ptr();
+        scratch.push_back(at::zeros({N, m, m}, opts)); a.SI[j] = scratch.back().data_ptr();
+        scratch.push_back(at::empty({N, n}, opts)); a.x_prior[j] = scratch.back().data_ptr();
+        scratch.push_back(at::empty({N, n, n}, opts)); a.P_prior[j] = scratch.back().data_ptr();
+        scratch.push_back(at::empty({N}, opts.dtype(at::kInt))); a.status[j] = scratch.back().data_ptr<int32_t>();
+    }
+    same(mu, {N, M}, at::kDouble, "mu"); same(cbar, {N, M}, at::kDouble, "cbar"); same(trans, {M, M}, at::kDouble, "trans");
+    at::Tensor omega = at::empty({N, M, M}, opts.dtype(at::kDouble));
+    a.mu = mu.data_ptr<double>(); a.cbar = cbar.data_ptr<double>(); a.omega = omega.data_ptr<double>(); a.trans = trans.data_ptr<double>();
+    a.zs = zs.data_ptr();
+    at::Tensor valid;
+    if (zs_valid.has_value() && zs_valid->defined()) {
+        TORCH_CHECK(zs_valid->device() == x0.device() && zs_valid->sizes() == at::IntArrayRef({T, N}), "bke: zs_valid is [T, N] on x's device");
+        valid = zs_valid->to(at::kByte).contiguous();
+        a.zs_valid = valid.data_ptr<uint8_t>();
+    }
+    at::Tensor means = at::empty({T, N, n}, opts), covs = at::empty({T, N, n, n}, opts);
+    at::Tensor means_p = at::empty({T, N, n}, opts), covs_p = at::empty({T, N, n, n}, opts);
+    at::Tensor mus = at::empty({T, N, M}, opts.dtype(at::kDouble));
+    a.means = means.data_ptr(); a.covariances = covs.data_ptr(); a.means_p = means_p.data_ptr();
+    a.covariances_p = covs_p.data_ptr(); a.mus = mus.data_ptr<double>();
+    check_rc(bke_imm_batch_filter(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_imm_batch_filter");
+    return std::make_tuple(means, covs, means_p, covs_p, mus);
+}
+
 // smooth_batch(zs, N) from (x, P): returns (xSmooth [T, N, n], xhat [T, N, n]); x and P are not changed
 std::tuple<at::Tensor, at::Tensor> fls_smooth_batch(const at::Tensor &x, const at::Tensor &P, const at::Tensor &F, const at::Tensor &H,
                                                     const at::Tensor &Q, const at::Tensor &R, const at::Tensor &zs, int64_t lag)
@@ -639,6 +709,9 @@ TORCH_LIBRARY(bke, m)
           "Tensor? dt2, Tensor? hdt2, int family, int order, bool batch=False) -> (Tensor, Tensor, Tensor, Tensor, Tensor, Tensor)");
     m.def("score_measurements(Tensor z, Tensor? x, Tensor? mean, Tensor? P, Tensor? S, Tensor? H, Tensor? R, Tensor? valid, "
           "str[] outputs) -> Tensor[]");
+    m.def("imm_batch_filter(Tensor(a!)[] x, Tensor(b!)[] P, Tensor[] F, Tensor[] Q, Tensor[] H, Tensor[] R, float[] alpha_sq, "
+          "Tensor(c!)[] S, Tensor(d!)[] log_likelihood, Tensor(e!) mu, Tensor(f!) cbar, Tensor trans, Tensor zs, "
+          "Tensor? zs_valid=None) -> (Tensor, Tensor, Tensor, Tensor, Tensor)");
     m.def("fls_smooth_batch(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor zs, int N) -> (Tensor, Tensor)");
     m.def("systematic_resample(Tensor weights, float u) -> Tensor");
     m.def("stratified_resample(Tensor weights, Tensor uniforms) -> Tensor");
@@ -665,6 +738,7 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("if_step", &if_step);
     m.impl("poly_filter", &poly_filter);
     m.impl("score_measurements", &score_measurements);
+    m.impl("imm_batch_filter", &imm_batch_filter);
     m.impl("fls_smooth_batch", &fls_smooth_batch);
     m.impl("systematic_resample", &systematic_resample);
     m.impl("stratified_resample", &stratified_resample);

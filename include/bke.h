@@ -1100,6 +1100,56 @@ int bke_mm_probabilities(const bke_mm_args *args, void *stream);
 int bke_mm_mix(const bke_mm_args *args, void *stream);
 int bke_mm_estimate(const bke_mm_args *args, void *stream);
 
+/* IMMEstimator.batch_filter: n_steps epochs of IMMEstimator.predict(); update(z) (filterpy/kalman/IMM.py:160-226)
+ * for N tracks of M = n_models linear Kalman filters, in ONE launch.  Per track and epoch:
+ *   mix (IMM.py:201-213, omega from mu and cbar) -> every model's predict (x = F x, P = alpha_sq[j] F P F' + Q)
+ *   -> combined prior (:228-237) -> every model's update with its log-likelihood -> mu, cbar, omega (:178-184,
+ *   :239-247, L = max(exp(ll), DBL_MIN)) -> combined posterior,
+ * with the formulas and the order of summation of bke_mm_* and bke_kf_step.  A track without a measurement
+ * (zs_valid[t,i] == 0) behaves as update(None): each model keeps its prior, y = 0, and its log-likelihood is
+ * log N(0; 0, S) of the S of its last real update (-inf where det S <= 0; S is 0 before the first).  A model
+ * whose S is singular keeps its prior and its previous log-likelihood; its S is still stored, and status is
+ * BKE_STATUS_SINGULAR_S for that epoch.
+ *   Per model j: x[j] [N,n], P[j] [N,n,n] (read, then the posterior of the last epoch), F/Q [N,n,n], H [N,m,n],
+ *   R [N,m,m] per track or shared (stride 0), alpha_sq[j], and the filter's diagnostics, read at the start
+ *   and written at the end as the loop leaves them: S[j] (the kept S), log_likelihood[j] [N], K[j] [N,n,m],
+ *   y[j] [N,m], SI[j] [N,m,m], x_prior[j] / P_prior[j] (the last epoch's predicted state, written only) and
+ *   status[j] [N] (int32, written only: the last epoch's, or with BKE_STATUS_STICKY the worst of the call's).
+ *   mu [N,M] and cbar [N,M] (fp64) are read and written; omega [N,M,M] (fp64) is written (it is derived from
+ *   mu and cbar); trans [M,M] (fp64).  zs [T,N,m], zs_valid [T,N] (uint8, NULL = every track measured).
+ *   Outputs: means [T,N,n], covariances [T,N,n,n] (combined posteriors), means_p, covariances_p (combined
+ *   priors), mus [T,N,M] (fp64, mu after each update).
+ * A bad size, stride, dtype, flag or model count (2 .. BKE_MM_MAX_MODELS), a NULL pointer the call reads or
+ * writes, or an output that overlaps another array is BKE_ERR_BAD_ARG; a shape without a fused instance
+ * ((n, m) other than 2/1, 3/1, 4/2, 6/3), or a state, diagnostic or output array that is not 16-byte aligned,
+ * is BKE_ERR_UNSUPPORTED (the caller then runs the separate launches).  Both before any device is touched.
+ * The call allocates nothing and can be captured in a graph. */
+typedef struct bke_imm_batch_args {
+    int64_t n_tracks;
+    int32_t dim_x, dim_z, n_models, dtype;
+    int64_t n_steps;
+    uint32_t flags;                                  /* 0 or BKE_STATUS_STICKY */
+    uint32_t reserved;
+    void *x[BKE_MM_MAX_MODELS], *P[BKE_MM_MAX_MODELS];
+    const void *F[BKE_MM_MAX_MODELS]; int64_t F_stride[BKE_MM_MAX_MODELS];
+    const void *Q[BKE_MM_MAX_MODELS]; int64_t Q_stride[BKE_MM_MAX_MODELS];
+    const void *H[BKE_MM_MAX_MODELS]; int64_t H_stride[BKE_MM_MAX_MODELS];
+    const void *R[BKE_MM_MAX_MODELS]; int64_t R_stride[BKE_MM_MAX_MODELS];
+    double alpha_sq[BKE_MM_MAX_MODELS];
+    void *S[BKE_MM_MAX_MODELS], *log_likelihood[BKE_MM_MAX_MODELS];
+    void *K[BKE_MM_MAX_MODELS], *y[BKE_MM_MAX_MODELS], *SI[BKE_MM_MAX_MODELS];
+    void *x_prior[BKE_MM_MAX_MODELS], *P_prior[BKE_MM_MAX_MODELS];
+    int32_t *status[BKE_MM_MAX_MODELS];
+    double *mu, *cbar, *omega;
+    const double *trans;
+    const void *zs;
+    const uint8_t *zs_valid;
+    void *means, *covariances, *means_p, *covariances_p;
+    double *mus;
+} bke_imm_batch_args;
+
+int bke_imm_batch_filter(const bke_imm_batch_args *args, void *stream);
+
 /* ---- the callers either side of a resample -----------------------------------------------------
  *
  * bke_cumsum_exact: cumsum_out[j] = np.cumsum(weights)[j] bit for bit (the strictly sequential fp64
