@@ -6,10 +6,12 @@ point reports no CUDA device, an exception is raised.
 """
 import ctypes
 import os
-from ctypes import c_double, c_int32, c_int64, c_size_t, c_uint32, c_uint64, c_void_p
+from ctypes import (POINTER, c_char_p, c_double, c_int, c_int32, c_int64, c_size_t, c_uint32, c_uint64,
+                    c_void_p)
 
 from . import _build
 
+BKE_ABI_VERSION = 1
 BKE_F32, BKE_F64 = 0, 1
 BKE_OK, BKE_ERR_BAD_ARG, BKE_ERR_UNSUPPORTED, BKE_ERR_CUDA = 0, 1, 2, 3
 BKE_STATUS_OK, BKE_STATUS_SINGULAR_S, BKE_STATUS_NOT_PD = 0, 1, 2
@@ -21,41 +23,6 @@ BKE_HX_LINEAR, BKE_HX_RANGE_AZ_EL, BKE_HX_RANGE_BEARING = 0, 1, 2
 BKE_FX_USER = BKE_HX_USER = 100
 # the UKF / CKF hooks compiled from source text (bke_ukf_model_compile_hooks)
 BKE_HOOK_X_MEAN, BKE_HOOK_Z_MEAN, BKE_HOOK_RESIDUAL_X, BKE_HOOK_RESIDUAL_Z, BKE_HOOK_STATE_ADD = 1, 2, 4, 8, 16
-
-# every symbol include/bke.h declares (tests check that the library exports all of them)
-EXPORTED_SYMBOLS = [
-    "bke_abi_version", "bke_last_error", "bke_device_count",
-    "bke_kf_step", "bke_kf_step_correlated", "bke_kf_update_rows", "bke_kf_batch_filter", "bke_ukf_step",
-    "bke_fls_workspace_bytes", "bke_fls_smooth",
-    "bke_kf_sym_models_bytes", "bke_kf_pack_sym_models", "bke_kf_step_sym",
-    "bke_kf_scan_models", "bke_kf_packed_models_bytes", "bke_kf_pack_models", "bke_kf_step_packed",
-    "bke_kf_steps_packed", "bke_capture_node_count",
-    "bke_resample_workspace_bytes", "bke_systematic_resample", "bke_stratified_resample",
-    "bke_weights_sum", "bke_weights_scale", "bke_resample_shard", "bke_resample_normalized",
-    "bke_resample_composite_bytes", "bke_resample_shard_compose", "bke_resample_compose_carry", "bke_resample_shard_stage",
-    "bke_merwe_sigma_points", "bke_simplex_sigma_points", "bke_unscented_transform",
-    "bke_ukf_model_compile_points", "bke_debug_ukf_model_points_cubin_bytes",
-    "bke_ukf_model_compile", "bke_ukf_model_log", "bke_ukf_model_registers", "bke_ukf_model_free", "bke_ukf_step_model",
-    "bke_debug_ukf_model_cubin_bytes", "bke_ukf_rts_smoother_model",
-    "bke_ckf_step", "bke_ckf_model_compile", "bke_ckf_step_model", "bke_debug_ckf_model_cubin_bytes",
-    "bke_ukf_model_compile_hooks", "bke_debug_ukf_model_hooks_cubin_bytes",
-    "bke_ckf_model_compile_hooks", "bke_debug_ckf_model_hooks_cubin_bytes",
-    "bke_enkf_initialize", "bke_enkf_step", "bke_enkf_model_compile", "bke_enkf_step_model", "bke_debug_enkf_model_cubin_bytes",
-    "bke_srkf_step", "bke_cholesky_lower",
-    "bke_if_step", "bke_inverse",
-    "bke_poly_filter",
-    "bke_imm_batch_filter",
-    "bke_score_measurements",
-    "bke_kf_rts_smoother", "bke_ukf_rts_smoother", "bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate", "bke_cumsum_exact", "bke_searchsorted", "bke_multinomial_resample", "bke_gather_rows",
-    "bke_resample_bank", "bke_gather_rows_bank",
-    "bke_multinomial_resample_bank_workspace_bytes", "bke_multinomial_resample_bank",
-    "bke_residual_resample_bank_workspace_bytes", "bke_residual_resample_bank_prepare",
-    "bke_residual_resample_bank_search",
-    "bke_resample_bank_gated_workspace_bytes", "bke_resample_bank_gated", "bke_resample_bank_gated_stats",
-    "bke_resample_bank_gated_apply",
-    "bke_residual_workspace_bytes", "bke_residual_prepare", "bke_searchsorted_bracket_sweep",
-]
-
 
 class KfArgs(ctypes.Structure):
     _fields_ = [
@@ -411,6 +378,119 @@ class ImmBatchArgs(ctypes.Structure):
     ]
 
 
+_MODEL = [c_int32] * 5        # dim_x, dim_z, dtype, fx_model, hx_model of the run-time compiled models
+
+# Every prototype of include/bke.h, in header order: symbol -> (restype, argtypes).  A struct pointer is typed
+# POINTER(its Structure) except where the caller passes device memory (bke_kf_scan_models' map).
+_SIGNATURES = {
+    "bke_abi_version": (c_int, []),
+    "bke_last_error": (c_char_p, []),
+    "bke_device_count": (c_int, []),
+    "bke_kf_step": (c_int, [POINTER(KfArgs), c_void_p]),
+    "bke_kf_step_correlated": (c_int, [POINTER(KfArgs), c_void_p, c_int64, c_void_p]),
+    "bke_kf_update_rows": (c_int, [POINTER(KfRowsArgs), c_void_p]),
+    "bke_kf_sym_models_bytes": (c_size_t, [c_int64]),
+    "bke_kf_pack_sym_models": (c_int, [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p]),
+    "bke_kf_step_sym": (c_int, [POINTER(KfArgs), c_void_p, c_void_p]),
+    "bke_kf_scan_models": (c_int, [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_void_p]),
+    "bke_kf_packed_models_bytes": (c_size_t, [c_int64, c_uint64]),
+    "bke_kf_pack_models": (c_int, [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_uint64, c_void_p, c_void_p]),
+    "bke_kf_step_packed": (c_int, [POINTER(KfArgs), c_void_p, POINTER(KfModelMap), c_void_p]),
+    "bke_kf_steps_packed": (c_int, [POINTER(KfArgs), c_void_p, POINTER(KfModelMap), POINTER(c_void_p), c_int32,
+                                    c_void_p]),
+    "bke_capture_node_count": (c_int, [c_void_p, POINTER(c_int64)]),
+    "bke_kf_batch_filter": (c_int, [POINTER(KfBatchArgs), c_void_p]),
+    "bke_fls_workspace_bytes": (c_size_t, [c_int64, c_int32, c_int32, c_int32, c_int32, c_int64]),
+    "bke_fls_smooth": (c_int, [POINTER(FlsArgs), c_void_p]),
+    "bke_ukf_step": (c_int, [POINTER(UkfArgs), c_void_p]),
+    "bke_ukf_model_compile": (c_int, _MODEL + [c_char_p, c_char_p, POINTER(c_void_p)]),
+    "bke_ukf_model_log": (c_char_p, [c_void_p]),
+    "bke_ukf_model_registers": (c_int, [c_void_p, c_int32]),
+    "bke_ukf_model_free": (None, [c_void_p]),
+    "bke_ukf_step_model": (c_int, [POINTER(UkfArgs), c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
+    "bke_debug_ukf_model_cubin_bytes": (c_size_t, _MODEL + [c_char_p, c_char_p]),
+    "bke_ukf_model_compile_hooks": (c_int, _MODEL + [c_uint32, c_char_p, c_char_p, POINTER(c_void_p)]),
+    "bke_debug_ukf_model_hooks_cubin_bytes": (c_size_t, _MODEL + [c_uint32, c_char_p, c_char_p]),
+    "bke_ukf_model_compile_points": (c_int, _MODEL + [c_uint32, c_uint32, c_char_p, c_char_p, POINTER(c_void_p)]),
+    "bke_debug_ukf_model_points_cubin_bytes": (c_size_t, _MODEL + [c_uint32, c_uint32, c_char_p, c_char_p]),
+    "bke_ckf_step": (c_int, [POINTER(CkfArgs), c_void_p]),
+    "bke_ckf_model_compile": (c_int, _MODEL + [c_char_p, c_char_p, POINTER(c_void_p)]),
+    "bke_ckf_step_model": (c_int, [POINTER(CkfArgs), c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
+    "bke_debug_ckf_model_cubin_bytes": (c_size_t, _MODEL + [c_char_p, c_char_p]),
+    "bke_ckf_model_compile_hooks": (c_int, _MODEL + [c_uint32, c_char_p, c_char_p, POINTER(c_void_p)]),
+    "bke_debug_ckf_model_hooks_cubin_bytes": (c_size_t, _MODEL + [c_uint32, c_char_p, c_char_p]),
+    "bke_enkf_initialize": (c_int, [c_int64, c_int32, c_int32, c_int32, c_uint32, c_uint32, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_void_p]),
+    "bke_enkf_step": (c_int, [POINTER(EnkfArgs), c_void_p]),
+    "bke_enkf_model_compile": (c_int, _MODEL + [c_char_p, c_char_p, POINTER(c_void_p)]),
+    "bke_enkf_step_model": (c_int, [POINTER(EnkfArgs), c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
+    "bke_debug_enkf_model_cubin_bytes": (c_size_t, _MODEL + [c_char_p, c_char_p]),
+    "bke_srkf_step": (c_int, [POINTER(SrkfArgs), c_void_p]),
+    "bke_cholesky_lower": (c_int, [c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "bke_if_step": (c_int, [POINTER(IfArgs), c_void_p]),
+    "bke_inverse": (c_int, [c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "bke_poly_filter": (c_int, [POINTER(PolyArgs), c_void_p]),
+    "bke_score_measurements": (c_int, [POINTER(ScoreArgs), c_void_p]),
+    "bke_merwe_sigma_points": (c_int, [c_int64, c_int32, c_int32, c_double, c_double, c_double, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_void_p]),
+    "bke_simplex_sigma_points": (c_int, [c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                         c_void_p]),
+    "bke_unscented_transform": (c_int, [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_int64, c_void_p, c_void_p, c_void_p]),
+    "bke_resample_workspace_bytes": (c_size_t, [c_int64]),
+    "bke_systematic_resample": (c_int, [c_int64, c_void_p, c_double, c_void_p, c_void_p, c_size_t, c_void_p,
+                                        c_void_p, c_void_p]),
+    "bke_stratified_resample": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p,
+                                        c_void_p, c_void_p]),
+    "bke_resample_normalized": (c_int, [c_int64, c_void_p, c_double, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
+    "bke_resample_shard": (c_int, [POINTER(ResampleShardArgs), c_void_p]),
+    "bke_resample_composite_bytes": (c_size_t, []),
+    "bke_resample_shard_stage": (c_int, [POINTER(ResampleShardArgs), POINTER(ResampleShardExt), c_int32,
+                                         c_void_p]),
+    "bke_resample_shard_compose": (c_int, [POINTER(ResampleShardArgs), c_void_p, c_void_p]),
+    "bke_resample_compose_carry": (c_int, [c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "bke_resample_bank": (c_int, [POINTER(ResampleBankArgs), c_void_p]),
+    "bke_resample_bank_gated_workspace_bytes": (c_size_t, [c_int64]),
+    "bke_resample_bank_gated": (c_int, [POINTER(ResampleBankGatedArgs), c_void_p]),
+    "bke_resample_bank_gated_stats": (c_int, [POINTER(ResampleBankGatedArgs), c_void_p]),
+    "bke_resample_bank_gated_apply": (c_int, [POINTER(ResampleBankGatedArgs), c_void_p]),
+    "bke_multinomial_resample_bank_workspace_bytes": (c_size_t, [c_int64, c_int64]),
+    "bke_multinomial_resample_bank": (c_int, [POINTER(MultinomialResampleBankArgs), c_void_p]),
+    "bke_residual_resample_bank_workspace_bytes": (c_size_t, [c_int64, c_int64]),
+    "bke_residual_resample_bank_prepare": (c_int, [POINTER(ResidualResampleBankArgs), c_void_p]),
+    "bke_residual_resample_bank_search": (c_int, [POINTER(ResidualResampleBankArgs), c_void_p]),
+    "bke_weights_sum": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "bke_weights_scale": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "bke_kf_rts_smoother": (c_int, [POINTER(RtsArgs), c_void_p]),
+    "bke_ukf_rts_smoother": (c_int, [POINTER(UkfRtsArgs), c_void_p]),
+    "bke_ukf_rts_smoother_model": (c_int, [POINTER(UkfRtsArgs), c_void_p, c_void_p, c_int64, c_void_p]),
+    "bke_mm_probabilities": (c_int, [POINTER(MmArgs), c_void_p]),
+    "bke_mm_mix": (c_int, [POINTER(MmArgs), c_void_p]),
+    "bke_mm_estimate": (c_int, [POINTER(MmArgs), c_void_p]),
+    "bke_imm_batch_filter": (c_int, [POINTER(ImmBatchArgs), c_void_p]),
+    "bke_cumsum_exact": (c_int, [c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "bke_searchsorted": (c_int, [c_int64, c_void_p, c_int64, c_void_p, c_int32, c_void_p, c_void_p]),
+    "bke_multinomial_resample": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                         c_size_t, c_void_p, c_void_p]),
+    "bke_gather_rows": (c_int, [c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                                c_void_p]),
+    "bke_gather_rows_bank": (c_int, [c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                                     c_void_p]),
+    "bke_residual_workspace_bytes": (c_size_t, [c_int64]),
+    "bke_residual_prepare": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                     c_void_p]),
+    "bke_searchsorted_bracket_sweep": (c_int, [c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                               c_void_p, c_void_p]),
+}
+
+# every symbol include/bke.h declares (build() and the tests check that the library exports all of them)
+EXPORTED_SYMBOLS = list(_SIGNATURES)
+
+
 class BkeError(RuntimeError):
     pass
 
@@ -452,195 +532,19 @@ def load():
         if not os.path.exists(path):
             raise BkeError("BKE_LIB_PATH=%s does not exist" % path)
     else:
-      try:
-        if _build.needs_build():
-            _build.build()
-      except Exception as e:  # stale or missing and not buildable
-        if not os.path.exists(path):
-            raise BkeError("libbke.so is missing and could not be built (%s); the engine has no "
-                           "CPU fallback" % e)
+        try:
+            if _build.needs_build():
+                _build.build()
+        except Exception as e:  # stale or missing and not buildable
+            if not os.path.exists(path):
+                raise BkeError("libbke.so is missing and could not be built (%s); the engine has no "
+                               "CPU fallback" % e)
     _point_at_nvrtc()
     lib = ctypes.CDLL(path)
-    lib.bke_abi_version.restype = ctypes.c_int
-    lib.bke_last_error.restype = ctypes.c_char_p
-    lib.bke_device_count.restype = ctypes.c_int
-    lib.bke_kf_step.argtypes = [ctypes.POINTER(KfArgs), c_void_p]
-    lib.bke_kf_step.restype = ctypes.c_int
-    lib.bke_kf_step_correlated.argtypes = [ctypes.POINTER(KfArgs), c_void_p, c_int64, c_void_p]
-    lib.bke_kf_step_correlated.restype = ctypes.c_int
-    lib.bke_kf_update_rows.argtypes = [ctypes.POINTER(KfRowsArgs), c_void_p]
-    lib.bke_kf_update_rows.restype = ctypes.c_int
-    lib.bke_kf_sym_models_bytes.argtypes = [c_int64]
-    lib.bke_kf_sym_models_bytes.restype = c_size_t
-    lib.bke_kf_pack_sym_models.argtypes = [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
-                                           c_void_p]
-    lib.bke_kf_pack_sym_models.restype = ctypes.c_int
-    lib.bke_kf_step_sym.argtypes = [ctypes.POINTER(KfArgs), c_void_p, c_void_p]
-    lib.bke_kf_step_sym.restype = ctypes.c_int
-    lib.bke_kf_scan_models.argtypes = [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
-                                       c_void_p, c_void_p]
-    lib.bke_kf_scan_models.restype = ctypes.c_int
-    lib.bke_kf_packed_models_bytes.argtypes = [c_int64, c_uint64]
-    lib.bke_kf_packed_models_bytes.restype = c_size_t
-    lib.bke_kf_pack_models.argtypes = [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
-                                       c_uint64, c_void_p, c_void_p]
-    lib.bke_kf_pack_models.restype = ctypes.c_int
-    lib.bke_kf_step_packed.argtypes = [ctypes.POINTER(KfArgs), c_void_p, ctypes.POINTER(KfModelMap), c_void_p]
-    lib.bke_kf_step_packed.restype = ctypes.c_int
-    lib.bke_kf_steps_packed.argtypes = [ctypes.POINTER(KfArgs), c_void_p, ctypes.POINTER(KfModelMap),
-                                        ctypes.POINTER(c_void_p), c_int32, c_void_p]
-    lib.bke_kf_steps_packed.restype = ctypes.c_int
-    lib.bke_capture_node_count.argtypes = [c_void_p, ctypes.POINTER(c_int64)]
-    lib.bke_capture_node_count.restype = ctypes.c_int
-    lib.bke_kf_batch_filter.argtypes = [ctypes.POINTER(KfBatchArgs), c_void_p]
-    lib.bke_kf_batch_filter.restype = ctypes.c_int
-    lib.bke_fls_workspace_bytes.argtypes = [c_int64, c_int32, c_int32, c_int32, c_int32, c_int64]
-    lib.bke_fls_workspace_bytes.restype = c_size_t
-    lib.bke_fls_smooth.argtypes = [ctypes.POINTER(FlsArgs), c_void_p]
-    lib.bke_fls_smooth.restype = ctypes.c_int
-    lib.bke_ukf_step.argtypes = [ctypes.POINTER(UkfArgs), c_void_p]
-    lib.bke_ukf_step.restype = ctypes.c_int
-    lib.bke_ukf_model_compile.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p,
-                                          ctypes.POINTER(c_void_p)]
-    lib.bke_ukf_model_compile.restype = ctypes.c_int
-    lib.bke_ukf_model_log.argtypes = [c_void_p]
-    lib.bke_ukf_model_log.restype = ctypes.c_char_p
-    lib.bke_ukf_model_registers.argtypes = [c_void_p, c_int32]
-    lib.bke_ukf_model_registers.restype = ctypes.c_int
-    lib.bke_ukf_model_free.argtypes = [c_void_p]
-    lib.bke_ukf_model_free.restype = None
-    lib.bke_ukf_step_model.argtypes = [ctypes.POINTER(UkfArgs), c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]
-    lib.bke_ukf_step_model.restype = ctypes.c_int
-    lib.bke_ukf_rts_smoother_model.argtypes = [ctypes.POINTER(UkfRtsArgs), c_void_p, c_void_p, c_int64, c_void_p]
-    lib.bke_ukf_rts_smoother_model.restype = ctypes.c_int
-    lib.bke_debug_ukf_model_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p]
-    lib.bke_debug_ukf_model_cubin_bytes.restype = c_size_t
-    lib.bke_ukf_model_compile_points.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_uint32, c_uint32,
-                                                 ctypes.c_char_p, ctypes.c_char_p, ctypes.POINTER(c_void_p)]
-    lib.bke_ukf_model_compile_points.restype = ctypes.c_int
-    lib.bke_debug_ukf_model_points_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_uint32, c_uint32,
-                                                           ctypes.c_char_p, ctypes.c_char_p]
-    lib.bke_debug_ukf_model_points_cubin_bytes.restype = c_size_t
-    for fam in ("ukf", "ckf"):
-        f = getattr(lib, "bke_%s_model_compile_hooks" % fam)
-        f.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_uint32, ctypes.c_char_p, ctypes.c_char_p,
-                      ctypes.POINTER(c_void_p)]
-        f.restype = ctypes.c_int
-        f = getattr(lib, "bke_debug_%s_model_hooks_cubin_bytes" % fam)
-        f.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_uint32, ctypes.c_char_p, ctypes.c_char_p]
-        f.restype = c_size_t
-    lib.bke_ckf_step.argtypes = [ctypes.POINTER(CkfArgs), c_void_p]
-    lib.bke_ckf_step.restype = ctypes.c_int
-    lib.bke_ckf_model_compile.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p,
-                                          ctypes.POINTER(c_void_p)]
-    lib.bke_ckf_model_compile.restype = ctypes.c_int
-    lib.bke_ckf_step_model.argtypes = [ctypes.POINTER(CkfArgs), c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]
-    lib.bke_ckf_step_model.restype = ctypes.c_int
-    lib.bke_debug_ckf_model_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p]
-    lib.bke_debug_ckf_model_cubin_bytes.restype = c_size_t
-    lib.bke_enkf_initialize.argtypes = [c_int64, c_int32, c_int32, c_int32, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p,
-                                        c_void_p, c_void_p]
-    lib.bke_enkf_initialize.restype = ctypes.c_int
-    lib.bke_enkf_step.argtypes = [ctypes.POINTER(EnkfArgs), c_void_p]
-    lib.bke_enkf_step.restype = ctypes.c_int
-    lib.bke_enkf_model_compile.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p,
-                                           ctypes.POINTER(c_void_p)]
-    lib.bke_enkf_model_compile.restype = ctypes.c_int
-    lib.bke_enkf_step_model.argtypes = [ctypes.POINTER(EnkfArgs), c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]
-    lib.bke_enkf_step_model.restype = ctypes.c_int
-    lib.bke_debug_enkf_model_cubin_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, ctypes.c_char_p, ctypes.c_char_p]
-    lib.bke_debug_enkf_model_cubin_bytes.restype = c_size_t
-    lib.bke_srkf_step.argtypes = [ctypes.POINTER(SrkfArgs), c_void_p]
-    lib.bke_srkf_step.restype = ctypes.c_int
-    lib.bke_cholesky_lower.argtypes = [c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
-    lib.bke_cholesky_lower.restype = ctypes.c_int
-    lib.bke_if_step.argtypes = [ctypes.POINTER(IfArgs), c_void_p]
-    lib.bke_if_step.restype = ctypes.c_int
-    lib.bke_inverse.argtypes = [c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
-    lib.bke_inverse.restype = ctypes.c_int
-    lib.bke_poly_filter.argtypes = [ctypes.POINTER(PolyArgs), c_void_p]
-    lib.bke_poly_filter.restype = ctypes.c_int
-    lib.bke_score_measurements.argtypes = [ctypes.POINTER(ScoreArgs), c_void_p]
-    lib.bke_score_measurements.restype = ctypes.c_int
-    lib.bke_resample_workspace_bytes.argtypes = [c_int64]
-    lib.bke_resample_workspace_bytes.restype = c_size_t
-    lib.bke_systematic_resample.argtypes = [c_int64, c_void_p, c_double, c_void_p, c_void_p, c_size_t,
-                                            c_void_p, c_void_p, c_void_p]
-    lib.bke_systematic_resample.restype = ctypes.c_int
-    lib.bke_stratified_resample.argtypes = [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
-                                            c_void_p, c_void_p, c_void_p]
-    lib.bke_stratified_resample.restype = ctypes.c_int
-    lib.bke_resample_normalized.argtypes = [c_int64, c_void_p, c_double, c_void_p, c_void_p, c_void_p, c_void_p,
-                                            c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]
-    lib.bke_resample_normalized.restype = ctypes.c_int
-    lib.bke_weights_sum.argtypes = [c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]
-    lib.bke_weights_sum.restype = ctypes.c_int
-    lib.bke_weights_scale.argtypes = [c_int64, c_void_p, c_void_p, c_void_p, c_void_p]
-    lib.bke_weights_scale.restype = ctypes.c_int
-    lib.bke_resample_composite_bytes.argtypes = []
-    lib.bke_resample_composite_bytes.restype = c_size_t
-    lib.bke_resample_shard_compose.argtypes = [ctypes.POINTER(ResampleShardArgs), c_void_p, c_void_p]
-    lib.bke_resample_shard_compose.restype = ctypes.c_int
-    lib.bke_resample_compose_carry.argtypes = [c_int32, c_void_p, c_void_p, c_void_p, c_void_p]
-    lib.bke_resample_compose_carry.restype = ctypes.c_int
-    lib.bke_resample_shard_stage.argtypes = [ctypes.POINTER(ResampleShardArgs), ctypes.POINTER(ResampleShardExt), c_int32, c_void_p]
-    lib.bke_resample_shard_stage.restype = ctypes.c_int
-    lib.bke_resample_shard.argtypes = [ctypes.POINTER(ResampleShardArgs), c_void_p]
-    lib.bke_resample_shard.restype = ctypes.c_int
-    lib.bke_merwe_sigma_points.argtypes = [c_int64, c_int32, c_int32, c_double, c_double, c_double,
-                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
-    lib.bke_merwe_sigma_points.restype = ctypes.c_int
-    lib.bke_simplex_sigma_points.argtypes = [c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
-    lib.bke_simplex_sigma_points.restype = ctypes.c_int
-    lib.bke_unscented_transform.argtypes = [c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
-                                            c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
-    lib.bke_unscented_transform.restype = ctypes.c_int
-    lib.bke_kf_rts_smoother.argtypes = [ctypes.POINTER(RtsArgs), c_void_p]
-    lib.bke_kf_rts_smoother.restype = ctypes.c_int
-    lib.bke_ukf_rts_smoother.argtypes = [ctypes.POINTER(UkfRtsArgs), c_void_p]
-    lib.bke_ukf_rts_smoother.restype = ctypes.c_int
-    lib.bke_imm_batch_filter.argtypes = [ctypes.POINTER(ImmBatchArgs), c_void_p]
-    lib.bke_imm_batch_filter.restype = ctypes.c_int
-    for name in ("bke_mm_probabilities", "bke_mm_mix", "bke_mm_estimate"):
-        getattr(lib, name).argtypes = [ctypes.POINTER(MmArgs), c_void_p]
-        getattr(lib, name).restype = ctypes.c_int
-    lib.bke_cumsum_exact.argtypes = [c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_size_t, c_void_p, c_void_p]
-    lib.bke_cumsum_exact.restype = ctypes.c_int
-    lib.bke_searchsorted.argtypes = [c_int64, c_void_p, c_int64, c_void_p, c_int32, c_void_p, c_void_p]
-    lib.bke_searchsorted.restype = ctypes.c_int
-    lib.bke_multinomial_resample.argtypes = [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                             c_size_t, c_void_p, c_void_p]
-    lib.bke_multinomial_resample.restype = ctypes.c_int
-    lib.bke_gather_rows.argtypes = [c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
-                                    c_void_p]
-    lib.bke_gather_rows.restype = ctypes.c_int
-    lib.bke_gather_rows_bank.argtypes = [c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
-                                         c_void_p]
-    lib.bke_gather_rows_bank.restype = ctypes.c_int
-    lib.bke_resample_bank.argtypes = [ctypes.POINTER(ResampleBankArgs), c_void_p]
-    lib.bke_resample_bank.restype = ctypes.c_int
-    for name in ("bke_multinomial_resample_bank_workspace_bytes", "bke_residual_resample_bank_workspace_bytes"):
-        getattr(lib, name).argtypes = [c_int64, c_int64]
-        getattr(lib, name).restype = c_size_t
-    lib.bke_multinomial_resample_bank.argtypes = [ctypes.POINTER(MultinomialResampleBankArgs), c_void_p]
-    lib.bke_multinomial_resample_bank.restype = ctypes.c_int
-    lib.bke_resample_bank_gated_workspace_bytes.argtypes = [c_int64]
-    lib.bke_resample_bank_gated_workspace_bytes.restype = c_size_t
-    for name in ("bke_resample_bank_gated", "bke_resample_bank_gated_stats", "bke_resample_bank_gated_apply"):
-        getattr(lib, name).argtypes = [ctypes.POINTER(ResampleBankGatedArgs), c_void_p]
-        getattr(lib, name).restype = ctypes.c_int
-    for name in ("bke_residual_resample_bank_prepare", "bke_residual_resample_bank_search"):
-        getattr(lib, name).argtypes = [ctypes.POINTER(ResidualResampleBankArgs), c_void_p]
-        getattr(lib, name).restype = ctypes.c_int
-    lib.bke_residual_workspace_bytes.argtypes = [c_int64]
-    lib.bke_residual_workspace_bytes.restype = c_size_t
-    lib.bke_residual_prepare.argtypes = [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
-                                         c_void_p]
-    lib.bke_residual_prepare.restype = ctypes.c_int
-    lib.bke_searchsorted_bracket_sweep.argtypes = [c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                   c_void_p, c_void_p]
-    lib.bke_searchsorted_bracket_sweep.restype = ctypes.c_int
-    if lib.bke_abi_version() != 1:
+    for name, (restype, argtypes) in _SIGNATURES.items():
+        f = getattr(lib, name)
+        f.restype, f.argtypes = restype, argtypes
+    if lib.bke_abi_version() != BKE_ABI_VERSION:
         raise BkeError("libbke.so ABI version mismatch")
     _lib = lib
     return lib

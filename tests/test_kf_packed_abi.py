@@ -1,34 +1,10 @@
-"""The C-ABI of the packed model words of the 4/2 fp32 step: the map's layout, the record's size and
-the argument checks, without a GPU."""
-import ctypes
-import os
-import subprocess
-
+"""The C-ABI of the packed model words of the 4/2 fp32 step: the record's size and the argument
+checks, without a GPU."""
 from filterpy_b200 import _lib
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def test_map_layout_matches_header(tmp_path):
-    fields = [f for f, _ in _lib.KfModelMap._fields_]
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "bke.h"', 'int main(void) {',
-             'printf("sizeof %zu\\n", sizeof(bke_kf_model_map));',
-             'printf("words_len %zu\\n", sizeof(((bke_kf_model_map *)0)->words) / sizeof(float));',
-             'printf("BKE_KF42_MODEL_WORDS %d\\n", BKE_KF42_MODEL_WORDS);']
-    lines += ['printf("%s %%zu\\n", offsetof(bke_kf_model_map, %s));' % (f, f) for f in fields]
-    lines += ['return 0; }']
-    src = tmp_path / "probe.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "probe"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    got = dict(ln.split() for ln in subprocess.check_output([str(exe)]).decode().split("\n") if ln.strip())
-    assert int(got.pop("sizeof")) == ctypes.sizeof(_lib.KfModelMap)
-    assert int(got.pop("words_len")) == int(got.pop("BKE_KF42_MODEL_WORDS")) == _lib.BKE_KF42_MODEL_WORDS == 37
-    for f in fields:
-        assert int(got[f]) == getattr(_lib.KfModelMap, f).offset, f
 
 
 def test_record_size_is_whole_tiles_of_the_varying_planes():
+    assert _lib.BKE_KF42_MODEL_WORDS == 37
     lib = _lib.load()
     bench = (1 << 1) | (1 << 11) | sum(1 << e for e in (16, 17, 20, 23, 24, 25)) | (1 << 34) | (1 << 36)   # k = 10
     assert lib.bke_kf_packed_models_bytes(0, bench) == 0

@@ -14,8 +14,6 @@ def test_header_declares_the_ring_and_its_limit():
     assert int(re.search(r"#define BKE_KF42_MAX_RING (\d+)", hdr).group(1)) == _lib.BKE_KF42_MAX_RING == 8
     sig = re.search(r"int bke_kf_steps_packed\(([^;]*)\);", hdr).group(1)
     assert [p.strip().split()[-1].lstrip("*") for p in sig.split(",")] == ["args", "record", "host_map", "zs", "n_steps", "stream"]
-    lib = _lib.load()
-    assert len(lib.bke_kf_steps_packed.argtypes) == 6 and len(lib.bke_capture_node_count.argtypes) == 2
 
 
 def _args(fake):

@@ -98,12 +98,6 @@ def _refused(a):
     return lib.bke_if_step(ctypes.byref(a), None) == _lib.BKE_ERR_BAD_ARG
 
 
-def test_if_step_struct_matches_the_header():
-    assert ctypes.sizeof(_lib.IfArgs) == 8 + 4 * 4 + 4 + 4 + 5 * 8 + 7 * 16 + 2 * 8 + 6 * 8 + 8
-    assert _lib.IfArgs.no_information.offset == 64
-    assert _lib.IfArgs.status.offset == ctypes.sizeof(_lib.IfArgs) - 8
-
-
 @pytest.mark.parametrize("field,value", [
     ("dim_x", 0), ("dim_z", 0), ("dim_u", -1), ("n_filters", -1), ("dtype", 7), ("flags", 0),
     ("flags", _lib.BKE_DO_UPDATE | _lib.BKE_UPDATE_FIRST), ("no_information", None), ("x", None), ("P_inv_out", None),

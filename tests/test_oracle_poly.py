@@ -1,6 +1,6 @@
 """CPU: the fp64 oracle of the polynomial trackers against the reference's golden vectors, bit for bit; the argument
-checks of bke_poly_filter (made before any device is needed); the struct layout; the gain helpers against the
-reference's values; and that the fp64 kernels carry no contracted multiply-add."""
+checks of bke_poly_filter (made before any device is needed); the gain helpers against the reference's values;
+and that the fp64 kernels carry no contracted multiply-add."""
 import ctypes
 import glob
 import os
@@ -93,16 +93,17 @@ def test_gain_helper_exceptions():
 
 
 # ---------------------------------------------------------------------------------------------- the C-ABI
-def test_poly_struct_matches_the_header():
-    assert ctypes.sizeof(_lib.PolyArgs) == 2 * 8 + 4 * 4 + 3 * 8 + 6 * 16 + 2 * 8 + 8 + 7 * 8
-    assert _lib.PolyArgs.x.offset == 32
-    assert _lib.PolyArgs.n.offset == 32 + 3 * 8 + 6 * 16
-    assert _lib.PolyArgs.K.offset == ctypes.sizeof(_lib.PolyArgs) - 8
+def _zeros(n, dtype=np.float64):
+    """np.zeros(n), page-locked where there is a device: a call that passes the checks then runs its kernel, which
+    reads and writes these buffers through their host addresses."""
+    import torch
+    z = np.zeros(n, dtype)
+    return torch.from_numpy(z).pin_memory().numpy() if torch.cuda.is_available() else z
 
 
 def _args(family=_lib.BKE_POLY_GH, order=1, N=8, T=3, mode=_lib.BKE_POLY_UPDATE):
-    keep = {k: np.zeros(N * 3 * (T + 1) + 16) for k in ("x", "dx", "ddx", "p", "z", "o")}
-    keep["n"] = np.zeros(N, np.int64)
+    keep = {k: _zeros(N * 3 * (T + 1) + 16) for k in ("x", "dx", "ddx", "p", "z", "o")}
+    keep["n"] = _zeros(N, np.int64)
     a = _lib.PolyArgs()
     a.n_filters, a.n_steps, a.family, a.order, a.dtype, a.mode = N, T, family, order, _lib.BKE_F64, mode
     a.x, a.dx, a.ddx, a.z = (keep[k].ctypes.data for k in ("x", "dx", "ddx", "z"))

@@ -1,16 +1,10 @@
 """The gated bank resampler without a GPU: NumPy's pairwise sum restated, the golden file against the oracle
-loop and its draw order, the C-ABI struct layout, argument checks and no CPU fallback."""
-import ctypes
-import os
-import subprocess
-
+loop and its draw order, argument checks and no CPU fallback."""
 import numpy as np
 import pytest
 
 from oracle import resample as ors
 import resample_bank_gated_oracle as rgo
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _lengths():
@@ -86,24 +80,6 @@ def test_golden_covers_the_gate_and_special_rows(golden):
     k = meta[meta[:, 4] >= 0][0][0]
     wf = g["w%d" % k][meta[k][4]]
     assert np.cumsum(wf / np.sum(wf))[-1] < 1
-
-
-def test_gated_args_layout_matches_header(tmp_path):
-    from filterpy_b200 import _lib
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "bke.h"', 'int main(void) {',
-             'printf("sizeof %zu\\n", sizeof(bke_resample_bank_gated_args));']
-    for fname, _ in _lib.ResampleBankGatedArgs._fields_:
-        lines.append('printf("%s %%zu\\n", offsetof(bke_resample_bank_gated_args, %s));' % (fname, fname))
-    lines += ['return 0; }']
-    src = tmp_path / "probe.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "probe"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    out = dict(ln.split() for ln in subprocess.check_output([str(exe)]).decode().splitlines() if ln.strip())
-    assert int(out.pop("sizeof")) == ctypes.sizeof(_lib.ResampleBankGatedArgs)
-    assert len(out) == len(_lib.ResampleBankGatedArgs._fields_)
-    for fname, val in out.items():
-        assert getattr(_lib.ResampleBankGatedArgs, fname).offset == int(val), fname
 
 
 def _args(L, **kw):

@@ -1,6 +1,5 @@
 """Multinomial / residual bank resampling without a GPU: the oracles against the reference's golden loop,
-the C-ABI struct layouts, argument checks, no spills in the new kernels, and no CPU fallback."""
-import ctypes
+argument checks, no spills in the new kernels, and no CPU fallback."""
 import os
 import subprocess
 
@@ -70,27 +69,6 @@ def test_golden_covers_special_rows_and_failures(golden):
         # residual's cumulative sum is not monotone on ordinary rows
         _, _, c = mro.residual_prepare_bank(g["w3"])
         assert (np.diff(c[:, :-1], axis=1) < 0).any()
-
-
-@pytest.mark.parametrize("sname,cls", [("bke_multinomial_resample_bank_args", "MultinomialResampleBankArgs"),
-                                       ("bke_residual_resample_bank_args", "ResidualResampleBankArgs")])
-def test_args_layout_matches_header(tmp_path, sname, cls):
-    from filterpy_b200 import _lib
-    C = getattr(_lib, cls)
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "bke.h"', 'int main(void) {',
-             'printf("sizeof %%zu\\n", sizeof(%s));' % sname]
-    for fname, _ in C._fields_:
-        lines.append('printf("%s %%zu\\n", offsetof(%s, %s));' % (fname, sname, fname))
-    lines += ['return 0; }']
-    src = tmp_path / "probe.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "probe"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    out = dict(ln.split() for ln in subprocess.check_output([str(exe)]).decode().splitlines() if ln.strip())
-    assert int(out.pop("sizeof")) == ctypes.sizeof(C)
-    assert len(out) == len(C._fields_)
-    for fname, val in out.items():
-        assert getattr(C, fname).offset == int(val), fname
 
 
 FAKE = 1 << 20          # never dereferenced: every refused call below fails before a launch
