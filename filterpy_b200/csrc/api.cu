@@ -43,7 +43,7 @@ int sm_count()
     return cached[dev];
 }
 
-static int require_device()
+int require_device()
 {
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
@@ -55,119 +55,123 @@ static int require_device()
     return BKE_OK;
 }
 
-static int validate_kf(const bke_kf_args *a, bool need_z)
+int check_dtype(int32_t dtype)
 {
-    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    if (a->n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
-    if (a->dim_x < 1) { set_error("dim_x must be 1 or greater"); return BKE_ERR_BAD_ARG; }   // kalman_filter.py:388
-    if (a->dim_z < 1) { set_error("dim_z must be 1 or greater"); return BKE_ERR_BAD_ARG; }   // :390
-    if (a->dim_u < 0) { set_error("dim_u must be 0 or greater"); return BKE_ERR_BAD_ARG; }   // :392
-    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
-    if (!(a->flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
-    if (!a->x || !a->P || !a->x_out || !a->P_out) { set_error("x, P, x_out, P_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    if (a->flags & BKE_DO_PREDICT) {
-        if (!a->F || !a->Q) { set_error("predict needs F and Q"); return BKE_ERR_BAD_ARG; }
-        if ((a->B == nullptr) != (a->u == nullptr) && a->dim_u > 0 && a->B && !a->u) { /* u=None: no control, kalman_filter.py:472 */ }
-    }
-    if (a->flags & BKE_DO_UPDATE) {
-        if (!a->H || !a->R) { set_error("update needs H and R"); return BKE_ERR_BAD_ARG; }
-        if (need_z && !a->z) { set_error("update needs z"); return BKE_ERR_BAD_ARG; }
-    }
-    const int64_t n = a->dim_x, m = a->dim_z;
-    auto bad_stride = [](int64_t s, int64_t full) { return s != 0 && s != full; };
-    if (bad_stride(a->F_stride, n * n) || bad_stride(a->Q_stride, n * n) || bad_stride(a->H_stride, m * n) ||
-        bad_stride(a->R_stride, m * m)) {
-        set_error("model strides must be 0 (shared) or the dense per-filter size");
-        return BKE_ERR_BAD_ARG;
-    }
+    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
     return BKE_OK;
 }
 
-static int validate_srkf(const bke_srkf_args *a)
+int check_bank(int64_t n, int64_t dim_x, int64_t dim_z, int64_t dim_u)
 {
-    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    if (a->n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
-    if (a->dim_x < 1) { set_error("dim_x must be 1 or greater"); return BKE_ERR_BAD_ARG; }   // square_root.py:128-133
-    if (a->dim_z < 1) { set_error("dim_z must be 1 or greater"); return BKE_ERR_BAD_ARG; }
-    if (a->dim_u < 0) { set_error("dim_u must be 0 or greater"); return BKE_ERR_BAD_ARG; }
-    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
-    if (!(a->flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
-    if (a->flags & ~(BKE_DO_PREDICT | BKE_DO_UPDATE)) { set_error("flags may only hold BKE_DO_PREDICT and BKE_DO_UPDATE"); return BKE_ERR_BAD_ARG; }
-    if (!a->x || !a->L || !a->x_out || !a->L_out) { set_error("x, L, x_out, L_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    if ((a->flags & BKE_DO_PREDICT) && (!a->F || !a->Lq)) { set_error("predict needs F and Lq"); return BKE_ERR_BAD_ARG; }   // :240-243
-    if ((a->flags & BKE_DO_UPDATE) && (!a->H || !a->Lr || !a->z)) { set_error("update needs H, Lr and z"); return BKE_ERR_BAD_ARG; }   // :204-215
-    if ((a->B != nullptr || a->u != nullptr) && (!a->B || !a->u || a->dim_u < 1)) {
-        set_error("a control input needs B, u and dim_u >= 1");                                       // :240
-        return BKE_ERR_BAD_ARG;
-    }
-    const int64_t n = a->dim_x, m = a->dim_z, du = a->dim_u;
-    auto bad_stride = [](int64_t s, int64_t full) { return s != 0 && s != full; };
-    if (bad_stride(a->F_stride, n * n) || bad_stride(a->Lq_stride, n * n) || bad_stride(a->H_stride, m * n) ||
-        bad_stride(a->Lr_stride, m * m) || bad_stride(a->B_stride, n * du) || bad_stride(a->u_stride, du)) {
-        set_error("model strides must be 0 (shared) or the dense per-filter size");
-        return BKE_ERR_BAD_ARG;
-    }
+    const char *why = n < 0 ? "n_filters < 0" : dim_x < 1 ? "dim_x must be 1 or greater" : dim_z < 1 ? "dim_z must be 1 or greater"
+                    : dim_u < 0 ? "dim_u must be 0 or greater" : nullptr;
+    if (!why) return BKE_OK;
+    set_error("bad dimensions: %s", why);
+    return BKE_ERR_BAD_ARG;
+}
+
+int check_predict_update(uint32_t flags)
+{
+    if (!(flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
     return BKE_OK;
+}
+
+int check_flag_bits(uint32_t flags, uint32_t allowed)
+{
+    if (!(flags & ~allowed)) return BKE_OK;
+    set_error("flags may only hold the bits this call takes, here only%s%s%s%s", allowed & BKE_DO_PREDICT ? " BKE_DO_PREDICT" : "",
+              allowed & BKE_DO_UPDATE ? " BKE_DO_UPDATE" : "", allowed & BKE_STATUS_STICKY ? " BKE_STATUS_STICKY" : "",
+              allowed & BKE_REVERSE_TILES ? " BKE_REVERSE_TILES" : "");
+    return BKE_ERR_BAD_ARG;
+}
+
+int check_strides(std::initializer_list<std::pair<int64_t, int64_t>> strides)
+{
+    for (const auto &s : strides)
+        if (s.first != 0 && s.first != s.second) { set_error("model strides must be 0 (shared) or the dense per-filter size"); return BKE_ERR_BAD_ARG; }
+    return BKE_OK;
+}
+
+int check_control(const void *B, const void *u, int64_t dim_u)
+{
+    if ((B || u) && (!B || !u || dim_u < 1)) { set_error("a control input needs B, u and dim_u >= 1"); return BKE_ERR_BAD_ARG; }
+    return BKE_OK;
+}
+
+static int validate_kf(const bke_kf_args &a, bool need_z)
+{
+    int rc;
+    if ((rc = check_bank(a.n_filters, a.dim_x, a.dim_z, a.dim_u)) || (rc = check_dtype(a.dtype)) || (rc = check_predict_update(a.flags)))
+        return rc;                                                       // kalman_filter.py:388-392
+    if (!a.x || !a.P || !a.x_out || !a.P_out) { set_error("x, P, x_out, P_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if ((a.flags & BKE_DO_PREDICT) && (!a.F || !a.Q)) { set_error("predict needs F and Q"); return BKE_ERR_BAD_ARG; }
+    if (a.flags & BKE_DO_UPDATE) {
+        if (!a.H || !a.R) { set_error("update needs H and R"); return BKE_ERR_BAD_ARG; }
+        if (need_z && !a.z) { set_error("update needs z"); return BKE_ERR_BAD_ARG; }
+    }
+    const int64_t n = a.dim_x, m = a.dim_z;
+    return check_strides({{a.F_stride, n * n}, {a.Q_stride, n * n}, {a.H_stride, m * n}, {a.R_stride, m * m}});
+}
+
+static int validate_srkf(const bke_srkf_args &a)
+{
+    int rc;
+    if ((rc = check_bank(a.n_filters, a.dim_x, a.dim_z, a.dim_u)) || (rc = check_dtype(a.dtype)) || (rc = check_predict_update(a.flags)) ||
+        (rc = check_flag_bits(a.flags, BKE_DO_PREDICT | BKE_DO_UPDATE)))
+        return rc;                                                       // square_root.py:128-133
+    if (!a.x || !a.L || !a.x_out || !a.L_out) { set_error("x, L, x_out, L_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if ((a.flags & BKE_DO_PREDICT) && (!a.F || !a.Lq)) { set_error("predict needs F and Lq"); return BKE_ERR_BAD_ARG; }   // square_root.py:240-243
+    if ((a.flags & BKE_DO_UPDATE) && (!a.H || !a.Lr || !a.z)) { set_error("update needs H, Lr and z"); return BKE_ERR_BAD_ARG; }   // :204-215
+    if ((rc = check_control(a.B, a.u, a.dim_u))) return rc;                                           // :240
+    const int64_t n = a.dim_x, m = a.dim_z, du = a.dim_u;
+    return check_strides({{a.F_stride, n * n}, {a.Lq_stride, n * n}, {a.H_stride, m * n}, {a.Lr_stride, m * m}, {a.B_stride, n * du},
+                          {a.u_stride, du}});
 }
 
 // the checks of bke_if_step
-static int validate_if(const bke_if_args *a)
+static int validate_if(const bke_if_args &a)
 {
-    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    if (a->n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
-    if (a->dim_x < 1) { set_error("dim_x must be 1 or greater"); return BKE_ERR_BAD_ARG; }   // information_filter.py:132-137
-    if (a->dim_z < 1) { set_error("dim_z must be 1 or greater"); return BKE_ERR_BAD_ARG; }
-    if (a->dim_u < 0) { set_error("dim_u must be 0 or greater"); return BKE_ERR_BAD_ARG; }
-    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
-    if (!(a->flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
-    if (a->flags & ~(BKE_DO_PREDICT | BKE_DO_UPDATE | BKE_STATUS_STICKY)) {
-        set_error("flags may only hold BKE_DO_PREDICT, BKE_DO_UPDATE and BKE_STATUS_STICKY");
-        return BKE_ERR_BAD_ARG;
-    }
-    if (!a->x || !a->P_inv || !a->x_out || !a->P_inv_out) { set_error("x, P_inv, x_out, P_inv_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    if (!a->no_information) { set_error("no_information must be non-NULL (the per-filter flag is read and written)"); return BKE_ERR_BAD_ARG; }
-    if ((a->flags & BKE_DO_PREDICT) && (!a->F || !a->F_inv || !a->Q)) { set_error("predict needs F, F_inv and Q"); return BKE_ERR_BAD_ARG; }
-    if ((a->flags & BKE_DO_UPDATE) && (!a->H || !a->R_inv || !a->z)) { set_error("update needs H, R_inv and z"); return BKE_ERR_BAD_ARG; }
-    if ((a->B != nullptr || a->u != nullptr) && (!a->B || !a->u || a->dim_u < 1)) {
-        set_error("a control input needs B, u and dim_u >= 1");                                       // :274
-        return BKE_ERR_BAD_ARG;
-    }
-    const int64_t n = a->dim_x, m = a->dim_z, du = a->dim_u;
-    auto bad_stride = [](int64_t s, int64_t full) { return s != 0 && s != full; };
-    if (bad_stride(a->F_stride, n * n) || bad_stride(a->F_inv_stride, n * n) || bad_stride(a->Q_stride, n * n) ||
-        bad_stride(a->H_stride, m * n) || bad_stride(a->R_inv_stride, m * m) || bad_stride(a->B_stride, n * du) ||
-        bad_stride(a->u_stride, du)) {
-        set_error("model strides must be 0 (shared) or the dense per-filter size");
-        return BKE_ERR_BAD_ARG;
-    }
-    if (a->ll_mode != BKE_IF_LL_NONE && a->ll_mode != BKE_IF_LL_FULL && a->ll_mode != BKE_IF_LL_BROADCAST) {
+    int rc;
+    if ((rc = check_bank(a.n_filters, a.dim_x, a.dim_z, a.dim_u)) || (rc = check_dtype(a.dtype)) || (rc = check_predict_update(a.flags)) ||
+        (rc = check_flag_bits(a.flags, BKE_DO_PREDICT | BKE_DO_UPDATE | BKE_STATUS_STICKY)))
+        return rc;                                                       // information_filter.py:132-137
+    if (!a.x || !a.P_inv || !a.x_out || !a.P_inv_out) { set_error("x, P_inv, x_out, P_inv_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if (!a.no_information) { set_error("no_information must be non-NULL (the per-filter flag is read and written)"); return BKE_ERR_BAD_ARG; }
+    if ((a.flags & BKE_DO_PREDICT) && (!a.F || !a.F_inv || !a.Q)) { set_error("predict needs F, F_inv and Q"); return BKE_ERR_BAD_ARG; }
+    if ((a.flags & BKE_DO_UPDATE) && (!a.H || !a.R_inv || !a.z)) { set_error("update needs H, R_inv and z"); return BKE_ERR_BAD_ARG; }
+    if ((rc = check_control(a.B, a.u, a.dim_u))) return rc;                                           // information_filter.py:274
+    const int64_t n = a.dim_x, m = a.dim_z, du = a.dim_u;
+    if ((rc = check_strides({{a.F_stride, n * n}, {a.F_inv_stride, n * n}, {a.Q_stride, n * n}, {a.H_stride, m * n},
+                             {a.R_inv_stride, m * m}, {a.B_stride, n * du}, {a.u_stride, du}})))
+        return rc;
+    if (a.ll_mode != BKE_IF_LL_NONE && a.ll_mode != BKE_IF_LL_FULL && a.ll_mode != BKE_IF_LL_BROADCAST) {
         set_error("ll_mode must be BKE_IF_LL_NONE, BKE_IF_LL_FULL or BKE_IF_LL_BROADCAST");
         return BKE_ERR_BAD_ARG;
     }
-    if ((a->ll_mode == BKE_IF_LL_FULL && m != n) || (a->ll_mode == BKE_IF_LL_BROADCAST && m != 1)) {
-        set_error("ll_mode %s needs %s", a->ll_mode == BKE_IF_LL_FULL ? "BKE_IF_LL_FULL" : "BKE_IF_LL_BROADCAST",
-                  a->ll_mode == BKE_IF_LL_FULL ? "dim_z == dim_x" : "dim_z == 1");
+    if ((a.ll_mode == BKE_IF_LL_FULL && m != n) || (a.ll_mode == BKE_IF_LL_BROADCAST && m != 1)) {
+        set_error("ll_mode %s needs %s", a.ll_mode == BKE_IF_LL_FULL ? "BKE_IF_LL_FULL" : "BKE_IF_LL_BROADCAST",
+                  a.ll_mode == BKE_IF_LL_FULL ? "dim_z == dim_x" : "dim_z == 1");
         return BKE_ERR_BAD_ARG;
     }
-    if (a->ll_mode != BKE_IF_LL_NONE && !a->log_likelihood) { set_error("ll_mode needs log_likelihood"); return BKE_ERR_BAD_ARG; }
+    if (a.ll_mode != BKE_IF_LL_NONE && !a.log_likelihood) { set_error("ll_mode needs log_likelihood"); return BKE_ERR_BAD_ARG; }
     return BKE_OK;
 }
 
 // the checks of bke_poly_filter
-static int validate_poly(const bke_poly_args *a)
+static int validate_poly(const bke_poly_args &a)
 {
-    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    if (a->n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
-    if (a->n_steps < 1) { set_error("n_steps must be 1 or greater"); return BKE_ERR_BAD_ARG; }
-    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
-    const int fam = a->family;
+    int rc;
+    if ((rc = check_bank(a.n_filters))) return rc;
+    if (a.n_steps < 1) { set_error("n_steps must be 1 or greater"); return BKE_ERR_BAD_ARG; }
+    if ((rc = check_dtype(a.dtype))) return rc;
+    const int fam = a.family;
     if (fam < BKE_POLY_GH || fam > BKE_POLY_FADING) { set_error("family must be one of BKE_POLY_*"); return BKE_ERR_BAD_ARG; }
     const bool gh = fam == BKE_POLY_GH || fam == BKE_POLY_GHK;
-    if (!gh && (a->order < 0 || a->order > 2)) { set_error("order must be between 0 and 2"); return BKE_ERR_BAD_ARG; }
-    if (a->mode != BKE_POLY_UPDATE && a->mode != BKE_POLY_BATCH) { set_error("mode must be BKE_POLY_UPDATE or BKE_POLY_BATCH"); return BKE_ERR_BAD_ARG; }
-    const bool batch = a->mode == BKE_POLY_BATCH;
-    const int ord = fam == BKE_POLY_GH ? 1 : fam == BKE_POLY_GHK ? 2 : a->order;
-    if (a->n_filters == 0) return BKE_OK;
+    if (!gh && (a.order < 0 || a.order > 2)) { set_error("order must be between 0 and 2"); return BKE_ERR_BAD_ARG; }
+    if (a.mode != BKE_POLY_UPDATE && a.mode != BKE_POLY_BATCH) { set_error("mode must be BKE_POLY_UPDATE or BKE_POLY_BATCH"); return BKE_ERR_BAD_ARG; }
+    const bool batch = a.mode == BKE_POLY_BATCH;
+    const int ord = fam == BKE_POLY_GH ? 1 : fam == BKE_POLY_GHK ? 2 : a.order;
+    if (a.n_filters == 0) return BKE_OK;
     // what the instance reads
     const bool need_dx = gh, need_ddx = fam == BKE_POLY_GHK && !batch;
     const bool need_g = fam != BKE_POLY_LSQ;
@@ -176,32 +180,30 @@ static int validate_poly(const bke_poly_args *a)
     const bool need_dt = ord >= 1;
     const bool need_dt2 = (fam == BKE_POLY_GHK && !batch) || (!gh && ord == 2);
     const bool need_hdt2 = fam == BKE_POLY_LSQ && ord == 2;
-    if (!a->x || !a->z || (need_dx && !a->dx) || (need_ddx && !a->ddx)) { set_error("the state and z must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    if ((need_g && !a->g) || (need_h && !a->h) || (need_k && !a->k) || (need_dt && !a->dt) || (need_dt2 && !a->dt2) ||
-        (need_hdt2 && !a->hdt2)) {
+    if (!a.x || !a.z || (need_dx && !a.dx) || (need_ddx && !a.ddx)) { set_error("the state and z must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if ((need_g && !a.g) || (need_h && !a.h) || (need_k && !a.k) || (need_dt && !a.dt) || (need_dt2 && !a.dt2) ||
+        (need_hdt2 && !a.hdt2)) {
         set_error("a parameter this family and order read is NULL");
         return BKE_ERR_BAD_ARG;
     }
-    auto bad_stride = [](const void *p, int64_t s) { return p && s != 0 && s != 1; };
-    if (bad_stride(a->g, a->g_stride) || bad_stride(a->h, a->h_stride) || bad_stride(a->k, a->k_stride) ||
-        bad_stride(a->dt, a->dt_stride) || bad_stride(a->dt2, a->dt2_stride) || bad_stride(a->hdt2, a->hdt2_stride)) {
-        set_error("parameter strides must be 0 (shared) or 1 (per filter)");
-        return BKE_ERR_BAD_ARG;
-    }
+    // a parameter per filter is one element; the stride of an absent one is not read
+    if ((rc = check_strides({{a.g ? a.g_stride : 0, 1}, {a.h ? a.h_stride : 0, 1}, {a.k ? a.k_stride : 0, 1},
+                             {a.dt ? a.dt_stride : 0, 1}, {a.dt2 ? a.dt2_stride : 0, 1}, {a.hdt2 ? a.hdt2_stride : 0, 1}})))
+        return rc;
     // the outputs each family and mode have
-    if (a->predictions && !(gh && batch)) { set_error("predictions is an output of the GH / GHK batch_filter only"); return BKE_ERR_BAD_ARG; }
-    if (a->y && (batch || fam == BKE_POLY_LSQ || fam == BKE_POLY_FADING)) {
+    if (a.predictions && !(gh && batch)) { set_error("predictions is an output of the GH / GHK batch_filter only"); return BKE_ERR_BAD_ARG; }
+    if (a.y && (batch || fam == BKE_POLY_LSQ || fam == BKE_POLY_FADING)) {
         set_error("y is an output of the GH, GHK and GH_ORDER update only");      // least_squares.py:128 never stores y
         return BKE_ERR_BAD_ARG;
     }
-    if ((a->x_prediction || a->dx_prediction) && !(gh && !batch)) { set_error("x_prediction / dx_prediction are outputs of the GH / GHK update only"); return BKE_ERR_BAD_ARG; }
-    if (a->ddx_prediction && !(fam == BKE_POLY_GHK && !batch)) { set_error("ddx_prediction is an output of the GHK update only"); return BKE_ERR_BAD_ARG; }
-    if (a->K && !(fam == BKE_POLY_LSQ && !batch)) { set_error("K is an output of the LSQ update only"); return BKE_ERR_BAD_ARG; }
+    if ((a.x_prediction || a.dx_prediction) && !(gh && !batch)) { set_error("x_prediction / dx_prediction are outputs of the GH / GHK update only"); return BKE_ERR_BAD_ARG; }
+    if (a.ddx_prediction && !(fam == BKE_POLY_GHK && !batch)) { set_error("ddx_prediction is an output of the GHK update only"); return BKE_ERR_BAD_ARG; }
+    if (a.K && !(fam == BKE_POLY_LSQ && !batch)) { set_error("K is an output of the LSQ update only"); return BKE_ERR_BAD_ARG; }
     if (fam == BKE_POLY_LSQ) {
-        if (!a->n) { set_error("LSQ needs the counter n"); return BKE_ERR_BAD_ARG; }
+        if (!a.n) { set_error("LSQ needs the counter n"); return BKE_ERR_BAD_ARG; }
         // the largest counter the call reaches, and the product of it the order's gains form (least_squares.py:131-145)
         int64_t top, p;
-        if (a->n_max < 0 || __builtin_add_overflow(a->n_max, a->n_steps, &top) ||
+        if (a.n_max < 0 || __builtin_add_overflow(a.n_max, a.n_steps, &top) ||
             (ord >= 1 && __builtin_mul_overflow(top, top + 1, &p)) ||
             (ord == 2 && (__builtin_mul_overflow(p, top + 2, &p) || __builtin_mul_overflow(top, 3 * top, &p)))) {
             set_error("the LSQ counter n_max + n_steps overflows int64 in n(n+1)(n+2) (or the product its order forms)");
@@ -215,22 +217,17 @@ static int validate_poly(const bke_poly_args *a)
 static int validate_imm(const bke_imm_batch_args *a)
 {
     if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    if (a->n_tracks < 0) { set_error("n_tracks < 0"); return BKE_ERR_BAD_ARG; }
+    int rc;
+    if ((rc = check_bank(a->n_tracks, a->dim_x, a->dim_z))) return rc;
     if (a->n_steps < 0) { set_error("n_steps < 0"); return BKE_ERR_BAD_ARG; }
-    if (a->dim_x < 1 || a->dim_z < 1) { set_error("dim_x and dim_z must be 1 or greater"); return BKE_ERR_BAD_ARG; }
-    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if ((rc = check_dtype(a->dtype))) return rc;
     if (a->n_models < 2 || a->n_models > BKE_MM_MAX_MODELS) { set_error("n_models must be in [2, %d]", BKE_MM_MAX_MODELS); return BKE_ERR_BAD_ARG; }
-    if (a->flags & ~BKE_STATUS_STICKY) { set_error("flags may only hold BKE_STATUS_STICKY"); return BKE_ERR_BAD_ARG; }
+    if ((rc = check_flag_bits(a->flags, BKE_STATUS_STICKY))) return rc;
     const int M = a->n_models;
     const int64_t N = a->n_tracks, T = a->n_steps, n = a->dim_x, m = a->dim_z;
-    auto bad_stride = [](int64_t s, int64_t full) { return s != 0 && s != full; };
-    for (int j = 0; j < M; j++) {
-        if (bad_stride(a->F_stride[j], n * n) || bad_stride(a->Q_stride[j], n * n) || bad_stride(a->H_stride[j], m * n) ||
-            bad_stride(a->R_stride[j], m * m)) {
-            set_error("model %d: strides must be 0 (shared) or the dense per-track size", j);
-            return BKE_ERR_BAD_ARG;
-        }
-    }
+    for (int j = 0; j < M; j++)
+        if ((rc = check_strides({{a->F_stride[j], n * n}, {a->Q_stride[j], n * n}, {a->H_stride[j], m * n}, {a->R_stride[j], m * m}})))
+            return rc;
     if (N == 0 || T == 0) return BKE_OK;
     for (int j = 0; j < M; j++) {
         if (!a->x[j] || !a->P[j] || !a->F[j] || !a->Q[j] || !a->H[j] || !a->R[j] || !a->S[j] || !a->log_likelihood[j] ||
@@ -247,7 +244,7 @@ static int validate_imm(const bke_imm_batch_args *a)
     // every array the call writes must be clear of every other array it touches
     struct Span { const void *p; int64_t bytes; bool written; };
     const int64_t es = a->dtype == BKE_F32 ? 4 : 8;
-    Span sp[14 * BKE_MM_MAX_MODELS + 10];
+    Span sp[14 * BKE_MM_MAX_MODELS + 11];      // 14 arrays per model, 11 shared (zs_valid among them)
     int ns = 0;
     auto add = [&](const void *p, int64_t elems, bool written) { sp[ns++] = Span{p, elems, written}; };
     for (int j = 0; j < M; j++) {
@@ -288,40 +285,35 @@ static int validate_imm(const bke_imm_batch_args *a)
 }
 
 // the checks of bke_score_measurements
-static int validate_score(const bke_score_args *a)
+static int validate_score(const bke_score_args &a)
 {
-    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    if (a->n_tracks < 0 || a->n_candidates < 0) { set_error("n_tracks and n_candidates must be 0 or greater"); return BKE_ERR_BAD_ARG; }
-    if (a->dtype != BKE_F32 && a->dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
-    const bool uses_n = a->x || a->P;
-    if (a->dim_z < 1 || a->dim_z > 1024 || (uses_n && (a->dim_x < 1 || a->dim_x > 1024))) {
+    if (a.n_tracks < 0 || a.n_candidates < 0) { set_error("n_tracks and n_candidates must be 0 or greater"); return BKE_ERR_BAD_ARG; }
+    if (int rc = check_dtype(a.dtype)) return rc;
+    const bool uses_n = a.x || a.P;
+    if (a.dim_z < 1 || a.dim_z > 1024 || (uses_n && (a.dim_x < 1 || a.dim_x > 1024))) {
         set_error("dim_z (and dim_x, when x or P is given) must be between 1 and 1024");
         return BKE_ERR_BAD_ARG;
     }
-    const int64_t n = a->dim_x, m = a->dim_z;
-    if (!a->x == !a->mean) { set_error("exactly one of x and mean must be given"); return BKE_ERR_BAD_ARG; }
-    if (a->P && a->S) { set_error("at most one of P and S may be given"); return BKE_ERR_BAD_ARG; }
-    if (a->H && !uses_n) { set_error("H maps x or P: it is read only with one of them"); return BKE_ERR_BAD_ARG; }
-    if (uses_n && !a->H && n != m) { set_error("without H (the identity) dim_x must equal dim_z"); return BKE_ERR_BAD_ARG; }
-    if (a->P && !a->R) { set_error("S = H P H' + R needs R"); return BKE_ERR_BAD_ARG; }
-    if (a->R && !a->P) { set_error("R is read only with P"); return BKE_ERR_BAD_ARG; }
-    if ((a->H && a->H_stride != 0 && a->H_stride != m * n) || (a->R && a->R_stride != 0 && a->R_stride != m * m) ||
-        (a->S && a->S_stride != 0 && a->S_stride != m * m)) {
-        set_error("H, R and S strides must be 0 (shared) or the dense per-track size");
-        return BKE_ERR_BAD_ARG;
-    }
-    const bool scores = a->d2 || a->mahalanobis || a->log_likelihood || a->likelihood;
-    if (!(a->zhat || a->y || scores || a->status)) { set_error("no output is requested"); return BKE_ERR_BAD_ARG; }
-    if ((scores || a->status) && !a->P && !a->S) { set_error("the scores and status need a covariance: P or S"); return BKE_ERR_BAD_ARG; }
-    if ((a->y || scores) && !a->z) { set_error("y and the scores need z"); return BKE_ERR_BAD_ARG; }
-    if (a->z_track_stride < 0 || a->z_cand_stride < 0) { set_error("z strides must be 0 or greater"); return BKE_ERR_BAD_ARG; }
+    const int64_t n = a.dim_x, m = a.dim_z;
+    if (!a.x == !a.mean) { set_error("exactly one of x and mean must be given"); return BKE_ERR_BAD_ARG; }
+    if (a.P && a.S) { set_error("at most one of P and S may be given"); return BKE_ERR_BAD_ARG; }
+    if (a.H && !uses_n) { set_error("H maps x or P: it is read only with one of them"); return BKE_ERR_BAD_ARG; }
+    if (uses_n && !a.H && n != m) { set_error("without H (the identity) dim_x must equal dim_z"); return BKE_ERR_BAD_ARG; }
+    if (a.P && !a.R) { set_error("S = H P H' + R needs R"); return BKE_ERR_BAD_ARG; }
+    if (a.R && !a.P) { set_error("R is read only with P"); return BKE_ERR_BAD_ARG; }
+    if (int rc = check_strides({{a.H ? a.H_stride : 0, m * n}, {a.R ? a.R_stride : 0, m * m}, {a.S ? a.S_stride : 0, m * m}})) return rc;
+    const bool scores = a.d2 || a.mahalanobis || a.log_likelihood || a.likelihood;
+    if (!(a.zhat || a.y || scores || a.status)) { set_error("no output is requested"); return BKE_ERR_BAD_ARG; }
+    if ((scores || a.status) && !a.P && !a.S) { set_error("the scores and status need a covariance: P or S"); return BKE_ERR_BAD_ARG; }
+    if ((a.y || scores) && !a.z) { set_error("y and the scores need z"); return BKE_ERR_BAD_ARG; }
+    if (a.z_track_stride < 0 || a.z_cand_stride < 0) { set_error("z strides must be 0 or greater"); return BKE_ERR_BAD_ARG; }
     // every offset the kernel forms fits int64: pair * m, and z's last element
     int64_t pairs, t, u, last;
-    if (__builtin_mul_overflow(a->n_tracks, a->n_candidates, &pairs) || __builtin_mul_overflow(pairs, m, &t) ||
-        (a->n_tracks > 0 && __builtin_mul_overflow(a->n_tracks - 1, a->z_track_stride, &t)) ||
-        (a->n_candidates > 0 && __builtin_mul_overflow(a->n_candidates - 1, a->z_cand_stride, &u)) ||
-        (a->n_tracks > 0 && a->n_candidates > 0 && __builtin_add_overflow(t, u, &last)) ||
-        (a->n_tracks > 0 && a->n_candidates > 0 && __builtin_add_overflow(last, m, &last))) {
+    if (__builtin_mul_overflow(a.n_tracks, a.n_candidates, &pairs) || __builtin_mul_overflow(pairs, m, &t) ||
+        (a.n_tracks > 0 && __builtin_mul_overflow(a.n_tracks - 1, a.z_track_stride, &t)) ||
+        (a.n_candidates > 0 && __builtin_mul_overflow(a.n_candidates - 1, a.z_cand_stride, &u)) ||
+        (a.n_tracks > 0 && a.n_candidates > 0 && __builtin_add_overflow(t, u, &last)) ||
+        (a.n_tracks > 0 && a.n_candidates > 0 && __builtin_add_overflow(last, m, &last))) {
         set_error("N * K * dim_z or the z offsets overflow int64");
         return BKE_ERR_BAD_ARG;
     }
@@ -332,8 +324,8 @@ static int validate_score(const bke_score_args *a)
 template <typename Args>
 static int validate_sigma(const Args &a)
 {
-    if (a.dtype != BKE_F32 && a.dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
-    if (!(a.flags & (BKE_DO_PREDICT | BKE_DO_UPDATE))) { set_error("flags selects neither predict nor update"); return BKE_ERR_BAD_ARG; }
+    int rc;
+    if ((rc = check_dtype(a.dtype)) || (rc = check_predict_update(a.flags))) return rc;
     if (!a.x || !a.P || !a.x_out || !a.P_out) { set_error("x, P, x_out, P_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
     if ((a.flags & BKE_DO_PREDICT) && !a.Q) { set_error("predict needs Q"); return BKE_ERR_BAD_ARG; }
     if ((a.flags & BKE_DO_UPDATE) && (!a.R || !a.z)) { set_error("update needs R and z"); return BKE_ERR_BAD_ARG; }
@@ -347,8 +339,8 @@ static int validate_sigma(const Args &a)
 // a compiled model)
 int validate_ukf(const bke_ukf_args &a)
 {
-    if (a.n_filters < 0 || a.dim_x < 1 || a.dim_z < 1) { set_error("bad dimensions"); return BKE_ERR_BAD_ARG; }
-    if (int rc = validate_sigma(a)) return rc;
+    int rc;
+    if ((rc = check_bank(a.n_filters, a.dim_x, a.dim_z)) || (rc = validate_sigma(a))) return rc;
     const double lam_n = a.alpha * a.alpha * (a.dim_x + a.kappa);
     if (!(a.flags & BKE_UKF_SIMPLEX) && !(lam_n != 0.0)) { set_error("alpha^2 (n + kappa) must be non-zero"); return BKE_ERR_BAD_ARG; }
     return BKE_OK;
@@ -356,8 +348,8 @@ int validate_ukf(const bke_ukf_args &a)
 
 int validate_ckf(const bke_ckf_args &a)
 {
-    if (a.n_filters < 0 || a.dim_x < 1 || a.dim_z < 1) { set_error("bad dimensions"); return BKE_ERR_BAD_ARG; }
-    if (int rc = validate_sigma(a)) return rc;
+    int rc;
+    if ((rc = check_bank(a.n_filters, a.dim_x, a.dim_z)) || (rc = validate_sigma(a))) return rc;
     if ((a.flags & BKE_DO_UPDATE) && !(a.flags & BKE_DO_PREDICT) && !a.sigmas_f) {
         set_error("an update without predict reads the propagated points of the last predict: sigmas_f must be non-NULL");
         return BKE_ERR_BAD_ARG;
@@ -367,20 +359,22 @@ int validate_ckf(const bke_ckf_args &a)
 
 int validate_enkf(const bke_enkf_args &a)
 {
-    if (a.n_filters < 0 || a.dim_x < 1 || a.dim_x > 16 || a.dim_z < 1) { set_error("bad dimensions (1 <= dim_x <= 16, 1 <= dim_z)"); return BKE_ERR_BAD_ARG; }
+    int rc;
+    if ((rc = check_bank(a.n_filters, a.dim_x, a.dim_z))) return rc;
+    if (a.dim_x > 16) { set_error("bad dimensions: dim_x must be 16 or less"); return BKE_ERR_BAD_ARG; }
     if (a.n_members < 2) { set_error("n_members must be 2 or greater (the covariances divide by n_members - 1)"); return BKE_ERR_BAD_ARG; }
-    if (int rc = validate_sigma(a)) return rc;
-    if (a.flags & ~(BKE_DO_PREDICT | BKE_DO_UPDATE)) { set_error("flags: only BKE_DO_PREDICT and BKE_DO_UPDATE apply to the EnKF"); return BKE_ERR_BAD_ARG; }
+    if ((rc = validate_sigma(a)) || (rc = check_flag_bits(a.flags, BKE_DO_PREDICT | BKE_DO_UPDATE))) return rc;
     if (!a.sigmas || !a.sigmas_out) { set_error("sigmas and sigmas_out must be non-NULL"); return BKE_ERR_BAD_ARG; }
     if (a.Q_stride < 0 || a.R_stride < 0 || a.F_stride < 0 || a.H_stride < 0) { set_error("negative model stride"); return BKE_ERR_BAD_ARG; }
     if (a.n_members > (1 << 24)) { set_error("n_members must be at most 2^24"); return BKE_ERR_BAD_ARG; }
     return BKE_OK;
 }
 
-// the pre-built steps: a known model id, and a range model at the shape it is written for
-template <typename Args>
-static int validate_builtin_models(const Args &a)
+// the pre-built steps: the family's checks, then a known model id, and a range model at the shape it is written for
+template <typename Args, int (*validate)(const Args &)>
+static int validate_prebuilt(const Args &a)
 {
+    if (int rc = validate(a)) return rc;
     if (a.hx_model == BKE_HX_RANGE_AZ_EL && !(a.dim_x == 6 && a.dim_z == 3)) { set_error("BKE_HX_RANGE_AZ_EL needs dim_x=6, dim_z=3"); return BKE_ERR_BAD_ARG; }
     if (a.hx_model == BKE_HX_RANGE_BEARING && !(a.dim_x == 4 && a.dim_z == 2)) { set_error("BKE_HX_RANGE_BEARING needs dim_x=4, dim_z=2"); return BKE_ERR_BAD_ARG; }
     if (a.fx_model < 0 || a.fx_model > BKE_FX_CONST_VEL || a.hx_model < 0 || a.hx_model > BKE_HX_RANGE_BEARING) {
@@ -389,16 +383,21 @@ static int validate_builtin_models(const Args &a)
     return BKE_OK;
 }
 
-// bke_ukf_step, bke_ckf_step, bke_enkf_step
-template <typename Args>
-static int sigma_step(const Args *args, int (*validate)(const Args &), int (*launch)(const Args &, cudaStream_t), void *stream)
+template <typename Args> static bool empty_bank(const Args &a) { return a.n_filters == 0; }
+static bool empty_bank(const bke_kf_rows_args &a) { return a.step.n_filters == 0; }
+static bool empty_bank(const bke_kf_batch_args &a) { return a.step.n_filters == 0; }
+static bool empty_bank(const bke_fls_args &a) { return a.step.n_filters == 0; }
+static bool empty_bank(const bke_score_args &a) { return a.n_tracks == 0 || a.n_candidates == 0; }
+
+// the body of an entry point: its argument checks, then the device, then an empty bank returns at once, then the launch
+template <typename Args, typename Validate, typename Launch>
+static int checked_launch(const Args *args, Validate validate, Launch launch, void *stream)
 {
     if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    const Args &a = *args;
-    int rc = validate(a);
-    if (rc || (rc = validate_builtin_models(a)) || (rc = require_device())) return rc;
-    if (a.n_filters == 0) return BKE_OK;
-    return launch(a, (cudaStream_t)stream);
+    int rc = validate(*args);
+    if (rc || (rc = require_device())) return rc;
+    if (empty_bank(*args)) return BKE_OK;
+    return launch(*args, (cudaStream_t)stream);
 }
 
 }  // namespace bke
@@ -432,82 +431,77 @@ int bke_device_count(void)
 
 int bke_kf_step(const bke_kf_args *args, void *stream)
 {
-    int rc = validate_kf(args, true);
-    if (rc) return rc;
-    if ((rc = require_device())) return rc;
-    if (args->n_filters == 0) return BKE_OK;
-    cudaStream_t s = (cudaStream_t)stream;
-    return launch_kf_any(*args, s);
+    return checked_launch(args, [](const bke_kf_args &a) { return validate_kf(a, true); }, launch_kf_any, stream);
 }
 
 // the flags of the two other update forms: an update, optionally after a predict
-static int validate_update_form(const bke_kf_args *a)
+static int validate_update_form(const bke_kf_args &a)
 {
-    if (!(a->flags & BKE_DO_UPDATE) || (a->flags & ~(BKE_DO_PREDICT | BKE_DO_UPDATE | BKE_STATUS_STICKY | BKE_REVERSE_TILES))) {
-        set_error("flags must be BKE_DO_UPDATE, optionally with BKE_DO_PREDICT and BKE_STATUS_STICKY");
-        return BKE_ERR_BAD_ARG;
-    }
+    if (int rc = check_flag_bits(a.flags, BKE_DO_PREDICT | BKE_DO_UPDATE | BKE_STATUS_STICKY | BKE_REVERSE_TILES)) return rc;
+    if (!(a.flags & BKE_DO_UPDATE)) { set_error("flags must hold BKE_DO_UPDATE"); return BKE_ERR_BAD_ARG; }
     return BKE_OK;
 }
 
 int bke_kf_step_correlated(const bke_kf_args *args, const void *M, int64_t M_stride, void *stream)
 {
-    int rc = validate_kf(args, true);
-    if (rc || (rc = validate_update_form(args))) return rc;
-    if (!M) { set_error("M is NULL"); return BKE_ERR_BAD_ARG; }
-    if (M_stride != 0 && M_stride != (int64_t)args->dim_x * args->dim_z) {
-        set_error("M_stride must be 0 (shared) or dim_x * dim_z");
-        return BKE_ERR_BAD_ARG;
-    }
-    if ((rc = require_device())) return rc;
-    if (args->n_filters == 0) return BKE_OK;
-    cudaStream_t s = (cudaStream_t)stream;
-    rc = launch_kf_direct_correlated(*args, M, M_stride, s);
-    if (rc == BKE_ERR_UNSUPPORTED) rc = launch_kf_generic_correlated(*args, M, M_stride, s);
-    return rc;
+    auto validate = [&](const bke_kf_args &a) {
+        int rc;
+        if ((rc = validate_kf(a, true)) || (rc = validate_update_form(a))) return rc;
+        if (!M) { set_error("M is NULL"); return BKE_ERR_BAD_ARG; }
+        return check_strides({{M_stride, (int64_t)a.dim_x * a.dim_z}});
+    };
+    auto launch = [&](const bke_kf_args &a, cudaStream_t s) {
+        int rc = launch_kf_direct_correlated(a, M, M_stride, s);
+        return rc == BKE_ERR_UNSUPPORTED ? launch_kf_generic_correlated(a, M, M_stride, s) : rc;
+    };
+    return checked_launch(args, validate, launch, stream);
 }
 
-int bke_kf_update_rows(const bke_kf_rows_args *args, void *stream)
+static int validate_rows(const bke_kf_rows_args &r)
 {
-    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    const bke_kf_args &a = args->step;
-    const int64_t n = a.dim_x, m = a.dim_z, L = args->rows, start = args->start;
+    const bke_kf_args &a = r.step;
+    const int64_t n = a.dim_x, m = a.dim_z, L = r.rows, start = r.start;
     if (L < 1 || start < 0 || start + L > m) {
         set_error("the block of rows %lld .. %lld is not within the %lld rows of z", (long long)start, (long long)(start + L - 1), (long long)m);
         return BKE_ERR_BAD_ARG;
     }
-    if (args->H_i_stride != 0 && args->H_i_stride != L * n) { set_error("H_i_stride must be 0 (shared) or rows * dim_x"); return BKE_ERR_BAD_ARG; }
-    if (args->R_i_stride != 0 && args->R_i_stride != L * L) { set_error("R_i_stride must be 0 (shared) or rows * rows"); return BKE_ERR_BAD_ARG; }
+    int rc;
+    if ((rc = check_strides({{r.H_i_stride, L * n}, {r.R_i_stride, L * L}}))) return rc;
     if (a.S || a.SI || a.log_likelihood) { set_error("update_rows does not write S, SI or log_likelihood: they must be NULL"); return BKE_ERR_BAD_ARG; }
     // the checks of bke_kf_step on the bank's arrays; a caller-supplied block stands in for H or R there
     bke_kf_args chk = a;
-    if (args->H_i) { chk.H = args->H_i; chk.H_stride = 0; }
-    if (args->R_i) { chk.R = args->R_i; chk.R_stride = 0; }
-    int rc = validate_kf(&chk, true);
-    if (rc || (rc = validate_update_form(&a))) return rc;
-    if ((rc = require_device())) return rc;
-    if (a.n_filters == 0) return BKE_OK;
-    // the block as an update of L rows: H_i is contiguous in the bank's H, R_i has the row pitch m there
+    if (r.H_i) { chk.H = r.H_i; chk.H_stride = 0; }
+    if (r.R_i) { chk.R = r.R_i; chk.R_stride = 0; }
+    if ((rc = validate_kf(chk, true))) return rc;
+    return validate_update_form(a);
+}
+
+// the block as an update of L rows: H_i is contiguous in the bank's H, R_i has the row pitch m there
+static int launch_rows(const bke_kf_rows_args &r, cudaStream_t s)
+{
+    const bke_kf_args &a = r.step;
+    const int64_t n = a.dim_x, m = a.dim_z, L = r.rows, start = r.start;
     const size_t es = a.dtype == BKE_F32 ? 4 : 8;
     bke_kf_args b = a;
     b.dim_z = (int32_t)L;
-    if (args->H_i) { b.H = args->H_i; b.H_stride = args->H_i_stride; }
+    if (r.H_i) { b.H = r.H_i; b.H_stride = r.H_i_stride; }
     else b.H = (const char *)a.H + start * n * es;
     int rpitch = (int)L;
-    if (args->R_i) { b.R = args->R_i; b.R_stride = args->R_i_stride; }
+    if (r.R_i) { b.R = r.R_i; b.R_stride = r.R_i_stride; }
     else { b.R = (const char *)a.R + (start * m + start) * es; rpitch = (int)m; }
-    cudaStream_t s = (cudaStream_t)stream;
-    rc = launch_kf_direct_rows(b, (int)m, (int)start, rpitch, args->z_record, s);
-    if (rc == BKE_ERR_UNSUPPORTED) rc = launch_kf_generic_rows(b, (int)m, (int)start, rpitch, args->z_record, s);
+    int rc = launch_kf_direct_rows(b, (int)m, (int)start, rpitch, r.z_record, s);
+    if (rc == BKE_ERR_UNSUPPORTED) rc = launch_kf_generic_rows(b, (int)m, (int)start, rpitch, r.z_record, s);
     return rc;
 }
+
+int bke_kf_update_rows(const bke_kf_rows_args *args, void *stream) { return checked_launch(args, validate_rows, launch_rows, stream); }
 
 size_t bke_kf_sym_models_bytes(int64_t n_filters) { return kf_sym_models_bytes(n_filters); }
 
 int bke_kf_pack_sym_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *Q,
                            const void *R, void *record, int32_t *asymmetric, void *stream)
 {
-    if (n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    if (int rc = check_bank(n_filters)) return rc;
     if (n_filters > 0 && (!Q || !R || !record)) { set_error("Q, R and record must be non-NULL"); return BKE_ERR_BAD_ARG; }
     if (!asymmetric) { set_error("asymmetric must be non-NULL"); return BKE_ERR_BAD_ARG; }
     if (!(dim_x == 4 && dim_z == 2 && dtype == BKE_F32)) {
@@ -521,7 +515,8 @@ int bke_kf_pack_sym_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int3
 
 int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream)
 {
-    int rc = validate_kf(args, true);
+    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    int rc = validate_kf(*args, true);
     if (rc) return rc;
     if (!record) { set_error("record is NULL"); return BKE_ERR_BAD_ARG; }
     if ((rc = require_device())) return rc;
@@ -537,7 +532,7 @@ int bke_kf_step_sym(const bke_kf_args *args, const void *record, void *stream)
 static int validate_models(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dtype, const void *F, const void *Q,
                            const void *H, const void *R)
 {
-    if (n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    if (int rc = check_bank(n_filters)) return rc;
     if (n_filters > 0 && (!F || !Q || !H || !R)) { set_error("F, Q, H and R must be non-NULL"); return BKE_ERR_BAD_ARG; }
     if (!(dim_x == 4 && dim_z == 2 && dtype == BKE_F32)) {
         set_error("packed models exist for dim_x = 4, dim_z = 2, BKE_F32 only");
@@ -582,7 +577,8 @@ static int validate_packed(const void *record, const bke_kf_model_map *host_map)
 
 int bke_kf_step_packed(const bke_kf_args *args, const void *record, const bke_kf_model_map *host_map, void *stream)
 {
-    int rc = validate_kf(args, true);
+    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    int rc = validate_kf(*args, true);
     if (rc) return rc;
     if ((rc = validate_packed(record, host_map))) return rc;
     if ((rc = require_device())) return rc;
@@ -598,7 +594,8 @@ int bke_kf_step_packed(const bke_kf_args *args, const void *record, const bke_kf
 int bke_kf_steps_packed(const bke_kf_args *args, const void *record, const bke_kf_model_map *host_map,
                         const void *const *zs, int32_t n_steps, void *stream)
 {
-    int rc = validate_kf(args, false);
+    if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    int rc = validate_kf(*args, false);
     if (rc) return rc;
     if ((rc = validate_packed(record, host_map))) return rc;
     if (!zs) { set_error("zs is NULL"); return BKE_ERR_BAD_ARG; }
@@ -648,20 +645,20 @@ int bke_capture_node_count(void *stream, int64_t *n_nodes)
     return BKE_OK;
 }
 
+static int validate_kf_batch(const bke_kf_batch_args &a)
+{
+    if (int rc = validate_kf(a.step, false)) return rc;
+    if (a.n_steps < 0) { set_error("n_steps < 0"); return BKE_ERR_BAD_ARG; }
+    if (a.n_steps > 0 && !a.zs) { set_error("zs is NULL"); return BKE_ERR_BAD_ARG; }
+    return BKE_OK;
+}
+
 int bke_kf_batch_filter(const bke_kf_batch_args *args, void *stream)
 {
     if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    bke_kf_args st = args->step;
-    st.flags |= BKE_DO_PREDICT | BKE_DO_UPDATE;
-    int rc = validate_kf(&st, false);
-    if (rc) return rc;
-    if (args->n_steps < 0) { set_error("n_steps < 0"); return BKE_ERR_BAD_ARG; }
-    if (args->n_steps > 0 && !args->zs) { set_error("zs is NULL"); return BKE_ERR_BAD_ARG; }
-    if ((rc = require_device())) return rc;
-    if (st.n_filters == 0) return BKE_OK;
     bke_kf_batch_args a = *args;
-    a.step = st;
-    return launch_kf_batch(a, (cudaStream_t)stream);
+    a.step.flags |= BKE_DO_PREDICT | BKE_DO_UPDATE;
+    return checked_launch(&a, validate_kf_batch, launch_kf_batch, stream);
 }
 
 size_t bke_fls_workspace_bytes(int64_t n_filters, int32_t dim_x, int32_t dim_z, int32_t dim_u, int32_t dtype, int64_t lag)
@@ -669,103 +666,82 @@ size_t bke_fls_workspace_bytes(int64_t n_filters, int32_t dim_x, int32_t dim_z, 
     return fls_workspace_bytes(n_filters, dim_x, dim_z, dim_u, dtype, lag);
 }
 
+static int validate_fls(const bke_fls_args &a)
+{
+    int rc;
+    if ((rc = validate_kf(a.step, false))) return rc;
+    if (a.n_steps < 1) { set_error("n_steps must be 1 or greater"); return BKE_ERR_BAD_ARG; }
+    if (a.lag < 0) { set_error("lag < 0"); return BKE_ERR_BAD_ARG; }
+    if (a.count < 0) { set_error("count < 0"); return BKE_ERR_BAD_ARG; }
+    if (!a.zs) { set_error("zs is NULL"); return BKE_ERR_BAD_ARG; }
+    if (!a.xs_smooth) { set_error("xs_smooth (the history) is NULL"); return BKE_ERR_BAD_ARG; }
+    if (a.us && (rc = check_control(a.step.B, a.us, a.step.dim_u))) return rc;     // us stands in for u
+    return BKE_OK;
+}
+
 int bke_fls_smooth(const bke_fls_args *args, void *stream)
 {
     if (!args) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
-    bke_kf_args st = args->step;
-    st.flags = BKE_DO_PREDICT | BKE_DO_UPDATE;
-    int rc = validate_kf(&st, false);
-    if (rc) return rc;
-    if (args->n_steps < 1) { set_error("n_steps must be 1 or greater"); return BKE_ERR_BAD_ARG; }
-    if (args->lag < 0) { set_error("lag < 0"); return BKE_ERR_BAD_ARG; }
-    if (args->count < 0) { set_error("count < 0"); return BKE_ERR_BAD_ARG; }
-    if (!args->zs) { set_error("zs is NULL"); return BKE_ERR_BAD_ARG; }
-    if (!args->xs_smooth) { set_error("xs_smooth (the history) is NULL"); return BKE_ERR_BAD_ARG; }
-    if (args->us && (!st.B || st.dim_u < 1)) { set_error("a control input needs us, step.B and dim_u >= 1"); return BKE_ERR_BAD_ARG; }
-    if ((rc = require_device())) return rc;
-    if (st.n_filters == 0) return BKE_OK;
     bke_fls_args a = *args;
-    a.step = st;
-    return launch_fls(a, (cudaStream_t)stream);
+    a.step.flags = BKE_DO_PREDICT | BKE_DO_UPDATE;
+    return checked_launch(&a, validate_fls, launch_fls, stream);
 }
 
-int bke_ukf_step(const bke_ukf_args *args, void *stream) { return sigma_step(args, validate_ukf, launch_ukf, stream); }
+int bke_ukf_step(const bke_ukf_args *args, void *stream) { return checked_launch(args, validate_prebuilt<bke_ukf_args, validate_ukf>, launch_ukf, stream); }
 
-int bke_ckf_step(const bke_ckf_args *args, void *stream) { return sigma_step(args, validate_ckf, launch_ckf, stream); }
+int bke_ckf_step(const bke_ckf_args *args, void *stream) { return checked_launch(args, validate_prebuilt<bke_ckf_args, validate_ckf>, launch_ckf, stream); }
 
-int bke_enkf_step(const bke_enkf_args *args, void *stream) { return sigma_step(args, validate_enkf, launch_enkf, stream); }
+int bke_enkf_step(const bke_enkf_args *args, void *stream) { return checked_launch(args, validate_prebuilt<bke_enkf_args, validate_enkf>, launch_enkf, stream); }
 
 int bke_enkf_initialize(int64_t n_filters, int32_t dim_x, int32_t n_members, int32_t dtype, uint32_t seed, uint32_t counter,
                         const void *x, const void *P, void *sigmas, int32_t *status, void *stream)
 {
-    if (n_filters < 0 || dim_x < 1 || dim_x > 16) { set_error("bke_enkf_initialize: n_filters >= 0 and 1 <= dim_x <= 16"); return BKE_ERR_BAD_ARG; }
+    int rc;
+    if ((rc = check_bank(n_filters, dim_x))) return rc;
+    if (dim_x > 16) { set_error("bke_enkf_initialize: 1 <= dim_x <= 16"); return BKE_ERR_BAD_ARG; }
     if (n_members < 2 || n_members > (1 << 24)) { set_error("bke_enkf_initialize: 2 <= n_members <= 2^24"); return BKE_ERR_BAD_ARG; }
-    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if ((rc = check_dtype(dtype))) return rc;
     if (!x || !P || !sigmas) { set_error("x, P and sigmas must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    int rc = require_device();
-    if (rc) return rc;
+    if ((rc = require_device())) return rc;
     if (n_filters == 0) return BKE_OK;
     return launch_enkf_init(n_filters, dim_x, n_members, dtype, seed, counter, x, P, sigmas, status, (cudaStream_t)stream);
 }
 
-int bke_srkf_step(const bke_srkf_args *args, void *stream)
-{
-    int rc = validate_srkf(args);
-    if (rc) return rc;
-    if ((rc = require_device())) return rc;
-    if (args->n_filters == 0) return BKE_OK;
-    return launch_srkf(*args, (cudaStream_t)stream);
-}
+int bke_srkf_step(const bke_srkf_args *args, void *stream) { return checked_launch(args, validate_srkf, launch_srkf, stream); }
 
 int bke_cholesky_lower(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *L,
                        int32_t *status, void *stream)
 {
-    if (n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    int rc;
+    if ((rc = check_bank(n_filters))) return rc;
     if (k < 1) { set_error("k must be 1 or greater"); return BKE_ERR_BAD_ARG; }
-    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
-    if (stride != 0 && stride != (int64_t)k * k) { set_error("stride must be 0 (shared) or k*k"); return BKE_ERR_BAD_ARG; }
+    if ((rc = check_dtype(dtype)) || (rc = check_strides({{stride, (int64_t)k * k}}))) return rc;
     if (n_filters > 0 && (!A || !L)) { set_error("A and L must be non-NULL"); return BKE_ERR_BAD_ARG; }
     if (k > BKE_CHOLESKY_MAX_DIM) {
         set_error("bke_cholesky_lower: k=%d is above BKE_CHOLESKY_MAX_DIM=%d", k, BKE_CHOLESKY_MAX_DIM);
         return BKE_ERR_UNSUPPORTED;
     }
-    int rc = require_device();
-    if (rc) return rc;
+    if ((rc = require_device())) return rc;
     if (n_filters == 0) return BKE_OK;
     return launch_cholesky_lower(n_filters, k, dtype, A, stride, L, status, (cudaStream_t)stream);
 }
 
-int bke_if_step(const bke_if_args *args, void *stream)
-{
-    int rc = validate_if(args);
-    if (rc) return rc;
-    if ((rc = require_device())) return rc;
-    if (args->n_filters == 0) return BKE_OK;
-    return launch_if(*args, (cudaStream_t)stream);
-}
+int bke_if_step(const bke_if_args *args, void *stream) { return checked_launch(args, validate_if, launch_if, stream); }
 
 int bke_inverse(int64_t n_filters, int32_t k, int32_t dtype, const void *A, int64_t stride, void *Ai, int32_t *status,
                 void *stream)
 {
-    if (n_filters < 0) { set_error("n_filters < 0"); return BKE_ERR_BAD_ARG; }
+    int rc;
+    if ((rc = check_bank(n_filters))) return rc;
     if (k < 1) { set_error("k must be 1 or greater"); return BKE_ERR_BAD_ARG; }
-    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
-    if (stride != 0 && stride != (int64_t)k * k) { set_error("stride must be 0 (shared) or k*k"); return BKE_ERR_BAD_ARG; }
+    if ((rc = check_dtype(dtype)) || (rc = check_strides({{stride, (int64_t)k * k}}))) return rc;
     if (n_filters > 0 && (!A || !Ai)) { set_error("A and Ai must be non-NULL"); return BKE_ERR_BAD_ARG; }
-    int rc = require_device();
-    if (rc) return rc;
+    if ((rc = require_device())) return rc;
     if (n_filters == 0) return BKE_OK;
     return launch_inverse(n_filters, k, dtype, A, stride, Ai, status, (cudaStream_t)stream);
 }
 
-int bke_poly_filter(const bke_poly_args *args, void *stream)
-{
-    int rc = validate_poly(args);
-    if (rc) return rc;
-    if ((rc = require_device())) return rc;
-    if (args->n_filters == 0) return BKE_OK;
-    return launch_poly(*args, (cudaStream_t)stream);
-}
+int bke_poly_filter(const bke_poly_args *args, void *stream) { return checked_launch(args, validate_poly, launch_poly, stream); }
 
 int bke_imm_batch_filter(const bke_imm_batch_args *args, void *stream)
 {
@@ -776,13 +752,6 @@ int bke_imm_batch_filter(const bke_imm_batch_args *args, void *stream)
     return launch_imm_batch(*args, (cudaStream_t)stream);
 }
 
-int bke_score_measurements(const bke_score_args *args, void *stream)
-{
-    int rc = validate_score(args);
-    if (rc) return rc;
-    if ((rc = require_device())) return rc;
-    if (args->n_tracks == 0 || args->n_candidates == 0) return BKE_OK;
-    return launch_score(*args, (cudaStream_t)stream);
-}
+int bke_score_measurements(const bke_score_args *args, void *stream) { return checked_launch(args, validate_score, launch_score, stream); }
 
 }  // extern "C"

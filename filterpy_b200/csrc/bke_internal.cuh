@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <initializer_list>
+#include <utility>
 #endif
 #include "../../include/bke.h"
 
@@ -15,6 +17,18 @@ int check_cuda(cudaError_t e, const char *what);
 // sets the kernel's dynamic shared-memory limit to smem bytes and launches it on grid x block threads with
 // the one parameter block *params; `what` names the launch in the error
 int launch_kernel(const void *kern, unsigned grid, unsigned block, size_t smem, void *params, cudaStream_t s, const char *what);
+
+// the argument checks the filter-bank entry points share: each sets the error and returns BKE_ERR_BAD_ARG
+// (require_device: BKE_ERR_CUDA), or BKE_OK
+int require_device();                                    // the engine has no CPU fallback
+int check_dtype(int32_t dtype);                          // BKE_F32 or BKE_F64
+// n >= 0 filters, dim_x >= 1, dim_z >= 1, dim_u >= 0 (the defaults pass); upper bounds are the caller's
+int check_bank(int64_t n, int64_t dim_x = 1, int64_t dim_z = 1, int64_t dim_u = 0);
+int check_predict_update(uint32_t flags);                // flags select predict, update or both
+int check_flag_bits(uint32_t flags, uint32_t allowed);   // no bit outside `allowed`
+// each (stride, dense size): a model stride is 0 (one model shared by the bank) or the dense per-filter size
+int check_strides(std::initializer_list<std::pair<int64_t, int64_t>> strides);
+int check_control(const void *B, const void *u, int64_t dim_u);   // a control input needs B, u and dim_u >= 1
 
 // Number of SMs of the current device (cached).
 int sm_count();
@@ -72,6 +86,8 @@ int launch_fls(const bke_fls_args &a, cudaStream_t s);
 int validate_ukf(const bke_ukf_args &a);
 int validate_ckf(const bke_ckf_args &a);
 int validate_enkf(const bke_enkf_args &a);
+// the UKF smoother's, pre-built or compiled (user_fx: around a user fx, served besides the built-in ones); -1 = go
+int validate_ukf_rts(const bke_ukf_rts_args &a, bool user_fx);
 int launch_ukf(const bke_ukf_args &a, cudaStream_t s);
 int launch_ckf(const bke_ckf_args &a, cudaStream_t s);
 int launch_enkf(const bke_enkf_args &a, cudaStream_t s);

@@ -336,11 +336,11 @@ extern "C" int bke_kf_rts_smoother(const bke_rts_args *args, void *stream)
     const bke_rts_args &a = *args;
     if (a.n_filters < 0 || a.n_steps < 0) { set_error("negative sizes"); return BKE_ERR_BAD_ARG; }
     if (a.dim_x < 1 || a.dim_x > RTS_MAXN) { set_error("bke_kf_rts_smoother: dim_x must be in [1, %d]", RTS_MAXN); return BKE_ERR_UNSUPPORTED; }
-    if (a.dtype != BKE_F32 && a.dtype != BKE_F64) { set_error("bad dtype"); return BKE_ERR_BAD_ARG; }
+    if (int rc = check_dtype(a.dtype)) return rc;
     if (a.model_shift != 0 && a.model_shift != 1) { set_error("model_shift must be 0 or 1"); return BKE_ERR_BAD_ARG; }
     if (a.n_filters == 0 || a.n_steps == 0) return BKE_OK;
     if (!a.Xs || !a.Ps || !a.F || !a.Q || !a.x_out || !a.P_out) { set_error("NULL argument"); return BKE_ERR_BAD_ARG; }
     if (a.F_stride < 0 || a.Q_stride < 0 || a.F_step_stride < 0 || a.Q_step_stride < 0) { set_error("negative stride"); return BKE_ERR_BAD_ARG; }
-    if (bke_device_count() <= 0) { set_error("no CUDA device"); return BKE_ERR_CUDA; }
+    if (int rc = require_device()) return rc;
     return launch_rts(a, (cudaStream_t)stream);
 }

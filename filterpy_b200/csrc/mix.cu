@@ -360,7 +360,7 @@ int validate(const bke_mm_args *args, int op)
     const bke_mm_args &a = *args;
     if (a.n_tracks < 0) { set_error("n_tracks < 0"); return BKE_ERR_BAD_ARG; }
     if (a.n_models < 1 || a.n_models > BKE_MM_MAX_MODELS) { set_error("n_models must be in [1, %d]", BKE_MM_MAX_MODELS); return BKE_ERR_UNSUPPORTED; }
-    if (a.dtype != BKE_F32 && a.dtype != BKE_F64) { set_error("bad dtype"); return BKE_ERR_BAD_ARG; }
+    if (int rc = check_dtype(a.dtype)) return rc;
     if (op != 0 && (a.dim_x < 1 || a.dim_x > 64)) { set_error("dim_x must be in [1, 64]"); return BKE_ERR_BAD_ARG; }
     if (a.n_tracks == 0) return BKE_OK;
     const int M = a.n_models;
@@ -381,7 +381,7 @@ int validate(const bke_mm_args *args, int op)
         if (op == 2 && !a.mu) { set_error("mu is NULL"); return BKE_ERR_BAD_ARG; }
         if (a.weights_stride < 0) { set_error("negative stride"); return BKE_ERR_BAD_ARG; }
     }
-    if (bke_device_count() <= 0) { set_error("no CUDA device"); return BKE_ERR_CUDA; }
+    if (int rc = require_device()) return rc;
     return -1;      // go
 }
 

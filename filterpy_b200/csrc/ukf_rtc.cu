@@ -172,7 +172,7 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
                    : hooks ? (ckf ? "bke_ckf_model_compile_hooks" : "bke_ukf_model_compile_hooks")
                            : enkf ? "bke_enkf_model_compile" : ckf ? "bke_ckf_model_compile" : "bke_ukf_model_compile";
     if (dim_x < 1 || dim_x > 16 || dim_z < 1 || dim_z > dim_x + 8) { set_error("%s: 1 <= dim_x <= 16, 1 <= dim_z", fn); return BKE_ERR_BAD_ARG; }
-    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (int rc = check_dtype(dtype)) return rc;
     const bool ufx = fx_model == BKE_FX_USER, uhx = hx_model == BKE_HX_USER;
     const unsigned all_hooks = BKE_HOOK_X_MEAN | BKE_HOOK_Z_MEAN | BKE_HOOK_RESIDUAL_X | BKE_HOOK_RESIDUAL_Z | BKE_HOOK_STATE_ADD;
     if (hooks) {
@@ -447,11 +447,11 @@ int bke_ukf_rts_smoother_model(const bke_ukf_rts_args *args, const bke_ukf_model
                   model->simplex ? "simplex" : "Merwe", model->simplex ? "Merwe" : "simplex");
         return BKE_ERR_BAD_ARG;
     }
-    if (a.fx_model == BKE_FX_CONST_VEL && (a.dim_x & 1)) { set_error("BKE_FX_CONST_VEL needs an even dim_x"); return BKE_ERR_BAD_ARG; }
-    if (a.fx_model == BKE_FX_LINEAR && (!a.F || a.F_stride < 0)) { set_error("BKE_FX_LINEAR needs F"); return BKE_ERR_BAD_ARG; }
-    if (a.n_filters < 0 || a.n_steps < 0 || fx_args_stride < 0 || a.Q_stride < 0) { set_error("negative sizes"); return BKE_ERR_BAD_ARG; }
-    if (a.n_filters == 0 || a.n_steps == 0) return BKE_OK;
-    if (!a.Xs || !a.Ps || !a.Q || !a.x_out || !a.P_out) { set_error("NULL argument"); return BKE_ERR_BAD_ARG; }
+    // unlike the pre-built smoother, F and the strides are checked for an empty bank too
+    if (a.fx_model == BKE_FX_LINEAR && (!a.F || a.F_stride < 0)) { set_error("BKE_FX_LINEAR needs F and F_stride >= 0"); return BKE_ERR_BAD_ARG; }
+    if (fx_args_stride < 0 || a.Q_stride < 0) { set_error("negative stride"); return BKE_ERR_BAD_ARG; }
+    const int v = validate_ukf_rts(a, model->fx_model == BKE_FX_USER);
+    if (v >= 0) return v;
     void *params[1];
     UrP<float> pf; UrP<double> pd;
     if (a.dtype == BKE_F32) { ukf_rts_fill_params<float>(a, pf); pf.fx_args = (const float *)fx_args; pf.s_fx_args = fx_args_stride; params[0] = &pf; }

@@ -157,10 +157,10 @@ int bke_merwe_sigma_points(int64_t n_filters, int32_t dim_x, int32_t dtype, doub
 {
     (void)beta;
     if (n_filters < 0 || dim_x < 1 || dim_x > 32) { set_error("bad dimensions (1 <= dim_x <= 32)"); return BKE_ERR_BAD_ARG; }
-    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (int rc = check_dtype(dtype)) return rc;
     if (n_filters == 0) return BKE_OK;
     if (!x || !P || !sigmas) { set_error("NULL argument"); return BKE_ERR_BAD_ARG; }
-    if (bke_device_count() <= 0) { set_error("no CUDA device available; the engine has no CPU fallback"); return BKE_ERR_CUDA; }
+    if (int rc = require_device()) return rc;
     return dtype == BKE_F32 ? sigma_t<float>(n_filters, dim_x, alpha, kappa, x, P, sigmas, status, (cudaStream_t)stream)
                             : sigma_t<double>(n_filters, dim_x, alpha, kappa, x, P, sigmas, status, (cudaStream_t)stream);
 }
@@ -169,10 +169,10 @@ int bke_simplex_sigma_points(int64_t n_filters, int32_t dim_x, int32_t dtype, co
                              int32_t *status, void *stream)
 {
     if (n_filters < 0 || dim_x < 1 || dim_x > 32) { set_error("bad dimensions (1 <= dim_x <= 32)"); return BKE_ERR_BAD_ARG; }
-    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (int rc = check_dtype(dtype)) return rc;
     if (n_filters == 0) return BKE_OK;
     if (!x || !P || !sigmas) { set_error("NULL argument"); return BKE_ERR_BAD_ARG; }
-    if (bke_device_count() <= 0) { set_error("no CUDA device available; the engine has no CPU fallback"); return BKE_ERR_CUDA; }
+    if (int rc = require_device()) return rc;
     return dtype == BKE_F32 ? simplex_t<float>(n_filters, dim_x, x, P, sigmas, status, (cudaStream_t)stream)
                             : simplex_t<double>(n_filters, dim_x, x, P, sigmas, status, (cudaStream_t)stream);
 }
@@ -182,10 +182,10 @@ int bke_unscented_transform(int64_t n_filters, int32_t n_sigmas, int32_t dim, in
                             void *x_out, void *P_out, void *stream)
 {
     if (n_filters < 0 || n_sigmas < 1 || dim < 1 || dim > 64 || n_sigmas > 256) { set_error("bad dimensions"); return BKE_ERR_BAD_ARG; }
-    if (dtype != BKE_F32 && dtype != BKE_F64) { set_error("dtype must be BKE_F32 or BKE_F64"); return BKE_ERR_BAD_ARG; }
+    if (int rc = check_dtype(dtype)) return rc;
     if (n_filters == 0) return BKE_OK;
     if (!sigmas || !Wm || !Wc || !x_out || !P_out) { set_error("NULL argument"); return BKE_ERR_BAD_ARG; }
-    if (bke_device_count() <= 0) { set_error("no CUDA device available; the engine has no CPU fallback"); return BKE_ERR_CUDA; }
+    if (int rc = require_device()) return rc;
     return dtype == BKE_F32 ? ut_t<float>(n_filters, n_sigmas, dim, sigmas, Wm, Wc, noise_cov, noise_stride, x_out, P_out, (cudaStream_t)stream)
                             : ut_t<double>(n_filters, n_sigmas, dim, sigmas, Wm, Wc, noise_cov, noise_stride, x_out, P_out, (cudaStream_t)stream);
 }

@@ -142,6 +142,17 @@ def test_a_shape_without_a_fused_instance_is_unsupported(n, m, dtype):
     assert _rc(a) == _lib.BKE_ERR_UNSUPPORTED
 
 
+def test_the_overlap_check_holds_every_array_of_the_largest_bank():
+    """BKE_MM_MAX_MODELS models with zs_valid: the most arrays a call can pass all go through the overlap check.
+    The shape has no fused instance, so no machine launches a kernel."""
+    a, keep = _args(n=5, m=2, M=_lib.BKE_MM_MAX_MODELS)
+    valid = np.ones(3 * 8, np.uint8)
+    a.zs_valid = valid.ctypes.data
+    assert _rc(a) == _lib.BKE_ERR_UNSUPPORTED
+    a.zs_valid = a.means
+    assert _rc(a) == _lib.BKE_ERR_BAD_ARG
+
+
 @pytest.mark.parametrize("field", ["covariances", ("x", 1), ("S", 0)])
 def test_a_misaligned_array_is_unsupported(field):
     a, keep = _args()
