@@ -104,6 +104,20 @@ struct WordPattern {
     static constexpr uint32_t H1(int a) { return (uint32_t)(O >> (W_H + 4 * a)) & 15u; }
     static constexpr bool Q0(int i, int j) { return (Z >> q_word(i, j)) & 1; }
     static constexpr bool R0(int a, int b) { return (Z >> (W_R + a + b)) & 1; }
+    // row a of H is +0 outside block b (A = {0, 1}, B = {2, 3}); the block it touches
+    static constexpr bool h_in(int a, int b) { return (H0(a) & blk_other(2 * b)) == blk_other(2 * b); }
+    static constexpr int HB(int a) { return h_in(a, 0) ? 0 : 1; }
+    // the structural +0 words make F, Q, H and R block-diagonal over A and B: the cross words of F and Q are +0,
+    // each row of H touches one block, the two rows different ones, and R01 is +0.  Such an instance runs a warp
+    // whose filters have zeros in the cross words of P on the two blocks (reg_predict_blk, reg_update_blk).
+    static constexpr bool blocks()
+    {
+        for (int i = 0; i < 4; i++)
+            for (int k = 0; k < 4; k++)
+                if (blk_cross(i, k) && !(((Z >> (W_F + 4 * i + k)) & 1) && Q0(i, k))) return false;
+        const bool rows = (h_in(0, 0) && h_in(1, 1)) || (h_in(0, 1) && h_in(1, 0));
+        return rows && R0(0, 1);
+    }
 };
 // every word as it comes: the generic kernels
 struct NoPattern : WordPattern<0, 0> {};
@@ -518,8 +532,32 @@ kf42_f32_kernel(const __grid_constant__ FastP<4, 2> p)
             }
             // the steps of the ring, back to back on the registers; the loop stays rolled and the
             // measurements rotate through z[0] instead of being indexed
+            // PAT::blocks: a warp whose filters all enter with zeros (of either sign) in the 8 cross words of P runs
+            // the two axis blocks.  They leave every step with zeros there again (reg_update_blk), so the choice
+            // holds for the whole ring.  A lane past the bank's end stores nothing and does not hold its warp back.
+            bool blk = false;
+            if constexpr (PAT::blocks()) {
+                uint32_t c = 0;
+#pragma unroll
+                for (int i = 0; i < N; i++)
+#pragma unroll
+                    for (int j = 0; j < N; j++)
+                        if (blk_cross(i, j)) c |= __float_as_uint(P[i][j]);
+                blk = __all_sync(FULL, !live || (c & 0x7fffffffu) == 0);
+                if (blk) {
 #pragma unroll 1
-            for (int k = 0; k < p.n_steps; k++) {
+                    for (int k = 0; k < p.n_steps; k++) {
+                        reg_predict_blk<PAT, N>(x, P, F, Q, p.alpha_sq);
+                        reg_update_blk<PAT, N, M>(x, P, H, R, z[0]);
+#pragma unroll
+                        for (int j = 0; j + 1 < ZS; j++) { z[j][0] = z[j + 1][0]; z[j][1] = z[j + 1][1]; }
+                    }
+                }
+            }
+            // the steps of the ring, back to back on the registers; the loop stays rolled and the
+            // measurements rotate through z[0] instead of being indexed
+#pragma unroll 1
+            for (int k = 0; k < (blk ? 0 : p.n_steps); k++) {       // (none left after the block path)
                 if (PAT::any) {
                     reg_predict_pat<PAT, N>(x, P, F, Q, p.alpha_sq);
                     reg_update_pat<PAT, N, M>(x, P, H, R, z[0]);
