@@ -111,9 +111,17 @@ def kf_update_bank(x, P, z, H, R, valid=None):
     return dict(x=xn, P=Pn, y=y, K=K, S=S, SI=SI)
 
 
-def kf_step_bank(x, P, z, F, H, Q, R, alpha_sq=1.0, valid=None):
-    """predict + update for a bank; returns dict with priors as well."""
-    xp, Pp = kf_predict_bank(x, P, F, Q, alpha_sq)
+def kf_step_bank(x, P, z, F, H, Q, R, alpha_sq=1.0, valid=None, B=None, u=None, update_first=False):
+    """predict + update for a bank; returns dict with priors as well.  ``B`` [N,n,k] or [n,k] and ``u``
+    [N,k] add the control input to the predict; ``update_first`` runs the update on (x, P) and then the
+    predict on the posterior (batch_filter's update_first order, kalman_filter.py:963-973), and the
+    returned x / P / x_prior / P_prior are that predict's."""
+    if update_first:
+        out = kf_update_bank(x, P, z, H, R, valid)
+        out["x"], out["P"] = kf_predict_bank(out["x"], out["P"], F, Q, alpha_sq, B, u)
+        out["x_prior"], out["P_prior"] = out["x"], out["P"]
+        return out
+    xp, Pp = kf_predict_bank(x, P, F, Q, alpha_sq, B, u)
     out = kf_update_bank(xp, Pp, z, H, R, valid)
     out["x_prior"], out["P_prior"] = xp, Pp
     return out
@@ -183,14 +191,18 @@ def rts_smoother(Xs, Ps, Fs, Qs, shift=1):
 
 
 def rts_smoother_bank(Xs, Ps, F, Q, shift=1):
-    """The same for a bank: Xs (T,N,n), Ps (T,N,n,n), F/Q (n,n) shared, (N,n,n) per filter,
-    (T,n,n) is NOT accepted here (pass lists through rts_smoother per filter)."""
+    """The same for a bank: Xs (T,N,n), Ps (T,N,n,n), F/Q (n,n) shared, (N,n,n) per filter or
+    (T,N,n,n) per epoch and filter; (T,n,n) is NOT accepted here (pass lists through rts_smoother
+    per filter)."""
     T, N, n = Xs.shape
     outs = [np.empty_like(Xs), np.empty_like(Ps), np.empty_like(Ps), np.empty_like(Ps)]
+
+    def models(A, i):
+        if np.ndim(A) == 4:
+            return [A[k, i] for k in range(T)]
+        return [A[i] if np.ndim(A) == 3 else A] * T
     for i in range(N):
-        Fi = F[i] if np.ndim(F) == 3 else F
-        Qi = Q[i] if np.ndim(Q) == 3 else Q
-        r = rts_smoother(Xs[:, i], Ps[:, i], [Fi] * T, [Qi] * T, shift)
+        r = rts_smoother(Xs[:, i], Ps[:, i], models(F, i), models(Q, i), shift)
         for o, v in zip(outs, r):
             o[:, i] = v
     return tuple(outs)

@@ -250,13 +250,24 @@ def test_singular_S_reports_status():
         kf.check()
 
 
-@pytest.mark.parametrize("shape,dtype", [((9, 3), np.float64), ((4, 2), np.float64), ((6, 3), np.float64),
-                                         ((6, 3), np.float32)])
+@pytest.mark.parametrize("shape,dtype", [((9, 3), np.float64), ((6, 3), np.float64)], ids=["shape0-float64", "shape2-float64"])
 @pytest.mark.parametrize("N", [1, 9, 10, 11, 160, 40003])
 def test_rowblock_kernel_vs_oracle(shape, dtype, N):
     """The sub-warp row-block kernel (TMA bulk-staged; config C3's 9/3 fp64 and friends), ragged
     sizes included (the tail shorter than a warp tile runs on the catch-all kernel), with missing
     measurements."""
+    _two_steps_vs_oracle(shape, dtype, N)
+
+
+@pytest.mark.parametrize("shape,dtype", [((4, 2), np.float64), ((6, 3), np.float32)], ids=["shape1-float64", "shape3-float32"])
+@pytest.mark.parametrize("N", [1, 9, 10, 11, 160, 40003])
+def test_direct_kernel_vs_oracle(shape, dtype, N):
+    """The same two steps on shapes of the register-tile kernel kf_direct (4/2 fp64, 6/3 fp32), which takes every
+    call of these shapes whose per-filter arrays are 16-byte aligned."""
+    _two_steps_vs_oracle(shape, dtype, N)
+
+
+def _two_steps_vs_oracle(shape, dtype, N):
     from filterpy_b200.kalman import KalmanFilter
     from filterpy_b200.common import workloads as wl
     from oracle import kf as okf

@@ -41,8 +41,9 @@ def test_tc_predict_vs_fp64(n, N, alpha):
 
 @pytest.mark.parametrize("n,m", [(16, 4), (16, 2), (32, 4), (32, 6)])
 def test_tc_fused_steps_vs_oracle(n, m):
-    """predict on the tensor cores + update on the CUDA cores (row-block update-only instance for 16/4 and 16/2,
-    the catch-all kernel otherwise), three steps with a measurement mask, against the fp64 oracle."""
+    """Shared F, Q, H and R: 16/4, 16/2 and 32/4 run fused on the tensor cores (kf_cov_tc_kernel<NX, dim_z>); 32/6
+    (dim_z > 4) runs its predict there and its update on the catch-all kernel.  Three steps with a measurement mask,
+    against the fp64 oracle."""
     import torch
     from filterpy_b200.kalman import KalmanFilter
     from oracle import kf as okf
