@@ -43,6 +43,20 @@ int sm_count()
     return cached[dev];
 }
 
+int warp_shape(const void *kern, size_t bytes_per_warp, size_t budget, int64_t items, WarpShape &w)
+{
+    int wpb = 4;
+    while (wpb > 1 && bytes_per_warp * wpb > budget) wpb >>= 1;
+    if (bytes_per_warp * wpb > budget) return BKE_ERR_UNSUPPORTED;
+    const size_t smem = bytes_per_warp * wpb;
+    if (smem > 48 * 1024 &&
+        check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute"))
+        return BKE_ERR_CUDA;
+    const int64_t want = (items + wpb - 1) / wpb, cap = (int64_t)sm_count() * 16;
+    w = {wpb, smem, (int)(want < cap ? (want > 0 ? want : 1) : cap)};
+    return BKE_OK;
+}
+
 int require_device()
 {
     int n = 0;

@@ -32,6 +32,18 @@ int check_control(const void *B, const void *u, int64_t dim_u);   // a control i
 
 // Number of SMs of the current device (cached).
 int sm_count();
+
+// Launch shape of a kernel that gives each of `items` one warp and bytes_per_warp of dynamic shared memory:
+// 4 warps per block, or 2 / 1 when their slices exceed `budget` bytes; grid = ceil(items / wpb) blocks, at
+// least 1 and at most 16 per SM.  Raises the kernel's dynamic shared-memory limit when smem > 48 KB.
+// Returns BKE_ERR_UNSUPPORTED, with no error text (the caller names what did not fit), when one warp's
+// slice exceeds the budget.
+struct WarpShape {
+    int wpb;
+    size_t smem;
+    int grid;
+};
+int warp_shape(const void *kern, size_t bytes_per_warp, size_t budget, int64_t items, WarpShape &w);
 #endif
 
 constexpr unsigned FULL = 0xffffffffu;

@@ -16,6 +16,7 @@
 // as P (A^i g) with A = (F - K H)' and g = H' (SI y): 2n^2 FMAs per lag row instead of n^2 m + n^3.
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
+#include "kf_rowio.cuh"
 
 namespace bke {
 namespace {
@@ -31,19 +32,6 @@ struct FlsP {
     int32_t *status;
 };
 
-template <typename T, int CNT>
-__device__ __forceinline__ void load_n(T *dst, const T *src)
-{
-#pragma unroll
-    for (int i = 0; i < CNT; i++) dst[i] = src[i];
-}
-template <typename T, int CNT>
-__device__ __forceinline__ void store_n(T *dst, const T *src)
-{
-#pragma unroll
-    for (int i = 0; i < CNT; i++) dst[i] = src[i];
-}
-
 template <typename T, int N, int M>
 __global__ void __launch_bounds__(FLS_THREADS) fls_fused_kernel(FlsP<T> p)
 {
@@ -57,12 +45,12 @@ __global__ void __launch_bounds__(FLS_THREADS) fls_fused_kernel(FlsP<T> p)
     auto slot = [&](int64_t s, int c) -> T & { return win[((int)s * N + c) * bd + tid]; };
 
     T x[N], P[N][N], F[N][N], Q[N][N], H[M][N], R[M][M];
-    load_n<T, N>(x, p.x + f * N);
-    load_n<T, N * N>(&P[0][0], p.P + f * N * N);
-    load_n<T, N * N>(&F[0][0], p.F + f * p.sF);
-    load_n<T, N * N>(&Q[0][0], p.Q + f * p.sQ);
-    load_n<T, M * N>(&H[0][0], p.H + f * p.sH);
-    load_n<T, M * M>(&R[0][0], p.R + f * p.sR);
+    ld_scalar<T, N>(x, p.x + f * N);
+    ld_scalar<T, N * N>(&P[0][0], p.P + f * N * N);
+    ld_scalar<T, N * N>(&F[0][0], p.F + f * p.sF);
+    ld_scalar<T, N * N>(&Q[0][0], p.Q + f * p.sQ);
+    ld_scalar<T, M * N>(&H[0][0], p.H + f * p.sH);
+    ld_scalar<T, M * M>(&R[0][0], p.R + f * p.sR);
     // the live rows count-N+1 .. count-1 (fixed_lag_smoother.py: rows a later epoch still corrects)
     for (int64_t r = (c0 - L + 1 > 0 ? c0 - L + 1 : 0); r < c0; r++) {
         const T *src = row_ptr(r);
@@ -72,13 +60,13 @@ __global__ void __launch_bounds__(FLS_THREADS) fls_fused_kernel(FlsP<T> p)
     }
     int st = BKE_STATUS_OK;
     T zn[M];
-    load_n<T, M>(zn, p.zs + f * M);
+    ld_scalar<T, M>(zn, p.zs + f * M);
     for (int64_t t = 0; t < p.Tn; t++) {
         const int64_t k = c0 + t;
         T z[M];
 #pragma unroll
         for (int a = 0; a < M; a++) z[a] = zn[a];
-        if (t + 1 < p.Tn) load_n<T, M>(zn, p.zs + ((t + 1) * Nf + f) * M);   // fetched while epoch t computes
+        if (t + 1 < p.Tn) ld_scalar<T, M>(zn, p.zs + ((t + 1) * Nf + f) * M);   // fetched while epoch t computes
         reg_predict<T, N>(x, P, F, Q, T(1));                 // :174-178, no fading factor
         T xp[N];
 #pragma unroll
@@ -86,13 +74,13 @@ __global__ void __launch_bounds__(FLS_THREADS) fls_fused_kernel(FlsP<T> p)
         KfUpdateOut<T, N, M> o;
         reg_update<T, N, M>(x, P, H, R, z, o);               // :181-191; a singular S keeps the prior
         if (!o.ok) st = BKE_STATUS_SINGULAR_S;
-        if (p.xhat) store_n<T, N>(p.xhat + (t * Nf + f) * N, x);
+        if (p.xhat) st_scalar<T, N>(p.xhat + (t * Nf + f) * N, x);
         if (t + 1 == p.Tn) {
-            if (p.y) store_n<T, M>(p.y + f * M, o.y);
-            if (p.S) store_n<T, M * M>(p.S + f * M * M, &o.S[0][0]);
+            if (p.y) st_scalar<T, M>(p.y + f * M, o.y);
+            if (p.S) st_scalar<T, M * M>(p.S + f * M * M, &o.S[0][0]);
         }
         if (L == 0) {                                        // every row is x_pre and nothing is corrected
-            store_n<T, N>(row_ptr(k), xp);
+            st_scalar<T, N>(row_ptr(k), xp);
             continue;
         }
         const int64_t sk = k % L;
@@ -170,8 +158,8 @@ __global__ void __launch_bounds__(FLS_THREADS) fls_fused_kernel(FlsP<T> p)
             for (int c = 0; c < N; c++) dst[c] = slot(s, c);
         }
     }
-    store_n<T, N>(p.x_out + f * N, x);
-    store_n<T, N * N>(p.P_out + f * N * N, &P[0][0]);
+    st_scalar<T, N>(p.x_out + f * N, x);
+    st_scalar<T, N * N>(p.P_out + f * N * N, &P[0][0]);
     if (p.status) p.status[f] = st;
 }
 

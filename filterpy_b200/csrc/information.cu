@@ -546,20 +546,14 @@ int launch_warp(const bke_if_args &a, cudaStream_t s)
     IfP<T> p = params<T>(a);
     const int per_warp = (if_per_warp(a.dim_x, a.dim_z) + 3) & ~3;
     const size_t bytes_per_warp = (size_t)per_warp * sizeof(T), budget = 200 * 1024;
-    int wpb = 4;
-    while (wpb > 1 && bytes_per_warp * wpb > budget) wpb >>= 1;
-    if (bytes_per_warp * wpb > budget) {
-        set_error("bke_if_step: dim_x=%d dim_z=%d needs %zu B of shared memory per filter (> %zu)", a.dim_x, a.dim_z,
-                  bytes_per_warp, budget);
-        return BKE_ERR_UNSUPPORTED;
+    WarpShape w;
+    if (int rc = warp_shape((const void *)if_warp_kernel<T>, bytes_per_warp, budget, p.N, w)) {
+        if (rc == BKE_ERR_UNSUPPORTED)
+            set_error("bke_if_step: dim_x=%d dim_z=%d needs %zu B of shared memory per filter (> %zu)", a.dim_x, a.dim_z,
+                      bytes_per_warp, budget);
+        return rc;
     }
-    const size_t smem = bytes_per_warp * wpb;
-    if (smem > 48 * 1024 &&
-        check_cuda(cudaFuncSetAttribute(if_warp_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute"))
-        return BKE_ERR_CUDA;
-    const int64_t want = (p.N + wpb - 1) / wpb, cap = (int64_t)sm_count() * 16;
-    const int grid = (int)(want < cap ? (want > 0 ? want : 1) : cap);
-    if_warp_kernel<T><<<grid, wpb * 32, smem, s>>>(p, per_warp);
+    if_warp_kernel<T><<<w.grid, w.wpb * 32, w.smem, s>>>(p, per_warp);
     return check_cuda(cudaGetLastError(), "if_warp_kernel launch");
 }
 
@@ -610,19 +604,13 @@ int launch_inv(int64_t N, int k, const void *A, int64_t stride, void *Ai, int32_
 {
     const int per_warp = (2 * k * k + k + 3) & ~3;
     const size_t bytes_per_warp = (size_t)per_warp * sizeof(T), budget = 200 * 1024;
-    int wpb = 4;
-    while (wpb > 1 && bytes_per_warp * wpb > budget) wpb >>= 1;
-    if (bytes_per_warp * wpb > budget) {
-        set_error("bke_inverse: k=%d needs %zu B of shared memory per matrix (> %zu)", k, bytes_per_warp, budget);
-        return BKE_ERR_UNSUPPORTED;
+    WarpShape w;
+    if (int rc = warp_shape((const void *)inverse_kernel<T>, bytes_per_warp, budget, N, w)) {
+        if (rc == BKE_ERR_UNSUPPORTED)
+            set_error("bke_inverse: k=%d needs %zu B of shared memory per matrix (> %zu)", k, bytes_per_warp, budget);
+        return rc;
     }
-    const size_t smem = bytes_per_warp * wpb;
-    if (smem > 48 * 1024 &&
-        check_cuda(cudaFuncSetAttribute(inverse_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute"))
-        return BKE_ERR_CUDA;
-    const int64_t want = (N + wpb - 1) / wpb, cap = (int64_t)sm_count() * 16;
-    const int grid = (int)(want < cap ? (want > 0 ? want : 1) : cap);
-    inverse_kernel<T><<<grid, wpb * 32, smem, s>>>(N, k, (const T *)A, stride, (T *)Ai, status, per_warp);
+    inverse_kernel<T><<<w.grid, w.wpb * 32, w.smem, s>>>(N, k, (const T *)A, stride, (T *)Ai, status, per_warp);
     return check_cuda(cudaGetLastError(), "inverse_kernel launch");
 }
 

@@ -13,9 +13,9 @@
 // Shapes without a register-tiled instantiation fall back to looping bke_kf_step on the host
 // (still on the GPU, one launch per epoch).
 #include <stdlib.h>
-#include <type_traits>
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
+#include "kf_rowio.cuh"
 #include "ptx.cuh"
 
 namespace bke {
@@ -32,26 +32,6 @@ struct BatchP {
     T *x_out, *P_out, *means, *covs, *means_p, *covs_p;
     int32_t *status;
 };
-
-template <typename T, int CNT>
-__device__ __forceinline__ void load_vec(T *dst, const T *src)
-{
-#pragma unroll
-    for (int i = 0; i < CNT; i++) dst[i] = src[i];
-}
-template <typename T, int CNT>
-__device__ __forceinline__ void store_vec(T *dst, const T *src)
-{
-    constexpr int VEC = 16 / sizeof(T);
-    if constexpr (CNT % VEC == 0) {
-        using V = typename std::conditional<sizeof(T) == 4, float4, double2>::type;
-#pragma unroll
-        for (int i = 0; i < CNT / VEC; i++) reinterpret_cast<V *>(dst)[i] = *reinterpret_cast<const V *>(src + i * VEC);
-    } else {
-#pragma unroll
-        for (int i = 0; i < CNT; i++) dst[i] = src[i];
-    }
-}
 
 // per-warp staging of one epoch's outputs: [means_p | covs_p | means | covs], each 32 filters deep
 template <typename T, int N>
@@ -75,19 +55,19 @@ __global__ void __launch_bounds__(128) kf_batch_kernel(BatchP<T> p)
     unsigned char *wst = bsm + (size_t)(threadIdx.x >> 5) * 2 * St::BYTES;
     if (f >= p.N) return;
     T x[N], P[N][N], F[N][N], Q[N][N], H[M][N], R[M][M];
-    load_vec<T, N>(x, p.x + f * N);
-    load_vec<T, N * N>(&P[0][0], p.P + f * N * N);
-    load_vec<T, N * N>(&F[0][0], p.F + f * p.sF);
-    load_vec<T, N * N>(&Q[0][0], p.Q + f * p.sQ);
-    load_vec<T, M * N>(&H[0][0], p.H + f * p.sH);
-    load_vec<T, M * M>(&R[0][0], p.R + f * p.sR);
+    ld_scalar<T, N>(x, p.x + f * N);
+    ld_scalar<T, N * N>(&P[0][0], p.P + f * N * N);
+    ld_scalar<T, N * N>(&F[0][0], p.F + f * p.sF);
+    ld_scalar<T, N * N>(&Q[0][0], p.Q + f * p.sQ);
+    ld_scalar<T, M * N>(&H[0][0], p.H + f * p.sH);
+    ld_scalar<T, M * M>(&R[0][0], p.R + f * p.sR);
     int st = BKE_STATUS_OK;
     // the measurement of epoch t+1 is fetched while epoch t computes: one exposed DRAM latency per
     // epoch was the dominant stall of the first version (long_scoreboard 7 per issue)
     T zn[M];
     bool has_zn = true;
     if (p.Tn > 0) {
-        load_vec<T, M>(zn, p.zs + f * M);
+        ld_scalar<T, M>(zn, p.zs + f * M);
         has_zn = p.valid == nullptr || p.valid[f] != 0;
     }
     for (int64_t t = 0; t < p.Tn; t++) {
@@ -102,7 +82,7 @@ __global__ void __launch_bounds__(128) kf_batch_kernel(BatchP<T> p)
         for (int a = 0; a < M; a++) z[a] = zn[a];
         const bool has_z = has_zn;
         if (t + 1 < p.Tn) {
-            load_vec<T, M>(zn, p.zs + (tf + p.N) * M);
+            ld_scalar<T, M>(zn, p.zs + (tf + p.N) * M);
             has_zn = p.valid == nullptr || p.valid[tf + p.N] != 0;
         }
         auto upd = [&]() {
@@ -112,21 +92,21 @@ __global__ void __launch_bounds__(128) kf_batch_kernel(BatchP<T> p)
                 if (!o.ok) st = BKE_STATUS_SINGULAR_S;
             }
             if (staged) {
-                store_vec<T, N>(reinterpret_cast<T *>(buf + St::O_X) + lane * N, x);
-                store_vec<T, N * N>(reinterpret_cast<T *>(buf + St::O_P) + lane * N * N, &P[0][0]);
+                stv<T, N>(reinterpret_cast<T *>(buf + St::O_X) + lane * N, x);
+                stv<T, N * N>(reinterpret_cast<T *>(buf + St::O_P) + lane * N * N, &P[0][0]);
             } else {
-                if (p.means) store_vec<T, N>(p.means + tf * N, x);
-                if (p.covs) store_vec<T, N * N>(p.covs + tf * N * N, &P[0][0]);
+                if (p.means) stv<T, N>(p.means + tf * N, x);
+                if (p.covs) stv<T, N * N>(p.covs + tf * N * N, &P[0][0]);
             }
         };
         auto pred = [&]() {
             reg_predict<T, N>(x, P, F, Q, p.alpha_sq);
             if (staged) {
-                store_vec<T, N>(reinterpret_cast<T *>(buf + St::O_XP) + lane * N, x);
-                store_vec<T, N * N>(reinterpret_cast<T *>(buf + St::O_PP) + lane * N * N, &P[0][0]);
+                stv<T, N>(reinterpret_cast<T *>(buf + St::O_XP) + lane * N, x);
+                stv<T, N * N>(reinterpret_cast<T *>(buf + St::O_PP) + lane * N * N, &P[0][0]);
             } else {
-                if (p.means_p) store_vec<T, N>(p.means_p + tf * N, x);
-                if (p.covs_p) store_vec<T, N * N>(p.covs_p + tf * N * N, &P[0][0]);
+                if (p.means_p) stv<T, N>(p.means_p + tf * N, x);
+                if (p.covs_p) stv<T, N * N>(p.covs_p + tf * N * N, &P[0][0]);
             }
         };
         if (p.update_first) { upd(); pred(); } else { pred(); upd(); }
@@ -144,8 +124,8 @@ __global__ void __launch_bounds__(128) kf_batch_kernel(BatchP<T> p)
         }
     }
     if (staged && lane == 0) bulk_wait_all();
-    store_vec<T, N>(p.x_out + f * N, x);
-    store_vec<T, N * N>(p.P_out + f * N * N, &P[0][0]);
+    stv<T, N>(p.x_out + f * N, x);
+    stv<T, N * N>(p.P_out + f * N * N, &P[0][0]);
     if (p.status) p.status[f] = st;
 }
 

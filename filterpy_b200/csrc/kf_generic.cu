@@ -284,20 +284,14 @@ int launch_t(const bke_kf_args &a, cudaStream_t s, const KfP<T> *form = nullptr)
     // layout must match the kernel: x, xp, P, F, T1, T2, H, PHT, K, R, S, SI, SA, y, col (, Mc, G)
     int per_warp = 2 * n + 4 * (n * n) + 3 * (n * m) + 4 * (m * m) + 2 * m + (FORM == FORM_CORRELATED ? 2 * n * m : 0);
     per_warp = (per_warp + 3) & ~3;
-    size_t bytes_per_warp = (size_t)per_warp * sizeof(T);
-    int wpb = 4;
-    const size_t budget = 200 * 1024;
-    while (wpb > 1 && bytes_per_warp * wpb > budget) wpb >>= 1;
-    if (bytes_per_warp * wpb > budget) { set_error("bke_kf_step: dim_x=%d dim_z=%d needs %zu B of shared memory per filter (> %zu)", n, m, bytes_per_warp, budget); return BKE_ERR_UNSUPPORTED; }
-    size_t smem = bytes_per_warp * wpb;
-    if (smem > 48 * 1024) {
-        if (check_cuda(cudaFuncSetAttribute(kf_generic_kernel<T, FORM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
+    const size_t bytes_per_warp = (size_t)per_warp * sizeof(T), budget = 200 * 1024;
+    WarpShape w;
+    if (int rc = warp_shape((const void *)kf_generic_kernel<T, FORM>, bytes_per_warp, budget, p.N, w)) {
+        if (rc == BKE_ERR_UNSUPPORTED)
+            set_error("bke_kf_step: dim_x=%d dim_z=%d needs %zu B of shared memory per filter (> %zu)", n, m, bytes_per_warp, budget);
+        return rc;
     }
-    int64_t want = (p.N + wpb - 1) / wpb;
-    int64_t cap = (int64_t)sm_count() * 16;
-    int grid = (int)(want < cap ? want : cap);
-    if (grid < 1) grid = 1;
-    kf_generic_kernel<T, FORM><<<grid, wpb * 32, smem, s>>>(p, per_warp);
+    kf_generic_kernel<T, FORM><<<w.grid, w.wpb * 32, w.smem, s>>>(p, per_warp);
     return check_cuda(cudaGetLastError(), "kf_generic_kernel launch");
 }
 

@@ -1,6 +1,6 @@
-// Thread-per-filter row loads and stores of the register-tile kernels (kf_direct.cu, srkf.cu): every
-// thread reads its own rows of the AoS arrays with 16-byte accesses when a row is a whole number of
-// 16-byte vectors, so every fetched sector is used.
+// Thread-per-filter row loads and stores of the register-tile kernels: every thread reads its own rows
+// of the AoS arrays with 16-byte accesses when a row is a whole number of 16-byte vectors, so every
+// fetched sector is used.
 #pragma once
 #include <type_traits>
 #include "bke_internal.cuh"
@@ -47,6 +47,20 @@ __device__ __forceinline__ void stv(T *dst, const T *src)
 #pragma unroll
         for (int i = 0; i < CNT; i++) dst[i] = src[i];
     }
+}
+
+// element by element, for rows with no 16-byte alignment guarantee
+template <typename T, int CNT>
+__device__ __forceinline__ void ld_scalar(T *dst, const T *src)
+{
+#pragma unroll
+    for (int i = 0; i < CNT; i++) dst[i] = src[i];
+}
+template <typename T, int CNT>
+__device__ __forceinline__ void st_scalar(T *dst, const T *src)
+{
+#pragma unroll
+    for (int i = 0; i < CNT; i++) dst[i] = src[i];
 }
 
 // 16-byte vector accesses are used for the arrays whose row is a multiple of 16 bytes: their base

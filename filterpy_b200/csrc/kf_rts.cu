@@ -12,9 +12,9 @@
 // consecutive threads = consecutive filters read consecutive rows).  One thread owns one filter and
 // carries the smoothed (x, P) of epoch k+1 in registers; per filter-step it reads x[k], P[k] and
 // writes x, P, K, Pp: (2n + 4n^2) scalars = 288 B at n = 4 fp32.
-#include <type_traits>
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
+#include "kf_rowio.cuh"
 
 namespace bke {
 namespace {
@@ -30,33 +30,6 @@ struct RtsP {
     int32_t *status;
 };
 
-template <typename T, int CNT>
-__device__ __forceinline__ void ld(T *dst, const T *src)
-{
-    constexpr int VEC = 16 / sizeof(T);
-    if constexpr (CNT % VEC == 0) {
-        using V = typename std::conditional<sizeof(T) == 4, float4, double2>::type;
-#pragma unroll
-        for (int i = 0; i < CNT / VEC; i++) *reinterpret_cast<V *>(dst + i * VEC) = reinterpret_cast<const V *>(src)[i];
-    } else {
-#pragma unroll
-        for (int i = 0; i < CNT; i++) dst[i] = src[i];
-    }
-}
-template <typename T, int CNT>
-__device__ __forceinline__ void st(T *dst, const T *src)
-{
-    constexpr int VEC = 16 / sizeof(T);
-    if constexpr (CNT % VEC == 0) {
-        using V = typename std::conditional<sizeof(T) == 4, float4, double2>::type;
-#pragma unroll
-        for (int i = 0; i < CNT / VEC; i++) reinterpret_cast<V *>(dst)[i] = *reinterpret_cast<const V *>(src + i * VEC);
-    } else {
-#pragma unroll
-        for (int i = 0; i < CNT; i++) dst[i] = src[i];
-    }
-}
-
 // time-constant models, everything in registers
 template <typename T, int N>
 __global__ void __launch_bounds__(128) rts_reg_kernel(RtsP<T> p)
@@ -67,38 +40,38 @@ __global__ void __launch_bounds__(128) rts_reg_kernel(RtsP<T> p)
     // ~290, so Q is re-read every epoch (an L1 hit) and nothing is prefetched
     constexpr bool LEAN = sizeof(T) == 8 && N >= 4;
     T F[N][N], Q[N][N];
-    ld<T, N * N>(&F[0][0], p.F + f * p.sF);
-    if constexpr (!LEAN) ld<T, N * N>(&Q[0][0], p.Q + f * p.sQ);
+    ldv_rw<T, N * N>(&F[0][0], p.F + f * p.sF);
+    if constexpr (!LEAN) ldv_rw<T, N * N>(&Q[0][0], p.Q + f * p.sQ);
     T xs[N], Ps[N][N];                                  // smoothed state of epoch k+1
     int64_t tf = (p.Tn - 1) * p.N + f;
-    ld<T, N>(xs, p.Xs + tf * N);
-    ld<T, N * N>(&Ps[0][0], p.Ps + tf * N * N);
-    st<T, N>(p.x_out + tf * N, xs);
-    st<T, N * N>(p.P_out + tf * N * N, &Ps[0][0]);
-    if (p.Pp) st<T, N * N>(p.Pp + tf * N * N, &Ps[0][0]);      // Pp = Ps.copy() (:1065)
+    ldv_rw<T, N>(xs, p.Xs + tf * N);
+    ldv_rw<T, N * N>(&Ps[0][0], p.Ps + tf * N * N);
+    stv<T, N>(p.x_out + tf * N, xs);
+    stv<T, N * N>(p.P_out + tf * N * N, &Ps[0][0]);
+    if (p.Pp) stv<T, N * N>(p.Pp + tf * N * N, &Ps[0][0]);      // Pp = Ps.copy() (:1065)
     if (p.K) {
         T Z[N * N];
 #pragma unroll
         for (int i = 0; i < N * N; i++) Z[i] = T(0);
-        st<T, N * N>(p.K + tf * N * N, Z);
+        stv<T, N * N>(p.K + tf * N * N, Z);
     }
     int stt = BKE_STATUS_OK;
     T xk[N], Pk[N][N];
     if (p.Tn > 1) {
         tf -= p.N;
-        ld<T, N>(xk, p.Xs + tf * N);
-        ld<T, N * N>(&Pk[0][0], p.Ps + tf * N * N);
+        ldv_rw<T, N>(xk, p.Xs + tf * N);
+        ldv_rw<T, N * N>(&Pk[0][0], p.Ps + tf * N * N);
     }
     for (int64_t k = p.Tn - 2; k >= 0; k--) {
         // prefetch epoch k-1 while epoch k computes
         T xn[N], Pn[N][N];
         if constexpr (!LEAN) {
             if (k > 0) {
-                ld<T, N>(xn, p.Xs + (tf - p.N) * N);
-                ld<T, N * N>(&Pn[0][0], p.Ps + (tf - p.N) * N * N);
+                ldv_rw<T, N>(xn, p.Xs + (tf - p.N) * N);
+                ldv_rw<T, N * N>(&Pn[0][0], p.Ps + (tf - p.N) * N * N);
             }
         } else {
-            ld<T, N * N>(&Q[0][0], p.Q + f * p.sQ);
+            ldv_rw<T, N * N>(&Q[0][0], p.Q + f * p.sQ);
         }
         T FP[N][N], Pp[N][N], PFt[N][N];
 #pragma unroll
@@ -168,10 +141,10 @@ __global__ void __launch_bounds__(128) rts_reg_kernel(RtsP<T> p)
                 for (int q = 1; q < N; q++) s += KD[i][q] * K[j][q];
                 Pk[i][j] += s;
             }
-        st<T, N>(p.x_out + tf * N, xk);
-        st<T, N * N>(p.P_out + tf * N * N, &Pk[0][0]);
-        if (p.K) st<T, N * N>(p.K + tf * N * N, &K[0][0]);
-        if (p.Pp) st<T, N * N>(p.Pp + tf * N * N, &Pp[0][0]);
+        stv<T, N>(p.x_out + tf * N, xk);
+        stv<T, N * N>(p.P_out + tf * N * N, &Pk[0][0]);
+        if (p.K) stv<T, N * N>(p.K + tf * N * N, &K[0][0]);
+        if (p.Pp) stv<T, N * N>(p.Pp + tf * N * N, &Pp[0][0]);
 #pragma unroll
         for (int i = 0; i < N; i++) {
             xs[i] = xk[i];
@@ -187,8 +160,8 @@ __global__ void __launch_bounds__(128) rts_reg_kernel(RtsP<T> p)
                 for (int j = 0; j < N; j++) Pk[i][j] = Pn[i][j];
             }
         } else if (k > 0) {
-            ld<T, N>(xk, p.Xs + tf * N);
-            ld<T, N * N>(&Pk[0][0], p.Ps + tf * N * N);
+            ldv_rw<T, N>(xk, p.Xs + tf * N);
+            ldv_rw<T, N * N>(&Pk[0][0], p.Ps + tf * N * N);
         }
     }
     if (p.status) p.status[f] = stt;

@@ -16,8 +16,8 @@
 // omega) are re-read by the threads of a track from L1.  All HBM-bound: per track the mix reads and
 // writes M (n + n^2) scalars.
 #include <float.h>
-#include <type_traits>
 #include "bke_internal.cuh"
+#include "kf_rowio.cuh"
 
 namespace bke {
 namespace {
@@ -163,33 +163,6 @@ __global__ void __launch_bounds__(256) k_mm_estimate(MixP<T> p)
 // loads each model's whole x and row r of its P with 16-byte loads, forms the mixed mean once and
 // writes row r of every output covariance (plus element r of the mean): no redundant work across
 // the threads of a row, a quarter of the threads of the element-parallel form.
-template <typename T, int CNT>
-__device__ __forceinline__ void ld_row(T *dst, const T *src)
-{
-    constexpr int VEC = 16 / sizeof(T);
-    if constexpr (CNT % VEC == 0) {
-        using V = typename std::conditional<sizeof(T) == 4, float4, double2>::type;
-#pragma unroll
-        for (int i = 0; i < CNT / VEC; i++) *reinterpret_cast<V *>(dst + i * VEC) = __ldg(reinterpret_cast<const V *>(src) + i);
-    } else {
-#pragma unroll
-        for (int i = 0; i < CNT; i++) dst[i] = __ldg(src + i);
-    }
-}
-template <typename T, int CNT>
-__device__ __forceinline__ void st_row(T *dst, const T *src)
-{
-    constexpr int VEC = 16 / sizeof(T);
-    if constexpr (CNT % VEC == 0) {
-        using V = typename std::conditional<sizeof(T) == 4, float4, double2>::type;
-#pragma unroll
-        for (int i = 0; i < CNT / VEC; i++) reinterpret_cast<V *>(dst)[i] = *reinterpret_cast<const V *>(src + i * VEC);
-    } else {
-#pragma unroll
-        for (int i = 0; i < CNT; i++) dst[i] = src[i];
-    }
-}
-
 // MIX = true: IMM.py:201-213 for every target model; MIX = false: IMM.py:228-237 (one output)
 template <typename T, int NX, int MM, bool MIX>
 __global__ void __launch_bounds__(256) k_mm_rows(MixP<T> p)
@@ -201,8 +174,8 @@ __global__ void __launch_bounds__(256) k_mm_rows(MixP<T> p)
         T xv[MM][NX], Pr[MM][NX];
 #pragma unroll
         for (int j = 0; j < MM; j++) {
-            ld_row<T, NX>(xv[j], p.x[j] + t * NX);
-            ld_row<T, NX>(Pr[j], p.P[j] + g * NX);
+            ldv<T, NX>(xv[j], p.x[j] + t * NX);
+            ldv<T, NX>(Pr[j], p.P[j] + g * NX);
         }
         const double *wd = p.w + t * p.sw;
         constexpr int OUTS = MIX ? MM : 1;
@@ -236,7 +209,7 @@ __global__ void __launch_bounds__(256) k_mm_rows(MixP<T> p)
                 for (int j = 0; j < MM; j++) sacc += w[j] * (xr[j] * (xv[j][c] - m[c]) + Pr[j][c]);
                 out[c] = sacc;
             }
-            st_row<T, NX>(p.Po[i] + g * NX, out);
+            stv<T, NX>(p.Po[i] + g * NX, out);
             p.xo[i][g] = mr;
         }
     }

@@ -389,19 +389,13 @@ int launch_warp(const bke_srkf_args &a, cudaStream_t s)
     int per_warp = 2 * n + m + nn + (nn > nm ? nn : nm) + 2 * nm + 2 * m * m + (2 * nn > D * D ? 2 * nn : D * D);
     per_warp = (per_warp + 3) & ~3;
     const size_t bytes_per_warp = (size_t)per_warp * sizeof(T), budget = 200 * 1024;
-    int wpb = 4;
-    while (wpb > 1 && bytes_per_warp * wpb > budget) wpb >>= 1;
-    if (bytes_per_warp * wpb > budget) {
-        set_error("bke_srkf_step: dim_x=%d dim_z=%d needs %zu B of shared memory per filter (> %zu)", n, m, bytes_per_warp, budget);
-        return BKE_ERR_UNSUPPORTED;
+    WarpShape w;
+    if (int rc = warp_shape((const void *)srkf_warp_kernel<T>, bytes_per_warp, budget, p.N, w)) {
+        if (rc == BKE_ERR_UNSUPPORTED)
+            set_error("bke_srkf_step: dim_x=%d dim_z=%d needs %zu B of shared memory per filter (> %zu)", n, m, bytes_per_warp, budget);
+        return rc;
     }
-    const size_t smem = bytes_per_warp * wpb;
-    if (smem > 48 * 1024 &&
-        check_cuda(cudaFuncSetAttribute(srkf_warp_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute"))
-        return BKE_ERR_CUDA;
-    const int64_t want = (p.N + wpb - 1) / wpb, cap = (int64_t)sm_count() * 16;
-    const int grid = (int)(want < cap ? (want > 0 ? want : 1) : cap);
-    srkf_warp_kernel<T><<<grid, wpb * 32, smem, s>>>(p, per_warp);
+    srkf_warp_kernel<T><<<w.grid, w.wpb * 32, w.smem, s>>>(p, per_warp);
     return check_cuda(cudaGetLastError(), "srkf_warp_kernel launch");
 }
 

@@ -126,22 +126,21 @@ template <typename T>
 int ut_t(int64_t N, int ns, int n, const void *sig, const void *Wm, const void *Wc, const void *noise, int64_t nstride,
          void *x_out, void *P_out, cudaStream_t s)
 {
-    // 4 warps per block, or 2 / 1 when their slices exceed the device's opt-in shared memory per block:
-    // one warp's slice (at most 8 * (256 * 64 + 64) B = 131,584 B) always fits an H100's 227 KB
+    // the budget is the device's opt-in shared memory per block: one warp's slice (at most
+    // 8 * (256 * 64 + 64) B = 131,584 B) always fits an H100's 227 KB
     const size_t per_warp = sizeof(T) * (size_t)(ns * n + n);
     int dev = 0, optin = 0;
     if (check_cuda(cudaGetDevice(&dev), "cudaGetDevice") ||
         check_cuda(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev), "cudaDeviceGetAttribute"))
         return BKE_ERR_CUDA;
-    int wpb = 4;
-    while (wpb > 1 && per_warp * wpb > (size_t)optin) wpb >>= 1;
-    const size_t smem = per_warp * wpb;
-    if (smem > 48 * 1024) {
-        if (check_cuda(cudaFuncSetAttribute(k_unscented_transform<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) return BKE_ERR_CUDA;
+    WarpShape w;
+    if (int rc = warp_shape((const void *)k_unscented_transform<T>, per_warp, (size_t)optin, N, w)) {
+        if (rc == BKE_ERR_UNSUPPORTED)
+            set_error("bke_unscented_transform: n_sigmas=%d dim=%d needs %zu B of shared memory per filter (> %d)", ns, n, per_warp, optin);
+        return rc;
     }
-    int64_t grid = (N + wpb - 1) / wpb, cap = (int64_t)sm_count() * 16;
-    k_unscented_transform<T><<<(unsigned)(grid < cap ? grid : cap), 32 * wpb, smem, s>>>(N, ns, n, (const T *)sig, (const T *)Wm, (const T *)Wc,
-                                                                                       (const T *)noise, nstride, (T *)x_out, (T *)P_out);
+    k_unscented_transform<T><<<w.grid, 32 * w.wpb, w.smem, s>>>(N, ns, n, (const T *)sig, (const T *)Wm, (const T *)Wc,
+                                                              (const T *)noise, nstride, (T *)x_out, (T *)P_out);
     return check_cuda(cudaGetLastError(), "k_unscented_transform launch");
 }
 
