@@ -70,6 +70,12 @@ def dgeqr2_pivot_ratio(A):
     norm = sqrt(alpha^2 + |sub|^2) (1.0 when it applies none).  Near 0, a rounding difference can flip the sign
     of a row of R: alpha near 0 changes the sign of beta, and a sub-column of rounding noise decides between a
     reflection (which negates the row) and none."""
+    ra, rs = _dgeqr2(A)[1:]
+    return float(np.min(ra)), float(np.min(rs))
+
+
+def dgeqr2_pivot_ratios(A):
+    """dgeqr2_pivot_ratio per matrix: two arrays of the leading shape of A[..., r, c]."""
     return _dgeqr2(A)[1:]
 
 
@@ -77,16 +83,16 @@ def _dgeqr2(A):
     A = np.array(A, copy=True)
     rows, cols = A.shape[-2:]
     one = A.dtype.type(1)
-    ra = rs = 1.0
+    ra, rs = np.ones(A.shape[:-2]), np.ones(A.shape[:-2])
     for j in range(min(rows - 1, cols)):
         sub = A[..., j + 1:, j]
         ss = np.sum(sub * sub, axis=-1)
         act = ss != 0
         alpha = A[..., j, j]
-        if np.any(act):
-            nrm = np.sqrt(alpha * alpha + ss)[act]
-            ra = min(ra, float((np.abs(alpha[act]) / nrm).min()))
-            rs = min(rs, float((np.sqrt(ss[act]) / nrm).min()))
+        with np.errstate(divide="ignore", invalid="ignore"):
+            nrm = np.sqrt(alpha * alpha + ss)
+            ra = np.where(act, np.minimum(ra, np.abs(alpha) / nrm), ra)
+            rs = np.where(act, np.minimum(rs, np.sqrt(ss) / nrm), rs)
         beta = -np.copysign(np.sqrt(alpha * alpha + ss), alpha)
         with np.errstate(divide="ignore", invalid="ignore"):
             tau = np.where(act, (beta - alpha) / beta, 0)

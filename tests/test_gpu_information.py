@@ -1,7 +1,6 @@
-"""GPU: InformationFilter banks on every register-tile instance and on the warp-per-filter kernel, in fp32 and
-fp64, against the reference's golden vectors and the fp64 oracle; both branches in one warp, valid, shared and
-per-filter models, status and BKE_STATUS_STICKY, fused against split launches, single mode's exceptions and the
-torch op."""
+"""GPU: InformationFilter banks, in fp32 and fp64, against the reference's golden vectors; status and
+BKE_STATUS_STICKY through the mirror, fused against split launches, single mode's exceptions and the torch op.
+Every kernel instance against the fp64 oracle: test_gpu_if_instances."""
 
 import numpy as np
 import pytest
@@ -10,14 +9,11 @@ import torch
 from filterpy_b200 import _lib
 from filterpy_b200.kalman import InformationFilter
 
-import information_oracle as io
-from test_oracle_information import GOLDEN, STEPS, ll_mode
+from test_oracle_information import GOLDEN, STEPS
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 TOL = {np.float64: 1e-6, np.float32: 1e-3}
-# the register tiles (kf_direct.cu's shapes); 6/3 is a register tile in fp32 and the warp kernel in fp64
-TILES = [(1, 1), (2, 1), (2, 2), (3, 1), (4, 1), (4, 2), (4, 4), (6, 3)]
 DIVERGING = "if_noinfo_4_2"           # x grows about tenfold per step: fp32 is held to the branch only
 
 
@@ -166,7 +162,7 @@ def test_single_mode_attributes():
 
 
 # ---------------------------------------------------------------------------------------------- random banks
-def _random(N, n, m, seed, shared=False, ni_frac=0.3, du=0):
+def _random(N, n, m, seed, shared=False, ni_frac=0.3):
     rng = np.random.default_rng(seed)
     F = np.eye(n) + 0.1 * rng.standard_normal((N, n, n))
     H = np.eye(m, n) + 0.3 * rng.standard_normal((N, m, n))     # H' H well conditioned where m >= n
@@ -184,49 +180,7 @@ def _random(N, n, m, seed, shared=False, ni_frac=0.3, du=0):
     g = dict(x=rng.standard_normal((N, n)), P_inv=P_inv, F=F, H=H, Q=Q, R_inv=np.linalg.inv(R),
              zs=rng.standard_normal((4, N, m)), valid=valid, order=np.array("pu"),
              compute_ll=np.array(m in (1, n)))
-    if du:
-        g["B"] = rng.standard_normal((N, n, du)); g["us"] = rng.standard_normal((4, N, du))
     return g
-
-
-def _per_filter(g):
-    N = g["x"].shape[0]
-    out = dict(g)
-    for k in ("F", "H", "Q", "R_inv"):
-        if g[k].ndim == 2:
-            out[k] = np.broadcast_to(g[k], (N,) + g[k].shape).copy()
-    out["F_inv"] = np.linalg.inv(out["F"])
-    return out
-
-
-@pytest.mark.parametrize("dtype", [np.float64, np.float32])
-@pytest.mark.parametrize("shared", [False, True])
-@pytest.mark.parametrize("shape", TILES + [(5, 5), (9, 3), (3, 4)])
-def test_random_bank_matches_oracle(shape, shared, dtype):
-    n, m = shape
-    N = 600
-    g = _random(N, n, m, seed=100 * n + m + shared, shared=shared)
-    o = io.run_bank(_per_filter(g), ll_mode(g))
-    f = _bank(g, dtype)
-    for t in range(4):
-        _step(f, g, t)
-        assert np.array_equal(_np(f._no_information), o["ni"][t]), t
-        for sel in (o["ni"][t] != 0, o["ni"][t] == 0):        # each branch on its own scale
-            assert _err(_np(f.x)[sel], o["x"][t][sel]) < TOL[dtype] * 10, t
-            assert _err(_np(f.P_inv)[sel], o["P_inv"][t][sel]) < TOL[dtype] * 10, t
-        if bool(g["compute_ll"]):
-            assert _err(f.log_likelihood, o["ll"][t]) < TOL[dtype] * 10, t
-    assert o["ni"][0].any() and not o["ni"][0].all()
-
-
-@pytest.mark.parametrize("dtype", [np.float64, np.float32])
-def test_control_input_runs_the_warp_kernel(dtype):
-    g = _random(300, 3, 2, seed=5, du=2)
-    o = io.run_bank(_per_filter(g))
-    f = _bank(g, dtype)
-    for t in range(4):
-        _step(f, g, t)
-    assert _err(f.x, o["x"][-1]) < TOL[dtype] * 10
 
 
 @pytest.mark.parametrize("shape", [(4, 2), (5, 3)])
