@@ -192,6 +192,8 @@ struct FlsCorrP {
     const T *F, *H;
     int64_t sF, sH;
     const T *x_post, *P_post, *x_pre, *K, *y, *SI;
+    const T *z;                                              // the epoch's measurements [Nf,m]
+    T *y_last;                                               // the last epoch's y in the workspace, else NULL
     const int32_t *st_epoch;
     T *v, *vn, *w;                                           // per-filter scratch [Nf,n], [Nf,n], [Nf,m]
     T *xs, *xhat;
@@ -209,6 +211,16 @@ __global__ void __launch_bounds__(128) fls_correct_kernel(FlsCorrP<T> p)
     const int32_t st = p.st_epoch[f];
     if (st != BKE_STATUS_OK && p.status) p.status[f] = st;
     const T *xpost = p.x_post + f * n, *xpre = p.x_pre + f * n;
+    if (st != BKE_STATUS_OK && p.y_last) {
+        // the step leaves y alone where S is singular; the call's y is still z - H x_pre (the reference sets
+        // self.y before inv(S) raises, and the fused kernel stores it too)
+        const T *H = p.H + f * p.sH, *z = p.z + f * m;
+        for (int a = 0; a < m; a++) {
+            T s = z[a];
+            for (int j = 0; j < n; j++) s -= H[a * n + j] * xpre[j];
+            p.y_last[f * m + a] = s;
+        }
+    }
     if (p.xhat)
         for (int i = 0; i < n; i++) p.xhat[(p.t * Nf + f) * n + i] = xpost[i];
     T *rk = p.xs + (k * Nf + f) * n;
@@ -311,6 +323,7 @@ int launch_per_epoch(const bke_fls_args &a, cudaStream_t s)
         int rc = launch_kf_any(k, s);
         if (rc) return rc;
         c.k = a.count + t; c.t = t;
+        c.z = (const T *)k.z; c.y_last = (t + 1 == a.n_steps && k0.y) ? (T *)(wb + ws.y) : nullptr;
         fls_correct_kernel<T><<<grid, 128, 0, s>>>(c);
         if ((rc = check_cuda(cudaGetLastError(), "fls_correct_kernel launch"))) return rc;
     }

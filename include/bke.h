@@ -299,7 +299,7 @@ int bke_kf_batch_filter(const bke_kf_batch_args *args, void *stream);
  * Every measurement is present (the reference has no missing-measurement rule: z = None raises TypeError).
  * Where the reference's inv(S) raises LinAlgError, status[f] = BKE_STATUS_SINGULAR_S (sticky over the call's
  * epochs), that filter keeps its prior for the epoch (x = x_pre, P = the predicted P), its row k is x_pre
- * and no row is corrected.
+ * and no row is corrected; y and S are still the epoch's z - H x_pre and H P H' + R, on both paths.
  * The workspace (bke_fls_workspace_bytes, 16-byte aligned) is only needed when the call runs the per-epoch
  * path: the size is 0 when the fused kernel covers the shape.  Fused (DESIGN.md §3.4b): 1/1, 2/1 and 4/2,
  * fp32 and fp64, without control input, lag <= BKE_FLS_FUSED_MAX_LAG; the lag window stays in shared memory
@@ -1121,8 +1121,9 @@ int bke_mm_estimate(const bke_mm_args *args, void *stream);
  *   priors), mus [T,N,M] (fp64, mu after each update).
  * A bad size, stride, dtype, flag or model count (2 .. BKE_MM_MAX_MODELS), a NULL pointer the call reads or
  * writes, or an output that overlaps another array is BKE_ERR_BAD_ARG; a shape without a fused instance
- * ((n, m) other than 2/1, 3/1, 4/2, 6/3), or a state, diagnostic or output array that is not 16-byte aligned,
- * is BKE_ERR_UNSUPPORTED (the caller then runs the separate launches).  Both before any device is touched.
+ * ((n, m) other than 2/1 and 3/1 in fp32 and fp64, and 4/2 in fp32), or a state, diagnostic or output array that
+ * is not 16-byte aligned, is BKE_ERR_UNSUPPORTED (the caller then runs the separate launches).  Both before any
+ * device is touched.
  * The call allocates nothing and can be captured in a graph. */
 typedef struct bke_imm_batch_args {
     int64_t n_tracks;

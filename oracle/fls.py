@@ -81,6 +81,7 @@ def fls_bank(x, P, F, H, Q, R, zs, N, B=None, us=None, count=0, hist=None):
         xs[:count] = hist
     xhat = np.zeros((T, Nf, n))
     status = np.zeros(Nf, np.int32)
+    cond = np.ones(Nf)
     eye = np.eye(n)
     HT, FT = np.swapaxes(H, 1, 2), np.swapaxes(F, 1, 2)
     for t in range(T):
@@ -94,6 +95,8 @@ def fls_bank(x, P, F, H, Q, R, zs, N, B=None, us=None, count=0, hist=None):
         ok = np.abs(np.linalg.det(S)) > 0
         SI = np.zeros_like(S)
         SI[ok] = np.linalg.inv(S[ok])
+        if ok.any():
+            cond[ok] = np.maximum(cond[ok], np.linalg.cond(S[ok]))
         K = Pp @ HT @ SI
         xn = x_pre + np.einsum("fia,fa->fi", K, y)
         I_KH = eye - K @ H
@@ -113,4 +116,4 @@ def fls_bank(x, P, F, H, Q, R, zs, N, B=None, us=None, count=0, hist=None):
                 xs[k - i, ok] += np.einsum("fia,fa->fi", Ki, y)[ok]
         else:
             xs[k] = x
-    return dict(xs=xs, xhat=xhat, x=x, P=P, y=y, S=S, status=status)
+    return dict(xs=xs, xhat=xhat, x=x, P=P, y=y, S=S, status=status, cond=cond)
