@@ -249,6 +249,23 @@ class ScoreArgs(ctypes.Structure):
     ]
 
 
+class UkfScoreArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_filters", c_int64), ("n_candidates", c_int64),
+        ("dim_x", c_int32), ("dim_z", c_int32), ("dtype", c_int32), ("flags", c_uint32),
+        ("hx_model", c_int32), ("reserved", c_int32),
+        ("alpha", c_double), ("beta", c_double), ("kappa", c_double),
+        ("x", c_void_p), ("P", c_void_p),
+        ("R", c_void_p), ("R_stride", c_int64),
+        ("H", c_void_p), ("H_stride", c_int64),
+        ("z", c_void_p), ("z_track_stride", c_int64), ("z_cand_stride", c_int64),
+        ("z_valid", c_void_p),
+        ("zhat", c_void_p), ("y", c_void_p), ("d2", c_void_p), ("mahalanobis", c_void_p),
+        ("log_likelihood", c_void_p), ("likelihood", c_void_p),
+        ("status", c_void_p),
+    ]
+
+
 class ResampleShardArgs(ctypes.Structure):
     _fields_ = [
         ("n_local", c_int64), ("n_global", c_int64), ("j_offset", c_int64), ("capacity", c_int64),
@@ -434,6 +451,9 @@ _SIGNATURES = {
     "bke_inverse": (c_int, [c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "bke_poly_filter": (c_int, [POINTER(PolyArgs), c_void_p]),
     "bke_score_measurements": (c_int, [POINTER(ScoreArgs), c_void_p]),
+    "bke_ukf_score": (c_int, [POINTER(UkfScoreArgs), c_void_p]),
+    "bke_ukf_score_model": (c_int, [POINTER(UkfScoreArgs), c_void_p, c_void_p, c_int64, c_void_p]),
+    "bke_debug_ukf_score_model_cubin_bytes": (c_size_t, _MODEL + [c_uint32, c_uint32, c_char_p, c_char_p]),
     "bke_merwe_sigma_points": (c_int, [c_int64, c_int32, c_int32, c_double, c_double, c_double, c_void_p, c_void_p,
                                        c_void_p, c_void_p, c_void_p]),
     "bke_simplex_sigma_points": (c_int, [c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -298,6 +298,9 @@ static int validate_imm(const bke_imm_batch_args *a)
     return -1;
 }
 
+template <typename Args>
+static int check_candidates(const Args &a, int64_t N, int64_t m);
+
 // the checks of bke_score_measurements
 static int validate_score(const bke_score_args &a)
 {
@@ -319,19 +322,47 @@ static int validate_score(const bke_score_args &a)
     const bool scores = a.d2 || a.mahalanobis || a.log_likelihood || a.likelihood;
     if (!(a.zhat || a.y || scores || a.status)) { set_error("no output is requested"); return BKE_ERR_BAD_ARG; }
     if ((scores || a.status) && !a.P && !a.S) { set_error("the scores and status need a covariance: P or S"); return BKE_ERR_BAD_ARG; }
+    return check_candidates(a, a.n_tracks, m);
+}
+
+// the candidates and outputs of the measurement scores (bke_score_args and bke_ukf_score_args alike)
+template <typename Args>
+static int check_candidates(const Args &a, int64_t N, int64_t m)
+{
+    const bool scores = a.d2 || a.mahalanobis || a.log_likelihood || a.likelihood;
     if ((a.y || scores) && !a.z) { set_error("y and the scores need z"); return BKE_ERR_BAD_ARG; }
     if (a.z_track_stride < 0 || a.z_cand_stride < 0) { set_error("z strides must be 0 or greater"); return BKE_ERR_BAD_ARG; }
     // every offset the kernel forms fits int64: pair * m, and z's last element
     int64_t pairs, t, u, last;
-    if (__builtin_mul_overflow(a.n_tracks, a.n_candidates, &pairs) || __builtin_mul_overflow(pairs, m, &t) ||
-        (a.n_tracks > 0 && __builtin_mul_overflow(a.n_tracks - 1, a.z_track_stride, &t)) ||
+    if (__builtin_mul_overflow(N, a.n_candidates, &pairs) || __builtin_mul_overflow(pairs, m, &t) ||
+        (N > 0 && __builtin_mul_overflow(N - 1, a.z_track_stride, &t)) ||
         (a.n_candidates > 0 && __builtin_mul_overflow(a.n_candidates - 1, a.z_cand_stride, &u)) ||
-        (a.n_tracks > 0 && a.n_candidates > 0 && __builtin_add_overflow(t, u, &last)) ||
-        (a.n_tracks > 0 && a.n_candidates > 0 && __builtin_add_overflow(last, m, &last))) {
+        (N > 0 && a.n_candidates > 0 && __builtin_add_overflow(t, u, &last)) ||
+        (N > 0 && a.n_candidates > 0 && __builtin_add_overflow(last, m, &last))) {
         set_error("N * K * dim_z or the z offsets overflow int64");
         return BKE_ERR_BAD_ARG;
     }
     return BKE_OK;
+}
+
+// bke_ukf_score and bke_ukf_score_model: the bank as a UKF step reads it, then the candidates as the linear scores
+int validate_ukf_score(const bke_ukf_score_args &a)
+{
+    int rc;
+    if (a.n_candidates < 0) { set_error("n_candidates must be 0 or greater"); return BKE_ERR_BAD_ARG; }
+    if ((rc = check_bank(a.n_filters, a.dim_x, a.dim_z)) || (rc = check_dtype(a.dtype))) return rc;
+    if (a.flags & ~BKE_UKF_SIMPLEX) { set_error("flags must be 0 or BKE_UKF_SIMPLEX"); return BKE_ERR_BAD_ARG; }
+    if (!a.x || !a.P || !a.R) { set_error("x, P and R must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    if (a.hx_model == BKE_HX_LINEAR && !a.H) { set_error("BKE_HX_LINEAR needs H"); return BKE_ERR_BAD_ARG; }
+    const int64_t n = a.dim_x, m = a.dim_z;
+    if ((rc = check_strides({{a.R_stride, m * m}, {a.hx_model == BKE_HX_LINEAR ? a.H_stride : 0, m * n}}))) return rc;
+    const double lam_n = a.alpha * a.alpha * (a.dim_x + a.kappa);
+    if (!(a.flags & BKE_UKF_SIMPLEX) && !(lam_n != 0.0)) { set_error("alpha^2 (n + kappa) must be non-zero"); return BKE_ERR_BAD_ARG; }
+    if (!(a.zhat || a.y || a.d2 || a.mahalanobis || a.log_likelihood || a.likelihood || a.status)) {
+        set_error("no output is requested");
+        return BKE_ERR_BAD_ARG;
+    }
+    return check_candidates(a, a.n_filters, m);
 }
 
 // the checks every sigma-point step (UKF, CKF, EnKF; pre-built and run-time compiled) makes
@@ -402,6 +433,7 @@ static bool empty_bank(const bke_kf_rows_args &a) { return a.step.n_filters == 0
 static bool empty_bank(const bke_kf_batch_args &a) { return a.step.n_filters == 0; }
 static bool empty_bank(const bke_fls_args &a) { return a.step.n_filters == 0; }
 static bool empty_bank(const bke_score_args &a) { return a.n_tracks == 0 || a.n_candidates == 0; }
+static bool empty_bank(const bke_ukf_score_args &a) { return a.n_filters == 0 || a.n_candidates == 0; }
 
 // the body of an entry point: its argument checks, then the device, then an empty bank returns at once, then the launch
 template <typename Args, typename Validate, typename Launch>
@@ -767,5 +799,20 @@ int bke_imm_batch_filter(const bke_imm_batch_args *args, void *stream)
 }
 
 int bke_score_measurements(const bke_score_args *args, void *stream) { return checked_launch(args, validate_score, launch_score, stream); }
+
+// the pre-built hx models at the shapes they are written for
+static int validate_ukf_score_prebuilt(const bke_ukf_score_args &a)
+{
+    if (int rc = validate_ukf_score(a)) return rc;
+    if (a.hx_model == BKE_HX_RANGE_AZ_EL && !(a.dim_x == 6 && a.dim_z == 3)) { set_error("BKE_HX_RANGE_AZ_EL needs dim_x=6, dim_z=3"); return BKE_ERR_BAD_ARG; }
+    if (a.hx_model == BKE_HX_RANGE_BEARING && !(a.dim_x == 4 && a.dim_z == 2)) { set_error("BKE_HX_RANGE_BEARING needs dim_x=4, dim_z=2"); return BKE_ERR_BAD_ARG; }
+    if (a.hx_model < 0 || a.hx_model > BKE_HX_RANGE_BEARING) { set_error("unknown hx model id"); return BKE_ERR_BAD_ARG; }
+    return BKE_OK;
+}
+
+int bke_ukf_score(const bke_ukf_score_args *args, void *stream)
+{
+    return checked_launch(args, validate_ukf_score_prebuilt, launch_ukf_score, stream);
+}
 
 }  // extern "C"

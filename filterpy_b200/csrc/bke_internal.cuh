@@ -98,6 +98,8 @@ int launch_fls(const bke_fls_args &a, cudaStream_t s);
 int validate_ukf(const bke_ukf_args &a);
 int validate_ckf(const bke_ckf_args &a);
 int validate_enkf(const bke_enkf_args &a);
+// bke_ukf_score and bke_ukf_score_model (api.cu)
+int validate_ukf_score(const bke_ukf_score_args &a);
 // the UKF smoother's, pre-built or compiled (user_fx: around a user fx, served besides the built-in ones); -1 = go
 int validate_ukf_rts(const bke_ukf_rts_args &a, bool user_fx);
 int launch_ukf(const bke_ukf_args &a, cudaStream_t s);
@@ -113,6 +115,7 @@ int launch_inverse(int64_t n_filters, int32_t k, int32_t dtype, const void *A, i
                    cudaStream_t s);
 int launch_poly(const bke_poly_args &a, cudaStream_t s);
 int launch_score(const bke_score_args &a, cudaStream_t s);
+int launch_ukf_score(const bke_ukf_score_args &a, cudaStream_t s);
 // the (dim_x, dim_z, dtype) combinations bke_imm_batch_filter has a fused kernel for
 bool imm_batch_has_instance(int dim_x, int dim_z, int dtype);
 int launch_imm_batch(const bke_imm_batch_args &a, cudaStream_t s);

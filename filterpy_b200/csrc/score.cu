@@ -12,13 +12,16 @@
 //            which makes every score of the track NaN without a branch in phase B.
 //   phase B  the tile's outputs out[t0 : t0 + nt, 0 : K] are one contiguous range of nt * K words: the threads walk
 //            it in pair order, so stores (and the loads of per-track candidates [N, K, m]) are coalesced for any K.
-//            m <= 4 keeps y in registers; a larger m re-reads z_ik (L1) instead.
+//            The per-pair work is score_pairs.cuh's (shared with bke_ukf_score): m <= 4 keeps y in registers; a
+//            larger m re-reads z_ik (L1) instead.
 #include "bke_internal.cuh"
 #include "kf_regtile.cuh"
 #include "kf_warp.cuh"
+#include "score_pairs.cuh"
 
 namespace bke {
 namespace {
+using namespace scorek;
 
 constexpr int THREADS = 128;
 
@@ -33,12 +36,6 @@ struct ScP {
     T *zhat, *y, *d2, *maha, *ll, *lk;
     int32_t *status;
 };
-
-template <typename T>
-__device__ __forceinline__ T qnan() { return T(__int_as_float(0x7fc00000)); }
-
-// the track's slot in the tile: zhat[m], SI[m*m], log|det S|
-__host__ __device__ __forceinline__ int slot_words(int m) { return m + m * m + 1; }
 
 // ---- phase A, one thread per track: compile-time n = N, m = M
 template <typename T, int N, int M>
@@ -180,75 +177,6 @@ __device__ void track_warp(const ScP<T> &p, int64_t f, T *slot, T *scr, int lane
     __syncwarp();
 }
 
-template <typename T>
-__device__ __forceinline__ T log_dbl_min() { return T(-708.39641853226408); }      // log(sys.float_info.min)
-
-// the scores of one pair from d2 = y' SI y (valid) and write-out
-template <typename T>
-__device__ __forceinline__ void put_scores(const ScP<T> &p, int64_t pr, bool valid, T q, T logdet, int m)
-{
-    const T ll = valid ? T(-0.5) * (q + logdet + T(m) * T(LOG_2PI)) : log_dbl_min<T>();
-    if (!valid) q = T(0);
-    if (p.d2) p.d2[pr] = q;
-    if (p.maha) p.maha[pr] = sqrt(q);
-    if (p.ll) p.ll[pr] = ll;
-    if (p.lk) p.lk[pr] = exp(ll);
-}
-
-// ---- phase B, one pair, m = M in registers
-template <typename T, int M>
-__device__ __forceinline__ void pair_reg(const ScP<T> &p, int64_t f, int64_t k, const T *slot, bool cov)
-{
-    const int64_t pr = f * p.K + k;
-    const bool valid = !p.valid || p.valid[pr];
-    T y[M];
-    if (valid) {
-        const T *z = p.z + f * p.zt + k * p.zc;
-#pragma unroll
-        for (int a = 0; a < M; a++) y[a] = z[a] - slot[a];
-    } else {
-#pragma unroll
-        for (int a = 0; a < M; a++) y[a] = T(0);
-    }
-    if (p.y) {
-#pragma unroll
-        for (int a = 0; a < M; a++) p.y[pr * M + a] = y[a];
-    }
-    if (!cov) return;
-    const T *SI = slot + M;
-    T q = T(0);
-#pragma unroll
-    for (int a = 0; a < M; a++) {
-        T s = T(0);
-#pragma unroll
-        for (int b = 0; b < M; b++) s += SI[a * M + b] * y[b];
-        q += y[a] * s;
-    }
-    put_scores(p, pr, valid, q, slot[M + M * M], M);
-}
-
-// ---- phase B, one pair, any m: y_a is formed again where it is needed (z_ik stays in L1)
-template <typename T>
-__device__ __forceinline__ void pair_any(const ScP<T> &p, int64_t f, int64_t k, const T *slot, bool cov)
-{
-    const int m = p.m;
-    const int64_t pr = f * p.K + k;
-    const bool valid = !p.valid || p.valid[pr];
-    const T *z = p.z + f * p.zt + k * p.zc;
-    if (p.y)
-        for (int a = 0; a < m; a++) p.y[pr * m + a] = valid ? z[a] - slot[a] : T(0);
-    if (!cov) return;
-    const T *SI = slot + m;
-    T q = T(0);
-    if (valid)
-        for (int a = 0; a < m; a++) {
-            T s = T(0);
-            for (int b = 0; b < m; b++) s += SI[a * m + b] * (z[b] - slot[b]);
-            q += (z[a] - slot[a]) * s;
-        }
-    put_scores(p, pr, valid, q, slot[m + m * m], m);
-}
-
 // N > 0: phase A in registers at n = N (M > 0);  N == 0: phase A by warps.  M > 0: phase B at m = M;  M == 0: any m.
 template <typename T, int N, int M>
 __global__ void __launch_bounds__(THREADS) score_kernel(const ScP<T> p)
@@ -271,11 +199,12 @@ __global__ void __launch_bounds__(THREADS) score_kernel(const ScP<T> p)
         }
         __syncthreads();
         if (sweep) {
-            // thread t starts at pair t of the tile
+            // thread t starts at pair t of the tile (the walk stays written out here: routed through a shared
+            // function it changed every instance's code)
             int64_t i = threadIdx.x < K ? 0 : (int)threadIdx.x / (int)K, k = threadIdx.x - i * K;
             while (i < nt) {
-                if constexpr (M > 0) pair_reg<T, M>(p, t0 + i, k, tile + i * per, cov);
-                else pair_any<T>(p, t0 + i, k, tile + i * per, cov);
+                if constexpr (M > 0) pair_reg<T, M, SubResidual>(p, t0 + i, k, tile + i * per, cov);
+                else pair_any<T>(p, t0 + i, k, tile + i * per, cov, p.m);
                 k += dk; i += di;
                 if (k >= K) { k -= K; i++; }
             }

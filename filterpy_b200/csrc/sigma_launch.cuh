@@ -1,11 +1,12 @@
 // sigma_launch.cuh — host side shared by the sigma-point families (UKF, CKF, EnKF), pre-built (ukf.cu,
-// ukf_simplex.cu, ckf.cu, enkf.cu) and run-time compiled (ukf_rtc.cu): the instance table, parameter
+// ukf_simplex.cu, ukf_score.cu, ckf.cu, enkf.cu) and run-time compiled (ukf_rtc.cu): the instance table, parameter
 // blocks, dynamic shared-memory sizes, grids and occupancy caps.  (The launch, launch_kernel, and the
 // argument checks, validate_*, live in api.cu.)
 #pragma once
 #include <math.h>
 #include "ckf_kernel.cuh"
 #include "enkf_kernel.cuh"
+#include "ukf_score_kernel.cuh"
 
 // The pre-built (dim_x, dim_z, fx, hx) instances of every family, in dispatch order.  X(n, m, fx, hx) per row.
 #define BKE_SIGMA_INSTANCES(X)                     \
@@ -71,11 +72,10 @@ inline void set_user_args(Prm &p, const void *fx_args, int64_t s_fx, const void 
     p.hx_args = (const T *)hx_args; p.s_hx_args = s_hx;
 }
 
-template <typename T>
-inline void ukf_fill_params(const bke_ukf_args &a, int N, ukfk::UkfP<T> &p)
+// the point set's scale and weights: Merwe's (alpha, beta, kappa) or the simplex set's (BKE_UKF_SIMPLEX in a.flags)
+template <typename T, typename Args, typename Prm>
+inline void ukf_set_weights(const Args &a, int N, Prm &p)
 {
-    fill_common<T>(a, p);
-    p.y = (T *)a.y; p.ll = (T *)a.log_likelihood;
     if (a.flags & BKE_UKF_SIMPLEX) {                                        // sigma_points.py:516-522
         p.scale = T(1);
         p.wm0 = p.wc0 = p.wi = (T)(1. / (N + 1));
@@ -87,6 +87,39 @@ inline void ukf_fill_params(const bke_ukf_args &a, int N, ukfk::UkfP<T> &p)
         p.wc0 = (T)(lambda_ / (N + lambda_) + (1 - a.alpha * a.alpha + a.beta));
         p.wi = (T)c;
     }
+}
+
+template <typename T>
+inline void ukf_fill_params(const bke_ukf_args &a, int N, ukfk::UkfP<T> &p)
+{
+    fill_common<T>(a, p);
+    p.y = (T *)a.y; p.ll = (T *)a.log_likelihood;
+    ukf_set_weights<T>(a, N, p);
+}
+
+// the UKF score's parameter block (no user-model arguments: set_user_args)
+template <typename T>
+inline void ukf_score_fill_params(const bke_ukf_score_args &a, ukfk::UkfScoreP<T> &p)
+{
+    p.N = a.n_filters; p.K = a.n_candidates;
+    p.di = ukfk::UB / p.K; p.dk = ukfk::UB - p.di * p.K;
+    ukf_set_weights<T>(a, a.dim_x, p);
+    p.x = (const T *)a.x; p.P = (const T *)a.P; p.R = (const T *)a.R; p.H = (const T *)a.H; p.z = (const T *)a.z;
+    p.sR = a.R_stride; p.sH = a.H_stride; p.zt = a.z_track_stride; p.zc = a.z_cand_stride;
+    p.valid = a.z_valid;
+    p.zhat = (T *)a.zhat; p.y = (T *)a.y; p.d2 = (T *)a.d2; p.maha = (T *)a.mahalanobis;
+    p.ll = (T *)a.log_likelihood; p.lk = (T *)a.likelihood; p.status = a.status;
+    p.hx_args = nullptr; p.s_hx_args = 0;
+}
+
+// the UKF score's dynamic shared memory: the hx slab (or one P tile), the tile's slots and the staged H
+template <typename T>
+inline size_t ukf_score_smem_bytes(int N, int M, bool simplex, bool hx_linear, bool H_shared)
+{
+    const int PADP = (N * N) | 1, zs = (simplex ? N + 1 : 2 * N + 1) * M;
+    size_t smem = sizeof(T) * ((size_t)(zs > PADP ? zs : PADP) + (size_t)(M + M * M + 1)) * ukfk::UB;
+    if (hx_linear) smem += sizeof(T) * (H_shared ? M * N : M * N * ukfk::UB);
+    return smem;
 }
 
 template <typename T>

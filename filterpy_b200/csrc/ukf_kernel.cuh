@@ -340,6 +340,168 @@ __device__ __forceinline__ void slab_store(T *g, const T *slab, int cnt)
     for (int e = threadIdx.x; e < cnt * PER; e += UB) g[e] = slab[(e / PER) * PAD + (e % PER)];
 }
 
+// The measurement half of the update (UKF.py:407, 462-473): sigma points of (x, P) (U: the Cholesky rows, or
+// the simplex offsets), hx of every point into the slab zs ([NS*M][UB]), z^ = zm (or z_mean_fn), S = Sc
+// (residual_z, then + R) and its inverse.  Returns false where S is singular; a failed Cholesky sets
+// st = BKE_STATUS_NOT_PD.  p is the kernel's parameter block (its scale, wm0, wc0 and wi are read).  The fused step
+// and the measurement scores (ukf_score_kernel.cuh) share it:
+//   after_chol()           once U is drawn (the step parks P there)
+//   prefetch(Rv)           loads R [M][M] ahead of the covariance pass (the step fetches z with it)
+//   cross(IntC<S>, w, dz)  every point's weighted residual dz (the step accumulates Pxz)
+template <typename T, int N, int M, int HX, bool SPX, typename PP, typename AfterChol, typename Prefetch, typename Cross>
+__device__ __forceinline__ bool meas_ut(const PP &p, const T (&x)[N], const T (&P)[N][N], T (&U)[SPX ? N + 1 : N][N], T *zs, int tid,
+                                        const T *Hp, int hstride, const T *hxa, int &st, T (&zm)[M], T (&Sc)[M][M], T (&SI)[M][M], T &logdet, AfterChol &&after_chol, Prefetch &&prefetch,
+                                        Cross &&cross)
+{
+    constexpr int NS = SPX ? N + 1 : 2 * N + 1;
+    // sigma points regenerated from the prior (UKF.py:407); scipy's cholesky reads the upper triangle
+    {
+        T A[N][N];
+#pragma unroll
+        for (int i = 0; i < N; i++)
+#pragma unroll
+            for (int j = i; j < N; j++) A[i][j] = p.scale * P[i][j];
+        if (!chol_upper<T, N>(A, U)) st = BKE_STATUS_NOT_PD;
+        if constexpr (SPX) simplex_offsets<T, N>(U);
+    }
+    after_chol();
+#pragma unroll
+    for (int a = 0; a < M; a++) zm[a] = T(0);
+    if constexpr (HX == BKE_HX_LINEAR || HX == BKE_HX_USER) {
+        for_sigma<0, NS>([&](auto sc) {
+            constexpr int S = decltype(sc)::value;
+            T sp[N], h[M];
+            point<T, N, S>(x, U, sp);
+            apply_hx<T, N, M, HX>(sp, h, Hp, hstride, hxa);
+            const T w = (S == 0) ? p.wm0 : p.wi;
+#pragma unroll
+            for (int a = 0; a < M; a++) { zm[a] += w * h[a]; zs[(S * M + a) * UB + tid] = h[a]; }
+        });
+    } else if constexpr (SPX) {
+        // The transcendental models on the simplex set: as below, the positions are parked and a
+        // run-time loop evaluates hx in place, but no point equals x, so hx(x) (weight 0) is the
+        // reference direction of the relative angles.  D_j with j - 1 past the last position
+        // component leaves the positions of x unchanged: that point's hx is hx(x).
+        for_sigma<0, NS>([&](auto sc) {
+            constexpr int S = decltype(sc)::value;
+            T sp[N];
+            point<T, N, S>(x, U, sp);
+#pragma unroll
+            for (int a = 0; a < M; a++) zs[(S * M + a) * UB + tid] = sp[2 * a];
+        });
+        T h0[M], pos0[M];
+#pragma unroll
+        for (int a = 0; a < M; a++) pos0[a] = x[2 * a];
+        hx_positions<T, M, HX>(pos0, h0);
+        const T rho0 = sqrt(pos0[0] * pos0[0] + pos0[1] * pos0[1]);
+#pragma unroll 1
+        for (int s = 0; s < NS; s++) {
+            T h[M];
+            if (s >= 2 && hx_ignores_row<HX, N>(s - 1)) {
+#pragma unroll
+                for (int a = 0; a < M; a++) h[a] = h0[a];
+            } else {
+                T pa[M];
+#pragma unroll
+                for (int a = 0; a < M; a++) pa[a] = zs[(s * M + a) * UB + tid];
+                hx_positions_rel<T, M, HX>(pa, pos0, rho0, h0, h);
+            }
+#pragma unroll
+            for (int a = 0; a < M; a++) { zm[a] += p.wi * h[a]; zs[(s * M + a) * UB + tid] = h[a]; }
+        }
+    } else {
+        // Transcendental measurement models: the inputs hx reads (M position components per
+        // sigma point) are parked in the slab first, then a run-time loop over the n offset
+        // rows evaluates hx in place for the +row / -row pair (two independent chains per
+        // iteration).  Unrolling 2n+1 inlined atan2/sqrt bodies made the fp64 kernel 117 KB of
+        // code (instruction-cache hit rate 83 %, `no_instruction` the second largest stall).
+        for_sigma<0, NS>([&](auto sc) {
+            constexpr int S = decltype(sc)::value;
+            T sp[N];
+            sigma_point<T, N, S>(x, U, sp);
+#pragma unroll
+            for (int a = 0; a < M; a++) zs[(S * M + a) * UB + tid] = sp[2 * a];      // positions sit at 0, 2, 4
+        });
+        T h0[M], pos0[M];
+        {
+#pragma unroll
+            for (int a = 0; a < M; a++) pos0[a] = zs[a * UB + tid];
+            hx_positions<T, M, HX>(pos0, h0);
+#pragma unroll
+            for (int a = 0; a < M; a++) { zm[a] += p.wm0 * h0[a]; zs[a * UB + tid] = h0[a]; }
+        }
+        const T rho0 = sqrt(pos0[0] * pos0[0] + pos0[1] * pos0[1]);
+#pragma unroll 1
+        for (int k = 0; k < N; k++) {
+            const int sa = k + 1, sb = k + 1 + N;
+            T ha[M], hb[M];
+            if (hx_ignores_row<HX, N>(k)) {               // this offset row leaves the positions alone
+#pragma unroll
+                for (int a = 0; a < M; a++) { ha[a] = h0[a]; hb[a] = h0[a]; }
+            } else {
+                T pa[M], pb[M];
+#pragma unroll
+                for (int a = 0; a < M; a++) { pa[a] = zs[(sa * M + a) * UB + tid]; pb[a] = zs[(sb * M + a) * UB + tid]; }
+                hx_positions_rel<T, M, HX>(pa, pos0, rho0, h0, ha);
+                hx_positions_rel<T, M, HX>(pb, pos0, rho0, h0, hb);
+            }
+#pragma unroll
+            for (int a = 0; a < M; a++) {
+                zm[a] += p.wi * ha[a]; zm[a] += p.wi * hb[a];
+                zs[(sa * M + a) * UB + tid] = ha[a]; zs[(sb * M + a) * UB + tid] = hb[a];
+            }
+        }
+    }
+    if constexpr (HOOKS & BKE_HOOK_Z_MEAN) {                // z_mean_fn(sigmas_h, Wm) (UKF.py:469)
+        T sh[NS * M], Wm[NS];
+#pragma unroll
+        for (int s = 0; s < NS; s++) {
+            Wm[s] = (s == 0) ? p.wm0 : p.wi;
+#pragma unroll
+            for (int a = 0; a < M; a++) sh[s * M + a] = zs[(s * M + a) * UB + tid];
+        }
+        bke_hook_z_mean<T>(sh, Wm, zm);
+    }
+    // R is needed after the covariance pass below: fetch it now so that its latency hides behind it (with z
+    // in the step, they were the largest long-scoreboard stalls of the update)
+    T Rv[M][M];
+    prefetch(Rv);
+#pragma unroll
+    for (int a = 0; a < M; a++)
+#pragma unroll
+        for (int b = a; b < M; b++) Sc[a][b] = T(0);
+    for_sigma<0, NS>([&](auto sc) {
+        constexpr int S = decltype(sc)::value;
+        T dz[M];
+        if constexpr (HOOKS & BKE_HOOK_RESIDUAL_Z) {
+            T h[M];
+#pragma unroll
+            for (int a = 0; a < M; a++) h[a] = zs[(S * M + a) * UB + tid];
+            bke_hook_residual_z<T>(h, zm, dz);
+        } else {
+#pragma unroll
+            for (int a = 0; a < M; a++) dz[a] = zs[(S * M + a) * UB + tid] - zm[a];
+        }
+        const T w = (S == 0) ? p.wc0 : p.wi;
+#pragma unroll
+        for (int a = 0; a < M; a++) {
+            T wd = w * dz[a];
+#pragma unroll
+            for (int b = a; b < M; b++) Sc[a][b] += wd * dz[b];
+        }
+        cross(sc, w, dz);
+    });
+#pragma unroll
+    for (int a = 0; a < M; a++)
+#pragma unroll
+        for (int b = a; b < M; b++) {
+            const T sab = Sc[a][b];
+            Sc[a][b] = sab + Rv[a][b];
+            if (b > a) Sc[b][a] = sab + Rv[b][a];
+        }
+    return reg_inverse<T, M>(Sc, SI, logdet);
+}
+
 // UKF_EXTRAS: the optional outputs (priors, K, y, S, SI, log-likelihood) are compiled in; the plain
 // instantiation is 2-4 % faster without their tests and live ranges.
 // SPX: the simplex point set (n + 1 points, p.scale = 1, every weight 1/(n+1)) instead of Merwe's.
@@ -487,212 +649,76 @@ __global__ void __launch_bounds__(UB, OCC) ukf_kernel(UkfP<T> p)
     if (do_u) {
         const bool has_z = (p.valid == nullptr) || (p.valid[fc] != 0);
         if (has_z && st == BKE_STATUS_OK) {
-            // sigma points regenerated from the prior (UKF.py:407); scipy's cholesky reads the upper triangle
-            {
-                T A[N][N];
-#pragma unroll
-                for (int i = 0; i < N; i++)
-#pragma unroll
-                    for (int j = i; j < N; j++) A[i][j] = p.scale * P[i][j];
-                if (!chol_upper<T, N>(A, U)) st = BKE_STATUS_NOT_PD;
-                if constexpr (SPX) simplex_offsets<T, N>(U);
-            }
-            // P is not needed again until the posterior: park its upper triangle in shared memory and
-            // free the registers.  A (never expected) non-symmetric P keeps its lower triangle in P_out.
             bool asym = false;
-#pragma unroll
-            for (int i = 0; i < N; i++)
-#pragma unroll
-                for (int j = i; j < N; j++) {
-                    park[tri_index<N>(i, j) * UB + tid] = P[i][j];
-                    if (j > i) asym = asym || (P[j][i] != P[i][j]);
-                }
-            if (asym && live) {
-#pragma unroll
-                for (int i = 0; i < N; i++)
-#pragma unroll
-                    for (int j = 0; j < i; j++) p.P_out[f * N * N + i * N + j] = P[i][j];
-            }
             T zm[M];
+            KfUpdateOut<T, N, M> o;
+            T Pxz[N][M], zv[M];
+            o.ok = meas_ut<T, N, M, HX, SPX>(p, x, P, U, zs, tid, Hp, hstride, hxa, st, zm, o.S, o.SI, o.logdet,
+                [&] {
+                    // P is not needed again until the posterior: park its upper triangle in shared memory and
+                    // free the registers.  A (never expected) non-symmetric P keeps its lower triangle in P_out.
 #pragma unroll
-            for (int a = 0; a < M; a++) zm[a] = T(0);
-            if constexpr (HX == BKE_HX_LINEAR || HX == BKE_HX_USER) {
-                for_sigma<0, NS>([&](auto sc) {
-                    constexpr int S = decltype(sc)::value;
-                    T sp[N], h[M];
-                    point<T, N, S>(x, U, sp);
-                    apply_hx<T, N, M, HX>(sp, h, Hp, hstride, hxa);
-                    const T w = (S == 0) ? p.wm0 : p.wi;
+                    for (int i = 0; i < N; i++)
 #pragma unroll
-                    for (int a = 0; a < M; a++) { zm[a] += w * h[a]; zs[(S * M + a) * UB + tid] = h[a]; }
-                });
-            } else if constexpr (SPX) {
-                // The transcendental models on the simplex set: as below, the positions are parked and a
-                // run-time loop evaluates hx in place, but no point equals x, so hx(x) (weight 0) is the
-                // reference direction of the relative angles.  D_j with j - 1 past the last position
-                // component leaves the positions of x unchanged: that point's hx is hx(x).
-                for_sigma<0, NS>([&](auto sc) {
-                    constexpr int S = decltype(sc)::value;
-                    T sp[N];
-                    point<T, N, S>(x, U, sp);
+                        for (int j = i; j < N; j++) {
+                            park[tri_index<N>(i, j) * UB + tid] = P[i][j];
+                            if (j > i) asym = asym || (P[j][i] != P[i][j]);
+                        }
+                    if (asym && live) {
 #pragma unroll
-                    for (int a = 0; a < M; a++) zs[(S * M + a) * UB + tid] = sp[2 * a];
-                });
-                T h0[M], pos0[M];
+                        for (int i = 0; i < N; i++)
 #pragma unroll
-                for (int a = 0; a < M; a++) pos0[a] = x[2 * a];
-                hx_positions<T, M, HX>(pos0, h0);
-                const T rho0 = sqrt(pos0[0] * pos0[0] + pos0[1] * pos0[1]);
-#pragma unroll 1
-                for (int s = 0; s < NS; s++) {
-                    T h[M];
-                    if (s >= 2 && hx_ignores_row<HX, N>(s - 1)) {
-#pragma unroll
-                        for (int a = 0; a < M; a++) h[a] = h0[a];
-                    } else {
-                        T pa[M];
-#pragma unroll
-                        for (int a = 0; a < M; a++) pa[a] = zs[(s * M + a) * UB + tid];
-                        hx_positions_rel<T, M, HX>(pa, pos0, rho0, h0, h);
+                            for (int j = 0; j < i; j++) p.P_out[f * N * N + i * N + j] = P[i][j];
                     }
-#pragma unroll
-                    for (int a = 0; a < M; a++) { zm[a] += p.wi * h[a]; zs[(s * M + a) * UB + tid] = h[a]; }
-                }
-            } else {
-                // Transcendental measurement models: the inputs hx reads (M position components per
-                // sigma point) are parked in the slab first, then a run-time loop over the n offset
-                // rows evaluates hx in place for the +row / -row pair (two independent chains per
-                // iteration).  Unrolling 2n+1 inlined atan2/sqrt bodies made the fp64 kernel 117 KB of
-                // code (instruction-cache hit rate 83 %, `no_instruction` the second largest stall).
-                for_sigma<0, NS>([&](auto sc) {
-                    constexpr int S = decltype(sc)::value;
-                    T sp[N];
-                    sigma_point<T, N, S>(x, U, sp);
-#pragma unroll
-                    for (int a = 0; a < M; a++) zs[(S * M + a) * UB + tid] = sp[2 * a];      // positions sit at 0, 2, 4
-                });
-                T h0[M], pos0[M];
-                {
-#pragma unroll
-                    for (int a = 0; a < M; a++) pos0[a] = zs[a * UB + tid];
-                    hx_positions<T, M, HX>(pos0, h0);
-#pragma unroll
-                    for (int a = 0; a < M; a++) { zm[a] += p.wm0 * h0[a]; zs[a * UB + tid] = h0[a]; }
-                }
-                const T rho0 = sqrt(pos0[0] * pos0[0] + pos0[1] * pos0[1]);
-#pragma unroll 1
-                for (int k = 0; k < N; k++) {
-                    const int sa = k + 1, sb = k + 1 + N;
-                    T ha[M], hb[M];
-                    if (hx_ignores_row<HX, N>(k)) {               // this offset row leaves the positions alone
-#pragma unroll
-                        for (int a = 0; a < M; a++) { ha[a] = h0[a]; hb[a] = h0[a]; }
-                    } else {
-                        T pa[M], pb[M];
-#pragma unroll
-                        for (int a = 0; a < M; a++) { pa[a] = zs[(sa * M + a) * UB + tid]; pb[a] = zs[(sb * M + a) * UB + tid]; }
-                        hx_positions_rel<T, M, HX>(pa, pos0, rho0, h0, ha);
-                        hx_positions_rel<T, M, HX>(pb, pos0, rho0, h0, hb);
-                    }
+                },
+                [&](T (&Rv)[M][M]) {
+                    // z is needed after the covariance pass too: it comes with R
+                    const T *Rf = p.R + fc * p.sR;
 #pragma unroll
                     for (int a = 0; a < M; a++) {
-                        zm[a] += p.wi * ha[a]; zm[a] += p.wi * hb[a];
-                        zs[(sa * M + a) * UB + tid] = ha[a]; zs[(sb * M + a) * UB + tid] = hb[a];
+                        zv[a] = p.z[fc * M + a];
+#pragma unroll
+                        for (int b = 0; b < M; b++) Rv[a][b] = Rf[a * M + b];
                     }
-                }
-            }
-            if constexpr (HOOKS & BKE_HOOK_Z_MEAN) {                // z_mean_fn(sigmas_h, Wm) (UKF.py:469)
-                T sh[NS * M], Wm[NS];
 #pragma unroll
-                for (int s = 0; s < NS; s++) {
-                    Wm[s] = (s == 0) ? p.wm0 : p.wi;
+                    for (int i = 0; i < N; i++)
 #pragma unroll
-                    for (int a = 0; a < M; a++) sh[s * M + a] = zs[(s * M + a) * UB + tid];
-                }
-                bke_hook_z_mean<T>(sh, Wm, zm);
-            }
-            KfUpdateOut<T, N, M> o;
-            T Pxz[N][M];
-            // R and z are needed after the covariance pass below: fetch them now so that their latency
-            // hides behind it (they were the largest long-scoreboard stalls of the update)
-            T Rv[M][M], zv[M];
-            {
-                const T *Rf = p.R + fc * p.sR;
+                        for (int a = 0; a < M; a++) Pxz[i][a] = T(0);
+                },
+                [&](auto sc, T w, const T (&dz)[M]) {
+                    constexpr int S = decltype(sc)::value;
+                    if constexpr (HOOKS & BKE_HOOK_RESIDUAL_X) {
+                        // dx = residual_x(sigma, x) (UKF.py:501): the point itself, not the offset row
+                        T sp[N], dx[N];
+                        point<T, N, S>(x, U, sp);
+                        bke_hook_residual_x<T>(sp, x, dx);
 #pragma unroll
-                for (int a = 0; a < M; a++) {
-                    zv[a] = p.z[fc * M + a];
+                        for (int i = 0; i < N; i++) {
+                            T wd = w * dx[i];
 #pragma unroll
-                    for (int b = 0; b < M; b++) Rv[a][b] = Rf[a * M + b];
-                }
-            }
+                            for (int a = 0; a < M; a++) Pxz[i][a] += wd * dz[a];
+                        }
+                    } else if constexpr (SPX) {
+                        // dx = sigma - x = D_S: row N of U, or row S-1 (zero left of column S-1)
+                        constexpr int k = S == 0 ? 0 : S - 1, row = S == 0 ? N : S - 1;
 #pragma unroll
-            for (int a = 0; a < M; a++)
+                        for (int i = k; i < N; i++) {
+                            T wd = w * U[row][i];
 #pragma unroll
-                for (int b = a; b < M; b++) o.S[a][b] = T(0);
+                            for (int a = 0; a < M; a++) Pxz[i][a] += wd * dz[a];
+                        }
+                    } else if constexpr (S > 0) {
+                        // dx = sigma - x is the sigma offset itself: row k of +-U, zero left of the diagonal
+                        constexpr int k = (S - 1) % N;
+                        const T ws = (S <= N) ? w : -w;
 #pragma unroll
-            for (int i = 0; i < N; i++)
+                        for (int i = k; i < N; i++) {
+                            T wd = ws * U[k][i];
 #pragma unroll
-                for (int a = 0; a < M; a++) Pxz[i][a] = T(0);
-            for_sigma<0, NS>([&](auto sc) {
-                constexpr int S = decltype(sc)::value;
-                T dz[M];
-                if constexpr (HOOKS & BKE_HOOK_RESIDUAL_Z) {
-                    T h[M];
-#pragma unroll
-                    for (int a = 0; a < M; a++) h[a] = zs[(S * M + a) * UB + tid];
-                    bke_hook_residual_z<T>(h, zm, dz);
-                } else {
-#pragma unroll
-                    for (int a = 0; a < M; a++) dz[a] = zs[(S * M + a) * UB + tid] - zm[a];
-                }
-                const T w = (S == 0) ? p.wc0 : p.wi;
-#pragma unroll
-                for (int a = 0; a < M; a++) {
-                    T wd = w * dz[a];
-#pragma unroll
-                    for (int b = a; b < M; b++) o.S[a][b] += wd * dz[b];
-                }
-                if constexpr (HOOKS & BKE_HOOK_RESIDUAL_X) {
-                    // dx = residual_x(sigma, x) (UKF.py:501): the point itself, not the offset row
-                    T sp[N], dx[N];
-                    point<T, N, S>(x, U, sp);
-                    bke_hook_residual_x<T>(sp, x, dx);
-#pragma unroll
-                    for (int i = 0; i < N; i++) {
-                        T wd = w * dx[i];
-#pragma unroll
-                        for (int a = 0; a < M; a++) Pxz[i][a] += wd * dz[a];
+                            for (int a = 0; a < M; a++) Pxz[i][a] += wd * dz[a];
+                        }
                     }
-                } else if constexpr (SPX) {
-                    // dx = sigma - x = D_S: row N of U, or row S-1 (zero left of column S-1)
-                    constexpr int k = S == 0 ? 0 : S - 1, row = S == 0 ? N : S - 1;
-#pragma unroll
-                    for (int i = k; i < N; i++) {
-                        T wd = w * U[row][i];
-#pragma unroll
-                        for (int a = 0; a < M; a++) Pxz[i][a] += wd * dz[a];
-                    }
-                } else if constexpr (S > 0) {
-                    // dx = sigma - x is the sigma offset itself: row k of +-U, zero left of the diagonal
-                    constexpr int k = (S - 1) % N;
-                    const T ws = (S <= N) ? w : -w;
-#pragma unroll
-                    for (int i = k; i < N; i++) {
-                        T wd = ws * U[k][i];
-#pragma unroll
-                        for (int a = 0; a < M; a++) Pxz[i][a] += wd * dz[a];
-                    }
-                }
-            });
-#pragma unroll
-            for (int a = 0; a < M; a++)
-#pragma unroll
-                for (int b = a; b < M; b++) {
-                    const T sab = o.S[a][b];
-                    o.S[a][b] = sab + Rv[a][b];
-                    if (b > a) o.S[b][a] = sab + Rv[b][a];
-                }
-            o.ok = reg_inverse<T, M>(o.S, o.SI, o.logdet);
+                });
             if (!o.ok) st = BKE_STATUS_SINGULAR_S;
             const bool good = o.ok && st == BKE_STATUS_OK;
             T SK[M][N];

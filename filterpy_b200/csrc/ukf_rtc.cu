@@ -14,11 +14,15 @@
 // Program text handed to NVRTC (the user's part between the markers):
 //     typedef double real;                       // or float
 //     #define BKE_DIM_X 6 / BKE_DIM_Z 3
-//     #include "ukf_kernel.cuh"
+//     #include "ukf_kernel.cuh"                  // (UKF: also ukf_rts_kernel.cuh)
 //     /* user */ __device__ void fx(const real *x, real *out, real dt, const real *args) { ... }
 //     /* user */ __device__ void hx(const real *x, real *z, const real *args) { ... }
 //     template <> bke_user_fx<real> -> ::fx, bke_user_hx<real> -> ::hx
+// A UKF handle's measurement scores (bke_ukf_score_model) are compiled on the first call, as a program of their own: the
+// same text with ukf_score_kernel.cuh included and the score kernel as its one name.  Compiling them with the step would
+// add a quarter or more to every handle's compile time, whether it ever scores or not.
 #include <dlfcn.h>
+#include <mutex>
 #include <nvrtc.h>
 #include <stdlib.h>
 #include <string.h>
@@ -36,6 +40,9 @@ struct bke_ukf_model {
     cudaLibrary_t lib;
     cudaKernel_t kern[2];          // [0] plain, [1] with the optional outputs
     cudaKernel_t kern_rts;         // RTS smoother around the user's fx or hooks (NULL: neither, or dim_x > UR_MAXN)
+    cudaLibrary_t score_lib;       // UKF: the measurement scores (bke_ukf_score_model), compiled on its first call
+    cudaKernel_t kern_score;
+    std::string source, include_dirs;   // what the score program is compiled from
     unsigned hooks;                // BKE_HOOK_* mask the program was compiled with
     bool simplex;                  // UKF: compiled for the simplex point set (BKE_UKF_SIMPLEX)
     int regs[2];
@@ -161,11 +168,12 @@ using namespace bke;
 extern "C" {
 
 // NVRTC half of bke_ukf_model_compile / bke_ckf_model_compile (needs no GPU): program text -> sm_90a cubin
-// + the lowered names of the kernel instances of the family (the step with / without the optional outputs
-// and, for a UKF around a user fx or hooks, the RTS smoother)
+// + the lowered names of the kernel instances of the family (the step with / without the optional outputs and,
+// for a UKF around a user fx or hooks, the RTS smoother); `score`: the UKF's measurement-score program instead, whose
+// one name is lowered[3]
 static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, unsigned hooks,
-                         bool simplex, const char *source, const char *include_dirs, std::vector<char> &cubin, std::string (&lowered)[3],
-                         std::string &log)
+                         bool simplex, const char *source, const char *include_dirs, std::vector<char> &cubin, std::string (&lowered)[4],
+                         std::string &log, bool score = false)
 {
     const bool ckf = family == BKE_FAMILY_CKF, enkf = family == BKE_FAMILY_ENKF;
     const char *fn = simplex ? "bke_ukf_model_compile_points"
@@ -210,6 +218,7 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     if (hooks || simplex)
         text += "#define BKE_N_SIGMAS " + std::to_string(ckf ? 2 * dim_x : simplex ? dim_x + 1 : 2 * dim_x + 1) + "\n";
     text += enkf ? "#include \"enkf_kernel.cuh\"\n" : ckf ? "#include \"ckf_kernel.cuh\"\n" : "#include \"ukf_kernel.cuh\"\n#include \"ukf_rts_kernel.cuh\"\n";
+    if (score) text += "#include \"ukf_score_kernel.cuh\"\n";
     text += "#line 1 \"user_model.cu\"\n";
     text += source;
     text += "\n#line 1 \"bke_glue.cu\"\nnamespace bke { namespace ukfk {\n";
@@ -242,12 +251,17 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     }
     std::vector<const char *> copts;
     for (auto &o : opts) copts.push_back(o.c_str());
-    // the step kernel with / without the optional outputs and, around a user fx or hooks, the RTS smoother
-    const bool with_rts = !ckf && !enkf && (ufx || hooks) && dim_x <= UR_MAXN;
-    const int n_names = with_rts ? 3 : 2;
-    const std::string names[3] = {kernel_name(tmp, occ, false), kernel_name(tmp, occ, true),
-                                  std::string("bke::ukf_rts_kernel<real, ") + (ufx ? "true" : "false") + (simplex ? ", true>" : ">")};
-    for (int i = 0; i < n_names; i++) rt->add_name(prog, names[i].c_str());
+    // the step kernel with / without the optional outputs and, around a user fx or hooks, the RTS smoother; or the
+    // measurement scores alone (an empty name: no such kernel in this program)
+    const bool with_rts = !score && !ckf && !enkf && (ufx || hooks) && dim_x <= UR_MAXN;
+    std::string names[4];
+    if (!score) { names[0] = kernel_name(tmp, occ, false); names[1] = kernel_name(tmp, occ, true); }
+    if (with_rts) names[2] = std::string("bke::ukf_rts_kernel<real, ") + (ufx ? "true" : "false") + (simplex ? ", true>" : ">");
+    if (score)
+        names[3] = "bke::ukfk::ukf_score_kernel<real, " + std::to_string(dim_x) + ", " + std::to_string(dim_z) + ", " +
+                   std::to_string(hx_model) + ", " + std::to_string(occ) + (simplex ? ", true>" : ", false>");
+    for (int i = 0; i < 4; i++)
+        if (!names[i].empty()) rt->add_name(prog, names[i].c_str());
     r = rt->compile(prog, (int)copts.size(), copts.data());
     size_t lsz = 0;
     rt->log_size(prog, &lsz);
@@ -262,8 +276,9 @@ static int compile_cubin(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     rt->cubin_size(prog, &csz);
     cubin.resize(csz);
     rt->cubin(prog, cubin.data());
-    lowered[2].clear();
-    for (int i = 0; i < n_names; i++) {
+    for (int i = 0; i < 4; i++) {
+        lowered[i].clear();
+        if (names[i].empty()) continue;
         const char *ln = nullptr;
         if (rt->lowered(prog, names[i].c_str(), &ln) != NVRTC_SUCCESS || !ln) {
             set_error("nvrtcGetLoweredName failed for %s", names[i].c_str());
@@ -282,7 +297,7 @@ static int model_compile(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     if (!out) { set_error("out is NULL"); return BKE_ERR_BAD_ARG; }
     *out = nullptr;
     std::vector<char> cubin;
-    std::string lowered[3], log;
+    std::string lowered[4], log;
     int rc = compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, hooks, simplex, source, include_dirs, cubin, lowered, log);
     if (rc != BKE_OK) return rc;
     bke_ukf_model *m = new bke_ukf_model();
@@ -290,6 +305,10 @@ static int model_compile(int family, int32_t dim_x, int32_t dim_z, int32_t dtype
     m->hooks = hooks;
     m->simplex = simplex;
     m->kern_rts = nullptr;
+    m->score_lib = nullptr;
+    m->kern_score = nullptr;
+    m->source = source;
+    m->include_dirs = include_dirs;
     if (check_cuda(cudaLibraryLoadData(&m->lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0), "cudaLibraryLoadData")) { delete m; return BKE_ERR_CUDA; }
     for (int i = 0; i < 2; i++) {
         if (check_cuda(cudaLibraryGetKernel(&m->kern[i], m->lib, lowered[i].c_str()), "cudaLibraryGetKernel")) {
@@ -356,11 +375,12 @@ int bke_ckf_model_compile_hooks(int32_t dim_x, int32_t dim_z, int32_t dtype, int
 
 // the NVRTC half alone (CPU-only check that a model's text compiles for sm_90a): cubin size or 0
 static size_t cubin_bytes(int family, int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model, unsigned hooks,
-                          const char *source, const char *include_dirs, bool simplex = false)
+                          const char *source, const char *include_dirs, bool simplex = false, bool score = false)
 {
     std::vector<char> cubin;
-    std::string lowered[3], log;
-    if (compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, hooks, simplex, source, include_dirs, cubin, lowered, log) != BKE_OK) return 0;
+    std::string lowered[4], log;
+    if (compile_cubin(family, dim_x, dim_z, dtype, fx_model, hx_model, hooks, simplex, source, include_dirs, cubin, lowered, log, score) != BKE_OK)
+        return 0;
     return cubin.size();
 }
 
@@ -401,6 +421,13 @@ size_t bke_debug_ukf_model_points_cubin_bytes(int32_t dim_x, int32_t dim_z, int3
     return cubin_bytes(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs, points != 0u);
 }
 
+size_t bke_debug_ukf_score_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
+                                              uint32_t hooks, uint32_t points, const char *source, const char *include_dirs)
+{
+    if (check_points(points)) return 0;
+    return cubin_bytes(BKE_FAMILY_UKF, dim_x, dim_z, dtype, fx_model, hx_model, hooks, source, include_dirs, points != 0u, true);
+}
+
 const char *bke_ukf_model_log(const bke_ukf_model *m) { return m ? m->log.c_str() : ""; }
 
 int bke_ukf_model_registers(const bke_ukf_model *m, int32_t extras) { return m ? m->regs[extras ? 1 : 0] : -1; }
@@ -409,6 +436,7 @@ void bke_ukf_model_free(bke_ukf_model *m)
 {
     if (!m) return;
     if (m->lib) cudaLibraryUnload(m->lib);
+    if (m->score_lib) cudaLibraryUnload(m->score_lib);
     delete m;
 }
 
@@ -459,6 +487,69 @@ int bke_ukf_rts_smoother_model(const bke_ukf_rts_args *args, const bke_ukf_model
     if (check_cuda(cudaLaunchKernel((const void *)model->kern_rts, dim3((unsigned)((a.n_filters + 63) / 64)), dim3(64), params, 0, (cudaStream_t)stream),
                    "ukf rts model launch")) return BKE_ERR_CUDA;
     return BKE_OK;
+}
+
+// the handle's measurement-score program, compiled and loaded on the first bke_ukf_score_model call
+static int load_score_kernel(bke_ukf_model &m)
+{
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lock(mu);
+    if (m.kern_score) return BKE_OK;
+    std::vector<char> cubin;
+    std::string lowered[4], log;
+    int rc = compile_cubin(m.family, m.n, m.m, m.dtype, m.fx_model, m.hx_model, m.hooks, m.simplex, m.source.c_str(), m.include_dirs.c_str(),
+                           cubin, lowered, log, true);
+    if (rc != BKE_OK) return rc;
+    cudaLibrary_t lib;
+    if (check_cuda(cudaLibraryLoadData(&lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0), "cudaLibraryLoadData (score)")) return BKE_ERR_CUDA;
+    cudaKernel_t k;
+    if (check_cuda(cudaLibraryGetKernel(&k, lib, lowered[3].c_str()), "cudaLibraryGetKernel (score)")) { cudaLibraryUnload(lib); return BKE_ERR_CUDA; }
+    m.score_lib = lib;
+    m.kern_score = k;
+    return BKE_OK;
+}
+
+}  // extern "C"
+
+template <typename T>
+static int launch_score_model(const bke_ukf_score_args &a, const bke_ukf_model &m, const void *hx_args, int64_t s_hx, cudaStream_t s)
+{
+    ukfk::UkfScoreP<T> p;
+    ukf_score_fill_params<T>(a, p);
+    p.hx_args = (const T *)hx_args; p.s_hx_args = s_hx;
+    const size_t smem = ukf_score_smem_bytes<T>(m.n, m.m, m.simplex, m.hx_model == BKE_HX_LINEAR, a.H_stride == 0);
+    // the slot of S^-1 grows with dim_z^2, so a model that steps may still not fit the score's shared memory
+    const size_t smem_max = 227 * 1024;                      // the most one CTA may use on sm_90
+    if (smem > smem_max) {
+        set_error("bke_ukf_score_model: dim_x=%d dim_z=%d needs %zu B of shared memory per CTA (> %zu)", m.n, m.m, smem, smem_max);
+        return BKE_ERR_UNSUPPORTED;
+    }
+    if (int rc = load_score_kernel(const_cast<bke_ukf_model &>(m))) return rc;
+    return launch_kernel((const void *)m.kern_score, ukf_grid(p.N), ukfk::UB, smem, &p, s, "ukf score model launch");
+}
+
+extern "C" {
+
+int bke_ukf_score_model(const bke_ukf_score_args *args, const bke_ukf_model *model, const void *hx_args, int64_t hx_args_stride, void *stream)
+{
+    if (!args || !model) { set_error("args / model is NULL"); return BKE_ERR_BAD_ARG; }
+    const bke_ukf_score_args &a = *args;
+    int rc;
+    if ((rc = check_family(*model, BKE_FAMILY_UKF, "bke_ukf_score_model")) || (rc = validate_ukf_score(a))) return rc;
+    if (a.dim_x != model->n || a.dim_z != model->m || a.dtype != model->dtype || a.hx_model != model->hx_model) {
+        set_error("bke_ukf_score_model: args (dim_x=%d dim_z=%d dtype=%d hx=%d) do not match the compiled model (%d %d %d %d)", a.dim_x,
+                  a.dim_z, a.dtype, a.hx_model, model->n, model->m, model->dtype, model->hx_model);
+        return BKE_ERR_BAD_ARG;
+    }
+    if (((a.flags & BKE_UKF_SIMPLEX) != 0) != model->simplex) {
+        set_error("bke_ukf_score_model: the model was compiled for the %s point set, the call asks for the %s set",
+                  model->simplex ? "simplex" : "Merwe", model->simplex ? "Merwe" : "simplex");
+        return BKE_ERR_BAD_ARG;
+    }
+    if (hx_args_stride < 0) { set_error("negative args stride"); return BKE_ERR_BAD_ARG; }
+    if (a.n_filters == 0 || a.n_candidates == 0) return BKE_OK;
+    return a.dtype == BKE_F32 ? launch_score_model<float>(a, *model, hx_args, hx_args_stride, (cudaStream_t)stream)
+                              : launch_score_model<double>(a, *model, hx_args, hx_args_stride, (cudaStream_t)stream);
 }
 
 int bke_ckf_step_model(const bke_ckf_args *args, const bke_ukf_model *model, const void *fx_args, int64_t fx_args_stride,

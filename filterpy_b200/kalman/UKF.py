@@ -24,7 +24,8 @@ import numpy as np
 import torch
 
 from .. import _lib
-from .._dev import bke_dtype, ptr, stream_ptr
+from .._dev import bke_dtype, ptr, stream_ptr, to_dev
+from ..stats.stats import _candidates, _valid
 from ._bank import _BankMirror, _model_prop
 from .sigma_points import SimplexSigmaPoints
 
@@ -352,6 +353,69 @@ class UnscentedKalmanFilter(_SigmaPointBank):
         if not self._point_flag:
             a.alpha, a.beta, a.kappa = self.points_fn.alpha, self.points_fn.beta, self.points_fn.kappa
         self._step(a, self._lib.bke_ukf_step, self._lib.bke_ukf_step_model)
+
+    # ------------------------------------------------------------------ scores without a step
+    def score_measurements(self, z, valid=None, **hx_args):
+        """Gate candidates against the bank: for every track and candidate, the ``log_likelihood`` and
+        ``mahalanobis`` the reference reports right after ``update(z)`` from the track's current state
+        (UKF.py:459-477, 742-777), computed without updating: the sigma points of (x, P), hx, the unscented
+        transform with R (and z_mean_fn / residual_z when given), then the scores of each candidate.  A pending
+        ``predict`` is committed first, so the scores are against the prior the next ``update`` uses; x, P and
+        the diagnostics are otherwise left exactly as they were.
+
+        Bank mode: ``z`` is ``[N, m]`` (results ``[N]``), ``[N, K, m]`` or ``[1, K, m]`` (one scan for the whole
+        bank; results ``[N, K]``); ``valid`` (bool, one per pair) marks missing candidates, which score
+        log(DBL_MIN) and distance 0.  Returns device tensors ``(log_likelihood, mahalanobis)`` from one launch;
+        a track whose P is not positive definite or whose S is singular scores NaN.  Single mode: ``z`` holds
+        ``m`` values and the result is two floats; those failures raise ``LinAlgError``.  ``hx_args`` are the
+        DeviceHx arguments for this call only."""
+        self._flush()
+        N, m = self.n_filters, self.dim_z
+        if self._single:
+            zt, sq = to_dev(np.asarray(z, dtype=np.float64).reshape(1, 1, -1), self._dtype, self._device), True
+            if zt.shape[-1] != m:
+                raise ValueError("z must hold %d values, got %d" % (m, zt.shape[-1]))
+        else:
+            zt, sq = _candidates(z, N, m, self._dtype, self._device)
+        K = zt.shape[1]
+        vt = _valid(valid, N, K, self._device)
+        hx_t, hx_stride = self._hx_args
+        if hx_args:
+            if not isinstance(self.hx, _DeviceModel):
+                raise NotImplementedError("hx_args are arguments of a Python callback; the built-in measurement models take none")
+            kept = dict(self.hx.values)
+            try:
+                hx_t, hx_stride = self.hx.pack(hx_args, N, self._dtype, self._device)
+            finally:
+                self.hx.values = kept
+        if isinstance(self.hx, _DeviceModel) and self.hx.arg_names and hx_t is None:
+            raise TypeError("hx needs values for its arguments %s" % list(self.hx.arg_names))
+        kw = dict(dtype=self._dtype, device=self._device)
+        ll, maha = torch.empty(N, K, **kw), torch.empty(N, K, **kw)
+        status = torch.empty(N, dtype=torch.int32, device=self._device)
+        a = _lib.UkfScoreArgs()
+        a.n_filters, a.n_candidates, a.dim_x, a.dim_z = N, K, self.dim_x, m
+        a.dtype, a.flags, a.hx_model = bke_dtype(self._dtype), self._point_flag, self.hx.model
+        if not self._point_flag:
+            a.alpha, a.beta, a.kappa = self.points_fn.alpha, self.points_fn.beta, self.points_fn.kappa
+        a.x, a.P = ptr(self._x), ptr(self._P)
+        a.R, a.R_stride = ptr(self._R), self._stride(self._R)
+        if self._H is not None:
+            a.H, a.H_stride = ptr(self._H), self._stride(self._H)
+        a.z, a.z_track_stride, a.z_cand_stride = ptr(zt), (0 if zt.shape[0] == 1 else K * m), m
+        a.z_valid = ptr(vt)
+        a.log_likelihood, a.mahalanobis, a.status = ptr(ll), ptr(maha), ptr(status)
+        if K > 0:
+            if self._user_model is None:
+                self._run(self._lib.bke_ukf_score, ctypes.byref(a), stream_ptr(self._device))
+            else:
+                self._run(self._lib.bke_ukf_score_model, ctypes.byref(a), self._user_model, ptr(hx_t), hx_stride,
+                          stream_ptr(self._device))
+        if self._single:
+            if int(status[0].item()) != 0:
+                raise np.linalg.LinAlgError(self._FAILURE)
+            return float(ll[0, 0].item()), float(maha[0, 0].item())
+        return (ll[:, 0], maha[:, 0]) if sq else (ll, maha)
 
     def rts_smoother(self, Xs, Ps, Qs=None, dts=None, UT=None):
         """UKF.py:634-739 on the GPU.  Bank mode: ``Xs[T,N,n]``, ``Ps[T,N,n,n]`` (what

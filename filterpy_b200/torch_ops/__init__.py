@@ -18,6 +18,8 @@ The same symbols exposed as torch.ops.* via a C++ extension for zero-copy CUDA t
                                                                    # gh_filter.py, least_squares.py, fading_memory.py
     ll, d = torch.ops.bke.score_measurements(z, x, None, P, None, H, R, None, ["log_likelihood", "mahalanobis"])
                                                                    # stats.py:64-154, N tracks x K candidates z[N|1, K, m]
+    ll, d, status = torch.ops.bke.ukf_score_measurements(x, P, R, z, alpha, beta, kappa, hx_model)
+                                                                   # UKF update(z) log_likelihood / mahalanobis per candidate
     means, covs, means_p, covs_p, mus = torch.ops.bke.imm_batch_filter(xs, Ps, Fs, Qs, Hs, Rs, alpha_sqs, Ss, lls, mu, cbar,
                                                                        trans, zs, valid)   # IMMEstimator.batch_filter
     xs, xhat = torch.ops.bke.fls_smooth_batch(x, P, F, H, Q, R, zs, N)   # fixed_lag_smoother.py:217-311

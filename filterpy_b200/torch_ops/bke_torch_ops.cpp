@@ -14,6 +14,8 @@
 //                                                      update (T epochs) and the g-h batch_filter, gh_filter.py, least_squares.py, fading_memory.py
 //   bke::score_measurements   bke_score_measurements   stats.mahalanobis / log_likelihood / logpdf / NEES and
 //                                                      KalmanFilter.log_likelihood_of, N tracks x K candidates
+//   bke::ukf_score_measurements  bke_ukf_score        UnscentedKalmanFilter.score_measurements: the log_likelihood and
+//                                                      mahalanobis of update(z_ik), N tracks x K candidates, UKF.py:459-477
 //   bke::imm_batch_filter     bke_imm_batch_filter     IMMEstimator.batch_filter: T epochs of predict(); update(z), IMM.py:160-247
 //   bke::fls_smooth_batch     bke_fls_smooth           FixedLagSmoother.smooth_batch, fixed_lag_smoother.py:217-311
 //   bke::systematic_resample  bke_systematic_resample  monte_carlo/resampling.py:117-150
@@ -336,6 +338,42 @@ std::vector<at::Tensor> score_measurements(const at::Tensor &z, const c10::optio
     if (N > 0 && K > 0)     // an empty tensor has no data pointer to pass
         check_rc(bke_score_measurements(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_score_measurements");
     return out;
+}
+
+// N UKF tracks against K candidates (bke_ukf_score, pre-built hx models): x [N, n], P [N, n, n], R and H shared
+// [r, c] or per track [N, r, c], z [N, K, m] or [1, K, m], valid [N, K] uint8.  Returns (log_likelihood, mahalanobis,
+// status), [N, K], [N, K] and [N].
+std::tuple<at::Tensor, at::Tensor, at::Tensor> ukf_score_measurements(const at::Tensor &x, const at::Tensor &P, const at::Tensor &R,
+                                                                      const at::Tensor &z, double alpha, double beta, double kappa,
+                                                                      int64_t hx_model, const c10::optional<at::Tensor> &H,
+                                                                      const c10::optional<at::Tensor> &valid, bool simplex)
+{
+    TORCH_CHECK(x.is_cuda() && P.is_cuda() && x.is_contiguous() && P.is_contiguous() && x.dim() == 2 && P.dim() == 3, "bke: x is [N, n], P is [N, n, n] on the GPU");
+    TORCH_CHECK(z.is_cuda() && z.device() == x.device() && z.is_contiguous() && z.scalar_type() == x.scalar_type() && z.dim() == 3,
+                "bke: z is a contiguous CUDA tensor [N, K, m] or [1, K, m] of x's dtype, on x's device");
+    c10::cuda::CUDAGuard guard(x.device());
+    const int64_t N = x.size(0), n = x.size(1), K = z.size(1), m = z.size(2);
+    TORCH_CHECK(z.size(0) == N || z.size(0) == 1, "bke: z is [N, K, m] or [1, K, m]");
+    bke_ukf_score_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_filters = N; a.n_candidates = K; a.dim_x = (int32_t)n; a.dim_z = (int32_t)m; a.dtype = dtype_of(x);
+    a.flags = simplex ? BKE_UKF_SIMPLEX : 0u; a.hx_model = (int32_t)hx_model;
+    a.alpha = alpha; a.beta = beta; a.kappa = kappa;
+    a.x = x.data_ptr(); a.P = P.data_ptr();
+    a.R = model(R, N, m, m, &a.R_stride, x, "R");
+    if (H.has_value() && H->defined()) a.H = model(*H, N, m, n, &a.H_stride, x, "H");
+    a.z = z.data_ptr(); a.z_track_stride = z.size(0) == 1 ? 0 : K * m; a.z_cand_stride = m;
+    if (valid.has_value() && valid->defined()) {
+        TORCH_CHECK(valid->is_cuda() && valid->device() == x.device() && valid->scalar_type() == at::kByte &&
+                    valid->is_contiguous() && valid->numel() == N * K, "bke: valid is a contiguous uint8 CUDA tensor [N, K] on x's device");
+        a.z_valid = valid->data_ptr<uint8_t>();
+    }
+    at::Tensor ll = at::empty({N, K}, x.options()), maha = at::empty({N, K}, x.options());
+    at::Tensor status = at::empty({N}, x.options().dtype(at::kInt));
+    a.log_likelihood = ll.data_ptr(); a.mahalanobis = maha.data_ptr(); a.status = status.data_ptr<int32_t>();
+    if (N > 0 && K > 0)     // an empty tensor has no data pointer to pass
+        check_rc(bke_ukf_score(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_ukf_score");
+    return std::make_tuple(ll, maha, status);
 }
 
 // a polynomial tracker parameter: 0-d (shared, stride 0) or [N] (per filter, stride 1); undefined = not given
@@ -709,6 +747,8 @@ TORCH_LIBRARY(bke, m)
           "Tensor? dt2, Tensor? hdt2, int family, int order, bool batch=False) -> (Tensor, Tensor, Tensor, Tensor, Tensor, Tensor)");
     m.def("score_measurements(Tensor z, Tensor? x, Tensor? mean, Tensor? P, Tensor? S, Tensor? H, Tensor? R, Tensor? valid, "
           "str[] outputs) -> Tensor[]");
+    m.def("ukf_score_measurements(Tensor x, Tensor P, Tensor R, Tensor z, float alpha, float beta, float kappa, int hx_model, "
+          "Tensor? H=None, Tensor? valid=None, bool simplex=False) -> (Tensor, Tensor, Tensor)");
     m.def("imm_batch_filter(Tensor(a!)[] x, Tensor(b!)[] P, Tensor[] F, Tensor[] Q, Tensor[] H, Tensor[] R, float[] alpha_sq, "
           "Tensor(c!)[] S, Tensor(d!)[] log_likelihood, Tensor(e!) mu, Tensor(f!) cbar, Tensor trans, Tensor zs, "
           "Tensor? zs_valid=None) -> (Tensor, Tensor, Tensor, Tensor, Tensor)");
@@ -732,6 +772,7 @@ TORCH_LIBRARY_IMPL(bke, CUDA, m)
     m.impl("kf_step_correlated", &kf_step_correlated);
     m.impl("kf_update_rows", &kf_update_rows);
     m.impl("ukf_step", &ukf_step);
+    m.impl("ukf_score_measurements", &ukf_score_measurements);
     m.impl("ckf_step", &ckf_step);
     m.impl("enkf_step", &enkf_step);
     m.impl("srkf_step", &srkf_step);

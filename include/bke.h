@@ -768,6 +768,53 @@ typedef struct bke_score_args {
 
 int bke_score_measurements(const bke_score_args *args, void *stream);
 
+/* Measurement scoring against UKF banks: N tracks against K candidates each, without stepping anything.  Per
+ * track i and candidate z_ik, what UnscentedKalmanFilter reports as log_likelihood and mahalanobis right after
+ * update(z_ik) from the track's current (x, P) (UKF.py:459-477, 742-777):
+ *   sigma points of (x, P) (Merwe, or the simplex set with BKE_UKF_SIMPLEX: UKF.py:407);  Zs = hx(Xs);
+ *   (zhat, S) = UT(Zs, Wm, Wc, R) with z_mean_fn / residual_z where a run-time model has them;
+ *   y = residual_z(z_ik, zhat);  d2 = y' S^-1 y;  mahalanobis = sqrt(d2);
+ *   log_likelihood = -0.5 (d2 + log|det S| + m log 2pi);  likelihood = exp(log_likelihood)
+ * with S^-1 and log|det S| from the step kernels' inverse.  Every field shared with bke_score_args has its meaning,
+ * shape and NULL rule there: a pair with z_valid == 0 scores y = d2 = mahalanobis = 0 and log(DBL_MIN); a singular S
+ * is status[i] = BKE_STATUS_SINGULAR_S and a P whose Cholesky fails BKE_STATUS_NOT_PD, and the track's valid pairs
+ * then get NaN scores.  x[N,n], P[N,n,n], R[N,m,m] (stride m*m or 0) and, for BKE_HX_LINEAR, H (stride m*n or 0)
+ * are read and nothing else is touched.  hx_model is one of the pre-built models (BKE_HX_*, in the dim_x / dim_z
+ * instances bke_ukf_step has); bke_ukf_score_model runs a handle of bke_ukf_model_compile[_hooks|_points] (its
+ * dim_x, dim_z, dtype, hx_model and point set must match; hx_args as for bke_ukf_step_model) and refuses a CKF or
+ * EnKF handle.  A CTA of 128 tracks holds the hx of their sigma points and 128 slots of m + m^2 + 1 words in shared
+ * memory: the pre-built instances need 2.5-73 KB; a run-time model whose score needs more than 227 KB (large dim_z,
+ * e.g. dim_x = 4, dim_z = 12 in fp64: 265 KB, where the step needs 118 KB) returns BKE_ERR_UNSUPPORTED from
+ * bke_ukf_score_model even where it can step.
+ * N = 0 or K = 0 launches nothing.  The call allocates nothing, so it can be captured.
+ * Kernel (DESIGN.md §3.5h): a CTA per tile of 128 tracks runs the step's measurement half into shared memory, then
+ * sweeps the tile's pairs as bke_score_measurements does. */
+typedef struct bke_ukf_score_args {
+    int64_t n_filters;               /* N */
+    int64_t n_candidates;            /* K */
+    int32_t dim_x, dim_z;            /* n, m */
+    int32_t dtype;
+    uint32_t flags;                  /* 0 or BKE_UKF_SIMPLEX */
+    int32_t hx_model;
+    int32_t reserved;
+    double alpha, beta, kappa;       /* MerweScaledSigmaPoints(n, alpha, beta, kappa); ignored with BKE_UKF_SIMPLEX */
+    const void *x, *P;               /* [N,n], [N,n,n] */
+    const void *R; int64_t R_stride; /* [N,m,m] */
+    const void *H; int64_t H_stride; /* [N,m,n]; BKE_HX_LINEAR only */
+    const void *z; int64_t z_track_stride, z_cand_stride;
+    const uint8_t *z_valid;          /* [N,K] or NULL */
+    void *zhat, *y, *d2, *mahalanobis, *log_likelihood, *likelihood;
+    int32_t *status;
+} bke_ukf_score_args;
+
+int bke_ukf_score(const bke_ukf_score_args *args, void *stream);
+int bke_ukf_score_model(const bke_ukf_score_args *args, const bke_ukf_model *model, const void *hx_args, int64_t hx_args_stride,
+                        void *stream);
+/* A handle compiles its score kernel (NVRTC, its own program) on its first bke_ukf_score_model call with N, K > 0; make
+ * that call before capturing one.  The NVRTC half alone (needs no GPU): cubin size of that program, 0 on failure. */
+size_t bke_debug_ukf_score_model_cubin_bytes(int32_t dim_x, int32_t dim_z, int32_t dtype, int32_t fx_model, int32_t hx_model,
+                                              uint32_t hooks, uint32_t points, const char *source, const char *include_dirs);
+
 /* Stand-alone pieces of the unscented path for callers that use them directly:
  *   MerweScaledSigmaPoints.sigma_points(x, P)   filterpy/kalman/sigma_points.py:124-177
  *       x[N,n], P[N,n,n] -> sigmas[N,2n+1,n]; status[N] = BKE_STATUS_NOT_PD where scipy's cholesky
