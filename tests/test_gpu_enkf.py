@@ -4,7 +4,7 @@ KalmanFilter bank, and the failure statuses."""
 import numpy as np
 import pytest
 
-from test_gpu_kf import rel_close, RTOL
+from gpu_harness import rel_close, RTOL
 from test_oracle_enkf import GOLDEN, update_R
 from oracle import enkf as oe
 

@@ -3,7 +3,7 @@ vectors and the vectorised oracle."""
 import numpy as np
 import pytest
 
-from test_gpu_kf import rel_close, RTOL
+from gpu_harness import rel_close, RTOL
 from test_oracle_fls import BANKS, bank_inputs
 
 pytestmark = pytest.mark.gpu

@@ -25,12 +25,9 @@ import re
 import numpy as np
 import pytest
 
-from test_gpu_imm_instances import stable_F
-from test_gpu_kf_instances import Bufs, _body, _ptr, _rd, _spd, _src, k_direct, k_fast, k_gen, k_rb, rb_fpw
+from gpu_harness import (F32, F64, ROOT, TNAME, Bufs, body, call, check_launch_order, close, k_direct, k_fast, k_gen,
+                         k_rb, mag, profiled_names, ptr, rb_fpw, rd, spd, src, stable_F)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-F32, F64 = np.float32, np.float64
-TNAME = {F32: "float", F64: "double"}
 MAX_LAG = 16                                     # BKE_FLS_FUSED_MAX_LAG
 THREADS = 128                                    # fls.cu FLS_THREADS
 
@@ -38,6 +35,12 @@ TOL = {
     "fused": {F64: 3e-14, F32: 1.7e-5},
     "epoch": {F64: 2.5e-14, F32: 8e-6},
 }
+
+
+def _bound(c):
+    """Case c's tolerance and the label of its BKE_TEST_ERRLOG lines."""
+    return TOL[c.family][c.dt], "test_gpu_fls_instances %s %s" % (c.family, np.dtype(c.dt).name)
+
 
 FUSED = [(1, 1), (2, 1), (4, 2)]
 ERR_WS = ("bke_fls_smooth: this call runs the per-epoch path and needs a workspace of %d bytes "
@@ -155,19 +158,19 @@ RUNS = [c for c in CASES if c.kind != "refused"]
 
 # ------------------------------------------------------------------------------------------ the table vs the source
 def _dispatched():
-    src = _src("fls.cu")
-    fs = _body(src, "bool fused_shape(int n, int m, int du_used, int dtype, int64_t lag)")
+    text = src("fls.cu")
+    fs = body(text, "bool fused_shape(int n, int m, int du_used, int dtype, int64_t lag)")
     assert "du_used == 0 && lag <= BKE_FLS_FUSED_MAX_LAG" in fs
     shapes = [(int(a), int(b)) for a, b in re.findall(r"\(n == (\d+) && m == (\d+)\)", fs)]
-    lf = _body(src, "int launch_fls(const bke_fls_args &a, cudaStream_t s)")
+    lf = body(text, "int launch_fls(const bke_fls_args &a, cudaStream_t s)")
     inst = set()
     for t, n, m in re.findall(r"launch_fused<(\w+), (\d+), (\d+)>\(a, s\)", lf):
         inst.add("fls_fused_kernel<%s, %s, %s>" % (t, n, m))
     assert "launch_per_epoch<float>(a, s) : launch_per_epoch<double>(a, s)" in lf
-    assert "fls_correct_kernel<T><<<" in _body(src, "int launch_per_epoch(const bke_fls_args &a, cudaStream_t s)")
-    assert "int rc = launch_kf_any(k, s);" in src
-    assert re.search(r"constexpr int FLS_THREADS = %d;" % THREADS, src)
-    assert "const size_t smem = (size_t)a.lag * N * FLS_THREADS * sizeof(T);" in src
+    assert "fls_correct_kernel<T><<<" in body(text, "int launch_per_epoch(const bke_fls_args &a, cudaStream_t s)")
+    assert "int rc = launch_kf_any(k, s);" in text
+    assert re.search(r"constexpr int FLS_THREADS = %d;" % THREADS, text)
+    assert "const size_t smem = (size_t)a.lag * N * FLS_THREADS * sizeof(T);" in text
     assert ERR_WS.replace("%d", "%zu") in lf.replace('"\n                  "', "") and ERR_WS_ALIGN in lf
     with open(os.path.join(ROOT, "include", "bke.h")) as fh:
         assert re.search(r"#define BKE_FLS_FUSED_MAX_LAG %d\b" % MAX_LAG, fh.read())
@@ -221,14 +224,14 @@ def fls_inputs(c, g, seed):
     rng = np.random.default_rng(seed)
     n, m, N, T, dt = c.n, c.m, g.N, g.T, c.dt
     cnt = () if g.shared else (N,)
-    d = dict(x=rng.normal(size=(N, n)) * 3, P=_spd(rng, (N,), n, 2.0),
-             F=stable_F(rng, cnt, n), Q=_spd(rng, cnt, n, 0.05),
-             H=rng.normal(size=cnt + (m, n)), R=_spd(rng, cnt, m, 0.5), zs=rng.normal(size=(T, N, m)) * 3,
+    d = dict(x=rng.normal(size=(N, n)) * 3, P=spd(rng, (N,), n, 2.0),
+             F=stable_F(rng, cnt, n), Q=spd(rng, cnt, n, 0.05),
+             H=rng.normal(size=cnt + (m, n)), R=spd(rng, cnt, m, 0.5), zs=rng.normal(size=(T, N, m)) * 3,
              hist=rng.normal(size=(g.count, N, n)) * 3)
     if c.ctrl:
         d["B"] = rng.normal(size=cnt + (n, 2))
         d["us"] = rng.normal(size=(T, N, 2))
-    return {k: _rd(v, dt) for k, v in d.items()}
+    return {k: rd(v, dt) for k, v in d.items()}
 
 
 def run_fls(c, g, d, ws=None):
@@ -243,30 +246,30 @@ def run_fls(c, g, d, ws=None):
     k = a.step
     k.n_filters, k.dim_x, k.dim_z = N, n, m
     k.dtype = _lib.BKE_F32 if dt == F32 else _lib.BKE_F64
-    k.x, k.P = _ptr(bf.put(d["x"])), _ptr(bf.put(d["P"]))
+    k.x, k.P = ptr(bf.put(d["x"])), ptr(bf.put(d["P"]))
     xo, Po = bf.out((N, n), fill=nan), bf.out((N, n, n), fill=nan)
-    k.x_out, k.P_out = _ptr(xo), _ptr(Po)
+    k.x_out, k.P_out = ptr(xo), ptr(Po)
     for name in "FQHR":
         arr = d[name]
-        setattr(k, name, _ptr(bf.put(arr)))
+        setattr(k, name, ptr(bf.put(arr)))
         setattr(k, name + "_stride", 0 if arr.ndim == 2 else arr.shape[-1] * arr.shape[-2])
     if c.ctrl:
         k.dim_u = 2
-        k.B = _ptr(bf.put(d["B"])); k.B_stride = 0 if d["B"].ndim == 2 else 2 * n
-        a.us = _ptr(bf.put(d["us"]))
+        k.B = ptr(bf.put(d["B"])); k.B_stride = 0 if d["B"].ndim == 2 else 2 * n
+        a.us = ptr(bf.put(d["us"]))
     outs = {}
     if not g.null:
         outs["y"], outs["S"] = bf.out((N, m), fill=nan), bf.out((N, m, m), fill=nan)
-        k.y, k.S = _ptr(outs["y"]), _ptr(outs["S"])
+        k.y, k.S = ptr(outs["y"]), ptr(outs["S"])
         outs["xhat"] = bf.out((T, N, n), fill=nan)
-        a.xhat = _ptr(outs["xhat"])
+        a.xhat = ptr(outs["xhat"])
     st = bf.out((N,), dtype=np.int32, fill=5)
-    k.status = _ptr(st)
+    k.status = ptr(st)
     hist = np.concatenate([d["hist"], np.full((T, N, n), nan)])
     xs = bf.put(hist, out=True)
-    a.xs_smooth = _ptr(xs)
+    a.xs_smooth = ptr(xs)
     a.n_steps, a.lag, a.count = T, g.lag, g.count
-    a.zs = _ptr(bf.put(d["zs"]))
+    a.zs = ptr(bf.put(d["zs"]))
     need = lib.bke_fls_workspace_bytes(N, n, m, 2 if c.ctrl else 0, k.dtype, g.lag)
     wsbuf = torch.full((need + 32,), 255, dtype=torch.uint8, device="cuda")
     base = wsbuf.data_ptr()
@@ -278,9 +281,7 @@ def run_fls(c, g, d, ws=None):
         a.workspace, a.workspace_bytes = base + 4, need
     elif need:
         a.workspace, a.workspace_bytes = base, need
-    rc = lib.bke_fls_smooth(ctypes.byref(a), torch.cuda.current_stream().cuda_stream)
-    err = lib.bke_last_error().decode()
-    torch.cuda.synchronize()
+    rc, err = call("bke_fls_smooth", ctypes.byref(a))
     got = dict(x=xo.cpu().numpy().reshape(N, n), P=Po.cpu().numpy().reshape(N, n, n), status=st.cpu().numpy(),
                xs=xs.cpu().numpy().reshape(g.count + T, N, n))
     for name, shp in (("y", (N, m)), ("S", (N, m, m)), ("xhat", (T, N, n))):
@@ -295,50 +296,26 @@ def fls_oracle(c, d, g):
                          count=g.count, hist=d["hist"] if g.count else None)
 
 
-# ------------------------------------------------------------------------------------------ comparisons
-def _errlog(c, what, err, tol):
-    log = os.environ.get("BKE_TEST_ERRLOG")
-    if log:
-        with open(log, "a") as fh:
-            fh.write("test_gpu_fls_instances %s %s %s max_err=%.3e tol=%.1e\n"
-                     % (c.family, np.dtype(c.dt).name, what, err, tol))
-
-
-def _close(c, got, want, scale, cond, what):
-    """|got - want| <= TOL * scale * cond per filter (axis 0)."""
-    tol = TOL[c.family][c.dt]
-    got = np.asarray(got, np.float64); want = np.asarray(want, np.float64)
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    assert np.all(np.isfinite(got)), "%s: not finite (a row never written?)" % what
-    sh = (-1,) + (1,) * (want.ndim - 1)
-    err = np.abs(got - want) / (np.maximum(scale, 1e-300).reshape(sh) * cond.reshape(sh))
-    _errlog(c, what, err.max(), tol)
-    assert err.max() <= tol, "%s: max err %.3e of the filter's scale x cond > %.1e" % (what, err.max(), tol)
-
-
-def _fmax(*arrs):
-    return np.max([np.abs(a).reshape(a.shape[0], -1).max(axis=1) for a in arrs], axis=0)
-
-
 def check_fls(c, g, d, got, want, what):
     sw = lambda a: np.swapaxes(a, 0, 1)
     cond = want["cond"]
+    tol, label = _bound(c)
     L0 = max(g.count - g.lag + 1, 0) if g.lag else g.count
     # the final rows before the live window are left as they were
     assert np.array_equal(got["xs"][:L0], d["hist"][:L0]), what + " a final history row changed"
-    sx = _fmax(d["x"], sw(want["xs"]), sw(want["xhat"]), want["x"])
-    _close(c, sw(got["xs"]), sw(want["xs"]), sx, cond, what + " xs")
-    _close(c, got["x"], want["x"], sx, cond, what + " x_out")
-    _close(c, got["P"], want["P"], _fmax(d["P"], want["P"]), cond, what + " P_out")
+    sx = mag(d["x"], sw(want["xs"]), sw(want["xhat"]), want["x"])
+    close(sw(got["xs"]), sw(want["xs"]), sx, cond, tol, what + " xs", label)
+    close(got["x"], want["x"], sx, cond, tol, what + " x_out", label)
+    close(got["P"], want["P"], mag(d["P"], want["P"]), cond, tol, what + " P_out", label)
     assert np.array_equal(got["status"], want["status"]), what + " status"
     if g.null:
         return
-    _close(c, sw(got["xhat"]), sw(want["xhat"]), sx, cond, what + " xhat")
+    close(sw(got["xhat"]), sw(want["xhat"]), sx, cond, tol, what + " xhat", label)
     H = np.broadcast_to(d["H"], (g.N, c.m, c.n))
     sy = np.abs(d["zs"][-1]).max(axis=1) + np.abs(H).max(axis=(1, 2)) * np.abs(want["xs"][-1]).sum(axis=1) + \
-        _fmax(want["y"])
-    _close(c, got["y"], want["y"], sy, cond, what + " y")
-    _close(c, got["S"], want["S"], _fmax(want["S"]), cond, what + " S")
+        mag(want["y"])
+    close(got["y"], want["y"], sy, cond, tol, what + " y", label)
+    close(got["S"], want["S"], mag(want["S"]), cond, tol, what + " S", label)
 
 
 @pytest.mark.gpu
@@ -402,15 +379,14 @@ def test_refused_workspace(case):
 
 
 # ------------------------------------------------------------------------------------------ which kernel runs
+def _run_cases():
+    for c in CASES:
+        g = c.cfgs[0]
+        run_fls(c, g, fls_inputs(c, g, seed=1), ws=c.ws)
+
+
 def _profiled_names():
-    from torch.profiler import profile, ProfilerActivity
-    from test_gpu_imm_instances import _kernel_name
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for c in CASES:
-            g = c.cfgs[0]
-            run_fls(c, g, fls_inputs(c, g, seed=1), ws=c.ws)
-    names = [_kernel_name(e.name) for e in sorted(prof.events(), key=lambda e: e.time_range.start)]
-    return [k for k in names if k]
+    return profiled_names(_run_cases, r"kf\w*_kernel|fls_\w+_kernel")
 
 
 @pytest.mark.gpu
@@ -418,22 +394,4 @@ def test_dispatch_runs_the_kernels_of_the_table():
     """Each CASES entry, run once at its first configuration, launches the kernels the table names, in order: one
     fused kernel, or T x (the step kernel, fls_correct_kernel); a refused call launches nothing.  The profile is
     taken in a process of its own."""
-    import json
-    import subprocess
-    import sys
-    here = os.path.dirname(os.path.abspath(__file__))
-    code = ("import json, sys; sys.path[:0] = %r; import test_gpu_fls_instances as t; "
-            "print(json.dumps(t._profiled_names()))" % [here, os.path.dirname(here)])
-    r = subprocess.run([sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    names = json.loads(r.stdout.strip().splitlines()[-1])
-    pos, bad = 0, []
-    for c in CASES:
-        want = c.launches()
-        got = names[pos:pos + len(want)]
-        if got != want:
-            bad.append((c.id, want, got))
-            break
-        pos += len(want)
-    assert not bad and pos == len(names), (bad, names[pos:pos + 5])
+    check_launch_order("test_gpu_fls_instances", [(c.id, c.launches()) for c in CASES])

@@ -23,18 +23,15 @@ each:
     inv   inverse_kernel               2.4e-16    1e-15     7.7e-8      4e-7
 """
 import ctypes
-import os
 import re
 from fractions import Fraction
 
 import numpy as np
 import pytest
 
-from test_gpu_kf_instances import Bufs, _body, _mag, _ptr, _rd, _src
-from test_gpu_srkf_instances import BUDGET, _lib_call
+from gpu_harness import (BUDGET, F32, F64, TNAME, Bufs, b, body, call, check_launch_order, close, mag, profiled_names,
+                         ptr, rd, src)
 
-F32, F64 = np.float32, np.float64
-TNAME = {F32: "float", F64: "double"}
 LL_NONE, LL_FULL, LL_BROADCAST = 0, 1, 2
 
 TOL = {
@@ -44,13 +41,15 @@ TOL = {
 }
 
 
-# ------------------------------------------------------------------------------------------ kernel names
-def _b(v):
-    return "true" if v else "false"
+def _bound(c):
+    """Case c's tolerance and the label of its BKE_TEST_ERRLOG lines."""
+    return TOL[c.family][c.dt], "test_gpu_if_instances %s %s" % (c.family, np.dtype(c.dt).name)
 
+
+# ------------------------------------------------------------------------------------------ kernel names
 
 def k_reg(dt, n, m, ex):
-    return "if_reg_kernel<%s, %d, %d, %s>" % (TNAME[dt], n, m, _b(ex))
+    return "if_reg_kernel<%s, %d, %d, %s>" % (TNAME[dt], n, m, b(ex))
 
 
 def k_warp(dt):
@@ -201,8 +200,8 @@ CASES = _cases()
 # ------------------------------------------------------------------------------------------ the table vs the source
 def _dispatched():
     """Every kernel instance information.cu's dispatch() and launch_inv can launch, parsed from the source."""
-    src = _src("information.cu")
-    d = _body(src, "int dispatch(const bke_if_args &a, cudaStream_t s)")
+    text = src("information.cu")
+    d = body(text, "int dispatch(const bke_if_args &a, cudaStream_t s)")
     assert d.count("if constexpr (sizeof(T) == 4)") == 1, "the fp32-only register shapes are not where they were"
     both, f32only = d.split("if constexpr (sizeof(T) == 4)")
     pat = r"n == (\d+) && m == (\d+)\) rc = launch_reg<T, (\d+), (\d+)>"
@@ -214,11 +213,11 @@ def _dispatched():
                 reg[dt].append((int(a), int(b)))
     assert "return rc == BKE_ERR_UNSUPPORTED ? launch_warp<T>(a, s) : rc;" in d
     assert "if (a.B == nullptr || a.u == nullptr) {" in d
-    lr = _body(src, "int launch_reg(const bke_if_args &a, cudaStream_t s)")
+    lr = body(text, "int launch_reg(const bke_if_args &a, cudaStream_t s)")
     assert set(re.findall(r"if_reg_kernel<T, N, M, (true|false)><<<", lr)) == {"true", "false"}
     inst = {k_reg(dt, n, m, ex) for dt, shapes in reg.items() for n, m in shapes for ex in (True, False)}
     inst |= {k_warp(dt) for dt in (F32, F64)} | {k_inv(dt) for dt in (F32, F64)}
-    assert "inverse_kernel<T><<<" in _body(src, "int launch_inv(int64_t N, int k, const void *A, int64_t stride, "
+    assert "inverse_kernel<T><<<" in body(text, "int launch_inv(int64_t N, int k, const void *A, int64_t stride, "
                                                 "void *Ai, int32_t *status, cudaStream_t s)")
     return inst, reg
 
@@ -249,9 +248,9 @@ def test_instance_table_matches_dispatch():
             assert {c.models for c in w} == {"per", "shared"}
         assert any(c.ctrl for c in CASES if c.dt == dt)
         assert {c.n for c in CASES if c.family == "inv" and c.dt == dt} >= set(range(1, 9)) | {31, 32, 33, 64}
-    src = _src("information.cu")
-    assert "return 4 * n + 2 * m + 6 * n * n + 4 * m * n + m * m;" in _body(src, "inline int if_per_warp(int n, int m)")
-    assert "const int per_warp = (2 * k * k + k + 3) & ~3;" in src and "budget = 200 * 1024" in src
+    text = src("information.cu")
+    assert "return 4 * n + 2 * m + 6 * n * n + 4 * m * n + m * m;" in body(text, "inline int if_per_warp(int n, int m)")
+    assert "const int per_warp = (2 * k * k + k + 3) & ~3;" in text and "budget = 200 * 1024" in text
 
 
 # ------------------------------------------------------------------------------------------ inputs
@@ -314,7 +313,7 @@ def if_inputs(c, N, seed):
                 sel = f % 11 == 6
                 d["P_inv"][sel] = np.array([[1, -1], [-1, 1]]) * EDGE_A; d["H"][sel] = 0; ni[sel] = False
                 fail[sel] = "edge"
-    d = {k: _rd(v, c.dt) for k, v in d.items()}
+    d = {k: rd(v, c.dt) for k, v in d.items()}
     d["ni"] = ni
     return d, fail
 
@@ -412,32 +411,32 @@ def run_step(c, N, seed=0, sticky=False):
     a.flags = c.mode | (_lib.BKE_STATUS_STICKY if sticky else 0)
     a.ll_mode = c.ll_mode
     xv, Pv = bf.put(d["x"], c.mis == "x", out=c.inplace), bf.put(d["P_inv"], c.mis == "P_inv", out=c.inplace)
-    a.x, a.P_inv = _ptr(xv), _ptr(Pv)
+    a.x, a.P_inv = ptr(xv), ptr(Pv)
     xo, Po = (xv, Pv) if c.inplace else (bf.out((N, n), c.mis == "x_out"), bf.out((N, n, n), c.mis == "P_inv_out"))
-    a.x_out, a.P_inv_out = _ptr(xo), _ptr(Po)
+    a.x_out, a.P_inv_out = ptr(xo), ptr(Po)
     niv = bf.put(d["ni"].astype(np.uint8), dtype=np.uint8)
-    a.no_information = _ptr(niv)
+    a.no_information = ptr(niv)
     for k in ("F", "F_inv", "Q", "H", "R_inv"):
         arr = d[k]
-        setattr(a, k, _ptr(bf.put(arr, c.mis == k)))
+        setattr(a, k, ptr(bf.put(arr, c.mis == k)))
         setattr(a, k + "_stride", 0 if arr.ndim == 2 else arr.shape[-1] * arr.shape[-2])
     if c.ctrl:
         a.dim_u = 2
-        a.B = _ptr(bf.put(d["B"])); a.B_stride = 0 if d["B"].ndim == 2 else 2 * n
-        a.u = _ptr(bf.put(d["u"])); a.u_stride = 2
-    a.z = _ptr(bf.put(d["z"], c.mis == "z"))
+        a.B = ptr(bf.put(d["B"])); a.B_stride = 0 if d["B"].ndim == 2 else 2 * n
+        a.u = ptr(bf.put(d["u"])); a.u_stride = 2
+    a.z = ptr(bf.put(d["z"], c.mis == "z"))
     if c.mode & 2:
-        a.z_valid = _ptr(bf.put(valid.astype(np.uint8), dtype=np.uint8))
+        a.z_valid = ptr(bf.put(valid.astype(np.uint8), dtype=np.uint8))
     outs = {}
     if c.ex:
         for k, s in OUT_SHAPES(n, m).items():
             outs[k] = bf.out((N,) + s, c.mis == k)
-            setattr(a, k, _ptr(outs[k]))
+            setattr(a, k, ptr(outs[k]))
     ll = bf.out((N,))
-    a.log_likelihood = _ptr(ll)
+    a.log_likelihood = ptr(ll)
     st = bf.out((N,), dtype=np.int32, fill=5)
-    a.status = _ptr(st)
-    rc, err = _lib_call("bke_if_step", ctypes.byref(a))
+    a.status = ptr(st)
+    rc, err = call("bke_if_step", ctypes.byref(a))
     if rc:
         return rc, err, None, d, fail, valid
     bf.check_guards()
@@ -448,61 +447,37 @@ def run_step(c, N, seed=0, sticky=False):
     return rc, err, got, d, fail, valid
 
 
-# ------------------------------------------------------------------------------------------ comparisons
-def _errlog(c, what, err, tol):
-    log = os.environ.get("BKE_TEST_ERRLOG")
-    if log:
-        with open(log, "a") as fh:
-            fh.write("test_gpu_if_instances %s %s %s max_err=%.3e tol=%.1e\n"
-                     % (c.family, np.dtype(c.dt).name, what, err, tol))
-
-
-def _close(c, got, want, scale, cond, what, rows=None):
-    """|got - want| <= TOL * scale * cond per filter (axis 0)."""
-    tol = TOL[c.family][c.dt]
-    got = np.asarray(got, np.float64); want = np.asarray(want, np.float64)
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    if rows is not None:
-        got, want, scale, cond = got[rows], want[rows], scale[rows], cond[rows]
-    if got.size == 0:
-        return
-    assert np.all(np.isfinite(got)), "%s: not finite" % what
-    sh = (-1,) + (1,) * (want.ndim - 1)
-    err = np.abs(got - want) / (np.maximum(scale, 1e-300).reshape(sh) * cond.reshape(sh))
-    _errlog(c, what, err.max(), tol)
-    assert err.max() <= tol, "%s: max err %.3e of the filter's scale x cond > %.1e" % (what, err.max(), tol)
-
-
 def check_step(c, N, seed, sticky):
     rc, err, got, d, fail, valid = run_step(c, N, seed, sticky)
     assert rc == 0, err
     want, w, cp, ct = if_oracle(c, d, valid)
     what = "%s N=%d seed=%d%s" % (c.id, N, seed, " sticky" if sticky else "")
+    tol, label = _bound(c)
     st_want = want["status"].astype(np.int32)
     if sticky:
         st_want[st_want == 0] = 5                   # BKE_STATUS_STICKY: written only where the step failed
     assert np.array_equal(got["status"], st_want), (what + " status", np.nonzero(got["status"] != st_want))
     assert np.array_equal(got["ni"], want["ni"].astype(np.uint8)), what + " no_information"
     pw = w["prior"]
-    sx = _mag(d["x"], np.where(pw[:, None], want["x_prior"], 0), want["x"])
-    sP = _mag(d["P_inv"], np.where(pw[:, None, None], want["P_inv_prior"], 0), want["P_inv"])
-    _close(c, got["x"], want["x"], sx, ct, what + " x")
-    _close(c, got["P_inv"], want["P_inv"], sP, ct, what + " P_inv")
+    sx = mag(d["x"], np.where(pw[:, None], want["x_prior"], 0), want["x"])
+    sP = mag(d["P_inv"], np.where(pw[:, None, None], want["P_inv_prior"], 0), want["P_inv"])
+    close(got["x"], want["x"], sx, ct, tol, what + " x", label)
+    close(got["P_inv"], want["P_inv"], sP, ct, tol, what + " P_inv", label)
     S = Bufs.SENT
-    _close(c, got["ll"], want["ll"], np.maximum(np.abs(want["ll"]), 1.0), ct, what + " log_likelihood", w["ll"])
+    close(got["ll"], want["ll"], np.maximum(np.abs(want["ll"]), 1.0), ct, tol, what + " log_likelihood", label, w["ll"])
     assert np.all(got["ll"][~w["ll"]] == S), what + " log_likelihood written"
     if not c.ex:
         return
-    _close(c, got["x_prior"], want["x_prior"], sx, cp, what + " x_prior", pw)
-    _close(c, got["P_inv_prior"], want["P_inv_prior"], sP, cp, what + " P_inv_prior", pw)
+    close(got["x_prior"], want["x_prior"], sx, cp, tol, what + " x_prior", label, pw)
+    close(got["P_inv_prior"], want["P_inv_prior"], sP, cp, tol, what + " P_inv_prior", label, pw)
     assert np.all(got["x_prior"][~pw] == S) and np.all(got["P_inv_prior"][~pw] == S), what + " prior written"
     ys, kw = w["yS"], w["K"]
     ux = np.where(pw[:, None], want["x_prior"], d["x"])
     H = np.broadcast_to(d["H"], (N,) + d["H"].shape[-2:])
     sy = np.abs(H).max(axis=(1, 2)) * np.abs(ux).sum(axis=1) + np.abs(d["z"]).max(axis=1)
-    _close(c, got["y"], want["y"], sy, cp, what + " y", ys)
-    _close(c, got["S"], want["S"], _mag(want["S"]), cp, what + " S", ys)
-    _close(c, got["K"], want["K"], _mag(want["K"]), ct, what + " K", kw)
+    close(got["y"], want["y"], sy, cp, tol, what + " y", label, ys)
+    close(got["S"], want["S"], mag(want["S"]), cp, tol, what + " S", label, ys)
+    close(got["K"], want["K"], mag(want["K"]), ct, tol, what + " K", label, kw)
     for k, m_ in (("y", ys), ("S", ys), ("K", kw)):
         assert np.all(got[k][~m_] == S), what + " %s written" % k
     if N >= 11 and c.models == "per":
@@ -547,14 +522,14 @@ def run_inv(c, N, seed=0):
     if c.models == "per" and N > 1:
         sing[3::7] = True
         A[sing, rng.integers(0, k), :] = 0
-    A = _rd(A, dt)
+    A = rd(A, dt)
     bf = Bufs(dt)
     Av = bf.put(A)
     Ao = bf.out((N, k, k))
     st = bf.out((N,), dtype=np.int32, fill=5)
-    rc, err = _lib_call("bke_inverse", ctypes.c_int64(N), ctypes.c_int32(k), ctypes.c_int32(0 if dt == F32 else 1),
-                        ctypes.c_void_p(_ptr(Av)), ctypes.c_int64(0 if c.models == "shared" else k * k),
-                        ctypes.c_void_p(_ptr(Ao)), ctypes.c_void_p(_ptr(st)))
+    rc, err = call("bke_inverse", ctypes.c_int64(N), ctypes.c_int32(k), ctypes.c_int32(0 if dt == F32 else 1),
+                   ctypes.c_void_p(ptr(Av)), ctypes.c_int64(0 if c.models == "shared" else k * k),
+                   ctypes.c_void_p(ptr(Ao)), ctypes.c_void_p(ptr(st)))
     if rc:
         return rc, err, None, None, None, None
     bf.check_guards()
@@ -575,6 +550,7 @@ def test_inverse_instance_vs_numpy(case):
                        % (c.n, inv_per_warp(c.n) * np.dtype(c.dt).itemsize, BUDGET)), err
         return
     Ns = c.Ns + ((_grid_N(c),) if c.grid else ())
+    tol, label = _bound(c)
     for N in Ns:
         rc, err, Ai, st, A, sing = run_inv(c, N, seed=N)
         assert rc == 0, err
@@ -582,54 +558,23 @@ def test_inverse_instance_vs_numpy(case):
         assert np.array_equal(st, sing.astype(np.int32)), what + " status"
         ok = ~sing
         want = np.linalg.inv(A[ok])
-        _close(c, Ai[ok], want, _mag(want), np.linalg.cond(A[ok]), what + " inverse")
+        close(Ai[ok], want, mag(want), np.linalg.cond(A[ok]), tol, what + " inverse", label)
 
 
 # ------------------------------------------------------------------------------------------ which kernel runs
-def _kernel_name(s):
-    """'if_reg_kernel<double, 4, 2, true>' out of a demangled launch name (namespaces dropped)."""
-    s = re.sub(r"\(anonymous namespace\)::|\b\w+::", "", s)
-    mt = re.search(r"\b(if_\w+_kernel|inverse_kernel)<", s)
-    if not mt:
-        return None
-    depth, i = 0, mt.end() - 1
-    for j in range(i, len(s)):
-        depth += {"<": 1, ">": -1}.get(s[j], 0)
-        if depth == 0:
-            return re.sub(r"\s+", " ", s[mt.start():j + 1])
-    return None
+def _run_cases():
+    for c in CASES:
+        rc, err = (run_inv(c, c.Np) if c.family == "inv" else run_step(c, c.Np))[:2]
+        assert (rc != 0) == c.refused, (c.id, err)
 
 
 def _profiled_names():
-    """The kernel names of every CASES entry run once at its N, in launch order (torch.profiler, CUDA activity)."""
-    from torch.profiler import profile, ProfilerActivity
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for c in CASES:
-            rc, err = (run_inv(c, c.Np) if c.family == "inv" else run_step(c, c.Np))[:2]
-            assert (rc != 0) == c.refused, (c.id, err)
-    names = [_kernel_name(e.name) for e in sorted(prof.events(), key=lambda e: e.time_range.start)]
-    return [k for k in names if k]
+    """The kernel names of every CASES entry run once at its N, in launch order."""
+    return profiled_names(_run_cases, r"if_\w+_kernel|inverse_kernel")
 
 
 @pytest.mark.gpu
 def test_dispatch_runs_the_kernels_of_the_table():
     """Each CASES entry, run once at its N, launches the kernels the table names, in order, template arguments included
-    (a refused shape launches none).  The profile is taken in a process of its own, as in test_gpu_kf_instances."""
-    import json
-    import subprocess
-    import sys
-    here = os.path.dirname(os.path.abspath(__file__))
-    code = ("import json, sys; sys.path[:0] = %r; import test_gpu_if_instances as t; print(json.dumps(t._profiled_names()))"
-            % [here, os.path.dirname(here)])
-    r = subprocess.run([sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    names = json.loads(r.stdout.strip().splitlines()[-1])
-    pos, bad = 0, []
-    for c in CASES:
-        got = names[pos:pos + len(c.kernels)]
-        if got != c.kernels:
-            bad.append((c.id, c.kernels, got))
-            break                                       # everything after a wrong count is shifted
-        pos += len(c.kernels)
-    assert not bad and pos == len(names), (bad, names[pos:pos + 5])
+    (a refused shape launches none)."""
+    check_launch_order("test_gpu_if_instances", [(c.id, c.kernels) for c in CASES])

@@ -47,11 +47,9 @@ import re
 import numpy as np
 import pytest
 
-from test_gpu_kf_instances import Bufs, _body, _ptr, _rd, _spd, _src
+from gpu_harness import (F32, F64, ROOT, TNAME, Bufs, body, call, check_launch_order, close, mag, profiled_names, ptr, rd,
+                         spd, src, stable_F)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-F32, F64 = np.float32, np.float64
-TNAME = {F32: "float", F64: "double"}
 BLOCK = 128                                     # imm.cu kImmBlock
 MAX_MODELS = 8                                  # BKE_MM_MAX_MODELS
 
@@ -62,6 +60,12 @@ TOL = {
     "ll": {F64: {1: 4e-15, 2: 1e-14, 8: 4e-13, 32: 8e-13}, F32: {1: 1.5e-6, 2: 5e-6, 8: 3.5e-4}},
     "mu": {F64: {1: 5e-15, 2: 1e-14, 8: 1e-13, 32: 8e-13}, F32: {1: 1.5e-6, 2: 4e-6, 8: 5e-5}},
 }
+
+
+def _bound(c, fam):
+    """Family fam's tolerance at case c's dtype and T, and the label of its BKE_TEST_ERRLOG lines."""
+    return TOL[fam][c.dt][c.T], "test_gpu_imm_instances %s %s T=%d" % (fam, np.dtype(c.dt).name, c.T)
+
 
 INSTANCES = {F32: [(2, 1), (3, 1), (4, 2)], F64: [(2, 1), (3, 1)]}
 # the arrays validate_imm requires on a 16-byte boundary (per model, then shared)
@@ -134,8 +138,8 @@ RUN = [c for c in CASES if c.kind == "run"]
 def _dispatched():
     """(the instances launch_imm_batch can launch, {M: G} of launch_shape, the shapes imm_batch_has_instance accepts,
     the arrays validate_imm aligns), parsed from the source."""
-    src = _src("imm.cu")
-    li = _body(src, "int launch_imm_batch(const bke_imm_batch_args &a, cudaStream_t s)")
+    text = src("imm.cu")
+    li = body(text, "int launch_imm_batch(const bke_imm_batch_args &a, cudaStream_t s)")
     f32part, f64part = li.split("} else {")
     shapes = {F32: [], F64: []}
     for part, dt in ((f32part, F32), (f64part, F64)):
@@ -144,24 +148,24 @@ def _dispatched():
             assert (a, b) == (c, e) and t == TNAME[dt]
             shapes[dt].append((int(a), int(b)))
     assert 'set_error("%s", n, m);' % ERR_SHAPE in li
-    ls = _body(src, "int launch_shape(const bke_imm_batch_args &a, cudaStream_t s)")
+    ls = body(text, "int launch_shape(const bke_imm_batch_args &a, cudaStream_t s)")
     steps = [(int(k), int(g)) for k, g in re.findall(r"if \(a\.n_models <= (\d+)\) return launch_g<T, N, MZ, (\d+)>", ls)]
     last = re.findall(r"\n\s*return launch_g<T, N, MZ, (\d+)>\(a, s\);", ls)
     assert len(last) == 1
     gmap = {}
     for M in range(2, MAX_MODELS + 1):
         gmap[M] = next((g for k, g in steps if M <= k), int(last[0]))
-    lg = _body(src, "int launch_g(const bke_imm_batch_args &a, cudaStream_t s)")
+    lg = body(text, "int launch_g(const bke_imm_batch_args &a, cudaStream_t s)")
     assert "imm_batch_kernel<T, N, MZ, G>" in lg and "grid, kImmBlock, 0, &p, s" in lg
-    assert re.search(r"constexpr int kImmBlock = %d;" % BLOCK, src)
+    assert re.search(r"constexpr int kImmBlock = %d;" % BLOCK, text)
     inst = {k_imm(dt, n, m, g) for dt, shp in shapes.items() for n, m in shp for g in set(gmap.values())}
-    has = _body(src, "bool imm_batch_has_instance(int dim_x, int dim_z, int dtype)")
+    has = body(text, "bool imm_batch_has_instance(int dim_x, int dim_z, int dtype)")
     accepted = {F32: [], F64: []}
     for a, b, f32 in re.findall(r"\(dim_x == (\d+) && dim_z == (\d+)( && dtype == BKE_F32)?\)", has):
         for dt in ((F32,) if f32 else (F32, F64)):
             accepted[dt].append((int(a), int(b)))
-    api = _src("api.cu")
-    v = _body(api, "static int validate_imm(const bke_imm_batch_args *a)")
+    api = src("api.cu")
+    v = body(api, "static int validate_imm(const bke_imm_batch_args *a)")
     al = v[v.index("auto al16"):]
     aligned = (set(re.findall(r"al16\(a->(\w+)\[j\]\)", al)), set(re.findall(r"al16\(a->(\w+)\)", al)))
     assert ERR_ALIGN in al and "return BKE_ERR_UNSUPPORTED;" in al
@@ -229,14 +233,6 @@ def _layout(j):
     return dict(F=j % 2 == 1, Q=j % 3 == 2, H=j % 2 == 0 and j > 0, R=j % 3 == 1)
 
 
-def stable_F(rng, shape, n):
-    """I + 0.15 G, scaled to a spectral radius of at most 0.98: a recursion of 32 epochs neither grows nor decays so
-    far that its rounding says more about the model than about the kernel."""
-    F = np.eye(n) + 0.15 * rng.normal(size=shape + (n, n))
-    rho = np.abs(np.linalg.eigvals(F)).max(axis=-1)
-    return F * np.minimum(1.0, 0.98 / rho)[..., None, None]
-
-
 def imm_inputs(c, N, seed):
     """The arrays of one call, rounded to the case's dtype, and the tracks whose starting S is 0 / that never measure."""
     rng = np.random.default_rng(seed)
@@ -246,13 +242,13 @@ def imm_inputs(c, N, seed):
         sh = _layout(j)
         cnt = lambda k: () if sh[k] else (N,)
         d["F"].append(stable_F(rng, cnt("F"), n))
-        d["Q"].append(_spd(rng, cnt("Q"), n, 0.02 * (j + 1)))
+        d["Q"].append(spd(rng, cnt("Q"), n, 0.02 * (j + 1)))
         d["H"].append(rng.normal(size=cnt("H") + (m, n)))
-        d["R"].append(_spd(rng, cnt("R"), m, 0.3 + 0.2 * j))
+        d["R"].append(spd(rng, cnt("R"), m, 0.3 + 0.2 * j))
     d["alpha_sq"] = np.array([(1.0 + 0.01 * (j + 1)) ** 2 for j in range(M)])
     d["x"] = rng.normal(size=(N, M, n)) * 3
-    d["P"] = _spd(rng, (N, M), n, 2.0)
-    d["S"] = _spd(rng, (N, M), m, 1.0)
+    d["P"] = spd(rng, (N, M), n, 2.0)
+    d["S"] = spd(rng, (N, M), m, 1.0)
     d["SI"] = rng.normal(size=(N, M, m, m))
     d["K"] = rng.normal(size=(N, M, n, m))
     d["y"] = rng.normal(size=(N, M, m))
@@ -274,9 +270,9 @@ def imm_inputs(c, N, seed):
         valid[:, never] = False
     d["valid"] = valid
     for k in ("x", "P", "S", "SI", "K", "y", "ll", "zs"):
-        d[k] = _rd(d[k], dt)
+        d[k] = rd(d[k], dt)
     for k in "FQHR":
-        d[k] = [_rd(a, dt) for a in d[k]]
+        d[k] = [rd(a, dt) for a in d[k]]
     return d
 
 
@@ -291,19 +287,9 @@ def imm_oracle(d, N):
                      d["valid"], S0=d["S"], ll0=d["ll"], K0=d["K"], y0=d["y"], SI0=d["SI"], cbar0=d["cbar"])
 
 
-# ------------------------------------------------------------------------------------------ running a call
-def _lib_rc(a):
-    import torch
-    from filterpy_b200 import _lib
-    lib = _lib.load()
-    rc = lib.bke_imm_batch_filter(ctypes.byref(a), torch.cuda.current_stream().cuda_stream)
-    return rc, lib.bke_last_error().decode()
-
-
 def run_imm(c, N, d, sticky=False, mis=None):
     """One bke_imm_batch_filter call on the inputs d: (rc, error text, the outputs host-side, Bufs).  Every output
     starts as NaN (status as 5), so an element the kernel never writes shows up."""
-    import torch
     from filterpy_b200 import _lib
     dt, n, m, M, T = c.dt, c.n, c.m, c.M, c.T
     bf = Bufs(dt)
@@ -324,30 +310,29 @@ def run_imm(c, N, d, sticky=False, mis=None):
             else:
                 v = bf.out((N,) + shp, off, fill=nan)
             views[(k, j)] = v
-            getattr(a, k)[j] = _ptr(v)
+            getattr(a, k)[j] = ptr(v)
         st = bf.out((N,), dtype=np.int32, fill=5)
         views[("status", j)] = st
-        a.status[j] = _ptr(st)
+        a.status[j] = ptr(st)
         for k in "FQHR":
             arr = d[k][j]
-            getattr(a, k)[j] = _ptr(bf.put(arr))
+            getattr(a, k)[j] = ptr(bf.put(arr))
             getattr(a, k + "_stride")[j] = 0 if arr.ndim == 2 else arr.shape[-1] * arr.shape[-2]
         a.alpha_sq[j] = float(d["alpha_sq"][j])
     for k in ("mu", "cbar"):
         views[k] = bf.put(d[k], out=True, dtype=F64)
-        setattr(a, k, _ptr(views[k]))
+        setattr(a, k, ptr(views[k]))
     views["omega"] = bf.out((N, M, M), dtype=F64, fill=nan)
-    a.omega = _ptr(views["omega"])
-    a.trans = _ptr(bf.put(d["trans"], dtype=F64))
-    a.zs = _ptr(bf.put(d["zs"]))
-    a.zs_valid = _ptr(bf.put(d["valid"].astype(np.uint8), dtype=np.uint8))
+    a.omega = ptr(views["omega"])
+    a.trans = ptr(bf.put(d["trans"], dtype=F64))
+    a.zs = ptr(bf.put(d["zs"]))
+    a.zs_valid = ptr(bf.put(d["valid"].astype(np.uint8), dtype=np.uint8))
     for k, shp in (("means", (n,)), ("covariances", (n, n)), ("means_p", (n,)), ("covariances_p", (n, n))):
         views[k] = bf.out((T, N) + shp, mis == k, fill=nan)
-        setattr(a, k, _ptr(views[k]))
+        setattr(a, k, ptr(views[k]))
     views["mus"] = bf.out((T, N, M), dtype=F64, fill=nan)
-    a.mus = _ptr(views["mus"])
-    rc, err = _lib_rc(a)
-    torch.cuda.synchronize()
+    a.mus = ptr(views["mus"])
+    rc, err = call("bke_imm_batch_filter", ctypes.byref(a))
     got = {}
     for key, v in views.items():
         h = v.cpu().numpy()
@@ -366,60 +351,35 @@ def run_imm(c, N, d, sticky=False, mis=None):
     return rc, err, got, bf
 
 
-# ------------------------------------------------------------------------------------------ comparisons
-def _errlog(c, fam, what, err, tol):
-    log = os.environ.get("BKE_TEST_ERRLOG")
-    if log:
-        with open(log, "a") as fh:
-            fh.write("test_gpu_imm_instances %s %s T=%d %s max_err=%.3e tol=%.1e\n"
-                     % (fam, np.dtype(c.dt).name, c.T, what, err, tol))
-
-
-def _close(c, fam, got, want, scale, cond, what):
-    """|got - want| <= TOL * scale * cond per track (axis 0); -inf only where the oracle has it."""
-    tol = TOL[fam][c.dt][c.T]
-    got = np.asarray(got, np.float64); want = np.asarray(want, np.float64)
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    inf = np.isinf(want)
-    assert np.array_equal(got[inf], want[inf]), "%s: an infinity differs" % what
-    assert np.all(np.isfinite(got[~inf])), "%s: not finite" % what
-    if not (~inf).any():
-        return
-    sh = (-1,) + (1,) * (want.ndim - 1)
-    e = np.where(inf, 0.0, np.abs(got - np.where(inf, 0.0, want)))
-    err = e / (np.broadcast_to(np.maximum(scale, 1e-300).reshape(sh), e.shape) * cond.reshape(sh))
-    _errlog(c, fam, what, err.max(), tol)
-    assert err.max() <= tol, "%s: max err %.3e of the track's scale x cond > %.1e" % (what, err.max(), tol)
-
-
-def _tmax(*arrs):
-    """Per track (axis 0): the largest |entry| over the given arrays."""
-    return np.max([np.abs(a).reshape(a.shape[0], -1).max(axis=1) for a in arrs], axis=0)
-
-
 def check_imm(c, N, d, got, want, sticky, what):
     sw = lambda a: np.swapaxes(a, 0, 1)                             # [T, N, ...] -> [N, T, ...]
     cond = want["cond"]
-    sx = _tmax(d["x"], sw(want["x"]), sw(want["xp"]), sw(want["fx"]), want["fxp"])
-    sP = _tmax(d["P"], sw(want["P"]), sw(want["Pp"]), sw(want["fP"]), want["fPp"])
+
+    def _cmp(fam, got_, want_, scale, what_):
+        """Per track (axis 0), relative to its scale x cond; -inf only where the oracle has it."""
+        tol, label = _bound(c, fam)
+        close(got_, want_, scale, cond, tol, what_, label, match_inf=True)
+
+    sx = mag(d["x"], sw(want["x"]), sw(want["xp"]), sw(want["fx"]), want["fxp"])
+    sP = mag(d["P"], sw(want["P"]), sw(want["Pp"]), sw(want["fP"]), want["fPp"])
     for k, w, s in (("means", "x", sx), ("means_p", "xp", sx), ("covariances", "P", sP), ("covariances_p", "Pp", sP)):
-        _close(c, "state", sw(got[k]), sw(want[w]), s, cond, what + " " + k)
-    _close(c, "mu", sw(got["mus"]), sw(want["mu"]), np.ones(N), cond, what + " mus")
+        _cmp("state", sw(got[k]), sw(want[w]), s, what + " " + k)
+    _cmp("mu", sw(got["mus"]), sw(want["mu"]), np.ones(N), what + " mus")
     for k, w, s in (("x", "fx", sx), ("P", "fP", sP)):
-        _close(c, "state", got[k], want[w][-1], s, cond, what + " " + k)
-    _close(c, "state", got["x_prior"], want["fxp"], sx, cond, what + " x_prior")
-    _close(c, "state", got["P_prior"], want["fPp"], sP, cond, what + " P_prior")
+        _cmp("state", got[k], want[w][-1], s, what + " " + k)
+    _cmp("state", got["x_prior"], want["fxp"], sx, what + " x_prior")
+    _cmp("state", got["P_prior"], want["fPp"], sP, what + " P_prior")
     Hmax = np.max([np.abs(_per_track(h, N)).reshape(N, -1).max(axis=1) for h in d["H"]], axis=0)
-    sy = _tmax(sw(d["zs"]), d["y"]) + Hmax * np.abs(want["fxp"]).sum(axis=2).max(axis=1)
-    _close(c, "diag", got["y"], want["fy"], sy, cond, what + " y")
-    for k, w, s in (("S", "fS", _tmax(d["S"], want["fS"])), ("SI", "fSI", _tmax(d["SI"], want["fSI"])),
-                    ("K", "fK", _tmax(d["K"], want["fK"]))):
-        _close(c, "diag", got[k], want[w], s, cond, what + " " + k)
+    sy = mag(sw(d["zs"]), d["y"]) + Hmax * np.abs(want["fxp"]).sum(axis=2).max(axis=1)
+    _cmp("diag", got["y"], want["fy"], sy, what + " y")
+    for k, w, s in (("S", "fS", mag(d["S"], want["fS"])), ("SI", "fSI", mag(d["SI"], want["fSI"])),
+                    ("K", "fK", mag(d["K"], want["fK"]))):
+        _cmp("diag", got[k], want[w], s, what + " " + k)
     fin = np.where(np.isinf(want["fll"]), 1.0, np.abs(want["fll"]))
-    _close(c, "ll", got["log_likelihood"] / np.maximum(fin, 1.0), want["fll"] / np.maximum(fin, 1.0), np.ones(N),
-           cond, what + " log_likelihood")
+    _cmp("ll", got["log_likelihood"] / np.maximum(fin, 1.0), want["fll"] / np.maximum(fin, 1.0), np.ones(N),
+         what + " log_likelihood")
     for k, w in (("mu", "mu"), ("cbar", "cbar"), ("omega", "omega")):
-        _close(c, "mu", got[k], want[w][-1], np.ones(N), cond, what + " " + k)
+        _cmp("mu", got[k], want[w][-1], np.ones(N), what + " " + k)
     st_want = want["status_any"] if sticky else want["status"]
     assert np.array_equal(got["status"], st_want), what + " status"
 
@@ -503,49 +463,18 @@ def test_refused_and_empty_calls(case):
 
 
 # ------------------------------------------------------------------------------------------ which kernel runs
-def _kernel_name(s):
-    s = re.sub(r"\(anonymous namespace\)::|\b\w+::", "", s)
-    mt = re.search(r"\b(imm_batch_kernel|kf\w*_kernel|fls_\w+_kernel)<", s)
-    if not mt:
-        return None
-    depth, i = 0, mt.end() - 1
-    for j in range(i, len(s)):
-        depth += {"<": 1, ">": -1}.get(s[j], 0)
-        if depth == 0:
-            return re.sub(r"\s+", " ", s[mt.start():j + 1])
-    return None
+def _run_cases():
+    for c in CASES:
+        run_imm(c, c.Np, imm_inputs(c, c.Np, seed=1), mis=c.mis)
 
 
 def _profiled_names():
-    """The kernel names of every CASES entry run once at its Np, in launch order (torch.profiler, CUDA activity)."""
-    from torch.profiler import profile, ProfilerActivity
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for c in CASES:
-            d = imm_inputs(c, c.Np, seed=1)
-            run_imm(c, c.Np, d, mis=c.mis)
-    names = [_kernel_name(e.name) for e in sorted(prof.events(), key=lambda e: e.time_range.start)]
-    return [k for k in names if k]
+    """The kernel names of every CASES entry run once at its Np, in launch order."""
+    return profiled_names(_run_cases, r"imm_batch_kernel|kf\w*_kernel|fls_\w+_kernel")
 
 
 @pytest.mark.gpu
 def test_dispatch_runs_the_kernels_of_the_table():
     """Each CASES entry, run once at its Np, launches the kernels the table names, in order, template arguments
-    included; refused and empty calls launch nothing.  The profile is taken in a process of its own."""
-    import json
-    import subprocess
-    import sys
-    here = os.path.dirname(os.path.abspath(__file__))
-    code = ("import json, sys; sys.path[:0] = %r; import test_gpu_imm_instances as t; "
-            "print(json.dumps(t._profiled_names()))" % [here, os.path.dirname(here)])
-    r = subprocess.run([sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    names = json.loads(r.stdout.strip().splitlines()[-1])
-    pos, bad = 0, []
-    for c in CASES:
-        got = names[pos:pos + len(c.kernels)]
-        if got != c.kernels:
-            bad.append((c.id, c.kernels, got))
-            break
-        pos += len(c.kernels)
-    assert not bad and pos == len(names), (bad, names[pos:pos + 5])
+    included; refused and empty calls launch nothing."""
+    check_launch_order("test_gpu_imm_instances", [(c.id, c.kernels) for c in CASES])

@@ -1,35 +1,12 @@
 """GPU parity: linear KF bank (CUDA through the C-ABI) vs the oracle and the reference's golden
 vectors.  Tolerances are north_star's: 1e-6 rel for fp64, 1e-3 rel for fp32 (the fp32 kernel is
 compared with the fp64 reference because the reference silently promotes)."""
-import os
-
 import numpy as np
 import pytest
 
+from gpu_harness import RTOL, rel_close
+
 pytestmark = pytest.mark.gpu
-
-RTOL = {np.float64: 1e-6, np.float32: 1e-3}
-
-
-def rel_close(got, want, rtol, what=""):
-    """|got - want| <= rtol * max(|want|, 1e-2 * max|want| of the same filter): element-wise
-    relative error, with entries that are (near) zero by cancellation measured against the
-    filter's own scale."""
-    got = np.asarray(got, dtype=np.float64); want = np.asarray(want, dtype=np.float64)
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    assert np.all(np.isfinite(got)), what
-    if want.ndim > 1:
-        floor = 1e-2 * np.abs(want).max(axis=tuple(range(1, want.ndim)), keepdims=True)
-    else:
-        floor = 1e-2 * np.abs(want)
-    err = np.abs(got - want) / np.maximum(np.maximum(np.abs(want), floor), 1e-300)
-    log = os.environ.get("BKE_TEST_ERRLOG")
-    if log and err.size:
-        import inspect
-        caller = inspect.stack()[1]
-        with open(log, "a") as fh:
-            fh.write("%s:%d %s max_rel_err=%.3e rtol=%.1e\n" % (os.path.basename(caller.filename), caller.lineno, what, err.max(), rtol))
-    assert err.size == 0 or err.max() <= rtol, "%s: max rel err %.3e > %.1e" % (what, err.max(), rtol)
 
 
 def make_bank(g, dtype, diagnostics=True):

@@ -27,15 +27,14 @@ error / (scale * cond) over every case, output and bank size of the family, and 
     rts       rts_*_kernel             6.1e-16    3e-15     5.3e-7      2e-6
 """
 import ctypes
-import os
 import re
 
 import numpy as np
 import pytest
 
-CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "filterpy_b200", "csrc")
-F32, F64 = np.float32, np.float64
-TNAME = {F32: "float", F64: "double"}
+from gpu_harness import (F32, F64, TNAME, Bufs, b, body, call_ok, check_launch_order, close, k_direct, k_fast, k_gen,
+                         k_rb, mag, profiled_names, ptr, rb_fpw, rd, spd, src)
+
 ALPHA_SQ = 1.01 ** 2
 
 TOL = {
@@ -50,33 +49,18 @@ TOL = {
 }
 
 
+def _bound(c):
+    """Case c's tolerance and the label of its BKE_TEST_ERRLOG lines."""
+    return TOL[c.family][c.dt], "test_gpu_kf_instances %s %s" % (c.family, np.dtype(c.dt).name)
+
+
 # ------------------------------------------------------------------------------------------ kernel names
-def _b(v):
-    return "true" if v else "false"
-
-
-def k_direct(dt, n, m, ex):
-    return "kf_direct_kernel<%s, %d, %d, %s, 0>" % (TNAME[dt], n, m, _b(ex))
-
-
-def k_rb(dt, n, m, rpl, ex, mode, shared):
-    return "kf_rowblock_kernel<%s, %d, %d, %d, %s, %d, %s>" % (TNAME[dt], n, m, rpl, _b(ex), mode, _b(shared))
-
-
 def k_tc(nx, M):
     return "kf_cov_tc_kernel<%d, %d>" % (nx, M)
 
 
-def k_gen(dt):
-    return "kf_generic_kernel<%s, 0>" % TNAME[dt]
-
-
-def k_fast(mode, shared, ex):
-    return "kf42_f32_kernel<%d, %d, %s, 0, 0, NoPattern>" % (mode, shared, _b(ex))
-
-
 def k_batch(dt, n, m, staged):
-    return "kf_batch_kernel<%s, %d, %d, %s>" % (TNAME[dt], n, m, _b(staged))
+    return "kf_batch_kernel<%s, %d, %d, %s>" % (TNAME[dt], n, m, b(staged))
 
 
 def k_rts(dt, n=None):
@@ -119,15 +103,6 @@ class Case:
         if self.entry == "rts":
             s += "-shift%d" % self.shift
         return s + "-N%d" % self.Np
-
-
-def rb_fpw(dt, n, m, rpl):
-    """kf_rowblock.cu's pick_fpw: filters per warp tile, lowered until every tile array is a multiple of 16 bytes."""
-    es = np.dtype(dt).itemsize
-    for f in range(32 // (n // rpl), 0, -1):
-        if all((f * es * k) % 16 == 0 for k in (n, n * n, m * n, m * m, m)):
-            return f
-    raise AssertionError("no warp tile")
 
 
 def _sweep(tile):
@@ -267,24 +242,11 @@ CASES = _cases()
 CASE_IDS = [c.id for c in CASES]
 
 
-# ------------------------------------------------------------------------------------------ the table vs the source
-def _body(text, signature):
-    """The body of the function whose definition starts with ``signature`` (up to the closing brace at column 0)."""
-    i = text.index(signature)
-    return text[i:text.index("\n}\n", i)]
-
-
-def _src(name):
-    """The source without its comments (a commented-out dispatch line is not dispatched)."""
-    with open(os.path.join(CSRC, name)) as fh:
-        return re.sub(r"//[^\n]*|/\*.*?\*/", "", fh.read(), flags=re.S)
-
-
 def _dispatched():
     """Every kernel instance the five dispatch functions can launch, parsed from the source."""
     inst = set()
     # kf_direct.cu dispatch(): the shapes (those after `if constexpr (sizeof(T) == 4)` are fp32 only), EX both ways
-    d = _body(_src("kf_direct.cu"), "int dispatch(const bke_kf_args &a, cudaStream_t s)")
+    d = body(src("kf_direct.cu"), "int dispatch(const bke_kf_args &a, cudaStream_t s)")
     both, f32only = d.split("if constexpr (sizeof(T) == 4)") if "if constexpr" in d else (d, "")
     pat = r"a\.dim_x == (\d+) && a\.dim_z == (\d+)\) return launch_inst<T, (\d+), (\d+)>"
     direct = {F64: [], F32: []}
@@ -293,7 +255,7 @@ def _dispatched():
             assert (a, b) == (c, e)
             for dt in dts:
                 direct[dt].append((int(a), int(b)))
-    li = _body(_src("kf_direct.cu"), "int launch_inst(const bke_kf_args &a, cudaStream_t s, const DirP<T> *form")
+    li = body(src("kf_direct.cu"), "int launch_inst(const bke_kf_args &a, cudaStream_t s, const DirP<T> *form")
     exs = set(re.findall(r"kf_direct_kernel<T, N, M, (true|false), FORM>", li))
     assert exs == {"true", "false"}
     for dt, shapes in direct.items():
@@ -301,8 +263,8 @@ def _dispatched():
             for ex in (True, False):
                 inst.add(k_direct(dt, n, m, ex))
     # kf_rowblock.cu launch_kf_rowblock: shapes and RPL per dtype; launch_rb: the (EX, MODE, SHARED) instances
-    rbsrc = _src("kf_rowblock.cu")
-    lr = _body(rbsrc, "int launch_kf_rowblock(const bke_kf_args &a, cudaStream_t s)")
+    rbsrc = src("kf_rowblock.cu")
+    lr = body(rbsrc, "int launch_kf_rowblock(const bke_kf_args &a, cudaStream_t s)")
     f64part, f32part = lr.split("} else {")
     rows = {F64: [], F32: []}
     for part, dt in ((f64part, F64), (f32part, F32)):
@@ -310,24 +272,24 @@ def _dispatched():
             assert (a, b) == (c, e) and t == TNAME[dt]
             rows[dt].append((int(a), int(b), int(rpl)))
     variants = set(re.findall(r"kf_rowblock_kernel<T, N, M, RPL, (true|false), (\d), (true|false)>",
-                              _body(rbsrc, "int launch_rb(const bke_kf_args &a, cudaStream_t s)")))
+                              body(rbsrc, "int launch_rb(const bke_kf_args &a, cudaStream_t s)")))
     assert len(variants) == 7
     for dt, shapes in rows.items():
         for n, m, rpl in shapes:
             for ex, mode, sh in variants:
                 inst.add(k_rb(dt, n, m, rpl, ex == "true", int(mode), sh == "true"))
     # kf_tc.cu: the NX of launch_kf_tc and the M of launch_m (its default is M = 4)
-    tcsrc = _src("kf_tc.cu")
+    tcsrc = src("kf_tc.cu")
     nxs = sorted(int(v) for v in re.findall(r"tc::launch_m<(\d+)>\(p, m_here, s\)", tcsrc))
-    lm = _body(tcsrc, "int launch_m(const TcP &p, int m, cudaStream_t s)")
+    lm = body(tcsrc, "int launch_m(const TcP &p, int m, cudaStream_t s)")
     ms = [(c, v) for c, v in re.findall(r"case (\d+): return launch_t<NX, (\d+)>", lm)]
     assert all(c == v for c, v in ms)
     ms = sorted({int(v) for _, v in ms} | {int(v) for v in re.findall(r"default: return launch_t<NX, (\d+)>", lm)})
     inst |= {k_tc(nx, M) for nx in nxs for M in ms}
     # kf_batch.cu launch_kf_batch: the register shapes, staged and unstaged; everything else is the host loop
-    bsrc = _src("kf_batch.cu")
-    lb = _body(bsrc, "int launch_kf_batch(const bke_kf_batch_args &a, cudaStream_t s)")
-    stg = set(re.findall(r"kf_batch_kernel<T, N, M, (true|false)>", _body(bsrc, "int launch_reg(const bke_kf_batch_args &a")))
+    bsrc = src("kf_batch.cu")
+    lb = body(bsrc, "int launch_kf_batch(const bke_kf_batch_args &a, cudaStream_t s)")
+    stg = set(re.findall(r"kf_batch_kernel<T, N, M, (true|false)>", body(bsrc, "int launch_reg(const bke_kf_batch_args &a")))
     assert stg == {"true", "false"}
     for d_, a, b, t, c, e in re.findall(r"k\.dtype == BKE_(F32|F64) && k\.dim_x == (\d+) && k\.dim_z == (\d+)\) "
                                         r"return launch_reg<(\w+), (\d+), (\d+)>", lb):
@@ -337,7 +299,7 @@ def _dispatched():
             inst.add(k_batch(dt, int(a), int(b), s))
     assert "return launch_host_loop(a, s);" in lb
     # kf_rts.cu launch_t: the register dims and the generic kernel, both dtypes
-    lt = _body(_src("kf_rts.cu"), "int launch_t(const bke_rts_args &a, cudaStream_t s)")
+    lt = body(src("kf_rts.cu"), "int launch_t(const bke_rts_args &a, cudaStream_t s)")
     for dt in (F32, F64):
         inst |= {k_rts(dt, int(v)) for v in re.findall(r"a\.dim_x == (\d+)\) \{ rts_reg_kernel<T, \1>", lt)}
         assert "rts_generic_kernel<T><<<" in lt
@@ -385,71 +347,9 @@ def test_instance_table_matches_dispatch():
     assert {"kf_direct_kernel", "kf_rowblock_kernel"} <= host_uf
     assert any(c.family == "host" and c.uf and any(k.startswith("kf_cov_tc") for k in c.kernels) for c in CASES)
     # the dispatch conditions the table relies on
-    assert "if (a.flags & BKE_UPDATE_FIRST) return BKE_ERR_UNSUPPORTED;" in _src("kf_direct.cu")
-    assert "if (dense && shared) return BKE_ERR_UNSUPPORTED;" in _src("kf_rowblock.cu")
-    assert "const bool staged = ((size_t)p.N * N * sizeof(T)) % 16 == 0 && p.N >= 32;" in _src("kf_batch.cu")
-
-
-# ------------------------------------------------------------------------------------------ buffers
-class Bufs:
-    """Device buffers, each with a 16-byte NaN guard before it (plus one element when it is misaligned) and five NaN
-    elements after it; outputs start as a finite sentinel, so an element a kernel must leave alone can be checked."""
-    SENT = 12345.0
-
-    def __init__(self, dt):
-        self.dt, self.keep, self.outs = dt, [], []
-
-    def put(self, a, mis=False, out=False, dtype=None):
-        import torch
-        dtype = dtype or self.dt
-        a = np.ascontiguousarray(a, dtype=dtype)
-        es = a.itemsize
-        off = 16 // es + (1 if mis else 0)
-        tdt = {np.dtype(F32): torch.float32, np.dtype(F64): torch.float64, np.dtype(np.int32): torch.int32,
-               np.dtype(np.uint8): torch.uint8}[a.dtype]
-        fill = float("nan") if tdt in (torch.float32, torch.float64) else -7
-        buf = torch.full((off + a.size + 5,), fill, dtype=tdt, device="cuda")
-        buf[off:off + a.size] = torch.from_numpy(a.reshape(-1)).cuda()
-        view = buf[off:off + a.size]
-        self.keep.append(buf)
-        if out:
-            self.outs.append((buf, off, a.size, a.shape))
-        return view
-
-    def out(self, shape, mis=False, dtype=None, fill=None):
-        return self.put(np.full(shape, self.SENT if fill is None else fill), mis, True, dtype)
-
-    def check_guards(self):
-        for buf, off, cnt, _ in self.outs:
-            h = buf.cpu().numpy()
-            pre, post = h[:off], h[off + cnt:]
-            if h.dtype.kind == "f":
-                assert np.all(np.isnan(pre)) and np.all(np.isnan(post)), "write outside an output array"
-            else:
-                assert np.all(pre == -7) and np.all(post == -7), "write outside an output array"
-
-
-def _ptr(t):
-    return None if t is None else t.data_ptr()
-
-
-def _call(fn, a):
-    import torch
-    from filterpy_b200 import _lib
-    lib = _lib.load()
-    rc = getattr(lib, fn)(ctypes.byref(a), torch.cuda.current_stream().cuda_stream)
-    assert rc == _lib.BKE_OK, lib.bke_last_error()
-    torch.cuda.synchronize()
-
-
-# ------------------------------------------------------------------------------------------ inputs
-def _rd(a, dt):
-    return np.asarray(a, np.float64).astype(dt).astype(np.float64)
-
-
-def _spd(rng, shape, k, scale):
-    a = rng.normal(size=shape + (k, k))
-    return scale * (a @ np.swapaxes(a, -1, -2) / k + np.eye(k))
+    assert "if (a.flags & BKE_UPDATE_FIRST) return BKE_ERR_UNSUPPORTED;" in src("kf_direct.cu")
+    assert "if (dense && shared) return BKE_ERR_UNSUPPORTED;" in src("kf_rowblock.cu")
+    assert "const bool staged = ((size_t)p.N * N * sizeof(T)) % 16 == 0 && p.N >= 32;" in src("kf_batch.cu")
 
 
 def _inputs(c, N, seed, singular):
@@ -460,9 +360,9 @@ def _inputs(c, N, seed, singular):
     n, m, dt = c.n, c.m, c.dt
     shared = {"per": "", "shared": "FQHR", "mixed": "FQ", "FH": "FH"}[c.models]
     cnt = lambda k: () if k in shared else (N,)
-    d = dict(x=rng.normal(size=(N, n)) * 3, P=_spd(rng, (N,), n, 2.0),
-             F=np.eye(n) + 0.1 * rng.normal(size=cnt("F") + (n, n)), Q=_spd(rng, cnt("Q"), n, 0.05),
-             H=rng.normal(size=cnt("H") + (m, n)), R=_spd(rng, cnt("R"), m, 0.5), z=rng.normal(size=(N, m)) * 3)
+    d = dict(x=rng.normal(size=(N, n)) * 3, P=spd(rng, (N,), n, 2.0),
+             F=np.eye(n) + 0.1 * rng.normal(size=cnt("F") + (n, n)), Q=spd(rng, cnt("Q"), n, 0.05),
+             H=rng.normal(size=cnt("H") + (m, n)), R=spd(rng, cnt("R"), m, 0.5), z=rng.normal(size=(N, m)) * 3)
     if c.ctrl:
         d["B"] = rng.normal(size=(N, n, 2)) if c.models == "per" else rng.normal(size=(n, 2))
         d["u"] = rng.normal(size=(N, 2))
@@ -480,7 +380,7 @@ def _inputs(c, N, seed, singular):
             R[-1, :] = 0; R[:, -1] = 0
         d["Q"], d["R"] = Q, R
         d["P"][sing] = 0
-    d = {k: _rd(v, dt) for k, v in d.items()}
+    d = {k: rd(v, dt) for k, v in d.items()}
     return d, sing
 
 
@@ -535,36 +435,6 @@ def _oracle_step(d, N, do_p, do_u, uf, valid, sing, alpha_sq):
     return o, upd, bad
 
 
-# ------------------------------------------------------------------------------------------ comparisons
-def _errlog(case, what, err, tol):
-    log = os.environ.get("BKE_TEST_ERRLOG")
-    if log:
-        with open(log, "a") as fh:
-            fh.write("test_gpu_kf_instances %s %s %s max_err=%.3e tol=%.1e\n"
-                     % (case.family, np.dtype(case.dt).name, what, err, tol))
-
-
-def _close(case, got, want, scale, cond, what, rows=None):
-    """|got - want| <= TOL * scale * cond per filter (axis 0, or axis 1 for [T, N, ...] arrays with rows=None)."""
-    tol = TOL[case.family][case.dt]
-    got = np.asarray(got, np.float64); want = np.asarray(want, np.float64)
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    if rows is not None:
-        got, want, scale, cond = got[rows], want[rows], scale[rows], cond[rows]
-    if got.size == 0:
-        return
-    assert np.all(np.isfinite(got)), "%s: not finite" % what
-    sh = (-1,) + (1,) * (want.ndim - 1)
-    err = np.abs(got - want) / (np.maximum(scale, 1e-300).reshape(sh) * cond.reshape(sh))
-    _errlog(case, what, err.max(), tol)
-    assert err.max() <= tol, "%s: max err %.3e of the filter's scale x cond > %.1e" % (what, err.max(), tol)
-
-
-def _mag(*arrs):
-    """Per filter (axis 0): the largest |entry| over the given arrays."""
-    return np.max([np.abs(a).reshape(a.shape[0], -1).max(axis=1) for a in arrs], axis=0)
-
-
 # ------------------------------------------------------------------------------------------ running a case
 def run_step(c, N, seed=0, variant="plain"):
     """One bke_kf_step call of case c on N filters: (got, want, masks) with every output host-side."""
@@ -586,34 +456,34 @@ def run_step(c, N, seed=0, variant="plain"):
     a.alpha_sq = ALPHA_SQ
     bank_mis = c.mis == "bank"
     xv = bf.put(d["x"], bank_mis, out=c.inplace); Pv = bf.put(d["P"], bank_mis, out=c.inplace)
-    a.x, a.P = _ptr(xv), _ptr(Pv)
+    a.x, a.P = ptr(xv), ptr(Pv)
     if c.inplace:
         xo, Po = xv, Pv
     else:
         xo, Po = bf.out((N, n), bank_mis), bf.out((N, n, n), bank_mis)
-    a.x_out, a.P_out = _ptr(xo), _ptr(Po)
+    a.x_out, a.P_out = ptr(xo), ptr(Po)
     for k in "FQHR":
         arr = d[k]
         v = bf.put(arr, c.mis == "F" and k == "F")
-        setattr(a, k, _ptr(v))
+        setattr(a, k, ptr(v))
         setattr(a, k + "_stride", 0 if arr.ndim == 2 else arr.shape[-1] * arr.shape[-2])
     if c.ctrl:
         a.dim_u = 2
-        a.B = _ptr(bf.put(d["B"])); a.B_stride = 0 if d["B"].ndim == 2 else 2 * n
-        a.u = _ptr(bf.put(d["u"])); a.u_stride = 2
-    a.z = _ptr(bf.put(d["z"]))
+        a.B = ptr(bf.put(d["B"])); a.B_stride = 0 if d["B"].ndim == 2 else 2 * n
+        a.u = ptr(bf.put(d["u"])); a.u_stride = 2
+    a.z = ptr(bf.put(d["z"]))
     if valid is not None:
-        a.z_valid = _ptr(bf.put(valid.astype(np.uint8), dtype=np.uint8))
+        a.z_valid = ptr(bf.put(valid.astype(np.uint8), dtype=np.uint8))
     outs = {}
     if c.ex:
         shapes = dict(x_prior=(N, n), P_prior=(N, n, n), K=(N, n, m), y=(N, m), S=(N, m, m), SI=(N, m, m),
                       log_likelihood=(N,))
         for k, s in shapes.items():
             outs[k] = bf.out(s)
-            setattr(a, k, _ptr(outs[k]))
+            setattr(a, k, ptr(outs[k]))
     st = bf.out((N,), dtype=np.int32, fill=5)
-    a.status = _ptr(st)
-    _call("bke_kf_step", a)
+    a.status = ptr(st)
+    call_ok("bke_kf_step", ctypes.byref(a))
     bf.check_guards()
     want, upd, bad = _oracle_step(d, N, do_p, do_u, c.uf, valid, sing, ALPHA_SQ)
     got = dict(x=xo.cpu().numpy().reshape(N, n), P=Po.cpu().numpy().reshape(N, n, n),
@@ -628,12 +498,13 @@ def check_step(c, N, seed, variant):
     got, want, d, upd, bad, valid, sticky = run_step(c, N, seed, variant)
     do_p, do_u = bool(c.mode & 1), bool(c.mode & 2)
     what = "%s N=%d %s" % (c.id, N, variant)
+    tol, label = _bound(c)
     cond = want["cond"]
     prior_x = want.get("x_prior", d["x"]); prior_P = want.get("P_prior", d["P"])
-    sx = _mag(d["x"], prior_x, want["x"])
-    sP = _mag(d["P"], prior_P, want["P"])
-    _close(c, got["x"], want["x"], sx, cond, what + " x")
-    _close(c, got["P"], want["P"], sP, cond, what + " P")
+    sx = mag(d["x"], prior_x, want["x"])
+    sP = mag(d["P"], prior_P, want["P"])
+    close(got["x"], want["x"], sx, cond, tol, what + " x", label)
+    close(got["P"], want["P"], sP, cond, tol, what + " P", label)
     st_want = want["status"].copy()
     if sticky:
         st_want[st_want == 0] = 5                   # BKE_STATUS_STICKY: written only where the step failed
@@ -643,8 +514,8 @@ def check_step(c, N, seed, variant):
     S = Bufs.SENT
     if do_p:                                        # (update first: the prior is predicted from the posterior)
         pc = cond if c.uf else np.ones(N)
-        _close(c, got["x_prior"], want["x_prior"], sx, pc, what + " x_prior")
-        _close(c, got["P_prior"], want["P_prior"], sP, pc, what + " P_prior")
+        close(got["x_prior"], want["x_prior"], sx, pc, tol, what + " x_prior", label)
+        close(got["P_prior"], want["P_prior"], sP, pc, tol, what + " P_prior", label)
     else:
         assert np.all(got["x_prior"] == S) and np.all(got["P_prior"] == S), what + " prior written without a predict"
     if not do_u:
@@ -655,14 +526,14 @@ def check_step(c, N, seed, variant):
     ux = d["x"] if (c.uf or not do_p) else prior_x
     H = _full(d["H"], N)
     sy = np.abs(H).max(axis=(1, 2)) * np.abs(ux).sum(axis=1) + np.abs(d["z"]).max(axis=1)
-    _close(c, got["y"], want["y"], sy, cond, what + " y", upd)
+    close(got["y"], want["y"], sy, cond, tol, what + " y", label, upd)
     miss = ~valid if valid is not None else np.zeros(N, bool)
     assert np.all(got["y"][miss] == 0), what + " y of a missed measurement"
     for k, w in (("K", "K"), ("S", "S"), ("SI", "SI")):
-        _close(c, got[k], want[w], _mag(np.nan_to_num(want[w])), cond, what + " " + k, upd)
+        close(got[k], want[w], mag(np.nan_to_num(want[w])), cond, tol, what + " " + k, label, upd)
         assert np.all(got[k][miss] == S), what + " %s written for a missed measurement" % k
-    _close(c, got["log_likelihood"], want["ll"], np.maximum(np.abs(np.nan_to_num(want["ll"])), 1.0), cond,
-           what + " log_likelihood", upd)
+    close(got["log_likelihood"], want["ll"], np.maximum(np.abs(np.nan_to_num(want["ll"])), 1.0), cond, tol,
+          what + " log_likelihood", label, upd)
     assert np.all(got["log_likelihood"][miss] == S), what + " log_likelihood written for a missed measurement"
 
 
@@ -689,7 +560,7 @@ def run_batch(c, N, seed=0, singular=False):
         T = 1                     # a shared Q = 0 and a singular R would make every filter's S degenerate over the epochs
     d, sing = _inputs(c, N, seed, singular)
     rng = np.random.default_rng(seed + 2)
-    zs = _rd(rng.normal(size=(T, N, m)) * 3, dt)
+    zs = rd(rng.normal(size=(T, N, m)) * 3, dt)
     valid = rng.random((T, N)) > 0.2
     bf = Bufs(dt)
     ba = _lib.KfBatchArgs()
@@ -699,30 +570,30 @@ def run_batch(c, N, seed=0, singular=False):
     a.flags = _lib.BKE_DO_PREDICT | _lib.BKE_DO_UPDATE | (_lib.BKE_UPDATE_FIRST if c.uf else 0)
     a.alpha_sq = ALPHA_SQ
     xv = bf.put(d["x"], out=c.inplace); Pv = bf.put(d["P"], out=c.inplace)
-    a.x, a.P = _ptr(xv), _ptr(Pv)
+    a.x, a.P = ptr(xv), ptr(Pv)
     xo, Po = (xv, Pv) if c.inplace else (bf.out((N, n)), bf.out((N, n, n)))
-    a.x_out, a.P_out = _ptr(xo), _ptr(Po)
+    a.x_out, a.P_out = ptr(xo), ptr(Po)
     for k in "FQHR":
         arr = d[k]
-        setattr(a, k, _ptr(bf.put(arr)))
+        setattr(a, k, ptr(bf.put(arr)))
         setattr(a, k + "_stride", 0 if arr.ndim == 2 else arr.shape[-1] * arr.shape[-2])
     if c.ctrl:
         a.dim_u = 2
-        a.B = _ptr(bf.put(d["B"])); a.B_stride = 0 if d["B"].ndim == 2 else 2 * n
-        a.u = _ptr(bf.put(d["u"])); a.u_stride = 2
+        a.B = ptr(bf.put(d["B"])); a.B_stride = 0 if d["B"].ndim == 2 else 2 * n
+        a.u = ptr(bf.put(d["u"])); a.u_stride = 2
     st = bf.out((N,), dtype=np.int32, fill=5)
-    a.status = _ptr(st)
+    a.status = ptr(st)
     ba.n_steps = T
-    ba.zs = _ptr(bf.put(zs))
-    ba.zs_valid = _ptr(bf.put(valid.astype(np.uint8), dtype=np.uint8))
+    ba.zs = ptr(bf.put(zs))
+    ba.zs_valid = ptr(bf.put(valid.astype(np.uint8), dtype=np.uint8))
     outs = {}
     if c.ex:
         mis = c.mis == "means"
         for k, s in (("means", (T, N, n)), ("covariances", (T, N, n, n)), ("means_p", (T, N, n)),
                      ("covariances_p", (T, N, n, n))):
             outs[k] = bf.out(s, mis)
-            setattr(ba, k, _ptr(outs[k]))
-    _call("bke_kf_batch_filter", ba)
+            setattr(ba, k, ptr(outs[k]))
+    call_ok("bke_kf_batch_filter", ctypes.byref(ba))
     bf.check_guards()
     # the oracle: epoch by epoch
     want = dict(means=np.zeros((T, N, n)), covariances=np.zeros((T, N, n, n)), means_p=np.zeros((T, N, n)),
@@ -754,17 +625,18 @@ def run_batch(c, N, seed=0, singular=False):
 def test_batch_instance_vs_oracle(case):
     """bke_kf_batch_filter: means, covariances, means_p, covariances_p, the final x / P and status against the fp64
     oracle, with a z_valid mask, alpha^2 != 1 and filters whose S is singular every epoch."""
+    tol, label = _bound(case)
     for i, N in enumerate(case.Ns):
         for singular in ((False, True) if N == case.Ns[-1] else (False,)):
             got, want, last, cond, status = run_batch(case, N, seed=N + i, singular=singular)
             what = "%s N=%d%s" % (case.id, N, " singular" if singular else "")
-            sx = np.maximum(_mag(*[np.swapaxes(want[k], 0, 1) for k in ("means", "means_p")]), 1e-300)
-            sP = np.maximum(_mag(*[np.swapaxes(want[k], 0, 1) for k in ("covariances", "covariances_p")]), 1e-300)
+            sx = np.maximum(mag(*[np.swapaxes(want[k], 0, 1) for k in ("means", "means_p")]), 1e-300)
+            sP = np.maximum(mag(*[np.swapaxes(want[k], 0, 1) for k in ("covariances", "covariances_p")]), 1e-300)
             for k, sc in (("means", sx), ("means_p", sx), ("covariances", sP), ("covariances_p", sP)):
                 if k in got:
-                    _close(case, np.swapaxes(got[k], 0, 1), np.swapaxes(want[k], 0, 1), sc, cond, what + " " + k)
-            _close(case, got["x"], last["x"], sx, cond, what + " x")
-            _close(case, got["P"], last["P"], sP, cond, what + " P")
+                    close(np.swapaxes(got[k], 0, 1), np.swapaxes(want[k], 0, 1), sc, cond, tol, what + " " + k, label)
+            close(got["x"], last["x"], sx, cond, tol, what + " x", label)
+            close(got["P"], last["P"], sP, cond, tol, what + " P", label)
             assert np.array_equal(got["status"], status), what + " status"
 
 
@@ -775,35 +647,35 @@ def run_rts(c, N, seed=0, singular=False):
     dt, n, T = c.dt, c.n, c.T
     rng = np.random.default_rng(seed)
     Xs = rng.normal(size=(T, N, n)) * 3
-    Ps = _spd(rng, (T, N), n, 1.0)
+    Ps = spd(rng, (T, N), n, 1.0)
     shape = {"shared": (), "per": (N,), "epoch": (T, N)}[c.models]
     F = np.eye(n) + 0.2 * rng.normal(size=shape + (n, n))
-    Q = _spd(rng, shape, n, 0.1)
+    Q = spd(rng, shape, n, 0.1)
     sing = np.zeros(N, bool)
     if singular and T > 1:
         sing[::7] = True
         Q = Q * 0
         Ps[T - 2, sing] = 0                            # Pp[T-2] = F 0 F' + 0
-    Xs, Ps, F, Q = (_rd(v, dt) for v in (Xs, Ps, F, Q))
+    Xs, Ps, F, Q = (rd(v, dt) for v in (Xs, Ps, F, Q))
     bf = Bufs(dt)
     a = _lib.RtsArgs()
     a.n_filters, a.n_steps, a.dim_x = N, T, n
     a.dtype = _lib.BKE_F32 if dt == F32 else _lib.BKE_F64
     a.model_shift = c.shift
     mis = c.mis == "bank"
-    a.Xs, a.Ps = _ptr(bf.put(Xs, mis)), _ptr(bf.put(Ps, mis))
-    a.F, a.Q = _ptr(bf.put(F)), _ptr(bf.put(Q))
+    a.Xs, a.Ps = ptr(bf.put(Xs, mis)), ptr(bf.put(Ps, mis))
+    a.F, a.Q = ptr(bf.put(F)), ptr(bf.put(Q))
     a.F_stride = a.Q_stride = 0 if c.models == "shared" else n * n
     a.F_step_stride = a.Q_step_stride = N * n * n if c.models == "epoch" else 0
     xo, Po = bf.out((T, N, n), mis), bf.out((T, N, n, n), mis)
-    a.x_out, a.P_out = _ptr(xo), _ptr(Po)
+    a.x_out, a.P_out = ptr(xo), ptr(Po)
     K = Pp = None
     if c.ex:
         K, Pp = bf.out((T, N, n, n), mis), bf.out((T, N, n, n), mis)
-        a.K, a.Pp = _ptr(K), _ptr(Pp)
+        a.K, a.Pp = ptr(K), ptr(Pp)
     st = bf.out((N,), dtype=np.int32, fill=5)
-    a.status = _ptr(st)
-    _call("bke_kf_rts_smoother", a)
+    a.status = ptr(st)
+    call_ok("bke_kf_rts_smoother", ctypes.byref(a))
     bf.check_guards()
     g = ~sing
     want = [v for v in okf.rts_smoother_bank(Xs[:, g], Ps[:, g], F[:, g] if c.models == "epoch" else
@@ -821,6 +693,7 @@ def run_rts(c, N, seed=0, singular=False):
 def test_rts_instance_vs_oracle(case):
     """bke_kf_rts_smoother: smoothed x, P, K, Pp and status against the fp64 oracle; a filter whose Pp is singular
     reports it."""
+    tol, label = _bound(case)
     for i, N in enumerate(case.Ns):
         for singular in ((False, True) if (N == case.Ns[-1] and case.T > 1) else (False,)):
             got, want, status, sing, (Xs, Ps) = run_rts(case, N, seed=N + i, singular=singular)
@@ -833,29 +706,15 @@ def test_rts_instance_vs_oracle(case):
             if case.T > 1:
                 cond = np.linalg.cond(wPp[:-1].reshape(-1, case.n, case.n)).reshape(case.T - 1, -1).max(axis=0)
             sw = lambda v: np.swapaxes(v, 0, 1)
-            sx = _mag(sw(Xs), sw(wx)); sP = _mag(sw(Ps), sw(wP), sw(wPp))
-            _close(case, sw(got[0]), sw(wx), sx, cond, what + " x")
-            _close(case, sw(got[1]), sw(wP), sP, cond, what + " P")
+            sx = mag(sw(Xs), sw(wx)); sP = mag(sw(Ps), sw(wP), sw(wPp))
+            close(sw(got[0]), sw(wx), sx, cond, tol, what + " x", label)
+            close(sw(got[1]), sw(wP), sP, cond, tol, what + " P", label)
             if case.ex:
-                _close(case, sw(got[2]), sw(wK), np.maximum(_mag(sw(wK)), 1.0), cond, what + " K")
-                _close(case, sw(got[3]), sw(wPp), sP, cond, what + " Pp")
+                close(sw(got[2]), sw(wK), np.maximum(mag(sw(wK)), 1.0), cond, tol, what + " K", label)
+                close(sw(got[3]), sw(wPp), sP, cond, tol, what + " Pp", label)
 
 
 # ------------------------------------------------------------------------------------------ which kernel runs
-def _kernel_name(s):
-    """'kf_direct_kernel<double, 4, 2, true, 0>' out of a demangled launch name (namespaces dropped)."""
-    s = re.sub(r"\(anonymous namespace\)::|\b\w+::", "", s)
-    mt = re.search(r"\b(kf\w*_kernel|rts_\w+_kernel)<", s)
-    if not mt:
-        return None
-    depth, i = 0, mt.end() - 1
-    for j in range(i, len(s)):
-        depth += {"<": 1, ">": -1}.get(s[j], 0)
-        if depth == 0:
-            return re.sub(r"\s+", " ", s[mt.start():j + 1])
-    return None
-
-
 def run_case(c, N):
     if c.entry == "step":
         return run_step(c, N)
@@ -865,36 +724,13 @@ def run_case(c, N):
 
 
 def _profiled_names():
-    """The kernel names of every CASES entry run once at its N, in launch order (torch.profiler, CUDA activity)."""
-    from torch.profiler import profile, ProfilerActivity
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for c in CASES:
-            run_case(c, c.Np)
-    names = [_kernel_name(e.name) for e in sorted(prof.events(), key=lambda e: e.time_range.start)]
-    return [k for k in names if k]
+    """The kernel names of every CASES entry run once at its N, in launch order."""
+    return profiled_names(lambda: [run_case(c, c.Np) for c in CASES], r"kf\w*_kernel|rts_\w+_kernel")
 
 
 @pytest.mark.gpu
 def test_dispatch_runs_the_kernels_of_the_table():
-    """Each CASES entry, run once at its N, launches the kernels the table names, in order, template arguments included.
-    The profile is taken in a process of its own: after a session of this size the profiler of the same process
-    reports no kernels to the sessions that follow it (other tests')."""
-    import json
-    import subprocess
-    import sys
-    here = os.path.dirname(os.path.abspath(__file__))
-    code = ("import json, sys; sys.path[:0] = %r; import test_gpu_kf_instances as t; print(json.dumps(t._profiled_names()))"
-            % [here, os.path.dirname(here)])
-    r = subprocess.run([sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    names = json.loads(r.stdout.strip().splitlines()[-1])
-    pos, bad = 0, []
-    for c in CASES:
-        want = c.kernels * (c.T if c.family == "host" else 1)
-        got = names[pos:pos + len(want)]
-        if got != want:
-            bad.append((c.id, want, got))
-            break                                       # everything after a wrong count is shifted
-        pos += len(want)
-    assert not bad and pos == len(names), (bad, names[pos:pos + 5])
+    """Each CASES entry, run once at its N, launches the kernels the table names, in order, template arguments included
+    (a batch host loop once per epoch)."""
+    check_launch_order("test_gpu_kf_instances",
+                       [(c.id, c.kernels * (c.T if c.family == "host" else 1)) for c in CASES])

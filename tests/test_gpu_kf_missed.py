@@ -12,7 +12,7 @@ import sys
 import numpy as np
 import pytest
 
-from test_gpu_kf import rel_close, RTOL
+from gpu_harness import rel_close, RTOL
 
 pytestmark = pytest.mark.gpu
 F32, F64 = np.float32, np.float64

@@ -6,7 +6,7 @@ import ctypes
 import numpy as np
 import pytest
 
-from test_gpu_kf import rel_close
+from gpu_harness import rel_close
 from test_gpu_kf_sym import MODES, NS, _args, _mirror, _oracle_step, _outputs, _uses_record
 
 pytestmark = pytest.mark.gpu

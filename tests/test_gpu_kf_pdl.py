@@ -6,7 +6,7 @@ steps with the oracle."""
 import numpy as np
 import pytest
 
-from test_gpu_kf import rel_close
+from gpu_harness import rel_close
 
 pytestmark = pytest.mark.gpu
 

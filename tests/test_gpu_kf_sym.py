@@ -4,7 +4,7 @@ exactly symmetric banks; never used once Q or R may have changed under it."""
 import numpy as np
 import pytest
 
-from test_gpu_kf import rel_close
+from gpu_harness import rel_close
 
 pytestmark = pytest.mark.gpu
 

@@ -15,12 +15,13 @@ import re
 import numpy as np
 import pytest
 
-CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "filterpy_b200", "csrc")
-F32, F64 = np.float32, np.float64
+from gpu_harness import CSRC, F32, F64, TNAME, call_ok, check_launch_order, close, mag, profiled_names
+
 # Relative to the track's scale: the largest |x_j| of its inputs for x (a combined mean can cancel to ~0), the
 # largest |entry| of the output for P.  Worst cases measured on an H100 with BKE_TEST_ERRLOG: x 2.7e-16 and
 # P 7.7e-16 (fp64), x 1.4e-7 and P 3.3e-7 (fp32); the probabilities 3.9 ulp.
 TOL = {F64: 1e-14, F32: 2e-6}
+LABEL = "test_gpu_mm_instances"
 PROB_ULPS = 6
 
 
@@ -100,30 +101,6 @@ def _args(n_tracks, dim_x, M, dtype, flags=0):
     return a
 
 
-def _run(fn, a):
-    import torch
-    from filterpy_b200 import _lib
-    lib = _lib.load()
-    rc = getattr(lib, fn)(ctypes.byref(a), torch.cuda.current_stream().cuda_stream)
-    assert rc == _lib.BKE_OK, lib.bke_last_error()
-    torch.cuda.synchronize()
-
-
-def _track_close(got, want, tol, what, scale=None):
-    """|got - want| <= tol * scale of the same track (axis 0 is the track); scale defaults to max|want|."""
-    got = np.asarray(got, np.float64); want = np.asarray(want, np.float64)
-    assert got.shape == want.shape and np.all(np.isfinite(got)), what
-    if scale is None:
-        scale = np.abs(want).reshape(want.shape[0], -1).max(axis=1)
-    scale = np.asarray(scale).reshape((-1,) + (1,) * (want.ndim - 1))
-    err = np.abs(got - want) / np.maximum(scale, 1e-300)
-    log = os.environ.get("BKE_TEST_ERRLOG")
-    if log:
-        with open(log, "a") as fh:
-            fh.write("test_gpu_mm_instances %s max_rel_err=%.3e tol=%.1e\n" % (what, err.max(), tol))
-    assert err.max() <= tol, "%s: max err %.3e of the track's scale > %.1e" % (what, err.max(), tol)
-
-
 def _inputs(N, n, M, dtype, seed):
     """Per-model states (M, N, n) / (M, N, n, n) with spread means and SPD covariances, rounded to ``dtype``;
     mixing weights omega (N, M, M) whose columns sum to 1, and mode probabilities mu (N, M)."""
@@ -164,11 +141,11 @@ def run_instance(op, dtype, n, M, misaligned, N, shared, seed=0):
     keep.append(wd)
     if op == "mix":
         a.omega, a.weights_stride = wd.data_ptr(), (0 if shared else M * M)
-        _run("bke_mm_mix", a)
+        call_ok("bke_mm_mix", ctypes.byref(a))
         want = oimm.mm_mix_bank(xs, Ps, w)
     else:
         a.mu, a.weights_stride = wd.data_ptr(), (0 if shared else M)
-        _run("bke_mm_estimate", a)
+        call_ok("bke_mm_estimate", ctypes.byref(a))
         wx, wP = oimm.mm_estimate_bank(xs, Ps, w, mmae=(op == "mmae"))
         want = (wx[None], wP[None])
     for (v, b), cnt in [(t, N * n) for t in xo] + [(t, N * n * n) for t in Po]:
@@ -187,28 +164,32 @@ def test_instance_vs_bank_oracle(inst):
             (gx, gP), (wx, wP), xs = run_instance(op, dtype, n, M, mis, N, shared, seed=N + M)
             what = "%s %s n=%d M=%d N=%d shared=%d" % (op, np.dtype(dtype).name, n, M, N, shared)
             for i in range(gx.shape[0]):
-                _track_close(gx[i], wx[i], TOL[dtype], what + " x[%d]" % i, xs)
-                _track_close(gP[i], wP[i], TOL[dtype], what + " P[%d]" % i)
+                close(gx[i], wx[i], xs, 1, TOL[dtype], what + " x[%d]" % i, LABEL)
+                close(gP[i], wP[i], mag(wP[i]), 1, TOL[dtype], what + " P[%d]" % i, LABEL)
+
+
+def _kernel(op, dtype, kern):
+    """The launch name of INSTANCES' kernel ``kern`` of op in dtype."""
+    k, args = re.match(r"(\w+)<([\d,]+)>", kern).groups()
+    if k == "rows":
+        return "k_mm_rows<%s, %s, %s>" % (TNAME[dtype], ", ".join(args.split(",")), "true" if op == "mix" else "false")
+    return "k_mm_%s<%s, %s>" % (k, TNAME[dtype], args)
+
+
+def _run_cases():
+    for op, dtype, n, M, mis, _ in INSTANCES:
+        run_instance(op, dtype, n, M, mis, 1, False)
+
+
+def _profiled_names():
+    return profiled_names(_run_cases, r"k_mm_\w+")
 
 
 @pytest.mark.gpu
 def test_dispatch_runs_the_kernel_of_the_table():
     """Each INSTANCES entry launches the kernel the table names (kernel names from torch.profiler)."""
-    from torch.profiler import profile, ProfilerActivity
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        for op, dtype, n, M, mis, _ in INSTANCES:
-            run_instance(op, dtype, n, M, mis, 1, False)
-    names = [e.name for e in sorted(prof.events(), key=lambda e: e.time_range.start) if "k_mm_" in e.name]
-    want = []
-    for op, dtype, n, M, mis, kern in INSTANCES:
-        T = "float" if dtype == F32 else "double"
-        k, args = re.match(r"(\w+)<([\d,]+)>", kern).groups()
-        if k == "rows":
-            want.append("k_mm_rows<%s, %s, %s>" % (T, ", ".join(args.split(",")), "true" if op == "mix" else "false"))
-        else:
-            want.append("k_mm_%s<%s, %s>" % (k, T, args))
-    got = [re.search(r"k_mm_\w+<[^>]*>", s).group(0) for s in names]
-    assert got == want
+    check_launch_order("test_gpu_mm_instances",
+                       [(i, [_kernel(op, dt, kern)]) for i, (op, dt, _, _, _, kern) in zip(INSTANCE_IDS, INSTANCES)])
 
 
 @pytest.mark.gpu
@@ -218,8 +199,8 @@ def test_mix_and_estimate_grid_stride_2e20_tracks():
         for mis in (False, True):
             (gx, gP), (wx, wP), xs = run_instance(op, F32, 4, 3, mis, 1 << 20, False, seed=7)
             for i in range(gx.shape[0]):
-                _track_close(gx[i], wx[i], TOL[F32], "%s 2^20 mis=%d x[%d]" % (op, mis, i), xs)
-                _track_close(gP[i], wP[i], TOL[F32], "%s 2^20 mis=%d P[%d]" % (op, mis, i))
+                close(gx[i], wx[i], xs, 1, TOL[F32], "%s 2^20 mis=%d x[%d]" % (op, mis, i), LABEL)
+                close(gP[i], wP[i], mag(wP[i]), 1, TOL[F32], "%s 2^20 mis=%d P[%d]" % (op, mis, i), LABEL)
 
 
 # ------------------------------------------------------------------------------------------ probabilities
@@ -273,7 +254,7 @@ def test_probabilities_vs_bank_oracle(mode, case, dtype):
         t = {k: torch.from_numpy(np.ascontiguousarray(v)).cuda() for k, v in
              dict(mu=mu, cbar=cbar, trans=trans, omega=np.zeros((N, M, M))).items()}
         a.mu, a.cbar, a.omega, a.trans = (t[k].data_ptr() for k in ("mu", "cbar", "omega", "trans"))
-        _run("bke_mm_probabilities", a)
+        call_ok("bke_mm_probabilities", ctypes.byref(a))
         what = "%s %s %s N=%d" % (mode, case, np.dtype(dtype).name, N)
         llf = ll.astype(F64)
         if mode == "mmae":

@@ -12,7 +12,7 @@ import re
 import numpy as np
 import pytest
 
-from test_gpu_kf import rel_close, RTOL
+from gpu_harness import rel_close, RTOL
 
 CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "filterpy_b200", "csrc")
 DT = 0.1

@@ -3,7 +3,7 @@ reference's golden vectors and the dgeqr2 oracle."""
 import numpy as np
 import pytest
 
-from test_gpu_kf import rel_close, RTOL
+from gpu_harness import rel_close, RTOL
 from test_oracle_srkf import GOLDEN, _ops, bank_replay
 
 pytestmark = pytest.mark.gpu

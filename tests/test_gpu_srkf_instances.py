@@ -27,11 +27,9 @@ import re
 import numpy as np
 import pytest
 
-from test_gpu_kf_instances import Bufs, _body, _mag, _ptr, _rd, _src
+from gpu_harness import (BUDGET, F32, F64, ROOT, TNAME, Bufs, b, body, call, check_launch_order, close, mag,
+                         profiled_names, ptr, rd, src)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-F32, F64 = np.float32, np.float64
-TNAME = {F32: "float", F64: "double"}
 MARGIN = 1e-3                     # the smallest dgeqr2 pivot ratio a compared filter may have
 
 TOL = {
@@ -41,13 +39,15 @@ TOL = {
 }
 
 
-# ------------------------------------------------------------------------------------------ kernel names
-def _b(v):
-    return "true" if v else "false"
+def _bound(c):
+    """Case c's tolerance and the label of its BKE_TEST_ERRLOG lines."""
+    return TOL[c.family][c.dt], "test_gpu_srkf_instances %s %s" % (c.family, np.dtype(c.dt).name)
 
+
+# ------------------------------------------------------------------------------------------ kernel names
 
 def k_reg(dt, n, m, ex):
-    return "srkf_reg_kernel<%s, %d, %d, %s>" % (TNAME[dt], n, m, _b(ex))
+    return "srkf_reg_kernel<%s, %d, %d, %s>" % (TNAME[dt], n, m, b(ex))
 
 
 def k_warp(dt):
@@ -59,9 +59,6 @@ def k_chol(dt, k):
 
 
 # ------------------------------------------------------------------------------------------ the launch shape
-BUDGET = 200 * 1024
-
-
 def sr_per_warp(n, m):
     """srkf.cu launch_warp: the elements of one warp's slice (x, xp, y, L, T1, H, K, S, SI, W), rounded up to 4."""
     nn, nm, D = n * n, n * m, n + m
@@ -185,26 +182,26 @@ CASES = _cases()
 # ------------------------------------------------------------------------------------------ the table vs the source
 def _dispatched():
     """Every kernel instance srkf.cu's dispatch() and launch_chol can launch, parsed from the source."""
-    src = _src("srkf.cu")
-    d = _body(src, "int dispatch(const bke_srkf_args &a, cudaStream_t s)")
+    text = src("srkf.cu")
+    d = body(text, "int dispatch(const bke_srkf_args &a, cudaStream_t s)")
     shapes = []
     for a, b, c, e in re.findall(r"n == (\d+) && m == (\d+)\) rc = launch_reg<T, (\d+), (\d+)>", d):
         assert (a, b) == (c, e)
         shapes.append((int(a), int(b)))
     assert "return rc == BKE_ERR_UNSUPPORTED ? launch_warp<T>(a, s) : rc;" in d
     assert "if (a.B == nullptr || a.u == nullptr) {" in d
-    lr = _body(src, "int launch_reg(const bke_srkf_args &a, cudaStream_t s)")
+    lr = body(text, "int launch_reg(const bke_srkf_args &a, cudaStream_t s)")
     assert set(re.findall(r"srkf_reg_kernel<T, N, M, (true|false)><<<", lr)) == {"true", "false"}
     inst = {k_reg(dt, n, m, ex) for dt in (F32, F64) for n, m in shapes for ex in (True, False)}
     inst |= {k_warp(dt) for dt in (F32, F64)}
     # launch_chol recurses from K = 1 (launch_cholesky_lower) up to BKE_CHOLESKY_MAX_DIM
     with open(os.path.join(ROOT, "include", "bke.h")) as fh:
         kmax = int(re.search(r"#define BKE_CHOLESKY_MAX_DIM (\d+)", fh.read()).group(1))
-    lc = _body(src, "int launch_chol(int64_t N, int32_t k, const void *A, int64_t stride, void *L, int32_t *status, "
+    lc = body(text, "int launch_chol(int64_t N, int32_t k, const void *A, int64_t stride, void *L, int32_t *status, "
                     "cudaStream_t s)")
     assert "if constexpr (K < BKE_CHOLESKY_MAX_DIM) return launch_chol<T, K + 1>" in lc
     assert "chol_lower_kernel<T, K><<<" in lc
-    assert "launch_chol<float, 1>(" in src and "launch_chol<double, 1>(" in src
+    assert "launch_chol<float, 1>(" in text and "launch_chol<double, 1>(" in text
     inst |= {k_chol(dt, k) for dt in (F32, F64) for k in range(1, kmax + 1)}
     return inst, shapes, kmax
 
@@ -234,7 +231,7 @@ def test_instance_table_matches_dispatch():
         assert warps_per_block(top + 1, 3, dt) == 0 and any(c.refused and c.n == top + 1 for c in w)
         assert {c.models for c in CASES if c.family == "chol" and c.dt == dt} == {"per", "shared"}
     # the launch formula the warp shapes are chosen from is the launch's own
-    lw = _body(_src("srkf.cu"), "int launch_warp(const bke_srkf_args &a, cudaStream_t s)")
+    lw = body(src("srkf.cu"), "int launch_warp(const bke_srkf_args &a, cudaStream_t s)")
     assert ("int per_warp = 2 * n + m + nn + (nn > nm ? nn : nm) + 2 * nm + 2 * m * m + (2 * nn > D * D ? 2 * nn : D * D);"
             in lw and "per_warp = (per_warp + 3) & ~3;" in lw and "budget = 200 * 1024" in lw)
 
@@ -305,32 +302,22 @@ def sr_inputs(c, N, seed):
                     **({"B": rng.normal(size=cnt + (n, 2))} if c.ctrl else {}))
 
     d = dict(draw(N), **models())
-    d = {k: _rd(v, dt) for k, v in d.items()}
+    d = {k: rd(v, dt) for k, v in d.items()}
     for _ in range(50):
         bad = ~_margin_ok(d, bool(c.mode & 1))
         if not bad.any():
             break
         if c.models == "shared" and bad.all():
-            d.update({k: _rd(v, dt) for k, v in models().items()})
+            d.update({k: rd(v, dt) for k, v in models().items()})
             continue
-        new = {k: _rd(v, dt) for k, v in draw(int(bad.sum())).items()}
+        new = {k: rd(v, dt) for k, v in draw(int(bad.sum())).items()}
         if c.models == "per":
-            new.update({k: _rd(v[:int(bad.sum())], dt) for k, v in models().items()})
+            new.update({k: rd(v[:int(bad.sum())], dt) for k, v in models().items()})
         for k, v in new.items():
             d[k] = d[k].copy()
             d[k][bad] = v
     assert _margin_ok(d, bool(c.mode & 1)).all(), "no draw keeps every filter clear of a dgeqr2 sign decision"
     return d
-
-
-# ------------------------------------------------------------------------------------------ running a step
-def _lib_call(fn, *args):
-    import torch
-    from filterpy_b200 import _lib
-    lib = _lib.load()
-    rc = getattr(lib, fn)(*args, torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    return rc, lib.bke_last_error().decode() if rc else ""
 
 
 def run_step(c, N, seed=0, sing=None, d=None):
@@ -355,28 +342,28 @@ def run_step(c, N, seed=0, sing=None, d=None):
     a.dtype = _lib.BKE_F32 if dt == F32 else _lib.BKE_F64
     a.flags = c.mode
     xv, Lv = bf.put(d["x"], c.mis == "x", out=c.inplace), bf.put(d["L"], c.mis == "L", out=c.inplace)
-    a.x, a.L = _ptr(xv), _ptr(Lv)
+    a.x, a.L = ptr(xv), ptr(Lv)
     xo, Lo = (xv, Lv) if c.inplace else (bf.out((N, n), c.mis == "x_out"), bf.out((N, n, n), c.mis == "L_out"))
-    a.x_out, a.L_out = _ptr(xo), _ptr(Lo)
+    a.x_out, a.L_out = ptr(xo), ptr(Lo)
     for k in ("F", "H", "Lq", "Lr"):
         arr = d[k]
-        setattr(a, k, _ptr(bf.put(arr, c.mis == k)))
+        setattr(a, k, ptr(bf.put(arr, c.mis == k)))
         setattr(a, k + "_stride", 0 if arr.ndim == 2 else arr.shape[-1] * arr.shape[-2])
     if c.ctrl:
         a.dim_u = 2
-        a.B = _ptr(bf.put(d["B"])); a.B_stride = 0 if d["B"].ndim == 2 else 2 * n
-        a.u = _ptr(bf.put(d["u"])); a.u_stride = 2
-    a.z = _ptr(bf.put(d["z"], c.mis == "z"))
+        a.B = ptr(bf.put(d["B"])); a.B_stride = 0 if d["B"].ndim == 2 else 2 * n
+        a.u = ptr(bf.put(d["u"])); a.u_stride = 2
+    a.z = ptr(bf.put(d["z"], c.mis == "z"))
     if valid is not None:
-        a.z_valid = _ptr(bf.put(valid.astype(np.uint8), dtype=np.uint8))
+        a.z_valid = ptr(bf.put(valid.astype(np.uint8), dtype=np.uint8))
     outs = {}
     if c.ex:
         for k, s in OUT_SHAPES(n, m).items():
             outs[k] = bf.out((N,) + s, c.mis == k)
-            setattr(a, k, _ptr(outs[k]))
+            setattr(a, k, ptr(outs[k]))
     st = bf.out((N,), dtype=np.int32, fill=5)
-    a.status = _ptr(st)
-    rc, err = _lib_call("bke_srkf_step", ctypes.byref(a))
+    a.status = ptr(st)
+    rc, err = call("bke_srkf_step", ctypes.byref(a))
     if rc:
         return rc, err, None, d, valid
     bf.check_guards()
@@ -400,49 +387,25 @@ def sr_oracle(c, d, valid):
     return o, cond
 
 
-# ------------------------------------------------------------------------------------------ comparisons
-def _errlog(c, what, err, tol):
-    log = os.environ.get("BKE_TEST_ERRLOG")
-    if log:
-        with open(log, "a") as fh:
-            fh.write("test_gpu_srkf_instances %s %s %s max_err=%.3e tol=%.1e\n"
-                     % (c.family, np.dtype(c.dt).name, what, err, tol))
-
-
-def _close(c, got, want, scale, cond, what, rows=None):
-    """|got - want| <= TOL * scale * cond per filter (axis 0)."""
-    tol = TOL[c.family][c.dt]
-    got = np.asarray(got, np.float64); want = np.asarray(want, np.float64)
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    if rows is not None:
-        got, want, scale, cond = got[rows], want[rows], scale[rows], cond[rows]
-    if got.size == 0:
-        return
-    assert np.all(np.isfinite(got)), "%s: not finite" % what
-    sh = (-1,) + (1,) * (want.ndim - 1)
-    err = np.abs(got - want) / (np.maximum(scale, 1e-300).reshape(sh) * cond.reshape(sh))
-    _errlog(c, what, err.max(), tol)
-    assert err.max() <= tol, "%s: max err %.3e of the filter's scale x cond > %.1e" % (what, err.max(), tol)
-
-
 def check_step(c, N, seed, sing=None):
     rc, err, got, d, valid = run_step(c, N, seed, sing)
     assert rc == 0, err
     want, cond = sr_oracle(c, d, valid)
     what = "%s N=%d seed=%d%s" % (c.id, N, seed, "" if sing is None else " singular")
+    tol, label = _bound(c)
     do_p, do_u = bool(c.mode & 1), bool(c.mode & 2)
     prior_x, prior_L = want.get("x_prior", d["x"]), want.get("L_prior", d["L"])
-    sx, sL = _mag(d["x"], prior_x, want["x"]), _mag(d["L"], prior_L, want["L"])
-    _close(c, got["x"], want["x"], sx, cond, what + " x")
-    _close(c, got["L"], want["L"], sL, cond, what + " L")
+    sx, sL = mag(d["x"], prior_x, want["x"]), mag(d["L"], prior_L, want["L"])
+    close(got["x"], want["x"], sx, cond, tol, what + " x", label)
+    close(got["L"], want["L"], sL, cond, tol, what + " L", label)
     assert np.array_equal(got["status"], want["status"]), what + " status"
     assert np.all(np.triu(got["L"], 1) == 0), what + " L above its diagonal"
     if not c.ex:
         return got, want
     S = Bufs.SENT
     if do_p:
-        _close(c, got["x_prior"], want["x_prior"], sx, cond, what + " x_prior")
-        _close(c, got["L_prior"], want["L_prior"], sL, cond, what + " L_prior")
+        close(got["x_prior"], want["x_prior"], sx, cond, tol, what + " x_prior", label)
+        close(got["L_prior"], want["L_prior"], sL, cond, tol, what + " L_prior", label)
     else:
         assert np.all(got["x_prior"] == S) and np.all(got["L_prior"] == S), what + " prior written without a predict"
     keys = ("K", "y", "S1_2", "SI1_2")
@@ -453,9 +416,9 @@ def check_step(c, N, seed, sing=None):
     upd = valid
     H = np.broadcast_to(d["H"], (N,) + d["H"].shape[-2:])
     sy = np.abs(H).max(axis=(1, 2)) * np.abs(prior_x).sum(axis=1) + np.abs(d["z"]).max(axis=1)
-    _close(c, got["y"], want["y"], sy, cond, what + " y", upd)
+    close(got["y"], want["y"], sy, cond, tol, what + " y", label, upd)
     for k in ("K", "S1_2", "SI1_2"):
-        _close(c, got[k], want[k], _mag(np.nan_to_num(want[k])), cond, what + " " + k, upd)
+        close(got[k], want[k], mag(np.nan_to_num(want[k])), cond, tol, what + " " + k, label, upd)
     for k in keys:
         assert np.all(got[k][~upd] == S), what + " %s written for a missed measurement" % k
     bad = want["status"] != 0
@@ -519,7 +482,7 @@ def chol_inputs(c, N, seed):
     shape = () if c.models == "shared" else (N,)
     a = rng.normal(size=shape + (k, k))
     A = a @ np.swapaxes(a, -1, -2) / k + 0.5 * np.eye(k)
-    A = _rd(A, c.dt)
+    A = rd(A, c.dt)
     if c.models == "per" and N >= 8:
         j = rng.integers(0, k, size=N)
         f = np.arange(3, N, 7)
@@ -556,10 +519,9 @@ def run_chol(c, N, seed=0):
     Av = bf.put(Ak)
     Lo = bf.out((N, k, k))
     st = bf.out((N,), dtype=np.int32, fill=5)
-    rc, err = _lib_call("bke_cholesky_lower", ctypes.c_int64(N), ctypes.c_int32(k),
-                        ctypes.c_int32(0 if dt == F32 else 1), ctypes.c_void_p(_ptr(Av)),
-                        ctypes.c_int64(0 if c.models == "shared" else k * k), ctypes.c_void_p(_ptr(Lo)),
-                        ctypes.c_void_p(_ptr(st)))
+    rc, err = call("bke_cholesky_lower", ctypes.c_int64(N), ctypes.c_int32(k), ctypes.c_int32(0 if dt == F32 else 1),
+                   ctypes.c_void_p(ptr(Av)), ctypes.c_int64(0 if c.models == "shared" else k * k),
+                   ctypes.c_void_p(ptr(Lo)), ctypes.c_void_p(ptr(st)))
     assert rc == 0, err
     bf.check_guards()
     return Lo.cpu().numpy().reshape(N, k, k), st.cpu().numpy(), np.broadcast_to(A, (N, k, k))
@@ -573,6 +535,7 @@ def test_cholesky_instance_vs_scipy(case):
     triangle (NaN here) never read, and BKE_STATUS_NOT_PD exactly where scipy raises."""
     from filterpy_b200 import _lib
     assert (_lib.BKE_F32, _lib.BKE_F64) == (0, 1)
+    tol, label = _bound(case)
     for i, N in enumerate(case.Ns):
         L, st, A = run_chol(case, N, seed=N + i)
         want, wst = chol_oracle(A)
@@ -582,58 +545,27 @@ def test_cholesky_instance_vs_scipy(case):
             assert (wst == 2).sum() >= 3
         ok = wst == 0
         assert np.all(np.triu(L[ok], 1) == 0), what + " L above its diagonal"
-        _close(case, L, want, _mag(np.nan_to_num(want)), np.linalg.cond(np.where(ok[:, None, None], A, np.eye(case.n))),
-               what + " L", ok)
+        close(L, want, mag(np.nan_to_num(want)), np.linalg.cond(np.where(ok[:, None, None], A, np.eye(case.n))), tol,
+              what + " L", label, ok)
 
 
 # ------------------------------------------------------------------------------------------ which kernel runs
-def _kernel_name(s):
-    """'srkf_reg_kernel<double, 4, 2, true>' out of a demangled launch name (namespaces dropped)."""
-    s = re.sub(r"\(anonymous namespace\)::|\b\w+::", "", s)
-    mt = re.search(r"\b(srkf_\w+_kernel|chol_lower_kernel)<", s)
-    if not mt:
-        return None
-    depth, i = 0, mt.end() - 1
-    for j in range(i, len(s)):
-        depth += {"<": 1, ">": -1}.get(s[j], 0)
-        if depth == 0:
-            return re.sub(r"\s+", " ", s[mt.start():j + 1])
-    return None
+def _run_cases():
+    for c in CASES:
+        if c.family == "chol":
+            run_chol(c, c.Np)
+        else:
+            rc, err, _, _, _ = run_step(c, c.Np)
+            assert (rc != 0) == c.refused, (c.id, err)
 
 
 def _profiled_names():
-    """The kernel names of every CASES entry run once at its N, in launch order (torch.profiler, CUDA activity)."""
-    from torch.profiler import profile, ProfilerActivity
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for c in CASES:
-            if c.family == "chol":
-                run_chol(c, c.Np)
-            else:
-                rc, err, _, _, _ = run_step(c, c.Np)
-                assert (rc != 0) == c.refused, (c.id, err)
-    names = [_kernel_name(e.name) for e in sorted(prof.events(), key=lambda e: e.time_range.start)]
-    return [k for k in names if k]
+    """The kernel names of every CASES entry run once at its N, in launch order."""
+    return profiled_names(_run_cases, r"srkf_\w+_kernel|chol_lower_kernel")
 
 
 @pytest.mark.gpu
 def test_dispatch_runs_the_kernels_of_the_table():
     """Each CASES entry, run once at its N, launches the kernels the table names, in order, template arguments included
-    (a refused shape launches none).  The profile is taken in a process of its own, as in test_gpu_kf_instances."""
-    import json
-    import subprocess
-    import sys
-    here = os.path.dirname(os.path.abspath(__file__))
-    code = ("import json, sys; sys.path[:0] = %r; import test_gpu_srkf_instances as t; print(json.dumps(t._profiled_names()))"
-            % [here, os.path.dirname(here)])
-    r = subprocess.run([sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    names = json.loads(r.stdout.strip().splitlines()[-1])
-    pos, bad = 0, []
-    for c in CASES:
-        got = names[pos:pos + len(c.kernels)]
-        if got != c.kernels:
-            bad.append((c.id, c.kernels, got))
-            break                                       # everything after a wrong count is shifted
-        pos += len(c.kernels)
-    assert not bad and pos == len(names), (bad, names[pos:pos + 5])
+    (a refused shape launches none)."""
+    check_launch_order("test_gpu_srkf_instances", [(c.id, c.kernels) for c in CASES])

@@ -2,7 +2,7 @@
 import numpy as np
 import pytest
 
-from test_gpu_kf import rel_close, RTOL
+from gpu_harness import rel_close, RTOL
 
 pytestmark = pytest.mark.gpu
 

@@ -5,7 +5,7 @@ import pytest
 
 import ukf_hooks_oracle as oh
 from oracle import ukf as oukf
-from test_gpu_kf import rel_close, RTOL
+from gpu_harness import rel_close, RTOL
 
 pytestmark = pytest.mark.gpu
 

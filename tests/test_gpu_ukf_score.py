@@ -6,7 +6,7 @@ import pytest
 import torch
 
 import ukf_score_oracle as uso
-from test_gpu_kf import RTOL
+from gpu_harness import RTOL
 from test_gpu_sigma_instances import INSTANCES, INSTANCE_IDS, FX, HX, _corr_spd
 from test_oracle_ukf_score import CASES, load
 from oracle import ukf as oukf

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 import ukf_simplex_oracle as osx
-from test_gpu_kf import rel_close, RTOL
+from gpu_harness import rel_close, RTOL
 from test_gpu_sigma_instances import (INSTANCES, INSTANCE_IDS, DT, FX, HX, DTYPES, STEP_TOL, _problem, _take, _compare,
                                       _per_filter)
 
