@@ -1,6 +1,7 @@
 // kf_rowblock.cu — fused predict+update for shapes whose covariance does not fit one thread's
-// registers (BASELINE config 3: dim_x=9, dim_z=3, fp64; also 4/2 fp64, 6/3): a sub-warp of G lanes
-// owns one filter, each lane owns RPL consecutive ROWS of every n x n matrix.
+// registers (BASELINE config 3: dim_x=9, dim_z=3, fp64; also 9/3 fp32, 6/3 fp64, 16/4 and 16/2 in both
+// dtypes, 32/4 fp32): a sub-warp of G lanes owns one filter, each lane owns RPL consecutive ROWS of every
+// n x n matrix.
 //
 //   * every row-block product C[r,:] = sum_k A[r,k] * B[k,:] keeps A's rows and C's rows in the
 //     owning lane's registers and reads B from shared memory — the same address for the G lanes of
@@ -528,9 +529,15 @@ int launch_rb(const bke_kf_args &a, cudaStream_t s)
         if (mode == 1) kern = kf_rowblock_kernel<T, N, M, RPL, true, 1, false>;     // the single-mode and the
         if (mode == 2) kern = kf_rowblock_kernel<T, N, M, RPL, true, 2, false>;     // shared-model kernels always
         if (shared) {                                                                                     // carry the optional outputs
-            kern = kf_rowblock_kernel<T, N, M, RPL, true, 3, true>;
-            if (mode == 1) kern = kf_rowblock_kernel<T, N, M, RPL, true, 1, true>;
-            if (mode == 2) kern = kf_rowblock_kernel<T, N, M, RPL, true, 2, true>;
+            // fp32 dim_x = 16 / 32: the tensor-core tile (kf_tc.cu) takes every shared-model predict, alone or fused
+            if constexpr (sizeof(T) == 4 && (N == 16 || N == 32)) {
+                if (mode != 2) return BKE_ERR_UNSUPPORTED;
+                kern = kf_rowblock_kernel<T, N, M, RPL, true, 2, true>;
+            } else {
+                kern = kf_rowblock_kernel<T, N, M, RPL, true, 3, true>;
+                if (mode == 1) kern = kf_rowblock_kernel<T, N, M, RPL, true, 1, true>;
+                if (mode == 2) kern = kf_rowblock_kernel<T, N, M, RPL, true, 2, true>;
+            }
         }
         const bool kern_extras = extras || mode != 3 || shared;      // the instance selected above carries them
         const int smem = RB_WARPS * (Gm::WARP_BYTES + (kern_extras ? Gm::EX_BYTES : 0) + (shared ? Gm::SH_BYTES : 0));
@@ -592,7 +599,6 @@ int launch_kf_rowblock(const bke_kf_args &a, cudaStream_t s)
     const int n = a.dim_x, m = a.dim_z;
     if (a.dtype == BKE_F64) {
         if (n == 9 && m == 3) return launch_rb<double, 9, 3, 3>(a, s);
-        if (n == 4 && m == 2) return launch_rb<double, 4, 2, 2>(a, s);
         if (n == 6 && m == 3) return launch_rb<double, 6, 3, 3>(a, s);
         // dim_x = 16: one row per lane, 16 lanes per filter, 2 filters per warp tile
         if (n == 16 && m == 4) return launch_rb<double, 16, 4, 1>(a, s);
@@ -602,7 +608,6 @@ int launch_kf_rowblock(const bke_kf_args &a, cudaStream_t s)
         if (n == 16 && m == 2) return launch_rb<float, 16, 2, 2>(a, s);
         // dim_x = 32: one row per lane, the whole warp on one filter (the update half of the tensor-core predict, kf_tc.cu)
         if (n == 32 && m == 4) return launch_rb<float, 32, 4, 1>(a, s);
-        if (n == 6 && m == 3) return launch_rb<float, 6, 3, 3>(a, s);
         if (n == 9 && m == 3) return launch_rb<float, 9, 3, 3>(a, s);        // 8 filters per warp tile (see pick_fpw)
     }
     return BKE_ERR_UNSUPPORTED;

@@ -94,7 +94,7 @@ int bke_device_count(void);
  * SI[N,m,m], log_likelihood[N] (log N(y; 0, S), kalman_filter.py:1203-1210), status[N].
  * x_out/P_out may alias x/P (in-place update).
  * Kernels behind this call (same arithmetic, picked by shape; DESIGN.md §3): 4/2 fp32 TMA register tile, register tiles
- * with direct loads (4/2 fp64, 1/1 .. 4/4, 6/3 fp32), row blocks (9/3, 6/3, 16/4, 16/2, 32/4 fp32), a catch-all for any
+ * with direct loads (4/2 fp64, 1/1 .. 4/4, 6/3 fp32), row blocks (9/3, 16/4, 16/2, 6/3 fp64, 32/4 fp32), a catch-all for any
  * shape, and — fp32 banks with dim_x = 16 or 32 whose F and Q are shared (stride 0) — the wgmma tile: F P F' as
  * three-term TF32 products accumulated in fp32 (everything else of the
  * step in plain fp32), the whole predict+update in one launch when H and R are shared too and dim_z <= 4.

@@ -6,8 +6,7 @@ bke_kf_step tries, in order, the tensor-core tile kf_cov_tc_kernel<NX, M> (csrc/
 kf_rowblock_kernel<T, N, M, RPL, EX, MODE, SHARED> (csrc/kf_rowblock.cu, a ragged tail goes to the catch-all) and the
 catch-all kf_generic_kernel<T> (csrc/kf_generic.cu).  bke_kf_batch_filter runs kf_batch_kernel<T, N, M, STAGED>
 (csrc/kf_batch.cu) or a host loop of bke_kf_step epochs; bke_kf_rts_smoother runs rts_reg_kernel<T, N> or
-rts_generic_kernel<T> (csrc/kf_rts.cu).  CASES reaches every instance these dispatches can reach; rb_unreachable names
-the row-block instances no call can reach (an earlier family always takes their calls), with the reason.
+rts_generic_kernel<T> (csrc/kf_rts.cu).  CASES reaches every instance these dispatches can launch.
 
 Inputs are rounded to the kernel's dtype before the oracle sees them, so only the kernel's own arithmetic is measured.
 Each error is taken relative to the filter's own scale (the largest |entry| of the same quantity of that filter, the
@@ -111,21 +110,9 @@ def _sweep(tile):
 
 DIRECT = {F64: [(4, 2), (2, 1), (1, 1), (2, 2), (3, 1), (4, 1), (4, 4)],
           F32: [(4, 2), (2, 1), (1, 1), (2, 2), (3, 1), (4, 1), (4, 4), (6, 3), (6, 2)]}
-ROWBLOCK = {F64: [(9, 3, 3), (4, 2, 2), (6, 3, 3), (16, 4, 1), (16, 2, 1)],
-            F32: [(16, 4, 2), (16, 2, 2), (32, 4, 1), (6, 3, 3), (9, 3, 3)]}
+ROWBLOCK = {F64: [(9, 3, 3), (6, 3, 3), (16, 4, 1), (16, 2, 1)],
+            F32: [(16, 4, 2), (16, 2, 2), (32, 4, 1), (9, 3, 3)]}
 TC_DIMS = (16, 32)
-
-
-def rb_unreachable(dt, n, m, mode, shared):
-    """Why no bke_kf_step call reaches this row-block instance, or None.  kf_direct takes every call of its shapes
-    whose per-filter arrays it can load (its alignment checks cover everything the row block checks), so only a shared
-    model at an address it refuses reaches the row block there; the tensor-core kernel takes every shared-model
-    predict of fp32 dim_x = 16 / 32 (alone or fused), which leaves the row block only the update-only call."""
-    if (n, m) in DIRECT[dt] and not shared:
-        return "kf_direct takes every per-filter call of this shape"
-    if dt == F32 and n in TC_DIMS and shared and mode != 2:
-        return "kf_cov_tc_kernel takes every shared-model predict of this shape"
-    return None
 
 
 def _cases():
@@ -140,24 +127,24 @@ def _cases():
                     models = mod or (("per", "shared")[(mode + ex) % 2])
                     out.append(Case("step", "direct", dt, n, m, [k_direct(dt, n, m, ex)], 129, _sweep(128),
                                     models=models, ex=ex, mode=mode, inplace=(mode == 2 and not ex)))
-    # the row blocks: every shape x MODE x SHARED (x EX for the fused per-filter instance) that a call can reach
+    # the row blocks: every shape x MODE x SHARED (x EX for the fused per-filter instance), except the shared-model
+    # predicts of fp32 dim_x = 16 / 32, which the tensor-core kernel takes (alone or fused)
     for dt in (F64, F32):
         for n, m, rpl in ROWBLOCK[dt]:
             fpw = rb_fpw(dt, n, m, rpl)
             Np = 3 * fpw
             for mode in (3, 1, 2):
                 for shared in (False, True):
-                    if rb_unreachable(dt, n, m, mode, shared):
+                    if shared and mode != 2 and dt == F32 and n in TC_DIMS:
                         continue
                     exs = (True, False) if (mode == 3 and not shared) else ((mode == 1,) if not shared else (mode != 3,))
                     for ex in exs:
                         kern_ex = ex or mode != 3 or shared
-                        mis = "F" if (shared and (n, m) in DIRECT[dt]) else None
                         out.append(Case("step", "rowblock", dt, n, m, [k_rb(dt, n, m, rpl, kern_ex, mode, shared)], Np,
-                                        _sweep(fpw), models="shared" if shared else "per", mis=mis, ex=ex, mode=mode,
+                                        _sweep(fpw), models="shared" if shared else "per", ex=ex, mode=mode,
                                         inplace=(mode == 1 and shared)))
             # a ragged bank: the whole warp tiles on the row block, the tail on the catch-all kernel
-            if fpw > 1 and not rb_unreachable(dt, n, m, 3, False):
+            if fpw > 1:
                 out.append(Case("step", "rowblock", dt, n, m, [k_rb(dt, n, m, rpl, True, 3, False), k_gen(dt)],
                                 3 * fpw + 1, (fpw + 1, 2 * fpw - 1, 1037)))
     # the tensor cores: NX x M (M = dim_z of a fused step with shared H, R; 0 = the predict alone)
@@ -194,6 +181,12 @@ def _cases():
             Case("step", "generic", dt, 9, 3, [k_gen(dt)], 5, G, mis="bank"),                      # a misaligned bank
             Case("step", "generic", dt, 4, 4, [k_gen(dt)], 5, G, mis="bank", inplace=True),
         ]
+    # a shared F one element off a 16-byte boundary at a kf_direct shape: kf_direct refuses it, and the row block has
+    # no instance of these shapes
+    for dt, (n, m) in ((F64, (4, 2)), (F32, (6, 3))):
+        for mode in (3, 1, 2):
+            out.append(Case("step", "generic", dt, n, m, [k_gen(dt)], 48, _sweep(16), models="shared", mis="F",
+                            ex=(mode != 3), mode=mode, inplace=(mode == 1)))
     # batch_filter: the four register instances, staged (bulk copies, N >= 32 and an epoch's slice 16-byte aligned)
     # and unstaged, then the host loop of bke_kf_step epochs
     out += [
@@ -262,7 +255,8 @@ def _dispatched():
         for n, m in shapes:
             for ex in (True, False):
                 inst.add(k_direct(dt, n, m, ex))
-    # kf_rowblock.cu launch_kf_rowblock: shapes and RPL per dtype; launch_rb: the (EX, MODE, SHARED) instances
+    # kf_rowblock.cu launch_kf_rowblock: shapes and RPL per dtype; launch_rb: the (EX, MODE, SHARED) instances, where
+    # the fp32 shapes its `if constexpr` names take the first branch's shared-model instances instead of the second's
     rbsrc = src("kf_rowblock.cu")
     lr = body(rbsrc, "int launch_kf_rowblock(const bke_kf_args &a, cudaStream_t s)")
     f64part, f32part = lr.split("} else {")
@@ -271,12 +265,17 @@ def _dispatched():
         for a, b, t, c, e, rpl in re.findall(r"n == (\d+) && m == (\d+)\) return launch_rb<(\w+), (\d+), (\d+), (\d+)>", part):
             assert (a, b) == (c, e) and t == TNAME[dt]
             rows[dt].append((int(a), int(b), int(rpl)))
-    variants = set(re.findall(r"kf_rowblock_kernel<T, N, M, RPL, (true|false), (\d), (true|false)>",
-                              body(rbsrc, "int launch_rb(const bke_kf_args &a, cudaStream_t s)")))
-    assert len(variants) == 7
+    lrb = body(rbsrc, "int launch_rb(const bke_kf_args &a, cudaStream_t s)")
+    guard = re.search(r"if constexpr \(sizeof\(T\) == 4 && \(N == (\d+) \|\| N == (\d+)\)\) \{([^{}]*)\} else \{([^{}]*)\}",
+                      lrb)
+    vpat = r"kf_rowblock_kernel<T, N, M, RPL, (true|false), (\d), (true|false)>"
+    variants = set(re.findall(vpat, lrb.replace(guard.group(0), "")))
+    guarded, unguarded = (set(re.findall(vpat, guard.group(i))) for i in (3, 4))
+    assert len(variants | unguarded) == 7 and guarded < unguarded
+    guarded_n = {int(guard.group(1)), int(guard.group(2))}
     for dt, shapes in rows.items():
         for n, m, rpl in shapes:
-            for ex, mode, sh in variants:
+            for ex, mode, sh in variants | (guarded if dt == F32 and n in guarded_n else unguarded):
                 inst.add(k_rb(dt, n, m, rpl, ex == "true", int(mode), sh == "true"))
     # kf_tc.cu: the NX of launch_kf_tc and the M of launch_m (its default is M = 4)
     tcsrc = src("kf_tc.cu")
@@ -313,30 +312,19 @@ def test_instance_table_matches_dispatch():
     M in the dispatch, or a removed one, fails here, on a machine without a GPU too."""
     inst, direct, rows, nxs = _dispatched()
     assert direct == DIRECT and rows == ROWBLOCK and tuple(nxs) == TC_DIMS
-    unreachable = set()
-    for dt, shapes in rows.items():
-        for n, m, rpl in shapes:
-            for ex, mode, sh in ((True, 3, False), (False, 3, False), (True, 1, False), (True, 2, False), (True, 3, True),
-                                 (True, 1, True), (True, 2, True)):
-                if rb_unreachable(dt, n, m, mode, sh):
-                    unreachable.add(k_rb(dt, n, m, rpl, ex, mode, sh))
     table = {k for c in CASES for k in c.kernels if not k.startswith("kf42_")}
-    assert not (table & unreachable)
-    assert table == inst - unreachable, (sorted(inst - unreachable - table), sorted(table - inst))
+    assert table == inst, (sorted(inst - table), sorted(table - inst))
     # every kf_direct shape x EX x mode
     got = {(c.dt, c.n, c.m, c.ex, c.mode) for c in CASES if c.family == "direct"}
     assert got == {(dt, n, m, ex, mode) for dt in (F32, F64) for n, m in DIRECT[dt] for ex in (True, False)
                    for mode in (1, 2, 3)}
-    # the row-block instances that only a misaligned shared model reaches are run that way
-    for c in CASES:
-        if c.family == "rowblock" and c.models == "shared" and (c.n, c.m) in DIRECT[c.dt]:
-            assert c.mis == "F"
-    # the catch-all's features, both dtypes
+    # the catch-all's features, both dtypes (mis="F": a shared model kf_direct refuses at one of its shapes)
     gen = [c for c in CASES if c.family == "generic"]
     for dt in (F32, F64):
         g = [c for c in gen if c.dt == dt]
         assert any(c.uf for c in g) and any(c.ctrl for c in g) and any(c.models == "mixed" for c in g)
         assert any(c.mis == "bank" for c in g) and any((c.n, c.m) == (12, 3) for c in g)
+        assert any(c.mis == "F" and (c.n, c.m) in DIRECT[dt] for c in g)
     # both plain TMA 4/2 calls, the two-launch steps, the host loop with update_first on each kind of epoch kernel
     assert {c.models for c in CASES if c.family == "fast"} == {"per", "shared"}
     assert any(c.kernels[0].startswith("kf_cov_tc") and c.kernels[1].startswith("kf_rowblock") for c in CASES
