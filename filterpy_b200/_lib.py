@@ -395,6 +395,23 @@ class ImmBatchArgs(ctypes.Structure):
     ]
 
 
+BKE_DB_NORMALIZE, BKE_DB_CONSTANT = 1, 2
+
+
+class DbArgs(ctypes.Structure):
+    _fields_ = [
+        ("n_rows", c_int64), ("n_bins", c_int64),
+        ("dtype", c_int32), ("flags", c_uint32),
+        ("kernel", c_void_p), ("kernel_len", c_int64), ("kernel_stride", c_int64),
+        ("offsets", c_void_p), ("offset", c_int64),
+        ("cval", c_double),
+        ("pdf", c_void_p), ("likelihood", c_void_p),
+        ("out", c_void_p),
+        ("sums", c_void_p),
+        ("workspace", c_void_p), ("workspace_bytes", c_size_t),
+    ]
+
+
 _MODEL = [c_int32] * 5        # dim_x, dim_z, dtype, fx_model, hx_model of the run-time compiled models
 
 # Every prototype of include/bke.h, in header order: symbol -> (restype, argtypes).  A struct pointer is typed
@@ -505,6 +522,8 @@ _SIGNATURES = {
                                      c_void_p]),
     "bke_searchsorted_bracket_sweep": (c_int, [c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
                                                c_void_p, c_void_p]),
+    "bke_db_workspace_bytes": (c_size_t, [c_int64, c_int32]),
+    "bke_db_step": (c_int, [POINTER(DbArgs), c_void_p]),
 }
 
 # every symbol include/bke.h declares (build() and the tests check that the library exports all of them)

@@ -815,4 +815,56 @@ int bke_ukf_score(const bke_ukf_score_args *args, void *stream)
     return checked_launch(args, validate_ukf_score_prebuilt, launch_ukf_score, stream);
 }
 
+size_t bke_db_workspace_bytes(int64_t n_bins, int32_t dtype) { return check_dtype(dtype) ? 0 : db_workspace_bytes(n_bins, dtype); }
+
+// the checks of bke_db_step; -1 = go
+static int validate_db(const bke_db_args *a)
+{
+    if (!a) { set_error("args is NULL"); return BKE_ERR_BAD_ARG; }
+    int rc;
+    if (a->n_rows < 0 || a->n_bins < 1) { set_error("bad sizes: n_rows must be >= 0 and n_bins >= 1"); return BKE_ERR_BAD_ARG; }
+    if (a->n_rows >= ((int64_t)1 << 31) || a->n_bins >= ((int64_t)1 << 31)) { set_error("n_rows and n_bins must be < 2^31"); return BKE_ERR_BAD_ARG; }
+    if ((rc = check_dtype(a->dtype))) return rc;
+    if (a->flags & ~(BKE_DB_NORMALIZE | BKE_DB_CONSTANT)) { set_error("flags may only hold BKE_DB_NORMALIZE and BKE_DB_CONSTANT"); return BKE_ERR_BAD_ARG; }
+    if (a->kernel && a->kernel_len < 1) { set_error("kernel_len must be 1 or greater"); return BKE_ERR_BAD_ARG; }
+    if (a->kernel && (rc = check_strides({{a->kernel_stride, a->kernel_len}}))) return rc;
+    if (a->sums && !(a->flags & BKE_DB_NORMALIZE)) { set_error("sums is an output of BKE_DB_NORMALIZE only"); return BKE_ERR_BAD_ARG; }
+    if (a->n_rows == 0) return BKE_OK;
+    if (!a->pdf || !a->out) { set_error("pdf and out must be non-NULL"); return BKE_ERR_BAD_ARG; }
+    const int64_t B = a->n_rows, M = a->n_bins, es = a->dtype == BKE_F32 ? 4 : 8;
+    const size_t need = db_workspace_bytes(M, a->dtype);
+    if (need) {
+        if (!a->workspace || ((uintptr_t)a->workspace & 255)) { set_error("workspace must be non-NULL and 256-byte aligned"); return BKE_ERR_BAD_ARG; }
+        if (a->workspace_bytes < need) { set_error("workspace too small: %zu < %zu", a->workspace_bytes, need); return BKE_ERR_BAD_ARG; }
+    }
+    // out may be pdf itself; every array the call writes must otherwise be clear of every other array it touches
+    struct Span { const void *p; int64_t bytes; bool written; };
+    const Span sp[] = {{a->out, B * M * es, true}, {a->pdf, B * M * es, false}, {a->likelihood, B * M * es, false},
+                       {a->kernel, (a->kernel_stride ? B : 1) * a->kernel_len * 8, false},
+                       {a->offsets, B * 8, false}, {a->sums, B * 8, true},
+                       {need ? a->workspace : nullptr, (int64_t)need, true}};
+    const int ns = sizeof(sp) / sizeof(sp[0]);
+    for (int i = 0; i < ns; i++) {
+        for (int k = i + 1; k < ns; k++) {
+            if (!sp[i].p || !sp[k].p || (!sp[i].written && !sp[k].written) || (i == 0 && k == 1 && sp[0].p == sp[1].p)) continue;
+            if (!a->kernel && (i == 3 || k == 3)) continue;
+            const uintptr_t p0 = (uintptr_t)sp[i].p, p1 = (uintptr_t)sp[k].p;
+            if (p0 < p1 + (uintptr_t)sp[k].bytes && p1 < p0 + (uintptr_t)sp[i].bytes) {
+                set_error("an array bke_db_step writes overlaps another of its arrays (only out == pdf may alias)");
+                return BKE_ERR_BAD_ARG;
+            }
+        }
+    }
+    return -1;
+}
+
+int bke_db_step(const bke_db_args *args, void *stream)
+{
+    const int v = validate_db(args);
+    if (v >= 0) return v;
+    int rc = require_device();
+    if (rc) return rc;
+    return launch_db(*args, (cudaStream_t)stream);
+}
+
 }  // extern "C"

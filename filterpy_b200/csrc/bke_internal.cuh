@@ -119,6 +119,14 @@ int launch_ukf_score(const bke_ukf_score_args &a, cudaStream_t s);
 // the (dim_x, dim_z, dtype) combinations bke_imm_batch_filter has a fused kernel for
 bool imm_batch_has_instance(int dim_x, int dim_z, int dtype);
 int launch_imm_batch(const bke_imm_batch_args &a, cudaStream_t s);
+// np.cumsum(weights) bit for bit into cumsum_out (resample.cu's parity-map scan), its last element also to the
+// device double *total_out when that is non-NULL (bke_cumsum_exact and the discrete Bayes rows too long to stage)
+size_t cumsum_workspace_bytes(int64_t n);
+int cumsum_exact(int64_t n, const double *weights, double *cumsum_out, int last_one, double *total_out, void *workspace,
+                 size_t workspace_bytes, int32_t *info, cudaStream_t stream);
+// bke_db_step after its argument checks (discrete_bayes.cu)
+size_t db_workspace_bytes(int64_t n_bins, int32_t dtype);
+int launch_db(const bke_db_args &a, cudaStream_t s);
 #endif
 
 }  // namespace bke

@@ -1907,10 +1907,8 @@ int bke_weights_scale(int64_t n, const double *weights, const double *divisor, d
 int bke_cumsum_exact(int64_t n, const double *weights, double *cumsum_out, int32_t last_one, void *workspace,
                      size_t workspace_bytes, int32_t *info, void *stream)
 {
-    if (n > 0 && !cumsum_out) { set_error("cumsum_out is NULL"); return BKE_ERR_BAD_ARG; }
-    rs::RunArgs a = whole_array(n, weights, 0.0, nullptr, nullptr, workspace, workspace_bytes, info, nullptr);
-    a.cumsum_out = cumsum_out; a.last_one = last_one ? 1 : 0;
-    return rs::run(a, (cudaStream_t)stream);
+    return bke::cumsum_exact(n, weights, cumsum_out, last_one, nullptr, workspace, workspace_bytes, info,
+                             (cudaStream_t)stream);
 }
 
 int bke_searchsorted(int64_t n, const double *sorted, int64_t n_keys, const double *keys, int32_t side_right,
@@ -1982,3 +1980,18 @@ int bke_gather_rows_bank(int64_t n_sets, int64_t set_len, int64_t row_bytes, con
 }
 
 }  // extern "C"
+
+namespace bke {
+
+size_t cumsum_workspace_bytes(int64_t n) { return bke_resample_workspace_bytes(n); }
+
+int cumsum_exact(int64_t n, const double *weights, double *cumsum_out, int last_one, double *total_out, void *workspace,
+                 size_t workspace_bytes, int32_t *info, cudaStream_t stream)
+{
+    if (n > 0 && !cumsum_out) { set_error("cumsum_out is NULL"); return BKE_ERR_BAD_ARG; }
+    rs::RunArgs a = whole_array(n, weights, 0.0, nullptr, nullptr, workspace, workspace_bytes, info, total_out);
+    a.cumsum_out = cumsum_out; a.last_one = last_one ? 1 : 0;
+    return rs::run(a, stream);
+}
+
+}  // namespace bke

@@ -32,6 +32,8 @@ The same symbols exposed as torch.ops.* via a C++ extension for zero-copy CUDA t
     res, neff = torch.ops.bke.systematic_resample_bank_if_degenerate(weights, particles, u, threshold)
     res, neff = torch.ops.bke.stratified_resample_bank_if_degenerate(weights, particles, uniforms, threshold)
                                      # normalise, neff, resample + gather the sets with neff < threshold, in place
+    post = torch.ops.bke.discrete_bayes_step(pdf, kernel, offsets, offset, likelihood, normalize, constant, cval)
+                                     # discrete_bayes.py predict / update / normalize of every row of pdf[B, M]
 
 Models are shared by the bank when 2-D (stride 0) and per filter when 3-D.  Only the CUDA backend is
 registered: CPU tensors raise ``NotImplementedError`` (no CPU fallback).  The operators run on the

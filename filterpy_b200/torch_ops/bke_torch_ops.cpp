@@ -26,6 +26,8 @@
 //   bke::residual_resample_bank    bke_residual_resample_bank_prepare / _search   resampling.py:27-76 per row
 //   bke::systematic_resample_bank_if_degenerate  bke_resample_bank_gated   normalise, neff, resample + gather where
 //   bke::stratified_resample_bank_if_degenerate  bke_resample_bank_gated   neff < threshold, in place, per row
+//   bke::discrete_bayes_step  bke_db_step              discrete_bayes.py predict / update / normalize of every row
+//                                                      of pdf[B, M]
 #include <limits>
 
 #include <ATen/ATen.h>
@@ -726,6 +728,52 @@ std::tuple<at::Tensor, at::Tensor> stratified_resample_bank_if_degenerate(at::Te
 
 }  // namespace
 
+// discrete_bayes.py:26-128 on every row of pdf[B, M]: predict when kernel ([K] or [B, K], float64) is given (offsets
+// [B] int64 per row, else `offset`), update when likelihood is given, then normalize when asked; a new tensor
+at::Tensor discrete_bayes_step(const at::Tensor &pdf, const c10::optional<at::Tensor> &kernel,
+                               const c10::optional<at::Tensor> &offsets, int64_t offset,
+                               const c10::optional<at::Tensor> &likelihood, bool normalize, bool constant, double cval)
+{
+    TORCH_CHECK(pdf.is_cuda() && pdf.is_contiguous() && pdf.dim() == 2, "bke: pdf must be a contiguous 2-D CUDA tensor");
+    const int dt = dtype_of(pdf);
+    c10::cuda::CUDAGuard guard(pdf.device());
+    const int64_t B = pdf.size(0), M = pdf.size(1);
+    bke_db_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_rows = B; a.n_bins = M; a.dtype = dt;
+    a.flags = (normalize ? BKE_DB_NORMALIZE : 0u) | (constant ? BKE_DB_CONSTANT : 0u);
+    if (kernel) {
+        const at::Tensor &k = *kernel;
+        TORCH_CHECK(k.is_cuda() && k.is_contiguous() && k.scalar_type() == at::kDouble && k.device() == pdf.device() &&
+                    (k.dim() == 1 || (k.dim() == 2 && k.size(0) == B)), "bke: kernel must be a contiguous float64 CUDA tensor [K] or [B, K]");
+        a.kernel = (const double *)k.data_ptr(); a.kernel_len = k.size(-1); a.kernel_stride = k.dim() == 2 ? k.size(1) : 0;
+        a.offset = offset; a.cval = cval;
+        if (offsets) {
+            TORCH_CHECK(offsets->is_cuda() && offsets->is_contiguous() && offsets->scalar_type() == at::kLong &&
+                        offsets->dim() == 1 && offsets->size(0) == B && offsets->device() == pdf.device(),
+                        "bke: offsets must be a contiguous int64 CUDA tensor [B]");
+            a.offsets = (const int64_t *)offsets->data_ptr();
+        }
+    }
+    if (likelihood) {
+        TORCH_CHECK(likelihood->is_cuda() && likelihood->is_contiguous() && likelihood->scalar_type() == pdf.scalar_type() &&
+                    likelihood->sizes() == pdf.sizes() && likelihood->device() == pdf.device(),
+                    "bke: likelihood must be a contiguous CUDA tensor of the pdf's shape and dtype");
+        a.likelihood = likelihood->data_ptr();
+    }
+    at::Tensor out = at::empty_like(pdf);
+    a.pdf = pdf.data_ptr(); a.out = out.data_ptr();
+    const size_t wsb = bke_db_workspace_bytes(M, dt);
+    at::Tensor ws;
+    if (wsb && B) {
+        ws = at::empty({(int64_t)wsb + 256}, pdf.options().dtype(at::kByte));
+        const uintptr_t p = (uintptr_t)ws.data_ptr();
+        a.workspace = (void *)((p + 255) & ~(uintptr_t)255); a.workspace_bytes = wsb;
+    }
+    check_rc(bke_db_step(&a, (void *)c10::cuda::getCurrentCUDAStream().stream()), "bke_db_step");
+    return out;
+}
+
 TORCH_LIBRARY(bke, m)
 {
     m.def("kf_step(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor z, float alpha_sq=1.0) -> (Tensor, Tensor)");
@@ -753,6 +801,8 @@ TORCH_LIBRARY(bke, m)
           "Tensor(c!)[] S, Tensor(d!)[] log_likelihood, Tensor(e!) mu, Tensor(f!) cbar, Tensor trans, Tensor zs, "
           "Tensor? zs_valid=None) -> (Tensor, Tensor, Tensor, Tensor, Tensor)");
     m.def("fls_smooth_batch(Tensor x, Tensor P, Tensor F, Tensor H, Tensor Q, Tensor R, Tensor zs, int N) -> (Tensor, Tensor)");
+    m.def("discrete_bayes_step(Tensor pdf, Tensor? kernel, Tensor? offsets, int offset, Tensor? likelihood, bool normalize, "
+          "bool constant=False, float cval=0.0) -> Tensor");
     m.def("systematic_resample(Tensor weights, float u) -> Tensor");
     m.def("stratified_resample(Tensor weights, Tensor uniforms) -> Tensor");
     m.def("systematic_resample_bank(Tensor weights, Tensor u) -> Tensor");
@@ -767,6 +817,7 @@ TORCH_LIBRARY(bke, m)
 
 TORCH_LIBRARY_IMPL(bke, CUDA, m)
 {
+    m.impl("discrete_bayes_step", &discrete_bayes_step);
     m.impl("kf_step", &kf_step);
     m.impl("kf_predict", &kf_predict);
     m.impl("kf_step_correlated", &kf_step_correlated);

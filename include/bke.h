@@ -1250,6 +1250,49 @@ int bke_residual_prepare(int64_t n, const double *weights, int32_t *indexes, dou
 int bke_searchsorted_bracket_sweep(int64_t n, const double *arr, int64_t n_keys, const double *keys, const int64_t *prev,
                                    int64_t *next, int32_t *indexes32, int32_t *changed, void *stream);
 
+/* ---- discrete Bayes filter banks (filterpy/discrete_bayes/discrete_bayes.py) ----------------------
+ *
+ * bke_db_step: any subset of predict, update and normalize on every row of pdf[n_rows, n_bins] (one 1-D
+ *   histogram filter per row), fp32 or fp64, bit for bit per row:
+ *     predict (kernel != NULL)      wrap: convolve(np.roll(pdf, offset), kernel, mode='wrap') (:124-125);
+ *                                   BKE_DB_CONSTANT: convolve(shift(pdf, offset, cval=cval), kernel,
+ *                                   mode='constant', cval=cval) (:127-128) for an integer offset, which is the
+ *                                   exact shift where the reference's spline shift is so up to its roundoff;
+ *                                   fp64 sums in scipy's window order, weights |w| <= DBL_EPSILON skipped as
+ *                                   scipy skips them, rounded once to the dtype;
+ *     update (likelihood != NULL)   prior * likelihood in the dtype (:88);
+ *     normalize (BKE_DB_NORMALIZE)  p / sum(p) with the builtin sum's sequential fp64 chain 0 + p0 + p1 + ...
+ *                                   and an fp64 division rounded once to the dtype (:47); sums[n_rows] (fp64,
+ *                                   or NULL) receives each row's sum.
+ *   kernel [kernel_len] shared (kernel_stride 0) or [n_rows, kernel_len] (kernel_stride kernel_len), fp64 as
+ *   scipy converts it; offsets[n_rows] (int64) per row, or NULL for `offset` on every row.  Any offset is
+ *   legal, as is kernel_len > n_bins.  out[n_rows, n_bins] may be pdf itself; no other array may overlap
+ *   out, sums or the workspace.  Rows of up to 28928 fp32 / 14464 fp64 bins run one CTA per row; longer
+ *   rows run one at a time in three passes, the sum by bke_cumsum_exact's parity-map scan, and need
+ *   bke_db_workspace_bytes(n_bins, dtype) bytes of 256-byte aligned device workspace (0 for short rows).
+ *   A bad size, flag, dtype, stride or pointer is BKE_ERR_BAD_ARG before any device is touched.  The call
+ *   allocates nothing and can be captured in a graph. */
+#define BKE_DB_NORMALIZE 1u
+#define BKE_DB_CONSTANT 2u
+typedef struct {
+    int64_t n_rows, n_bins;
+    int32_t dtype;
+    uint32_t flags;                                  /* BKE_DB_NORMALIZE | BKE_DB_CONSTANT */
+    const double *kernel;                            /* NULL: no predict */
+    int64_t kernel_len, kernel_stride;
+    const int64_t *offsets;                          /* NULL: `offset` for every row */
+    int64_t offset;
+    double cval;                                     /* BKE_DB_CONSTANT only */
+    const void *pdf, *likelihood;                    /* likelihood NULL: no update */
+    void *out;
+    double *sums;                                    /* NULL or [n_rows], with BKE_DB_NORMALIZE */
+    void *workspace;
+    size_t workspace_bytes;
+} bke_db_args;
+
+size_t bke_db_workspace_bytes(int64_t n_bins, int32_t dtype);
+int bke_db_step(const bke_db_args *args, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
