@@ -77,8 +77,10 @@ __device__ __forceinline__ void philox4x32_10(uint32_t (&c)[4], uint32_t k0, uin
 }
 
 // Box-Muller on one Philox output.  fp64: u1 = (c0:c1 top 53 bits + 1) 2^-53 in (0, 1], u2 = (c2:c3 top 53
-// bits) 2^-53.  fp32: the same uniforms rounded to float from c0 and c2 alone (they agree with the fp64 ones
-// to float rounding).  z0 = sqrt(-2 ln u1) cos(2 pi u2), z1 = sqrt(-2 ln u1) sin(2 pi u2).
+// bits) 2^-53.  fp32: u1 = (float(c0) + 1) 2^-32 in (0, 1] and u2 = float(c2) 2^-32 (u2 may round up to 1),
+// 24-bit uniforms from one word each.  They are not the fp64 uniforms rounded: the fp32 normals differ from
+// the fp64 stream by up to about 1e-3 sigma in the tails (small c0, c0 near 2^32), and oracle/enkf.py draws
+// the fp32 stream from these uniforms.  z0 = sqrt(-2 ln u1) cos(2 pi u2), z1 = sqrt(-2 ln u1) sin(2 pi u2).
 template <typename T>
 __device__ __forceinline__ void box_muller(const uint32_t (&c)[4], T &z0, T &z1)
 {

@@ -29,21 +29,33 @@ def philox4x32_10(ctr, key):
     return c
 
 
-def box_muller(c):
-    """The kernel's fp64 Box-Muller of one Philox output: u1 in (0, 1], u2 in [0, 1)."""
-    u1 = (((c[0] << np.uint64(21)) | (c[1] >> np.uint64(11))) + np.uint64(1)).astype(np.float64) * 2.0 ** -53
-    u2 = ((c[2] << np.uint64(21)) | (c[3] >> np.uint64(11))).astype(np.float64) * 2.0 ** -53
+def box_muller(c, dtype=np.float64):
+    """The kernel's Box-Muller of one Philox output for element type ``dtype``: u1 in (0, 1]; u2 in [0, 1) in fp64,
+    [0, 1] in fp32.
+
+    fp64: u1 = (c0:c1 top 53 bits + 1) 2^-53, u2 = (c2:c3 top 53 bits) 2^-53.  fp32: u1 = (float(c0) + 1) 2^-32
+    and u2 = float(c2) 2^-32 in float arithmetic (round to nearest), 24 bits from one word each, so u2 may round
+    up to 1.  The radius and the angle are evaluated in fp64 either way: against the kernel's fp32 stream this
+    measures its logf / sqrtf / sincospif, not the uniforms."""
+    if np.dtype(dtype) == np.float32:
+        f32 = np.float32
+        u1 = ((np.asarray(c[0]).astype(np.float64).astype(f32) + f32(1.0)) * f32(2.0 ** -32)).astype(np.float64)
+        u2 = (np.asarray(c[2]).astype(np.float64).astype(f32) * f32(2.0 ** -32)).astype(np.float64)
+    else:
+        u1 = (((c[0] << np.uint64(21)) | (c[1] >> np.uint64(11))) + np.uint64(1)).astype(np.float64) * 2.0 ** -53
+        u2 = ((c[2] << np.uint64(21)) | (c[3] >> np.uint64(11))).astype(np.float64) * 2.0 ** -53
     r = np.sqrt(-2.0 * np.log(u1))
     return r * np.cos(2.0 * np.pi * u2), r * np.sin(2.0 * np.pi * u2)
 
 
-def std_normals(seed, f, call, n_members, k):
-    """(n_members, k) standard normals of filter ``f``, draw call ``call`` (components 2q, 2q+1 from counter q)."""
+def std_normals(seed, f, call, n_members, k, dtype=np.float64):
+    """(n_members, k) standard normals of filter ``f``, draw call ``call`` (components 2q, 2q+1 from counter q),
+    as the kernel of element type ``dtype`` draws them."""
     out = np.empty((n_members, k))
     member = np.arange(n_members, dtype=np.uint64)
     for q in range((k + 1) // 2):
-        c = philox4x32_10((q, member, call, int(f) >> 32), (seed, int(f) & 0xffffffff))
-        z0, z1 = box_muller(c)
+        c = philox4x32_10((q, member, int(call) & 0xffffffff, int(f) >> 32), (seed, int(f) & 0xffffffff))
+        z0, z1 = box_muller(c, dtype)
         out[:, 2 * q] = z0
         if 2 * q + 1 < k:
             out[:, 2 * q + 1] = z1
@@ -73,17 +85,18 @@ def psd_factor(C, eps=np.finfo(np.float64).eps):
 
 class Stream(object):
     """The noise of one filter: ``draw(call, mean, cov, size)`` = mean + xi L' (what the golden generator
-    substitutes for the reference's ``multivariate_normal``)."""
+    substitutes for the reference's ``multivariate_normal``).  ``dtype`` is the element type of the kernel the
+    stream stands for: its uniforms (box_muller) and the eps of its semi-definite factor (psd_factor)."""
 
-    def __init__(self, seed, f):
-        self.seed, self.f = int(seed), int(f)
+    def __init__(self, seed, f, dtype=np.float64):
+        self.seed, self.f, self.dtype = int(seed), int(f), np.dtype(dtype).type
 
     def draw(self, call, mean, cov, size):
         cov = np.atleast_2d(np.asarray(cov, dtype=np.float64))
-        L, ok = psd_factor(cov)
+        L, ok = psd_factor(cov, np.finfo(self.dtype).eps)
         if not ok:
             raise np.linalg.LinAlgError("covariance is not positive semi-definite")
-        xi = std_normals(self.seed, self.f, call, size, cov.shape[0])
+        xi = std_normals(self.seed, self.f, call, size, cov.shape[0], self.dtype)
         return np.asarray(mean, dtype=np.float64) + xi @ L.T
 
 

@@ -12,7 +12,7 @@ import re
 import numpy as np
 import pytest
 
-from gpu_harness import rel_close, RTOL
+from gpu_harness import corr_spd as _corr_spd, sigma_problem as _problem, rel_close, RTOL
 
 CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "filterpy_b200", "csrc")
 DT = 0.1
@@ -58,54 +58,6 @@ def test_instance_table_is_the_dispatch_table(src):
 
 
 # ----------------------------------------------------------------------------------------------- problems
-def _corr_spd(rng, N, d, sd):
-    """N random SPD matrices with correlated entries: sd_i sd_j (A A'/d + I/2)_ij, A standard normal."""
-    A = rng.standard_normal((N, d, d))
-    return (A @ np.swapaxes(A, 1, 2) / d + 0.5 * np.eye(d)) * np.outer(sd, sd)
-
-
-def _problem(n, m, fx, hx, N=1037, T=3, seed=0):
-    """x, correlated P, the model matrices in both layouts (shared by the bank / one per filter), T epochs of
-    z and a ~20 % mask of missing measurements.  The range models see targets 100-500 m from a sensor at the
-    origin, well inside (-pi, pi) in azimuth."""
-    from oracle import ukf as oukf
-    rng = np.random.default_rng(seed)
-    ranged = hx != "LINEAR"
-    if ranged:
-        x = np.zeros((N, n))
-        x[:, 1::2] = rng.uniform(-10, 10, (N, n // 2))
-        x[:, 0] = rng.uniform(100, 500, N); x[:, 2] = rng.uniform(-300, 300, N)
-        if n == 6:
-            x[:, 4] = rng.uniform(20, 200, N)
-        sd = np.tile([2.0, 0.5], n // 2)
-        rsd = np.array([1.0, 0.005, 0.005])[:m]
-    else:
-        x = rng.normal(0.0, 5.0, (N, n))
-        sd = rng.uniform(0.5, 2.0, n)
-        rsd = rng.uniform(0.5, 2.0, m)
-    P = _corr_spd(rng, N, n, sd)
-    Q = _corr_spd(rng, N, n, 0.1 * sd)
-    R = _corr_spd(rng, N, m, rsd)
-    F = Fpf = H = Hpf = None
-    if fx == "LINEAR":
-        F = np.eye(n)
-        if n % 2 == 0:
-            F[np.arange(0, n, 2), np.arange(1, n, 2)] = DT
-        eps = 0.002 if ranged else 0.1
-        F = F + eps * rng.standard_normal((n, n))
-        Fpf = F + eps * rng.standard_normal((N, n, n))
-    if hx == "LINEAR":
-        H = rng.standard_normal((m, n))
-        Hpf = H + 0.1 * rng.standard_normal((N, m, n))
-    truth = x + sd * rng.standard_normal((N, n))
-    zs = np.empty((T, N, m))
-    for t in range(T):
-        truth = oukf.fx_apply(FX[fx], truth, DT, Fpf)
-        zs[t] = oukf.hx_apply(HX[hx], truth, Hpf) + rsd * rng.standard_normal((N, m))
-    valid = rng.random((T, N)) >= 0.2
-    return dict(x=x, P=P, zs=zs, valid=valid, shared=dict(F=F, H=H, Q=Q[0], R=R[0]), per=dict(F=Fpf, H=Hpf, Q=Q, R=R))
-
-
 def _take(mats, N):
     return {k: (v[:N] if v is not None and v.ndim == 3 else v) for k, v in mats.items()}
 

@@ -88,6 +88,56 @@ def test_box_muller_uniforms_exclude_zero():
     assert oe.box_muller(full) == (0.0, -0.0) or max(abs(v) for v in oe.box_muller(full)) == 0.0
 
 
+def test_box_muller_f32_uniforms_at_the_ends_of_the_word():
+    """fp32: u1 = (float(c0) + 1) 2^-32 in (0, 1] and u2 = float(c2) 2^-32, both rounded to float; c2 = 2^32 - 1
+    rounds u2 up to exactly 1 (angle 2 pi), which the fp64 uniforms never reach."""
+    top = 0xffffffff
+    z0, z1 = oe.box_muller([np.uint64(0)] * 4, np.float32)     # u1 = 2^-32 exactly: the largest fp32 radius
+    assert z0 == np.sqrt(-2 * np.log(2.0 ** -32)) and z1 == 0.0
+    z0, z1 = oe.box_muller([np.uint64(top), np.uint64(0), np.uint64(0), np.uint64(0)], np.float32)
+    assert z0 == 0.0 and z1 == 0.0                              # float(2^32 - 1) + 1 = 2^32: u1 = 1, radius 0
+    z0, z1 = oe.box_muller([np.uint64(0), np.uint64(0), np.uint64(top), np.uint64(0)], np.float32)
+    assert z0 == np.sqrt(-2 * np.log(2.0 ** -32)) and abs(z1) < 1e-14 * z0     # u2 = 1: cos 2 pi, sin 2 pi
+    # float(2^32 - 100) = 2^32: u1 = 1; float(2^32 - 200) = 2^32 - 256: u1 = 1 - 2^-24, the smallest radius > 0
+    assert oe.box_muller([np.uint64(top - 100), np.uint64(0), np.uint64(0), np.uint64(0)], np.float32)[0] == 0.0
+    z0, _ = oe.box_muller([np.uint64(top - 200), np.uint64(0), np.uint64(0), np.uint64(0)], np.float32)
+    assert z0 == np.sqrt(-2 * np.log(1 - 2.0 ** -24))
+    # the fp32 uniforms are float(word) + 1 (u1) and float(word) (u2), scaled: exact at small words
+    for w in (1, 5, 1 << 20, 123456789):
+        z0, z1 = oe.box_muller([np.uint64(w), np.uint64(0), np.uint64(w), np.uint64(0)], np.float32)
+        u1 = float(np.float32(np.float32(w) + np.float32(1))) * 2.0 ** -32
+        u2 = float(np.float32(w)) * 2.0 ** -32
+        r = np.sqrt(-2 * np.log(u1))
+        assert z0 == r * np.cos(2 * np.pi * u2) and z1 == r * np.sin(2 * np.pi * u2)
+
+
+def test_f32_stream_agrees_with_the_f64_stream_to_the_24_bit_uniforms():
+    """The fp32 normals differ from the fp64 ones only by the uniforms' lost bits: within 1e-3 absolute over 2^20
+    draws of each of three keys (median below 1e-6).  They are not the same stream, though: at c0 = c1 = 0 the
+    fp64 u1 is 2^-53 and the fp32 one 2^-32, radii 8.6 and 6.7, so an fp32 comparison needs the fp32 uniforms."""
+    for seed, f, call in ((0, 0, 0), (0xffffffff, 37, 0xffffffff), (7, 3, 2)):
+        a = oe.std_normals(seed, f, call, 1 << 18, 4)
+        b = oe.std_normals(seed, f, call, 1 << 18, 4, np.float32)
+        d = np.abs(a - b)
+        assert d.max() < 1e-3 and np.median(d) < 1e-6, (seed, f, call, d.max(), np.median(d))
+    zero = [np.uint64(0)] * 4
+    assert oe.box_muller(zero)[0] - oe.box_muller(zero, np.float32)[0] > 1.9
+
+
+def test_f32_stream_factors_with_the_f32_eps():
+    """Stream(dtype=float32) zeroes a pivot below 16 k eps32 max diag C, as the fp32 kernel does: a rank-one C
+    rounded to float, whose second pivot is float rounding rather than 0, draws inside its range."""
+    v = np.array([1.0, 1.0 / 3.0, 0.7])
+    C = np.outer(v, v).astype(np.float32).astype(np.float64)
+    assert not oe.psd_factor(C)[1] or oe.psd_factor(C)[0][1, 1] != 0.0       # fp64 eps sees the rounding
+    L, ok = oe.psd_factor(C, np.finfo(np.float32).eps)
+    assert ok and L[1, 1] == 0.0 and L[2, 2] == 0.0
+    e = oe.Stream(3, 1, np.float32).draw(0, np.zeros(3), C, 1000)
+    u = v / np.linalg.norm(v)
+    assert np.abs(e - np.outer(e @ u, u)).max() < 1e-6 * np.abs(e).max()
+    assert oe.Stream(3, 1).dtype is np.float64 and oe.Stream(3, 1, np.float32).dtype is np.float32
+
+
 def test_std_normals_statistics_and_keys():
     xi = oe.std_normals(7, 3, 0, 40000, 4)
     assert abs(xi.mean()) < 0.02 and abs(xi.var() - 1) < 0.02
