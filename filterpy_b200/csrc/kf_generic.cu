@@ -287,8 +287,12 @@ int launch_t(const bke_kf_args &a, cudaStream_t s, const KfP<T> *form = nullptr)
     const size_t bytes_per_warp = (size_t)per_warp * sizeof(T), budget = 200 * 1024;
     WarpShape w;
     if (int rc = warp_shape((const void *)kf_generic_kernel<T, FORM>, bytes_per_warp, budget, p.N, w)) {
+        // named after the entry point that made the call (a row block's m is its row count)
+        const char *entry = FORM == FORM_CORRELATED ? "bke_kf_step_correlated"
+                          : FORM == FORM_ROWS       ? "bke_kf_update_rows" : "bke_kf_step";
         if (rc == BKE_ERR_UNSUPPORTED)
-            set_error("bke_kf_step: dim_x=%d dim_z=%d needs %zu B of shared memory per filter (> %zu)", n, m, bytes_per_warp, budget);
+            set_error("%s: dim_x=%d %s=%d needs %zu B of shared memory per filter (> %zu)", entry, n,
+                      FORM == FORM_ROWS ? "rows" : "dim_z", m, bytes_per_warp, budget);
         return rc;
     }
     kf_generic_kernel<T, FORM><<<w.grid, w.wpb * 32, w.smem, s>>>(p, per_warp);

@@ -50,17 +50,18 @@ def kernel_name(s, prefix):
     return None
 
 
-# bke_kf_step's kernels: the KF instance table names them, and so do the FLS per-epoch routes that step on them
-def k_direct(dt, n, m, ex):
-    return "kf_direct_kernel<%s, %d, %d, %s, 0>" % (TNAME[dt], n, m, b(ex))
+# bke_kf_step's kernels: the KF instance table names them, and so do the FLS per-epoch routes that step on them.
+# form: the update form template argument (kf_direct.cu / kf_generic.cu FORM_PLAIN 0, FORM_CORRELATED 1, FORM_ROWS 2)
+def k_direct(dt, n, m, ex, form=0):
+    return "kf_direct_kernel<%s, %d, %d, %s, %d>" % (TNAME[dt], n, m, b(ex), form)
 
 
 def k_rb(dt, n, m, rpl, ex, mode, shared):
     return "kf_rowblock_kernel<%s, %d, %d, %d, %s, %d, %s>" % (TNAME[dt], n, m, rpl, b(ex), mode, b(shared))
 
 
-def k_gen(dt):
-    return "kf_generic_kernel<%s, 0>" % TNAME[dt]
+def k_gen(dt, form=0):
+    return "kf_generic_kernel<%s, %d>" % (TNAME[dt], form)
 
 
 def k_fast(mode, shared, ex):

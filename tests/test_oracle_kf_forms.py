@@ -130,6 +130,75 @@ def test_correlated_p_is_not_symmetrised(golden):
     assert np.abs(g["out_P"] - np.swapaxes(g["out_P"], 1, 2)).max() > 0
 
 
+def _bank(N, n, m, seed):
+    rng = np.random.default_rng(seed)
+    A = rng.normal(size=(N, n, n))
+    B = rng.normal(size=(N, m, m))
+    return dict(x=rng.normal(size=(N, n)), P=A @ np.swapaxes(A, 1, 2) + np.eye(n), H=rng.normal(size=(N, m, n)),
+                R=B @ np.swapaxes(B, 1, 2) + np.eye(m), M=0.3 * rng.normal(size=(N, n, m)), z=rng.normal(size=(N, m)))
+
+
+def test_sequential_bank_with_one_singular_block():
+    """A singular S_i (L > 1) in one filter gives that filter status 1, its prior and no y, K or z, and leaves every
+    other filter as a bank without it computes them (np.linalg.inv of the whole stack would raise)."""
+    N, n, m, start, L = 6, 4, 4, 1, 2
+    w = _bank(N, n, m, 0)
+    y0, K0, z0 = np.full((N, m), 7.0), np.full((N, n, m), 7.0), np.full((N, m), 7.0)
+    zi = w["z"][:, start:start + L]
+    clean = kfo.kf_update_sequential_bank(w["x"], w["P"], start, zi, w["H"], w["R"], y0, K0, z0)
+    H, R = w["H"].copy(), w["R"].copy()
+    H[3, start + L - 1] = 0; R[3, start + L - 1] = 0; R[3, :, start + L - 1] = 0
+    o = kfo.kf_update_sequential_bank(w["x"], w["P"], start, zi, H, R, y0, K0, z0)
+    np.testing.assert_array_equal(o["status"], [0, 0, 0, 1, 0, 0])
+    assert np.array_equal(o["x"][3], w["x"][3]) and np.array_equal(o["P"][3], w["P"][3])
+    assert np.all(o["y"][3] == 7) and np.all(o["K"][3] == 7) and np.all(o["z"][3] == 7)
+    ok = np.arange(N) != 3
+    for k in ("x", "P", "y", "K", "z"):
+        np.testing.assert_allclose(o[k][ok], clean[k][ok], rtol=1e-12, atol=1e-12)
+    # BKE_STATUS_STICKY keeps the starting word where the update succeeds
+    st = kfo.kf_update_sequential_bank(w["x"], w["P"], start, zi, H, R, y0, K0, z0, status=np.full(N, 5),
+                                       sticky=True)["status"]
+    np.testing.assert_array_equal(st, [5, 5, 5, 1, 5, 5])
+    # L = 1 with S_i = 0: the reciprocal's inf / NaN, status 0
+    Hi = np.zeros((N, 1, n)); Hi[:, 0, 0] = 1
+    P = w["P"].copy(); P[:, 0, 0] = 2.0
+    o = kfo.kf_update_sequential_bank(w["x"], P, 0, w["z"][:, :1], w["H"], w["R"], y0, K0, z0,
+                                      R_i=np.full((N, 1, 1), -2.0), H_i=Hi)
+    assert np.all(o["status"] == 0) and np.all(np.isinf(o["K"][:, 0, 0])) and np.isnan(o["P"]).any()
+
+
+def test_zero_pivot_is_exact_singularity():
+    """zero_pivot calls singular only an exact zero pivot: not an ill-conditioned or indefinite S, which
+    np.linalg.matrix_rank's tolerance calls singular at cond 1e17."""
+    U = np.linalg.qr(np.random.default_rng(1).normal(size=(3, 3)))[0]
+    ill = (U * [1.0, 1e-9, 1e-17]) @ U.T
+    assert np.linalg.matrix_rank(ill) < 3
+    S = np.stack([ill, np.diag([1.0, -2.0, 3.0]), np.array([[1.0, 2.0, 0.0], [2.0, 4.0, 0.0], [0.0, 0.0, 1.0]]),
+                  np.zeros((3, 3)), np.array([[0.0, 1.0, 0.0], [1.0, 0.0, 0.0], [0.0, 0.0, 1.0]])])
+    np.testing.assert_array_equal(kfo.zero_pivot(S), [False, False, True, True, False])
+
+
+def test_correlated_bank_singular_rule():
+    """update_correlated's bank: an exactly singular S (a zero row of H, R and M') gives status 1, the prior and no y;
+    an ill-conditioned S is inverted; a filter without a measurement gets y = 0 and status 0 whatever its S."""
+    N, n, m = 5, 4, 3
+    w = _bank(N, n, m, 2)
+    H, R, M = w["H"].copy(), w["R"].copy(), w["M"].copy()
+    H[1, -1] = 0; R[1, -1] = 0; R[1, :, -1] = 0; M[1, :, -1] = 0
+    H[4] = H[1]; R[4] = R[1]; M[4] = M[1]
+    U = np.linalg.qr(np.random.default_rng(3).normal(size=(m, m)))[0]
+    HM = H[2] @ M[2]
+    R[2] = (U * [1.0, 1e-6, 1e-12]) @ U.T - (H[2] @ w["P"][2] @ H[2].T + HM + HM.T)
+    valid = np.array([True, True, True, True, False])
+    o = kfo.kf_update_correlated_bank(w["x"], w["P"], w["z"], H, R, M, valid=valid)
+    np.testing.assert_array_equal(o["status"], [0, 1, 0, 0, 0])
+    assert np.array_equal(o["x"][1], w["x"][1]) and np.all(np.isnan(o["y"][1])) and np.all(o["y"][4] == 0)
+    np.testing.assert_allclose(o["SI"][2] @ o["S"][2], np.eye(m), atol=1e-3)
+    st = kfo.kf_update_correlated_bank(w["x"], w["P"], w["z"], H, R, M, valid=valid, status=np.full(N, 5),
+                                       sticky=True)["status"]
+    np.testing.assert_array_equal(st, [5, 1, 5, 5, 5])
+
+
 # ---------------------------------------------------------------------------------------------- C-ABI checks
 def _rows_args(N=4, n=4, m=3, start=0, rows=1):
     x = np.zeros((N, n)); P = np.zeros((N, n, n)); H = np.zeros((m, n)); R = np.eye(m); z = np.zeros((N, rows))
