@@ -124,7 +124,7 @@ class Bufs:
         es = a.itemsize
         off = 16 // es + (1 if mis else 0)
         tdt = {np.dtype(F32): torch.float32, np.dtype(F64): torch.float64, np.dtype(np.int32): torch.int32,
-               np.dtype(np.uint8): torch.uint8}[a.dtype]
+               np.dtype(np.int64): torch.int64, np.dtype(np.uint8): torch.uint8}[a.dtype]
         fill = float("nan") if tdt in (torch.float32, torch.float64) else -7
         buf = torch.full((off + a.size + 5,), fill, dtype=tdt, device="cuda")
         buf[off:off + a.size] = torch.from_numpy(a.reshape(-1)).cuda()

@@ -59,3 +59,46 @@ def score(z, zhat, S, valid=None):
 def innovation_cov(P, H, R):
     """S = H P H' + R per track (H, R [m, .] shared or [N, m, .])."""
     return np.einsum("...an,...nk,...bk->...ab", H, P, H) + R
+
+
+def inverse_bank(S):
+    """inverse() over a bank S[N, m, m], vectorised: (S^-1 [N, m, m], log|det S| [N], ok [N]); a track with an exactly
+    zero pivot has ok False (and meaningless S^-1, log|det S|)."""
+    A = np.array(S, dtype=np.float64)
+    N, m, _ = A.shape
+    X = np.broadcast_to(np.eye(m), A.shape).copy()
+    ld, ok, ar = np.zeros(N), np.ones(N, bool), np.arange(N)
+    for c in range(m):
+        p = c + np.argmax(np.abs(A[:, c:, c]), axis=1)
+        for M in (A, X):
+            rc, rp = M[ar, c].copy(), M[ar, p].copy()
+            M[ar, c], M[ar, p] = rp, rc
+        piv = A[:, c, c]
+        ok &= piv != 0
+        piv = np.where(ok, piv, 1.0)
+        ld += np.log(np.abs(piv))
+        A[:, c] /= piv[:, None]
+        X[:, c] /= piv[:, None]
+        f = A[:, :, c].copy()
+        f[:, c] = 0.0
+        A -= f[:, :, None] * A[:, c][:, None, :]
+        X -= f[:, :, None] * X[:, c][:, None, :]
+    return X, ld, ok
+
+
+def score_bank(z, zhat, S, valid=None):
+    """score() with inverse_bank: the same outputs, vectorised over the tracks."""
+    z = np.asarray(z, np.float64)
+    N, K, m = z.shape
+    y = z - np.asarray(zhat, np.float64)[:, None, :]
+    SI, ld, ok = inverse_bank(S)
+    with np.errstate(invalid="ignore", over="ignore"):
+        d2 = np.einsum("nka,nab,nkb->nk", y, SI, y)
+        ll = -0.5 * (d2 + ld[:, None] + m * math.log(2 * math.pi))
+        d2[~ok], ll[~ok] = np.nan, np.nan
+        if valid is not None:
+            v = np.asarray(valid, bool)
+            y[~v] = 0.0
+            d2[~v], ll[~v] = 0.0, LOG_DBL_MIN
+        return dict(y=y, d2=d2, mahalanobis=np.sqrt(d2), log_likelihood=ll, likelihood=np.exp(ll),
+                    status=(~ok).astype(np.int32), SI=SI, logdet=ld)
